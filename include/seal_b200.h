@@ -76,7 +76,9 @@ size_t sb200_device_bytes(const sb200_context *ctx);
  *   SB200_LIMIT_KS_ALGORITHM      key switching: 0 = 64-bit digit transforms per output prime; 1 (default, env SB200_KS_ALGO) =
  *                                 automatic: the exact integer convolution on 29-bit auxiliary primes where it is available
  *                                 (n >= 4096) and pays (levels with >= 16 digits, env SB200_KS_MIN_DIGITS); 2 = that path at every
- *                                 level.  Results are identical words in every mode. */
+ *                                 level.  In modes 1 and 2, levels with more digits than the path's unreduced 64-bit product sums
+ *                                 hold (L (p_max - 1)^2 >= 2^64: above 64 digits at n = 4096) take the 64-bit digit transforms.
+ *                                 Results are identical words in every mode. */
 #define SB200_LIMIT_SCRATCH_BYTES 0
 #define SB200_LIMIT_KS_CHUNK 1
 #define SB200_LIMIT_HOST_STAGE_BYTES 2

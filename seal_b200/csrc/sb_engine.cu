@@ -462,7 +462,8 @@ namespace sb
 
     // general-size tensor in an arbitrary base (evaluator.cpp:664-700 / :796-833 NTT-form schemes, :524-560 BFV):
     // out[k] = sum_{i+j=k} x_i * y_j for 0 <= k < s1+s2-1.  x = [B][s1][nb][n] at xa (+ b*xa_bs), y likewise; the prime of
-    // row i is pid_tab[i] (or i).  At most min(s1,s2) <= 16 products of canonical residues meet in one 128-bit sum.
+    // row i is pid_tab[i] (or i).  The words are canonicalised on the way in (canon_in: the reference's dyadic products accept any
+    // 64-bit representative), so at most min(s1,s2) <= 16 products below q^2 < 2^122 meet in one 128-bit sum.
     __global__ void __launch_bounds__(256) tensor_general_kernel(const u64 *__restrict__ xa, long long xa_bs, const u64 *__restrict__ xb,
                                                                   long long xb_bs, u64 *__restrict__ out, const PrimeDev *__restrict__ primes,
                                                                   const int *__restrict__ pid_tab, int logn, int nb, int s1, int s2,
@@ -482,7 +483,7 @@ namespace sb
             const int i0 = k - (s2 - 1) > 0 ? k - (s2 - 1) : 0, i1 = k < s1 - 1 ? k : s1 - 1;
             u64 lo = 0, hi = 0;
             for (int a = i0; a <= i1; a++)
-                mac128(lo, hi, px[a * poly], py[(k - a) * poly]);
+                mac128(lo, hi, canon_in(px[a * poly], P), canon_in(py[(k - a) * poly], P));
             po[k * poly] = barrett128(lo, hi, P.q, P.ratio_lo, P.ratio_hi);
         }
     }

@@ -129,10 +129,15 @@ namespace sb
         LaunchStats stats;
         KsInt ksint;                         // integer key-switching path (sb_ksint.cuh); ready = tables built
         // key switching: 0 = 64-bit digit transforms, 1 = automatic (the integer path from ks_min_digits digits on: below that the
-        // L (L+1) large transforms are cheaper than S L + 2 S (L+1) small ones plus the reconstruction), 2 = integer path always
+        // L (L+1) large transforms are cheaper than S L + 2 S (L+1) small ones plus the reconstruction), 2 = integer path always.
+        // In both modes 1 and 2, levels with more than ksint.max_digits digits (65 and up at n = 4096) take the 64-bit path: the
+        // unreduced 64-bit sums of the integer path's product kernels would overflow there.
         int ks_algo = 1;
         size_t ks_min_digits = 16; // H100: the 64-bit path is still ahead at 15 digits, the integer path at 31 (DESIGN.md 3.2)
-        bool ksint_on(size_t L) const { return ksint.ready && (ks_algo == 2 || (ks_algo == 1 && L >= ks_min_digits)); }
+        bool ksint_on(size_t L) const
+        {
+            return ksint.ready && L <= ksint.max_digits && (ks_algo == 2 || (ks_algo == 1 && L >= ks_min_digits));
+        }
         IoArena io;
         std::mutex mu;
         // cross-stream ordering of calls that share the scratch arenas (sb_api.cu: StreamOrder)

@@ -451,6 +451,8 @@ namespace sbh
             have += std::log2(static_cast<long double>(cand));
         }
         const int S = h.S = static_cast<int>(h.p.size());
+        const u64 pm1 = *std::max_element(h.p.begin(), h.p.end()) - 1;
+        h.max_digits = static_cast<std::size_t>(~u64(0) / (pm1 * pm1));
         const std::size_t nb = std::size_t(1) << h.r;
         auto pair32 = [](u64 w, u64 p, std::uint32_t *dst) {
             dst[0] = static_cast<std::uint32_t>(w);

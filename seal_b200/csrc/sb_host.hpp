@@ -112,6 +112,9 @@ namespace sbh
     {
         int S = 0;     // auxiliary primes
         int r = 0;     // stages of the outer pass: logn - 12 (the local pass transforms 4096-element blocks in shared memory)
+        // most digits the product kernels sum in 64 bits without a reduction: the largest L with L (max p - 1)^2 < 2^64 (the
+        // transformed digits and key words are canonical); levels with more digits take the 64-bit path (Context::ksint_on)
+        std::size_t max_digits = 0;
         std::vector<std::uint32_t> p;          // [S]
         std::vector<std::uint32_t> red;        // [S][2]: 2^32 mod p with its quotient (reduction of 64-bit words)
         std::vector<std::uint32_t> mu;         // [S]: floor(2^32 / p)

@@ -856,6 +856,7 @@ namespace sb
             return;
         KsInt &d = c.ksint;
         d.prm.S = h.S, d.prm.r = h.r, d.prm.logn = c.logn;
+        d.max_digits = h.max_digits; // the 64-bit sums of ks32_mac / ks32_mac_tile: deeper levels take the 64-bit path
         for (int t = 0; t < h.S; t++)
         {
             d.prm.p[t] = h.p[t], d.prm.mu[t] = h.mu[t], d.prm.c2[t] = h.c2[t];

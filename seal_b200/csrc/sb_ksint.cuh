@@ -37,6 +37,7 @@ namespace sb
         bool ready = false;
         bool mac_tile = true;  // product kernel with the key tile in shared memory (env SB200_KS_MAC_TILE)
         bool fuse_crt = true;  // outer inverse stages inside the reconstruction kernel (env SB200_KS_FUSE_CRT)
+        size_t max_digits = 0; // sbh::KsIntHost::max_digits (64 at n = 4096)
         KsIntParams prm;
         uint2 *d_fwd_outer = nullptr, *d_inv_outer = nullptr; // [S][2^r]
         uint2 *d_fwd_local = nullptr, *d_inv_local = nullptr; // [S][2^r][4096]

@@ -19,3 +19,64 @@ def rand_ct(rng, moduli, n, size, L, batch=None):
     if batch is None:
         return one()
     return np.stack([one() for _ in range(batch)])
+
+
+# ---- structured inputs at the arithmetic bounds (tests/test_gpu_bounds.py) ----
+# Each generator returns words laid out like rand_ct, [size][L][n] or [batch][size][L][n]; the prime of row i is moduli[i].
+
+def fill_ct(moduli, n, size, L, word, batch=None):
+    """every word of row i = word(q_i) (a Python int below 2^64), e.g. `lambda q: q - 1` or `lambda q: 0`"""
+    rows = np.stack([np.full(n, word(int(moduli[i])), dtype=np.uint64) for i in range(L)])
+    shape = (size, L, n) if batch is None else (batch, size, L, n)
+    return np.broadcast_to(rows, shape).copy()  # a writable array of its own
+
+
+def max_ct(moduli, n, size, L, batch=None):
+    """all words q - 1: the largest canonical residue"""
+    return fill_ct(moduli, n, size, L, lambda q: q - 1, batch)
+
+
+def zero_ct(moduli, n, size, L, batch=None):
+    return fill_ct(moduli, n, size, L, lambda q: 0, batch)
+
+
+def alternating_ct(moduli, n, size, L, batch=None):
+    """words 0, q - 1, 0, q - 1, ... along every row"""
+    out = max_ct(moduli, n, size, L, batch)
+    out[..., 0::2] = 0
+    return out
+
+
+def largest_representative(x, q):
+    """the largest 64-bit word congruent to x mod q: x + q * floor((2^64 - 1 - x) / q)"""
+    x = np.asarray(x, dtype=np.uint64)
+    return x + np.uint64(q) * ((np.uint64(2 ** 64 - 1) - x) // np.uint64(q))
+
+
+def unreduce(a, moduli, axis_prime=-2):
+    """every word replaced by its largest 64-bit representative (the prime of a row is moduli[index along axis_prime])"""
+    out = np.array(a, dtype=np.uint64, copy=True)
+    view = np.moveaxis(out, axis_prime, 0)
+    for i in range(view.shape[0]):
+        view[i] = largest_representative(view[i], int(moduli[i]))
+    return out
+
+
+def const_ntt_row(c, n):
+    """the NTT form of the constant polynomial c * delta_0: the word c at every point (c below the row's prime).  Its transform
+    modulo any auxiliary prime p_t is c mod p_t at every point, so c = p_t - 1 maximises the integer key-switching path's
+    transformed digits and key words for prime t."""
+    return np.full(n, c, dtype=np.uint64)
+
+
+def all_coeffs_ntt(ntt_rows, moduli, n, L):
+    """NTT form of the polynomial whose every coefficient is q_i - 1 (row i), [L][n]; ntt_rows maps a coefficient-form [L][n]
+    array to NTT form (the oracle's ntt_row per row at small n, the library's transform_to_ntt at large n).  For two such
+    polynomials alpha and beta the negacyclic product is alpha beta (2x + 2 - n): the digit sums of key switching reach
+    +L n (q_J - 1)(q_I - 1) at x = n - 1 and nearly as much, negative, at x = 0."""
+    return ntt_rows(max_ct(moduli, n, 1, L)[0])
+
+
+def negacyclic_ones_square(n):
+    """coefficient x of (1 + x + ... + x^(n-1))^2 mod x^n + 1, as Python ints: 2x + 2 - n"""
+    return [2 * x + 2 - n for x in range(n)]

@@ -3,6 +3,7 @@
 // three radix-16 passes per 4096-block with the transposed last-pass twiddles) and must satisfy the round trip and the
 // convolution theorem; the CRT constants must reconstruct known integers.  No GPU, no CUDA.
 #include "../../seal_b200/csrc/sb_host.hpp"
+#include <algorithm>
 #include <cstdio>
 #include <cstdlib>
 #include <random>
@@ -179,15 +180,18 @@ int main(int argc, char **argv)
             if (prod[x] % p != mulmod(acc, n % p, p)) { bad++; std::printf("convolution fails, prime %d index %zu\n", t, x); break; }
         }
     }
-    // (2) CRT constants: value v in (-B, B) from its residues, as ks32_crt_kernel evaluates it
+    // (2) CRT constants: value v in (-B, B) from its residues, as ks32_crt_kernel evaluates it; the first trials are the exact
+    // extremes +-L n (q_J - 1)(q_I - 1) with the largest primes (what all-(q - 1) digits and keys reach), then random magnitudes
     u128 Bound = static_cast<u128>(k - 1) * n;
-    for (int trial = 0; trial < 2000; trial++)
+    const u64 qmax = *std::max_element(q.begin(), q.end());
+    for (int trial = 0; trial < 2000 + 2 * static_cast<int>(k); trial++)
     {
-        // v = +- (a * b) with a, b < max q: stays far inside the 256-bit range of this test? use a 2-limb magnitude instead
-        const u64 m1 = rng() % q[k - 1], m2 = rng() % q[0];
-        const bool neg = rng() & 1;
-        const u64 mult = rng() % static_cast<u64>(Bound); // |v| = m1 * m2 * mult < L n q q
-        const size_t i = rng() % k;
+        const bool extreme = trial < 2 * static_cast<int>(k);
+        // v = +- m1 * m2 * mult, |v| <= L n (max q - 1)^2
+        const u64 m1 = extreme ? qmax - 1 : rng() % q[k - 1], m2 = extreme ? qmax - 1 : rng() % q[0];
+        const bool neg = extreme ? (trial & 1) : (rng() & 1);
+        const u64 mult = extreme ? static_cast<u64>(Bound) : rng() % static_cast<u64>(Bound);
+        const size_t i = extreme ? static_cast<size_t>(trial >> 1) : rng() % k;
         const u64 qi = q[i];
         u64 vq = mulmod(mulmod(m1 % qi, m2 % qi, qi), mult % qi, qi);
         if (neg) vq = (qi - vq) % qi;
@@ -206,8 +210,19 @@ int main(int argc, char **argv)
         const int alpha = static_cast<int>(f >> 60);
         if (alpha < 0 || alpha >= h.S) { bad++; std::printf("alpha out of range\n"); break; }
         acc += h.neg_mod_q[i * h.S + alpha];
-        if (static_cast<u64>(acc % qi) != vq) { bad++; std::printf("CRT reconstruction fails (trial %d)\n", trial); break; }
+        if (static_cast<u64>(acc % qi) != vq) { bad++; std::printf("CRT reconstruction fails (trial %d%s)\n", trial, extreme ? ", extreme" : ""); break; }
     }
+    // (3) the product kernels' 64-bit sums: max_digits products of (max p - 1)^2 fit, one more does not
+    {
+        const u64 pm1 = *std::max_element(h.p.begin(), h.p.end()) - 1;
+        const u128 sq = static_cast<u128>(pm1) * pm1, lim = static_cast<u128>(1) << 64;
+        if (h.max_digits < 1 || static_cast<u128>(h.max_digits) * sq >= lim || static_cast<u128>(h.max_digits + 1) * sq < lim)
+            bad++, std::printf("max_digits %zu is not the largest L with L (p - 1)^2 < 2^64\n", h.max_digits);
+    }
+    std::printf("auxiliary primes:");
+    for (int t = 0; t < h.S; t++)
+        std::printf(" %u", h.p[t]);
+    std::printf("\nmax_digits %zu\n", h.max_digits);
     std::printf("ksint host check n=%zu S=%d r=%d: %s\n", n, h.S, h.r, bad ? "FAILED" : "ok");
     return bad ? 1 : 0;
 }

@@ -313,16 +313,51 @@ def test_batch_index_map_matches_oracle():
         assert (tt.ntt_row(0, oc.batch_codec(v, False)) == scattered).all()
 
 
+def _ksint_host_check(args):
+    cpp = os.path.join(ROOT, "tests", "cpp")
+    subprocess.check_call(["make", "-C", cpp, "ksint"], stdout=subprocess.DEVNULL)
+    r = subprocess.run([os.path.join(cpp, "_bin", "ksint_host_check")] + args, capture_output=True, text=True, timeout=600)
+    assert r.returncode == 0 and "ok" in r.stdout, r.stdout + r.stderr
+    lines = r.stdout.splitlines()
+    aux = [int(v) for v in next(x for x in lines if x.startswith("auxiliary primes:")).split(":")[1].split()]
+    max_digits = int(next(x for x in lines if x.startswith("max_digits")).split()[1])
+    return aux, max_digits
+
+
 @pytest.mark.parametrize("args", [["4096", "36", "36", "37"], ["8192", "55", "55", "55", "56"], ["16384", "60", "60", "60"],
-                                  ["32768"] + ["55"] * 16])
+                                  ["32768"] + ["55"] * 16, ["131072"] + ["60"] * 61, ["131072"] + ["60"] * 62])
 def test_ksint_host_tables_transforms_and_crt(args):
     """integer key-switching path (seal_b200/csrc/sb_ksint.cu): the tables sbh::build_ksint produces, driven on the CPU with
     the kernels' own index scheme, give transforms that invert each other and satisfy the convolution theorem, and CRT
-    constants that reconstruct signed integers inside the bound L n q^2 exactly (tests/cpp/ksint_host_check.cpp)"""
-    cpp = os.path.join(ROOT, "tests", "cpp")
-    subprocess.check_call(["make", "-C", cpp, "ksint"], stdout=subprocess.DEVNULL)
-    r = subprocess.run([os.path.join(cpp, "_bin", "ksint_host_check")] + args, capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0 and "ok" in r.stdout, r.stdout + r.stderr
+    constants that reconstruct signed integers inside the bound L n q^2 exactly, the extremes +-L n (max q - 1)^2 included
+    (tests/cpp/ksint_host_check.cpp).  In Python integers: P > 4 L n max q^2 and S is minimal (without the last auxiliary prime
+    the bound fails).  n = 131072 with 61 primes of 60 bits is the tightest five-prime case (0.02 bits of margin), 62 primes
+    need six."""
+    aux, _ = _ksint_host_check(args)
+    n = int(args[0])
+    mods = O.coeff_modulus_create(n, [int(b) for b in args[1:]])
+    L, qmax = len(mods) - 1, max(mods)
+    P = 1
+    for p in aux:
+        P *= p
+    assert P > 4 * L * n * qmax ** 2
+    assert P // aux[-1] <= 4 * L * n * qmax ** 2, "S is not minimal"
+    if n == 131072:
+        assert len(aux) == {61: 5, 62: 6}[len(mods)]
+
+
+def test_integer_path_accumulator_rule():
+    """the product kernels of the integer path (ks32_mac, ks32_mac_tile) sum L products of canonical words modulo an auxiliary
+    prime in 64 bits without a reduction: every level the path accepts (L <= sbh::KsIntHost::max_digits, Context::ksint_on) must
+    satisfy L (p_max - 1)^2 < 2^64, and max_digits is the largest such L, for every transform size.  At n = 4096 that is 64
+    digits: a context may have up to 256 primes, so deeper levels exist and take the 64-bit path."""
+    for logn in range(12, 18):
+        n = 1 << logn
+        aux, max_digits = _ksint_host_check([str(n), "30", "30", "30"])
+        pm1 = max(aux) - 1
+        assert max_digits * pm1 ** 2 < 2 ** 64 <= (max_digits + 1) * pm1 ** 2
+        if n == 4096:
+            assert max(aux) == 536813569 and max_digits == 64
 
 
 def test_ksint_swizzle_conflict_free():
