@@ -1,6 +1,8 @@
 // seal_b200/csrc/sb_api.cu -- the extern "C" boundary declared in include/seal_b200.h.
 // Exceptions never cross it: they are mapped to status codes the way the reference's C layer maps them to HRESULTs
-// (native/src/seal/c/defines.h:72-96) and the message is kept in a thread-local string.
+// (native/src/seal/c/defines.h:72-96) and the message is kept in a thread-local string.  The evaluator operations, the CKKS
+// encoder and the decryptor are each described once (what they check, their slab layout, their launch on a chunk of the batch)
+// and get their stream and host-buffer entry points from the two drivers on_stream and on_host.
 #include "../../include/seal_b200.h"
 #include "sb_engine.cuh"
 #include <random>
@@ -9,6 +11,7 @@
 #include <cstdio>
 #include <cstring>
 #include <new>
+#include <type_traits>
 #include <thread>
 
 using namespace sb;
@@ -696,6 +699,7 @@ int sb200_kswitch_key_destroy(sb200_kswitch_key *key)
     delete key;
     return SB200_OK;
 }
+} // extern "C"
 
 #define SB_ENTER(ctx)                                      \
     SB_NEED(ctx);                                          \
@@ -729,211 +733,17 @@ namespace
     SB_ENTER(ctx)                    \
     StreamOrder order_(c, static_cast<cudaStream_t>(stream));
 
+static void check_batch(size_t batch)
+{
+    if (batch == 0)
+        throw std::invalid_argument("batch must be positive");
+}
+
 static void check_level(const Context &c, size_t L, size_t batch)
 {
     if (L < 1 || L > c.k)
         throw std::invalid_argument("encrypted is not valid for encryption parameters");
-    if (batch == 0)
-        throw std::invalid_argument("batch must be positive");
-}
-
-int sb200_ntt_forward(sb200_context *ctx, size_t L, size_t size, size_t batch, uint64_t *d, void *stream)
-{
-    SB_NEED(d);
-    SB_TRY
-    SB_ENTER_STREAM(ctx, stream)
-    check_level(c, L, batch);
-    op_ntt(c, false, L, size, batch, reinterpret_cast<u64 *>(d), static_cast<cudaStream_t>(stream));
-    return SB200_OK;
-    SB_CATCH
-}
-
-int sb200_ntt_inverse(sb200_context *ctx, size_t L, size_t size, size_t batch, uint64_t *d, void *stream)
-{
-    SB_NEED(d);
-    SB_TRY
-    SB_ENTER_STREAM(ctx, stream)
-    check_level(c, L, batch);
-    op_ntt(c, true, L, size, batch, reinterpret_cast<u64 *>(d), static_cast<cudaStream_t>(stream));
-    return SB200_OK;
-    SB_CATCH
-}
-
-int sb200_multiply(sb200_context *ctx, size_t L, size_t batch, const uint64_t *a, const uint64_t *b, uint64_t *out3, void *stream)
-{
-    SB_NEED(a);
-    SB_NEED(b);
-    SB_NEED(out3);
-    SB_TRY
-    SB_ENTER_STREAM(ctx, stream)
-    check_level(c, L, batch);
-    auto st = static_cast<cudaStream_t>(stream);
-    if (c.scheme != SB200_SCHEME_BFV) // CKKS and BGV share the NTT-form tensor (evaluator.cpp:569-708, :710-841)
-        op_ckks_multiply(c, L, batch, (const u64 *)a, (const u64 *)b, (u64 *)out3, st);
-    else
-        op_bfv_multiply(c, L, batch, (const u64 *)a, (const u64 *)b, (u64 *)out3, st);
-    return SB200_OK;
-    SB_CATCH
-}
-
-int sb200_multiply_sized(sb200_context *ctx, size_t L, size_t size_a, size_t size_b, size_t batch, const uint64_t *a, const uint64_t *b,
-                         uint64_t *out, void *stream)
-{
-    SB_NEED(a);
-    SB_NEED(b);
-    SB_NEED(out);
-    SB_TRY
-    SB_ENTER_STREAM(ctx, stream)
-    check_level(c, L, batch);
-    if (out == a || out == b)
-        throw std::invalid_argument("multiply: the output slab must not alias an input slab");
-    auto st = static_cast<cudaStream_t>(stream);
-    if (c.scheme != SB200_SCHEME_BFV)
-        op_ckks_multiply(c, L, size_a, size_b, batch, (const u64 *)a, (const u64 *)b, (u64 *)out, st);
-    else
-        op_bfv_multiply(c, L, size_a, size_b, batch, (const u64 *)a, (const u64 *)b, (u64 *)out, st);
-    return SB200_OK;
-    SB_CATCH
-}
-
-static int linear_dev(sb200_context *ctx, int mode, size_t L, size_t size, size_t batch, const uint64_t *a, const uint64_t *b, uint64_t *out,
-                      void *stream)
-{
-    SB_NEED(a);
-    SB_NEED(out);
-    if (mode != 2)
-        SB_NEED(b);
-    SB_TRY
-    SB_ENTER_STREAM(ctx, stream)
-    check_level(c, L, batch);
-    op_linear(c, mode, L, size, batch, (const u64 *)a, (const u64 *)b, (u64 *)out, static_cast<cudaStream_t>(stream));
-    return SB200_OK;
-    SB_CATCH
-}
-int sb200_add(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, const uint64_t *b, uint64_t *out, void *stream)
-{
-    return linear_dev(ctx, 0, L, size, batch, a, b, out, stream);
-}
-int sb200_sub(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, const uint64_t *b, uint64_t *out, void *stream)
-{
-    return linear_dev(ctx, 1, L, size, batch, a, b, out, stream);
-}
-int sb200_negate(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, uint64_t *out, void *stream)
-{
-    return linear_dev(ctx, 2, L, size, batch, a, nullptr, out, stream);
-}
-int sb200_multiply_plain(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, const uint64_t *plain, uint64_t *out,
-                         void *stream)
-{
-    SB_NEED(a);
-    SB_NEED(plain);
-    SB_NEED(out);
-    SB_TRY
-    SB_ENTER_STREAM(ctx, stream)
-    check_level(c, L, batch);
-    op_multiply_plain(c, L, size, batch, (const u64 *)a, (const u64 *)plain, (u64 *)out, static_cast<cudaStream_t>(stream));
-    return SB200_OK;
-    SB_CATCH
-}
-int sb200_plain_to_ntt(sb200_context *ctx, size_t L, size_t batch, const uint64_t *plain, uint64_t *out, void *stream)
-{
-    SB_NEED(plain);
-    SB_NEED(out);
-    SB_TRY
-    SB_ENTER_STREAM(ctx, stream)
-    check_level(c, L, batch);
-    op_plain_to_ntt(c, L, batch, (const u64 *)plain, nullptr, (u64 *)out, static_cast<cudaStream_t>(stream));
-    return SB200_OK;
-    SB_CATCH
-}
-
-int sb200_multiply_plain_coeff(sb200_context *ctx, size_t L, size_t size, size_t batch, int ct_is_ntt, const uint64_t *a, const uint64_t *plain,
-                               uint64_t *out, void *stream)
-{
-    SB_NEED(a);
-    SB_NEED(plain);
-    SB_NEED(out);
-    SB_TRY
-    SB_ENTER_STREAM(ctx, stream)
-    check_level(c, L, batch);
-    op_multiply_plain_coeff(c, L, size, batch, ct_is_ntt != 0, (const u64 *)a, (const u64 *)plain, (u64 *)out, static_cast<cudaStream_t>(stream));
-    return SB200_OK;
-    SB_CATCH
-}
-
-int sb200_add_plain_coeff(sb200_context *ctx, size_t L, size_t size, size_t batch, int subtract, const uint64_t *a, const uint64_t *plain,
-                          const uint64_t *h_correction_factors, uint64_t *out, void *stream)
-{
-    SB_NEED(a);
-    SB_NEED(plain);
-    SB_NEED(out);
-    SB_TRY
-    SB_ENTER_STREAM(ctx, stream)
-    check_level(c, L, batch);
-    op_add_plain_coeff(c, L, size, batch, subtract != 0, (const u64 *)a, (const u64 *)plain, (const u64 *)h_correction_factors, (u64 *)out,
-                       static_cast<cudaStream_t>(stream));
-    return SB200_OK;
-    SB_CATCH
-}
-
-static int batch_codec_dev(sb200_context *ctx, bool decode, size_t batch, const uint64_t *in, uint64_t *out, void *stream)
-{
-    SB_NEED(in);
-    SB_NEED(out);
-    SB_TRY
-    SB_ENTER_STREAM(ctx, stream)
-    if (batch == 0)
-        throw std::invalid_argument("batch must be positive");
-    if (decode)
-        op_batch_decode(c, batch, (const u64 *)in, (u64 *)out, static_cast<cudaStream_t>(stream));
-    else
-        op_batch_encode(c, batch, (const u64 *)in, (u64 *)out, static_cast<cudaStream_t>(stream));
-    return SB200_OK;
-    SB_CATCH
-}
-int sb200_batch_encode(sb200_context *ctx, size_t batch, const uint64_t *values, uint64_t *plain, void *stream)
-{
-    return batch_codec_dev(ctx, false, batch, values, plain, stream);
-}
-int sb200_batch_decode(sb200_context *ctx, size_t batch, const uint64_t *plain, uint64_t *values, void *stream)
-{
-    return batch_codec_dev(ctx, true, batch, plain, values, stream);
-}
-
-int sb200_square(sb200_context *ctx, size_t L, size_t batch, const uint64_t *a, uint64_t *out3, void *stream)
-{
-    return sb200_multiply(ctx, L, batch, a, a, out3, stream);
-}
-
-int sb200_relinearize(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in3, const sb200_kswitch_key *key, uint64_t *out2,
-                      void *stream)
-{
-    SB_NEED(in3);
-    SB_NEED(key);
-    SB_NEED(out2);
-    SB_TRY
-    SB_ENTER_STREAM(ctx, stream)
-    check_level(c, L, batch);
-    if (static_cast<const void *>(in3) == static_cast<const void *>(out2))
-        throw std::invalid_argument("relinearize: input and output slabs must not alias (different layouts)");
-    op_relinearize(c, L, batch, (const u64 *)in3, key->k, (u64 *)out2, static_cast<cudaStream_t>(stream));
-    return SB200_OK;
-    SB_CATCH
-}
-
-int sb200_multiply_relinearize(sb200_context *ctx, size_t L, size_t batch, const uint64_t *a, const uint64_t *b,
-                               const sb200_kswitch_key *key, uint64_t *out2, void *stream)
-{
-    SB_NEED(a);
-    SB_NEED(b);
-    SB_NEED(key);
-    SB_NEED(out2);
-    SB_TRY
-    SB_ENTER_STREAM(ctx, stream)
-    check_level(c, L, batch);
-    op_multiply_relinearize(c, L, batch, (const u64 *)a, (const u64 *)b, key->k, (u64 *)out2, static_cast<cudaStream_t>(stream));
-    return SB200_OK;
-    SB_CATCH
+    check_batch(batch);
 }
 
 static void check_size(size_t size)
@@ -942,83 +752,22 @@ static void check_size(size_t size)
         throw std::invalid_argument("invalid ciphertext size");
 }
 
-int sb200_rescale_to_next_sized(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *in, uint64_t *out, void *stream)
-{
-    SB_NEED(in);
-    SB_NEED(out);
-    SB_TRY
-    SB_ENTER_STREAM(ctx, stream)
-    check_level(c, L, batch);
-    check_size(size);
-    if (static_cast<const void *>(in) == static_cast<const void *>(out))
-        throw std::invalid_argument("rescale_to_next: input and output slabs must not alias (different layouts)");
-    op_rescale(c, L, batch * size, (const u64 *)in, (u64 *)out, static_cast<cudaStream_t>(stream));
-    return SB200_OK;
-    SB_CATCH
-}
-int sb200_rescale_to_next(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, uint64_t *out2, void *stream)
-{
-    return sb200_rescale_to_next_sized(ctx, L, 2, batch, in2, out2, stream);
-}
-
-int sb200_mod_switch_to_next_sized(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *in, uint64_t *out, void *stream)
-{
-    SB_NEED(in);
-    SB_NEED(out);
-    SB_TRY
-    SB_ENTER_STREAM(ctx, stream)
-    check_level(c, L, batch);
-    check_size(size);
-    if (static_cast<const void *>(in) == static_cast<const void *>(out))
-        throw std::invalid_argument("mod_switch_to_next: input and output slabs must not alias (different layouts)");
-    op_mod_switch(c, L, batch * size, (const u64 *)in, (u64 *)out, static_cast<cudaStream_t>(stream));
-    return SB200_OK;
-    SB_CATCH
-}
-int sb200_mod_switch_to_next(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, uint64_t *out2, void *stream)
-{
-    return sb200_mod_switch_to_next_sized(ctx, L, 2, batch, in2, out2, stream);
-}
-
-int sb200_relinearize_sized(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *in, const sb200_kswitch_key *key,
-                            uint64_t *out, void *stream)
-{
-    SB_NEED(in);
-    SB_NEED(key);
-    SB_NEED(out);
-    SB_TRY
-    SB_ENTER_STREAM(ctx, stream)
-    check_level(c, L, batch);
-    if (static_cast<const void *>(in) == static_cast<const void *>(out))
-        throw std::invalid_argument("relinearize: input and output slabs must not alias");
-    op_relinearize_sized(c, L, size, batch, (const u64 *)in, key->k, (u64 *)out, static_cast<cudaStream_t>(stream));
-    return SB200_OK;
-    SB_CATCH
-}
-
-int sb200_apply_galois(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, uint32_t elt, const sb200_kswitch_key *key,
-                       uint64_t *out2, void *stream)
-{
-    SB_NEED(in2);
-    SB_NEED(key);
-    SB_NEED(out2);
-    SB_TRY
-    SB_ENTER_STREAM(ctx, stream)
-    check_level(c, L, batch);
-    op_apply_galois(c, L, batch, (const u64 *)in2, elt, key->k, (u64 *)out2, static_cast<cudaStream_t>(stream));
-    return SB200_OK;
-    SB_CATCH
-}
-
-// ---- host-buffer variants ------------------------------------------------------------------------------------------
-// The batch is cut into chunks that flow through a 3-stage pipeline on three streams: H2D copy of chunk i+1 | kernels
-// of chunk i | D2H copy of chunk i-1, double-buffered device staging owned by the context (PCIe is full duplex, so with
-// pinned host buffers both copy directions overlap each other and the compute).  Pageable host memory works too, the
-// copies then serialise inside the driver.
-} // extern "C"
-
+// ---- evaluator operations, encoder and decryptor ---------------------------------------------------------------------
+// Each operation is described once: what it checks, the layout of one ciphertext's slabs, and the launch on a chunk of B
+// ciphertexts starting at ciphertext b0.  Two drivers turn a description into its entry points: on_stream (device slabs, the
+// whole batch in one launch on the caller's stream) and on_host (host buffers).  The host-buffer entry points cut the batch into
+// chunks that flow through a 3-stage pipeline on three streams: H2D copy of chunk i+1 | kernels of chunk i | D2H copy of chunk
+// i-1, double-buffered device staging owned by the context (PCIe is full duplex, so with pinned host buffers both copy
+// directions overlap each other and the compute).  Pageable host memory works too, the copies then serialise inside the driver.
 namespace
 {
+    struct Layout
+    {
+        size_t a, b, out;              // words per ciphertext of input a, input b (0 = none) and the output
+        bool in_place = false;         // the output overwrites input a (out = a)
+        const char *alias = nullptr;   // device slabs: the error when the output aliases an input (nullptr = allowed)
+    };
+
     struct HostPipe
     {
         Context &c;
@@ -1055,11 +804,11 @@ namespace
             }
             return io.buf[slot][which];
         }
-        // wa / wb / wo: words per ciphertext of input a, input b (0 = none), output (0 = in place in a)
-        template <class F>
-        void run(size_t batch, size_t wa, size_t wb, size_t wo, const uint64_t *ha, const uint64_t *hb, uint64_t *ho, F &&op)
+        template <class Op>
+        void run(size_t batch, const Layout &w, const u64 *ha, const u64 *hb, u64 *ho, const Op &op)
         {
             StreamOrder order(c, s_comp); // the operation's kernels (and the scratch arenas they use) run on s_comp
+            const size_t wa = w.a, wb = w.b, wo = w.in_place ? 0 : w.out;
             const size_t per_ct = (wa + wb + wo) * sizeof(u64);
             size_t chunk = std::max<size_t>(1, std::min<size_t>(batch, c.host_stage_bytes / std::max<size_t>(per_ct, 1)));
             if (chunk >= batch && batch >= 4)
@@ -1070,7 +819,7 @@ namespace
                 buffer(slot, 0, chunk * wa);
                 if (wb)
                     buffer(slot, 1, chunk * wb);
-                if (wo)
+                if (!w.in_place)
                     buffer(slot, 2, chunk * wo);
             }
             size_t i = 0;
@@ -1078,329 +827,548 @@ namespace
             {
                 const size_t B = std::min(chunk, batch - b0);
                 const int slot = static_cast<int>(i & 1);
-                u64 *da = buffer(slot, 0, B * wa), *db = wb ? buffer(slot, 1, B * wb) : nullptr, *dout = wo ? buffer(slot, 2, B * wo) : da;
+                u64 *da = buffer(slot, 0, B * wa), *db = wb ? buffer(slot, 1, B * wb) : nullptr, *dout = w.in_place ? da : buffer(slot, 2, B * wo);
                 if (i >= 2)
                 {
                     // inputs of this slot are free once its previous kernels finished (and, in place, once copied out)
-                    cuda_check(cudaStreamWaitEvent(s_in, wo ? ev_comp[slot] : ev_out[slot], 0), "wait");
+                    cuda_check(cudaStreamWaitEvent(s_in, w.in_place ? ev_out[slot] : ev_comp[slot], 0), "wait");
                 }
                 cuda_check(cudaMemcpyAsync(da, ha + b0 * wa, B * wa * sizeof(u64), cudaMemcpyHostToDevice, s_in), "H2D");
                 if (wb)
                     cuda_check(cudaMemcpyAsync(db, hb + b0 * wb, B * wb * sizeof(u64), cudaMemcpyHostToDevice, s_in), "H2D");
                 cuda_check(cudaEventRecord(ev_in[slot], s_in), "record");
                 cuda_check(cudaStreamWaitEvent(s_comp, ev_in[slot], 0), "wait");
-                if (i >= 2 && wo)
+                if (i >= 2 && !w.in_place)
                     cuda_check(cudaStreamWaitEvent(s_comp, ev_out[slot], 0), "wait"); // output staging of this slot drained
-                op(B, da, db, dout, s_comp);
+                op(c, b0, B, da, db, dout, s_comp);
                 cuda_check(cudaEventRecord(ev_comp[slot], s_comp), "record");
                 cuda_check(cudaStreamWaitEvent(s_out, ev_comp[slot], 0), "wait");
-                cuda_check(cudaMemcpyAsync(ho + b0 * (wo ? wo : wa), dout, B * (wo ? wo : wa) * sizeof(u64), cudaMemcpyDeviceToHost, s_out), "D2H");
+                cuda_check(cudaMemcpyAsync(ho + b0 * w.out, dout, B * w.out * sizeof(u64), cudaMemcpyDeviceToHost, s_out), "D2H");
                 cuda_check(cudaEventRecord(ev_out[slot], s_out), "record");
             }
             cuda_check(cudaStreamSynchronize(s_out), "synchronize");
             cuda_check(cudaStreamSynchronize(s_comp), "synchronize");
         }
     };
+
+    struct Ntt
+    {
+        bool inverse;
+        size_t L, size;
+        void check(const Context &c, size_t batch) const { check_level(c, L, batch); }
+        Layout layout(const Context &c) const { return { size * L * c.n, 0, size * L * c.n, true }; }
+        void operator()(Context &c, size_t, size_t B, const u64 *, const u64 *, u64 *out, cudaStream_t st) const { op_ntt(c, inverse, L, size, B, out, st); }
+    };
+
+    // two size-2 ciphertexts; square: b is a (one operand crosses the bus, the NTT-form schemes square with their own kernel when
+    // op_ckks_multiply sees a == b)
+    struct Multiply
+    {
+        size_t L;
+        bool square;
+        void check(const Context &c, size_t batch) const { check_level(c, L, batch); }
+        Layout layout(const Context &c) const { return { 2 * L * c.n, square ? 0 : 2 * L * c.n, 3 * L * c.n }; }
+        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *b, u64 *out, cudaStream_t st) const
+        {
+            if (square)
+                b = a;
+            if (c.scheme != SB200_SCHEME_BFV) // CKKS and BGV share the NTT-form tensor (evaluator.cpp:569-708, :710-841)
+                op_ckks_multiply(c, L, B, a, b, out, st);
+            else
+                op_bfv_multiply(c, L, B, a, b, out, st);
+        }
+    };
+
+    struct MultiplySized
+    {
+        size_t L, sa, sb;
+        void check(const Context &c, size_t batch) const
+        {
+            check_level(c, L, batch);
+            check_sizes(sa, sb);
+        }
+        Layout layout(const Context &c) const
+        {
+            return { sa * L * c.n, sb * L * c.n, (sa + sb - 1) * L * c.n, false, "multiply: the output slab must not alias an input slab" };
+        }
+        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *b, u64 *out, cudaStream_t st) const
+        {
+            if (c.scheme != SB200_SCHEME_BFV)
+                op_ckks_multiply(c, L, sa, sb, B, a, b, out, st);
+            else
+                op_bfv_multiply(c, L, sa, sb, B, a, b, out, st);
+        }
+    };
+
+    struct Linear // mode 0: a + b, 1: a - b, 2: -a
+    {
+        int mode;
+        size_t L, size;
+        void check(const Context &c, size_t batch) const { check_level(c, L, batch); }
+        Layout layout(const Context &c) const { return { size * L * c.n, mode == 2 ? 0 : size * L * c.n, size * L * c.n }; }
+        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *b, u64 *out, cudaStream_t st) const
+        {
+            op_linear(c, mode, L, size, B, a, b, out, st);
+        }
+    };
+
+    struct MultiplyPlain // b: NTT-form plaintexts [B][L][n]
+    {
+        size_t L, size;
+        void check(const Context &c, size_t batch) const { check_level(c, L, batch); }
+        Layout layout(const Context &c) const { return { size * L * c.n, L * c.n, size * L * c.n }; }
+        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *b, u64 *out, cudaStream_t st) const
+        {
+            op_multiply_plain(c, L, size, B, a, b, out, st);
+        }
+    };
+
+    struct PlainToNtt // a: coefficient-form plaintexts [B][n]
+    {
+        size_t L;
+        void check(const Context &c, size_t batch) const { check_level(c, L, batch); }
+        Layout layout(const Context &c) const { return { c.n, 0, L * c.n }; }
+        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
+        {
+            op_plain_to_ntt(c, L, B, a, nullptr, out, st);
+        }
+    };
+
+    struct MultiplyPlainCoeff // b: coefficient-form plaintexts [B][n]
+    {
+        size_t L, size;
+        bool ct_is_ntt;
+        void check(const Context &c, size_t batch) const { check_level(c, L, batch); }
+        Layout layout(const Context &c) const { return { size * L * c.n, c.n, size * L * c.n }; }
+        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *b, u64 *out, cudaStream_t st) const
+        {
+            op_multiply_plain_coeff(c, L, size, B, ct_is_ntt, a, b, out, st);
+        }
+    };
+
+    struct AddPlainCoeff // b: coefficient-form plaintexts [B][n]; cf: BGV correction factors on the host, one per ciphertext
+    {
+        size_t L, size;
+        bool subtract;
+        const u64 *cf;
+        void check(const Context &c, size_t batch) const { check_level(c, L, batch); }
+        Layout layout(const Context &c) const { return { size * L * c.n, c.n, size * L * c.n }; }
+        void operator()(Context &c, size_t b0, size_t B, const u64 *a, const u64 *b, u64 *out, cudaStream_t st) const
+        {
+            op_add_plain_coeff(c, L, size, B, subtract, a, b, cf ? cf + b0 : nullptr, out, st);
+        }
+    };
+
+    struct BatchCodec // values [B][n] <-> coefficient-form plaintexts [B][n]
+    {
+        bool decode;
+        void check(const Context &, size_t batch) const { check_batch(batch); }
+        Layout layout(const Context &c) const { return { c.n, 0, c.n }; }
+        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
+        {
+            if (decode)
+                op_batch_decode(c, B, a, out, st);
+            else
+                op_batch_encode(c, B, a, out, st);
+        }
+    };
+
+    struct Relinearize
+    {
+        size_t L;
+        const KSwitchKey &key;
+        void check(const Context &c, size_t batch) const { check_level(c, L, batch); }
+        Layout layout(const Context &c) const
+        {
+            return { 3 * L * c.n, 0, 2 * L * c.n, false, "relinearize: input and output slabs must not alias (different layouts)" };
+        }
+        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
+        {
+            op_relinearize(c, L, B, a, key, out, st);
+        }
+    };
+
+    struct MultiplyRelinearize
+    {
+        size_t L;
+        const KSwitchKey &key;
+        void check(const Context &c, size_t batch) const { check_level(c, L, batch); }
+        Layout layout(const Context &c) const { return { 2 * L * c.n, 2 * L * c.n, 2 * L * c.n }; }
+        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *b, u64 *out, cudaStream_t st) const
+        {
+            op_multiply_relinearize(c, L, B, a, b, key, out, st);
+        }
+    };
+
+    struct RelinearizeSized // one step of relinearize_internal's loop: (c_0, c_1) += switch_key(c_{size-1}), size unchanged
+    {
+        size_t L, size;
+        const KSwitchKey &key;
+        void check(const Context &c, size_t batch) const
+        {
+            check_level(c, L, batch);
+            check_size(size);
+        }
+        Layout layout(const Context &c) const
+        {
+            return { size * L * c.n, 0, size * L * c.n, false, "relinearize: input and output slabs must not alias" };
+        }
+        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
+        {
+            op_relinearize_sized(c, L, size, B, a, key, out, st);
+        }
+    };
+
+    struct ApplyGalois
+    {
+        size_t L;
+        uint32_t elt;
+        const KSwitchKey &key;
+        void check(const Context &c, size_t batch) const { check_level(c, L, batch); }
+        Layout layout(const Context &c) const { return { 2 * L * c.n, 0, 2 * L * c.n }; }
+        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
+        {
+            op_apply_galois(c, L, B, a, elt, key, out, st);
+        }
+    };
+
+    struct ModSwitch // rescale_to_next (CKKS) or mod_switch_to_next of ciphertexts of any size: L primes -> L - 1
+    {
+        bool rescale;
+        size_t L, size;
+        void check(const Context &c, size_t batch) const
+        {
+            check_level(c, L, batch);
+            check_size(size);
+            if (L < 2) // before the scheme, as the reference checks it (evaluator.cpp:1521, :1533)
+                throw std::invalid_argument("end of modulus switching chain reached");
+        }
+        Layout layout(const Context &c) const
+        {
+            return { size * L * c.n, 0, size * (L - 1) * c.n, false,
+                     rescale ? "rescale_to_next: input and output slabs must not alias (different layouts)"
+                             : "mod_switch_to_next: input and output slabs must not alias (different layouts)" };
+        }
+        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
+        {
+            if (rescale)
+                op_rescale(c, L, B * size, a, out, st);
+            else
+                op_mod_switch(c, L, B * size, a, out, st);
+        }
+    };
+
+    struct CkksEncode // a: values, count doubles (reals) or count (re, im) pairs per plaintext; may be null when count = 0
+    {
+        size_t L, count;
+        bool is_complex, has_values;
+        double scale;
+        void check(const Context &c, size_t batch) const
+        {
+            check_level(c, L, batch);
+            if (count && !has_values)
+                throw std::invalid_argument("values cannot be null");
+        }
+        Layout layout(const Context &c) const { return { count * (is_complex ? 2 : 1), 0, L * c.n }; }
+        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
+        {
+            op_ckks_encode(c, L, B, reinterpret_cast<const double *>(a), count, is_complex, scale, out, st);
+        }
+    };
+
+    struct CkksDecode // out: n / 2 complex values (n doubles) per plaintext
+    {
+        size_t L;
+        double scale;
+        void check(const Context &c, size_t batch) const { check_level(c, L, batch); }
+        Layout layout(const Context &c) const { return { L * c.n, 0, c.n }; }
+        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
+        {
+            op_ckks_decode(c, L, B, a, scale, reinterpret_cast<double *>(out), st);
+        }
+    };
+
+    struct Decrypt // out: CKKS NTT-form plaintexts [B][L][n], BFV / BGV coefficient-form plaintexts [B][n]; cf as in AddPlainCoeff
+    {
+        SecretKey &key;
+        size_t L, size;
+        const u64 *cf;
+        void check(const Context &c, size_t batch) const { check_level(c, L, batch); }
+        Layout layout(const Context &c) const { return { size * L * c.n, 0, c.scheme == SB200_SCHEME_CKKS ? L * c.n : c.n }; }
+        void operator()(Context &c, size_t b0, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
+        {
+            op_decrypt(c, key, L, size, B, a, cf ? cf + b0 : nullptr, out, st);
+        }
+    };
+
+    // an entry point's own last step, inside its lock and stream order (the decryption wipes)
+    using Then = void (*)(Context &c, cudaStream_t st);
+
+    template <class Op>
+    int on_stream(sb200_context *ctx, void *stream, size_t batch, const void *a, const void *b, void *out, const Op &op, Then then = nullptr)
+    {
+        if (!std::is_same<Op, CkksEncode>::value) // the encoder takes no values for an empty vector (checked by CkksEncode)
+            SB_NEED(a);
+        SB_NEED(out);
+        SB_TRY
+        SB_ENTER_STREAM(ctx, stream)
+        op.check(c, batch);
+        const Layout w = op.layout(c);
+        if (w.alias && (out == a || out == b))
+            throw std::invalid_argument(w.alias);
+        auto st = static_cast<cudaStream_t>(stream);
+        op(c, 0, batch, static_cast<const u64 *>(a), static_cast<const u64 *>(b), static_cast<u64 *>(out), st);
+        if (then)
+            then(c, st);
+        return SB200_OK;
+        SB_CATCH
+    }
+
+    template <class Op>
+    int on_host(sb200_context *ctx, size_t batch, const void *a, const void *b, void *out, const Op &op, Then then = nullptr)
+    {
+        if (!std::is_same<Op, CkksEncode>::value)
+            SB_NEED(a);
+        SB_NEED(out);
+        SB_TRY
+        SB_ENTER(ctx)
+        op.check(c, batch);
+        HostPipe(c).run(batch, op.layout(c), static_cast<const u64 *>(a), static_cast<const u64 *>(b), static_cast<u64 *>(out), op);
+        if (then)
+            then(c, c.io.s_comp);
+        return SB200_OK;
+        SB_CATCH
+    }
 } // namespace
 
 extern "C" {
 
-static int ntt_host(sb200_context *ctx, bool inverse, size_t L, size_t size, size_t batch, uint64_t *h)
+int sb200_ntt_forward(sb200_context *ctx, size_t L, size_t size, size_t batch, uint64_t *d, void *stream)
 {
-    SB_NEED(h);
-    SB_TRY
-    SB_ENTER(ctx)
-    check_level(c, L, batch);
-    HostPipe(c).run(batch, size * L * c.n, 0, 0, h, nullptr, h,
-                    [&](size_t B, u64 *da, u64 *, u64 *, cudaStream_t st) { op_ntt(c, inverse, L, size, B, da, st); });
-    return SB200_OK;
-    SB_CATCH
+    return on_stream(ctx, stream, batch, d, nullptr, d, Ntt{ false, L, size });
 }
 int sb200_ntt_forward_host(sb200_context *ctx, size_t L, size_t size, size_t batch, uint64_t *h)
 {
-    return ntt_host(ctx, false, L, size, batch, h);
+    return on_host(ctx, batch, h, nullptr, h, Ntt{ false, L, size });
+}
+int sb200_ntt_inverse(sb200_context *ctx, size_t L, size_t size, size_t batch, uint64_t *d, void *stream)
+{
+    return on_stream(ctx, stream, batch, d, nullptr, d, Ntt{ true, L, size });
 }
 int sb200_ntt_inverse_host(sb200_context *ctx, size_t L, size_t size, size_t batch, uint64_t *h)
 {
-    return ntt_host(ctx, true, L, size, batch, h);
+    return on_host(ctx, batch, h, nullptr, h, Ntt{ true, L, size });
 }
 
+int sb200_multiply(sb200_context *ctx, size_t L, size_t batch, const uint64_t *a, const uint64_t *b, uint64_t *out3, void *stream)
+{
+    SB_NEED(b);
+    return on_stream(ctx, stream, batch, a, b, out3, Multiply{ L, false });
+}
 int sb200_multiply_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *a, const uint64_t *b, uint64_t *out3)
 {
-    SB_NEED(a);
     SB_NEED(b);
-    SB_NEED(out3);
-    SB_TRY
-    SB_ENTER(ctx)
-    check_level(c, L, batch);
-    const size_t w = L * c.n;
-    HostPipe(c).run(batch, 2 * w, 2 * w, 3 * w, a, b, out3, [&](size_t B, u64 *da, u64 *db, u64 *dout, cudaStream_t st) {
-        if (c.scheme != SB200_SCHEME_BFV)
-            op_ckks_multiply(c, L, B, da, db, dout, st);
-        else
-            op_bfv_multiply(c, L, B, da, db, dout, st);
-    });
-    return SB200_OK;
-    SB_CATCH
+    return on_host(ctx, batch, a, b, out3, Multiply{ L, false });
+}
+int sb200_square(sb200_context *ctx, size_t L, size_t batch, const uint64_t *a, uint64_t *out3, void *stream)
+{
+    return on_stream(ctx, stream, batch, a, nullptr, out3, Multiply{ L, true });
+}
+int sb200_square_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *a, uint64_t *out3)
+{
+    return on_host(ctx, batch, a, nullptr, out3, Multiply{ L, true });
 }
 
+int sb200_multiply_sized(sb200_context *ctx, size_t L, size_t size_a, size_t size_b, size_t batch, const uint64_t *a, const uint64_t *b,
+                         uint64_t *out, void *stream)
+{
+    SB_NEED(b);
+    return on_stream(ctx, stream, batch, a, b, out, MultiplySized{ L, size_a, size_b });
+}
 int sb200_multiply_sized_host(sb200_context *ctx, size_t L, size_t size_a, size_t size_b, size_t batch, const uint64_t *a, const uint64_t *b,
                               uint64_t *out)
 {
-    SB_NEED(a);
     SB_NEED(b);
-    SB_NEED(out);
-    SB_TRY
-    SB_ENTER(ctx)
-    check_level(c, L, batch);
-    check_sizes(size_a, size_b);
-    const size_t w = L * c.n;
-    HostPipe(c).run(batch, size_a * w, size_b * w, (size_a + size_b - 1) * w, a, b, out,
-                    [&](size_t B, u64 *da, u64 *db, u64 *dout, cudaStream_t st) {
-                        if (c.scheme != SB200_SCHEME_BFV)
-                            op_ckks_multiply(c, L, size_a, size_b, B, da, db, dout, st);
-                        else
-                            op_bfv_multiply(c, L, size_a, size_b, B, da, db, dout, st);
-                    });
-    return SB200_OK;
-    SB_CATCH
+    return on_host(ctx, batch, a, b, out, MultiplySized{ L, size_a, size_b });
 }
 
-static int linear_host(sb200_context *ctx, int mode, size_t L, size_t size, size_t batch, const uint64_t *a, const uint64_t *b, uint64_t *out)
+int sb200_add(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, const uint64_t *b, uint64_t *out, void *stream)
 {
-    SB_NEED(a);
-    SB_NEED(out);
-    if (mode != 2)
-        SB_NEED(b);
-    SB_TRY
-    SB_ENTER(ctx)
-    check_level(c, L, batch);
-    const size_t w = size * L * c.n;
-    HostPipe(c).run(batch, w, mode == 2 ? 0 : w, w, a, b, out,
-                    [&](size_t B, u64 *da, u64 *db, u64 *dout, cudaStream_t st) { op_linear(c, mode, L, size, B, da, db, dout, st); });
-    return SB200_OK;
-    SB_CATCH
+    SB_NEED(b);
+    return on_stream(ctx, stream, batch, a, b, out, Linear{ 0, L, size });
 }
 int sb200_add_host(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, const uint64_t *b, uint64_t *out)
 {
-    return linear_host(ctx, 0, L, size, batch, a, b, out);
+    SB_NEED(b);
+    return on_host(ctx, batch, a, b, out, Linear{ 0, L, size });
+}
+int sb200_sub(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, const uint64_t *b, uint64_t *out, void *stream)
+{
+    SB_NEED(b);
+    return on_stream(ctx, stream, batch, a, b, out, Linear{ 1, L, size });
 }
 int sb200_sub_host(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, const uint64_t *b, uint64_t *out)
 {
-    return linear_host(ctx, 1, L, size, batch, a, b, out);
+    SB_NEED(b);
+    return on_host(ctx, batch, a, b, out, Linear{ 1, L, size });
+}
+int sb200_negate(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, uint64_t *out, void *stream)
+{
+    return on_stream(ctx, stream, batch, a, nullptr, out, Linear{ 2, L, size });
 }
 int sb200_negate_host(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, uint64_t *out)
 {
-    return linear_host(ctx, 2, L, size, batch, a, nullptr, out);
+    return on_host(ctx, batch, a, nullptr, out, Linear{ 2, L, size });
+}
+
+int sb200_multiply_plain(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, const uint64_t *plain, uint64_t *out,
+                         void *stream)
+{
+    SB_NEED(plain);
+    return on_stream(ctx, stream, batch, a, plain, out, MultiplyPlain{ L, size });
 }
 int sb200_multiply_plain_host(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, const uint64_t *plain, uint64_t *out)
 {
-    SB_NEED(a);
     SB_NEED(plain);
-    SB_NEED(out);
-    SB_TRY
-    SB_ENTER(ctx)
-    check_level(c, L, batch);
-    const size_t w = L * c.n;
-    HostPipe(c).run(batch, size * w, w, size * w, a, plain, out,
-                    [&](size_t B, u64 *da, u64 *db, u64 *dout, cudaStream_t st) { op_multiply_plain(c, L, size, B, da, db, dout, st); });
-    return SB200_OK;
-    SB_CATCH
+    return on_host(ctx, batch, a, plain, out, MultiplyPlain{ L, size });
+}
+
+int sb200_plain_to_ntt(sb200_context *ctx, size_t L, size_t batch, const uint64_t *plain, uint64_t *out, void *stream)
+{
+    return on_stream(ctx, stream, batch, plain, nullptr, out, PlainToNtt{ L });
 }
 int sb200_plain_to_ntt_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *plain, uint64_t *out)
 {
-    SB_NEED(plain);
-    SB_NEED(out);
-    SB_TRY
-    SB_ENTER(ctx)
-    check_level(c, L, batch);
-    HostPipe(c).run(batch, c.n, 0, L * c.n, plain, nullptr, out,
-                    [&](size_t B, u64 *da, u64 *, u64 *dout, cudaStream_t st) { op_plain_to_ntt(c, L, B, da, nullptr, dout, st); });
-    return SB200_OK;
-    SB_CATCH
+    return on_host(ctx, batch, plain, nullptr, out, PlainToNtt{ L });
 }
 
+int sb200_multiply_plain_coeff(sb200_context *ctx, size_t L, size_t size, size_t batch, int ct_is_ntt, const uint64_t *a, const uint64_t *plain,
+                               uint64_t *out, void *stream)
+{
+    SB_NEED(plain);
+    return on_stream(ctx, stream, batch, a, plain, out, MultiplyPlainCoeff{ L, size, ct_is_ntt != 0 });
+}
 int sb200_multiply_plain_coeff_host(sb200_context *ctx, size_t L, size_t size, size_t batch, int ct_is_ntt, const uint64_t *a,
                                     const uint64_t *plain, uint64_t *out)
 {
-    SB_NEED(a);
     SB_NEED(plain);
-    SB_NEED(out);
-    SB_TRY
-    SB_ENTER(ctx)
-    check_level(c, L, batch);
-    const size_t w = size * L * c.n;
-    HostPipe(c).run(batch, w, c.n, w, a, plain, out, [&](size_t B, u64 *da, u64 *db, u64 *dout, cudaStream_t st) {
-        op_multiply_plain_coeff(c, L, size, B, ct_is_ntt != 0, da, db, dout, st);
-    });
-    return SB200_OK;
-    SB_CATCH
+    return on_host(ctx, batch, a, plain, out, MultiplyPlainCoeff{ L, size, ct_is_ntt != 0 });
 }
 
+int sb200_add_plain_coeff(sb200_context *ctx, size_t L, size_t size, size_t batch, int subtract, const uint64_t *a, const uint64_t *plain,
+                          const uint64_t *h_correction_factors, uint64_t *out, void *stream)
+{
+    SB_NEED(plain);
+    return on_stream(ctx, stream, batch, a, plain, out, AddPlainCoeff{ L, size, subtract != 0, (const u64 *)h_correction_factors });
+}
 int sb200_add_plain_coeff_host(sb200_context *ctx, size_t L, size_t size, size_t batch, int subtract, const uint64_t *a, const uint64_t *plain,
                                const uint64_t *h_correction_factors, uint64_t *out)
 {
-    SB_NEED(a);
     SB_NEED(plain);
-    SB_NEED(out);
-    SB_TRY
-    SB_ENTER(ctx)
-    check_level(c, L, batch);
-    const size_t w = size * L * c.n;
-    size_t done = 0; // chunks arrive in order: the correction factors advance with them
-    HostPipe(c).run(batch, w, c.n, w, a, plain, out, [&](size_t B, u64 *da, u64 *db, u64 *dout, cudaStream_t st) {
-        op_add_plain_coeff(c, L, size, B, subtract != 0, da, db, h_correction_factors ? (const u64 *)h_correction_factors + done : nullptr, dout,
-                           st);
-        done += B;
-    });
-    return SB200_OK;
-    SB_CATCH
+    return on_host(ctx, batch, a, plain, out, AddPlainCoeff{ L, size, subtract != 0, (const u64 *)h_correction_factors });
 }
 
-static int batch_codec_host(sb200_context *ctx, bool decode, size_t batch, const uint64_t *in, uint64_t *out)
+int sb200_batch_encode(sb200_context *ctx, size_t batch, const uint64_t *values, uint64_t *plain, void *stream)
 {
-    SB_NEED(in);
-    SB_NEED(out);
-    SB_TRY
-    SB_ENTER(ctx)
-    if (batch == 0)
-        throw std::invalid_argument("batch must be positive");
-    HostPipe(c).run(batch, c.n, 0, c.n, in, nullptr, out, [&](size_t B, u64 *da, u64 *, u64 *dout, cudaStream_t st) {
-        if (decode)
-            op_batch_decode(c, B, da, dout, st);
-        else
-            op_batch_encode(c, B, da, dout, st);
-    });
-    return SB200_OK;
-    SB_CATCH
+    return on_stream(ctx, stream, batch, values, nullptr, plain, BatchCodec{ false });
 }
 int sb200_batch_encode_host(sb200_context *ctx, size_t batch, const uint64_t *values, uint64_t *plain)
 {
-    return batch_codec_host(ctx, false, batch, values, plain);
+    return on_host(ctx, batch, values, nullptr, plain, BatchCodec{ false });
+}
+int sb200_batch_decode(sb200_context *ctx, size_t batch, const uint64_t *plain, uint64_t *values, void *stream)
+{
+    return on_stream(ctx, stream, batch, plain, nullptr, values, BatchCodec{ true });
 }
 int sb200_batch_decode_host(sb200_context *ctx, size_t batch, const uint64_t *plain, uint64_t *values)
 {
-    return batch_codec_host(ctx, true, batch, plain, values);
+    return on_host(ctx, batch, plain, nullptr, values, BatchCodec{ true });
 }
 
-int sb200_square_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *a, uint64_t *out3)
+int sb200_relinearize(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in3, const sb200_kswitch_key *key, uint64_t *out2,
+                      void *stream)
 {
-    SB_NEED(a);
-    SB_NEED(out3);
-    SB_TRY
-    SB_ENTER(ctx)
-    check_level(c, L, batch);
-    const size_t w = L * c.n;
-    // one operand crosses the bus; the NTT-form schemes square with their own kernel (op_ckks_multiply sees a == b)
-    HostPipe(c).run(batch, 2 * w, 0, 3 * w, a, nullptr, out3, [&](size_t B, u64 *da, u64 *, u64 *dout, cudaStream_t st) {
-        if (c.scheme != SB200_SCHEME_BFV)
-            op_ckks_multiply(c, L, B, da, da, dout, st);
-        else
-            op_bfv_multiply(c, L, B, da, da, dout, st);
-    });
-    return SB200_OK;
-    SB_CATCH
+    SB_NEED(key);
+    return on_stream(ctx, stream, batch, in3, nullptr, out2, Relinearize{ L, key->k });
 }
-
 int sb200_relinearize_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in3, const sb200_kswitch_key *key, uint64_t *out2)
 {
-    SB_NEED(in3);
     SB_NEED(key);
-    SB_NEED(out2);
-    SB_TRY
-    SB_ENTER(ctx)
-    check_level(c, L, batch);
-    const size_t w = L * c.n;
-    HostPipe(c).run(batch, 3 * w, 0, 2 * w, in3, nullptr, out2,
-                    [&](size_t B, u64 *da, u64 *, u64 *dout, cudaStream_t st) { op_relinearize(c, L, B, da, key->k, dout, st); });
-    return SB200_OK;
-    SB_CATCH
+    return on_host(ctx, batch, in3, nullptr, out2, Relinearize{ L, key->k });
 }
 
+int sb200_multiply_relinearize(sb200_context *ctx, size_t L, size_t batch, const uint64_t *a, const uint64_t *b,
+                               const sb200_kswitch_key *key, uint64_t *out2, void *stream)
+{
+    SB_NEED(b);
+    SB_NEED(key);
+    return on_stream(ctx, stream, batch, a, b, out2, MultiplyRelinearize{ L, key->k });
+}
 int sb200_multiply_relinearize_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *a, const uint64_t *b,
                                     const sb200_kswitch_key *key, uint64_t *out2)
 {
-    SB_NEED(a);
     SB_NEED(b);
     SB_NEED(key);
-    SB_NEED(out2);
-    SB_TRY
-    SB_ENTER(ctx)
-    check_level(c, L, batch);
-    const size_t w = L * c.n;
-    HostPipe(c).run(batch, 2 * w, 2 * w, 2 * w, a, b, out2, [&](size_t B, u64 *da, u64 *db, u64 *dout, cudaStream_t st) {
-        op_multiply_relinearize(c, L, B, da, db, key->k, dout, st);
-    });
-    return SB200_OK;
-    SB_CATCH
+    return on_host(ctx, batch, a, b, out2, MultiplyRelinearize{ L, key->k });
 }
 
-static int modswitch_host(sb200_context *ctx, bool rescale, size_t L, size_t size, size_t batch, const uint64_t *in2, uint64_t *out2)
+int sb200_rescale_to_next_sized(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *in, uint64_t *out, void *stream)
 {
-    SB_NEED(in2);
-    SB_NEED(out2);
-    SB_TRY
-    SB_ENTER(ctx)
-    check_level(c, L, batch);
-    check_size(size);
-    if (L < 2)
-        throw std::invalid_argument("end of modulus switching chain reached");
-    HostPipe(c).run(batch, size * L * c.n, 0, size * (L - 1) * c.n, in2, nullptr, out2, [&](size_t B, u64 *da, u64 *, u64 *dout, cudaStream_t st) {
-        if (rescale)
-            op_rescale(c, L, B * size, da, dout, st);
-        else
-            op_mod_switch(c, L, B * size, da, dout, st);
-    });
-    return SB200_OK;
-    SB_CATCH
-}
-int sb200_rescale_to_next_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, uint64_t *out2)
-{
-    return modswitch_host(ctx, true, L, 2, batch, in2, out2);
-}
-int sb200_mod_switch_to_next_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, uint64_t *out2)
-{
-    return modswitch_host(ctx, false, L, 2, batch, in2, out2);
+    return on_stream(ctx, stream, batch, in, nullptr, out, ModSwitch{ true, L, size });
 }
 int sb200_rescale_to_next_sized_host(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *in, uint64_t *out)
 {
-    return modswitch_host(ctx, true, L, size, batch, in, out);
+    return on_host(ctx, batch, in, nullptr, out, ModSwitch{ true, L, size });
+}
+int sb200_rescale_to_next(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, uint64_t *out2, void *stream)
+{
+    return on_stream(ctx, stream, batch, in2, nullptr, out2, ModSwitch{ true, L, 2 });
+}
+int sb200_rescale_to_next_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, uint64_t *out2)
+{
+    return on_host(ctx, batch, in2, nullptr, out2, ModSwitch{ true, L, 2 });
+}
+int sb200_mod_switch_to_next_sized(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *in, uint64_t *out, void *stream)
+{
+    return on_stream(ctx, stream, batch, in, nullptr, out, ModSwitch{ false, L, size });
 }
 int sb200_mod_switch_to_next_sized_host(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *in, uint64_t *out)
 {
-    return modswitch_host(ctx, false, L, size, batch, in, out);
+    return on_host(ctx, batch, in, nullptr, out, ModSwitch{ false, L, size });
+}
+int sb200_mod_switch_to_next(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, uint64_t *out2, void *stream)
+{
+    return on_stream(ctx, stream, batch, in2, nullptr, out2, ModSwitch{ false, L, 2 });
+}
+int sb200_mod_switch_to_next_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, uint64_t *out2)
+{
+    return on_host(ctx, batch, in2, nullptr, out2, ModSwitch{ false, L, 2 });
+}
+
+int sb200_relinearize_sized(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *in, const sb200_kswitch_key *key,
+                            uint64_t *out, void *stream)
+{
+    SB_NEED(key);
+    return on_stream(ctx, stream, batch, in, nullptr, out, RelinearizeSized{ L, size, key->k });
 }
 int sb200_relinearize_sized_host(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *in, const sb200_kswitch_key *key,
                                  uint64_t *out)
 {
-    SB_NEED(in);
     SB_NEED(key);
-    SB_NEED(out);
-    SB_TRY
-    SB_ENTER(ctx)
-    check_level(c, L, batch);
-    check_size(size);
-    const size_t w = size * L * c.n;
-    HostPipe(c).run(batch, w, 0, w, in, nullptr, out,
-                    [&](size_t B, u64 *da, u64 *, u64 *dout, cudaStream_t st) { op_relinearize_sized(c, L, size, B, da, key->k, dout, st); });
-    return SB200_OK;
-    SB_CATCH
+    return on_host(ctx, batch, in, nullptr, out, RelinearizeSized{ L, size, key->k });
 }
 
+int sb200_apply_galois(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, uint32_t elt, const sb200_kswitch_key *key,
+                       uint64_t *out2, void *stream)
+{
+    SB_NEED(key);
+    return on_stream(ctx, stream, batch, in2, nullptr, out2, ApplyGalois{ L, elt, key->k });
+}
 int sb200_apply_galois_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, uint32_t elt, const sb200_kswitch_key *key,
                             uint64_t *out2)
 {
-    SB_NEED(in2);
     SB_NEED(key);
-    SB_NEED(out2);
-    SB_TRY
-    SB_ENTER(ctx)
-    check_level(c, L, batch);
-    const size_t w = 2 * L * c.n;
-    HostPipe(c).run(batch, w, 0, w, in2, nullptr, out2,
-                    [&](size_t B, u64 *da, u64 *, u64 *dout, cudaStream_t st) { op_apply_galois(c, L, B, da, elt, key->k, dout, st); });
-    return SB200_OK;
-    SB_CATCH
+    return on_host(ctx, batch, in2, nullptr, out2, ApplyGalois{ L, elt, key->k });
 }
 
 // ---- wire format (SURVEY 8f rank 3): Ciphertext::save / load, compr_mode none, between byte streams and device slabs ----
@@ -1615,78 +1583,21 @@ int sb200_encrypt_zero_asymmetric(sb200_context *ctx, sb200_public_key *key, siz
 int sb200_ckks_encode(sb200_context *ctx, size_t L, size_t batch, const double *d_values, size_t count, int is_complex, double scale,
                       uint64_t *d_plain, void *stream)
 {
-    SB_NEED(d_plain);
-    SB_TRY
-    SB_ENTER_STREAM(ctx, stream)
-    check_level(c, L, batch);
-    op_ckks_encode(c, L, batch, d_values, count, is_complex != 0, scale, (u64 *)d_plain, static_cast<cudaStream_t>(stream));
-    return SB200_OK;
-    SB_CATCH
+    return on_stream(ctx, stream, batch, d_values, nullptr, d_plain, CkksEncode{ L, count, is_complex != 0, d_values != nullptr, scale });
+}
+int sb200_ckks_encode_host(sb200_context *ctx, size_t L, size_t batch, const double *h_values, size_t count, int is_complex, double scale,
+                           uint64_t *h_plain)
+{
+    return on_host(ctx, batch, h_values, nullptr, h_plain, CkksEncode{ L, count, is_complex != 0, h_values != nullptr, scale });
 }
 
 int sb200_ckks_decode(sb200_context *ctx, size_t L, size_t batch, const uint64_t *d_plain, double scale, double *d_values, void *stream)
 {
-    SB_NEED(d_plain);
-    SB_NEED(d_values);
-    SB_TRY
-    SB_ENTER_STREAM(ctx, stream)
-    check_level(c, L, batch);
-    op_ckks_decode(c, L, batch, (const u64 *)d_plain, scale, d_values, static_cast<cudaStream_t>(stream));
-    return SB200_OK;
-    SB_CATCH
+    return on_stream(ctx, stream, batch, d_plain, nullptr, d_values, CkksDecode{ L, scale });
 }
-
-namespace
-{
-    struct DevBuf // scoped device allocation of the (not hot) host-buffer encoder entry points
-    {
-        void *p = nullptr;
-        explicit DevBuf(size_t bytes)
-        {
-            cuda_check(cudaMalloc(&p, bytes ? bytes : 16), "cudaMalloc");
-        }
-        ~DevBuf()
-        {
-            cudaFree(p);
-        }
-        DevBuf(const DevBuf &) = delete;
-        DevBuf &operator=(const DevBuf &) = delete;
-    };
-} // namespace
-
-int sb200_ckks_encode_host(sb200_context *ctx, size_t L, size_t batch, const double *h_values, size_t count, int is_complex, double scale,
-                           uint64_t *h_plain)
-{
-    SB_NEED(h_plain);
-    SB_TRY
-    SB_ENTER_STREAM(ctx, nullptr)
-    check_level(c, L, batch);
-    if (count && !h_values)
-        throw std::invalid_argument("values cannot be null");
-    const size_t vbytes = batch * count * (is_complex ? 16 : 8), pbytes = batch * L * c.n * sizeof(u64);
-    DevBuf v(vbytes), p(pbytes);
-    if (vbytes)
-        cuda_check(cudaMemcpy(v.p, h_values, vbytes, cudaMemcpyHostToDevice), "values H2D");
-    op_ckks_encode(c, L, batch, static_cast<const double *>(v.p), count, is_complex != 0, scale, static_cast<u64 *>(p.p), nullptr);
-    cuda_check(cudaMemcpy(h_plain, p.p, pbytes, cudaMemcpyDeviceToHost), "plain D2H");
-    return SB200_OK;
-    SB_CATCH
-}
-
 int sb200_ckks_decode_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *h_plain, double scale, double *h_values)
 {
-    SB_NEED(h_plain);
-    SB_NEED(h_values);
-    SB_TRY
-    SB_ENTER_STREAM(ctx, nullptr)
-    check_level(c, L, batch);
-    const size_t vbytes = batch * (c.n / 2) * 16, pbytes = batch * L * c.n * sizeof(u64);
-    DevBuf v(vbytes), p(pbytes);
-    cuda_check(cudaMemcpy(p.p, h_plain, pbytes, cudaMemcpyHostToDevice), "plain H2D");
-    op_ckks_decode(c, L, batch, static_cast<const u64 *>(p.p), scale, static_cast<double *>(v.p), nullptr);
-    cuda_check(cudaMemcpy(h_values, v.p, vbytes, cudaMemcpyDeviceToHost), "values D2H");
-    return SB200_OK;
-    SB_CATCH
+    return on_host(ctx, batch, h_plain, nullptr, h_values, CkksDecode{ L, scale });
 }
 
 // Encryptor::encrypt_zero_symmetric for a batch (sb_prng.cu); h_bootstrap_seeds == nullptr: fresh seeds from the OS entropy source,
@@ -1712,44 +1623,27 @@ int sb200_encrypt_zero_symmetric(sb200_context *ctx, sb200_secret_key *key, size
     SB_CATCH
 }
 
+// the decryption phases and plaintexts do not stay behind in the arenas (the reference decrypts inside a clear-on-destruction pool,
+// decryptor.cpp:106-109)
 int sb200_decrypt(sb200_context *ctx, sb200_secret_key *key, size_t L, size_t size, size_t batch, const uint64_t *ct,
                   const uint64_t *h_correction_factors, uint64_t *plain, void *stream)
 {
     SB_NEED(key);
-    SB_NEED(ct);
-    SB_NEED(plain);
-    SB_TRY
-    SB_ENTER_STREAM(ctx, stream)
-    check_level(c, L, batch);
-    op_decrypt(c, key->k, L, size, batch, (const u64 *)ct, (const u64 *)h_correction_factors, (u64 *)plain, static_cast<cudaStream_t>(stream));
-    c.wipe_scratch(static_cast<cudaStream_t>(stream)); // the decryption phases (decryptor.cpp:106-109 keeps them in a clearing pool)
-    return SB200_OK;
-    SB_CATCH
+    return on_stream(ctx, stream, batch, ct, nullptr, plain, Decrypt{ key->k, L, size, (const u64 *)h_correction_factors },
+                     [](Context &c, cudaStream_t st) { c.wipe_scratch(st); });
 }
 
 int sb200_decrypt_host(sb200_context *ctx, sb200_secret_key *key, size_t L, size_t size, size_t batch, const uint64_t *ct,
                        const uint64_t *h_correction_factors, uint64_t *plain)
 {
     SB_NEED(key);
-    SB_NEED(ct);
-    SB_NEED(plain);
-    SB_TRY
-    SB_ENTER(ctx)
-    check_level(c, L, batch);
-    const size_t wo = c.scheme == SB200_SCHEME_CKKS ? L * c.n : c.n;
-    size_t done = 0;
-    HostPipe(c).run(batch, size * L * c.n, 0, wo, ct, nullptr, plain, [&](size_t B, u64 *da, u64 *, u64 *dout, cudaStream_t st) {
-        op_decrypt(c, key->k, L, size, B, da, h_correction_factors ? (const u64 *)h_correction_factors + done : nullptr, dout, st);
-        done += B;
+    return on_host(ctx, batch, ct, nullptr, plain, Decrypt{ key->k, L, size, (const u64 *)h_correction_factors }, [](Context &c, cudaStream_t st) {
+        c.wipe_scratch(st);
+        for (int slot = 0; slot < 2; slot++) // and the output staging
+            if (c.io.buf[slot][2])
+                cuda_check(cudaMemsetAsync(c.io.buf[slot][2], 0, c.io.cap[slot][2] * sizeof(u64), st), "wipe staging");
+        cuda_check(cudaStreamSynchronize(st), "synchronize");
     });
-    // phases and plaintexts do not stay behind in the arenas (the reference decrypts inside a clear-on-destruction pool)
-    c.wipe_scratch(c.io.s_comp);
-    for (int slot = 0; slot < 2; slot++)
-        if (c.io.buf[slot][2])
-            cuda_check(cudaMemsetAsync(c.io.buf[slot][2], 0, c.io.cap[slot][2] * sizeof(u64), c.io.s_comp), "wipe staging");
-    cuda_check(cudaStreamSynchronize(c.io.s_comp), "synchronize");
-    return SB200_OK;
-    SB_CATCH
 }
 
 } // extern "C"

@@ -1,6 +1,8 @@
 """GPU parity tests proper (-m gpu): every call goes through the C-ABI of libseal_b200.so and is compared word for
 word with (i) committed golden vectors from the real reference, (ii) the plain-C oracle, (iii) the reference library
 itself (oracle/_ref/libsealref.so) where it travelled to the box.  Bar: bit-exact."""
+import ctypes as C
+
 import numpy as np
 import pytest
 
@@ -141,6 +143,119 @@ def test_bfv_keyswitch_vs_reference():
         assert (ms[i] == rb.mod_switch(L, a[i])).all()
 
 
+# The evaluator operations, encoder and decryptor each have a stream entry point sb200_<name> on device slabs and a host-buffer
+# entry point sb200_<name>_host with the same arguments minus the stream.  Argument order after the context handle: a / b are the
+# input slabs, out the output slab (NTT: a is transformed in place), cf host correction factors, flag the int argument.
+ABI_PAIRS = {
+    "ntt_forward": ("L", "size", "batch", "a"),
+    "ntt_inverse": ("L", "size", "batch", "a"),
+    "multiply": ("L", "batch", "a", "b", "out"),
+    "multiply_sized": ("L", "size_a", "size_b", "batch", "a", "b", "out"),
+    "square": ("L", "batch", "a", "out"),
+    "add": ("L", "size", "batch", "a", "b", "out"),
+    "sub": ("L", "size", "batch", "a", "b", "out"),
+    "negate": ("L", "size", "batch", "a", "out"),
+    "multiply_plain": ("L", "size", "batch", "a", "b", "out"),
+    "plain_to_ntt": ("L", "batch", "a", "out"),
+    "multiply_plain_coeff": ("L", "size", "batch", "flag", "a", "b", "out"),
+    "add_plain_coeff": ("L", "size", "batch", "flag", "a", "b", "cf", "out"),
+    "batch_encode": ("batch", "a", "out"),
+    "batch_decode": ("batch", "a", "out"),
+    "relinearize": ("L", "batch", "a", "key", "out"),
+    "multiply_relinearize": ("L", "batch", "a", "b", "key", "out"),
+    "rescale_to_next": ("L", "batch", "a", "out"),
+    "mod_switch_to_next": ("L", "batch", "a", "out"),
+    "rescale_to_next_sized": ("L", "size", "batch", "a", "out"),
+    "mod_switch_to_next_sized": ("L", "size", "batch", "a", "out"),
+    "relinearize_sized": ("L", "size", "batch", "a", "key", "out"),
+    "apply_galois": ("L", "batch", "a", "elt", "key", "out"),
+    "ckks_encode": ("L", "batch", "a", "count", "flag", "scale", "out"),
+    "ckks_decode": ("L", "batch", "a", "scale", "out"),
+    "decrypt": ("key", "L", "size", "batch", "a", "cf", "out"),
+}
+_ABI_SCALARS = {"L": C.c_size_t, "size": C.c_size_t, "size_a": C.c_size_t, "size_b": C.c_size_t, "batch": C.c_size_t, "count": C.c_size_t,
+                "flag": C.c_int, "elt": C.c_uint32, "scale": C.c_double}
+_abi_lib = None
+
+
+def abi_call(ctx_h, name, v, stream=None):
+    """sb200_<name>_host (stream None) or sb200_<name> on `stream`, arguments from v (pointers as c_void_p or None); returns the
+    status and sb200_last_error()"""
+    global _abi_lib
+    if _abi_lib is None:  # a handle of its own: no argtypes, every argument is passed with its C type
+        _abi_lib = C.CDLL(sb().LIB_PATH)
+        _abi_lib.sb200_last_error.restype = C.c_char_p
+    args = [ctx_h] + [_ABI_SCALARS[f](v[f]) if f in _ABI_SCALARS else v[f] for f in ABI_PAIRS[name]]
+    fn = getattr(_abi_lib, f"sb200_{name}_host" if stream is None else f"sb200_{name}")
+    rc = fn(*args) if stream is None else fn(*args, stream)
+    return rc, _abi_lib.sb200_last_error().decode()
+
+
+_PAIR_SCHEMES = {"plain_to_ntt": "bfv bgv", "multiply_plain_coeff": "bfv bgv", "add_plain_coeff": "bfv bgv", "batch_encode": "bfv bgv",
+                 "batch_decode": "bfv bgv", "rescale_to_next": "ckks", "rescale_to_next_sized": "ckks", "ckks_encode": "ckks", "ckks_decode": "ckks"}
+
+
+def _pair_inputs(name, ctx, rng, key, sk):
+    """seeded inputs of one call: slabs as uint64 arrays (values and complex outputs as their words), the rest as scalars / handles"""
+    n, mods, t, L, B = ctx.n, ctx.moduli, ctx.t, 2, 7
+    bgv = ctx.scheme == sb().BGV
+
+    def ct(size, lv=L):
+        return rand_ct(rng, mods, n, size, lv, B)
+
+    def zeros(*shape):
+        return np.zeros((B,) + shape, dtype=np.uint64)
+
+    def coeffs():
+        return rng.integers(0, t, (B, n), dtype=np.uint64)
+
+    cf = rng.integers(1, t, B, dtype=np.uint64) if bgv else None
+    v = dict(L=L, batch=B)
+    if name.startswith("ntt"):
+        v.update(size=2, a=ct(2))
+    elif name == "multiply":
+        v.update(a=ct(2), b=ct(2), out=zeros(3, L, n))
+    elif name == "multiply_sized":
+        v.update(L=1, size_a=3, size_b=2, a=ct(3, 1), b=ct(2, 1), out=zeros(4, 1, n))
+    elif name == "square":
+        v.update(a=ct(2), out=zeros(3, L, n))
+    elif name in ("add", "sub"):
+        v.update(size=2, a=ct(2), b=ct(2), out=zeros(2, L, n))
+    elif name == "negate":
+        v.update(size=2, a=ct(2), out=zeros(2, L, n))
+    elif name == "multiply_plain":
+        v.update(size=2, a=ct(2), b=ct(1)[:, 0].copy(), out=zeros(2, L, n))
+    elif name == "plain_to_ntt":
+        v.update(a=coeffs(), out=zeros(L, n))
+    elif name == "multiply_plain_coeff":
+        v.update(size=2, flag=int(bgv), a=ct(2), b=coeffs(), out=zeros(2, L, n))
+    elif name == "add_plain_coeff":
+        v.update(size=2, flag=1, a=ct(2), b=coeffs(), cf=cf, out=zeros(2, L, n))
+    elif name.startswith("batch_"):
+        v.update(a=coeffs(), out=zeros(n))
+    elif name == "relinearize":
+        v.update(a=ct(3), key=key, out=zeros(2, L, n))
+    elif name == "multiply_relinearize":
+        v.update(a=ct(2), b=ct(2), key=key, out=zeros(2, L, n))
+    elif name in ("rescale_to_next", "mod_switch_to_next"):
+        v.update(a=ct(2), out=zeros(2, L - 1, n))
+    elif name in ("rescale_to_next_sized", "mod_switch_to_next_sized"):
+        v.update(size=3, a=ct(3), out=zeros(3, L - 1, n))
+    elif name == "relinearize_sized":
+        v.update(size=4, a=ct(4), key=key, out=zeros(4, L, n))
+    elif name == "apply_galois":
+        v.update(a=ct(2), elt=3, key=key, out=zeros(2, L, n))
+    elif name == "ckks_encode":
+        count = n // 2 - 3
+        vals = (rng.standard_normal((B, count)) + 1j * rng.standard_normal((B, count))) * 100.0
+        v.update(a=np.ascontiguousarray(vals).view(np.uint64), count=count, flag=1, scale=2.0 ** 20, out=zeros(L, n))
+    elif name == "ckks_decode":
+        v.update(a=ct(1)[:, 0].copy(), scale=2.0 ** 20, out=zeros(n))  # n / 2 complex values: n words
+    elif name == "decrypt":
+        v.update(key=sk, size=3, a=ct(3), cf=cf, out=zeros(L, n) if ctx.scheme == sb().CKKS else zeros(n))
+    return v
+
+
 def test_device_api_matches_host_api():
     import torch
 
@@ -163,6 +278,42 @@ def test_device_api_matches_host_api():
     assert (out.cpu().numpy().view(np.uint64) == host).all()
     oc = O.Oracle(O.CKKS, n, mods)
     assert (host[0] == oc.multiply_relin(L, a[0], b[0], key)).all()
+
+
+@pytest.mark.parametrize("name", list(ABI_PAIRS))
+def test_stream_and_host_entry_points_agree(name):
+    """both entry points of every pair produce the same words: the host one through its chunked pipeline (batch 7 at a 64 KiB
+    staging limit: several chunks, most operations with a ragged last one), the stream one in one call on torch slabs"""
+    import torch
+
+    S = sb()
+    n, t = 256, 65537
+    mods = S.coeff_modulus_create(n, [40, 40, 40])
+    schemes = _PAIR_SCHEMES.get(name, "ckks bfv bgv").split()
+    for scheme in schemes:
+        sid = {"ckks": S.CKKS, "bfv": S.BFV, "bgv": S.BGV}[scheme]
+        ctx = S.Context(sid, n, mods, 0 if scheme == "ckks" else t)
+        ctx.set_limit(ctx.LIMIT_HOST_STAGE_BYTES, 1 << 16)
+        rng = np.random.default_rng((list(ABI_PAIRS).index(name), schemes.index(scheme)))
+        key = ctx.load_key(rng.integers(0, 1 << 39, (2, 2, 3, n), dtype=np.uint64))  # any residues < q work as a key for parity
+        sk = ctx.load_secret_key(rng.integers(0, 1 << 39, (3, n), dtype=np.uint64))
+        v = _pair_inputs(name, ctx, rng, key.h, sk.h)
+        outs = [f for f in ("a", "out") if f in ABI_PAIRS[name]][-1:]  # the NTT overwrites a
+        host = {f: v[f].copy() for f in ("a", "b", "out") if f in v}
+        dev = {f: torch.from_numpy(x.view(np.int64)).cuda() for f, x in host.items()}
+        cf = None if v.get("cf") is None else v["cf"].ctypes.data_as(C.c_void_p)
+        hv = dict(v, cf=cf, **{f: x.ctypes.data_as(C.c_void_p) for f, x in host.items()})
+        dv = dict(v, cf=cf, **{f: C.c_void_p(x.data_ptr()) for f, x in dev.items()})
+        before = ctx.launch_count
+        assert abi_call(ctx.h, name, dv, C.c_void_p(torch.cuda.current_stream().cuda_stream))[0] == 0, (name, scheme)
+        torch.cuda.synchronize()
+        # (the CKKS modulus switch drops the last prime with a device copy: no kernel)
+        assert ctx.launch_count > before or (name.startswith("mod_switch") and scheme == "ckks"), (name, scheme)
+        assert abi_call(ctx.h, name, hv)[0] == 0, (name, scheme)
+        for f in outs:
+            got = dev[f].cpu().numpy().view(np.uint64)
+            assert (host[f] != v[f]).any() if f == "a" else (host[f] != 0).any(), (name, scheme, "host output unchanged")
+            assert (got == host[f]).all(), (name, scheme)
 
 
 def test_one_context_on_two_streams():
@@ -601,10 +752,120 @@ def test_decrypt_vs_reference(scheme, n):
         assert (ctx.batch_decode(p) == slots).all()
 
 
+_INVALID, _BATCH = "encrypted is not valid for encryption parameters", "batch must be positive"
+# status and sb200_last_error() text of both entry points of a pair, per bad argument (pointer errors: the status only)
+_ABI_ERRORS = {
+    "null context": (-6, None),
+    "null a": (-6, None),
+    "null b": (-6, None),
+    "null out": (-6, None),
+    "null key": (-6, None),
+    "L = 0": (-1, _INVALID),
+    "L = k + 1": (-1, _INVALID),
+    "L = k": (-1, _INVALID),  # key switching: the key level carries no data
+    "batch = 0": (-1, _BATCH),
+}
+_ABI_BAD_SIZE = {  # the invalid size of each pair that takes one (the NTT transforms any number of polynomials)
+    "multiply_sized": ({"size_a": 1}, "invalid ciphertext sizes"),
+    "add": ({"size": 0}, _INVALID), "sub": ({"size": 0}, _INVALID), "negate": ({"size": 0}, _INVALID),
+    "multiply_plain": ({"size": 0}, _INVALID), "multiply_plain_coeff": ({"size": 0}, _INVALID),
+    "add_plain_coeff": ({"size": 0}, _INVALID), "decrypt": ({"size": 0}, _INVALID),
+    "rescale_to_next_sized": ({"size": 0}, "invalid ciphertext size"), "mod_switch_to_next_sized": ({"size": 0}, "invalid ciphertext size"),
+    "relinearize_sized": ({"size": 0}, "invalid ciphertext size"),
+}
+_ABI_ALIAS = {  # stream entry points that refuse an output slab aliasing an input slab (host buffers are staged apart)
+    "multiply_sized": "multiply: the output slab must not alias an input slab",
+    "relinearize": "relinearize: input and output slabs must not alias (different layouts)",
+    "relinearize_sized": "relinearize: input and output slabs must not alias",
+    "rescale_to_next": "rescale_to_next: input and output slabs must not alias (different layouts)",
+    "rescale_to_next_sized": "rescale_to_next: input and output slabs must not alias (different layouts)",
+    "mod_switch_to_next": "mod_switch_to_next: input and output slabs must not alias (different layouts)",
+    "mod_switch_to_next_sized": "mod_switch_to_next: input and output slabs must not alias (different layouts)",
+    "apply_galois": "apply_galois: in and out must not alias",
+    "batch_encode": "batch_encode: input and output must not alias",
+    "batch_decode": "batch_decode: input and output must not alias",
+}
+_END_OF_CHAIN = "end of modulus switching chain reached"
+
+
+def _abi_error_cases(name, k):
+    """(case, argument changes, expected status, expected text, variants) of one pair"""
+    order = ABI_PAIRS[name]
+    ks = name in ("relinearize", "multiply_relinearize", "relinearize_sized", "apply_galois")
+    cases = [("null context", {}, "both")]
+    cases += [(f"null {p}", {p: None}, "both") for p in ("a", "b", "out", "key") if p in order]
+    if "L" in order:
+        cases += [("L = 0", {"L": 0}, "both"), ("L = k", {"L": k}, "both") if ks else ("L = k + 1", {"L": k + 1}, "both")]
+    cases.append(("batch = 0", {"batch": 0}, "both"))
+    out = []
+    for case, change, variants in cases:
+        status, text = _ABI_ERRORS[case]
+        if name == "ckks_encode" and case == "null a":  # values may be null for an empty vector: not a pointer error
+            status, text = -1, "values cannot be null"
+        out.append((case, change, status, text, variants))
+    if name in _ABI_BAD_SIZE:
+        out.append(("invalid size", _ABI_BAD_SIZE[name][0], -1, _ABI_BAD_SIZE[name][1], "both"))
+    if name in _ABI_ALIAS:
+        out.append(("aliased slabs", {"out": "a"}, -1, _ABI_ALIAS[name], "stream"))
+    if name == "ckks_encode":
+        out.append(("count = 0, null values", {"count": 0, "a": None}, 0, None, "both"))
+    if name in ("rescale_to_next", "mod_switch_to_next", "rescale_to_next_sized", "mod_switch_to_next_sized"):
+        out.append(("L = 1", {"L": 1}, -1, _END_OF_CHAIN, "both"))
+    return out
+
+
+@pytest.mark.parametrize("name", list(ABI_PAIRS))
+def test_c_abi_argument_errors_of_every_pair(name):
+    """the table above for both entry points of `name`: every bad argument gets the same status (and text) from both"""
+    import torch
+
+    S = sb()
+    n, k = 256, 3
+    mods = S.coeff_modulus_create(n, [40, 40, 40])
+    scheme = S.BFV if _PAIR_SCHEMES.get(name, "ckks").split()[0] == "bfv" else S.CKKS
+    ctx = S.Context(scheme, n, mods, 65537 if scheme == S.BFV else 0)
+    rng = np.random.default_rng(3)
+    key = ctx.load_key(rng.integers(0, 1 << 39, (2, 2, k, n), dtype=np.uint64))
+    sk = ctx.load_secret_key(rng.integers(0, 1 << 39, (k, n), dtype=np.uint64))
+    words = 2 * 16 * k * n
+    host = {f: np.zeros(words, dtype=np.uint64) for f in ("a", "b", "out")}
+    dev = {f: torch.zeros(words, dtype=torch.int64, device="cuda") for f in ("a", "b", "out")}
+    base = dict(L=2, size=3 if name == "relinearize_sized" else 2, size_a=2, size_b=2, batch=1, flag=1, elt=3, count=4, scale=2.0 ** 20,
+                cf=None, key=sk.h if name == "decrypt" else key.h)
+    stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+    bad = []
+    for case, change, status, text, variants in _abi_error_cases(name, k):
+        for variant in ("host", "stream") if variants == "both" else (variants,):
+            bufs = host if variant == "host" else dev
+            v = dict(base, **{f: C.c_void_p(x.ctypes.data if variant == "host" else x.data_ptr()) for f, x in bufs.items()})
+            v.update({f: (v[x] if x in ("a", "b", "out") else x) if isinstance(x, str) else x for f, x in change.items()})
+            ctx_h = None if case == "null context" else ctx.h
+            got = abi_call(ctx_h, name, v, None if variant == "host" else stream)
+            torch.cuda.synchronize()
+            if got[0] != status or (text is not None and got[1] != text):
+                bad.append(f"{name} {variant} [{case}]: got {got}, want ({status}, {text!r})")
+    assert not bad, "\n".join(bad)
+
+
+def test_rescale_at_the_last_level_of_a_bfv_context():
+    """both entry points report the end of the modulus switching chain before the scheme (evaluator.cpp:1521 precedes :1533)"""
+    import torch
+
+    S = sb()
+    n = 256
+    ctx = S.Context(S.BFV, n, S.coeff_modulus_create(n, [40, 40, 40]), 65537)
+    a, out = np.zeros(2 * n, dtype=np.uint64), np.zeros(2 * n, dtype=np.uint64)
+    da, dout = torch.zeros(2 * n, dtype=torch.int64, device="cuda"), torch.zeros(2 * n, dtype=torch.int64, device="cuda")
+    for name in ("rescale_to_next", "rescale_to_next_sized"):
+        v = dict(L=1, size=2, batch=1, a=a.ctypes.data_as(C.c_void_p), out=out.ctypes.data_as(C.c_void_p))
+        assert abi_call(ctx.h, name, v) == (-1, _END_OF_CHAIN)
+        v.update(a=C.c_void_p(da.data_ptr()), out=C.c_void_p(dout.data_ptr()))
+        rc, text = abi_call(ctx.h, name, v, C.c_void_p(torch.cuda.current_stream().cuda_stream))
+        assert rc == -1 and text in (_END_OF_CHAIN, "unsupported operation for scheme type")
+
+
 def test_c_abi_pointer_and_argument_errors():
     # the reference's C layer rejects null handles with E_POINTER (native/tests/seal/cabi.cpp:339-425); same here
-    import ctypes as C
-
     s = sb()
     lib = s.lib()
     null = C.c_void_p(None)
