@@ -1248,45 +1248,7 @@ namespace sb
     }
 
     // ------------------------------------------------------------------------------------- key switching ----
-    // (1) target -> coefficient form (CKKS only): rows (b, J); evaluator.cpp:2651-2658
-    struct OpKsIntt
-    {
-        Src tgt;
-        u64 *D; // [B][L][n]
-        int logn, L;
-        __device__ __forceinline__ bool skip(int) const { return false; }
-        __device__ __forceinline__ int pid(int row) const { return row % L; }
-        __device__ __forceinline__ const u64 *direct(int row, const PrimeDev &) const { return tgt.plain() ? tgt.row(row / L, row % L) : nullptr; }
-        __device__ __forceinline__ u64 load1(int row, int idx, const PrimeDev &P) const
-        {
-            return tgt.get(row / L, row % L, idx, P.q);
-        }
-        __device__ __forceinline__ void load8(int row, int idx0, u64 (&a)[8], const PrimeDev &P) const
-        {
-            if (tgt.plain())
-            {
-                const ulonglong2 *p = reinterpret_cast<const ulonglong2 *>(tgt.row(row / L, row % L) + idx0);
-#pragma unroll
-                for (int j = 0; j < 4; j++)
-                {
-                    ulonglong2 v = p[j];
-                    a[2 * j] = v.x, a[2 * j + 1] = v.y;
-                }
-                return;
-            }
-#pragma unroll
-            for (int j = 0; j < 8; j++)
-                a[j] = load1(row, idx0 + j, P);
-        }
-        __device__ __forceinline__ u64 *mid(int row) const { return D + (static_cast<long long>(row) << logn); }
-        __device__ __forceinline__ void store1(int row, int idx, u64 v, const PrimeDev &P) const { mid(row)[idx] = csub(v, P.q); }
-        __device__ __forceinline__ void store8(int row, int idx0, u64 (&a)[8], const PrimeDev &P) const
-        {
-#pragma unroll
-            for (int j = 0; j < 8; j++)
-                store1(row, idx0 + j, a[j], P);
-        }
-    };
+    // (1) target -> coefficient form: OpKsIntt (sb_src.cuh)
 
     // (2) digit J re-reduced modulo output prime I and transformed: rows (b, I, J); evaluator.cpp:2682-2702
     struct OpKsDigit
@@ -1964,17 +1926,17 @@ namespace sb
     {
         const int n = static_cast<int>(c.n), Li = static_cast<int>(L), ki = static_cast<int>(c.k);
         const bool ntt_in = (c.scheme != 1), bgv = (c.scheme == 3);
+        if (c.ksint_on(L))
+        {
+            ksint_core(c, L, B, s.I, target, s.D, key, base, out, out_bs, st);
+            return;
+        }
         Src dsrc = target;
         if (ntt_in)
         {
             OpKsIntt op{ target, s.D, c.logn, Li };
             cuda_check(launch_ntt_inv(op, static_cast<int>(B * L), c.logn, c.d_primes, st, c.stats, "ks_target_intt"), "ks intt");
             dsrc = Src{ s.D, static_cast<long long>(L) * n, nullptr, 0, c.logn };
-        }
-        if (c.ksint_on(L))
-        {
-            ksint_core(c, L, B, s.I, dsrc, key, base, out, out_bs, st);
-            return;
         }
         const bool fused = c.logn >= 12; // two-pass transforms: fuse the in-block stages with the key multiply-accumulate
         double active_rows = 0;

@@ -39,39 +39,40 @@ namespace sb
         return mul32_lazy(hi, red, P.np) + (lo + __umulhi(lo, mu) * P.np);
     }
 
-    // LOG stages on 2^LOG registers; tw(lvl, g): twiddle of group g (< 2^lvl) of level lvl
-    template <int LOG, class TwF>
+    // LOG stages on 2^LOG registers; tw(lvl, g): twiddle of group g (< 2^lvl) of level lvl.  One level per instantiation: the gap
+    // is a compile-time constant, so every register index is one even inside a loop the compiler keeps rolled
+    template <int LOG, int LVL = 0, class TwF>
     __device__ __forceinline__ void radix_fwd(uint32_t *a, TwF tw, const P32 &P)
     {
-#pragma unroll
-        for (int lvl = 0; lvl < LOG; lvl++)
+        if constexpr (LVL < LOG)
         {
-            const int gap = (1 << (LOG > 0 ? LOG - 1 : 0)) >> lvl;
+            constexpr int gap = (1 << (LOG - 1)) >> LVL;
 #pragma unroll
-            for (int g = 0; g < (1 << lvl); g++)
+            for (int g = 0; g < (1 << LVL); g++)
             {
-                const uint2 w = tw(lvl, g);
+                const uint2 w = tw(LVL, g);
 #pragma unroll
                 for (int e = 0; e < gap; e++)
                     ct32(a[2 * g * gap + e], a[2 * g * gap + e + gap], w, P);
             }
+            radix_fwd<LOG, LVL + 1>(a, tw, P);
         }
     }
-    template <int LOG, class TwF>
+    template <int LOG, int LVL = LOG - 1, class TwF>
     __device__ __forceinline__ void radix_inv(uint32_t *a, TwF tw, const P32 &P)
     {
-#pragma unroll
-        for (int lvl = LOG - 1; lvl >= 0; lvl--)
+        if constexpr (LVL >= 0)
         {
-            const int gap = (1 << (LOG > 0 ? LOG - 1 : 0)) >> lvl;
+            constexpr int gap = (1 << (LOG - 1)) >> LVL;
 #pragma unroll
-            for (int g = 0; g < (1 << lvl); g++)
+            for (int g = 0; g < (1 << LVL); g++)
             {
-                const uint2 w = tw(lvl, g);
+                const uint2 w = tw(LVL, g);
 #pragma unroll
                 for (int e = 0; e < gap; e++)
                     gs32(a[2 * g * gap + e], a[2 * g * gap + e + gap], w, P);
             }
+            radix_inv<LOG, LVL - 1>(a, tw, P);
         }
     }
 
@@ -134,6 +135,62 @@ namespace sb
 #pragma unroll
             for (int e = 0; e < E; e++)
                 o[e << 12] = a[e];
+        }
+    }
+
+    // ------------------------------------------- (1a') forward, outer pass, as the epilogue of the target's inverse column pass ----
+    // The column pass of the 64-bit inverse transform of target row (b, J) owns the coefficients r 256 + col0 + c (r < NA, c < C);
+    // with n = 4096 2^R the groups j + 4096 e (e < 2^R) of ks32_fwd_outer are among them.  The finished words go to the shared tile
+    // and every (group, auxiliary prime) pair leaves it as the words ks32_fwd_outer forms from them: the digits D are never written.
+    template <int LOGNA>
+    __global__ void __launch_bounds__(kColThreads) ks32_intt_fwd_outer(OpKsIntt op, const PrimeDev *__restrict__ primes, KsIntParams prm,
+                                                                        const uint2 *__restrict__ tw_outer, uint32_t *__restrict__ Dh, RowMap map)
+    {
+        constexpr int NA = 1 << LOGNA, C = kTile / NA, R = LOGNA - 4, E = 1 << R, G = kTile / E;
+        __shared__ __align__(16) u64 tile[kTile];
+        __shared__ __align__(16) Tw tw_s[NA];
+        __shared__ __align__(8) u64 bar;
+        const int row = blockIdx.x, col0 = blockIdx.y * C, tid = threadIdx.x, c = tid % C, ridx = tid / C;
+        const int b = row / op.L, J = row - b * op.L;
+        const PrimeDev P = primes[J];
+        if (tid == 0)
+            mbar_init(&bar, 1);
+        __syncthreads();
+        if (tid == 0)
+        {
+            mbar_expect_tx(&bar, NA * sizeof(Tw));
+            tma_load_1d(tw_s, P.inv, NA * sizeof(Tw), &bar);
+        }
+        u64 a[8];
+        const u64 *mid = op.mid(row);
+#pragma unroll
+        for (int j = 0; j < 8; j++)
+            a[j] = mid[((8 * ridx + j) << kLocalLog) + col0 + c];
+        mbar_wait(&bar, 0);
+        inv_col_passes<LOGNA>(a, tile, tw_s, ridx, c, P);
+        __syncthreads();
+#pragma unroll
+        for (int j = 0; j < 8; j++)
+            tile[(ridx + j * (NA >> 3)) * C + c] = csub(a[j], P.q);
+        __syncthreads();
+        const int orow = map.out(row, b, J);
+#pragma unroll 1
+        for (int w = tid; w < G * prm.S; w += kColThreads)
+        {
+            const int t = w / G, grp = w - t * G, rl = grp / C, cc = grp - rl * C;
+            const P32 Pt = make_p32(prm.p[t]);
+            const uint2 red = prm.red[t];
+            const uint32_t mu = prm.mu[t];
+            uint32_t x[E];
+#pragma unroll
+            for (int e = 0; e < E; e++)
+                x[e] = reduce64(tile[(rl + 16 * e) * C + cc], red, mu, Pt);
+            const uint2 *tw = tw_outer + (t << R);
+            radix_fwd<R>(x, [&](int lvl, int g) { return __ldg(tw + (1 << lvl) + g); }, Pt);
+            uint32_t *o = Dh + ((static_cast<size_t>(t) * map.rows_out + orow) << prm.logn) + (rl << kLocalLog) + col0 + cc;
+#pragma unroll
+            for (int e = 0; e < E; e++)
+                o[e << 12] = x[e];
         }
     }
 
@@ -582,7 +639,7 @@ namespace sb
     // -------------------------------------------------------------- (4) reconstruction + mod-down, per coefficient ----
     struct CrtArgs
     {
-        const uint32_t *Acc;
+        uint32_t *Acc;           // ks32_crt_kernel<..., TOP = true> leaves U in place of the special prime's first two residue rows
         const u64 *punct, *neg; // [k][S]
         const PrimeDev *primes;
         const Tw *inv_top;       // q_sp^-1 mod q_i
@@ -597,17 +654,66 @@ namespace sb
         int L, k;
         long long total;         // B * 2 * n
     };
-    // One kernel, two shapes.  FUSE = false: a thread reconstructs one coefficient of one (ciphertext, component) for every output
-    // prime.  FUSE = true: a thread owns the 2^(LOGN-12) coefficients j + 4096 e and first runs the outer inverse stages on them (they
-    // are exactly the words those butterflies couple), so the outer pass of the inverse transforms never goes through memory.
     // Per output prime and coefficient: y_t = x_t c1_t + c2_t mod p_t (canonical), three 64-bit sums sum y_t C_t.lo, sum y_t C_t.hi,
     // sum y_t floor(2^60 / p_t) (the last one's top bits are alpha: the true fraction lies in (1/4, 3/4), the estimate is 2^-28 below
     // it), one barrett_wide of sum y_t (P/p_t) + (-(alpha P) - H) mod q, then the mod-down (evaluator.cpp:2762-2864) with lazy operands:
     // (a_i - ((u mod q_i) - half)) q_sp^-1 is formed from a_i + (2 q_i + half mod q_i) - u without reducing u when q_sp < 2 q_i.
-    // The instruction count per reconstruction (it is what bounds this kernel: ncu, issue slots 75 % busy in the first version) is
+    // The instruction count per reconstruction (it is what bounds this step: ncu, issue slots 75 % busy in the first version) is
     // ~2.5x lower than with a 96-bit carry chain, a 128-bit Barrett step and canonical intermediates.
+    // x in [0, 2p) -> y_t: (x n^-1 + H) (P/p_t)^-1 mod p_t, canonical: the three sums then stay inside 64 bits (S 2^29 2^32 < 2^64)
+    __device__ __forceinline__ uint32_t crt_y(uint32_t x, uint2 c1, uint32_t c2, const P32 &P)
+    {
+        return minsub(minsub(x * c1.x + c2 + __umulhi(x, c1.y) * P.np, P.p2), P.p);
+    }
+    __device__ __forceinline__ void crt_acc(uint32_t y, u64 C, uint32_t ip, u64 &a0, u64 &a1, u64 &f)
+    {
+        asm("mad.wide.u32 %0, %1, %2, %0;" : "+l"(a0) : "r"(y), "r"(static_cast<uint32_t>(C)));
+        asm("mad.wide.u32 %0, %1, %2, %0;" : "+l"(a1) : "r"(y), "r"(static_cast<uint32_t>(C >> 32)));
+        asm("mad.wide.u32 %0, %1, %2, %0;" : "+l"(f) : "r"(y), "r"(ip));
+    }
+    // the three sums -> the exact integer mod Q, < S 2^29 q + q;  neg = A.neg + ki * S
+    __device__ __forceinline__ u64 crt_finish(u64 a0, u64 a1, u64 f, const u64 *neg, const PrimeDev &Q)
+    {
+        const u64 ng = __ldg(neg + static_cast<int>(f >> 60));
+        u64 lo = a0 + (a1 << 32), hi = (a1 >> 32) + (lo < a0);
+        lo += ng;
+        hi += (lo < ng);
+        return barrett_wide(lo, hi, Q);
+    }
+    // the special prime's value: CKKS shifts it by half (evaluator.cpp:2809-2817); BGV keeps it and derives k = -u q_top^-1 mod t
+    // (evaluator.cpp:2770-2779, rns.cpp:1202-1213)
+    template <int MODE>
+    __device__ __forceinline__ u64 crt_top(u64 U, const PrimeDev &T)
+    {
+        return MODE == 3 ? U : csub(U + (T.q >> 1), T.q);
+    }
+    __device__ __forceinline__ u64 crt_top_k(u64 U, const CrtArgs &A)
+    {
+        const u64 r = barrett64(U, A.t, A.t_ratio);
+        return mul_shoup(r ? A.t - r : 0, A.inv_top_mod_t, A.t);
+    }
+    // residue a of output prime i, U = crt_top<MODE>(special prime's value), K = crt_top_k(U) (BGV) -> the mod-down result, canonical
+    template <int MODE>
+    __device__ __forceinline__ u64 crt_moddown(u64 a, u64 U, u64 K, int i, const PrimeDev &Q, const PrimeDev &T, const CrtArgs &A)
+    {
+        u64 x; // a_i - delta_i + (multiple of q_i), in (0, 4 q_i)
+        const u64 u = T.q < Q.q2 ? U : barrett64(U, Q.q, Q.ratio_hi); // u < q_top < 2 q_i: no reduction of u needed
+        if (MODE == 3)
+        {
+            const u64 kk = (A.t > Q.q) ? barrett64(K, Q.q, Q.ratio_hi) : K;
+            x = a + (Q.q2 + Q.q) - u - mul_shoup(kk, A.qtop_mod[i], Q.q); // rns.cpp:1216-1235
+        }
+        else
+            x = a + (Q.q2 + __ldg(A.half_mod + i)) - u; // evaluator.cpp:2819-2864
+        return mul_shoup(x, A.inv_top[i], Q.q);
+    }
+    // One kernel, two shapes.  FUSE = false: a thread reconstructs one coefficient of one (ciphertext, component) for every output
+    // prime.  FUSE = true: a thread owns the 2^(LOGN-12) coefficients j + 4096 e and first runs the outer inverse stages on them (they
+    // are exactly the words those butterflies couple), so the outer pass of the inverse transforms never goes through memory.
+    // TOP (with FUSE): only the special prime's value, crt_top<MODE>(U), stored as two 32-bit halves over the words of the special
+    // prime's residue rows t = 0, 1 that the same thread has just read; ks32_inv_crt_ntt does the rest.
     // MODE 0: CKKS (coefficient-form result to R), 1: BFV (result + base to out), 3: BGV (R)
-    template <int MODE, int LOGN, bool FUSE>
+    template <int MODE, int LOGN, bool FUSE, bool TOP = false>
     __global__ void __launch_bounds__(FUSE ? 128 : 256) ks32_crt_kernel(CrtArgs A, KsIntParams prm, const uint2 *__restrict__ tw_outer)
     {
         constexpr int R = LOGN - 12, E = FUSE ? (1 << R) : 1;
@@ -641,7 +747,7 @@ namespace sb
         // fused shape: the rows (output prime, auxiliary prime) are consecutive in memory; the 2^R words of the NEXT row are requested
         // before the butterflies of the current one (two warps per scheduler cannot hide a DRAM round trip per row otherwise)
         uint32_t nrow[FUSE ? E : 1];
-        int rows_left = FUSE ? (L + 1) * S : 0;
+        int rows_left = FUSE ? (TOP ? S : (L + 1) * S) : 0;
         auto fetch_row = [&]() {
             if (FUSE)
             {
@@ -694,64 +800,46 @@ namespace sb
                 const uint2 c1 = prm.c1[t];
                 const uint32_t c2 = prm.c2[t], ip = prm.inv60[t];
                 const u64 C = __ldg(punct + t);
-                const uint32_t C0 = static_cast<uint32_t>(C), C1 = static_cast<uint32_t>(C >> 32);
 #pragma unroll
                 for (int e = 0; e < E; e++)
-                {
-                    // (x n^-1 + H) (P/p_t)^-1 mod p_t, canonical: the three sums below then stay inside 64 bits (S 2^29 2^32 < 2^64)
-                    const uint32_t y = minsub(minsub(a[e] * c1.x + c2 + __umulhi(a[e], c1.y) * P.np, P.p2), P.p);
-                    asm("mad.wide.u32 %0, %1, %2, %0;" : "+l"(a0[e]) : "r"(y), "r"(C0));
-                    asm("mad.wide.u32 %0, %1, %2, %0;" : "+l"(a1[e]) : "r"(y), "r"(C1));
-                    asm("mad.wide.u32 %0, %1, %2, %0;" : "+l"(f[e]) : "r"(y), "r"(ip));
-                }
+                    crt_acc(crt_y(a[e], c1, c2, P), C, ip, a0[e], a1[e], f[e]);
             }
-            const u64 *neg = A.neg + ki * S;
 #pragma unroll
             for (int e = 0; e < E; e++)
-            {
-                const u64 ng = __ldg(neg + static_cast<int>(f[e] >> 60));
-                u64 lo = a0[e] + (a1[e] << 32), hi = (a1[e] >> 32) + (lo < a0[e]);
-                lo += ng;
-                hi += (lo < ng);
-                val[e] = barrett_wide(lo, hi, Q); // < S 2^29 q + q
-            }
+                val[e] = crt_finish(a0[e], a1[e], f[e], A.neg + ki * S, Q);
         };
         const PrimeDev T = A.primes[k - 1];
         u64 U[E], K[MODE == 3 ? E : 1];
         reconstruct(k - 1, T, U, L > 0);
 #pragma unroll
         for (int e = 0; e < E; e++)
+            U[e] = crt_top<MODE>(U[e], T);
+        if (TOP)
         {
-            if (MODE == 3)
+            uint32_t *o = A.Acc + ((static_cast<size_t>(bc) * (L + 1) * S) << LOGN) + j;
+#pragma unroll
+            for (int e = 0; e < E; e++)
             {
-                // evaluator.cpp:2770-2779, rns.cpp:1202-1213: k = -u q_top^-1 mod t
-                const u64 r = barrett64(U[e], A.t, A.t_ratio);
-                K[e] = mul_shoup(r ? A.t - r : 0, A.inv_top_mod_t, A.t);
+                o[e << 12] = static_cast<uint32_t>(U[e]);
+                o[(size_t(1) << LOGN) + (e << 12)] = static_cast<uint32_t>(U[e] >> 32);
             }
-            else
-                U[e] = csub(U[e] + (T.q >> 1), T.q); // evaluator.cpp:2809-2817
+            return;
+        }
+        if (MODE == 3)
+        {
+#pragma unroll
+            for (int e = 0; e < E; e++)
+                K[e] = crt_top_k(U[e], A);
         }
         for (int i = 0; i < L; i++)
         {
             const PrimeDev Q = A.primes[i];
             u64 a[E];
             reconstruct(i, Q, a, i + 1 < L);
-            const Tw inv = A.inv_top[i];
-            const bool same_size = T.q < Q.q2; // u < q_top < 2 q_i: no reduction of u needed
-            const u64 half_mod = __ldg(A.half_mod + i);
 #pragma unroll
             for (int e = 0; e < E; e++)
             {
-                u64 x; // a_i - delta_i + (multiple of q_i), in (0, 4 q_i)
-                const u64 u = same_size ? U[e] : barrett64(U[e], Q.q, Q.ratio_hi);
-                if (MODE == 3)
-                {
-                    const u64 kk = (A.t > Q.q) ? barrett64(K[e], Q.q, Q.ratio_hi) : K[e];
-                    x = a[e] + (Q.q2 + Q.q) - u - mul_shoup(kk, A.qtop_mod[i], Q.q); // rns.cpp:1216-1235
-                }
-                else
-                    x = a[e] + (Q.q2 + half_mod) - u; // evaluator.cpp:2819-2864
-                const u64 r = mul_shoup(x, inv, Q.q);
+                const u64 r = crt_moddown<MODE>(a[e], U[e], K[MODE == 3 ? e : 0], i, Q, T, A);
                 const int xi = j + (e << 12);
                 if (MODE == 1)
                     A.out[b * A.o_bs + c * A.o_ps + (static_cast<long long>(i) << LOGN) + xi] = csub(r + A.base.get(b, c, i, xi, Q.q), Q.q);
@@ -779,6 +867,114 @@ namespace sb
         case 15: launch_crt_logn<MODE, 15>(A, d, fuse, B, st); break;
         case 16: launch_crt_logn<MODE, 16>(A, d, fuse, B, st); break;
         case 17: launch_crt_logn<MODE, 17>(A, d, false, B, st); break; // 32 coefficients per thread do not fit the register file
+        default: throw std::logic_error("unsupported transform size");
+        }
+    }
+
+    // ---------------------------------- (4 + 5a) reconstruction and mod-down as the load of the result's forward column pass ----
+    // One CTA = the column pass of result row (b, c, i) over the coefficients r 256 + col0 + c (r < NA, c < C); with n = 4096 2^R the
+    // groups j + 4096 e (e < 2^R) that the outer inverse stages couple are among them.  (1) every (group, auxiliary prime t) pair runs
+    // the outer stages on the accumulated products of output prime i and leaves y_t in shared memory; (2) every thread reconstructs its
+    // 8 coefficients from their S values y_t and mods them down with U (ks32_crt_kernel<..., TOP = true>); (3) the column stages of the
+    // 64-bit forward transform, whose tile reuses the shared memory of (1).  The coefficient-form result never goes through memory.
+    // 2 CTAs per SM (64 registers): the launch bound of the plain column pass (SB_COL_MIN_BLOCKS) leaves too few for (2).
+    template <int LOGNA>
+    constexpr size_t crt_ntt_smem(int S) { return static_cast<size_t>(S > 2 ? S : 2) * kTile * 4 + (size_t(1) << LOGNA) * sizeof(Tw) + 8; }
+    template <int MODE, int LOGNA, bool FAST>
+    __global__ void __launch_bounds__(kColThreads, 2) ks32_inv_crt_ntt(CrtArgs A, KsIntParams prm, const uint2 *__restrict__ tw_outer, u64 *__restrict__ mid)
+    {
+        constexpr int NA = 1 << LOGNA, C = kTile / NA, R = LOGNA - 4, E = 1 << R, G = kTile / E, LOGN = LOGNA + kLocalLog;
+        extern __shared__ __align__(16) unsigned char ks_crt_smem[];
+        const int S = prm.S, L = A.L;
+        uint32_t *ys = reinterpret_cast<uint32_t *>(ks_crt_smem); // [t][r C + c]
+        u64 *tile = reinterpret_cast<u64 *>(ks_crt_smem);
+        Tw *tw_s = reinterpret_cast<Tw *>(ks_crt_smem + static_cast<size_t>(S > 2 ? S : 2) * kTile * 4);
+        u64 *bar = reinterpret_cast<u64 *>(tw_s + NA);
+        const int row = blockIdx.x, col0 = blockIdx.y * C, tid = threadIdx.x, c = tid % C, ridx = tid / C;
+        const int bc = row / L, i = row - bc * L;
+        const PrimeDev Q = A.primes[i];
+        if (tid == 0)
+            mbar_init(bar, 1);
+        __syncthreads();
+        if (tid == 0)
+        {
+            mbar_expect_tx(bar, NA * sizeof(Tw));
+            tma_load_1d(tw_s, Q.fwd, NA * sizeof(Tw), bar);
+        }
+        // (1) rows (bc, I' = i + 1, t) of the accumulated products
+        const uint32_t *acc = A.Acc + ((static_cast<size_t>(bc) * (L + 1) + i + 1) * S << LOGN) + col0;
+#pragma unroll 1
+        for (int w = tid; w < G * S; w += kColThreads)
+        {
+            const int t = w / G, grp = w - t * G, rl = grp / C, cc = grp - rl * C;
+            const P32 P = make_p32(prm.p[t]);
+            const uint32_t *p = acc + (static_cast<size_t>(t) << LOGN) + (rl << kLocalLog) + cc;
+            uint32_t x[E];
+#pragma unroll
+            for (int e = 0; e < E; e++)
+                x[e] = p[e << 12];
+            const uint2 *tw = tw_outer + (t << R);
+            radix_inv<R>(x, [&](int lvl, int g) { return __ldg(tw + (1 << lvl) + g); }, P);
+            const uint2 c1 = prm.c1[t];
+            const uint32_t c2 = prm.c2[t];
+#pragma unroll
+            for (int e = 0; e < E; e++)
+                ys[t * kTile + (rl + 16 * e) * C + cc] = crt_y(x[e], c1, c2, P);
+        }
+        __syncthreads();
+        // (2) coefficients r = ridx + j NA/8: the first layout of the column stages
+        const uint32_t *ulo = A.Acc + ((static_cast<size_t>(bc) * (L + 1) * S) << LOGN) + col0 + c, *uhi = ulo + (size_t(1) << LOGN);
+        const PrimeDev T = A.primes[A.k - 1];
+        const u64 *punct = A.punct + i * S;
+        u64 a[8];
+#pragma unroll
+        for (int j = 0; j < 8; j++)
+        {
+            const int r = ridx + j * (NA >> 3);
+            u64 a0 = 0, a1 = 0, f = 0;
+#pragma unroll
+            for (int t = 0; t < kKsMaxS; t++)
+            {
+                if (t >= S)
+                    break;
+                crt_acc(ys[t * kTile + r * C + c], __ldg(punct + t), prm.inv60[t], a0, a1, f);
+            }
+            const u64 U = pack64(ulo[r << kLocalLog], uhi[r << kLocalLog]);
+            a[j] = crt_moddown<MODE>(crt_finish(a0, a1, f, A.neg + i * S, Q), U, MODE == 3 ? crt_top_k(U, A) : 0, i, Q, T, A);
+        }
+        __syncthreads(); // the values y_t are consumed: the shared memory becomes the tile
+        mbar_wait(bar, 0);
+        // (3)
+        fwd_col_passes<LOGNA, FAST>(a, tile, tw_s, ridx, c, Q);
+        u64 *m = mid + (static_cast<size_t>(row) << LOGN);
+#pragma unroll
+        for (int j = 0; j < 8; j++)
+            m[((8 * ridx + j) << kLocalLog) + col0 + c] = a[j];
+    }
+    template <int MODE, int LOGNA>
+    static void launch_crt_ntt_logna(const CrtArgs &A, const KsInt &d, u64 *mid, size_t B, bool fast, bool top, cudaStream_t st)
+    {
+        if (top)
+        {
+            ks32_crt_kernel<MODE, LOGNA + kLocalLog, true, true><<<static_cast<unsigned>(B * 2 * 32), 128, 0, st>>>(A, d.prm, d.d_inv_outer);
+            return;
+        }
+        auto kern = fast ? ks32_inv_crt_ntt<MODE, LOGNA, true> : ks32_inv_crt_ntt<MODE, LOGNA, false>;
+        const size_t smem = crt_ntt_smem<LOGNA>(d.prm.S);
+        cuda_check(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)), "smem attr");
+        const dim3 grid(static_cast<unsigned>(B * 2 * A.L), static_cast<unsigned>((1 << kLocalLog) / (kTile >> LOGNA)));
+        kern<<<grid, kColThreads, smem, st>>>(A, d.prm, d.d_inv_outer, mid);
+    }
+    // top: the special prime's value (ks32_crt_kernel<..., TOP = true>); otherwise ks32_inv_crt_ntt into mid.  n = 8192 .. 65536
+    template <int MODE>
+    static void launch_crt_ntt(const CrtArgs &A, const KsInt &d, u64 *mid, size_t B, bool fast, bool top, int logn, cudaStream_t st)
+    {
+        switch (logn)
+        {
+        case 13: launch_crt_ntt_logna<MODE, 5>(A, d, mid, B, fast, top, st); break;
+        case 14: launch_crt_ntt_logna<MODE, 6>(A, d, mid, B, fast, top, st); break;
+        case 15: launch_crt_ntt_logna<MODE, 7>(A, d, mid, B, fast, top, st); break;
+        case 16: launch_crt_ntt_logna<MODE, 8>(A, d, mid, B, fast, top, st); break;
         default: throw std::logic_error("unsupported transform size");
         }
     }
@@ -880,6 +1076,8 @@ namespace sb
         cuda_check(cudaFuncSetAttribute(ks32_inv_local, cudaFuncAttributeMaxDynamicSharedMemorySize, kKsLocalSmem), "smem attr");
         if (const char *e = std::getenv("SB200_KS_FUSE_CRT"))
             d.fuse_crt = std::atoi(e) != 0;
+        if (const char *e = std::getenv("SB200_KS_FUSE_NTT"))
+            d.fuse_ntt = std::atoi(e) != 0;
         if (const char *e = std::getenv("SB200_KS_MAC_TILE"))
             d.mac_tile = std::atoi(e) != 0;
         d.ready = true;
@@ -929,16 +1127,20 @@ namespace sb
     }
 
     // rows of 64-bit words (dsrc rows (b, J), J < L) -> Dh[t][map.rows_out][n], transformed modulo every auxiliary prime
-    static void ksint_forward(Context &c, Src dsrc, int L, int rows, uint32_t *Dh, RowMap map, cudaStream_t st)
+    // (outer = false: the outer pass has been run, by ks32_intt_fwd_outer)
+    static void ksint_forward(Context &c, Src dsrc, int L, int rows, uint32_t *Dh, RowMap map, cudaStream_t st, bool outer = true)
     {
         const KsInt &d = c.ksint;
         const double n = static_cast<double>(c.n), S = d.prm.S;
         const bool plain = dsrc.perm == nullptr && dsrc.ginv == 0;
-        c.stats.begin("ks32_fwd_outer", 0, rows * n * (8.0 + 4.0 * S), st, 0, 0);
-        c.stats.work32(0.5 * rows * n * S * d.prm.r, 0);
-        plain ? launch_fwd_outer<true>(c, dsrc, L, rows, Dh, map, st) : launch_fwd_outer<false>(c, dsrc, L, rows, Dh, map, st);
-        c.stats.end(st);
-        cuda_check(cudaGetLastError(), "ks32_fwd_outer");
+        if (outer)
+        {
+            c.stats.begin("ks32_fwd_outer", 0, rows * n * (8.0 + 4.0 * S), st, 0, 0);
+            c.stats.work32(0.5 * rows * n * S * d.prm.r, 0);
+            plain ? launch_fwd_outer<true>(c, dsrc, L, rows, Dh, map, st) : launch_fwd_outer<false>(c, dsrc, L, rows, Dh, map, st);
+            c.stats.end(st);
+            cuda_check(cudaGetLastError(), "ks32_fwd_outer");
+        }
         // (padding rows of the digit layout are transformed too: a few uninitialised rows whose products are never stored)
         dim3 grid(static_cast<unsigned>((map.rows_out + kRowsPerCta - 1) / kRowsPerCta), static_cast<unsigned>(d.prm.S << d.prm.r));
         c.stats.begin("ks32_fwd_local", 0, rows * n * 8.0 * S, st, 0, 0);
@@ -987,8 +1189,36 @@ namespace sb
 
     static void launch_inverse(Context &c, uint32_t *data, int arows, cudaStream_t st, bool outer = true);
 
-    void ksint_core(Context &c, size_t L, size_t B, const KsIntScratch &s, Src dsrc, const KSwitchKey &key, BaseSrc base, u64 *out,
-                    long long o_bs, cudaStream_t st)
+    template <int LOGNA>
+    static void launch_intt_fwd_outer_logna(Context &c, const OpKsIntt &op, int rows, uint32_t *Dh, RowMap map, cudaStream_t st)
+    {
+        const dim3 grid(static_cast<unsigned>(rows), static_cast<unsigned>((1 << kLocalLog) / (kTile >> LOGNA)));
+        ks32_intt_fwd_outer<LOGNA><<<grid, kColThreads, 0, st>>>(op, c.d_primes, c.ksint.prm, c.ksint.d_fwd_outer, Dh, map);
+    }
+    // the target's inverse transforms (CKKS / BGV: NTT form); fused: their column passes end in the forward outer pass
+    static void ksint_target_intt(Context &c, const OpKsIntt &op, int rows, uint32_t *Dh, RowMap map, bool fused, cudaStream_t st)
+    {
+        cuda_check(launch_ntt_inv(op, rows, c.logn, c.d_primes, st, c.stats, "ks_target_intt", -1, fused), "ks intt");
+        if (!fused)
+            return;
+        const double n = static_cast<double>(c.n), S = c.ksint.prm.S;
+        // bytes and butterflies: the inverse column pass's read, ks32_fwd_outer's writes and 32-bit butterflies
+        c.stats.begin("ks_target_intt_aux", 1, rows * n * (8.0 + 4.0 * S), st, 0.5 * rows * n * (c.logn - kLocalLog));
+        c.stats.work32(0.5 * rows * n * S * c.ksint.prm.r, 0);
+        switch (c.logn)
+        {
+        case 13: launch_intt_fwd_outer_logna<5>(c, op, rows, Dh, map, st); break;
+        case 14: launch_intt_fwd_outer_logna<6>(c, op, rows, Dh, map, st); break;
+        case 15: launch_intt_fwd_outer_logna<7>(c, op, rows, Dh, map, st); break;
+        case 16: launch_intt_fwd_outer_logna<8>(c, op, rows, Dh, map, st); break;
+        default: throw std::logic_error("unsupported transform size");
+        }
+        c.stats.end(st);
+        cuda_check(cudaGetLastError(), "ks32_intt_fwd_outer");
+    }
+
+    void ksint_core(Context &c, size_t L, size_t B, const KsIntScratch &s, Src target, u64 *D, const KSwitchKey &key, BaseSrc base,
+                    u64 *out, long long o_bs, cudaStream_t st)
     {
         const KsInt &d = c.ksint;
         if (!d.ready || !key.d_key32)
@@ -996,9 +1226,19 @@ namespace sb
         const int Li = static_cast<int>(L), ki = static_cast<int>(c.k), Bi = static_cast<int>(B), S = d.prm.S;
         const double n = static_cast<double>(c.n);
         const int rows = Bi * Li, nic = 2 * (Li + 1), arows = Bi * nic;
+        const bool fuse_crt = d.fuse_crt && d.prm.r >= 1 && d.prm.r <= 4;
+        // CKKS / BGV at n = 8192 .. 65536: the path's entry and exit ride in the column passes of the 64-bit transforms
+        const bool fuse_ntt = d.fuse_ntt && c.scheme != 1 && d.prm.r >= 1 && d.prm.r <= 4;
         // (1) digits -> auxiliary primes, forward transforms
         const int nbt = (Bi + kMacTB - 1) / kMacTB, Bpad = nbt * kMacTB;
-        ksint_forward(c, dsrc, Li, rows, s.Dh, RowMap{ 1, Bpad, Li * Bpad }, st);
+        const RowMap map{ 1, Bpad, Li * Bpad };
+        Src dsrc = target;
+        if (c.scheme != 1)
+        {
+            ksint_target_intt(c, OpKsIntt{ target, D, c.logn, Li }, rows, s.Dh, map, fuse_ntt, st);
+            dsrc = Src{ D, static_cast<long long>(L * c.n), nullptr, 0, c.logn };
+        }
+        ksint_forward(c, dsrc, Li, rows, s.Dh, map, st, !fuse_ntt);
         // (2) products with the key, summed over the digits
         {
             // one pass over the key + the transformed digits in, the sums out
@@ -1019,7 +1259,6 @@ namespace sb
             cuda_check(cudaGetLastError(), "ks32_mac");
         }
         // (3) inverse transforms of the sums; the outer stages ride in the reconstruction kernel (fuse_crt) or run as their own pass
-        const bool fuse_crt = d.fuse_crt && d.prm.r >= 1 && d.prm.r <= 4;
         launch_inverse(c, s.Acc, arows, st, !fuse_crt);
         // (4) exact integers -> residues mod q_I, mod-down by the special prime in coefficient form
         const long long o_ps = static_cast<long long>(L) * c.n;
@@ -1032,16 +1271,36 @@ namespace sb
             A.half_mod = d.d_half_mod;
             A.R = s.R, A.out = out, A.o_bs = o_bs, A.o_ps = o_ps, A.base = base, A.L = Li, A.k = ki;
             A.total = static_cast<long long>(B) * 2 * c.n;
-            c.stats.begin("ks32_crt", 0, n * B * 2 * (4.0 * S * (L + 1) + 8.0 * L), st);
-            if (fuse_crt)
-                c.stats.work32(0.5 * arows * S * n * d.prm.r, 0);
             if (c.scheme == 3)
             {
                 A.qtop_mod = c.d_qmod + (c.k - 1) * c.k;
                 A.t = c.t, A.t_ratio = c.t_ratio;
                 A.inv_top_mod_t = Tw{ c.inv_q_mod_t[c.k - 1], sbh::shoup(c.inv_q_mod_t[c.k - 1], c.t) };
-                launch_crt<3>(A, d, fuse_crt, B, c.logn, st);
             }
+            if (fuse_ntt && fuse_crt)
+            {
+                // (4 + 5) the special prime's value in place, then the result's forward column passes reconstruct their own inputs
+                c.stats.begin("ks32_inv_crt_top", 0, n * B * 2 * (4.0 * S + 8.0), st);
+                c.stats.work32(0.5 * B * 2 * S * n * d.prm.r, 0);
+                c.scheme == 3 ? launch_crt_ntt<3>(A, d, s.R, B, c.fast_q, true, c.logn, st) : launch_crt_ntt<0>(A, d, s.R, B, c.fast_q, true, c.logn, st);
+                c.stats.end(st);
+                cuda_check(cudaGetLastError(), "ks32_crt_kernel");
+                const double rrows = 2.0 * B * L;
+                c.stats.begin("ks32_inv_crt_ntt", 0, n * rrows * (4.0 * S + 16.0), st, 0.5 * rrows * n * (c.logn - kLocalLog));
+                c.stats.work32(0.5 * rrows * S * n * d.prm.r, 0);
+                c.scheme == 3 ? launch_crt_ntt<3>(A, d, s.R, B, c.fast_q, false, c.logn, st) : launch_crt_ntt<0>(A, d, s.R, B, c.fast_q, false, c.logn, st);
+                c.stats.end(st);
+                cuda_check(cudaGetLastError(), "ks32_inv_crt_ntt");
+                OpAddBaseFwd op{ s.R, out, o_bs, o_ps, base, c.logn, Li };
+                cuda_check(launch_ntt_fwd(op, static_cast<int>(B * 2 * L), c.logn, c.d_primes, st, c.stats, "ks_result_ntt", -1, c.fast_q, true),
+                           "ks result ntt");
+                return;
+            }
+            c.stats.begin("ks32_crt", 0, n * B * 2 * (4.0 * S * (L + 1) + 8.0 * L), st);
+            if (fuse_crt)
+                c.stats.work32(0.5 * arows * S * n * d.prm.r, 0);
+            if (c.scheme == 3)
+                launch_crt<3>(A, d, fuse_crt, B, c.logn, st);
             else if (c.scheme == 1)
                 launch_crt<1>(A, d, fuse_crt, B, c.logn, st);
             else

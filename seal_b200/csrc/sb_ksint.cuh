@@ -37,6 +37,7 @@ namespace sb
         bool ready = false;
         bool mac_tile = true;  // product kernel with the key tile in shared memory (env SB200_KS_MAC_TILE)
         bool fuse_crt = true;  // outer inverse stages inside the reconstruction kernel (env SB200_KS_FUSE_CRT)
+        bool fuse_ntt = true;  // entry and exit inside the column passes of the 64-bit transforms (env SB200_KS_FUSE_NTT)
         size_t max_digits = 0; // sbh::KsIntHost::max_digits (64 at n = 4096)
         KsIntParams prm;
         uint2 *d_fwd_outer = nullptr, *d_inv_outer = nullptr; // [S][2^r]
@@ -60,9 +61,10 @@ namespace sb
     void ksint_free(Context &c);
     // khat[t][J][c][ki][n] from the uploaded key [digits][2][k][n]
     void ksint_prepare_key(Context &c, KSwitchKey &key, cudaStream_t st);
-    // digits (coefficient form, dsrc.get(b, J, idx, q_J)) -> out = base + key-switched polynomials; see key_switch_chunk
-    void ksint_core(Context &c, size_t L, size_t B, const KsIntScratch &s, Src dsrc, const KSwitchKey &key, BaseSrc base, u64 *out,
-                    long long o_bs, cudaStream_t st);
+    // target (CKKS / BGV: NTT form, BFV: coefficient form) -> out = base + key-switched polynomials; D: [B][L][n] scratch of the
+    // target's inverse transforms.  See key_switch_chunk
+    void ksint_core(Context &c, size_t L, size_t B, const KsIntScratch &s, Src target, u64 *D, const KSwitchKey &key, BaseSrc base,
+                    u64 *out, long long o_bs, cudaStream_t st);
     // arithmetic ceilings of this path measured in process: kind 0 = 32-bit forward butterflies, 1 = inverse, 2 = multiply-accumulates
     double ksint_selftest_rate(Context &c, int kind, cudaStream_t st);
     // parity-test access to the transforms: forward h_rows [rows][n] u64 -> h_io [S][rows][n]; inverse: h_io [rows][S][n] in place

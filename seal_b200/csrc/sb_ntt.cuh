@@ -363,38 +363,15 @@ namespace sb
     }
 
     // ---------------------------------------------------------------------------------- inverse: column pass ----
-    template <int LOGNA, class Op>
-    __global__ void __launch_bounds__(kColThreads) ntt_inv_col(Op op, const PrimeDev *__restrict__ primes)
+    // The log2(NA) column stages on one thread's 8 coefficients: in = layout r = 8*ridx + j, out = layout r = ridx + j*(NA/8),
+    // reduced to [0, 2q).  The last read of the shared tile is not followed by a barrier.
+    template <int LOGNA>
+    __device__ __forceinline__ void inv_col_passes(u64 (&a)[8], u64 *tile, const Tw *tw_s, int ridx, int c, const PrimeDev &P)
     {
         constexpr int NA = 1 << LOGNA;
         constexpr int C = kTile / NA;
         constexpr int NSTL = LOGNA % 3; // stages in the (partial) last pass
         constexpr int NFULL = LOGNA / 3;
-        __shared__ __align__(16) u64 tile[kTile];
-        __shared__ __align__(16) Tw tw_s[NA];
-        __shared__ __align__(8) u64 bar;
-
-        const int row = blockIdx.x, col0 = blockIdx.y * C;
-        if (op.skip(row))
-            return;
-        const int tid = threadIdx.x, c = tid % C, ridx = tid / C;
-        const PrimeDev P = primes[op.pid(row)];
-
-        if (tid == 0)
-            mbar_init(&bar, 1);
-        __syncthreads();
-        if (tid == 0)
-        {
-            mbar_expect_tx(&bar, NA * sizeof(Tw));
-            tma_load_1d(tw_s, P.inv, NA * sizeof(Tw), &bar);
-        }
-        u64 a[8];
-        const u64 *mid = op.mid(row);
-#pragma unroll
-        for (int j = 0; j < 8; j++)
-            a[j] = mid[((8 * ridx + j) << kLocalLog) + col0 + c];
-        mbar_wait(&bar, 0);
-
         int prev_g = 1;
 #pragma unroll
         for (int p = 0; p < NFULL; p++)
@@ -437,18 +414,44 @@ namespace sb
             // level 1: r-stride NA/4 -> m_r = 2 ; level 2: r-stride NA/2 -> m_r = 1 (final)
             auto twf = [&](int lvl, int k) { return tw_s[(lvl == 1 ? 2 : 1) + k]; };
             inv_regs<3 - NSTL, true>(a, twf, P);
-#pragma unroll
-            for (int j = 0; j < 8; j++)
-                op.store1(row, ((ridx + j * g) << kLocalLog) + col0 + c, a[j], P);
         }
-        else
+        // (without a partial last pass the last layout is r = rhi*8g + rlo + j*g with g = NA/8, i.e. rhi = 0, rlo = ridx)
+    }
+
+    template <int LOGNA, class Op>
+    __global__ void __launch_bounds__(kColThreads) ntt_inv_col(Op op, const PrimeDev *__restrict__ primes)
+    {
+        constexpr int NA = 1 << LOGNA;
+        constexpr int C = kTile / NA;
+        __shared__ __align__(16) u64 tile[kTile];
+        __shared__ __align__(16) Tw tw_s[NA];
+        __shared__ __align__(8) u64 bar;
+
+        const int row = blockIdx.x, col0 = blockIdx.y * C;
+        if (op.skip(row))
+            return;
+        const int tid = threadIdx.x, c = tid % C, ridx = tid / C;
+        const PrimeDev P = primes[op.pid(row)];
+
+        if (tid == 0)
+            mbar_init(&bar, 1);
+        __syncthreads();
+        if (tid == 0)
         {
-            constexpr int g = NA >> 3;
-            const int rhi = ridx / g, rlo = ridx % g; // rhi == 0
-#pragma unroll
-            for (int j = 0; j < 8; j++)
-                op.store1(row, ((rhi * 8 * g + rlo + j * g) << kLocalLog) + col0 + c, a[j], P);
+            mbar_expect_tx(&bar, NA * sizeof(Tw));
+            tma_load_1d(tw_s, P.inv, NA * sizeof(Tw), &bar);
         }
+        u64 a[8];
+        const u64 *mid = op.mid(row);
+#pragma unroll
+        for (int j = 0; j < 8; j++)
+            a[j] = mid[((8 * ridx + j) << kLocalLog) + col0 + c];
+        mbar_wait(&bar, 0);
+
+        inv_col_passes<LOGNA>(a, tile, tw_s, ridx, c, P);
+#pragma unroll
+        for (int j = 0; j < 8; j++)
+            op.store1(row, ((ridx + j * (NA >> 3)) << kLocalLog) + col0 + c, a[j], P);
     }
 
     // ------------------------------------------------------------------- small transforms (n < 4096): one CTA/row ----
@@ -575,7 +578,7 @@ namespace sb
 
     template <class Op>
     inline cudaError_t launch_ntt_fwd(const Op &op, int nrows, int logn, const PrimeDev *primes, cudaStream_t st, LaunchStats &ls,
-                                      const char *name = "ntt_fwd", int active_rows = -1, bool fast = false, bool col_only = false)
+                                      const char *name = "ntt_fwd", int active_rows = -1, bool fast = false, bool local_only = false)
     {
         if (nrows <= 0)
             return cudaSuccess;
@@ -591,20 +594,21 @@ namespace sb
         }
         const int logna = logn - kLocalLog, na = 1 << logna;
         dim3 gc(nrows, (1 << kLocalLog) / (kTile / na));
-        ls.begin(name, 1, bytes, st, bf_stage * logna); // column pass
-        switch (logna)
+        if (!local_only) // otherwise the caller's own column pass has written op.mid()
         {
-        case 4: fast ? ntt_fwd_col<4, true, Op><<<gc, kColThreads, 0, st>>>(op, primes) : ntt_fwd_col<4, false, Op><<<gc, kColThreads, 0, st>>>(op, primes); break;
-        case 5: fast ? ntt_fwd_col<5, true, Op><<<gc, kColThreads, 0, st>>>(op, primes) : ntt_fwd_col<5, false, Op><<<gc, kColThreads, 0, st>>>(op, primes); break;
-        case 6: fast ? ntt_fwd_col<6, true, Op><<<gc, kColThreads, 0, st>>>(op, primes) : ntt_fwd_col<6, false, Op><<<gc, kColThreads, 0, st>>>(op, primes); break;
-        case 7: fast ? ntt_fwd_col<7, true, Op><<<gc, kColThreads, 0, st>>>(op, primes) : ntt_fwd_col<7, false, Op><<<gc, kColThreads, 0, st>>>(op, primes); break;
-        case 8: fast ? ntt_fwd_col<8, true, Op><<<gc, kColThreads, 0, st>>>(op, primes) : ntt_fwd_col<8, false, Op><<<gc, kColThreads, 0, st>>>(op, primes); break;
-        case 9: fast ? ntt_fwd_col<9, true, Op><<<gc, kColThreads, 0, st>>>(op, primes) : ntt_fwd_col<9, false, Op><<<gc, kColThreads, 0, st>>>(op, primes); break;
-        default: return cudaErrorInvalidValue;
+            ls.begin(name, 1, bytes, st, bf_stage * logna); // column pass
+            switch (logna)
+            {
+            case 4: fast ? ntt_fwd_col<4, true, Op><<<gc, kColThreads, 0, st>>>(op, primes) : ntt_fwd_col<4, false, Op><<<gc, kColThreads, 0, st>>>(op, primes); break;
+            case 5: fast ? ntt_fwd_col<5, true, Op><<<gc, kColThreads, 0, st>>>(op, primes) : ntt_fwd_col<5, false, Op><<<gc, kColThreads, 0, st>>>(op, primes); break;
+            case 6: fast ? ntt_fwd_col<6, true, Op><<<gc, kColThreads, 0, st>>>(op, primes) : ntt_fwd_col<6, false, Op><<<gc, kColThreads, 0, st>>>(op, primes); break;
+            case 7: fast ? ntt_fwd_col<7, true, Op><<<gc, kColThreads, 0, st>>>(op, primes) : ntt_fwd_col<7, false, Op><<<gc, kColThreads, 0, st>>>(op, primes); break;
+            case 8: fast ? ntt_fwd_col<8, true, Op><<<gc, kColThreads, 0, st>>>(op, primes) : ntt_fwd_col<8, false, Op><<<gc, kColThreads, 0, st>>>(op, primes); break;
+            case 9: fast ? ntt_fwd_col<9, true, Op><<<gc, kColThreads, 0, st>>>(op, primes) : ntt_fwd_col<9, false, Op><<<gc, kColThreads, 0, st>>>(op, primes); break;
+            default: return cudaErrorInvalidValue;
+            }
+            ls.end(st);
         }
-        ls.end(st);
-        if (col_only)
-            return cudaGetLastError(); // the caller runs its own fused local pass on op.mid()
         ls.begin(name, 2, bytes, st, bf_stage * kLocalLog); // local pass
         if (fast)
         {
@@ -622,7 +626,7 @@ namespace sb
 
     template <class Op>
     inline cudaError_t launch_ntt_inv(const Op &op, int nrows, int logn, const PrimeDev *primes, cudaStream_t st, LaunchStats &ls,
-                                      const char *name = "ntt_inv", int active_rows = -1)
+                                      const char *name = "ntt_inv", int active_rows = -1, bool local_only = false)
     {
         if (nrows <= 0)
             return cudaSuccess;
@@ -641,6 +645,8 @@ namespace sb
         cudaFuncSetAttribute(ntt_inv_local<Op>, cudaFuncAttributeMaxDynamicSharedMemorySize, kLocalSmem);
         ntt_inv_local<Op><<<dim3(nrows, na / 8), 256, kLocalSmem, st>>>(op, primes, na);
         ls.end(st);
+        if (local_only)
+            return cudaGetLastError(); // the caller runs its own column pass on op.mid()
         dim3 gc(nrows, (1 << kLocalLog) / (kTile / na));
         ls.begin(name, 1, bytes, st, bf_stage * logna); // column pass
         switch (logna)

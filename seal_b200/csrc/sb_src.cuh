@@ -51,4 +51,43 @@ namespace sb
         }
     };
 
+    // (1) target -> coefficient form (CKKS / BGV): rows (b, J); evaluator.cpp:2651-2658
+    struct OpKsIntt
+    {
+        Src tgt;
+        u64 *D; // [B][L][n]
+        int logn, L;
+        __device__ __forceinline__ bool skip(int) const { return false; }
+        __device__ __forceinline__ int pid(int row) const { return row % L; }
+        __device__ __forceinline__ const u64 *direct(int row, const PrimeDev &) const { return tgt.plain() ? tgt.row(row / L, row % L) : nullptr; }
+        __device__ __forceinline__ u64 load1(int row, int idx, const PrimeDev &P) const
+        {
+            return tgt.get(row / L, row % L, idx, P.q);
+        }
+        __device__ __forceinline__ void load8(int row, int idx0, u64 (&a)[8], const PrimeDev &P) const
+        {
+            if (tgt.plain())
+            {
+                const ulonglong2 *p = reinterpret_cast<const ulonglong2 *>(tgt.row(row / L, row % L) + idx0);
+#pragma unroll
+                for (int j = 0; j < 4; j++)
+                {
+                    ulonglong2 v = p[j];
+                    a[2 * j] = v.x, a[2 * j + 1] = v.y;
+                }
+                return;
+            }
+#pragma unroll
+            for (int j = 0; j < 8; j++)
+                a[j] = load1(row, idx0 + j, P);
+        }
+        __device__ __forceinline__ u64 *mid(int row) const { return D + (static_cast<long long>(row) << logn); }
+        __device__ __forceinline__ void store1(int row, int idx, u64 v, const PrimeDev &P) const { mid(row)[idx] = csub(v, P.q); }
+        __device__ __forceinline__ void store8(int row, int idx0, u64 (&a)[8], const PrimeDev &P) const
+        {
+#pragma unroll
+            for (int j = 0; j < 8; j++)
+                store1(row, idx0 + j, a[j], P);
+        }
+    };
 } // namespace sb
