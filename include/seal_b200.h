@@ -156,7 +156,10 @@ int sb200_selftest_ksint_inverse(sb200_context *ctx, uint32_t *h_data, size_t ro
 int sb200_kswitch_key_create(sb200_context *ctx, const uint64_t *h_key, size_t digits, sb200_kswitch_key **out);
 int sb200_kswitch_key_destroy(sb200_kswitch_key *key);
 /* KSwitchKeys::load of the single entry data()[index] out of a RelinKeys / GaloisKeys stream saved with
- * compr_mode_type::none (kswitchkeys.cpp:42-160): the key polynomials go from the stream to the device directly.
+ * compr_mode_type::none or zlib (kswitchkeys.cpp:42-160): the key polynomials go from the stream to the device directly.
+ * Seed-compressed members (what KeyGenerator::create_relin_keys / create_galois_keys return as Serializable objects: c_0 and
+ * the seed of c_1, of either prng_type) upload c_0 only and expand every digit's c_1 on the device at the key level, bit for bit
+ * as Ciphertext::expand_seed does (ciphertext.cpp:118-150); the seeded relinearization key of n = 65536, k = 32 is half the bytes.
  * index = RelinKeys::get_index(2) = 0 for relinearization, GaloisKeys::get_index(galois_elt) = (galois_elt - 1) / 2 for a
  * rotation (relinkeys.h:58-65, galoiskeys.h:48-51).  SB200_E_OUT_OF_RANGE: no such slot; SB200_E_INVALID_ARG: empty slot. */
 int sb200_kswitch_key_load(sb200_context *ctx, const uint8_t *stream, size_t len, size_t index, sb200_kswitch_key **out);
@@ -263,10 +266,11 @@ int sb200_relinearize_sized_host(sb200_context *ctx, size_t L, size_t size, size
 /* ---- wire format (SURVEY 8f rank 3): Ciphertext::save / load with compr_mode_type::none, straight between a byte
  * stream and a device slab (ciphertext.cpp:190-359, serialization.h:76-91, dynarray.h:662-690).  Seed-compressed ciphertexts
  * (Serializable<Ciphertext> of a symmetric-key encryption: c_1 replaced by the seed of the PRNG that made it) are expanded on
- * the device -- Ciphertext::expand_seed -> sample_poly_uniform on a Blake2xbPRNG (ciphertext.cpp:118-150, util/rlwe.cpp:104-132,
- * randomgen.cpp:204-214), bit for bit -- so a fresh ciphertext crosses PCIe with half its bytes.  zlib-compressed objects
- * (compr_mode_type::zlib, serialization.cpp:236-300, util/ztools.cpp) are inflated on the host with the system's zlib before
- * they are parsed; zstd streams and the shake256 PRNG stay with the reference: load rejects them. */
+ * the device -- Ciphertext::expand_seed -> sample_poly_uniform on the PRNG the stream names, Blake2xbPRNG or Shake256PRNG
+ * (ciphertext.cpp:118-150, util/rlwe.cpp:104-132, randomgen.cpp:163-227), bit for bit -- so a fresh ciphertext crosses PCIe with
+ * half its bytes; one batch may mix both types and unseeded members.  zlib-compressed objects (compr_mode_type::zlib,
+ * serialization.cpp:236-300, util/ztools.cpp) are inflated on the host with the system's zlib before they are parsed; zstd
+ * streams stay with the reference: load rejects them. */
 typedef struct sb200_ct_info
 {
     uint64_t parms_id[4];         /* Ciphertext::parms_id() */
@@ -317,6 +321,11 @@ int sb200_public_key_create(sb200_context *ctx, const uint64_t *h_public_key, sb
 int sb200_public_key_destroy(sb200_public_key *key);
 int sb200_encrypt_zero_asymmetric(sb200_context *ctx, sb200_public_key *key, size_t L, size_t batch, const uint64_t *h_seeds,
                                   uint64_t *d_out, void *stream);
+/* the same with the PRNG type of parms.random_generator(), which draws u and both noise polynomials (util/rlwe.cpp:224):
+ * prng = SEAL's prng_type, 1 = blake2xb (sb200_encrypt_zero_asymmetric), 2 = shake256 (Shake256PRNG, randomgen.cpp:216-227:
+ * buffer b = SHAKE256(seed || b, 4096 bytes)); any other value returns SB200_E_INVALID_ARG. */
+int sb200_encrypt_zero_asymmetric_prng(sb200_context *ctx, sb200_public_key *key, size_t L, size_t batch, int prng, const uint64_t *h_seeds,
+                                       uint64_t *d_out, void *stream);
 
 /* ---- CKKSEncoder (SURVEY 8f: the data format either side of the path): CKKSEncoder::encode(values, parms_id, scale, plain) and
  * CKKSEncoder::decode(plain, values) (ckks.h:455-807) for a batch.  values = doubles: [batch][count] complex numbers as (re, im)
@@ -351,6 +360,14 @@ int sb200_secret_key_destroy(sb200_secret_key *key);
  * to obtain Encryptor::encrypt_symmetric (encryptor.cpp:199-262). */
 int sb200_encrypt_zero_symmetric(sb200_context *ctx, sb200_secret_key *key, size_t L, size_t batch, const uint64_t *h_bootstrap_seeds,
                                  int save_seed, uint64_t *d_out, uint64_t *h_public_seeds, void *stream);
+/* the same with both PRNG types given (SEAL's prng_type: 1 = blake2xb, 2 = shake256; any other value returns SB200_E_INVALID_ARG).
+ * bootstrap_prng = the type of parms.random_generator(), which draws the public seed and the noise (util/rlwe.cpp:322);
+ * ciphertext_prng = the type c_1 is expanded with, UniformRandomGeneratorFactory::DefaultFactory() (util/rlwe.cpp:329), i.e. the
+ * SEAL_DEFAULT_PRNG the reference was built with; a seeded stream of the result names this type.
+ * sb200_encrypt_zero_symmetric = this with 1, 1. */
+int sb200_encrypt_zero_symmetric_prng(sb200_context *ctx, sb200_secret_key *key, size_t L, size_t batch, int bootstrap_prng,
+                                      int ciphertext_prng, const uint64_t *h_bootstrap_seeds, int save_seed, uint64_t *d_out,
+                                      uint64_t *h_public_seeds, void *stream);
 /* d_ct [batch][size][L][n] in the scheme's own form -> d_plain: CKKS [batch][L][n] (NTT form, same level; the caller keeps
  * scale and parms_id); BFV [batch][n] coefficients mod t (dot product + decrypt_scale_and_round, rns.cpp:1133-1191);
  * BGV [batch][n] (dot product, INTT, exact base conversion rns.cpp:466-539, times the inverse of the ciphertext's

@@ -5,11 +5,14 @@
 //     seal_b200::Encryptor encryptor(context, public_key, evaluator);   // or (context, secret_key, evaluator), or both keys
 //     encryptor.encrypt(plain, ct);  encryptor.encrypt_symmetric(plain, ct);
 //
-// The PRNG stream (Blake2xb), the uniform polynomial, the centred binomial noise and c_0 = -(c_1 s + e) run on the device
-// (sb200_encrypt_zero_symmetric); the bootstrap seed of every encryption is drawn from the context's own random generator factory
-// (parms.random_generator()->create(), util/rlwe.cpp:288-292), so a context with a seeded factory reproduces the reference's
-// ciphertexts bit for bit and the default factory draws from the OS entropy source as the reference does.  Public-key encryption
-// (ternary u, two noise polynomials, the sample one level up divided down: sb200_encrypt_zero_asymmetric) follows the same rule.
+// The PRNG stream (Blake2xb or SHAKE256), the uniform polynomial, the centred binomial noise and c_0 = -(c_1 s + e) run on the
+// device (sb200_encrypt_zero_symmetric_prng); the bootstrap seed of every encryption is drawn from the context's own random
+// generator factory (parms.random_generator()->create(), util/rlwe.cpp:288-292), whose PRNG type the device follows, so a context
+// with a seeded factory (Blake2xbPRNGFactory or Shake256PRNGFactory) reproduces the reference's ciphertexts bit for bit and the
+// default factory draws from the OS entropy source as the reference does.  c_1 is expanded with the PRNG type of
+// UniformRandomGeneratorFactory::DefaultFactory() (util/rlwe.cpp:329), i.e. of the reference this header is compiled against.
+// Public-key encryption (ternary u, two noise polynomials, the sample one level up divided down:
+// sb200_encrypt_zero_asymmetric_prng) follows the same rule.  Only a custom factory (prng_type::unknown) is rejected.
 // The plaintext is added by the evaluator's device path.  The Serializable<Ciphertext> overloads (seeded output) stay with
 // seal::Encryptor: Serializable<> cannot be constructed outside the reference.
 #pragma once
@@ -140,8 +143,9 @@ namespace seal_b200
             DeviceSlab &operator=(const DeviceSlab &) = delete;
         };
 
-        // the bootstrap seeds of `count` encryptions, drawn exactly where the reference draws them (util/rlwe.cpp:288-292)
-        std::vector<std::uint64_t> bootstrap_seeds(std::size_t count) const
+        // the bootstrap seeds of `count` encryptions, drawn exactly where the reference draws them (util/rlwe.cpp:288-292), and the
+        // prng_type of their PRNGs (1 = blake2xb, 2 = shake256)
+        std::vector<std::uint64_t> bootstrap_seeds(std::size_t count, int &type) const
         {
             auto factory = context_.key_context_data()->parms().random_generator();
             if (!factory)
@@ -150,13 +154,19 @@ namespace seal_b200
             for (std::size_t b = 0; b < count; b++)
             {
                 auto prng = factory->create();
-                if (prng->info().type() != seal::prng_type::blake2xb)
-                    throw std::logic_error("unsupported prng_type: the device path implements Blake2xbPRNG");
+                type = prng_type_of(*prng);
                 const seal::prng_seed_type seed = prng->seed();
                 static_assert(sizeof(seed) == 64, "prng_seed_type is 512 bits");
                 std::memcpy(seeds.data() + b * 8, seed.data(), 64);
             }
             return seeds;
+        }
+        static int prng_type_of(seal::UniformRandomGenerator &prng)
+        {
+            const seal::prng_type t = prng.info().type();
+            if (t != seal::prng_type::blake2xb && t != seal::prng_type::shake256)
+                throw std::logic_error("unsupported prng_type: the device path implements Blake2xbPRNG and Shake256PRNG");
+            return static_cast<int>(t);
         }
 
         // encrypt_zero_internal (encryptor.cpp:88-174, symmetric branch) for `count` ciphertexts into a device slab that is either
@@ -175,13 +185,15 @@ namespace seal_b200
                 throw std::invalid_argument("parms_id is not valid for encryption parameters");
             auto &parms = cd->parms();
             const std::size_t L = parms.coeff_modulus().size(), n = parms.poly_modulus_degree(), words = 2 * L * n;
-            std::vector<std::uint64_t> seeds = bootstrap_seeds(count);
+            int prng = 0;
+            std::vector<std::uint64_t> seeds = bootstrap_seeds(count, prng);
+            const int ct_prng = prng_type_of(*seal::UniformRandomGeneratorFactory::DefaultFactory()->create());
             DeviceSlab local(ctx_, d_keep ? 1 : count * words);
             std::uint64_t *d = d_keep ? d_keep->d : local.d;
             if (is_asymmetric)
-                status(sb200_encrypt_zero_asymmetric(ctx_, pk_, L, count, seeds.data(), d, nullptr));
+                status(sb200_encrypt_zero_asymmetric_prng(ctx_, pk_, L, count, prng, seeds.data(), d, nullptr));
             else
-                status(sb200_encrypt_zero_symmetric(ctx_, key_, L, count, seeds.data(), 0, d, nullptr, nullptr));
+                status(sb200_encrypt_zero_symmetric_prng(ctx_, key_, L, count, prng, ct_prng, seeds.data(), 0, d, nullptr, nullptr));
             seal::util::seal_memzero(seeds.data(), seeds.size() * sizeof(std::uint64_t)); // the seeds determine the noise
             const bool ntt = parms.scheme() != seal::scheme_type::bfv;
             for (std::size_t b = 0; b < count; b++)

@@ -33,7 +33,7 @@ SYMBOLS = [
     "sb200_relinearize_host", "sb200_multiply_relinearize_host", "sb200_rescale_to_next_host",
     "sb200_mod_switch_to_next_host", "sb200_apply_galois_host", "sb200_get_parms_id", "sb200_ciphertext_inspect",
     "sb200_ciphertext_save_size", "sb200_ciphertext_load", "sb200_ciphertext_save", "sb200_secret_key_create",
-    "sb200_secret_key_destroy", "sb200_decrypt", "sb200_decrypt_host", "sb200_encrypt_zero_symmetric", "sb200_public_key_create", "sb200_public_key_destroy", "sb200_encrypt_zero_asymmetric", "sb200_ckks_encode", "sb200_ckks_decode", "sb200_ckks_encode_host", "sb200_ckks_decode_host",
+    "sb200_secret_key_destroy", "sb200_decrypt", "sb200_decrypt_host", "sb200_encrypt_zero_symmetric", "sb200_public_key_create", "sb200_public_key_destroy", "sb200_encrypt_zero_asymmetric", "sb200_encrypt_zero_symmetric_prng", "sb200_encrypt_zero_asymmetric_prng", "sb200_ckks_encode", "sb200_ckks_decode", "sb200_ckks_encode_host", "sb200_ckks_decode_host",
     "sb200_group_create", "sb200_group_destroy", "sb200_group_size", "sb200_group_context", "sb200_group_slice",
     "sb200_group_kswitch_key_create", "sb200_group_kswitch_key_destroy", "sb200_group_multiply_relinearize_host",
     "sb200_group_relinearize_host", "sb200_group_apply_galois_host", "sb200_group_multiply_host", "sb200_group_rescale_to_next_host",
@@ -150,6 +150,8 @@ def lib():
         L.sb200_public_key_destroy.argtypes = [vp]
         L.sb200_encrypt_zero_asymmetric.argtypes = [vp, vp, sz, sz, _u64p, vp, vp]
         L.sb200_encrypt_zero_symmetric.argtypes = [vp, vp, sz, sz, _u64p, i32, vp, _u64p, vp]
+        L.sb200_encrypt_zero_asymmetric_prng.argtypes = [vp, vp, sz, sz, i32, _u64p, vp, vp]
+        L.sb200_encrypt_zero_symmetric_prng.argtypes = [vp, vp, sz, sz, i32, i32, _u64p, i32, vp, _u64p, vp]
         L.sb200_decrypt_host.argtypes = [vp, vp, sz, sz, sz, _u64p, _u64p, _u64p]
         _lib = L
     return _lib
@@ -638,19 +640,24 @@ class Context:
     def load_public_key(self, host_key):
         return PublicKey(self, host_key)
 
-    def d_encrypt_zero_asymmetric(self, pk, out2, L, batch, seeds=None):
+    def d_encrypt_zero_asymmetric(self, pk, out2, L, batch, seeds=None, prng=1):
         """Encryptor(public key).encrypt_zero for a batch into the device slab out2 [batch][2][L][n]; seeds [batch][8] words (None =
-        fresh from the OS entropy source)"""
+        fresh from the OS entropy source) of PRNGs of type prng (SEAL's prng_type: 1 = blake2xb, 2 = shake256)"""
         seeds = None if seeds is None else np.ascontiguousarray(seeds, dtype=np.uint64).reshape(batch, 8)
-        _check(lib().sb200_encrypt_zero_asymmetric(self.h, pk.h, L, batch, None if seeds is None else _hp(seeds), _dp(out2), self._stream()))
+        _check(lib().sb200_encrypt_zero_asymmetric_prng(self.h, pk.h, L, batch, prng, None if seeds is None else _hp(seeds), _dp(out2),
+                                                        self._stream()))
 
-    def d_encrypt_zero_symmetric(self, sk, out2, L, batch, bootstrap_seeds=None, save_seed=False, want_public_seeds=False):
+    def d_encrypt_zero_symmetric(self, sk, out2, L, batch, bootstrap_seeds=None, save_seed=False, want_public_seeds=False,
+                                 bootstrap_prng=1, ciphertext_prng=1):
         """Encryptor.encrypt_zero_symmetric for a batch into the device slab out2 [batch][2][L][n]; bootstrap_seeds [batch][8] words
-        (None = fresh from the OS entropy source); returns the public seeds [batch][8] when asked for (the seeded wire form)"""
+        (None = fresh from the OS entropy source); returns the public seeds [batch][8] when asked for (the seeded wire form).
+        bootstrap_prng = prng_type of the bootstrap PRNGs (the parameters' random generator), ciphertext_prng = the one c_1 is expanded
+        with (the reference's default factory); 1 = blake2xb, 2 = shake256"""
         seeds = None if bootstrap_seeds is None else np.ascontiguousarray(bootstrap_seeds, dtype=np.uint64).reshape(batch, 8)
         pub = np.zeros((batch, 8), dtype=np.uint64) if want_public_seeds else None
-        _check(lib().sb200_encrypt_zero_symmetric(self.h, sk.h, L, batch, None if seeds is None else _hp(seeds), int(save_seed), _dp(out2),
-                                                  None if pub is None else _hp(pub), self._stream()))
+        _check(lib().sb200_encrypt_zero_symmetric_prng(self.h, sk.h, L, batch, bootstrap_prng, ciphertext_prng,
+                                                       None if seeds is None else _hp(seeds), int(save_seed), _dp(out2),
+                                                       None if pub is None else _hp(pub), self._stream()))
         return pub
 
     def d_relinearize(self, in3, key, out2, L, batch):

@@ -681,10 +681,29 @@ int sb200_kswitch_key_load(sb200_context *ctx, const uint8_t *stream, size_t len
     std::lock_guard<std::mutex> lock(c.mu);
     cuda_check(cudaSetDevice(c.device), "cudaSetDevice");
     cuda_check(cudaMalloc(reinterpret_cast<void **>(&h->k.d_key), digits * row), "cudaMalloc(key)");
-    for (size_t j = 0; j < digits; j++)
-        cuda_check(cudaMemcpy(reinterpret_cast<uint8_t *>(h->k.d_key) + j * row, stream + e.offsets[j], row, cudaMemcpyHostToDevice), "upload key");
     h->k.ctx = &c;
     h->k.digits = digits;
+    // a seed-compressed member carries c_0 only (k n words) and the seed of c_1 = sample_poly_uniform at the key level
+    // (KSwitchKeys::load -> PublicKey::load -> Ciphertext::expand_seed, ciphertext.cpp:118-150)
+    std::vector<u64> seeds;
+    std::vector<int> types;
+    std::vector<long long> seed_dst;
+    for (size_t j = 0; j < digits; j++)
+    {
+        cuda_check(cudaMemcpy(reinterpret_cast<uint8_t *>(h->k.d_key) + j * row, stream + e.offsets[j], e.seeded[j] ? row / 2 : row,
+                              cudaMemcpyHostToDevice),
+                   "upload key");
+        if (e.seeded[j])
+        {
+            u64 sd[8];
+            std::memcpy(sd, stream + e.seed_offsets[j], sizeof(sd));
+            seeds.insert(seeds.end(), sd, sd + 8);
+            types.push_back(e.seeded[j]);
+            seed_dst.push_back(static_cast<long long>((2 * j + 1) * c.k * c.n));
+        }
+    }
+    if (!seed_dst.empty())
+        op_expand_seeded(c, c.k, seed_dst.size(), seeds.data(), types.data(), seed_dst.data(), h->k.d_key, nullptr);
     if (!op_residues_in_range(c, c.k, digits * 2 * c.k, h->k.d_key, nullptr)) // KSwitchKeys::load ends in is_valid_for (kswitchkeys.cpp:149-153)
         throw std::logic_error("KSwitchKeys data is invalid");
     ksint_prepare_key(c, h->k, nullptr);
@@ -1423,8 +1442,11 @@ int sb200_ciphertext_load(sb200_context *ctx, size_t batch, const uint8_t *const
     check_level(c, L, batch);
     auto st = static_cast<cudaStream_t>(stream);
     const size_t words = size * L * c.n;
-    std::vector<u64> seeds;            // seeded members: 8 words each
-    std::vector<long long> seed_dst;   // word offset of their second polynomial in d_out
+    // seeded members, blake2xb ones first so that each PRNG type is one launch: 8 words of seed each, the prng_type, and the word
+    // offset of their second polynomial in d_out
+    std::vector<u64> seeds[2];
+    std::vector<int> types[2];
+    std::vector<long long> seed_dst[2];
     for (size_t b = 0; b < batch; b++)
     {
         sb200_ct_info info;
@@ -1440,8 +1462,6 @@ int sb200_ciphertext_load(sb200_context *ctx, size_t batch, const uint8_t *const
         }
         else
             sbw::inspect(src, lens[b], info);
-        if (info.seeded == 2)
-            throw std::logic_error("unsupported prng_type"); // shake256 streams stay with the reference (ciphertext.cpp:124-128)
         // is_metadata_valid_for (ciphertext.cpp:299-302): the stream must belong to this context at the level asked for
         if (info.poly_modulus_degree != c.n || info.coeff_modulus_size != L || info.size != size ||
             std::memcmp(info.parms_id, c.parms_ids[L - 1].data(), sizeof(info.parms_id)) != 0)
@@ -1450,16 +1470,21 @@ int sb200_ciphertext_load(sb200_context *ctx, size_t batch, const uint8_t *const
             infos[b] = info;
         // (pageable source: the call returns once the bytes have left the buffer, so `plain` may go out of scope)
         cuda_check(cudaMemcpyAsync(d_out + b * words, src + info.data_offset, info.data_words * sizeof(u64), cudaMemcpyHostToDevice, st), "H2D");
-        if (info.seeded)
+        if (info.seeded) // UniformRandomGeneratorInfo::make_prng: the stream names its PRNG (randomgen.cpp:163-177)
         {
+            const int t = info.seeded == kPrngShake256;
             u64 sd[8];
             std::memcpy(sd, src + info.seed_offset, sizeof(sd));
-            seeds.insert(seeds.end(), sd, sd + 8);
-            seed_dst.push_back(static_cast<long long>(b * words + L * c.n));
+            seeds[t].insert(seeds[t].end(), sd, sd + 8);
+            types[t].push_back(info.seeded);
+            seed_dst[t].push_back(static_cast<long long>(b * words + L * c.n));
         }
     }
-    if (!seed_dst.empty())
-        op_expand_seeded(c, L, seed_dst.size(), seeds.data(), seed_dst.data(), reinterpret_cast<u64 *>(d_out), st); // Ciphertext::expand_seed
+    seeds[0].insert(seeds[0].end(), seeds[1].begin(), seeds[1].end());
+    types[0].insert(types[0].end(), types[1].begin(), types[1].end());
+    seed_dst[0].insert(seed_dst[0].end(), seed_dst[1].begin(), seed_dst[1].end());
+    if (!seed_dst[0].empty()) // Ciphertext::expand_seed
+        op_expand_seeded(c, L, seed_dst[0].size(), seeds[0].data(), types[0].data(), seed_dst[0].data(), reinterpret_cast<u64 *>(d_out), st);
     if (validate && !op_residues_in_range(c, L, batch * size * L, reinterpret_cast<const u64 *>(d_out), st))
         throw std::logic_error("ciphertext data is invalid"); // Ciphertext::load -> is_valid_for (ciphertext.h:640-655)
     return SB200_OK;
@@ -1562,6 +1587,12 @@ namespace
 int sb200_encrypt_zero_asymmetric(sb200_context *ctx, sb200_public_key *key, size_t L, size_t batch, const uint64_t *h_seeds, uint64_t *d_out,
                                   void *stream)
 {
+    return sb200_encrypt_zero_asymmetric_prng(ctx, key, L, batch, kPrngBlake2xb, h_seeds, d_out, stream);
+}
+
+int sb200_encrypt_zero_asymmetric_prng(sb200_context *ctx, sb200_public_key *key, size_t L, size_t batch, int prng, const uint64_t *h_seeds,
+                                       uint64_t *d_out, void *stream)
+{
     SB_NEED(key);
     SB_NEED(d_out);
     SB_TRY
@@ -1574,7 +1605,8 @@ int sb200_encrypt_zero_asymmetric(sb200_context *ctx, sb200_public_key *key, siz
         h_seeds = reinterpret_cast<const uint64_t *>(fresh->words.data());
     }
     // returns after a stream synchronisation: the seeds may be wiped
-    op_encrypt_zero_asymmetric(c, key->k, L, batch, (const u64 *)h_seeds, (u64 *)d_out, static_cast<cudaStream_t>(stream));
+    check_prng_type(prng);
+    op_encrypt_zero_asymmetric(c, key->k, L, batch, (const u64 *)h_seeds, prng, (u64 *)d_out, static_cast<cudaStream_t>(stream));
     return SB200_OK;
     SB_CATCH
 }
@@ -1605,6 +1637,13 @@ int sb200_ckks_decode_host(sb200_context *ctx, size_t L, size_t batch, const uin
 int sb200_encrypt_zero_symmetric(sb200_context *ctx, sb200_secret_key *key, size_t L, size_t batch, const uint64_t *h_bootstrap_seeds,
                                  int save_seed, uint64_t *d_out, uint64_t *h_public_seeds, void *stream)
 {
+    return sb200_encrypt_zero_symmetric_prng(ctx, key, L, batch, kPrngBlake2xb, kPrngBlake2xb, h_bootstrap_seeds, save_seed, d_out, h_public_seeds,
+                                             stream);
+}
+
+int sb200_encrypt_zero_symmetric_prng(sb200_context *ctx, sb200_secret_key *key, size_t L, size_t batch, int bootstrap_prng, int ciphertext_prng,
+                                      const uint64_t *h_bootstrap_seeds, int save_seed, uint64_t *d_out, uint64_t *h_public_seeds, void *stream)
+{
     SB_NEED(key);
     SB_NEED(d_out);
     SB_TRY
@@ -1616,8 +1655,10 @@ int sb200_encrypt_zero_symmetric(sb200_context *ctx, sb200_secret_key *key, size
         fresh = std::make_unique<FreshSeeds>(batch);
         h_bootstrap_seeds = reinterpret_cast<const uint64_t *>(fresh->words.data());
     }
-    op_encrypt_zero_symmetric(c, key->k, L, batch, (const u64 *)h_bootstrap_seeds, save_seed != 0, (u64 *)d_out, (u64 *)h_public_seeds,
-                              static_cast<cudaStream_t>(stream));
+    check_prng_type(bootstrap_prng);
+    check_prng_type(ciphertext_prng);
+    op_encrypt_zero_symmetric(c, key->k, L, batch, (const u64 *)h_bootstrap_seeds, bootstrap_prng, ciphertext_prng, save_seed != 0, (u64 *)d_out,
+                              (u64 *)h_public_seeds, static_cast<cudaStream_t>(stream));
     // op_encrypt_zero_symmetric synchronised the stream while expanding c_1: the seeds have been consumed and may be wiped
     return SB200_OK;
     SB_CATCH

@@ -196,15 +196,22 @@ namespace sb
     size_t keyswitch_chunk(const Context &c, size_t L, size_t batch, bool fused);
     // arithmetic ceilings measured in process: warp-level butterflies (kind 0-2) / multiply-accumulates (kind 3) per second
     double selftest_rate(Context &c, int kind, cudaStream_t st);
-    // Ciphertext::expand_seed on the device (sb_prng.cu): seeds [B][8] host words, dst_off [B] host word offsets into d_out of the
-    // polynomial ([L][n]) each seed expands into; returns after the expansion has been enqueued and the host arrays are free
-    void op_expand_seeded(Context &c, size_t L, size_t B, const u64 *h_seeds, const long long *h_dst_off, u64 *d_out, cudaStream_t st);
-    // Encryptor::encrypt_zero_symmetric on the device (sb_prng.cu): bootstrap seeds [B][8] on the host, out [B][2][L][n]
-    void op_encrypt_zero_symmetric(Context &c, const SecretKey &sk, size_t L, size_t B, const u64 *h_boot_seeds, bool save_seed, u64 *d_out,
-                                   u64 *h_public_seeds, cudaStream_t st);
-    // Encryptor(public key)::encrypt_zero on the device (sb_prng.cu): seeds [B][8] on the host, out [B][2][L][n]
+    // SEAL's prng_type (randomgen.h:29-36) of a PRNG whose stream the device generates (sb_prng.cu); anything else is rejected by
+    // check_prng_type (std::invalid_argument)
+    constexpr int kPrngBlake2xb = 1, kPrngShake256 = 2;
+    void check_prng_type(int type);
+    // Ciphertext::expand_seed on the device (sb_prng.cu): seeds [B][8] host words, types [B] their prng_type, dst_off [B] host word
+    // offsets into d_out of the polynomial ([L][n]) each seed expands into; returns after the expansion has been enqueued and the
+    // host arrays are free
+    void op_expand_seeded(Context &c, size_t L, size_t B, const u64 *h_seeds, const int *h_types, const long long *h_dst_off, u64 *d_out,
+                          cudaStream_t st);
+    // Encryptor::encrypt_zero_symmetric on the device (sb_prng.cu): bootstrap seeds [B][8] on the host, out [B][2][L][n]; boot_prng =
+    // the type of the bootstrap PRNG (parms.random_generator()), ct_prng = the type c_1 is expanded with (the DefaultFactory's)
+    void op_encrypt_zero_symmetric(Context &c, const SecretKey &sk, size_t L, size_t B, const u64 *h_boot_seeds, int boot_prng, int ct_prng,
+                                   bool save_seed, u64 *d_out, u64 *h_public_seeds, cudaStream_t st);
+    // Encryptor(public key)::encrypt_zero on the device (sb_prng.cu): seeds [B][8] on the host for PRNGs of type prng, out [B][2][L][n]
     void public_key_create(Context &c, const u64 *h_pk, PublicKey &out);
-    void op_encrypt_zero_asymmetric(Context &c, const PublicKey &pk, size_t L, size_t B, const u64 *h_seeds, u64 *d_out, cudaStream_t st);
+    void op_encrypt_zero_asymmetric(Context &c, const PublicKey &pk, size_t L, size_t B, const u64 *h_seeds, int prng, u64 *d_out, cudaStream_t st);
     // CKKSEncoder::encode / decode (sb_ckks.cu): values = device doubles, [B][count] complex pairs (or reals); plain = [B][L][n] NTT form
     void op_ckks_encode(Context &c, size_t L, size_t B, const double *values, size_t count, bool is_complex, double scale, u64 *plain,
                         cudaStream_t st);

@@ -8,12 +8,13 @@
 // fresh ciphertext moves over PCIe.  What is reproduced, bit for bit:
 //   * the PRNG stream: buffer b (4096 bytes) = BLAKE2Xb(out 4096, in = 64-bit counter b, key = seed)  -- RFC 7693 BLAKE2b with
 //     the BLAKE2X parameter block: a keyed root hash over the counter, then 64 output blocks B_i = BLAKE2b(root) whose
-//     parameter block carries node_offset = i and xof_length = 4096 (util/blake2xb.c);
+//     parameter block carries node_offset = i and xof_length = 4096 (util/blake2xb.c); or, when the stream names prng_type
+//     shake256, buffer b = SHAKE256(seed || b, 4096 bytes) (Shake256PRNG, randomgen.cpp:216-227; FIPS 202);
 //   * sample_poly_uniform: the first L*n words of the stream fill the polynomial; every word >= max_multiple of its prime
 //     (rejection sampling for uniformity) is replaced, in coefficient order, by the next words of the stream; the survivors are
 //     reduced modulo the prime.
-// Parallel schedule: one thread per 64-byte output block generates the stream (root hash recomputed per thread: 3 compressions
-// per block), one CTA per ciphertext lists the rejected coefficients in order (two passes with a block-wide scan), one thread per
+// Parallel schedule: one thread per 64-byte output block generates a BLAKE2Xb stream (root hash recomputed per thread: 3
+// compressions per block), one thread per 4096-byte buffer a SHAKE256 stream (31 permutations in sequence; prng_stream picks), one CTA per ciphertext lists the rejected coefficients in order (two passes with a block-wide scan), one thread per
 // ciphertext consumes the replacement words (a few thousand sequential steps at n = 65536, 31 primes), one streaming kernel reduces.
 #include "sb_engine.cuh"
 
@@ -113,6 +114,88 @@ namespace sb
                 dst[i] = o[i];
         }
 
+        // Keccak-f[1600] (FIPS 202 section 3), lanes a[x + 5 y].  Every 64-bit rotation is two funnel shifts of the 32-bit halves
+        // (the shift amounts are constants once the round body is unrolled); chi's a ^ (~b & c) is one three-input logic op per half.
+        __constant__ u64 c_keccak_rc[24] = {
+            0x0000000000000001ull, 0x0000000000008082ull, 0x800000000000808Aull, 0x8000000080008000ull, 0x000000000000808Bull,
+            0x0000000080000001ull, 0x8000000080008081ull, 0x8000000000008009ull, 0x000000000000008Aull, 0x0000000000000088ull,
+            0x0000000080008009ull, 0x000000008000000Aull, 0x000000008000808Bull, 0x800000000000008Bull, 0x8000000000008089ull,
+            0x8000000000008003ull, 0x8000000000008002ull, 0x8000000000000080ull, 0x000000000000800Aull, 0x800000008000000Aull,
+            0x8000000080008081ull, 0x8000000000008080ull, 0x0000000080000001ull, 0x8000000080008008ull
+        };
+        __device__ __forceinline__ u64 rotl64(u64 v, int s)
+        {
+            const unsigned lo = static_cast<unsigned>(v), hi = static_cast<unsigned>(v >> 32);
+            unsigned rl, rh;
+            if (s == 0)
+                return v;
+            if (s < 32)
+                rh = __funnelshift_l(lo, hi, s), rl = __funnelshift_l(hi, lo, s);
+            else
+                rh = __funnelshift_l(hi, lo, s - 32), rl = __funnelshift_l(lo, hi, s - 32);
+            return (static_cast<u64>(rh) << 32) | rl;
+        }
+        __device__ __forceinline__ void keccak_f1600(u64 (&a)[25])
+        {
+            // rho offsets r[x + 5 y] (FIPS 202 table 2)
+            constexpr int rho[25] = { 0, 1, 62, 28, 27, 36, 44, 6, 55, 20, 3, 10, 43, 25, 39, 41, 45, 15, 21, 8, 18, 2, 61, 56, 14 };
+#pragma unroll 1
+            for (int r = 0; r < 24; r++)
+            {
+                u64 c[5], d[5], t[25];
+#pragma unroll
+                for (int x = 0; x < 5; x++) // theta
+                    c[x] = a[x] ^ a[x + 5] ^ a[x + 10] ^ a[x + 15] ^ a[x + 20];
+#pragma unroll
+                for (int x = 0; x < 5; x++)
+                    d[x] = c[(x + 4) % 5] ^ rotl64(c[(x + 1) % 5], 1);
+#pragma unroll
+                for (int y = 0; y < 5; y++) // rho and pi: lane (x, y) moves to (y, 2x + 3y)
+#pragma unroll
+                    for (int x = 0; x < 5; x++)
+                        t[y + 5 * ((2 * x + 3 * y) % 5)] = rotl64(a[x + 5 * y] ^ d[x], rho[x + 5 * y]);
+#pragma unroll
+                for (int y = 0; y < 5; y++) // chi
+#pragma unroll
+                    for (int x = 0; x < 5; x++)
+                        a[x + 5 * y] = t[x + 5 * y] ^ (~t[(x + 1) % 5 + 5 * y] & t[(x + 2) % 5 + 5 * y]);
+                a[0] ^= c_keccak_rc[r]; // iota
+            }
+        }
+
+        // thread = one PRNG buffer of one ciphertext, Shake256PRNG::refill_buffer (randomgen.cpp:216-227): W[b][buffer*512 .. +512) =
+        // SHAKE256(seed (64 bytes) || buffer index (8 bytes, little-endian), 4096 bytes).  The 72-byte message fits the 136-byte rate
+        // block: padding 0x1F at byte 72 and 0x80 at byte 135.  4096 bytes = 30 full squeezes of 17 lanes + 2 lanes of the 31st.
+        __global__ void __launch_bounds__(128) shake256_stream_kernel(const u64 *__restrict__ seeds, u64 *__restrict__ W, long long words_per_ct,
+                                                                       long long buffers_per_ct, long long total_buffers)
+        {
+            const long long g = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+            if (g >= total_buffers)
+                return;
+            const long long b = g / buffers_per_ct, buf = g % buffers_per_ct;
+            u64 a[25];
+#pragma unroll
+            for (int i = 0; i < 8; i++)
+                a[i] = seeds[b * 8 + i];
+            a[8] = static_cast<u64>(buf);
+            a[9] = 0x1Full;
+#pragma unroll
+            for (int i = 10; i < 25; i++)
+                a[i] = 0;
+            a[16] = 0x80ull << 56;
+            u64 *dst = W + b * words_per_ct + buf * kWordsPerBuffer;
+#pragma unroll 1
+            for (int s = 0; s < 30; s++, dst += 17)
+            {
+                keccak_f1600(a);
+#pragma unroll
+                for (int i = 0; i < 17; i++)
+                    dst[i] = a[i];
+            }
+            keccak_f1600(a);
+            dst[0] = a[0], dst[1] = a[1];
+        }
+
         // one CTA per ciphertext: list the rejected coefficients in order, then let one thread walk the replacement words
         __global__ void __launch_bounds__(1024) seed_reject_kernel(u64 *__restrict__ W, long long words_per_ct, const u64 *__restrict__ max_mult,
                                                                    unsigned *__restrict__ list, long long list_cap, int logn, int L, int *overflow)
@@ -188,15 +271,60 @@ namespace sb
         }
     } // namespace
 
-    // seeds: [B][8] words (prng_seed_type), on the host or (seeds_on_device) already on the device; dst_off: [B] host word offsets into
-    // d_out of the polynomial to fill ([L][n])
-    static void expand_impl(Context &c, size_t L, size_t B, const u64 *seeds, bool seeds_on_device, const long long *h_dst_off, u64 *d_out,
+    void check_prng_type(int type)
+    {
+        if (type != kPrngBlake2xb && type != kPrngShake256)
+            throw std::invalid_argument("prng_type is invalid"); // randomgen.h:29-36: unknown (0) makes no PRNG
+    }
+
+    // The one place that knows the PRNG formats: W[b][0, words_per_ct) = the output stream of ciphertext b's PRNG, whose type
+    // types[b] (host) is SEAL's prng_type and whose seed is d_seeds[b] (device, 8 words); words_per_ct is a whole number of 4096-byte
+    // buffers.  Every consumer reads the stream as one sequence of bytes, whichever PRNG made it.  A run of equal types is one
+    // launch; its profile entry is names[0] for blake2xb and names[1] for shake256 (string literals: the profile keeps the pointers).
+    static void prng_stream(Context &c, const char *const (&names)[2], const int *types, size_t B, const u64 *d_seeds, u64 *W, long long words_per_ct,
                             cudaStream_t st)
+    {
+        const long long buffers_per_ct = words_per_ct / kWordsPerBuffer;
+        for (size_t b0 = 0, b1; b0 < B; b0 = b1)
+        {
+            check_prng_type(types[b0]);
+            for (b1 = b0 + 1; b1 < B && types[b1] == types[b0];)
+                b1++;
+            const long long nb = static_cast<long long>(b1 - b0);
+            const u64 *seeds = d_seeds + b0 * 8;
+            u64 *w = W + b0 * words_per_ct;
+            if (types[b0] == kPrngBlake2xb)
+            {
+                const long long blocks_per_ct = words_per_ct / 8, total_blocks = blocks_per_ct * nb;
+                c.stats.begin(names[0], 0, 8.0 * nb * words_per_ct, st);
+                blake2xb_stream_kernel<<<static_cast<unsigned>((total_blocks + 127) / 128), 128, 0, st>>>(seeds, w, words_per_ct, blocks_per_ct,
+                                                                                                         total_blocks);
+                c.stats.end(st);
+                cuda_check(cudaGetLastError(), "blake2xb_stream_kernel");
+            }
+            else
+            {
+                const long long total_buffers = buffers_per_ct * nb;
+                c.stats.begin(names[1], 0, 8.0 * nb * words_per_ct, st);
+                shake256_stream_kernel<<<static_cast<unsigned>((total_buffers + 127) / 128), 128, 0, st>>>(seeds, w, words_per_ct, buffers_per_ct,
+                                                                                                          total_buffers);
+                c.stats.end(st);
+                cuda_check(cudaGetLastError(), "shake256_stream_kernel");
+            }
+        }
+    }
+
+    // seeds: [B][8] words (prng_seed_type), on the host or (seeds_on_device) already on the device; types: [B] host prng_type of each
+    // seed; dst_off: [B] host word offsets into d_out of the polynomial to fill ([L][n])
+    static void expand_impl(Context &c, size_t L, size_t B, const u64 *seeds, bool seeds_on_device, const int *types, const long long *h_dst_off,
+                            u64 *d_out, cudaStream_t st)
     {
         if (!B)
             return;
         if (L < 1 || L > c.k)
             throw std::invalid_argument("encrypted is not valid for encryption parameters");
+        for (size_t b = 0; b < B; b++)
+            check_prng_type(types[b]);
         const long long need = static_cast<long long>(L) * c.n;
         // rejection probability of prime j = (2^64 - max_multiple_j) / 2^64; spare stream words: twice the expectation + a margin
         std::vector<u64> mm(L);
@@ -225,11 +353,7 @@ namespace sb
             cuda_check(cudaMemcpyAsync(d_off, h_dst_off, B * sizeof(long long), cudaMemcpyHostToDevice, st), "offsets H2D");
             cuda_check(cudaMemcpyAsync(d_mm, mm.data(), L * sizeof(u64), cudaMemcpyHostToDevice, st), "thresholds H2D");
             cuda_check(cudaMemsetAsync(d_flag, 0, sizeof(int), st), "memset");
-            const long long blocks_per_ct = words_per_ct / 8, total_blocks = blocks_per_ct * static_cast<long long>(B);
-            c.stats.begin("seed_stream", 0, 8.0 * B * words_per_ct, st);
-            blake2xb_stream_kernel<<<static_cast<unsigned>((total_blocks + 127) / 128), 128, 0, st>>>(d_seeds, W, words_per_ct, blocks_per_ct, total_blocks);
-            c.stats.end(st);
-            cuda_check(cudaGetLastError(), "blake2xb_stream_kernel");
+            prng_stream(c, { "seed_stream", "seed_stream:shake256" }, types, B, d_seeds, W, words_per_ct, st);
             c.stats.begin("seed_reject", 0, 16.0 * B * need, st);
             seed_reject_kernel<<<static_cast<unsigned>(B), 1024, 0, st>>>(W, words_per_ct, d_mm, list, list_cap, c.logn, static_cast<int>(L), d_flag);
             c.stats.end(st);
@@ -250,9 +374,10 @@ namespace sb
         throw std::logic_error("seed expansion ran out of random words");
     }
 
-    void op_expand_seeded(Context &c, size_t L, size_t B, const u64 *h_seeds, const long long *h_dst_off, u64 *d_out, cudaStream_t st)
+    void op_expand_seeded(Context &c, size_t L, size_t B, const u64 *h_seeds, const int *h_types, const long long *h_dst_off, u64 *d_out,
+                          cudaStream_t st)
     {
-        expand_impl(c, L, B, h_seeds, false, h_dst_off, d_out, st);
+        expand_impl(c, L, B, h_seeds, false, h_types, h_dst_off, d_out, st);
     }
 
     // ------------------------------------------------------------------------------------------------------------------------------
@@ -325,9 +450,11 @@ namespace sb
 
     // h_boot_seeds [B][8]: the seeds of the bootstrap PRNGs (one fresh seed per ciphertext); d_out [B][2][L][n];
     // h_public_seeds: nullptr or [B][8], receives the seed c_1 of each ciphertext expands from (what Serializable<Ciphertext> stores)
-    void op_encrypt_zero_symmetric(Context &c, const SecretKey &sk, size_t L, size_t B, const u64 *h_boot_seeds, bool save_seed, u64 *d_out,
-                                   u64 *h_public_seeds, cudaStream_t st)
+    void op_encrypt_zero_symmetric(Context &c, const SecretKey &sk, size_t L, size_t B, const u64 *h_boot_seeds, int boot_prng, int ct_prng,
+                                   bool save_seed, u64 *d_out, u64 *h_public_seeds, cudaStream_t st)
     {
+        check_prng_type(boot_prng);
+        check_prng_type(ct_prng);
         if (!B)
             return;
         if (L < 1 || L > c.k || (c.k > 1 && L == c.k))
@@ -351,16 +478,13 @@ namespace sb
             cuda_check(cudaMemcpyAsync(d_mult, h_mult.data(), L * sizeof(u64), cudaMemcpyHostToDevice, st), "t mod q H2D");
             mult = d_mult;
         }
-        const long long blocks_per_ct = boot_words / 8, total_blocks = blocks_per_ct * static_cast<long long>(B);
-        c.stats.begin("enc_bootstrap_stream", 0, 8.0 * B * boot_words, st);
-        blake2xb_stream_kernel<<<static_cast<unsigned>((total_blocks + 127) / 128), 128, 0, st>>>(d_boot_seeds, Wb, boot_words, blocks_per_ct, total_blocks);
-        c.stats.end(st);
-        cuda_check(cudaGetLastError(), "blake2xb_stream_kernel");
+        const std::vector<int> boot_types(B, boot_prng), ct_types(B, ct_prng);
+        prng_stream(c, { "enc_bootstrap_stream", "enc_bootstrap_stream:shake256" }, boot_types.data(), B, d_boot_seeds, Wb, boot_words, st);
         cuda_check(cudaMemcpy2DAsync(d_pub, 64, Wb, boot_bytes, 64, B, cudaMemcpyDeviceToDevice, st), "public seeds");
         std::vector<long long> off(B);
         for (size_t b = 0; b < B; b++)
             off[b] = static_cast<long long>(b) * 2 * poly + poly;
-        expand_impl(c, L, B, d_pub, true, off.data(), d_out, st); // c_1 (synchronises the stream: the host vectors above are free)
+        expand_impl(c, L, B, d_pub, true, ct_types.data(), off.data(), d_out, st); // c_1 (synchronises the stream: the host vectors above are free)
         if (h_public_seeds)
             cuda_check(cudaMemcpyAsync(h_public_seeds, d_pub, B * 8 * sizeof(u64), cudaMemcpyDeviceToHost, st), "public seeds D2H");
         const unsigned grid = static_cast<unsigned>((total + 255) / 256);
@@ -514,8 +638,9 @@ namespace sb
     }
 
     // h_seeds [B][8]: the seed of each ciphertext's PRNG; d_out [B][2][L][n] at the level with L primes (L == k: the key level)
-    void op_encrypt_zero_asymmetric(Context &c, const PublicKey &pk, size_t L, size_t B, const u64 *h_seeds, u64 *d_out, cudaStream_t st)
+    void op_encrypt_zero_asymmetric(Context &c, const PublicKey &pk, size_t L, size_t B, const u64 *h_seeds, int prng, u64 *d_out, cudaStream_t st)
     {
+        check_prng_type(prng);
         if (!B)
             return;
         if (L < 1 || L > c.k)
@@ -546,11 +671,8 @@ namespace sb
             cuda_check(cudaMemcpyAsync(d_mult, h_mult.data(), Lp * sizeof(u64), cudaMemcpyHostToDevice, st), "t mod q H2D");
             mult = d_mult;
         }
-        const long long blocks_per_ct = words / 8, total_blocks = blocks_per_ct * static_cast<long long>(B);
-        c.stats.begin("enc_stream", 0, 8.0 * B * words, st);
-        blake2xb_stream_kernel<<<static_cast<unsigned>((total_blocks + 127) / 128), 128, 0, st>>>(d_seeds, W, words, blocks_per_ct, total_blocks);
-        c.stats.end(st);
-        cuda_check(cudaGetLastError(), "blake2xb_stream_kernel");
+        const std::vector<int> types(B, prng);
+        prng_stream(c, { "enc_stream", "enc_stream:shake256" }, types.data(), B, d_seeds, W, words, st);
         const long long bn = static_cast<long long>(B) * n;
         const int logn = c.logn, Lpi = static_cast<int>(Lp);
         c.stats.begin("enc_ternary", 0, (4.0 + 8.0 * Lp) * bn, st);

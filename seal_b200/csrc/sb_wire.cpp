@@ -279,6 +279,8 @@ namespace sbw
             throw std::logic_error("KSwitchKeys outer dimension is invalid"); // kswitchkeys.cpp:121-125
         entry.slots = static_cast<size_t>(dim1);
         entry.offsets.clear();
+        entry.seeded.clear();
+        entry.seed_offsets.clear();
         if (index >= dim1)
             throw std::out_of_range("kswitch_keys_index");
         for (uint64_t slot = 0; slot < dim1; slot++)
@@ -294,13 +296,13 @@ namespace sbw
                 inspect(r, static_cast<size_t>(end - r), info);
                 if (slot == index)
                 {
-                    if (info.seeded)
-                        throw std::logic_error("seeded keys must be expanded by the reference (KSwitchKeys::load) first");
                     if (info.size != 2 || !info.is_ntt_form || std::memcmp(info.parms_id, entry.parms_id, sizeof(info.parms_id)) != 0 ||
                         (j > 0 && (info.coeff_modulus_size != entry.L || info.poly_modulus_degree != entry.n)))
                         throw std::logic_error("key data is invalid");
                     entry.L = static_cast<size_t>(info.coeff_modulus_size), entry.n = static_cast<size_t>(info.poly_modulus_degree);
                     entry.offsets.push_back(static_cast<size_t>(r - p) + static_cast<size_t>(info.data_offset));
+                    entry.seeded.push_back(info.seeded);
+                    entry.seed_offsets.push_back(info.seeded ? static_cast<size_t>(r - p) + static_cast<size_t>(info.seed_offset) : 0);
                 }
                 r += info.stream_bytes;
             }

@@ -3,7 +3,7 @@
 //   * Ciphertext::save with compr_mode_type::none = SEALHeader + members + DynArray (ciphertext.cpp:190-247,
 //     serialization.h:76-91, dynarray.h:662-690)
 // so that serialized ciphertexts move between a byte stream and a device slab without a seal::Ciphertext in between
-// (SURVEY 8f rank 3).  Compressed streams and seed-compressed ciphertexts stay with the reference.
+// (SURVEY 8f rank 3).  Seed-compressed members are described here and expanded on the device (sb_prng.cu).
 #pragma once
 #include "../../include/seal_b200.h"
 #include <cstddef>
@@ -36,13 +36,16 @@ namespace sbw
     void write_prefix(const sb200_ct_info &info, uint8_t *out);
     // One entry of a serialized KSwitchKeys object (RelinKeys / GaloisKeys saved with compr_mode_type::none,
     // kswitchkeys.cpp:42-86: SEALHeader, parms_id, dim1, then per slot dim2 and dim2 PublicKey = Ciphertext streams).
-    // Returns the byte offsets (from p) of the coefficient words of data()[index][j], j < digits, each 2*L*n words.
+    // Returns the byte offsets (from p) of the coefficient words of data()[index][j], j < digits, each 2*L*n words, or L*n words
+    // (c_0 only) for a seed-compressed member (KeyGenerator::create_relin_keys / create_galois_keys save their keys so).
     struct KSwitchEntry
     {
         u64 parms_id[4];
         size_t slots = 0;               // data().size()
         size_t L = 0, n = 0;            // shape of every key polynomial pair
         std::vector<size_t> offsets;    // one per decomposition digit
+        std::vector<int> seeded;        // per digit: 0, or the prng_type c_1 expands with (1 = blake2xb, 2 = shake256)
+        std::vector<size_t> seed_offsets; // per digit: byte offset (from p) of the 64-byte seed of a seeded member, 0 otherwise
     };
     void inspect_kswitch(const uint8_t *p, size_t len, size_t index, KSwitchEntry &entry);
 } // namespace sbw

@@ -77,6 +77,64 @@ def main():
     return rows
 
 
+PRNG_CONFIGS = [(c[0], c[1], c[2], c[3], 1024 if c[0][:4] == "cfg2" else 32) for c in CONFIGS if c[0][:4] in ("cfg2", "cfg5")]
+PRNG_NAMES = {1: "blake2xb", 2: "shake256"}
+
+
+def seeded_stream(full, seed, prng):
+    """the seed-compressed form of a saved size-2 ciphertext (Serializable<Ciphertext>, ciphertext.cpp:325-352): c_0 only, then
+    UniformRandomGeneratorInfo behind its own SEALHeader (prng_type, 64-byte seed)"""
+    hdr, members, count = 16, 73, int.from_bytes(full[105:113], "little")
+    c0_words = count // 2
+    inner = (16 + 8 + 8 * c0_words).to_bytes(8, "little")
+    body = full[hdr:hdr + members] + full[89:97] + inner + c0_words.to_bytes(8, "little") + full[113:113 + 8 * c0_words]
+    info = full[:8] + (16 + 1 + 64).to_bytes(8, "little") + bytes([prng]) + seed.tobytes()
+    head = full[:8] + (hdr + len(body) + len(info)).to_bytes(8, "little")
+    return head + body + info
+
+
+def prng_main():
+    """per PRNG type at cfg2 / cfg5: seeded-load and encrypt_zero_symmetric ciphertexts/s, the PRNG stream kernels' algorithmic
+    GB/s (profile entries of the stream launcher: bytes written over device ms) and the batch-1 seeded-load latency"""
+    rows = []
+    for name, scheme, n, bits, batch in PRNG_CONFIGS:
+        mods = S.coeff_modulus_create(n, bits)
+        k, L = len(mods), len(mods) - 1
+        ctx = S.Context(scheme, n, mods)
+        rng = np.random.default_rng(5)
+        sk = ctx.load_secret_key(np.stack([rng.integers(0, mods[i], n, dtype=np.uint64) for i in range(k)]))
+        out = torch.empty((batch, 2, L, n), dtype=torch.int64, device="cuda")
+        for prng in (1, 2):
+            res = {"config": name, "batch": batch, "prng": PRNG_NAMES[prng]}
+            seeds = rng.integers(0, 2 ** 63, (batch, 8), dtype=np.uint64)
+            ms = timeit(lambda: ctx.d_encrypt_zero_symmetric(sk, out, L, batch, seeds, bootstrap_prng=prng, ciphertext_prng=prng))
+            res["encrypt_zero_symmetric"] = batch / ms * 1e3
+            pub = ctx.d_encrypt_zero_symmetric(sk, out, L, batch, seeds, save_seed=True, want_public_seeds=True, bootstrap_prng=prng,
+                                               ciphertext_prng=prng)
+            full = ctx.d_save_ciphertexts(out, L, 2, batch, is_ntt_form=True)
+            streams = [seeded_stream(f, pub[b], prng) for b, f in enumerate(full)]
+            dst = torch.empty_like(out)
+            ms = timeit(lambda: ctx.d_load_ciphertexts(streams, dst, L, 2))
+            res["seeded load"] = batch / ms * 1e3
+            torch.cuda.synchronize()
+            assert torch.equal(dst, out), "seeded load must re-create the encryptions"
+            ctx.profile(True)
+            ctx.d_load_ciphertexts(streams, dst, L, 2)
+            torch.cuda.synchronize()
+            ent = [e for e in ctx.profile_read() if e[0] == ("seed_stream" if prng == 1 else "seed_stream:shake256")]
+            ctx.profile(False)
+            res["prng_stream_GBps"] = ent[0][3] / (ent[0][1] * 1e-3) / 1e9
+            res["prng_stream_ms"] = ent[0][1]
+            if name.startswith("cfg5"):
+                one = dst[:1]
+                res["seeded load batch-1 latency ms"] = timeit(lambda: ctx.d_load_ciphertexts(streams[:1], one, L, 2), reps=10)
+            rows.append(res)
+            print(json.dumps(res), flush=True)
+        del ctx, sk, out
+        torch.cuda.empty_cache()
+    return rows
+
+
 # the reference on ONE core (BASELINE.md section 2, survey container), ops/s, for scale only
 CPU_1CORE = {
     "cfg1": {"multiply": 277.8, "relinearize": 1041.7, "multiply+relinearize": 219.3, "rotate (1 step)": 1408.5, "ct NTT+INTT": 3225.8},
@@ -102,7 +160,10 @@ def table(rows):
     for r in rows:
         cpu = CPU_1CORE.get(r["config"][:4], {})
         for op, v in r.items():
-            if op in ("config", "batch"):
+            if op in ("config", "batch", "prng", "prng_stream_ms"):
+                continue
+            if "prng" in r:
+                out.append(f"| {r['config']} | {r['batch']} | {r['prng']}: {op} | {v:.3g} | | |")
                 continue
             if op.endswith("_GBps"):
                 what = "NTT algorithmic GB/s (2*n*8 B per row per transform)" if op == "ntt_GBps" else \
@@ -117,5 +178,7 @@ def table(rows):
 if __name__ == "__main__":
     if len(sys.argv) == 3 and sys.argv[1] == "--table":
         sys.stdout.write(table([json.loads(ln) for ln in open(sys.argv[2]) if ln.startswith("{")]))
+    elif len(sys.argv) == 2 and sys.argv[1] == "--prng":
+        prng_main()
     else:
         main()
