@@ -376,6 +376,17 @@ int sb200_decrypt(sb200_context *ctx, sb200_secret_key *key, size_t L, size_t si
                   const uint64_t *h_correction_factors, uint64_t *d_plain, void *stream);
 int sb200_decrypt_host(sb200_context *ctx, sb200_secret_key *key, size_t L, size_t size, size_t batch, const uint64_t *h_ct,
                        const uint64_t *h_correction_factors, uint64_t *h_plain);
+/* Decryptor::invariant_noise_budget (decryptor.cpp:409-486) for a batch: d_ct [batch][size][L][n], BFV in coefficient form, BGV in
+ * NTT form -> d_budgets [batch] ints, max(0, bits(Q) - bits(||t c(s) mod Q||) - 1) for BFV, the same without the factor t for BGV,
+ * each equal to the reference's.  The phase is composed modulo Q exactly on the device and reduced to one int per ciphertext
+ * there; nothing but the budgets leaves the GPU, and the stream entry point does not synchronise with the host.  Sizes 2..16
+ * and levels of at most 60 primes, as sb200_decrypt (levels of 61-64 primes are rejected with SB200_E_INVALID_ARG for now, like
+ * decryption); a CKKS context gives SB200_E_LOGIC ("unsupported scheme", the reference has no noise budget for CKKS).  The
+ * scratch arena (and, for the host entry point, the output staging) is wiped afterwards, as after a decryption. */
+int sb200_invariant_noise_budget(sb200_context *ctx, sb200_secret_key *key, size_t L, size_t size, size_t batch, const uint64_t *d_ct,
+                                 int *d_budgets, void *stream);
+int sb200_invariant_noise_budget_host(sb200_context *ctx, sb200_secret_key *key, size_t L, size_t size, size_t batch, const uint64_t *h_ct,
+                                      int *h_budgets);
 
 /* ---- multi-device dispatch (SURVEY 8e): one context per CUDA device of the box, one host thread per device -----------
  * A batch of independent ciphertexts is cut into contiguous slices, slice i goes to device i through that device's own

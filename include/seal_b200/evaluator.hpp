@@ -27,6 +27,7 @@
 namespace seal_b200
 {
     class Evaluator;
+    class Decryptor;
 
     // ---- device-resident ciphertexts ---------------------------------------------------------------------------------
     // A batch of B ciphertexts of one shape that stays on the GPU between Evaluator calls.  It carries exactly the metadata
@@ -76,6 +77,7 @@ namespace seal_b200
 
     private:
         friend class Evaluator;
+        friend class Decryptor;
         sb200_context *ctx_ = nullptr;
         std::uint64_t *d_ = nullptr;
         std::size_t cap_ = 0; // words

@@ -33,7 +33,7 @@ SYMBOLS = [
     "sb200_relinearize_host", "sb200_multiply_relinearize_host", "sb200_rescale_to_next_host",
     "sb200_mod_switch_to_next_host", "sb200_apply_galois_host", "sb200_get_parms_id", "sb200_ciphertext_inspect",
     "sb200_ciphertext_save_size", "sb200_ciphertext_load", "sb200_ciphertext_save", "sb200_secret_key_create",
-    "sb200_secret_key_destroy", "sb200_decrypt", "sb200_decrypt_host", "sb200_encrypt_zero_symmetric", "sb200_public_key_create", "sb200_public_key_destroy", "sb200_encrypt_zero_asymmetric", "sb200_encrypt_zero_symmetric_prng", "sb200_encrypt_zero_asymmetric_prng", "sb200_ckks_encode", "sb200_ckks_decode", "sb200_ckks_encode_host", "sb200_ckks_decode_host",
+    "sb200_secret_key_destroy", "sb200_decrypt", "sb200_decrypt_host", "sb200_invariant_noise_budget", "sb200_invariant_noise_budget_host", "sb200_encrypt_zero_symmetric", "sb200_public_key_create", "sb200_public_key_destroy", "sb200_encrypt_zero_asymmetric", "sb200_encrypt_zero_symmetric_prng", "sb200_encrypt_zero_asymmetric_prng", "sb200_ckks_encode", "sb200_ckks_decode", "sb200_ckks_encode_host", "sb200_ckks_decode_host",
     "sb200_group_create", "sb200_group_destroy", "sb200_group_size", "sb200_group_context", "sb200_group_slice",
     "sb200_group_kswitch_key_create", "sb200_group_kswitch_key_destroy", "sb200_group_multiply_relinearize_host",
     "sb200_group_relinearize_host", "sb200_group_apply_galois_host", "sb200_group_multiply_host", "sb200_group_rescale_to_next_host",
@@ -153,6 +153,8 @@ def lib():
         L.sb200_encrypt_zero_asymmetric_prng.argtypes = [vp, vp, sz, sz, i32, _u64p, vp, vp]
         L.sb200_encrypt_zero_symmetric_prng.argtypes = [vp, vp, sz, sz, i32, i32, _u64p, i32, vp, _u64p, vp]
         L.sb200_decrypt_host.argtypes = [vp, vp, sz, sz, sz, _u64p, _u64p, _u64p]
+        L.sb200_invariant_noise_budget.argtypes = [vp, vp, sz, sz, sz, vp, vp, vp]
+        L.sb200_invariant_noise_budget_host.argtypes = [vp, vp, sz, sz, sz, _u64p, C.POINTER(i32)]
         _lib = L
     return _lib
 
@@ -501,6 +503,12 @@ class Context:
     def d_ckks_decode(self, plain, values, L, batch, scale):
         _check(lib().sb200_ckks_decode(self.h, L, batch, _dp(plain), float(scale), _dp(values), self._stream()))
 
+    def d_invariant_noise_budget(self, ct, sk, budgets, L, size, batch):
+        """invariant_noise_budget of the device slab ct [batch][size][L][n] into the int32 CUDA tensor budgets [batch], on the
+        current stream"""
+        assert budgets.is_cuda and budgets.is_contiguous() and budgets.element_size() == 4
+        _check(lib().sb200_invariant_noise_budget(self.h, sk.h, L, size, batch, _dp(ct), C.c_void_p(budgets.data_ptr()), self._stream()))
+
     def load_secret_key(self, host_key):
         return SecretKey(self, host_key)
 
@@ -512,6 +520,15 @@ class Context:
         cf = None if correction_factors is None else _hp(np.ascontiguousarray(correction_factors, dtype=np.uint64).reshape(B))
         _check(lib().sb200_decrypt_host(self.h, sk.h, L, size, B, _hp(a), cf, _hp(out)))
         return out[0] if single else out
+
+    def invariant_noise_budget(self, a, sk):
+        """Decryptor.invariant_noise_budget of BFV (coefficient form) / BGV (NTT form) ciphertexts [B][size][L][n] (or one
+        [size][L][n], B = 1) -> int32 [B]"""
+        a, _ = self._batched(a)
+        B, size, L, n = a.shape
+        out = np.zeros(B, dtype=np.int32)
+        _check(lib().sb200_invariant_noise_budget_host(self.h, sk.h, L, size, B, _hp(a), out.ctypes.data_as(C.POINTER(C.c_int))))
+        return out
 
     def plain_to_ntt(self, plain, L):
         """Evaluator.transform_to_ntt(Plaintext, parms_id of the level with L primes): [B][n] words < t -> [B][L][n]"""

@@ -785,6 +785,7 @@ namespace
         size_t a, b, out;              // words per ciphertext of input a, input b (0 = none) and the output
         bool in_place = false;         // the output overwrites input a (out = a)
         const char *alias = nullptr;   // device slabs: the error when the output aliases an input (nullptr = allowed)
+        size_t out_unit = sizeof(u64); // bytes of one output word (the noise budget returns one int per ciphertext)
     };
 
     struct HostPipe
@@ -828,7 +829,8 @@ namespace
         {
             StreamOrder order(c, s_comp); // the operation's kernels (and the scratch arenas they use) run on s_comp
             const size_t wa = w.a, wb = w.b, wo = w.in_place ? 0 : w.out;
-            const size_t per_ct = (wa + wb + wo) * sizeof(u64);
+            const size_t out_bytes = w.out * w.out_unit; // per ciphertext
+            const size_t per_ct = (wa + wb) * sizeof(u64) + (w.in_place ? 0 : out_bytes);
             size_t chunk = std::max<size_t>(1, std::min<size_t>(batch, c.host_stage_bytes / std::max<size_t>(per_ct, 1)));
             if (chunk >= batch && batch >= 4)
                 chunk = (batch + 1) / 2; // at least two chunks so the copies overlap the kernels
@@ -839,14 +841,14 @@ namespace
                 if (wb)
                     buffer(slot, 1, chunk * wb);
                 if (!w.in_place)
-                    buffer(slot, 2, chunk * wo);
+                    buffer(slot, 2, (chunk * wo * w.out_unit + sizeof(u64) - 1) / sizeof(u64));
             }
             size_t i = 0;
             for (size_t b0 = 0; b0 < batch; b0 += chunk, i++)
             {
                 const size_t B = std::min(chunk, batch - b0);
                 const int slot = static_cast<int>(i & 1);
-                u64 *da = buffer(slot, 0, B * wa), *db = wb ? buffer(slot, 1, B * wb) : nullptr, *dout = w.in_place ? da : buffer(slot, 2, B * wo);
+                u64 *da = buffer(slot, 0, B * wa), *db = wb ? buffer(slot, 1, B * wb) : nullptr, *dout = w.in_place ? da : buffer(slot, 2, (B * wo * w.out_unit + sizeof(u64) - 1) / sizeof(u64));
                 if (i >= 2)
                 {
                     // inputs of this slot are free once its previous kernels finished (and, in place, once copied out)
@@ -862,7 +864,7 @@ namespace
                 op(c, b0, B, da, db, dout, s_comp);
                 cuda_check(cudaEventRecord(ev_comp[slot], s_comp), "record");
                 cuda_check(cudaStreamWaitEvent(s_out, ev_comp[slot], 0), "wait");
-                cuda_check(cudaMemcpyAsync(ho + b0 * w.out, dout, B * w.out * sizeof(u64), cudaMemcpyDeviceToHost, s_out), "D2H");
+                cuda_check(cudaMemcpyAsync(reinterpret_cast<uint8_t *>(ho) + b0 * out_bytes, dout, B * out_bytes, cudaMemcpyDeviceToHost, s_out), "D2H");
                 cuda_check(cudaEventRecord(ev_out[slot], s_out), "record");
             }
             cuda_check(cudaStreamSynchronize(s_out), "synchronize");
@@ -1117,6 +1119,23 @@ namespace
         void operator()(Context &c, size_t b0, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
         {
             op_decrypt(c, key, L, size, B, a, cf ? cf + b0 : nullptr, out, st);
+        }
+    };
+
+    // budgets: one int per ciphertext (Layout::out_unit); ciphertexts in the scheme's own form (BFV coefficient, BGV NTT)
+    struct NoiseBudget
+    {
+        SecretKey &key;
+        size_t L, size;
+        void check(const Context &c, size_t batch) const
+        {
+            check_level(c, L, batch);
+            check_noise_budget(c, key, L, size);
+        }
+        Layout layout(const Context &c) const { return { size * L * c.n, 0, 1, false, nullptr, sizeof(int) }; }
+        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
+        {
+            op_invariant_noise_budget(c, key, L, size, B, a, reinterpret_cast<int *>(out), st);
         }
     };
 
@@ -1664,27 +1683,51 @@ int sb200_encrypt_zero_symmetric_prng(sb200_context *ctx, sb200_secret_key *key,
     SB_CATCH
 }
 
+} // extern "C"
+
 // the decryption phases and plaintexts do not stay behind in the arenas (the reference decrypts inside a clear-on-destruction pool,
 // decryptor.cpp:106-109)
+namespace
+{
+    void wipe_stream(Context &c, cudaStream_t st) { c.wipe_scratch(st); }
+    void wipe_host(Context &c, cudaStream_t st)
+    {
+        c.wipe_scratch(st);
+        for (int slot = 0; slot < 2; slot++) // and the output staging
+            if (c.io.buf[slot][2])
+                cuda_check(cudaMemsetAsync(c.io.buf[slot][2], 0, c.io.cap[slot][2] * sizeof(u64), st), "wipe staging");
+        cuda_check(cudaStreamSynchronize(st), "synchronize");
+    }
+} // namespace
+
+extern "C" {
 int sb200_decrypt(sb200_context *ctx, sb200_secret_key *key, size_t L, size_t size, size_t batch, const uint64_t *ct,
                   const uint64_t *h_correction_factors, uint64_t *plain, void *stream)
 {
     SB_NEED(key);
-    return on_stream(ctx, stream, batch, ct, nullptr, plain, Decrypt{ key->k, L, size, (const u64 *)h_correction_factors },
-                     [](Context &c, cudaStream_t st) { c.wipe_scratch(st); });
+    return on_stream(ctx, stream, batch, ct, nullptr, plain, Decrypt{ key->k, L, size, (const u64 *)h_correction_factors }, wipe_stream);
 }
 
 int sb200_decrypt_host(sb200_context *ctx, sb200_secret_key *key, size_t L, size_t size, size_t batch, const uint64_t *ct,
                        const uint64_t *h_correction_factors, uint64_t *plain)
 {
     SB_NEED(key);
-    return on_host(ctx, batch, ct, nullptr, plain, Decrypt{ key->k, L, size, (const u64 *)h_correction_factors }, [](Context &c, cudaStream_t st) {
-        c.wipe_scratch(st);
-        for (int slot = 0; slot < 2; slot++) // and the output staging
-            if (c.io.buf[slot][2])
-                cuda_check(cudaMemsetAsync(c.io.buf[slot][2], 0, c.io.cap[slot][2] * sizeof(u64), st), "wipe staging");
-        cuda_check(cudaStreamSynchronize(st), "synchronize");
-    });
+    return on_host(ctx, batch, ct, nullptr, plain, Decrypt{ key->k, L, size, (const u64 *)h_correction_factors }, wipe_host);
+}
+
+// Decryptor::invariant_noise_budget: the phases depend on the secret key, so the arenas are wiped as after a decryption
+int sb200_invariant_noise_budget(sb200_context *ctx, sb200_secret_key *key, size_t L, size_t size, size_t batch, const uint64_t *d_ct,
+                                 int *d_budgets, void *stream)
+{
+    SB_NEED(key);
+    return on_stream(ctx, stream, batch, d_ct, nullptr, d_budgets, NoiseBudget{ key->k, L, size }, wipe_stream);
+}
+
+int sb200_invariant_noise_budget_host(sb200_context *ctx, sb200_secret_key *key, size_t L, size_t size, size_t batch, const uint64_t *h_ct,
+                                      int *h_budgets)
+{
+    SB_NEED(key);
+    return on_host(ctx, batch, h_ct, nullptr, h_budgets, NoiseBudget{ key->k, L, size }, wipe_host);
 }
 
 } // extern "C"

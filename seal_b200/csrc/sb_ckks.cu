@@ -186,9 +186,8 @@ namespace sb
         }
 
         // ---- decode ----
-        // RNSBase::compose (rns.cpp:321-352) of one coefficient + the conversion to double (ckks.h:740-778).
+        // RNSBase::compose (rns.cpp:321-352) of one coefficient (crt_compose, sb_device.cuh) + the conversion to double (ckks.h:740-778).
         // big = [Q (L) | threshold (L) | punctured (L * L)] words; one thread per coefficient, the L-word integers in local memory
-        constexpr int kMaxWords = 64; // SEAL_COEFF_MOD_COUNT_MAX (util/defines.h)
         __global__ void __launch_bounds__(128) ckks_compose_kernel(const u64 *__restrict__ coef, const u64 *__restrict__ big, const Tw *__restrict__ invp,
                                                                    const PrimeDev *__restrict__ primes, double2 *__restrict__ V, int logn, int L,
                                                                    double inv_scale, long long total)
@@ -198,52 +197,9 @@ namespace sb
                 return;
             const long long n = 1ll << logn, b = e >> logn, i = e & (n - 1);
             const u64 *Q = big, *thr = big + L, *punct = big + 2 * L;
-            u64 val[kMaxWords];
-            for (int w = 0; w < L; w++)
-                val[w] = 0;
+            u64 val[kCrtMaxWords];
             const u64 *src = coef + b * L * n + i;
-            if (L == 1)
-                val[0] = src[0];
-            else
-                for (int j = 0; j < L; j++)
-                {
-                    const u64 t = mul_shoup(src[static_cast<long long>(j) * n], invp[j], primes[j].q);
-                    // val += punct_j * t  (punct_j * t < Q), then one conditional subtraction of Q
-                    u64 carry = 0, cy = 0;
-                    for (int w = 0; w < L; w++)
-                    {
-                        const u64 p = punct[j * L + w];
-                        const u64 lo = p * t, hi = __umul64hi(p, t);
-                        u64 term = lo + carry;
-                        carry = hi + (term < lo);
-                        u64 sum = val[w] + term;
-                        const u64 c1 = sum < term;
-                        sum += cy;
-                        cy = c1 | (sum < cy);
-                        val[w] = sum;
-                    }
-                    bool ge = cy != 0;
-                    if (!ge)
-                    {
-                        ge = true;
-                        for (int w = L - 1; w >= 0; w--)
-                            if (val[w] != Q[w])
-                            {
-                                ge = val[w] > Q[w];
-                                break;
-                            }
-                    }
-                    if (ge)
-                    {
-                        u64 bw = 0;
-                        for (int w = 0; w < L; w++)
-                        {
-                            const u64 a = val[w], s1 = a - Q[w], s2 = s1 - bw;
-                            bw = (a < Q[w]) | (s1 < bw);
-                            val[w] = s2;
-                        }
-                    }
-                }
+            crt_compose([&](int j) { return src[static_cast<long long>(j) * n]; }, Q, punct, invp, primes, L, val);
             bool upper = true; // is_greater_than_or_equal_uint(value, upper_half_threshold)
             for (int w = L - 1; w >= 0; w--)
                 if (val[w] != thr[w])
@@ -355,33 +311,6 @@ namespace sb
         return enc;
     }
 
-    static Context::CkksLevel &ckks_level(Context &c, size_t L)
-    {
-        auto it = c.ckks_levels.find(L);
-        if (it != c.ckks_levels.end())
-            return it->second;
-        const sbh::CkksLevelHost h = sbh::ckks_level(c.q.data(), L);
-        Context::CkksLevel lv;
-        lv.total_bits = h.total_bits;
-        std::vector<u64> big;
-        big.insert(big.end(), h.Q.begin(), h.Q.end());
-        big.insert(big.end(), h.threshold.begin(), h.threshold.end());
-        big.insert(big.end(), h.punctured.begin(), h.punctured.end());
-        std::vector<Tw> invp(L);
-        for (size_t j = 0; j < L; j++)
-            invp[j] = Tw{ h.inv_punctured[j].w, h.inv_punctured[j].wq };
-        cuda_check(cudaMalloc(&lv.d_big, big.size() * sizeof(u64)), "cudaMalloc(ckks level)");
-        cuda_check(cudaMalloc(&lv.d_invp, L * sizeof(Tw)), "cudaMalloc(ckks level)");
-        cuda_check(cudaMemcpy(lv.d_big, big.data(), big.size() * sizeof(u64), cudaMemcpyHostToDevice), "upload ckks level");
-        cuda_check(cudaMemcpy(lv.d_invp, invp.data(), L * sizeof(Tw), cudaMemcpyHostToDevice), "upload ckks level");
-        return c.ckks_levels.emplace(L, lv).first->second;
-    }
-
-    int ckks_total_bits(Context &c, size_t L)
-    {
-        return ckks_level(c, L).total_bits;
-    }
-
     // values: device, [B][count] complex (re, im) pairs or reals; plain: device, [B][L][n] NTT form.  Synchronises the stream once
     // (the reference's "encoded values are too large" check needs the largest coefficient before the plaintext is produced).
     void op_ckks_encode(Context &c, size_t L, size_t B, const double *values, size_t count, bool is_complex, double scale, u64 *plain,
@@ -394,7 +323,7 @@ namespace sb
             throw std::invalid_argument("values_size is too large");
         if (count && !values)
             throw std::invalid_argument("values cannot be null");
-        const int total_bits = ckks_level(c, L).total_bits;
+        const int total_bits = crt_level(c, L).total_bits;
         // ckks.h:494-499
         if (!std::isnormal(scale) || scale <= 0 || (static_cast<int>(std::log2(scale)) + 1 >= total_bits))
             throw std::invalid_argument("scale out of bounds");
@@ -466,9 +395,9 @@ namespace sb
     void op_ckks_decode(Context &c, size_t L, size_t B, const u64 *plain, double scale, double *values, cudaStream_t st)
     {
         auto &enc = ckks_encoder(c);
-        if (L < 1 || L > c.k || L > static_cast<size_t>(kMaxWords))
+        if (L < 1 || L > c.k || L > static_cast<size_t>(kCrtMaxWords))
             throw std::invalid_argument("plain is not valid for encryption parameters");
-        auto &lv = ckks_level(c, L);
+        auto &lv = crt_level(c, L);
         // ckks.h:712-716
         if (!std::isnormal(scale) || scale <= 0 || (static_cast<int>(std::log2(scale)) >= lv.total_bits))
             throw std::invalid_argument("scale out of bounds");

@@ -181,6 +181,61 @@ __device__ __forceinline__ void mac128(u64 &lo, u64 &hi, u64 a, u64 b)
     asm("mad.lo.cc.u64 %0, %2, %3, %0;\n\tmadc.hi.u64 %1, %2, %3, %1;" : "+l"(lo), "+l"(hi) : "l"(a), "l"(b));
 }
 
+// RNSBase::compose (rns.cpp:321-352) of one coefficient into val = L little-endian words in [0, Q): val = sum_j punct_j * (x_j *
+// (Q/q_j)^-1 mod q_j) with one conditional subtraction of Q per prime, x_j = residue(j) modulo prime j (the caller loads it).
+// Q = [L] words, punct = [L][L] words of Q / q_j, invp = (Q/q_j)^-1 mod q_j (sb_engine.cuh: Context::CrtLevel).  Used by CKKS
+// decode (sb_ckks.cu) and the invariant noise budget (sb_engine.cu); the integers live in local memory, one thread per coefficient.
+constexpr int kCrtMaxWords = 64; // SEAL_COEFF_MOD_COUNT_MAX (util/defines.h)
+template <class Residue>
+__device__ __forceinline__ void crt_compose(const Residue &residue, const u64 *__restrict__ Q, const u64 *__restrict__ punct,
+                                            const Tw *__restrict__ invp, const PrimeDev *__restrict__ primes, int L, u64 (&val)[kCrtMaxWords])
+{
+    for (int w = 0; w < L; w++)
+        val[w] = 0;
+    if (L == 1)
+        val[0] = residue(0);
+    else
+        for (int j = 0; j < L; j++)
+        {
+            const u64 t = mul_shoup(residue(j), invp[j], primes[j].q);
+            // val += punct_j * t  (punct_j * t < Q), then one conditional subtraction of Q
+            u64 carry = 0, cy = 0;
+            for (int w = 0; w < L; w++)
+            {
+                const u64 p = punct[j * L + w];
+                const u64 lo = p * t, hi = __umul64hi(p, t);
+                u64 term = lo + carry;
+                carry = hi + (term < lo);
+                u64 sum = val[w] + term;
+                const u64 c1 = sum < term;
+                sum += cy;
+                cy = c1 | (sum < cy);
+                val[w] = sum;
+            }
+            bool ge = cy != 0;
+            if (!ge)
+            {
+                ge = true;
+                for (int w = L - 1; w >= 0; w--)
+                    if (val[w] != Q[w])
+                    {
+                        ge = val[w] > Q[w];
+                        break;
+                    }
+            }
+            if (ge)
+            {
+                u64 bw = 0;
+                for (int w = 0; w < L; w++)
+                {
+                    const u64 a = val[w], s1 = a - Q[w], s2 = s1 - bw;
+                    bw = (a < Q[w]) | (s1 < bw);
+                    val[w] = s2;
+                }
+            }
+        }
+}
+
 // (hi:lo) += a*b for bounded operands (a < 2^63.25, b < 2^62: lazily grown transform outputs times canonical key words): four
 // wide multiplies -- p0 = a0*b0, mid = a0*b1 + a1*b0 (fits 64 bits under the bounds), p3 = a1*b1 -- and two carry chains over the
 // four 32-bit words of the sum.  ptxas expands the generic mac128 into 5-7 wide multiplies and ~10 adds per product.

@@ -48,7 +48,7 @@ namespace sb
         cudaFree(ckks.d_inv_roots);
         cudaFree(ckks.d_map);
         cudaFree(ckks.d_stat);
-        for (auto &kv : ckks_levels)
+        for (auto &kv : crt_levels)
         {
             cudaFree(kv.second.d_big);
             cudaFree(kv.second.d_invp);
@@ -1098,7 +1098,106 @@ namespace sb
         plain[e] = r;
     }
 
+    // Decryptor::invariant_noise_budget (decryptor.cpp:409-486), per coefficient: the coefficient-form phase (BFV: T + c_0 times t mod
+    // q_i, multiply_poly_scalar_coeffmod; BGV: T), composed modulo Q (compose_array), centred against (Q + 1) / 2 (Q - v above it,
+    // poly_infty_norm_coeffmod at :22-51) and its significant bit count.  The bit count of the maximum is the maximum of the bit counts,
+    // so the norm reduces to one int per ciphertext: warp max, CTA max, one atomicMax per CTA into bits[b] (zeroed by the caller).
+    // grid = (B, ceil(n / 128)): a CTA never spans two ciphertexts.  big / invp: Context::CrtLevel of the level.
+    template <bool BFV>
+    __global__ void __launch_bounds__(128) noise_norm_kernel(const u64 *__restrict__ T, const u64 *__restrict__ c0, long long c0_bs,
+                                                             const u64 *__restrict__ t_mod_q, const u64 *__restrict__ big, const Tw *__restrict__ invp,
+                                                             const PrimeDev *__restrict__ primes, int logn, int L, int *__restrict__ bits)
+    {
+        const long long b = blockIdx.x;
+        const int i = static_cast<int>(blockIdx.y * blockDim.x + threadIdx.x);
+        int nb = 0;
+        if (i < (1 << logn))
+        {
+            const u64 *Q = big, *thr = big + L, *punct = big + 2 * L;
+            const u64 *src = T + ((b * L) << logn) + i;
+            const u64 *s0 = c0 + b * c0_bs + i;
+            u64 val[kCrtMaxWords];
+            crt_compose(
+                [&](int j) {
+                    const long long off = static_cast<long long>(j) << logn;
+                    u64 x = src[off];
+                    if (BFV)
+                    {
+                        const PrimeDev &P = primes[j];
+                        x = mulmod_barrett(csub(x + s0[off], P.q), t_mod_q[j], P);
+                    }
+                    return x;
+                },
+                Q, punct, invp, primes, L, val);
+            bool upper = true; // is_greater_than_or_equal_uint(value, (Q + 1) / 2)
+            for (int w = L - 1; w >= 0; w--)
+                if (val[w] != thr[w])
+                {
+                    upper = val[w] > thr[w];
+                    break;
+                }
+            if (upper) // Q - value
+            {
+                u64 bw = 0;
+                for (int w = 0; w < L; w++)
+                {
+                    const u64 a = Q[w], s1 = a - val[w], s2 = s1 - bw;
+                    bw = (a < val[w]) | (s1 < bw);
+                    val[w] = s2;
+                }
+            }
+            for (int w = L - 1; w >= 0; w--) // get_significant_bit_count_uint
+                if (val[w])
+                {
+                    nb = 64 * w + 64 - __clzll(static_cast<long long>(val[w]));
+                    break;
+                }
+        }
+        nb = __reduce_max_sync(0xffffffffu, static_cast<unsigned>(nb));
+        __shared__ int warp_max[4];
+        if ((threadIdx.x & 31) == 0)
+            warp_max[threadIdx.x >> 5] = nb;
+        __syncthreads();
+        if (threadIdx.x == 0)
+        {
+            const int m = max(max(warp_max[0], warp_max[1]), max(warp_max[2], warp_max[3]));
+            if (m)
+                atomicMax(bits + b, m);
+        }
+    }
+
+    // bits of the largest centred noise coefficient -> max(0, total_bits - bits - 1), in place
+    __global__ void __launch_bounds__(256) noise_budget_kernel(int *__restrict__ budgets, int total_bits, long long B)
+    {
+        const long long e = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+        if (e >= B)
+            return;
+        budgets[e] = max(0, total_bits - budgets[e] - 1);
+    }
+
     static u64 mulmod_host(u64 a, u64 b, u64 m) { return static_cast<u64>(static_cast<unsigned __int128>(a) * b % m); }
+
+    Context::CrtLevel &crt_level(Context &c, size_t L)
+    {
+        auto it = c.crt_levels.find(L);
+        if (it != c.crt_levels.end())
+            return it->second;
+        const sbh::CkksLevelHost h = sbh::ckks_level(c.q.data(), L);
+        Context::CrtLevel lv;
+        lv.total_bits = h.total_bits;
+        std::vector<u64> big;
+        big.insert(big.end(), h.Q.begin(), h.Q.end());
+        big.insert(big.end(), h.threshold.begin(), h.threshold.end());
+        big.insert(big.end(), h.punctured.begin(), h.punctured.end());
+        std::vector<Tw> invp(L);
+        for (size_t j = 0; j < L; j++)
+            invp[j] = Tw{ h.inv_punctured[j].w, h.inv_punctured[j].wq };
+        cuda_check(cudaMalloc(&lv.d_big, big.size() * sizeof(u64)), "cudaMalloc(crt level)");
+        cuda_check(cudaMalloc(&lv.d_invp, L * sizeof(Tw)), "cudaMalloc(crt level)");
+        cuda_check(cudaMemcpy(lv.d_big, big.data(), big.size() * sizeof(u64), cudaMemcpyHostToDevice), "upload crt level");
+        cuda_check(cudaMemcpy(lv.d_invp, invp.data(), L * sizeof(Tw), cudaMemcpyHostToDevice), "upload crt level");
+        return c.crt_levels.emplace(L, lv).first->second;
+    }
     static const Context::DecryptLevel &decrypt_level(Context &c, size_t L)
     {
         plain_level(c, L); // t Barrett ratio, scheme check
@@ -1144,6 +1243,57 @@ namespace sb
         return c.decrypt_levels.emplace(L, dl).first->second;
     }
 
+    // The coefficient-form phase of ciphertexts ct [batch][size][L][n] (BFV / BGV), in chunks of the batch that fit the scratch arena:
+    // per chunk of B ciphertexts from b0, T [B][L][n] = BFV: INTT(sum_{p>=1} NTT(c_p) s^p) (decryptor.cpp:348-379; c_0 is left to the
+    // consumer, which adds it in its own pass), BGV: INTT(c_0 + sum_{p>=1} c_p s^p) (:159-197, :409-486).  Then
+    // consume(b0, B, T, in, extra): in = the chunk's ciphertexts, extra = B words of scratch the consumer may use.  The key powers
+    // s^1 .. s^(size-1) must be in place (ensure_key_powers).
+    template <class Consume>
+    static void decrypt_phases(Context &c, const SecretKey &sk, size_t L, size_t size, size_t batch, const u64 *ct, cudaStream_t st,
+                               const Consume &consume)
+    {
+        const bool bfv = c.scheme == 1;
+        const int n = static_cast<int>(c.n), npow = static_cast<int>(size - 1);
+        const long long poly = static_cast<long long>(L) * n, ct_bs = static_cast<long long>(size) * poly, sk_ps = static_cast<long long>(c.k) * n;
+        // scratch per ciphertext: T [L][n] (+ the transformed copy of c_1.. for BFV) (+ 1 word for the consumer)
+        const size_t per = (L * c.n * (bfv ? size : 1) + 1) * sizeof(u64);
+        size_t chunk = std::min(batch, std::max<size_t>(1, c.scratch_budget / per));
+        chunk = std::min<size_t>(chunk, std::max<size_t>(1, (size_t(1) << 30) / (size * L * c.n)));
+        for (size_t b0 = 0; b0 < batch; b0 += chunk)
+        {
+            const size_t B = std::min(chunk, batch - b0);
+            u64 *T = static_cast<u64 *>(c.ensure_scratch(per * B));
+            u64 *extra = T + B * L * c.n;
+            const u64 *in = ct + b0 * ct_bs;
+            const long long total = static_cast<long long>(B) * poly;
+            if (bfv)
+            {
+                // coefficient-form ciphertext: transform c_1.., accumulate, transform back
+                u64 *X = extra; // [B][size-1][L][n]
+                cuda_check(cudaMemcpy2DAsync(X, (size - 1) * poly * sizeof(u64), in + poly, ct_bs * sizeof(u64), (size - 1) * poly * sizeof(u64), B,
+                                             cudaMemcpyDeviceToDevice, st),
+                           "copy");
+                op_ntt(c, false, L, size - 1, B, X, st);
+                c.stats.begin("decrypt_phase", 0, 8.0 * total * size, st);
+                phase_kernel<false><<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(X, static_cast<long long>(size - 1) * poly, nullptr, 0,
+                                                                                                sk.d_pow, sk_ps, T, c.d_primes, c.logn,
+                                                                                                static_cast<int>(L), npow, total);
+                c.stats.end(st);
+                cuda_check(cudaGetLastError(), "phase_kernel");
+            }
+            else
+            {
+                c.stats.begin("decrypt_phase", 0, 8.0 * total * (size + 1), st);
+                phase_kernel<true><<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(in + poly, ct_bs, in, ct_bs, sk.d_pow, sk_ps, T,
+                                                                                               c.d_primes, c.logn, static_cast<int>(L), npow, total);
+                c.stats.end(st);
+                cuda_check(cudaGetLastError(), "phase_kernel");
+            }
+            op_ntt(c, true, L, 1, B, T, st);
+            consume(b0, B, T, in, extra);
+        }
+    }
+
     void op_decrypt(Context &c, SecretKey &sk, size_t L, size_t size, size_t batch, const u64 *ct, const u64 *h_cf, u64 *plain, cudaStream_t st)
     {
         if (sk.ctx != &c)
@@ -1172,51 +1322,28 @@ namespace sb
             return;
         }
         const Context::DecryptLevel &dl = decrypt_level(c, L);
-        const bool bfv = c.scheme == 1;
-        // scratch per ciphertext: T [L][n] (+ the transformed copy of c_1.. for BFV) (+ 1 word for the BGV factor)
-        const size_t per = (L * c.n * (bfv ? size : 1) + 1) * sizeof(u64);
-        size_t chunk = std::min(batch, std::max<size_t>(1, c.scratch_budget / per));
-        chunk = std::min<size_t>(chunk, std::max<size_t>(1, (size_t(1) << 30) / (size * L * c.n)));
-        u64 gamma = 1, g_rlo = 0, g_rhi = 0, inv_gamma_t = 0;
-        if (bfv)
+        if (c.scheme == 1)
         {
-            gamma = c.aux[1];
+            const u64 gamma = c.aux[1];
             const unsigned __int128 ratio = ~static_cast<unsigned __int128>(0) / gamma;
-            g_rlo = static_cast<u64>(ratio), g_rhi = static_cast<u64>(ratio >> 64);
+            const u64 g_rlo = static_cast<u64>(ratio), g_rhi = static_cast<u64>(ratio >> 64);
+            u64 inv_gamma_t = 0;
             if (!sbh::invmod(gamma % c.t, c.t, inv_gamma_t))
                 throw std::logic_error("invalid rns bases");
-        }
-        for (size_t b0 = 0; b0 < batch; b0 += chunk)
-        {
-            const size_t B = std::min(chunk, batch - b0);
-            u64 *T = static_cast<u64 *>(c.ensure_scratch(per * B));
-            u64 *extra = T + B * L * c.n;
-            const u64 *in = ct + b0 * ct_bs;
-            const long long total = static_cast<long long>(B) * poly, tn = static_cast<long long>(B) * n;
-            if (bfv)
-            {
-                // coefficient-form ciphertext (decryptor.cpp:348-379): transform c_1.., accumulate, transform back, add c_0
-                u64 *X = extra; // [B][size-1][L][n]
-                cuda_check(cudaMemcpy2DAsync(X, (size - 1) * poly * sizeof(u64), in + poly, ct_bs * sizeof(u64), (size - 1) * poly * sizeof(u64), B,
-                                             cudaMemcpyDeviceToDevice, st),
-                           "copy");
-                op_ntt(c, false, L, size - 1, B, X, st);
-                c.stats.begin("decrypt_phase", 0, 8.0 * total * size, st);
-                phase_kernel<false><<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(X, static_cast<long long>(size - 1) * poly, nullptr, 0,
-                                                                                                sk.d_pow, sk_ps, T, c.d_primes, c.logn,
-                                                                                                static_cast<int>(L), npow, total);
-                c.stats.end(st);
-                cuda_check(cudaGetLastError(), "phase_kernel");
-                op_ntt(c, true, L, 1, B, T, st);
+            decrypt_phases(c, sk, L, size, batch, ct, st, [&](size_t b0, size_t B, const u64 *T, const u64 *in, u64 *) {
+                const long long tn = static_cast<long long>(B) * n;
                 c.stats.begin("bfv_scale_round", 0, 8.0 * tn * (2 * L + 1), st);
                 bfv_scale_round_kernel<<<static_cast<unsigned>((tn + 127) / 128), 128, 0, st>>>(
                     T, in, ct_bs, plain + b0 * c.n, static_cast<const DecConst *>(dl.d_consts), c.d_primes, c.t, c.t_ratio_lo, c.t_ratio_hi, gamma,
                     g_rlo, g_rhi, dl.neg_inv_q_mod_t, dl.neg_inv_q_mod_g, inv_gamma_t, c.logn, static_cast<int>(L), tn);
                 c.stats.end(st);
                 cuda_check(cudaGetLastError(), "bfv_scale_round_kernel");
-                continue;
-            }
-            // bgv_decrypt (decryptor.cpp:159-197)
+            });
+            return;
+        }
+        // bgv_decrypt (decryptor.cpp:159-197)
+        decrypt_phases(c, sk, L, size, batch, ct, st, [&](size_t b0, size_t B, const u64 *T, const u64 *, u64 *extra) {
+            const long long tn = static_cast<long long>(B) * n;
             const u64 *d_fix = nullptr;
             std::vector<u64> fix;
             if (h_cf)
@@ -1232,19 +1359,55 @@ namespace sb
                 cuda_check(cudaStreamSynchronize(st), "synchronize"); // fix lives on this stack frame
                 d_fix = extra;
             }
-            c.stats.begin("decrypt_phase", 0, 8.0 * total * (size + 1), st);
-            phase_kernel<true><<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(in + poly, ct_bs, in, ct_bs, sk.d_pow, sk_ps, T, c.d_primes,
-                                                                                           c.logn, static_cast<int>(L), npow, total);
-            c.stats.end(st);
-            cuda_check(cudaGetLastError(), "phase_kernel");
-            op_ntt(c, true, L, 1, B, T, st);
             c.stats.begin("bgv_modt", 0, 8.0 * tn * (L + 1), st);
             bgv_modt_kernel<<<static_cast<unsigned>((tn + 127) / 128), 128, 0, st>>>(T, plain + b0 * c.n, static_cast<const DecConst *>(dl.d_consts),
                                                                                      c.d_primes, d_fix, c.t, c.t_ratio_lo, c.t_ratio_hi, dl.q_mod_t,
                                                                                      c.logn, static_cast<int>(L), tn);
             c.stats.end(st);
             cuda_check(cudaGetLastError(), "bgv_modt_kernel");
-        }
+        });
+    }
+
+    void check_noise_budget(const Context &c, const SecretKey &sk, size_t L, size_t size)
+    {
+        if (sk.ctx != &c)
+            throw std::invalid_argument("secret key is not valid for encryption parameters");
+        if (size < 2 || size > 16)
+            throw std::invalid_argument("encrypted is not valid for encryption parameters");
+        if (c.scheme != 1 && c.scheme != 3) // the reference has no noise budget for CKKS (decryptor.cpp:424-428)
+            throw std::logic_error("unsupported scheme");
+        if (L > 60) // the decryption limit (decrypt_level); the composition itself would take up to 64 primes
+            throw std::invalid_argument("decryption supports at most 60 primes per level");
+    }
+
+    void op_invariant_noise_budget(Context &c, SecretKey &sk, size_t L, size_t size, size_t batch, const u64 *ct, int *budgets, cudaStream_t st)
+    {
+        check_noise_budget(c, sk, L, size);
+        if (!batch)
+            return;
+        const Context::CrtLevel &lv = crt_level(c, L);
+        if (!c.d_t_mod_q)
+            plain_level(c, L); // t mod q_i (BFV multiplies the phase by t)
+        ensure_key_powers(c, sk, size - 1, st);
+        const bool bfv = c.scheme == 1;
+        const long long ct_bs = static_cast<long long>(size) * L * c.n;
+        cuda_check(cudaMemsetAsync(budgets, 0, batch * sizeof(int), st), "memset");
+        decrypt_phases(c, sk, L, size, batch, ct, st, [&](size_t b0, size_t B, const u64 *T, const u64 *in, u64 *) {
+            const dim3 grid(static_cast<unsigned>(B), static_cast<unsigned>((c.n + 127) / 128));
+            c.stats.begin("noise_norm", 0, 8.0 * B * c.n * (bfv ? 2 * L : L), st);
+            if (bfv)
+                noise_norm_kernel<true><<<grid, 128, 0, st>>>(T, in, ct_bs, c.d_t_mod_q, lv.d_big, lv.d_invp, c.d_primes, c.logn, static_cast<int>(L),
+                                                              budgets + b0);
+            else
+                noise_norm_kernel<false><<<grid, 128, 0, st>>>(T, in, ct_bs, c.d_t_mod_q, lv.d_big, lv.d_invp, c.d_primes, c.logn, static_cast<int>(L),
+                                                               budgets + b0);
+            c.stats.end(st);
+            cuda_check(cudaGetLastError(), "noise_norm_kernel");
+        });
+        c.stats.begin("noise_budget", 0, 8.0 * batch, st);
+        noise_budget_kernel<<<static_cast<unsigned>((batch + 255) / 256), 256, 0, st>>>(budgets, lv.total_bits, static_cast<long long>(batch));
+        c.stats.end(st);
+        cuda_check(cudaGetLastError(), "noise_budget_kernel");
     }
 
     // ------------------------------------------------------------------------------------- key switching ----

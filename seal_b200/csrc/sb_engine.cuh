@@ -98,7 +98,7 @@ namespace sb
             u64 q_mod_t = 0;        // ContextData::coeff_modulus_mod_plain_modulus
         };
         std::map<size_t, PlainLevel> plain_levels;
-        // CKKSEncoder on the device (sb_ckks.cu): complex root tables + slot map, built on first use; per-level big integers for decode
+        // CKKSEncoder on the device (sb_ckks.cu): complex root tables + slot map, built on first use
         struct CkksEncoder
         {
             bool ready = false;
@@ -106,13 +106,15 @@ namespace sb
             uint32_t *d_map = nullptr;                       // matrix_reps_index_map_
             void *d_stat = nullptr;                          // { max |coefficient| bits, flags }
         } ckks;
-        struct CkksLevel
+        // per-level big integers of the CRT composition (crt_compose, sb_device.cuh), built on first use (crt_level); they depend on
+        // the primes only: CKKS decode and the BFV / BGV invariant noise budget share them
+        struct CrtLevel
         {
             int total_bits = 0;
             u64 *d_big = nullptr; // [Q | (Q+1)/2 | Q/q_j ...] words
             Tw *d_invp = nullptr; // (Q/q_j)^-1 mod q_j
         };
-        std::map<size_t, CkksLevel> ckks_levels;
+        std::map<size_t, CrtLevel> crt_levels;
         u64 *d_t_mod_q = nullptr;   // [k]: t mod q_i
         u64 t_ratio_lo = 0, t_ratio_hi = 0; // floor(2^128 / t)
         std::vector<std::array<u64, 4>> parms_ids; // parms_ids[L-1] = parms_id of the level with L primes (sb_wire.hpp)
@@ -168,6 +170,14 @@ namespace sb
     // coefficient-form plaintexts [B][n].  h_cf: BGV correction factors per ciphertext (nullptr = 1).
     void secret_key_create(Context &c, const u64 *h_sk, SecretKey &out);
     void op_decrypt(Context &c, SecretKey &sk, size_t L, size_t size, size_t batch, const u64 *ct, const u64 *h_cf, u64 *plain, cudaStream_t st);
+    // Decryptor::invariant_noise_budget (decryptor.cpp:409-486) for a batch of BFV (coefficient form) / BGV (NTT form) ciphertexts
+    // [B][size][L][n] -> budgets [B] (device ints).  check_noise_budget throws what op_invariant_noise_budget would before any launch:
+    // a foreign key or a size outside 2..16 (invalid_argument), a CKKS context (logic_error), more than 60 primes (invalid_argument,
+    // the decryption limit).  Stream-ordered, no host synchronisation (beyond scratch growth).
+    void check_noise_budget(const Context &c, const SecretKey &sk, size_t L, size_t size);
+    void op_invariant_noise_budget(Context &c, SecretKey &sk, size_t L, size_t size, size_t batch, const u64 *ct, int *budgets, cudaStream_t st);
+    // the CRT composition tables of the level with L primes (Context::CrtLevel)
+    Context::CrtLevel &crt_level(Context &c, size_t L);
     // BatchEncoder::encode / decode (batchencoder.cpp:84-330): values [B][n] (< t) <-> coefficient-form plaintexts [B][n]
     void op_batch_encode(Context &c, size_t batch, const u64 *values, u64 *plain, cudaStream_t st);
     void op_batch_decode(Context &c, size_t batch, const u64 *plain, u64 *values, cudaStream_t st);

@@ -135,6 +135,54 @@ def prng_main():
     return rows
 
 
+NOISE_CONFIGS = [("BFV n=8192 BFVDefault", 8192, 1024), ("BFV n=32768 BFVDefault (15 data primes)", 32768, 128)]
+
+
+def noise_main():
+    """invariant_noise_budget of device-resident batches of fresh BFV encryptions: budgets/s, the noise_norm kernel's share of the
+    call (profile entries), and the reference's rate on one core on the same ciphertexts"""
+    import time
+
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import noise_ref as N
+    import refseal as R
+
+    print(json.dumps({"gpu": torch.cuda.get_device_name(0), "power_limit": os.popen(
+        "nvidia-smi --query-gpu=power.limit --format=csv,noheader -i 0").read().strip()}), flush=True)
+    rows = []
+    for name, n, batch in NOISE_CONFIGS:
+        mods = R.coeff_modulus_bfv_default(n)
+        t = R.plain_modulus_batching(n, 20)
+        L = len(mods) - 1
+        rc = R.RefContext(R.BFV, n, mods, t)
+        ctx = S.Context(S.BFV, n, mods, t)
+        sk = ctx.load_secret_key(rc.secret_key())
+        d = torch.empty((batch, 2, L, n), dtype=torch.int64, device="cuda")
+        ctx.d_encrypt_zero_symmetric(sk, d, L, batch)
+        out = torch.empty(batch, dtype=torch.int32, device="cuda")
+        res = {"config": name, "batch": batch}
+        ms = timeit(lambda: ctx.d_invariant_noise_budget(d, sk, out, L, 2, batch))
+        res["noise budgets/s"] = batch / ms * 1e3
+        ctx.profile(True)
+        ctx.d_invariant_noise_budget(d, sk, out, L, 2, batch)
+        torch.cuda.synchronize()
+        ent = ctx.profile_read()
+        ctx.profile(False)
+        total = sum(e[1] for e in ent)
+        res["noise_norm share of device time"] = sum(e[1] for e in ent if e[0] == "noise_norm") / total
+        host = d[:8].cpu().numpy().view(np.uint64)
+        N.ref_budget(rc, L, host[0], False)  # the reference's context and Decryptor are built on first use: not timed
+        t0 = time.perf_counter()
+        ref = [N.ref_budget(rc, L, c, False) for c in host]
+        res["reference 1-core budgets/s"] = len(host) / (time.perf_counter() - t0)
+        assert [r[1] for r in ref] == [int(x) for x in out[:8].cpu()], "device and reference budgets differ"
+        rows.append(res)
+        print(json.dumps(res), flush=True)
+        del ctx, sk, d, out
+        torch.cuda.empty_cache()
+    return rows
+
+
 # the reference on ONE core (BASELINE.md section 2, survey container), ops/s, for scale only
 CPU_1CORE = {
     "cfg1": {"multiply": 277.8, "relinearize": 1041.7, "multiply+relinearize": 219.3, "rotate (1 step)": 1408.5, "ct NTT+INTT": 3225.8},
@@ -180,5 +228,7 @@ if __name__ == "__main__":
         sys.stdout.write(table([json.loads(ln) for ln in open(sys.argv[2]) if ln.startswith("{")]))
     elif len(sys.argv) == 2 and sys.argv[1] == "--prng":
         prng_main()
+    elif len(sys.argv) == 2 and sys.argv[1] == "--noise-budget":
+        noise_main()
     else:
         main()
