@@ -170,7 +170,10 @@ int sb200_kswitch_key_load(sb200_context *ctx, const uint8_t *stream, size_t len
 /* Evaluator::transform_to_ntt_inplace / transform_from_ntt_inplace (evaluator.cpp:2289-2382) */
 int sb200_ntt_forward(sb200_context *ctx, size_t L, size_t size, size_t batch, uint64_t *d_data, void *stream);
 int sb200_ntt_inverse(sb200_context *ctx, size_t L, size_t size, size_t batch, uint64_t *d_data, void *stream);
-/* Evaluator::multiply (evaluator.cpp:352-708), size-2 x size-2 -> size-3; CKKS (NTT form) or BFV (BEHZ) per ctx */
+/* Evaluator::multiply (evaluator.cpp:352-708), size-2 x size-2 -> size-3; CKKS (NTT form) or BFV (BEHZ) per ctx.
+ * BFV multiplication (multiply, multiply_sized, square, multiply_relinearize) supports levels of at most 64 primes whose BEHZ
+ * base B holds at most 64 primes (63 primes when the plain modulus enlarges B); deeper levels are rejected with
+ * SB200_E_INVALID_ARG before any launch, as decryption rejects levels of more than 60 primes. */
 int sb200_multiply(sb200_context *ctx, size_t L, size_t batch, const uint64_t *d_a, const uint64_t *d_b,
                    uint64_t *d_out3, void *stream);
 /* the general-size branches of the same function (evaluator.cpp:524-560, :664-700, :796-833): size_a x size_b ->

@@ -887,7 +887,11 @@ namespace
     {
         size_t L;
         bool square;
-        void check(const Context &c, size_t batch) const { check_level(c, L, batch); }
+        void check(const Context &c, size_t batch) const
+        {
+            check_level(c, L, batch);
+            check_bfv_multiply_level(c, L);
+        }
         Layout layout(const Context &c) const { return { 2 * L * c.n, square ? 0 : 2 * L * c.n, 3 * L * c.n }; }
         void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *b, u64 *out, cudaStream_t st) const
         {
@@ -907,6 +911,7 @@ namespace
         {
             check_level(c, L, batch);
             check_sizes(sa, sb);
+            check_bfv_multiply_level(c, L);
         }
         Layout layout(const Context &c) const
         {
@@ -1013,7 +1018,11 @@ namespace
     {
         size_t L;
         const KSwitchKey &key;
-        void check(const Context &c, size_t batch) const { check_level(c, L, batch); }
+        void check(const Context &c, size_t batch) const
+        {
+            check_level(c, L, batch);
+            check_bfv_multiply_level(c, L);
+        }
         Layout layout(const Context &c) const { return { 2 * L * c.n, 2 * L * c.n, 2 * L * c.n }; }
         void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *b, u64 *out, cudaStream_t st) const
         {

@@ -60,6 +60,7 @@ namespace sb
             throw std::logic_error("BEHZ base exists for BFV contexts only");
         if (L < 1 || L > c.k)
             throw std::invalid_argument("encrypted is not valid for encryption parameters");
+        check_bfv_multiply_level(c, L);
         auto it = c.behz.find(L);
         if (it != c.behz.end())
             return *it->second;
@@ -299,6 +300,15 @@ namespace sb
 
     void op_ntt_rows(Context &c, bool inverse, u64 *d, size_t rows, size_t L, const int *pid_tab, cudaStream_t st);
 
+    // Every term of the three FastBConv dot products (q -> Bsk in the lift and in fast_floor, B -> q and B -> m_sk in
+    // fastbconv_sk) is below 2^122, so with at most 64 terms no 128-bit sum can wrap whatever the constants are.  The same limit
+    // keeps the shared memory of behz_floor_sk_kernel, (max(L, |Bsk|) + |Bsk|) * 128 words, below what a block may use.
+    void check_bfv_multiply_level(const Context &c, size_t L)
+    {
+        if (c.scheme == 1 && L >= 1 && L <= c.k && sbh::behz_base_size(c.q, L, c.t) > kBfvMultiplyMaxBase)
+            throw std::invalid_argument("BFV multiplication supports at most 64 primes per level (and in its auxiliary base B)");
+    }
+
     void op_bfv_multiply(Context &c, size_t L, size_t batch, const u64 *a, const u64 *b, u64 *out3, cudaStream_t st)
     {
         op_bfv_multiply(c, L, 2, 2, batch, a, b, out3, st);
@@ -308,6 +318,7 @@ namespace sb
     void op_bfv_multiply(Context &c, size_t L, size_t s1, size_t s2, size_t batch, const u64 *a, const u64 *b, u64 *out3, cudaStream_t st)
     {
         check_sizes(s1, s2);
+        check_bfv_multiply_level(c, L);
         BehzDev &d = behz_dev(c, L);
         const int n = static_cast<int>(c.n), Li = d.L, nS = d.nS, nB = d.nB;
         const size_t nin = s1 + s2, nout = s1 + s2 - 1;

@@ -223,8 +223,9 @@ namespace sb
         {
             if (t < 2 || (t >> 60))
                 throw std::invalid_argument("plain_modulus is invalid");
-            // all levels use prefixes of one auxiliary list: [m_sk, gamma, B_0, B_1, ...]  (rns.cpp:626-632)
-            size_t max_nb = (k > 1 ? k - 1 : 1) + 1;
+            // all levels use prefixes of one auxiliary list: [m_sk, gamma, B_0, B_1, ...]  (rns.cpp:626-632); the key level (L = k)
+            // may need k + 1 primes of B, and BFV multiplication takes at most kBfvMultiplyMaxBase
+            size_t max_nb = std::min(k + 1, kBfvMultiplyMaxBase);
             c->aux = sbh::get_primes(2 * static_cast<u64>(n), 61, max_nb + 2);
         }
         if (scheme == 3)

@@ -192,6 +192,11 @@ namespace sb
     void op_ckks_multiply(Context &c, size_t L, size_t s1, size_t s2, size_t batch, const u64 *a, const u64 *b, u64 *out, cudaStream_t st);
     void op_bfv_multiply(Context &c, size_t L, size_t s1, size_t s2, size_t batch, const u64 *a, const u64 *b, u64 *out, cudaStream_t st);
     void check_sizes(size_t s1, size_t s2);
+    // BFV multiplication accumulates its FastBConv sums unreduced in 128 bits: at most 64 products of words below 2^61 each, so a
+    // level whose base B would hold more than 64 primes (more than 64 primes in the level, or 64 with B enlarged) is rejected.
+    // check_bfv_multiply_level throws std::invalid_argument for such a level of a BFV context and does nothing otherwise.
+    constexpr size_t kBfvMultiplyMaxBase = 64;
+    void check_bfv_multiply_level(const Context &c, size_t L);
     void launch_tensor_general(Context &c, const u64 *xa, long long xa_bs, const u64 *xb, long long xb_bs, u64 *out, const int *pid_tab,
                                size_t nb, size_t s1, size_t s2, size_t B, cudaStream_t st);
     void op_relinearize(Context &c, size_t L, size_t batch, const u64 *in3, const KSwitchKey &key, u64 *out2, cudaStream_t st);

@@ -218,14 +218,19 @@ namespace sbh
         return b;
     }
 
+    std::size_t behz_base_size(const std::vector<u64> &q, std::size_t L, u64 t)
+    {
+        // rns.cpp:605-612: enlarge B by one prime when K*n*t*q^2 < q*prod(B)*m_sk would not hold
+        if (32 + bit_count(t) + product_bit_count(q.data(), L) >= 61 * static_cast<int>(L) + 61)
+            return L + 1;
+        return L;
+    }
+
     BehzLevel build_behz(std::size_t n, const std::vector<u64> &q, std::size_t L, u64 t)
     {
         BehzLevel b;
         b.L = L;
-        b.nB = L;
-        // rns.cpp:605-612: enlarge B by one prime when K*n*t*q^2 < q*prod(B)*m_sk would not hold
-        if (32 + bit_count(t) + product_bit_count(q.data(), L) >= 61 * static_cast<int>(L) + 61)
-            b.nB++;
+        b.nB = behz_base_size(q, L, t);
         b.nBsk = b.nB + 1;
         auto aux = get_primes(2 * static_cast<u64>(n), 61, b.nBsk + 1); // [m_sk, gamma, B...]  rns.cpp:626-632
         b.m_sk = aux[0];

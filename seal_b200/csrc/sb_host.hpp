@@ -99,6 +99,8 @@ namespace sbh
         TwPair inv_B_mod_msk{};
         std::vector<TwPair> prod_B_mod_q, neg_prod_B_mod_q; // [L]
     };
+    // |B| of the level with the first L primes of q: L, or L + 1 when K n t q^2 < q prod(B) m_sk needs it (rns.cpp:605-612)
+    std::size_t behz_base_size(const std::vector<u64> &q, std::size_t L, u64 t);
     BehzLevel build_behz(std::size_t n, const std::vector<u64> &q, std::size_t L, u64 t);
 
 

@@ -21,6 +21,15 @@ def rand_ct(rng, moduli, n, size, L, batch=None):
     return np.stack([one() for _ in range(batch)])
 
 
+def assert_words(got, want, what):
+    """word-for-word equality; on failure name the first mismatching index"""
+    got, want = np.asarray(got), np.asarray(want)
+    assert got.shape == want.shape, (what, got.shape, want.shape)
+    bad = np.argwhere(got != want)
+    assert len(bad) == 0, f"{what}: {len(bad)} words differ, first at index {tuple(int(v) for v in bad[0])}: " \
+                          f"got {int(got[tuple(bad[0])])}, want {int(want[tuple(bad[0])])}"
+
+
 # ---- structured inputs at the arithmetic bounds (tests/test_gpu_bounds.py) ----
 # Each generator returns words laid out like rand_ct, [size][L][n] or [batch][size][L][n]; the prime of row i is moduli[i].
 
@@ -80,3 +89,66 @@ def all_coeffs_ntt(ntt_rows, moduli, n, L):
 def negacyclic_ones_square(n):
     """coefficient x of (1 + x + ... + x^(n-1))^2 mod x^n + 1, as Python ints: 2x + 2 - n"""
     return [2 * x + 2 - n for x in range(n)]
+
+
+def product(values):
+    out = 1
+    for v in values:
+        out *= int(v)
+    return out
+
+
+def centred_extreme_ct(moduli, n, size, L, sign, batch=None):
+    """every coefficient the centred extreme of the level's modulus Q = q_0 ... q_{L-1}: floor(Q / 2) mod q_i (sign +1, the
+    largest positive centred value) or ceil(Q / 2) mod q_i (sign -1, the most negative one, -floor(Q / 2)).  Two such
+    constant-coefficient polynomials c (1 + x + ... + x^(n-1)) multiply to c^2 (2x + 2 - n): coefficient n - 1 of the tensor
+    reaches n floor(Q / 2)^2."""
+    Q = product(moduli[:L])
+    c = Q // 2 if sign > 0 else (Q + 1) // 2
+    rows = np.stack([np.full(n, c % int(moduli[i]), dtype=np.uint64) for i in range(L)])
+    shape = (size, L, n) if batch is None else (batch, size, L, n)
+    return np.broadcast_to(rows, shape).copy()
+
+
+def alternating_extreme_ct(moduli, n, size, L, batch=None):
+    """coefficients floor(Q / 2), ceil(Q / 2), floor(Q / 2), ... (the two centred extremes alternating along every row)"""
+    out = centred_extreme_ct(moduli, n, size, L, +1, batch)
+    out[..., 1::2] = centred_extreme_ct(moduli, n, size, L, -1, batch)[..., 1::2]
+    return out
+
+
+# ---- primes (numth.cpp:278-311) ----
+
+def is_prime(m):
+    """deterministic Miller-Rabin below 2^64"""
+    if m < 2:
+        return False
+    for p in (2, 3, 5, 7, 11, 13, 17, 19, 23, 29, 31, 37):
+        if m % p == 0:
+            return m == p
+    d, s = m - 1, 0
+    while d % 2 == 0:
+        d, s = d // 2, s + 1
+    for a in (2, 3, 5, 7, 11, 13, 17, 19, 23, 29, 31, 37):
+        x = pow(a, d, m)
+        if x in (1, m - 1):
+            continue
+        for _ in range(s - 1):
+            x = x * x % m
+            if x == m - 1:
+                break
+        else:
+            return False
+    return True
+
+
+def ntt_primes_below(bits, n, count):
+    """the `count` largest primes = 1 mod 2n below 2^bits, largest first: get_primes(2n, bits, count), the BEHZ auxiliary list
+    for bits = 61 (CoeffModulus::Create takes the same primes for equal bit sizes, smallest first)"""
+    out, c = [], ((1 << bits) - 1) // (2 * n) * (2 * n) + 1
+    while len(out) < count:
+        assert c > 1 << (bits - 1), "not enough primes"
+        if is_prime(c):
+            out.append(c)
+        c -= 2 * n
+    return out

@@ -9,7 +9,7 @@ import pytest
 
 import oracle as O
 import refseal as R
-from common import alternating_ct, const_ntt_row, max_ct, negacyclic_ones_square, rand_ct, unreduce, zero_ct
+from common import alternating_ct, assert_words, const_ntt_row, is_prime, max_ct, negacyclic_ones_square, ntt_primes_below, rand_ct, unreduce, zero_ct
 
 pytestmark = pytest.mark.gpu
 
@@ -20,48 +20,6 @@ def sb():
     import seal_b200
 
     return seal_b200
-
-
-def assert_words(got, want, what):
-    """word-for-word equality; on failure name the first mismatching index"""
-    got, want = np.asarray(got), np.asarray(want)
-    assert got.shape == want.shape, (what, got.shape, want.shape)
-    bad = np.argwhere(got != want)
-    assert len(bad) == 0, f"{what}: {len(bad)} words differ, first at index {tuple(int(v) for v in bad[0])}: " \
-                          f"got {int(got[tuple(bad[0])])}, want {int(want[tuple(bad[0])])}"
-
-
-def is_prime(m):
-    if m < 2:
-        return False
-    for p in (2, 3, 5, 7, 11, 13, 17, 19, 23, 29, 31, 37):
-        if m % p == 0:
-            return m == p
-    d, s = m - 1, 0
-    while d % 2 == 0:
-        d, s = d // 2, s + 1
-    for a in (2, 3, 5, 7, 11, 13, 17, 19, 23, 29, 31, 37):  # deterministic below 2^64
-        x = pow(a, d, m)
-        if x in (1, m - 1):
-            continue
-        for _ in range(s - 1):
-            x = x * x % m
-            if x == m - 1:
-                break
-        else:
-            return False
-    return True
-
-
-def ntt_primes_below(bits, n, count):
-    """the `count` largest primes = 1 mod 2n below 2^bits, largest first (CoeffModulus::Create for equal bit sizes)"""
-    out, c = [], ((1 << bits) // (2 * n)) * (2 * n) + 1
-    while len(out) < count:
-        c -= 2 * n
-        if c.bit_length() == bits and is_prime(c):
-            out.append(c)
-        assert c > 1 << (bits - 1), "not enough primes"
-    return out
 
 
 def mod_down(acc, acc_sp, q, qsp):
