@@ -139,13 +139,18 @@ int sb200_selftest_rate(sb200_context *ctx, int kind, double *warp_ops_per_secon
  * round (the product kernel's form: one three-input 64-bit add per pair), and with both.  The transforms modulo the
  * auxiliary primes are exposed for the parity tests: _info returns the primes (capacity 8), _forward maps rows of n 64-bit
  * words to h_out[prime][row][n] (canonical residues, transformed), _inverse transforms h_data[row][prime][n] in place (values
- * in [0, 2p), not scaled by n^-1). */
+ * in [0, 2p), not scaled by n^-1).  _product runs the product step alone: h_Dh[prime][digit][ciphertext][n] and
+ * h_key[prime][digit][component 2][output prime L + 1][n] (canonical residues) -> h_Acc[ciphertext][2][L + 1][prime][n] (values in
+ * [0, 2p)); kernel 0 = the integer-pipe kernels, 1 = the INT8 tensor-core kernel where the shape allows it (L <= 32 digits,
+ * B >= 16 ciphertexts); *ran (may be NULL) receives the kernel that ran: 0 register tile, 1 key tile, 2 tensor cores. */
 int sb200_profile_read_work32(sb200_context *ctx, size_t index, char *name, size_t name_capacity, double *total_ms,
                               unsigned long long *launches, double *algorithmic_bytes, double *butterflies, double *macs,
                               double *butterflies32, double *macs32);
 int sb200_selftest_ksint_info(sb200_context *ctx, int *count, uint32_t *primes);
 int sb200_selftest_ksint_forward(sb200_context *ctx, const uint64_t *h_rows, size_t rows, uint32_t *h_out);
 int sb200_selftest_ksint_inverse(sb200_context *ctx, uint32_t *h_data, size_t rows);
+int sb200_selftest_ksint_product(sb200_context *ctx, const uint32_t *h_Dh, const uint32_t *h_key, size_t L, size_t B, uint32_t *h_Acc,
+                                 int kernel, int *ran);
 
 /* ---- key-switching keys --------------------------------------------------------------------------------------
  * h_key = the flattened KSwitchKeys::data()[index]: [digit j < digits][component 2][key prime k][coeff n], i.e. for

@@ -25,7 +25,7 @@ _STATUS = {-1: ValueError, -2: RuntimeError, -3: IndexError, -4: RuntimeError, -
 SYMBOLS = [
     "sb200_last_error", "sb200_context_create", "sb200_context_destroy", "sb200_coeff_modulus_create",
     "sb200_get_ntt_tables", "sb200_get_base_bsk", "sb200_galois_elt_from_step", "sb200_launch_count",
-    "sb200_device_bytes", "sb200_context_set_limit", "sb200_device_malloc", "sb200_device_free", "sb200_host_malloc", "sb200_host_free", "sb200_memcpy_h2d", "sb200_memcpy_d2h", "sb200_memcpy_d2d", "sb200_memcpy_d2d_2d", "sb200_stream_synchronize", "sb200_upload_rows", "sb200_download_rows", "sb200_rescale_to_next_sized", "sb200_mod_switch_to_next_sized", "sb200_relinearize_sized", "sb200_rescale_to_next_sized_host", "sb200_mod_switch_to_next_sized_host", "sb200_relinearize_sized_host", "sb200_device_numa_node", "sb200_device_index", "sb200_keyswitch_chunk", "sb200_profile_enable", "sb200_profile_reset", "sb200_profile_read", "sb200_profile_read_work", "sb200_selftest_rate", "sb200_profile_read_work32", "sb200_selftest_ksint_info", "sb200_selftest_ksint_forward", "sb200_selftest_ksint_inverse",
+    "sb200_device_bytes", "sb200_context_set_limit", "sb200_device_malloc", "sb200_device_free", "sb200_host_malloc", "sb200_host_free", "sb200_memcpy_h2d", "sb200_memcpy_d2h", "sb200_memcpy_d2d", "sb200_memcpy_d2d_2d", "sb200_stream_synchronize", "sb200_upload_rows", "sb200_download_rows", "sb200_rescale_to_next_sized", "sb200_mod_switch_to_next_sized", "sb200_relinearize_sized", "sb200_rescale_to_next_sized_host", "sb200_mod_switch_to_next_sized_host", "sb200_relinearize_sized_host", "sb200_device_numa_node", "sb200_device_index", "sb200_keyswitch_chunk", "sb200_profile_enable", "sb200_profile_reset", "sb200_profile_read", "sb200_profile_read_work", "sb200_selftest_rate", "sb200_profile_read_work32", "sb200_selftest_ksint_info", "sb200_selftest_ksint_forward", "sb200_selftest_ksint_inverse", "sb200_selftest_ksint_product",
     "sb200_kswitch_key_create", "sb200_kswitch_key_load", "sb200_kswitch_key_destroy", "sb200_ntt_forward",
     "sb200_ntt_inverse", "sb200_multiply", "sb200_multiply_sized", "sb200_square", "sb200_add", "sb200_sub", "sb200_negate", "sb200_multiply_plain", "sb200_batch_encode", "sb200_batch_decode", "sb200_plain_to_ntt", "sb200_multiply_plain_coeff", "sb200_add_plain_coeff", "sb200_relinearize", "sb200_multiply_relinearize", "sb200_rescale_to_next",
     "sb200_mod_switch_to_next", "sb200_apply_galois", "sb200_ntt_forward_host", "sb200_ntt_inverse_host",
@@ -89,6 +89,7 @@ def lib():
         L.sb200_selftest_ksint_info.argtypes = [vp, C.POINTER(i32), C.POINTER(u32)]
         L.sb200_selftest_ksint_forward.argtypes = [vp, _u64p, sz, C.POINTER(u32)]
         L.sb200_selftest_ksint_inverse.argtypes = [vp, C.POINTER(u32), sz]
+        L.sb200_selftest_ksint_product.argtypes = [vp, C.POINTER(u32), C.POINTER(u32), sz, sz, C.POINTER(u32), i32, C.POINTER(i32)]
         L.sb200_kswitch_key_create.argtypes = [vp, _u64p, sz, C.POINTER(vp)]
         L.sb200_kswitch_key_destroy.argtypes = [vp]
         L.sb200_kswitch_key_load.argtypes = [vp, C.c_char_p, sz, sz, C.POINTER(vp)]
@@ -374,6 +375,21 @@ class Context:
         data32 = np.ascontiguousarray(data32, dtype=np.uint32).copy()
         _check(lib().sb200_selftest_ksint_inverse(self.h, data32.ctypes.data_as(C.POINTER(C.c_uint32)), data32.shape[0]))
         return data32
+
+    def ksint_product(self, dh, key32, kernel):
+        """the product step alone: dh [S][L][B][n], key32 [S][L][2][L+1][n] uint32 (canonical residues) -> (Acc [B][2][L+1][S][n]
+        with values in [0, 2p), the kernel that ran: 0 register tile, 1 key tile, 2 tensor cores); kernel 0 = the integer-pipe
+        kernels, 1 = the INT8 tensor-core kernel where the shape allows it (L <= 32, B >= 16)"""
+        dh = np.ascontiguousarray(dh, dtype=np.uint32)
+        key32 = np.ascontiguousarray(key32, dtype=np.uint32)
+        S, L, B, n = dh.shape
+        assert key32.shape == (S, L, 2, L + 1, n)
+        out = np.empty((B, 2, L + 1, S, n), dtype=np.uint32)
+        ran = C.c_int(-1)
+        _check(lib().sb200_selftest_ksint_product(self.h, dh.ctypes.data_as(C.POINTER(C.c_uint32)),
+                                                  key32.ctypes.data_as(C.POINTER(C.c_uint32)), L, B,
+                                                  out.ctypes.data_as(C.POINTER(C.c_uint32)), kernel, C.byref(ran)))
+        return out, ran.value
 
     def selftest_rate(self, kind):
         """warp-level butterflies (kind 0, 1, 2) / key multiply-accumulates (kind 3) per second, registers only"""

@@ -552,6 +552,26 @@ int sb200_selftest_ksint_inverse(sb200_context *ctx, uint32_t *h_data, size_t ro
     SB_CATCH
 }
 
+int sb200_selftest_ksint_product(sb200_context *ctx, const uint32_t *h_Dh, const uint32_t *h_key, size_t L, size_t B, uint32_t *h_Acc,
+                                 int kernel, int *ran)
+{
+    SB_NEED(ctx);
+    SB_NEED(h_Dh);
+    SB_NEED(h_key);
+    SB_NEED(h_Acc);
+    SB_TRY
+    Context &c = *ctx->c;
+    std::lock_guard<std::mutex> lock(c.mu);
+    cuda_check(cudaSetDevice(c.device), "cudaSetDevice");
+    if (L > 1024 || B > (size_t(1) << 20))
+        throw std::invalid_argument("product: L or B out of range");
+    const int r = ksint_selftest_product(c, h_Dh, h_key, static_cast<int>(L), static_cast<int>(B), h_Acc, kernel);
+    if (ran)
+        *ran = r;
+    return SB200_OK;
+    SB_CATCH
+}
+
 int sb200_selftest_rate(sb200_context *ctx, int kind, double *warp_ops_per_second)
 {
     SB_NEED(warp_ops_per_second);

@@ -617,10 +617,218 @@ namespace sb
             }
         }
     }
-    template <int LOGN>
-    static void launch_mac(const KsIntScratch &s, const uint32_t *key32, const KsInt &d, int L, int k, int digits, int B, int nbt, int n,
-                           cudaStream_t st)
+    // The same product on the INT8 tensor cores.  For one auxiliary prime t and coefficient x the sum is a small integer GEMM,
+    // [B x L] . [L x 2(L+1)] (ciphertexts x digits, digits x outputs).  Every canonical 29-bit word splits into four u8 limbs; the 16
+    // limb-pair products of one m16n8k32 step go to 7 s32 class accumulators C_s = sum_{l+m=s} sum_J d_l k_m, each below
+    // 4 * 32 * 255^2 < 2^31 (no wrap whatever the words), and sum_s C_s 2^(8s) is the exact 64-bit sum ks32_mac_tile forms: the same
+    // Acc words.  A CTA (8 warps) owns 8 coefficients of one auxiliary prime -- 32-byte runs of every Acc row -- and all outputs.  It
+    // stages the key of its coefficients once, split into limb planes in B-fragment order, and walks the chunk 16 ciphertexts at a
+    // time: the digit tile of the next 16 arrives by cp.async while the current one is byte-transposed into A fragments (one pass,
+    // shared by all output tiles) and multiplied.  Warp w takes output tiles w, w + 8 for all 8 coefficients, so a thread ends with
+    // the 8 consecutive x of each of its Acc rows (one 32-byte sector; stored by two lanes).  One K step: L <= 32 digits, and digits
+    // J >= L meet zero key limbs.  Shared memory 112 KB at L = 31: two CTAs per SM.
+    constexpr int kMmaX = 8, kMmaMaxDigits = 32;
+    constexpr int kMmaAfStride = 4 * 128 + 4; // words of one coefficient's A fragments; +4: the transposition's writes are conflict-free
+    constexpr size_t mac_mma_smem(int nt) { return static_cast<size_t>(nt) * 8192 + 2 * 16384 + kMmaX * kMmaAfStride * 4; }
+    __device__ __forceinline__ void cp_async16(uint32_t *dst_smem, const uint32_t *src)
     {
+        asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst_smem)), "l"(src) : "memory");
+    }
+    // 4 x 4 byte transpose: byte j of l[m] = byte m of w[j] (limb m of four consecutive digits: one fragment register)
+    __device__ __forceinline__ void limbs4(const uint32_t (&w)[4], uint32_t (&l)[4])
+    {
+        const uint32_t t0 = __byte_perm(w[0], w[1], 0x5140), t1 = __byte_perm(w[0], w[1], 0x7362);
+        const uint32_t t2 = __byte_perm(w[2], w[3], 0x5140), t3 = __byte_perm(w[2], w[3], 0x7362);
+        l[0] = __byte_perm(t0, t2, 0x5410), l[1] = __byte_perm(t0, t2, 0x7632);
+        l[2] = __byte_perm(t1, t3, 0x5410), l[3] = __byte_perm(t1, t3, 0x7632);
+    }
+    __device__ __forceinline__ void mma_u8(uint32_t (&c)[4], const uint4 &a, const uint2 &b)
+    {
+        asm("mma.sync.aligned.m16n8k32.row.col.s32.u8.u8.s32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+            : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
+            : "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w), "r"(b.x), "r"(b.y));
+    }
+    __device__ __forceinline__ u64 madw(uint32_t a, uint32_t b, u64 c)
+    {
+        asm("mad.wide.u32 %0, %1, %2, %0;" : "+l"(c) : "r"(a), "r"(b));
+        return c;
+    }
+    // grid = (n / 8, S); dynamic shared memory mac_mma_smem(ceil(2 (L + 1) / 8))
+    template <int LOGN>
+    __global__ void __launch_bounds__(256, 2) ks32_mac_mma(const uint32_t *__restrict__ Dh, const uint32_t *__restrict__ key32, uint32_t *__restrict__ Acc,
+                                                            KsIntParams prm, int L, int k, int digits, int B, int Bpad)
+    {
+        extern __shared__ __align__(16) unsigned char ks_mma_smem[];
+        const int NO = 2 * (L + 1), NT = (NO + 7) / 8;
+        uint2 *kf = reinterpret_cast<uint2 *>(ks_mma_smem);                  // [x][output tile][limb][lane]
+        uint32_t *ds = reinterpret_cast<uint32_t *>(ks_mma_smem + NT * 8192); // [stage][J][b][x]: 16-byte chunks, swizzled
+        uint32_t *af = ds + 2 * 4096;                                          // [x][limb][lane][4], kMmaAfStride words per x
+        const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+        const int x0 = blockIdx.x * kMmaX, t = blockIdx.y;
+        // digit rows (J, b0 + b) -> stage; chunk h of row (J, b) goes to chunk q ^ (b bit 3 -> bit 2) ^ (J bit 4 -> bit 0) so that the
+        // transposition's reads are conflict-free.  Rows past Bpad and digits past L are not copied: their stale words meet only
+        // products that are never stored, or zero key limbs
+        const uint32_t *dbase = Dh + ((static_cast<size_t>(t) * L * Bpad) << LOGN) + x0;
+        auto load_tile = [&](int b0, int stage) {
+            uint32_t *dst = ds + stage * 4096;
+            for (int it = tid; it < L * 32; it += 256)
+            {
+                const int J = it >> 5, b = (it >> 1) & 15, h = it & 1;
+                if (b0 + b < Bpad)
+                {
+                    const int q = ((J * 16 + b) * 2 + h) ^ (((b >> 3) & 1) << 2) ^ ((J >> 4) & 1);
+                    cp_async16(dst + q * 4, dbase + ((static_cast<size_t>(J) * Bpad + b0 + b) << LOGN) + 4 * h);
+                }
+            }
+            asm volatile("cp.async.commit_group;" ::: "memory");
+        };
+        load_tile(0, 0);
+        // the key of the 8 coefficients: lane (g, i) of output tile nt holds limb m of digits 4i .. 4i + 3 and 16 + 4i .. 16 + 4i + 3
+        // of output 8 nt + g (output o = c (L + 1) + I' is key row c k + I'); four items' loads are in flight together
+        {
+            const uint32_t *kbase = key32 + ((static_cast<size_t>(t) * digits * 2 * k) << LOGN) + x0;
+            for (int it0 = tid; it0 < NT * 256; it0 += 4 * 256)
+            {
+                uint32_t w[4][2][4];
+#pragma unroll
+                for (int u = 0; u < 4; u++)
+                {
+                    const int it = it0 + u * 256, x = it & 7, ln = (it >> 3) & 31, o = 8 * (it >> 8) + (ln >> 2);
+                    const int c = o > L ? 1 : 0, row = c * k + o - c * (L + 1);
+#pragma unroll
+                    for (int hh = 0; hh < 2; hh++)
+#pragma unroll
+                        for (int j = 0; j < 4; j++)
+                        {
+                            const int J = 16 * hh + 4 * (ln & 3) + j;
+                            w[u][hh][j] = (it < NT * 256 && J < L && o < NO) ? __ldg(kbase + (static_cast<size_t>(J * 2 * k + row) << LOGN) + x) : 0;
+                        }
+                }
+#pragma unroll
+                for (int u = 0; u < 4; u++)
+                {
+                    const int it = it0 + u * 256;
+                    if (it < NT * 256)
+                    {
+                        uint32_t l0[4], l1[4];
+                        limbs4(w[u][0], l0), limbs4(w[u][1], l1);
+#pragma unroll
+                        for (int m = 0; m < 4; m++)
+                            kf[(((it & 7) * NT + (it >> 8)) * 4 + m) * 32 + ((it >> 3) & 31)] = make_uint2(l0[m], l1[m]);
+                    }
+                }
+            }
+        }
+        const P32 P = make_p32(prm.p[t]);
+        const uint2 red = prm.red[t];
+        const uint32_t mu = prm.mu[t];
+        const int g = lane >> 2, tig = lane & 3;
+        int stage = 0;
+        for (int b0 = 0; b0 < B; b0 += 16, stage ^= 1)
+        {
+            asm volatile("cp.async.wait_group 0;" ::: "memory");
+            __syncthreads(); // this tile has landed; the other stage and the fragments are free
+            if (b0 + 16 < B)
+                load_tile(b0 + 16, stage ^ 1);
+            // transposition: an item (x, b, digit quad Jq) -> limb registers of the A fragment of x.  Lane bits: x & 3, b & 1, b >> 3,
+            // Jq >> 2; warp and round bits: x >> 2, (b >> 1) & 3, Jq & 3 (digit reads and fragment writes both conflict-free)
+            const uint32_t *src = ds + stage * 4096;
+#pragma unroll
+            for (int rr = 0; rr < 4; rr++)
+            {
+                const int r = warp * 4 + rr;
+                const int x = (r & 1) * 4 + (lane & 3), b = ((lane >> 3) & 1) * 8 + ((r >> 1) & 3) * 2 + ((lane >> 2) & 1);
+                const int Jq = (lane >> 4) * 4 + (r >> 3);
+                uint32_t w[4], l[4];
+#pragma unroll
+                for (int j = 0; j < 4; j++)
+                {
+                    const int J = 4 * Jq + j;
+                    const int q = ((J * 16 + b) * 2 + (x >> 2)) ^ (((b >> 3) & 1) << 2) ^ ((J >> 4) & 1);
+                    w[j] = src[q * 4 + (x & 3)];
+                }
+                limbs4(w, l);
+                // A fragment of m16n8k32: register 0 = row g, digits 4i ..; 1 = row g + 8; 2 = row g, digits 16 + 4i ..; 3 = row g + 8
+                const int fl = (b & 7) * 4 + (Jq & 3), reg = (b >> 3) + 2 * (Jq >> 2);
+#pragma unroll
+                for (int m = 0; m < 4; m++)
+                    af[x * kMmaAfStride + m * 128 + fl * 4 + reg] = l[m];
+            }
+            __syncthreads();
+            // output tile nt, all 8 coefficients; the A fragment of one limb is read just before its four products
+            for (int nt = warp; nt < NT; nt += 8)
+            {
+                uint32_t res[kMmaX][4];
+#pragma unroll
+                for (int x = 0; x < kMmaX; x++)
+                {
+                    uint2 bf[4];
+#pragma unroll
+                    for (int m = 0; m < 4; m++)
+                        bf[m] = kf[((x * NT + nt) * 4 + m) * 32 + lane];
+                    uint32_t cs[7][4];
+#pragma unroll
+                    for (int s = 0; s < 7; s++)
+#pragma unroll
+                        for (int e = 0; e < 4; e++)
+                            cs[s][e] = 0;
+#pragma unroll
+                    for (int l = 0; l < 4; l++)
+                    {
+                        const uint4 a = *reinterpret_cast<const uint4 *>(af + x * kMmaAfStride + l * 128 + lane * 4);
+#pragma unroll
+                        for (int m = 0; m < 4; m++)
+                            mma_u8(cs[l + m], a, bf[m]);
+                    }
+#pragma unroll
+                    for (int e = 0; e < 4; e++)
+                    {
+                        const u64 lo = madw(cs[3][e], 1u << 24, madw(cs[2][e], 1u << 16, madw(cs[1][e], 1u << 8, cs[0][e])));
+                        const u64 hi = madw(cs[6][e], 1u << 16, madw(cs[5][e], 1u << 8, cs[4][e]));
+                        res[x][e] = minsub(reduce64(lo + (hi << 32), red, mu, P), P.p2);
+                    }
+                }
+                // C fragment: e = 0, 1: row g, outputs 2i, 2i + 1; e = 2, 3: row g + 8.  Lanes i and i ^ 1 swap half of their words so
+                // that every store writes whole 32-byte sectors: the first store is row (2 (i & ~1) + e & 1) -- x 0..3 from the even
+                // lane, x 4..7 from the odd one -- the second row (2 (i | 1) + e & 1).  (Half-sector stores made the kernel 2.4x slower.)
+                const int half = tig & 1;
+#pragma unroll
+                for (int e = 0; e < 4; e++)
+                {
+                    uint32_t keep[4], recv[4];
+#pragma unroll
+                    for (int j = 0; j < 4; j++)
+                    {
+                        keep[j] = half ? res[4 + j][e] : res[j][e];
+                        recv[j] = __shfl_xor_sync(0xffffffffu, half ? res[j][e] : res[4 + j][e], 1);
+                    }
+                    const int b = b0 + g + 8 * (e >> 1), oA = 8 * nt + 2 * (tig & 2) + (e & 1), oB = oA + 2;
+                    const uint4 vA = half ? make_uint4(recv[0], recv[1], recv[2], recv[3]) : make_uint4(keep[0], keep[1], keep[2], keep[3]);
+                    const uint4 vB = half ? make_uint4(keep[0], keep[1], keep[2], keep[3]) : make_uint4(recv[0], recv[1], recv[2], recv[3]);
+                    if (b < B && oA < NO)
+                        *reinterpret_cast<uint4 *>(Acc + ((static_cast<size_t>(b * NO + oA) * prm.S + t) << LOGN) + x0 + 4 * half) = vA;
+                    if (b < B && oB < NO)
+                        *reinterpret_cast<uint4 *>(Acc + ((static_cast<size_t>(b * NO + oB) * prm.S + t) << LOGN) + x0 + 4 * half) = vB;
+                }
+            }
+        }
+    }
+    // returns the kernel that ran: 0 register tile, 1 key tile, 2 tensor cores
+    template <int LOGN>
+    static int launch_mac(const KsIntScratch &s, const uint32_t *key32, const KsInt &d, int L, int k, int digits, int B, int nbt, int n,
+                          cudaStream_t st)
+    {
+        // below 16 ciphertexts the key tile every CTA stages outweighs the products: the integer kernels take those chunks (H100,
+        // n = 65536, 31 digits, ms per multiply + relinearize call with / without the tensor cores: 3.1 / 1.6 at B = 1, 8.1 / 8.2 at
+        // B = 15, 8.4 / 9.0 at B = 16)
+        if (d.mac_mma && L <= kMmaMaxDigits && B >= 16)
+        {
+            const size_t smem = mac_mma_smem((2 * (L + 1) + 7) / 8);
+            cuda_check(cudaFuncSetAttribute(ks32_mac_mma<LOGN>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)), "smem attr");
+            const dim3 grid(static_cast<unsigned>(n / kMmaX), static_cast<unsigned>(d.prm.S));
+            ks32_mac_mma<LOGN><<<grid, 256, smem, st>>>(s.Dh, key32, s.Acc, d.prm, L, k, digits, B, nbt * kMacTB);
+            return 2;
+        }
         const int ntile = (L + kMacTC) / kMacTC, ny = (2 * ntile + 3) / 4;
         const size_t tile_smem = static_cast<size_t>(L) * 4096 + kMacRingBytes;
         // the tile kernel walks over all ciphertexts with one CTA per (coefficient tile, output group): worth it from a few tiles on
@@ -629,11 +837,27 @@ namespace sb
             cuda_check(cudaFuncSetAttribute(ks32_mac_tile<LOGN>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(tile_smem)), "smem attr");
             dim3 grid(static_cast<unsigned>(ny) * static_cast<unsigned>(n / 32), 1, static_cast<unsigned>(d.prm.S));
             ks32_mac_tile<LOGN><<<grid, 512, tile_smem, st>>>(s.Dh, key32, s.Acc, d.prm, L, k, digits, B, nbt * kMacTB);
-            return;
+            return 1;
         }
         cuda_check(cudaFuncSetAttribute(ks32_mac<LOGN>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMacSmem), "smem attr");
         dim3 grid(static_cast<unsigned>(nbt) * static_cast<unsigned>(ny) * static_cast<unsigned>(n / 32), 1, static_cast<unsigned>(d.prm.S));
         ks32_mac<LOGN><<<grid, 128, kMacSmem, st>>>(s.Dh, key32, s.Acc, d.prm, L, k, digits, B, nbt);
+        return 0;
+    }
+    static int launch_mac_logn(const KsIntScratch &s, const uint32_t *key32, const KsInt &d, int L, int k, int digits, int B, int nbt, int logn,
+                               cudaStream_t st)
+    {
+        const int n = 1 << logn;
+        switch (logn)
+        {
+        case 12: return launch_mac<12>(s, key32, d, L, k, digits, B, nbt, n, st);
+        case 13: return launch_mac<13>(s, key32, d, L, k, digits, B, nbt, n, st);
+        case 14: return launch_mac<14>(s, key32, d, L, k, digits, B, nbt, n, st);
+        case 15: return launch_mac<15>(s, key32, d, L, k, digits, B, nbt, n, st);
+        case 16: return launch_mac<16>(s, key32, d, L, k, digits, B, nbt, n, st);
+        case 17: return launch_mac<17>(s, key32, d, L, k, digits, B, nbt, n, st);
+        default: throw std::logic_error("unsupported transform size");
+        }
     }
 
     // -------------------------------------------------------------- (4) reconstruction + mod-down, per coefficient ----
@@ -1080,6 +1304,8 @@ namespace sb
             d.fuse_ntt = std::atoi(e) != 0;
         if (const char *e = std::getenv("SB200_KS_MAC_TILE"))
             d.mac_tile = std::atoi(e) != 0;
+        if (const char *e = std::getenv("SB200_KS_MAC_MMA"))
+            d.mac_mma = std::atoi(e) != 0;
         d.ready = true;
     }
     void ksint_free(Context &c)
@@ -1243,18 +1469,9 @@ namespace sb
         {
             // one pass over the key + the transformed digits in, the sums out
             c.stats.begin("ks32_mac", 0, 4.0 * n * S * (static_cast<double>(Li) * 2 * (Li + 1) + rows + arows), st);
-            c.stats.work32(0, static_cast<double>(arows) * Li * S * n);
-            const int dg = static_cast<int>(key.digits), ni = static_cast<int>(c.n);
-            switch (c.logn)
-            {
-            case 12: launch_mac<12>(s, key.d_key32, d, Li, ki, dg, Bi, nbt, ni, st); break;
-            case 13: launch_mac<13>(s, key.d_key32, d, Li, ki, dg, Bi, nbt, ni, st); break;
-            case 14: launch_mac<14>(s, key.d_key32, d, Li, ki, dg, Bi, nbt, ni, st); break;
-            case 15: launch_mac<15>(s, key.d_key32, d, Li, ki, dg, Bi, nbt, ni, st); break;
-            case 16: launch_mac<16>(s, key.d_key32, d, Li, ki, dg, Bi, nbt, ni, st); break;
-            case 17: launch_mac<17>(s, key.d_key32, d, Li, ki, dg, Bi, nbt, ni, st); break;
-            default: throw std::logic_error("unsupported transform size");
-            }
+            // integer-pipe multiply-accumulates only: the tensor-core kernel's products are not work against the mac32 ceiling (DESIGN 4)
+            if (launch_mac_logn(s, key.d_key32, d, Li, ki, static_cast<int>(key.digits), Bi, nbt, static_cast<int>(c.logn), st) != 2)
+                c.stats.work32(0, static_cast<double>(arows) * Li * S * n);
             c.stats.end(st);
             cuda_check(cudaGetLastError(), "ks32_mac");
         }
@@ -1366,6 +1583,33 @@ namespace sb
                           RowMap{ 0, 0, static_cast<int>(rows) }, nullptr);
         }
         cuda_check(cudaMemcpy(h_io, d32, out_bytes, cudaMemcpyDeviceToHost), "download");
+    }
+
+    int ksint_selftest_product(Context &c, const uint32_t *h_Dh, const uint32_t *h_key, int L, int B, uint32_t *h_Acc, int mma)
+    {
+        if (!c.ksint.ready)
+            throw std::logic_error("integer key-switching path is not available for this context");
+        if (L < 1 || B < 1 || static_cast<size_t>(L) > c.ksint.max_digits)
+            throw std::invalid_argument("product: 1 <= L <= max_digits and B >= 1");
+        KsInt d = c.ksint;
+        d.mac_mma = mma != 0;
+        const size_t S = d.prm.S, n = c.n, Bpad = (B + kMacTB - 1) / kMacTB * kMacTB, k = L + 1;
+        const size_t dh_words = S * L * Bpad * n, key_words = S * L * 2 * k * n, acc_words = B * 2 * k * S * n;
+        // + 8 key rows of slack, as ksint_prepare_key allocates them
+        uint32_t *base = static_cast<uint32_t *>(c.ensure_scratch((dh_words + key_words + 8 * n + acc_words) * sizeof(uint32_t)));
+        KsIntScratch s;
+        s.Dh = base;
+        uint32_t *key = base + dh_words;
+        s.Acc = key + key_words + 8 * n;
+        cuda_check(cudaMemset(s.Dh, 0, dh_words * sizeof(uint32_t)), "memset");
+        cuda_check(cudaMemcpy2D(s.Dh, Bpad * n * sizeof(uint32_t), h_Dh, B * n * sizeof(uint32_t), B * n * sizeof(uint32_t), S * L,
+                                cudaMemcpyHostToDevice), "upload");
+        cuda_check(cudaMemcpy(key, h_key, key_words * sizeof(uint32_t), cudaMemcpyHostToDevice), "upload");
+        cuda_check(cudaMemset(key + key_words, 0, 8 * n * sizeof(uint32_t)), "memset");
+        const int ran = launch_mac_logn(s, key, d, L, static_cast<int>(k), L, B, static_cast<int>(Bpad / kMacTB), static_cast<int>(c.logn), nullptr);
+        cuda_check(cudaGetLastError(), "ks32_mac");
+        cuda_check(cudaMemcpy(h_Acc, s.Acc, acc_words * sizeof(uint32_t), cudaMemcpyDeviceToHost), "download");
+        return ran;
     }
 
     // ---- arithmetic ceilings of this path, measured in process: the butterflies / multiply-accumulates on registers only ----

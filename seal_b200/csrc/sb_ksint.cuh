@@ -35,6 +35,7 @@ namespace sb
     struct KsInt
     {
         bool ready = false;
+        bool mac_mma = true;   // product kernel on the INT8 tensor cores (env SB200_KS_MAC_MMA)
         bool mac_tile = true;  // product kernel with the key tile in shared memory (env SB200_KS_MAC_TILE)
         bool fuse_crt = true;  // outer inverse stages inside the reconstruction kernel (env SB200_KS_FUSE_CRT)
         bool fuse_ntt = true;  // entry and exit inside the column passes of the 64-bit transforms (env SB200_KS_FUSE_NTT)
@@ -69,4 +70,8 @@ namespace sb
     double ksint_selftest_rate(Context &c, int kind, cudaStream_t st);
     // parity-test access to the transforms: forward h_rows [rows][n] u64 -> h_io [S][rows][n]; inverse: h_io [rows][S][n] in place
     void ksint_selftest_transform(Context &c, bool inverse, const u64 *h_rows, size_t rows, uint32_t *h_io);
+    // parity-test access to the product step alone: h_Dh [S][L][B][n], h_key [S][L][2][L+1][n] (canonical words) ->
+    // h_Acc [B][2][L+1][S][n]; mma = 0: the integer-pipe kernels, 1: the tensor-core kernel where it applies (L <= 32, B >= 16).
+    // Returns the kernel that ran: 0 register tile, 1 key tile, 2 tensor cores
+    int ksint_selftest_product(Context &c, const uint32_t *h_Dh, const uint32_t *h_key, int L, int B, uint32_t *h_Acc, int mma);
 } // namespace sb
