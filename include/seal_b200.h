@@ -376,6 +376,27 @@ int sb200_encrypt_zero_symmetric(sb200_context *ctx, sb200_secret_key *key, size
 int sb200_encrypt_zero_symmetric_prng(sb200_context *ctx, sb200_secret_key *key, size_t L, size_t batch, int bootstrap_prng,
                                       int ciphertext_prng, const uint64_t *h_bootstrap_seeds, int save_seed, uint64_t *d_out,
                                       uint64_t *h_public_seeds, void *stream);
+/* ---- key generation from a given secret key: KeyGenerator(context, secret_key) (keygenerator.cpp:35-52) ----------------------
+ * The secret key itself is not sampled here: it comes from seal::KeyGenerator or is loaded.  Every key below is made of key-level
+ * encryptions of zero under `key` in NTT form (for every scheme, BFV included; BGV multiplies the noise by t), each drawn from one
+ * bootstrap PRNG of type bootstrap_prng (parms.random_generator()) whose c_1 expands with ciphertext_prng, as in
+ * sb200_encrypt_zero_symmetric_prng; a bootstrap seed of the reference's factory gives its key bit for bit.  Seeds NULL = fresh
+ * seeds from the OS entropy source.  Both calls are synchronous (default stream) and wipe the noise and PRNG streams they used.
+ * Errors: a key of another context or a PRNG type other than 1 or 2: SB200_E_INVALID_ARG; both outputs NULL: SB200_E_POINTER. */
+/* KeyGenerator::create_relin_keys (galois_elt = 0) / one element of create_galois_keys (keygenerator.cpp:122-226, 327-360)
+ * for the secret key `key`: digits = k - 1 key-level encryptions of zero (NTT form, every scheme) with (q_special mod q_j) s'_j
+ * added to row j of c_0, s' = s^2 or s under the Galois automorphism.  h_bootstrap_seeds = [k-1][8] (one per digit, in the
+ * reference's draw order) or NULL.  Outputs, either may be NULL but not both: h_key = [k-1][2][k][n] (KSwitchKeys::data()[index]
+ * words) and *out = a device key handle, as sb200_kswitch_key_create would make from those words, without the host round trip.
+ * k < 2: SB200_E_LOGIC "keyswitching is not supported by the context"; an even galois_elt or one >= 2n: SB200_E_INVALID_ARG
+ * "Galois element is not valid".  The digits are generated in chunks that fit SB200_LIMIT_SCRATCH_BYTES; the words do not
+ * depend on it. */
+int sb200_kswitch_key_generate(sb200_context *ctx, sb200_secret_key *key, uint32_t galois_elt, int bootstrap_prng,
+                               int ciphertext_prng, const uint64_t *h_bootstrap_seeds, uint64_t *h_key, sb200_kswitch_key **out);
+/* KeyGenerator::create_public_key (keygenerator.cpp:96-120): h_public_key = [2][k][n] and / or *out = an Encryptor key handle;
+ * h_bootstrap_seed = [8] or NULL */
+int sb200_public_key_generate(sb200_context *ctx, sb200_secret_key *key, int bootstrap_prng, int ciphertext_prng,
+                              const uint64_t *h_bootstrap_seed, uint64_t *h_public_key, sb200_public_key **out);
 /* d_ct [batch][size][L][n] in the scheme's own form -> d_plain: CKKS [batch][L][n] (NTT form, same level; the caller keeps
  * scale and parms_id); BFV [batch][n] coefficients mod t (dot product + decrypt_scale_and_round, rns.cpp:1133-1191);
  * BGV [batch][n] (dot product, INTT, exact base conversion rns.cpp:466-539, times the inverse of the ciphertext's

@@ -33,7 +33,7 @@ SYMBOLS = [
     "sb200_relinearize_host", "sb200_multiply_relinearize_host", "sb200_rescale_to_next_host",
     "sb200_mod_switch_to_next_host", "sb200_apply_galois_host", "sb200_get_parms_id", "sb200_ciphertext_inspect",
     "sb200_ciphertext_save_size", "sb200_ciphertext_load", "sb200_ciphertext_save", "sb200_secret_key_create",
-    "sb200_secret_key_destroy", "sb200_decrypt", "sb200_decrypt_host", "sb200_invariant_noise_budget", "sb200_invariant_noise_budget_host", "sb200_encrypt_zero_symmetric", "sb200_public_key_create", "sb200_public_key_destroy", "sb200_encrypt_zero_asymmetric", "sb200_encrypt_zero_symmetric_prng", "sb200_encrypt_zero_asymmetric_prng", "sb200_ckks_encode", "sb200_ckks_decode", "sb200_ckks_encode_host", "sb200_ckks_decode_host",
+    "sb200_secret_key_destroy", "sb200_decrypt", "sb200_decrypt_host", "sb200_invariant_noise_budget", "sb200_invariant_noise_budget_host", "sb200_encrypt_zero_symmetric", "sb200_public_key_create", "sb200_public_key_destroy", "sb200_encrypt_zero_asymmetric", "sb200_encrypt_zero_symmetric_prng", "sb200_encrypt_zero_asymmetric_prng", "sb200_kswitch_key_generate", "sb200_public_key_generate", "sb200_ckks_encode", "sb200_ckks_decode", "sb200_ckks_encode_host", "sb200_ckks_decode_host",
     "sb200_group_create", "sb200_group_destroy", "sb200_group_size", "sb200_group_context", "sb200_group_slice",
     "sb200_group_kswitch_key_create", "sb200_group_kswitch_key_destroy", "sb200_group_multiply_relinearize_host",
     "sb200_group_relinearize_host", "sb200_group_apply_galois_host", "sb200_group_multiply_host", "sb200_group_rescale_to_next_host",
@@ -154,6 +154,8 @@ def lib():
         L.sb200_encrypt_zero_asymmetric_prng.argtypes = [vp, vp, sz, sz, i32, _u64p, vp, vp]
         L.sb200_encrypt_zero_symmetric_prng.argtypes = [vp, vp, sz, sz, i32, i32, _u64p, i32, vp, _u64p, vp]
         L.sb200_decrypt_host.argtypes = [vp, vp, sz, sz, sz, _u64p, _u64p, _u64p]
+        L.sb200_kswitch_key_generate.argtypes = [vp, vp, u32, i32, i32, _u64p, _u64p, C.POINTER(vp)]
+        L.sb200_public_key_generate.argtypes = [vp, vp, i32, i32, _u64p, _u64p, C.POINTER(vp)]
         L.sb200_invariant_noise_budget.argtypes = [vp, vp, sz, sz, sz, vp, vp, vp]
         L.sb200_invariant_noise_budget_host.argtypes = [vp, vp, sz, sz, sz, _u64p, C.POINTER(i32)]
         _lib = L
@@ -211,6 +213,13 @@ class KSwitchKey:
         _check(lib().sb200_kswitch_key_create(ctx.h, _hp(host_key), host_key.shape[0], C.byref(h)))
         self.h = h
 
+    @classmethod
+    def wrap(cls, ctx, handle):
+        """take ownership of a key handle the library made (sb200_kswitch_key_generate)"""
+        self = cls.__new__(cls)
+        self.ctx, self.h = ctx, handle
+        return self
+
     def __del__(self):
         try:
             if getattr(self, "h", None):
@@ -230,6 +239,13 @@ class PublicKey:
         h = C.c_void_p()
         _check(lib().sb200_public_key_create(ctx.h, _hp(host_key), C.byref(h)))
         self.h = h
+
+    @classmethod
+    def wrap(cls, ctx, handle):
+        """take ownership of a key handle the library made (sb200_public_key_generate)"""
+        self = cls.__new__(cls)
+        self.ctx, self.h = ctx, handle
+        return self
 
     def __del__(self):
         try:
@@ -692,6 +708,30 @@ class Context:
                                                        None if seeds is None else _hp(seeds), int(save_seed), _dp(out2),
                                                        None if pub is None else _hp(pub), self._stream()))
         return pub
+
+    # ---- KeyGenerator(context, secret_key) ----
+    def generate_kswitch_key(self, sk, galois_elt=0, seeds=None, bootstrap_prng=1, ciphertext_prng=1, host=True, device=True):
+        """KeyGenerator.create_relin_keys (galois_elt 0) / the Galois key of one element for the secret key sk, generated on the
+        device; seeds [k-1][8] bootstrap seeds, one per digit (None = fresh from the OS entropy source).  Returns (host words
+        [k-1][2][k][n] or None, KSwitchKey or None)"""
+        digits = self.k - 1
+        seeds = None if seeds is None else np.ascontiguousarray(seeds, dtype=np.uint64).reshape(max(digits, 1), 8)
+        words = np.zeros((digits, 2, self.k, self.n), dtype=np.uint64) if host else None
+        h = C.c_void_p()
+        _check(lib().sb200_kswitch_key_generate(self.h, sk.h, galois_elt, bootstrap_prng, ciphertext_prng,
+                                                None if seeds is None else _hp(seeds), None if words is None else _hp(words),
+                                                C.byref(h) if device else None))
+        return words, (KSwitchKey.wrap(self, h) if device else None)
+
+    def generate_public_key(self, sk, seed=None, bootstrap_prng=1, ciphertext_prng=1, host=True, device=True):
+        """KeyGenerator.create_public_key for the secret key sk on the device; seed [8] (None = fresh).  Returns (host words
+        [2][k][n] or None, PublicKey or None)"""
+        seed = None if seed is None else np.ascontiguousarray(seed, dtype=np.uint64).reshape(8)
+        words = np.zeros((2, self.k, self.n), dtype=np.uint64) if host else None
+        h = C.c_void_p()
+        _check(lib().sb200_public_key_generate(self.h, sk.h, bootstrap_prng, ciphertext_prng, None if seed is None else _hp(seed),
+                                               None if words is None else _hp(words), C.byref(h) if device else None))
+        return words, (PublicKey.wrap(self, h) if device else None)
 
     def d_relinearize(self, in3, key, out2, L, batch):
         _check(lib().sb200_relinearize(self.h, L, batch, _dp(in3), key.h, _dp(out2), self._stream()))

@@ -645,6 +645,30 @@ int sb200_profile_read_work32(sb200_context *ctx, size_t index, char *name, size
     SB_CATCH
 }
 
+} // extern "C"
+
+// A device key handle is built in two steps around filling its words: kswitch_key_alloc makes the handle with room for `digits`
+// digits ([digits][2][k][n] at d_key); kswitch_key_finish then checks every word is below its modulus (is_data_valid_for,
+// valcheck.cpp:412-456: the fused key-switch kernel relies on it to keep its 128-bit sums in range; false = out of range, the caller
+// throws its own error) and prepares the integer key-switching path's copy of the key.
+static std::unique_ptr<sb200_kswitch_key> kswitch_key_alloc(Context &c, size_t digits)
+{
+    auto h = std::make_unique<sb200_kswitch_key>();
+    cuda_check(cudaMalloc(reinterpret_cast<void **>(&h->k.d_key), digits * 2 * c.k * c.n * sizeof(u64)), "cudaMalloc(key)");
+    h->k.ctx = &c;
+    h->k.digits = digits;
+    return h;
+}
+
+static bool kswitch_key_finish(Context &c, KSwitchKey &k)
+{
+    if (!op_residues_in_range(c, c.k, k.digits * 2 * c.k, k.d_key, nullptr))
+        return false;
+    ksint_prepare_key(c, k, nullptr);
+    return true;
+}
+
+extern "C" {
 int sb200_kswitch_key_create(sb200_context *ctx, const uint64_t *h_key, size_t digits, sb200_kswitch_key **out)
 {
     SB_NEED(ctx);
@@ -656,19 +680,12 @@ int sb200_kswitch_key_create(sb200_context *ctx, const uint64_t *h_key, size_t d
         throw std::logic_error("keyswitching is not supported by the context");
     if (digits < 1 || digits > c.k - 1)
         throw std::invalid_argument("kswitch key has an invalid number of digits");
-    auto h = std::make_unique<sb200_kswitch_key>();
-    size_t bytes = digits * 2 * c.k * c.n * sizeof(u64);
     std::lock_guard<std::mutex> lock(c.mu);
     cuda_check(cudaSetDevice(c.device), "cudaSetDevice");
-    cuda_check(cudaMalloc(reinterpret_cast<void **>(&h->k.d_key), bytes), "cudaMalloc(key)");
-    cuda_check(cudaMemcpy(h->k.d_key, h_key, bytes, cudaMemcpyHostToDevice), "upload key");
-    h->k.ctx = &c;
-    h->k.digits = digits;
-    // is_data_valid_for (valcheck.cpp:412-456): every word below its modulus -- the fused key-switch kernel relies on it to
-    // keep its 128-bit sums in range
-    if (!op_residues_in_range(c, c.k, digits * 2 * c.k, h->k.d_key, nullptr))
+    auto h = kswitch_key_alloc(c, digits);
+    cuda_check(cudaMemcpy(h->k.d_key, h_key, digits * 2 * c.k * c.n * sizeof(u64), cudaMemcpyHostToDevice), "upload key");
+    if (!kswitch_key_finish(c, h->k))
         throw std::invalid_argument("kswitch key data is not valid for encryption parameters");
-    ksint_prepare_key(c, h->k, nullptr);
     *out = h.release();
     return SB200_OK;
     SB_CATCH
@@ -696,13 +713,10 @@ int sb200_kswitch_key_load(sb200_context *ctx, const uint8_t *stream, size_t len
     // is_valid_for(KSwitchKeys) (valcheck.cpp:292-323): one public key per decomposition prime, i.e. exactly k-1 digits
     if (digits != c.k - 1)
         throw std::logic_error("KSwitchKeys data is invalid");
-    auto h = std::make_unique<sb200_kswitch_key>();
     const size_t row = 2 * c.k * c.n * sizeof(u64);
     std::lock_guard<std::mutex> lock(c.mu);
     cuda_check(cudaSetDevice(c.device), "cudaSetDevice");
-    cuda_check(cudaMalloc(reinterpret_cast<void **>(&h->k.d_key), digits * row), "cudaMalloc(key)");
-    h->k.ctx = &c;
-    h->k.digits = digits;
+    auto h = kswitch_key_alloc(c, digits);
     // a seed-compressed member carries c_0 only (k n words) and the seed of c_1 = sample_poly_uniform at the key level
     // (KSwitchKeys::load -> PublicKey::load -> Ciphertext::expand_seed, ciphertext.cpp:118-150)
     std::vector<u64> seeds;
@@ -724,9 +738,8 @@ int sb200_kswitch_key_load(sb200_context *ctx, const uint8_t *stream, size_t len
     }
     if (!seed_dst.empty())
         op_expand_seeded(c, c.k, seed_dst.size(), seeds.data(), types.data(), seed_dst.data(), h->k.d_key, nullptr);
-    if (!op_residues_in_range(c, c.k, digits * 2 * c.k, h->k.d_key, nullptr)) // KSwitchKeys::load ends in is_valid_for (kswitchkeys.cpp:149-153)
+    if (!kswitch_key_finish(c, h->k)) // KSwitchKeys::load ends in is_valid_for (kswitchkeys.cpp:149-153)
         throw std::logic_error("KSwitchKeys data is invalid");
-    ksint_prepare_key(c, h->k, nullptr);
     *out = h.release();
     return SB200_OK;
     SB_CATCH
@@ -1708,6 +1721,73 @@ int sb200_encrypt_zero_symmetric_prng(sb200_context *ctx, sb200_secret_key *key,
     op_encrypt_zero_symmetric(c, key->k, L, batch, (const u64 *)h_bootstrap_seeds, bootstrap_prng, ciphertext_prng, save_seed != 0, (u64 *)d_out,
                               (u64 *)h_public_seeds, static_cast<cudaStream_t>(stream));
     // op_encrypt_zero_symmetric synchronised the stream while expanding c_1: the seeds have been consumed and may be wiped
+    return SB200_OK;
+    SB_CATCH
+}
+
+// ---- KeyGenerator(context, secret_key)::create_public_key / create_relin_keys / create_galois_keys (sb_prng.cu) ----
+// The key is generated into the storage of the handle it becomes; when only the host words are asked for, that handle is a
+// temporary that goes away after the download.
+int sb200_public_key_generate(sb200_context *ctx, sb200_secret_key *key, int bootstrap_prng, int ciphertext_prng, const uint64_t *h_bootstrap_seed,
+                              uint64_t *h_public_key, sb200_public_key **out)
+{
+    SB_NEED(key);
+    if (!h_public_key && !out)
+    {
+        g_last_error = "null pointer: h_public_key and out";
+        return SB200_E_POINTER;
+    }
+    SB_TRY
+    SB_ENTER_STREAM(ctx, nullptr)
+    std::unique_ptr<FreshSeeds> fresh;
+    if (!h_bootstrap_seed)
+    {
+        fresh = std::make_unique<FreshSeeds>(1);
+        h_bootstrap_seed = reinterpret_cast<const uint64_t *>(fresh->words.data());
+    }
+    const size_t bytes = 2 * c.k * c.n * sizeof(u64);
+    auto h = std::make_unique<sb200_public_key>();
+    cuda_check(cudaMalloc(reinterpret_cast<void **>(&h->k.d_key), bytes), "cudaMalloc(public key)");
+    h->k.ctx = &c;
+    op_generate_public_key(c, key->k, bootstrap_prng, ciphertext_prng, (const u64 *)h_bootstrap_seed, h->k.d_key, nullptr);
+    cuda_check(cudaStreamSynchronize(nullptr), "synchronize");
+    if (h_public_key)
+        cuda_check(cudaMemcpy(h_public_key, h->k.d_key, bytes, cudaMemcpyDeviceToHost), "download public key");
+    if (out)
+        *out = h.release();
+    return SB200_OK;
+    SB_CATCH
+}
+
+int sb200_kswitch_key_generate(sb200_context *ctx, sb200_secret_key *key, uint32_t galois_elt, int bootstrap_prng, int ciphertext_prng,
+                               const uint64_t *h_bootstrap_seeds, uint64_t *h_key, sb200_kswitch_key **out)
+{
+    SB_NEED(key);
+    if (!h_key && !out)
+    {
+        g_last_error = "null pointer: h_key and out";
+        return SB200_E_POINTER;
+    }
+    SB_TRY
+    SB_ENTER_STREAM(ctx, nullptr)
+    const size_t digits = std::max<size_t>(c.k, 2) - 1; // k < 2 is rejected by op_generate_kswitch_key
+    std::unique_ptr<FreshSeeds> fresh;
+    if (!h_bootstrap_seeds)
+    {
+        fresh = std::make_unique<FreshSeeds>(digits);
+        h_bootstrap_seeds = reinterpret_cast<const uint64_t *>(fresh->words.data());
+    }
+    auto h = kswitch_key_alloc(c, digits);
+    op_generate_kswitch_key(c, key->k, galois_elt, bootstrap_prng, ciphertext_prng, (const u64 *)h_bootstrap_seeds, h->k.d_key, nullptr);
+    cuda_check(cudaStreamSynchronize(nullptr), "synchronize");
+    if (h_key)
+        cuda_check(cudaMemcpy(h_key, h->k.d_key, digits * 2 * c.k * c.n * sizeof(u64), cudaMemcpyDeviceToHost), "download key");
+    if (out)
+    {
+        if (!kswitch_key_finish(c, h->k))
+            throw std::logic_error("kswitch key data is not valid for encryption parameters");
+        *out = h.release();
+    }
     return SB200_OK;
     SB_CATCH
 }

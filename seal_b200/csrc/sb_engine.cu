@@ -982,7 +982,7 @@ namespace sb
         out.ctx = &c, out.powers = 1;
     }
     // Decryptor::compute_secret_key_array (decryptor.cpp:199-310): s^p = s^(p-1) * s, dyadic at the key level
-    static void ensure_key_powers(Context &c, SecretKey &sk, size_t powers, cudaStream_t st)
+    void ensure_key_powers(Context &c, SecretKey &sk, size_t powers, cudaStream_t st)
     {
         if (powers <= sk.powers)
             return;

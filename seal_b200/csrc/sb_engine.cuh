@@ -224,6 +224,22 @@ namespace sb
     // the type of the bootstrap PRNG (parms.random_generator()), ct_prng = the type c_1 is expanded with (the DefaultFactory's)
     void op_encrypt_zero_symmetric(Context &c, const SecretKey &sk, size_t L, size_t B, const u64 *h_boot_seeds, int boot_prng, int ct_prng,
                                    bool save_seed, u64 *d_out, u64 *h_public_seeds, cudaStream_t st);
+    // KeyGenerator on the device (sb_prng.cu), for a secret key the caller supplies.  What turns a key-level encryption of zero into
+    // digit digit0 + b of a key-switching key: s'_j[i] = new_key[j][perm ? perm[i] : i] (sb_prng.cu: enc_kernel MODE 7)
+    struct KsFactor
+    {
+        const u64 *new_key = nullptr;   // [k][n], NTT form
+        const uint32_t *perm = nullptr; // NTT-form Galois table, or nullptr
+        long long digit0 = 0;
+    };
+    // KeyGenerator::create_public_key: h_boot_seed [8], d_out [2][k][n]
+    void op_generate_public_key(Context &c, const SecretKey &sk, int boot_prng, int ct_prng, const u64 *h_boot_seed, u64 *d_out, cudaStream_t st);
+    // KeyGenerator::create_relin_keys (galois_elt = 0) / the key of one Galois element: h_boot_seeds [k-1][8] (one per digit),
+    // d_out [k-1][2][k][n].  Returns once the host seeds have been consumed (they may be wiped then).
+    void op_generate_kswitch_key(Context &c, SecretKey &sk, uint32_t galois_elt, int boot_prng, int ct_prng, const u64 *h_boot_seeds, u64 *d_out,
+                                 cudaStream_t st);
+    // Decryptor::compute_secret_key_array (sb_engine.cu): s^1 .. s^powers at the key level in sk.d_pow
+    void ensure_key_powers(Context &c, SecretKey &sk, size_t powers, cudaStream_t st);
     // Encryptor(public key)::encrypt_zero on the device (sb_prng.cu): seeds [B][8] on the host for PRNGs of type prng, out [B][2][L][n]
     void public_key_create(Context &c, const u64 *h_pk, PublicKey &out);
     void op_encrypt_zero_asymmetric(Context &c, const PublicKey &pk, size_t L, size_t B, const u64 *h_seeds, int prng, u64 *d_out, cudaStream_t st);

@@ -412,10 +412,11 @@ namespace sb
         // MODE 4  c_0 = -(tmp + e)
         // MODE 5  c_0 = s c_1                 (BFV without the seed: both polynomials are inverse-transformed afterwards)
         // MODE 6  c_0 = -(c_0 + e)
+        // MODE 7  MODE 1, plus on row j = digit of each digit's c_0: (q_{k-1} mod q_j) s'_j  (a key-switching key, L = k)
         template <int MODE>
         __global__ void __launch_bounds__(256) enc_kernel(u64 *__restrict__ out, u64 *__restrict__ tmp, const u64 *__restrict__ sk,
                                                           const unsigned char *__restrict__ boot, long long boot_bytes, const u64 *__restrict__ mult,
-                                                          const PrimeDev *__restrict__ primes, int logn, int L, long long total)
+                                                          KsFactor ks, const PrimeDev *__restrict__ primes, int logn, int L, long long total)
         {
             const long long e = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; // over B * L * n
             if (e >= total)
@@ -443,24 +444,32 @@ namespace sb
                 *c0 = neg_sum(tmp[e], noise, P.q);
             else if (MODE == 5)
                 *c0 = mulmod_barrett(sk[r], *c1, P);
-            else
+            else if (MODE == 6)
                 *c0 = neg_sum(*c0, noise, P.q);
+            else
+            {
+                u64 v = neg_sum(mulmod_barrett(sk[r], *c1, P), tmp[e], P.q);
+                if (j == ks.digit0 + b)
+                {
+                    // keygenerator.cpp:349-356: barrett_reduce_64(q_{k-1}, q_j) s'_j, added mod q_j
+                    const u64 factor = barrett64(primes[L - 1].q, P.q, P.ratio_hi);
+                    const u64 s_new = ks.new_key[(static_cast<long long>(j) << logn) + (ks.perm ? ks.perm[i] : i)];
+                    v = csub(v + mulmod_barrett(factor, s_new, P), P.q);
+                }
+                *c0 = v;
+            }
         }
     } // namespace
 
-    // h_boot_seeds [B][8]: the seeds of the bootstrap PRNGs (one fresh seed per ciphertext); d_out [B][2][L][n];
-    // h_public_seeds: nullptr or [B][8], receives the seed c_1 of each ciphertext expands from (what Serializable<Ciphertext> stores)
-    void op_encrypt_zero_symmetric(Context &c, const SecretKey &sk, size_t L, size_t B, const u64 *h_boot_seeds, int boot_prng, int ct_prng,
-                                   bool save_seed, u64 *d_out, u64 *h_public_seeds, cudaStream_t st)
+    // util::encrypt_zero_symmetric (util/rlwe.cpp:264-408) at the level with L primes (1..k, the key level included), checks done by
+    // the callers.  h_boot_seeds [B][8]: the seeds of the bootstrap PRNGs (one per ciphertext); d_out [B][2][L][n]; is_ntt_form: the
+    // reference's argument of that name (true: NTT form for every scheme, as KeyGenerator asks; false: BFV's coefficient form);
+    // h_public_seeds: nullptr or [B][8], receives the seed c_1 of each ciphertext expands from (what Serializable<Ciphertext> stores);
+    // ks: nullptr, or the factor term that turns ciphertext b into digit ks->digit0 + b of a key-switching key (L = k, NTT form)
+    static void encrypt_zero_symmetric_impl(Context &c, const SecretKey &sk, size_t L, size_t B, const u64 *h_boot_seeds, int boot_prng,
+                                            int ct_prng, bool is_ntt_form, bool save_seed, const KsFactor *ks, u64 *d_out, u64 *h_public_seeds,
+                                            cudaStream_t st)
     {
-        check_prng_type(boot_prng);
-        check_prng_type(ct_prng);
-        if (!B)
-            return;
-        if (L < 1 || L > c.k || (c.k > 1 && L == c.k))
-            throw std::invalid_argument("parms_id is not valid for encryption parameters");
-        if (!sk.d_pow || sk.ctx != &c)
-            throw std::invalid_argument("secret key is not valid for encryption parameters");
         const long long poly = static_cast<long long>(L) * c.n, total = poly * static_cast<long long>(B);
         // bootstrap stream: whole PRNG buffers covering 64 + 6 n bytes
         const long long boot_words = ((64 + 6 * static_cast<long long>(c.n) + kXof - 1) / kXof) * kWordsPerBuffer, boot_bytes = boot_words * 8;
@@ -491,16 +500,24 @@ namespace sb
         const unsigned char *boot = reinterpret_cast<const unsigned char *>(Wb);
         const u64 *s = sk.d_pow; // s^1, [k][n] at the key level: the first L rows are the level's primes
         const int logn = c.logn, Li = static_cast<int>(L);
-#define SB_ENC(MODE, name)                                                                                        \
-    c.stats.begin(name, 0, 24.0 * total, st);                                                                      \
-    enc_kernel<MODE><<<grid, 256, 0, st>>>(d_out, tmp, s, boot, boot_bytes, mult, c.d_primes, logn, Li, total);    \
-    c.stats.end(st);                                                                                               \
+        const KsFactor f = ks ? *ks : KsFactor{};
+#define SB_ENC(MODE, name)                                                                                           \
+    c.stats.begin(name, 0, 24.0 * total, st);                                                                         \
+    enc_kernel<MODE><<<grid, 256, 0, st>>>(d_out, tmp, s, boot, boot_bytes, mult, f, c.d_primes, logn, Li, total);    \
+    c.stats.end(st);                                                                                                  \
     cuda_check(cudaGetLastError(), name);
-        if (c.scheme != 1 /* CKKS, BGV */)
+        if (is_ntt_form)
         {
             SB_ENC(0, "enc_noise")
             op_ntt(c, false, L, 1, B, tmp, st);
-            SB_ENC(1, "enc_combine")
+            if (ks)
+            {
+                SB_ENC(7, "enc_combine:kswitch")
+            }
+            else
+            {
+                SB_ENC(1, "enc_combine")
+            }
         }
         else if (save_seed)
         {
@@ -520,6 +537,72 @@ namespace sb
         c.wipe_aux(st); // bootstrap stream and noise: with c_0 they give c_1 s (util/rlwe.cpp:292: clear-on-destruction pool)
         if (h_public_seeds)
             cuda_check(cudaStreamSynchronize(st), "synchronize");
+    }
+
+    // h_boot_seeds [B][8]: the seeds of the bootstrap PRNGs (one fresh seed per ciphertext); d_out [B][2][L][n];
+    // h_public_seeds: nullptr or [B][8], receives the seed c_1 of each ciphertext expands from (what Serializable<Ciphertext> stores)
+    void op_encrypt_zero_symmetric(Context &c, const SecretKey &sk, size_t L, size_t B, const u64 *h_boot_seeds, int boot_prng, int ct_prng,
+                                   bool save_seed, u64 *d_out, u64 *h_public_seeds, cudaStream_t st)
+    {
+        check_prng_type(boot_prng);
+        check_prng_type(ct_prng);
+        if (!B)
+            return;
+        if (L < 1 || L > c.k || (c.k > 1 && L == c.k))
+            throw std::invalid_argument("parms_id is not valid for encryption parameters");
+        if (!sk.d_pow || sk.ctx != &c)
+            throw std::invalid_argument("secret key is not valid for encryption parameters");
+        encrypt_zero_symmetric_impl(c, sk, L, B, h_boot_seeds, boot_prng, ct_prng, c.scheme != 1 /* CKKS, BGV */, save_seed, nullptr, d_out,
+                                    h_public_seeds, st);
+    }
+
+    // ------------------------------------------------------------------------------------------------------------------------------
+    // KeyGenerator (keygenerator.cpp:96-120, 327-360): the public key and every key-switching key are key-level symmetric encryptions
+    // of zero in NTT form (is_ntt_form = true for every scheme, BFV included), drawn from one bootstrap PRNG each.
+    static void check_key(const Context &c, const SecretKey &sk, int boot_prng, int ct_prng)
+    {
+        check_prng_type(boot_prng);
+        check_prng_type(ct_prng);
+        if (!sk.d_pow || sk.ctx != &c)
+            throw std::invalid_argument("secret key is not valid for encryption parameters");
+    }
+
+    void op_generate_public_key(Context &c, const SecretKey &sk, int boot_prng, int ct_prng, const u64 *h_boot_seed, u64 *d_out, cudaStream_t st)
+    {
+        check_key(c, sk, boot_prng, ct_prng);
+        encrypt_zero_symmetric_impl(c, sk, c.k, 1, h_boot_seed, boot_prng, ct_prng, true, false, nullptr, d_out, nullptr, st);
+    }
+
+    // generate_one_kswitch_key: digit j = encrypt_zero_symmetric at the key level + (q_{k-1} mod q_j) s'_j on row j of c_0, with
+    // s' = s^2 (relinearization, the key array of compute_secret_key_array) or s seen through the NTT-form Galois permutation
+    // (apply_galois_ntt, galois.cpp:148-160), which the combine kernel reads in place: the permuted key is never stored.  The digits
+    // are cut into chunks by the scratch budget; each chunk is one batch of encryptions and wipes its noise and streams.
+    void op_generate_kswitch_key(Context &c, SecretKey &sk, uint32_t galois_elt, int boot_prng, int ct_prng, const u64 *h_boot_seeds, u64 *d_out,
+                                 cudaStream_t st)
+    {
+        if (galois_elt && (!(galois_elt & 1) || galois_elt >= 2 * c.n))
+            throw std::invalid_argument("Galois element is not valid"); // keygenerator.cpp:195-199
+        if (c.k < 2)
+            throw std::logic_error("keyswitching is not supported by the context"); // keygenerator.cpp:329-332
+        check_key(c, sk, boot_prng, ct_prng);
+        KsFactor f{};
+        if (galois_elt)
+            f.new_key = sk.d_pow, f.perm = c.galois_table(galois_elt);
+        else
+        {
+            ensure_key_powers(c, sk, 2, st);
+            f.new_key = sk.d_pow + c.k * c.n;
+        }
+        const size_t digits = c.k - 1, poly = c.k * c.n;
+        // per digit: the noise / product polynomial (aux arena) and the c_1 stream (scratch arena, expand_impl), plus the bootstrap stream
+        const size_t per = 2 * poly * sizeof(u64) + 6 * c.n + kXof + 64;
+        const size_t chunk = std::max<size_t>(1, std::min(digits, c.scratch_budget / per));
+        for (size_t d0 = 0; d0 < digits; d0 += chunk)
+        {
+            f.digit0 = static_cast<long long>(d0);
+            encrypt_zero_symmetric_impl(c, sk, c.k, std::min(chunk, digits - d0), h_boot_seeds + d0 * 8, boot_prng, ct_prng, true, false, &f,
+                                        d_out + d0 * 2 * poly, nullptr, st);
+        }
     }
 
     // ------------------------------------------------------------------------------------------------------------------------------

@@ -1,0 +1,119 @@
+#!/usr/bin/env python
+"""tools/keygen_bench.py -- key generation on the device against the reference's KeyGenerator, from the same secret key.
+
+    python tools/keygen_bench.py [--reps 3] [--ref-galois N]
+
+Shapes: BFV n = 16384, 8 primes of 54 bits (bench.py's rotation sweep) and CKKS n = 65536, 32 primes of 55 bits (the headline).
+Device (sb200_kswitch_key_generate), after a warm-up that makes every key of the shape once:
+  * the relinearization key into a host buffer (best of --reps);
+  * the default Galois set (GaloisTool::get_elts_all) into host buffers: one reused buffer, the keys made one after another;
+  * the same set into device handles (the handle also holds the integer key-switching path's copy of the key); each handle is
+    freed after it is timed, since the n = 65536 set does not fit in 80 GB at once.
+Every device time is a host clock around calls that end in a device synchronise.  Reference: seal::KeyGenerator
+(oracle/_ref/libsealref_keygen.so, one thread) for the relinearization key and the first --ref-galois elements of the default set
+(default: all of them), per key.  Prints the card's name and power limit, one line per measurement and one JSON line."""
+import argparse
+import ctypes as C
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+
+SHAPES = [("BFV", 1, 16384, [54] * 8), ("CKKS", 2, 65536, [55] * 32)]
+
+
+def card():
+    try:
+        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                              capture_output=True, text=True, check=True).stdout.strip().splitlines()[0]
+    except (OSError, subprocess.CalledProcessError, IndexError):
+        return "unknown"
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--ref-galois", type=int, default=None, help="reference Galois keys to time per shape (default: the whole set)")
+    args = ap.parse_args()
+
+    import torch
+
+    import keygen_ref as K
+    import refseal as R
+    import seal_b200 as S
+
+    if not torch.cuda.is_available():
+        raise SystemExit("no CUDA device: the device times need an H100")
+    if not K.ref_available():
+        raise SystemExit("oracle/_ref/libsealref_keygen.so is missing (oracle/keygen.mk)")
+    print(f"card: {card()}", flush=True)
+    lib, results = S.lib(), []
+    for name, scheme, n, bits in SHAPES:
+        mods = R.coeff_modulus_create(n, bits)
+        t = R.plain_modulus_batching(n, 20) if scheme == S.BFV else 0
+        k = len(mods)
+        ref = K.RefKeygen(scheme, n, mods, t)
+        elts = ref.galois_elts_all()
+        ctx = S.Context(scheme, n, mods, t)
+        skd = ctx.load_secret_key(ref.secret_key())
+        buf = np.zeros((k - 1, 2, k, n), dtype=np.uint64)
+        seeds = ref.boot_seeds(k - 1)
+
+        def to_host(elt):
+            S._check(lib.sb200_kswitch_key_generate(ctx.h, skd.h, elt, 1, 1, S._hp(seeds), S._hp(buf), None))
+
+        def to_handle(elt):
+            h = C.c_void_p()
+            S._check(lib.sb200_kswitch_key_generate(ctx.h, skd.h, elt, 1, 1, S._hp(seeds), None, C.byref(h)))
+            return h
+
+        def timed(fn):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            out = fn()
+            torch.cuda.synchronize()
+            return time.perf_counter() - t0, out
+
+        for elt in [0] + elts:  # warm-up: every key of the shape once, both outputs (also builds the Galois tables)
+            to_host(elt)
+            lib.sb200_kswitch_key_destroy(to_handle(elt))
+        relin = min(timed(lambda: to_host(0))[0] for _ in range(args.reps))
+        gal_host = sum(timed(lambda: to_host(e))[0] for e in elts)
+        gal_dev = 0.0
+        for e in elts:
+            dt, h = timed(lambda: to_handle(e))
+            gal_dev += dt
+            lib.sb200_kswitch_key_destroy(h)
+        ref_elts = elts if args.ref_galois is None else elts[:args.ref_galois]
+        t0 = time.perf_counter()
+        ref.kswitch_key(0, keep=False)
+        ref_relin = time.perf_counter() - t0
+        t0 = time.perf_counter()
+        for e in ref_elts:
+            ref.kswitch_key(e, keep=False)
+        ref_gal = time.perf_counter() - t0
+        gb = (k - 1) * 2 * k * n * 8 / 1e9
+        r = {"shape": f"{name} n={n} k={k}", "galois_keys": len(elts), "key_gb": round(gb, 3),
+             "device_relin_host_ms": round(relin * 1e3, 2), "device_galois_set_host_s": round(gal_host, 3),
+             "device_galois_set_handles_s": round(gal_dev, 3), "device_galois_host_ms_per_key": round(gal_host / len(elts) * 1e3, 2),
+             "ref_relin_ms": round(ref_relin * 1e3, 1), "ref_galois_keys_timed": len(ref_elts),
+             "ref_galois_ms_per_key": round(ref_gal / max(len(ref_elts), 1) * 1e3, 1),
+             "speedup_relin_host": round(ref_relin / relin, 1),
+             "speedup_galois_host_per_key": round(ref_gal / max(len(ref_elts), 1) / (gal_host / len(elts)), 1)}
+        print(f"{r['shape']}: relin key {r['device_relin_host_ms']} ms (device -> host) vs {r['ref_relin_ms']} ms (reference); "
+              f"{len(elts)} Galois keys {r['device_galois_set_host_s']} s (host) / {r['device_galois_set_handles_s']} s (handles) vs "
+              f"{r['ref_galois_ms_per_key']} ms per key (reference, {len(ref_elts)} keys)", flush=True)
+        results.append(r)
+        del ctx, skd, ref
+    print(json.dumps({"card": card(), "results": results}))
+
+
+if __name__ == "__main__":
+    main()
