@@ -65,7 +65,8 @@ int sb200_get_base_bsk(const sb200_context *ctx, size_t L, uint64_t *out, size_t
 uint32_t sb200_galois_elt_from_step(const sb200_context *ctx, int step);
 /* number of CUDA kernels launched through this context so far */
 unsigned long long sb200_launch_count(const sb200_context *ctx);
-/* device bytes currently held by the context (tables + scratch) */
+/* device bytes currently held by the context: its tables, including those built on first use (per-level decryption, plaintext
+ * and CRT constants, Galois permutations, encoder and BEHZ tables), plus the two scratch arenas */
 size_t sb200_device_bytes(const sb200_context *ctx);
 /* resource limits of a context (the reference's counterpart is the MemoryPoolHandle a caller passes to Evaluator members,
  * evaluator.h:219-252): how a batch is cut into device chunks.  Results never depend on them; the parity tests use them

@@ -22,32 +22,23 @@ struct sb200_context
 {
     std::unique_ptr<Context> c;
 };
+// the key's device memory is freed (the secret key's wiped first) by its members, on the context's device
 struct sb200_public_key
 {
     PublicKey k;
     ~sb200_public_key()
     {
-        if (k.d_key && k.ctx)
-        {
+        if (k.ctx)
             cudaSetDevice(k.ctx->device);
-            cudaFree(k.d_key);
-        }
     }
 };
 struct sb200_secret_key
 {
     SecretKey k;
-    // the reference keeps SecretKey data in a clear-on-destruction pool (secretkey.h:51-60): wipe before the memory goes back
-    // to the allocator
     ~sb200_secret_key()
     {
-        if (k.d_pow && k.ctx)
-        {
+        if (k.ctx)
             cudaSetDevice(k.ctx->device);
-            cudaMemset(k.d_pow, 0, k.powers * k.ctx->k * k.ctx->n * sizeof(u64));
-            cudaDeviceSynchronize();
-        }
-        cudaFree(k.d_pow);
     }
 };
 struct sb200_kswitch_key
@@ -57,8 +48,6 @@ struct sb200_kswitch_key
     {
         if (k.ctx)
             cudaSetDevice(k.ctx->device);
-        cudaFree(k.d_key);
-        cudaFree(k.d_key32);
     }
 };
 
@@ -209,7 +198,7 @@ unsigned long long sb200_launch_count(const sb200_context *ctx)
 
 size_t sb200_device_bytes(const sb200_context *ctx)
 {
-    return ctx ? ctx->c->table_bytes + ctx->c->scratch_bytes + ctx->c->aux_bytes : 0;
+    return ctx ? ctx->c->table_bytes + ctx->c->scratch.bytes() + ctx->c->aux_buf.bytes() : 0;
 }
 
 int sb200_context_set_limit(sb200_context *ctx, int which, size_t value)
@@ -367,26 +356,15 @@ namespace
         for (auto &x : th)
             x.join();
     }
-    void ensure_lane(Context &c, IoArena::Lane &ln, size_t bytes)
+    void ensure_lane(IoArena::Lane &ln, size_t bytes)
     {
         if (!ln.st)
-        {
-            cuda_check(cudaStreamCreateWithFlags(&ln.st, cudaStreamNonBlocking), "cudaStreamCreate");
-            cuda_check(cudaEventCreateWithFlags(&ln.order, cudaEventDisableTiming), "cudaEventCreate");
-            for (int i = 0; i < 2; i++)
-                cuda_check(cudaEventCreateWithFlags(&ln.ev[i], cudaEventDisableTiming), "cudaEventCreate");
-        }
-        if (ln.cap >= bytes)
-            return;
-        for (int i = 0; i < 2; i++)
-        {
-            cudaFreeHost(ln.pin[i]);
-            ln.pin[i] = nullptr;
-        }
-        ln.cap = 0;
-        for (int i = 0; i < 2; i++)
-            cuda_check(cudaHostAlloc(&ln.pin[i], bytes, cudaHostAllocDefault), "cudaHostAlloc(staging)");
-        ln.cap = bytes;
+            ln.st = make_stream();
+        for (auto *e : { &ln.order, &ln.ev[0], &ln.ev[1] })
+            if (!*e)
+                *e = make_event();
+        for (auto &p : ln.pin)
+            p.grow(bytes);
     }
     // The copies run on the lane's own non-blocking stream: they overlap kernels of other batches.  Ordering with the caller's
     // work: a download first waits for everything the legacy default stream has been given so far (the batch operations of the
@@ -399,12 +377,12 @@ namespace
         std::lock_guard<std::mutex> lock(ln.mu);
         cuda_check(cudaSetDevice(c.device), "cudaSetDevice");
         const size_t per = std::max<size_t>(1, (size_t(128) << 20) / row_bytes), stage_bytes = std::min(per, count) * row_bytes;
-        ensure_lane(c, ln, stage_bytes);
-        cudaStream_t st = ln.st;
+        ensure_lane(ln, stage_bytes);
+        cudaStream_t st = ln.st.get();
         if (!upload)
         {
-            cuda_check(cudaEventRecord(ln.order, nullptr), "record");
-            cuda_check(cudaStreamWaitEvent(st, ln.order, 0), "wait");
+            cuda_check(cudaEventRecord(ln.order.get(), nullptr), "record");
+            cuda_check(cudaStreamWaitEvent(st, ln.order.get(), 0), "wait");
         }
         uint8_t *d = reinterpret_cast<uint8_t *>(dev);
         size_t i = 0, pend[2] = { 0, 0 }, pend_n[2] = { 0, 0 };
@@ -413,10 +391,10 @@ namespace
         {
             const size_t r1 = std::min(count, r0 + per);
             const int slot = static_cast<int>(i & 1);
-            uint8_t *stage = static_cast<uint8_t *>(ln.pin[slot]);
+            uint8_t *stage = ln.pin[slot].get();
             if (used[slot])
             {
-                cuda_check(cudaEventSynchronize(ln.ev[slot]), "cudaEventSynchronize");
+                cuda_check(cudaEventSynchronize(ln.ev[slot].get()), "cudaEventSynchronize");
                 if (!upload)
                     rows_copy(false, stage, rows, row_bytes, pend[slot], pend[slot] + pend_n[slot]);
             }
@@ -427,16 +405,16 @@ namespace
             }
             else
                 cuda_check(cudaMemcpyAsync(stage, d + r0 * row_bytes, (r1 - r0) * row_bytes, cudaMemcpyDeviceToHost, st), "D2H");
-            cuda_check(cudaEventRecord(ln.ev[slot], st), "record");
+            cuda_check(cudaEventRecord(ln.ev[slot].get(), st), "record");
             used[slot] = true, pend[slot] = r0, pend_n[slot] = r1 - r0;
         }
         // drain in submission order
         for (size_t j = (i >= 2 ? i - 2 : 0); j < i; j++)
         {
             const int slot = static_cast<int>(j & 1);
-            cuda_check(cudaEventSynchronize(ln.ev[slot]), "cudaEventSynchronize");
+            cuda_check(cudaEventSynchronize(ln.ev[slot].get()), "cudaEventSynchronize");
             if (!upload)
-                rows_copy(false, static_cast<uint8_t *>(ln.pin[slot]), rows, row_bytes, pend[slot], pend[slot] + pend_n[slot]);
+                rows_copy(false, ln.pin[slot].get(), rows, row_bytes, pend[slot], pend[slot] + pend_n[slot]);
         }
     }
 } // namespace
@@ -654,7 +632,7 @@ int sb200_profile_read_work32(sb200_context *ctx, size_t index, char *name, size
 static std::unique_ptr<sb200_kswitch_key> kswitch_key_alloc(Context &c, size_t digits)
 {
     auto h = std::make_unique<sb200_kswitch_key>();
-    cuda_check(cudaMalloc(reinterpret_cast<void **>(&h->k.d_key), digits * 2 * c.k * c.n * sizeof(u64)), "cudaMalloc(key)");
+    h->k.d_key = DevBuf<u64>(digits * 2 * c.k * c.n);
     h->k.ctx = &c;
     h->k.digits = digits;
     return h;
@@ -662,7 +640,7 @@ static std::unique_ptr<sb200_kswitch_key> kswitch_key_alloc(Context &c, size_t d
 
 static bool kswitch_key_finish(Context &c, KSwitchKey &k)
 {
-    if (!op_residues_in_range(c, c.k, k.digits * 2 * c.k, k.d_key, nullptr))
+    if (!op_residues_in_range(c, c.k, k.digits * 2 * c.k, k.d_key.get(), nullptr))
         return false;
     ksint_prepare_key(c, k, nullptr);
     return true;
@@ -683,7 +661,7 @@ int sb200_kswitch_key_create(sb200_context *ctx, const uint64_t *h_key, size_t d
     std::lock_guard<std::mutex> lock(c.mu);
     cuda_check(cudaSetDevice(c.device), "cudaSetDevice");
     auto h = kswitch_key_alloc(c, digits);
-    cuda_check(cudaMemcpy(h->k.d_key, h_key, digits * 2 * c.k * c.n * sizeof(u64), cudaMemcpyHostToDevice), "upload key");
+    cuda_check(cudaMemcpy(h->k.d_key.get(), h_key, digits * 2 * c.k * c.n * sizeof(u64), cudaMemcpyHostToDevice), "upload key");
     if (!kswitch_key_finish(c, h->k))
         throw std::invalid_argument("kswitch key data is not valid for encryption parameters");
     *out = h.release();
@@ -724,7 +702,7 @@ int sb200_kswitch_key_load(sb200_context *ctx, const uint8_t *stream, size_t len
     std::vector<long long> seed_dst;
     for (size_t j = 0; j < digits; j++)
     {
-        cuda_check(cudaMemcpy(reinterpret_cast<uint8_t *>(h->k.d_key) + j * row, stream + e.offsets[j], e.seeded[j] ? row / 2 : row,
+        cuda_check(cudaMemcpy(reinterpret_cast<uint8_t *>(h->k.d_key.get()) + j * row, stream + e.offsets[j], e.seeded[j] ? row / 2 : row,
                               cudaMemcpyHostToDevice),
                    "upload key");
         if (e.seeded[j])
@@ -737,7 +715,7 @@ int sb200_kswitch_key_load(sb200_context *ctx, const uint8_t *stream, size_t len
         }
     }
     if (!seed_dst.empty())
-        op_expand_seeded(c, c.k, seed_dst.size(), seeds.data(), types.data(), seed_dst.data(), h->k.d_key, nullptr);
+        op_expand_seeded(c, c.k, seed_dst.size(), seeds.data(), types.data(), seed_dst.data(), h->k.d_key.get(), nullptr);
     if (!kswitch_key_finish(c, h->k)) // KSwitchKeys::load ends in is_valid_for (kswitchkeys.cpp:149-153)
         throw std::logic_error("KSwitchKeys data is invalid");
     *out = h.release();
@@ -769,14 +747,14 @@ namespace
         cudaStream_t st;
         StreamOrder(Context &ctx, cudaStream_t stream) : c(ctx), st(stream)
         {
+            if (!c.order_event)
+                c.order_event = make_event();
             if (c.order_valid && c.order_stream != st)
-                cuda_check(cudaStreamWaitEvent(st, c.order_event, 0), "cudaStreamWaitEvent(order)");
+                cuda_check(cudaStreamWaitEvent(st, c.order_event.get(), 0), "cudaStreamWaitEvent(order)");
         }
         ~StreamOrder()
         {
-            if (!c.order_event && cudaEventCreateWithFlags(&c.order_event, cudaEventDisableTiming) != cudaSuccess)
-                return;
-            if (cudaEventRecord(c.order_event, st) == cudaSuccess)
+            if (cudaEventRecord(c.order_event.get(), st) == cudaSuccess)
                 c.order_stream = st, c.order_valid = true;
         }
     };
@@ -829,33 +807,22 @@ namespace
         explicit HostPipe(Context &ctx) : c(ctx)
         {
             IoArena &io = c.io;
-            if (!io.ready)
-            {
-                for (auto *s : { &io.s_in, &io.s_comp, &io.s_out })
-                    cuda_check(cudaStreamCreateWithFlags(s, cudaStreamNonBlocking), "cudaStreamCreate");
-                for (int i = 0; i < 2; i++)
-                    for (auto *e : { &io.ev_in[i], &io.ev_comp[i], &io.ev_out[i] })
-                        cuda_check(cudaEventCreateWithFlags(e, cudaEventDisableTiming), "cudaEventCreate");
-                io.ready = true;
-            }
-            s_in = io.s_in, s_comp = io.s_comp, s_out = io.s_out;
+            for (auto *s : { &io.s_in, &io.s_comp, &io.s_out })
+                if (!*s)
+                    *s = make_stream();
             for (int i = 0; i < 2; i++)
-                ev_in[i] = io.ev_in[i], ev_comp[i] = io.ev_comp[i], ev_out[i] = io.ev_out[i];
+                for (auto *e : { &io.ev_in[i], &io.ev_comp[i], &io.ev_out[i] })
+                    if (!*e)
+                        *e = make_event();
+            s_in = io.s_in.get(), s_comp = io.s_comp.get(), s_out = io.s_out.get();
+            for (int i = 0; i < 2; i++)
+                ev_in[i] = io.ev_in[i].get(), ev_comp[i] = io.ev_comp[i].get(), ev_out[i] = io.ev_out[i].get();
         }
         u64 *buffer(int slot, int which, size_t words)
         {
-            IoArena &io = c.io;
-            size_t &cap = io.cap[slot][which];
-            if (words > cap)
-            {
-                cuda_check(cudaDeviceSynchronize(), "sync before io growth");
-                cudaFree(io.buf[slot][which]);
-                io.buf[slot][which] = nullptr;
-                cap = 0;
-                cuda_check(cudaMalloc(reinterpret_cast<void **>(&io.buf[slot][which]), words * sizeof(u64)), "cudaMalloc(io)");
-                cap = words;
-            }
-            return io.buf[slot][which];
+            DevBuf<u64> &b = c.io.buf[slot][which];
+            b.grow(words);
+            return b.get();
         }
         template <class Op>
         void run(size_t batch, const Layout &w, const u64 *ha, const u64 *hb, u64 *ho, const Op &op)
@@ -1215,7 +1182,7 @@ namespace
         op.check(c, batch);
         HostPipe(c).run(batch, op.layout(c), static_cast<const u64 *>(a), static_cast<const u64 *>(b), static_cast<u64 *>(out), op);
         if (then)
-            then(c, c.io.s_comp);
+            then(c, c.io.s_comp.get());
         return SB200_OK;
         SB_CATCH
     }
@@ -1745,14 +1712,14 @@ int sb200_public_key_generate(sb200_context *ctx, sb200_secret_key *key, int boo
         fresh = std::make_unique<FreshSeeds>(1);
         h_bootstrap_seed = reinterpret_cast<const uint64_t *>(fresh->words.data());
     }
-    const size_t bytes = 2 * c.k * c.n * sizeof(u64);
     auto h = std::make_unique<sb200_public_key>();
-    cuda_check(cudaMalloc(reinterpret_cast<void **>(&h->k.d_key), bytes), "cudaMalloc(public key)");
+    h->k.d_key = DevBuf<u64>(2 * c.k * c.n);
     h->k.ctx = &c;
-    op_generate_public_key(c, key->k, bootstrap_prng, ciphertext_prng, (const u64 *)h_bootstrap_seed, h->k.d_key, nullptr);
+    const size_t bytes = h->k.d_key.bytes();
+    op_generate_public_key(c, key->k, bootstrap_prng, ciphertext_prng, (const u64 *)h_bootstrap_seed, h->k.d_key.get(), nullptr);
     cuda_check(cudaStreamSynchronize(nullptr), "synchronize");
     if (h_public_key)
-        cuda_check(cudaMemcpy(h_public_key, h->k.d_key, bytes, cudaMemcpyDeviceToHost), "download public key");
+        cuda_check(cudaMemcpy(h_public_key, h->k.d_key.get(), bytes, cudaMemcpyDeviceToHost), "download public key");
     if (out)
         *out = h.release();
     return SB200_OK;
@@ -1778,10 +1745,10 @@ int sb200_kswitch_key_generate(sb200_context *ctx, sb200_secret_key *key, uint32
         h_bootstrap_seeds = reinterpret_cast<const uint64_t *>(fresh->words.data());
     }
     auto h = kswitch_key_alloc(c, digits);
-    op_generate_kswitch_key(c, key->k, galois_elt, bootstrap_prng, ciphertext_prng, (const u64 *)h_bootstrap_seeds, h->k.d_key, nullptr);
+    op_generate_kswitch_key(c, key->k, galois_elt, bootstrap_prng, ciphertext_prng, (const u64 *)h_bootstrap_seeds, h->k.d_key.get(), nullptr);
     cuda_check(cudaStreamSynchronize(nullptr), "synchronize");
     if (h_key)
-        cuda_check(cudaMemcpy(h_key, h->k.d_key, digits * 2 * c.k * c.n * sizeof(u64), cudaMemcpyDeviceToHost), "download key");
+        cuda_check(cudaMemcpy(h_key, h->k.d_key.get(), digits * 2 * c.k * c.n * sizeof(u64), cudaMemcpyDeviceToHost), "download key");
     if (out)
     {
         if (!kswitch_key_finish(c, h->k))
@@ -1804,7 +1771,7 @@ namespace
         c.wipe_scratch(st);
         for (int slot = 0; slot < 2; slot++) // and the output staging
             if (c.io.buf[slot][2])
-                cuda_check(cudaMemsetAsync(c.io.buf[slot][2], 0, c.io.cap[slot][2] * sizeof(u64), st), "wipe staging");
+                cuda_check(cudaMemsetAsync(c.io.buf[slot][2].get(), 0, c.io.buf[slot][2].bytes(), st), "wipe staging");
         cuda_check(cudaStreamSynchronize(st), "synchronize");
     }
 } // namespace

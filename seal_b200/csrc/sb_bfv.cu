@@ -20,39 +20,19 @@ namespace sb
         sbh::BehzLevel host;
         int L = 0, nB = 0, nS = 0;
         // device arrays
-        int *pids_bsk = nullptr;       // prime ids of Bsk                         [nS]
-        Tw *lift_c = nullptr;          // m_tilde * (q/q_i)^-1 mod q_i             [L]
-        Tw *inv_punc_q = nullptr;      //                                          [L]
-        u64 *q_to_bsk = nullptr;       //                                          [nS][L]
-        uint32_t *q_to_mt = nullptr;   // (q/q_i) mod 2^32                         [L]
-        Tw *prod_q_mod_bsk = nullptr, *inv_mt_mod_bsk = nullptr, *inv_q_mod_bsk = nullptr, *t_mod_bsk = nullptr; // [nS]
-        Tw *t_mod_q = nullptr, *prod_b_mod_q = nullptr, *neg_prod_b_mod_q = nullptr;                              // [L]
-        Tw *inv_punc_b = nullptr;      //                                          [nB]
-        u64 *b_to_q = nullptr;         //                                          [L][nB]
-        u64 *b_to_msk = nullptr;       //                                          [nB]
+        DevBuf<int> pids_bsk;          // prime ids of Bsk                         [nS]
+        DevBuf<Tw> lift_c;             // m_tilde * (q/q_i)^-1 mod q_i             [L]
+        DevBuf<Tw> inv_punc_q;         //                                          [L]
+        DevBuf<u64> q_to_bsk;          //                                          [nS][L]
+        DevBuf<uint32_t> q_to_mt;      // (q/q_i) mod 2^32                         [L]
+        DevBuf<Tw> prod_q_mod_bsk, inv_mt_mod_bsk, inv_q_mod_bsk, t_mod_bsk; // [nS]
+        DevBuf<Tw> t_mod_q, prod_b_mod_q, neg_prod_b_mod_q;                  // [L]
+        DevBuf<Tw> inv_punc_b;         //                                          [nB]
+        DevBuf<u64> b_to_q;            //                                          [L][nB]
+        DevBuf<u64> b_to_msk;          //                                          [nB]
         Tw inv_b_mod_msk{};
         uint32_t neg_inv_q_mod_mt = 0;
-        std::vector<void *> allocs;
-        ~BehzDev()
-        {
-            for (auto p : allocs)
-                cudaFree(p);
-        }
     };
-
-    template <class T, class S>
-    static T *upload(BehzDev &d, const std::vector<S> &h, Context &c)
-    {
-        static_assert(sizeof(T) == sizeof(S), "layout");
-        T *p = nullptr;
-        if (h.empty())
-            return p;
-        cuda_check(cudaMalloc(reinterpret_cast<void **>(&p), h.size() * sizeof(S)), "cudaMalloc(behz)");
-        cuda_check(cudaMemcpy(p, h.data(), h.size() * sizeof(S), cudaMemcpyHostToDevice), "upload behz");
-        d.allocs.push_back(p);
-        c.table_bytes += h.size() * sizeof(S);
-        return p;
-    }
 
     static BehzDev &behz_dev(Context &c, size_t L)
     {
@@ -77,7 +57,7 @@ namespace sb
             pids.push_back(static_cast<int>(c.k + 2 + i));
         }
         pids.push_back(static_cast<int>(c.k + 0));
-        d->pids_bsk = upload<int>(*d, pids, c);
+        d->pids_bsk = upload<int>(c, pids);
         std::vector<sbh::TwPair> lift;
         std::vector<uint32_t> qmt;
         for (size_t i = 0; i < L; i++)
@@ -86,20 +66,20 @@ namespace sb
             lift.push_back(sbh::TwPair{ v, sbh::shoup(v, c.q[i]) });
             qmt.push_back(static_cast<uint32_t>(h.q_to_mtilde[i]));
         }
-        d->lift_c = upload<Tw>(*d, lift, c);
-        d->inv_punc_q = upload<Tw>(*d, h.inv_punc_q, c);
-        d->q_to_bsk = upload<u64>(*d, h.q_to_Bsk, c);
-        d->q_to_mt = upload<uint32_t>(*d, qmt, c);
-        d->prod_q_mod_bsk = upload<Tw>(*d, h.prod_q_mod_Bsk, c);
-        d->inv_mt_mod_bsk = upload<Tw>(*d, h.inv_mtilde_mod_Bsk, c);
-        d->inv_q_mod_bsk = upload<Tw>(*d, h.inv_q_mod_Bsk, c);
-        d->t_mod_bsk = upload<Tw>(*d, h.t_mod_Bsk, c);
-        d->t_mod_q = upload<Tw>(*d, h.t_mod_q, c);
-        d->prod_b_mod_q = upload<Tw>(*d, h.prod_B_mod_q, c);
-        d->neg_prod_b_mod_q = upload<Tw>(*d, h.neg_prod_B_mod_q, c);
-        d->inv_punc_b = upload<Tw>(*d, h.inv_punc_B, c);
-        d->b_to_q = upload<u64>(*d, h.B_to_q, c);
-        d->b_to_msk = upload<u64>(*d, h.B_to_msk, c);
+        d->lift_c = upload<Tw>(c, lift);
+        d->inv_punc_q = upload<Tw>(c, h.inv_punc_q);
+        d->q_to_bsk = upload<u64>(c, h.q_to_Bsk);
+        d->q_to_mt = upload<uint32_t>(c, qmt);
+        d->prod_q_mod_bsk = upload<Tw>(c, h.prod_q_mod_Bsk);
+        d->inv_mt_mod_bsk = upload<Tw>(c, h.inv_mtilde_mod_Bsk);
+        d->inv_q_mod_bsk = upload<Tw>(c, h.inv_q_mod_Bsk);
+        d->t_mod_bsk = upload<Tw>(c, h.t_mod_Bsk);
+        d->t_mod_q = upload<Tw>(c, h.t_mod_q);
+        d->prod_b_mod_q = upload<Tw>(c, h.prod_B_mod_q);
+        d->neg_prod_b_mod_q = upload<Tw>(c, h.neg_prod_B_mod_q);
+        d->inv_punc_b = upload<Tw>(c, h.inv_punc_B);
+        d->b_to_q = upload<u64>(c, h.B_to_q);
+        d->b_to_msk = upload<u64>(c, h.B_to_msk);
         d->inv_b_mod_msk.w = h.inv_B_mod_msk.w, d->inv_b_mod_msk.wq = h.inv_B_mod_msk.wq;
         d->neg_inv_q_mod_mt = static_cast<uint32_t>(h.neg_inv_q_mod_mtilde);
         c.behz[L] = d;
@@ -342,48 +322,48 @@ namespace sb
             const u64 *pa = a + b0 * s1 * L * c.n, *pb = b + b0 * s2 * L * c.n;
             {
                 OpBfvFwdQ op{ pa, pb, XQ, c.logn, Li, static_cast<int>(s1), static_cast<int>(s2) };
-                cuda_check(launch_ntt_fwd(op, static_cast<int>(B * nin * L), c.logn, c.d_primes, st, c.stats, "bfv_ntt_q", -1, c.fast_q), "bfv ntt q");
+                cuda_check(launch_ntt_fwd(op, static_cast<int>(B * nin * L), c.logn, c.d_primes.get(), st, c.stats, "bfv_ntt_q", -1, c.fast_q), "bfv ntt q");
             }
             {
                 dim3 grid((n + TH - 1) / TH, static_cast<unsigned>(nin), static_cast<unsigned>(B));
                 c.stats.begin("behz_lift", 0, 8.0 * n * B * nin * (L + nS), st);
-                behz_lift_kernel<<<grid, TH, smem_lift, st>>>(pa, pb, XS, c.d_primes, d.pids_bsk, d.lift_c, d.q_to_bsk, d.q_to_mt, d.prod_q_mod_bsk,
-                                                              d.inv_mt_mod_bsk, d.neg_inv_q_mod_mt, c.logn, Li, nS, static_cast<int>(s1),
+                behz_lift_kernel<<<grid, TH, smem_lift, st>>>(pa, pb, XS, c.d_primes.get(), d.pids_bsk.get(), d.lift_c.get(), d.q_to_bsk.get(), d.q_to_mt.get(), d.prod_q_mod_bsk.get(),
+                                                              d.inv_mt_mod_bsk.get(), d.neg_inv_q_mod_mt, c.logn, Li, nS, static_cast<int>(s1),
                                                               static_cast<int>(s2));
                 c.stats.end(st);
                 cuda_check(cudaGetLastError(), "behz_lift_kernel");
             }
-            op_ntt_rows(c, false, XS, B * nin * nS, nS, d.pids_bsk, st);
+            op_ntt_rows(c, false, XS, B * nin * nS, nS, d.pids_bsk.get(), st);
             if (s1 != 2 || s2 != 2)
             {
                 launch_tensor_general(c, XQ, static_cast<long long>(nin * L) * n, XQ + s1 * L * c.n, static_cast<long long>(nin * L) * n, DQ,
                                       nullptr, L, s1, s2, B, st);
                 launch_tensor_general(c, XS, static_cast<long long>(nin) * nS * n, XS + s1 * nS * c.n, static_cast<long long>(nin) * nS * n, DS,
-                                      d.pids_bsk, nS, s1, s2, B, st);
+                                      d.pids_bsk.get(), nS, s1, s2, B, st);
             }
             else
             {
                 long long tq = static_cast<long long>(B) * L * n, ts = static_cast<long long>(B) * nS * n;
                 c.stats.begin("behz_tensor", 0, 56.0 * tq, st);
-                behz_tensor_kernel<<<static_cast<unsigned>((tq + 255) / 256), 256, 0, st>>>(XQ, DQ, c.d_primes, nullptr, c.logn, Li, tq);
+                behz_tensor_kernel<<<static_cast<unsigned>((tq + 255) / 256), 256, 0, st>>>(XQ, DQ, c.d_primes.get(), nullptr, c.logn, Li, tq);
                 c.stats.end(st);
                 c.stats.begin("behz_tensor", 0, 56.0 * ts, st);
-                behz_tensor_kernel<<<static_cast<unsigned>((ts + 255) / 256), 256, 0, st>>>(XS, DS, c.d_primes, d.pids_bsk, c.logn, nS, ts);
+                behz_tensor_kernel<<<static_cast<unsigned>((ts + 255) / 256), 256, 0, st>>>(XS, DS, c.d_primes.get(), d.pids_bsk.get(), c.logn, nS, ts);
                 c.stats.end(st);
                 cuda_check(cudaGetLastError(), "behz_tensor_kernel");
             }
             {
-                OpBfvInvMulT oq{ DQ, d.t_mod_q, nullptr, c.logn, Li };
-                cuda_check(launch_ntt_inv(oq, static_cast<int>(B * nout * L), c.logn, c.d_primes, st, c.stats, "bfv_intt_q"), "bfv intt q");
-                OpBfvInvMulT os{ DS, d.t_mod_bsk, d.pids_bsk, c.logn, nS };
-                cuda_check(launch_ntt_inv(os, static_cast<int>(B * nout * nS), c.logn, c.d_primes, st, c.stats, "bfv_intt_bsk"), "bfv intt bsk");
+                OpBfvInvMulT oq{ DQ, d.t_mod_q.get(), nullptr, c.logn, Li };
+                cuda_check(launch_ntt_inv(oq, static_cast<int>(B * nout * L), c.logn, c.d_primes.get(), st, c.stats, "bfv_intt_q"), "bfv intt q");
+                OpBfvInvMulT os{ DS, d.t_mod_bsk.get(), d.pids_bsk.get(), c.logn, nS };
+                cuda_check(launch_ntt_inv(os, static_cast<int>(B * nout * nS), c.logn, c.d_primes.get(), st, c.stats, "bfv_intt_bsk"), "bfv intt bsk");
             }
             {
                 dim3 grid((n + TH - 1) / TH, static_cast<unsigned>(nout), static_cast<unsigned>(B));
                 c.stats.begin("behz_floor_sk", 0, 8.0 * n * B * nout * (2 * L + nS), st);
-                behz_floor_sk_kernel<<<grid, TH, smem_floor, st>>>(DQ, DS, out3 + b0 * nout * L * c.n, c.d_primes, d.pids_bsk, d.inv_punc_q, d.q_to_bsk,
-                                                                  d.inv_q_mod_bsk, d.inv_punc_b, d.b_to_q, d.b_to_msk, d.inv_b_mod_msk,
-                                                                  d.prod_b_mod_q, d.neg_prod_b_mod_q, c.logn, Li, nB, nS);
+                behz_floor_sk_kernel<<<grid, TH, smem_floor, st>>>(DQ, DS, out3 + b0 * nout * L * c.n, c.d_primes.get(), d.pids_bsk.get(), d.inv_punc_q.get(), d.q_to_bsk.get(),
+                                                                  d.inv_q_mod_bsk.get(), d.inv_punc_b.get(), d.b_to_q.get(), d.b_to_msk.get(), d.inv_b_mod_msk,
+                                                                  d.prod_b_mod_q.get(), d.neg_prod_b_mod_q.get(), c.logn, Li, nB, nS);
                 c.stats.end(st);
                 cuda_check(cudaGetLastError(), "behz_floor_sk_kernel");
             }

@@ -292,23 +292,18 @@ namespace sb
 
     Context::CkksEncoder &ckks_encoder(Context &c)
     {
-        auto &enc = c.ckks;
-        if (enc.ready)
-            return enc;
+        if (c.ckks.d_stat)
+            return c.ckks;
         if (c.scheme != 2)
             throw std::invalid_argument("unsupported scheme");
         const sbh::CkksTables t = sbh::ckks_tables(c.n);
-        const std::vector<uint32_t> map = sbh::batch_index_map(c.n); // matrix_reps_index_map_: the same map BatchEncoder uses
-        cuda_check(cudaMalloc(&enc.d_roots, c.n * 16), "cudaMalloc(ckks roots)");
-        cuda_check(cudaMalloc(&enc.d_inv_roots, c.n * 16), "cudaMalloc(ckks inverse roots)");
-        cuda_check(cudaMalloc(&enc.d_map, c.n * sizeof(uint32_t)), "cudaMalloc(ckks index map)");
-        cuda_check(cudaMalloc(&enc.d_stat, 16), "cudaMalloc(ckks status)");
-        cuda_check(cudaMemcpy(enc.d_roots, t.roots.data(), c.n * 16, cudaMemcpyHostToDevice), "upload ckks roots");
-        cuda_check(cudaMemcpy(enc.d_inv_roots, t.inv_roots.data(), c.n * 16, cudaMemcpyHostToDevice), "upload ckks inverse roots");
-        cuda_check(cudaMemcpy(enc.d_map, map.data(), c.n * sizeof(uint32_t), cudaMemcpyHostToDevice), "upload ckks index map");
-        c.table_bytes += c.n * 36;
-        enc.ready = true;
-        return enc;
+        Context::CkksEncoder enc;
+        enc.d_roots = upload<double2>(c, t.roots);
+        enc.d_inv_roots = upload<double2>(c, t.inv_roots);
+        enc.d_map = upload<uint32_t>(c, sbh::batch_index_map(c.n)); // matrix_reps_index_map_: the same map BatchEncoder uses
+        enc.d_stat = DevBuf<u64>(2);
+        c.table_bytes += enc.d_stat.bytes();
+        return c.ckks = std::move(enc);
     }
 
     // values: device, [B][count] complex (re, im) pairs or reals; plain: device, [B][L][n] NTT form.  Synchronises the stream once
@@ -332,14 +327,14 @@ namespace sb
         const long long n = static_cast<long long>(c.n), logn = c.logn;
         double2 *V = static_cast<double2 *>(c.ensure_aux(B * c.n * sizeof(double2)));
         cuda_check(cudaMemsetAsync(V, 0, B * c.n * sizeof(double2), st), "memset");
-        cuda_check(cudaMemsetAsync(enc.d_stat, 0, 16, st), "memset");
-        unsigned long long *d_max = static_cast<unsigned long long *>(enc.d_stat);
+        cuda_check(cudaMemsetAsync(enc.d_stat.get(), 0, 16, st), "memset");
+        unsigned long long *d_max = enc.d_stat.get();
         int *d_flags = reinterpret_cast<int *>(d_max + 1);
         if (count)
         {
             const long long total = static_cast<long long>(B) * static_cast<long long>(count);
             c.stats.begin("ckks_scatter", 0, 48.0 * total, st);
-            ckks_scatter_kernel<<<grid_for(total, 256), 256, 0, st>>>(values, is_complex ? 1 : 0, static_cast<long long>(count), enc.d_map, V,
+            ckks_scatter_kernel<<<grid_for(total, 256), 256, 0, st>>>(values, is_complex ? 1 : 0, static_cast<long long>(count), enc.d_map.get(), V,
                                                                       static_cast<int>(logn), total, d_flags);
             c.stats.end(st);
             cuda_check(cudaGetLastError(), "ckks_scatter_kernel");
@@ -348,7 +343,7 @@ namespace sb
         const int local = static_cast<int>(std::min<long long>(logn, kFftLocalLog));
         c.stats.begin("ckks_ifft_local", 0, 32.0 * B * n, st);
         ckks_ifft_local_kernel<<<static_cast<unsigned>(B * (c.n >> local)), std::min(1024, 1 << (local > 0 ? local - 1 : 0)),
-                                 (size_t(1) << local) * sizeof(double2), st>>>(V, static_cast<const double2 *>(enc.d_inv_roots), static_cast<int>(logn), local, fix);
+                                 (size_t(1) << local) * sizeof(double2), st>>>(V, enc.d_inv_roots.get(), static_cast<int>(logn), local, fix);
         c.stats.end(st);
         cuda_check(cudaGetLastError(), "ckks_ifft_local_kernel");
         const long long bflies = static_cast<long long>(B) * (n / 2);
@@ -356,9 +351,9 @@ namespace sb
         {
             c.stats.begin("ckks_ifft_stage", s, 32.0 * B * n, st);
             if (s + 1 < logn)
-                ckks_ifft_stage_kernel<false><<<grid_for(bflies, 256), 256, 0, st>>>(V, static_cast<const double2 *>(enc.d_inv_roots), static_cast<int>(logn), s, fix, bflies);
+                ckks_ifft_stage_kernel<false><<<grid_for(bflies, 256), 256, 0, st>>>(V, enc.d_inv_roots.get(), static_cast<int>(logn), s, fix, bflies);
             else
-                ckks_ifft_stage_kernel<true><<<grid_for(bflies, 256), 256, 0, st>>>(V, static_cast<const double2 *>(enc.d_inv_roots), static_cast<int>(logn), s, fix, bflies);
+                ckks_ifft_stage_kernel<true><<<grid_for(bflies, 256), 256, 0, st>>>(V, enc.d_inv_roots.get(), static_cast<int>(logn), s, fix, bflies);
             c.stats.end(st);
             cuda_check(cudaGetLastError(), "ckks_ifft_stage_kernel");
         }
@@ -372,7 +367,7 @@ namespace sb
             unsigned long long max_bits;
             int flags, pad;
         } stat;
-        cuda_check(cudaMemcpyAsync(&stat, enc.d_stat, 16, cudaMemcpyDeviceToHost, st), "status D2H");
+        cuda_check(cudaMemcpyAsync(&stat, enc.d_stat.get(), 16, cudaMemcpyDeviceToHost, st), "status D2H");
         cuda_check(cudaStreamSynchronize(st), "synchronize");
         if (stat.flags & 1)
             throw std::invalid_argument("values must be finite");
@@ -385,7 +380,7 @@ namespace sb
         if (max_coeff_bit_count >= total_bits)
             throw std::invalid_argument("encoded values are too large");
         c.stats.begin("ckks_reduce", 0, (16.0 + 8.0 * L) * total, st);
-        ckks_reduce_kernel<<<grid_for(total, 256), 256, 0, st>>>(V, plain, c.d_primes, static_cast<int>(logn), static_cast<int>(L), total);
+        ckks_reduce_kernel<<<grid_for(total, 256), 256, 0, st>>>(V, plain, c.d_primes.get(), static_cast<int>(logn), static_cast<int>(L), total);
         c.stats.end(st);
         cuda_check(cudaGetLastError(), "ckks_reduce_kernel");
         op_ntt(c, false, L, 1, B, plain, st);
@@ -412,7 +407,7 @@ namespace sb
         op_ntt(c, true, L, 1, B, coef, st);
         const double inv_scale = 1.0 / scale;
         c.stats.begin("ckks_compose", 0, (8.0 * L + 16.0) * total, st);
-        ckks_compose_kernel<<<grid_for(total, 128), 128, 0, st>>>(coef, lv.d_big, lv.d_invp, c.d_primes, V, static_cast<int>(logn), static_cast<int>(L),
+        ckks_compose_kernel<<<grid_for(total, 128), 128, 0, st>>>(coef, lv.d_big.get(), lv.d_invp.get(), c.d_primes.get(), V, static_cast<int>(logn), static_cast<int>(L),
                                                                   inv_scale, total);
         c.stats.end(st);
         cuda_check(cudaGetLastError(), "ckks_compose_kernel");
@@ -421,17 +416,17 @@ namespace sb
         for (int s = static_cast<int>(logn) - 1; s >= local; s--)
         {
             c.stats.begin("ckks_fft_stage", s, 32.0 * B * n, st);
-            ckks_fft_stage_kernel<<<grid_for(bflies, 256), 256, 0, st>>>(V, static_cast<const double2 *>(enc.d_roots), static_cast<int>(logn), s, bflies);
+            ckks_fft_stage_kernel<<<grid_for(bflies, 256), 256, 0, st>>>(V, enc.d_roots.get(), static_cast<int>(logn), s, bflies);
             c.stats.end(st);
             cuda_check(cudaGetLastError(), "ckks_fft_stage_kernel");
         }
         c.stats.begin("ckks_fft_local", 0, 32.0 * B * n, st);
         ckks_fft_local_kernel<<<static_cast<unsigned>(B * (c.n >> local)), std::min(1024, 1 << (local > 0 ? local - 1 : 0)),
-                                (size_t(1) << local) * sizeof(double2), st>>>(V, static_cast<const double2 *>(enc.d_roots), static_cast<int>(logn), local);
+                                (size_t(1) << local) * sizeof(double2), st>>>(V, enc.d_roots.get(), static_cast<int>(logn), local);
         c.stats.end(st);
         cuda_check(cudaGetLastError(), "ckks_fft_local_kernel");
         c.stats.begin("ckks_gather", 0, 16.0 * total, st);
-        ckks_gather_kernel<<<grid_for(total / 2, 256), 256, 0, st>>>(V, enc.d_map, reinterpret_cast<double2 *>(values), static_cast<int>(logn), total / 2);
+        ckks_gather_kernel<<<grid_for(total / 2, 256), 256, 0, st>>>(V, enc.d_map.get(), reinterpret_cast<double2 *>(values), static_cast<int>(logn), total / 2);
         c.stats.end(st);
         cuda_check(cudaGetLastError(), "ckks_gather_kernel");
     }

@@ -26,119 +26,38 @@ namespace sb
     }
 
     // ------------------------------------------------------------------------------------------- context ----
-    Context::~Context()
-    {
-        cudaSetDevice(device);
-        for (auto p : d_fwd)
-            cudaFree(p);
-        for (auto p : d_inv)
-            cudaFree(p);
-        for (auto &kv : galois_tables)
-            cudaFree(kv.second);
-        cudaFree(d_primes);
-        cudaFree(d_invq);
-        cudaFree(d_qmod);
-        cudaFree(d_t_mod_q);
-        cudaFree(d_batch_inv_map);
-        for (auto &kv : decrypt_levels)
-            cudaFree(kv.second.d_consts);
-        for (auto &kv : plain_levels)
-            cudaFree(kv.second.d_delta);
-        cudaFree(ckks.d_roots);
-        cudaFree(ckks.d_inv_roots);
-        cudaFree(ckks.d_map);
-        cudaFree(ckks.d_stat);
-        for (auto &kv : crt_levels)
-        {
-            cudaFree(kv.second.d_big);
-            cudaFree(kv.second.d_invp);
-        }
-        ksint_free(*this);
-        cudaFree(scratch);
-        cudaFree(aux_buf);
-        cudaFree(d_flag);
-        if (order_event)
-            cudaEventDestroy(order_event);
-        for (auto &slot : io.buf)
-            for (auto p : slot)
-                cudaFree(p);
-        for (auto &ln : io.lane)
-        {
-            for (int i = 0; i < 2; i++)
-            {
-                cudaFreeHost(ln.pin[i]);
-                if (ln.ev[i])
-                    cudaEventDestroy(ln.ev[i]);
-            }
-            if (ln.order)
-                cudaEventDestroy(ln.order);
-            if (ln.st)
-                cudaStreamDestroy(ln.st);
-        }
-        if (io.ready)
-        {
-            for (auto s : { io.s_in, io.s_comp, io.s_out })
-                cudaStreamDestroy(s);
-            for (int i = 0; i < 2; i++)
-                for (auto e : { io.ev_in[i], io.ev_comp[i], io.ev_out[i] })
-                    cudaEventDestroy(e);
-        }
-    }
-
     void *Context::ensure_scratch(size_t bytes)
     {
-        if (bytes > scratch_bytes)
-        {
-            cuda_check(cudaDeviceSynchronize(), "sync before scratch growth");
-            cudaFree(scratch);
-            scratch = nullptr;
-            scratch_bytes = 0;
-            cuda_check(cudaMalloc(&scratch, bytes), "cudaMalloc(scratch)");
-            scratch_bytes = bytes;
-        }
+        scratch.grow(bytes);
         scratch_used = bytes;
-        return scratch;
+        return scratch.get();
     }
 
     void Context::wipe_scratch(cudaStream_t st)
     {
         if (scratch && scratch_used)
-            cuda_check(cudaMemsetAsync(scratch, 0, std::min(scratch_used, scratch_bytes), st), "wipe scratch");
+            cuda_check(cudaMemsetAsync(scratch.get(), 0, std::min(scratch_used, scratch.bytes()), st), "wipe scratch");
     }
 
     void Context::wipe_aux(cudaStream_t st)
     {
         if (aux_buf && aux_used)
-            cuda_check(cudaMemsetAsync(aux_buf, 0, std::min(aux_used, aux_bytes), st), "wipe aux");
+            cuda_check(cudaMemsetAsync(aux_buf.get(), 0, std::min(aux_used, aux_buf.bytes()), st), "wipe aux");
     }
 
     void *Context::ensure_aux(size_t bytes)
     {
-        if (bytes > aux_bytes)
-        {
-            cuda_check(cudaDeviceSynchronize(), "sync before aux growth");
-            cudaFree(aux_buf);
-            aux_buf = nullptr;
-            aux_bytes = 0;
-            cuda_check(cudaMalloc(&aux_buf, bytes), "cudaMalloc(aux)");
-            aux_bytes = bytes;
-        }
+        aux_buf.grow(bytes);
         aux_used = bytes;
-        return aux_buf;
+        return aux_buf.get();
     }
 
     const uint32_t *Context::galois_table(uint32_t elt)
     {
         auto it = galois_tables.find(elt);
-        if (it != galois_tables.end())
-            return it->second;
-        auto h = sbh::galois_table_ntt(n, elt);
-        uint32_t *d = nullptr;
-        cuda_check(cudaMalloc(&d, n * sizeof(uint32_t)), "cudaMalloc(galois table)");
-        cuda_check(cudaMemcpy(d, h.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice), "upload galois table");
-        table_bytes += n * sizeof(uint32_t);
-        galois_tables[elt] = d;
-        return d;
+        if (it == galois_tables.end())
+            it = galois_tables.emplace(elt, upload<uint32_t>(*this, sbh::galois_table_ntt(n, elt))).first;
+        return it->second.get();
     }
 
     static Tw to_tw(const sbh::TwPair &p)
@@ -152,15 +71,8 @@ namespace sb
     static void upload_prime(Context &c, const sbh::PrimeTables &pt, std::vector<PrimeDev> &hp)
     {
         static_assert(sizeof(sbh::TwPair) == sizeof(Tw), "layout");
-        Tw *f = nullptr, *i = nullptr;
-        size_t bytes = c.n * sizeof(Tw);
-        cuda_check(cudaMalloc(&f, bytes), "cudaMalloc(twiddles)");
-        cuda_check(cudaMalloc(&i, bytes), "cudaMalloc(twiddles)");
-        cuda_check(cudaMemcpy(f, pt.fwd.data(), bytes, cudaMemcpyHostToDevice), "upload twiddles");
-        cuda_check(cudaMemcpy(i, pt.inv.data(), bytes, cudaMemcpyHostToDevice), "upload twiddles");
-        c.d_fwd.push_back(f);
-        c.d_inv.push_back(i);
-        c.table_bytes += 2 * bytes;
+        c.d_fwd.push_back(upload<Tw>(c, pt.fwd));
+        c.d_inv.push_back(upload<Tw>(c, pt.inv));
         PrimeDev d;
         d.q = pt.q;
         d.q2 = 2 * pt.q;
@@ -171,8 +83,8 @@ namespace sb
         d.ratio_hi = pt.ratio_hi;
         d.inv_n = to_tw(pt.inv_n);
         d.inv_n_w = to_tw(pt.inv_n_w);
-        d.fwd = f;
-        d.inv = i;
+        d.fwd = c.d_fwd.back().get();
+        d.inv = c.d_inv.back().get();
         {
             int bits = 0;
             while (bits < 64 && (pt.q >> bits))
@@ -260,16 +172,15 @@ namespace sb
         {
             if (c->tabs[i].q == 0)
             {
-                c->d_fwd.push_back(nullptr);
-                c->d_inv.push_back(nullptr);
+                c->d_fwd.emplace_back();
+                c->d_inv.emplace_back();
                 hp.push_back(PrimeDev{});
                 continue;
             }
             upload_prime(*c, c->tabs[i], hp);
         }
         c->nprimes = hp.size();
-        cuda_check(cudaMalloc(&c->d_primes, hp.size() * sizeof(PrimeDev)), "cudaMalloc(primes)");
-        cuda_check(cudaMemcpy(c->d_primes, hp.data(), hp.size() * sizeof(PrimeDev), cudaMemcpyHostToDevice), "upload primes");
+        c->d_primes = upload<PrimeDev>(*c, hp);
         // q_j^-1 mod q_i (rns.cpp:767-776 for every level at once)
         std::vector<Tw> invq(k * k);
         for (size_t j = 0; j < k; j++)
@@ -286,18 +197,14 @@ namespace sb
                 }
                 invq[j * k + i] = tw;
             }
-        cuda_check(cudaMalloc(&c->d_invq, invq.size() * sizeof(Tw)), "cudaMalloc(invq)");
-        cuda_check(cudaMemcpy(c->d_invq, invq.data(), invq.size() * sizeof(Tw), cudaMemcpyHostToDevice), "upload invq");
-        c->table_bytes += hp.size() * sizeof(PrimeDev) + invq.size() * sizeof(Tw);
+        c->d_invq = upload<Tw>(*c, invq);
         if (c->t_pid >= 0)
         {
             const auto map = sbh::batch_index_map(n);
             std::vector<uint32_t> inv(n);
             for (size_t i = 0; i < n; i++)
                 inv[map[i]] = static_cast<uint32_t>(i);
-            cuda_check(cudaMalloc(&c->d_batch_inv_map, n * sizeof(uint32_t)), "cudaMalloc(batch map)");
-            cuda_check(cudaMemcpy(c->d_batch_inv_map, inv.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice), "upload batch map");
-            c->table_bytes += n * sizeof(uint32_t);
+            c->d_batch_inv_map = upload<uint32_t>(*c, inv);
         }
         for (size_t L = 1; L <= k; L++)
         {
@@ -315,9 +222,7 @@ namespace sb
                     const u64 v = c->q[j] % c->q[i];
                     qmod[j * k + i] = Tw{ v, sbh::shoup(v, c->q[i]) };
                 }
-            cuda_check(cudaMalloc(&c->d_qmod, qmod.size() * sizeof(Tw)), "cudaMalloc(qmod)");
-            cuda_check(cudaMemcpy(c->d_qmod, qmod.data(), qmod.size() * sizeof(Tw), cudaMemcpyHostToDevice), "upload qmod");
-            c->table_bytes += qmod.size() * sizeof(Tw);
+            c->d_qmod = upload<Tw>(*c, qmod);
         }
         if (const char *e = std::getenv("SB200_KS_ALGO"))
             c->ks_algo = std::atoi(e);
@@ -383,12 +288,12 @@ namespace sb
         if (inverse)
         {
             OpSlab<true> op{ d, c.logn, static_cast<int>(L), pid_tab };
-            cuda_check(launch_ntt_inv(op, static_cast<int>(rows), c.logn, c.d_primes, st, c.stats), "ntt_inv");
+            cuda_check(launch_ntt_inv(op, static_cast<int>(rows), c.logn, c.d_primes.get(), st, c.stats), "ntt_inv");
         }
         else
         {
             OpSlab<false> op{ d, c.logn, static_cast<int>(L), pid_tab };
-            cuda_check(launch_ntt_fwd(op, static_cast<int>(rows), c.logn, c.d_primes, st, c.stats, "ntt_fwd", -1, c.fast_q && !pid_tab), "ntt_fwd");
+            cuda_check(launch_ntt_fwd(op, static_cast<int>(rows), c.logn, c.d_primes.get(), st, c.stats, "ntt_fwd", -1, c.fast_q && !pid_tab), "ntt_fwd");
         }
     }
 
@@ -454,9 +359,9 @@ namespace sb
         unsigned blocks = static_cast<unsigned>((total / 2 + 255) / 256);
         c.stats.begin("ckks_tensor", 0, 7.0 * 8.0 * total, st); // 4 reads + 3 writes per coefficient (SURVEY 8d)
         if (fused)
-            ckks_tensor_kernel<true><<<blocks, 256, 0, st>>>(a, b, out, c2, c.d_primes, c.logn, static_cast<int>(L), total);
+            ckks_tensor_kernel<true><<<blocks, 256, 0, st>>>(a, b, out, c2, c.d_primes.get(), c.logn, static_cast<int>(L), total);
         else
-            ckks_tensor_kernel<false><<<blocks, 256, 0, st>>>(a, b, out, c2, c.d_primes, c.logn, static_cast<int>(L), total);
+            ckks_tensor_kernel<false><<<blocks, 256, 0, st>>>(a, b, out, c2, c.d_primes.get(), c.logn, static_cast<int>(L), total);
         c.stats.end(st);
         cuda_check(cudaGetLastError(), "ckks_tensor_kernel");
     }
@@ -495,7 +400,7 @@ namespace sb
         const long long total = static_cast<long long>(B) * nb * c.n;
         c.stats.begin("tensor_general", 0, 8.0 * total * (2.0 * (s1 + s2) - 1.0), st);
         tensor_general_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(
-            xa, xa_bs, xb, xb_bs, out, c.d_primes, pid_tab, c.logn, static_cast<int>(nb), static_cast<int>(s1), static_cast<int>(s2), total);
+            xa, xa_bs, xb, xb_bs, out, c.d_primes.get(), pid_tab, c.logn, static_cast<int>(nb), static_cast<int>(s1), static_cast<int>(s2), total);
         c.stats.end(st);
         cuda_check(cudaGetLastError(), "tensor_general_kernel");
     }
@@ -556,7 +461,7 @@ namespace sb
                 const long long total = static_cast<long long>(nb) * L * c.n;
                 c.stats.begin("ckks_square", 0, 5.0 * 8.0 * total, st); // 2 reads + 3 writes per coefficient
                 ckks_square_kernel<<<static_cast<unsigned>((total / 2 + 255) / 256), 256, 0, st>>>(a + b0 * 2 * L * c.n, out3 + b0 * 3 * L * c.n,
-                                                                                                     c.d_primes, c.logn, static_cast<int>(L), total);
+                                                                                                     c.d_primes.get(), c.logn, static_cast<int>(L), total);
                 c.stats.end(st);
                 cuda_check(cudaGetLastError(), "ckks_square_kernel");
             }
@@ -604,11 +509,11 @@ namespace sb
             auto po = reinterpret_cast<ulonglong2 *>(out + b0 * per);
             c.stats.begin(mode == 0 ? "add" : mode == 1 ? "sub" : "negate", 0, (mode == 2 ? 16.0 : 24.0) * total2 * 2, st);
             if (mode == 0)
-                linear_kernel<0><<<blocks, 256, 0, st>>>(pa, pb, po, c.d_primes, c.logn, static_cast<int>(L), total2);
+                linear_kernel<0><<<blocks, 256, 0, st>>>(pa, pb, po, c.d_primes.get(), c.logn, static_cast<int>(L), total2);
             else if (mode == 1)
-                linear_kernel<1><<<blocks, 256, 0, st>>>(pa, pb, po, c.d_primes, c.logn, static_cast<int>(L), total2);
+                linear_kernel<1><<<blocks, 256, 0, st>>>(pa, pb, po, c.d_primes.get(), c.logn, static_cast<int>(L), total2);
             else
-                linear_kernel<2><<<blocks, 256, 0, st>>>(pa, pb, po, c.d_primes, c.logn, static_cast<int>(L), total2);
+                linear_kernel<2><<<blocks, 256, 0, st>>>(pa, pb, po, c.d_primes.get(), c.logn, static_cast<int>(L), total2);
             c.stats.end(st);
             cuda_check(cudaGetLastError(), "linear_kernel");
         }
@@ -645,7 +550,7 @@ namespace sb
             c.stats.begin("multiply_plain", 0, 8.0 * (2.0 * nb * per + nb * L * c.n), st);
             plain_mul_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const ulonglong2 *>(a + b0 * per),
                                                      reinterpret_cast<const ulonglong2 *>(plain + b0 * L * c.n),
-                                                     reinterpret_cast<ulonglong2 *>(out + b0 * per), c.d_primes, c.logn, static_cast<int>(L),
+                                                     reinterpret_cast<ulonglong2 *>(out + b0 * per), c.d_primes.get(), c.logn, static_cast<int>(L),
                                                      static_cast<int>(size), total2);
             c.stats.end(st);
             cuda_check(cudaGetLastError(), "plain_mul_kernel");
@@ -662,8 +567,7 @@ namespace sb
             std::vector<u64> tm(c.k);
             for (size_t i = 0; i < c.k; i++)
                 tm[i] = c.t % c.q[i];
-            cuda_check(cudaMalloc(&c.d_t_mod_q, c.k * sizeof(u64)), "cudaMalloc(t_mod_q)");
-            cuda_check(cudaMemcpy(c.d_t_mod_q, tm.data(), c.k * sizeof(u64), cudaMemcpyHostToDevice), "upload t_mod_q");
+            c.d_t_mod_q = upload<u64>(c, tm);
             const unsigned __int128 ratio = ~static_cast<unsigned __int128>(0) / c.t; // floor((2^128 - 1) / t): at most 1 below floor(2^128 / t)
             c.t_ratio_lo = static_cast<u64>(ratio), c.t_ratio_hi = static_cast<u64>(ratio >> 64);
         }
@@ -686,9 +590,8 @@ namespace sb
             const u64 v = static_cast<u64>(static_cast<unsigned __int128>(r ? c.q[i] - r : 0) * inv % c.q[i]);
             delta[i] = Tw{ v, sbh::shoup(v, c.q[i]) };
         }
-        cuda_check(cudaMalloc(&pl.d_delta, L * sizeof(Tw)), "cudaMalloc(delta)");
-        cuda_check(cudaMemcpy(pl.d_delta, delta.data(), L * sizeof(Tw), cudaMemcpyHostToDevice), "upload delta");
-        return c.plain_levels.emplace(L, pl).first->second;
+        pl.d_delta = upload<Tw>(c, delta);
+        return c.plain_levels.emplace(L, std::move(pl)).first->second;
     }
 
     // per-ciphertext BGV correction factors -> device (behind the scratch words of this call); nullptr stays nullptr
@@ -749,8 +652,8 @@ namespace sb
     static void plain_to_ntt_dev(Context &c, size_t L, size_t B, const u64 *plain, const u64 *d_cf, u64 *out, cudaStream_t st)
     {
         plain_level(c, L);
-        OpPlainLift op{ plain, d_cf, c.d_t_mod_q, out, c.t, c.t_ratio_lo, c.t_ratio_hi, c.logn, static_cast<int>(L) };
-        cuda_check(launch_ntt_fwd(op, static_cast<int>(B * L), c.logn, c.d_primes, st, c.stats, "plain_lift_ntt", -1, c.fast_q), "plain lift ntt");
+        OpPlainLift op{ plain, d_cf, c.d_t_mod_q.get(), out, c.t, c.t_ratio_lo, c.t_ratio_hi, c.logn, static_cast<int>(L) };
+        cuda_check(launch_ntt_fwd(op, static_cast<int>(B * L), c.logn, c.d_primes.get(), st, c.stats, "plain_lift_ntt", -1, c.fast_q), "plain lift ntt");
     }
 
     void op_plain_to_ntt(Context &c, size_t L, size_t batch, const u64 *plain, const u64 *h_cf, u64 *out, cudaStream_t st)
@@ -866,7 +769,7 @@ namespace sb
                 const long long total = static_cast<long long>(B * c.n);
                 c.stats.begin("bfv_add_plain", 0, 8.0 * total * (1 + 2 * L), st);
                 bfv_add_plain_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(
-                    plain + b0 * c.n, o, static_cast<long long>(per), pl.d_delta, c.d_primes, c.t, c.t_ratio_lo, c.t_ratio_hi, pl.q_mod_t, c.logn,
+                    plain + b0 * c.n, o, static_cast<long long>(per), pl.d_delta.get(), c.d_primes.get(), c.t, c.t_ratio_lo, c.t_ratio_hi, pl.q_mod_t, c.logn,
                     static_cast<int>(L), subtract ? 1 : 0, total);
                 c.stats.end(st);
                 cuda_check(cudaGetLastError(), "bfv_add_plain_kernel");
@@ -877,7 +780,7 @@ namespace sb
             plain_to_ntt_dev(c, L, B, plain + b0 * c.n, d_cf, T, st);
             const long long total = static_cast<long long>(B * L * c.n);
             c.stats.begin("bgv_add_plain", 0, 24.0 * total, st);
-            add_c0_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(T, o, static_cast<long long>(per), c.d_primes, c.logn,
+            add_c0_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(T, o, static_cast<long long>(per), c.d_primes.get(), c.logn,
                                                                                       static_cast<int>(L), subtract ? 1 : 0, total);
             c.stats.end(st);
             cuda_check(cudaGetLastError(), "add_c0_kernel");
@@ -953,8 +856,8 @@ namespace sb
         for (size_t b0 = 0; b0 < batch; b0 += step)
         {
             const size_t B = std::min(step, batch - b0);
-            OpBatchEncode op{ values + b0 * c.n, c.d_batch_inv_map, plain + b0 * c.n, c.logn, c.t_pid };
-            cuda_check(launch_ntt_inv(op, static_cast<int>(B), c.logn, c.d_primes, st, c.stats, "batch_encode_intt"), "batch encode");
+            OpBatchEncode op{ values + b0 * c.n, c.d_batch_inv_map.get(), plain + b0 * c.n, c.logn, c.t_pid };
+            cuda_check(launch_ntt_inv(op, static_cast<int>(B), c.logn, c.d_primes.get(), st, c.stats, "batch_encode_intt"), "batch encode");
         }
     }
     void op_batch_decode(Context &c, size_t batch, const u64 *plain, u64 *values, cudaStream_t st)
@@ -967,8 +870,8 @@ namespace sb
         {
             const size_t B = std::min(step, batch - b0);
             u64 *tmp = static_cast<u64 *>(c.ensure_scratch(B * c.n * sizeof(u64)));
-            OpBatchDecode op{ plain + b0 * c.n, c.d_batch_inv_map, tmp, values + b0 * c.n, c.logn, c.t_pid };
-            cuda_check(launch_ntt_fwd(op, static_cast<int>(B), c.logn, c.d_primes, st, c.stats, "batch_decode_ntt", -1, (c.t >> 57) == 0),
+            OpBatchDecode op{ plain + b0 * c.n, c.d_batch_inv_map.get(), tmp, values + b0 * c.n, c.logn, c.t_pid };
+            cuda_check(launch_ntt_fwd(op, static_cast<int>(B), c.logn, c.d_primes.get(), st, c.stats, "batch_decode_ntt", -1, (c.t >> 57) == 0),
                        "batch decode");
         }
     }
@@ -976,9 +879,8 @@ namespace sb
     // ---- decryption (decryptor.cpp): phase = c_0 + sum c_p s^p, then per scheme ---------------------------------------
     void secret_key_create(Context &c, const u64 *h_sk, SecretKey &out)
     {
-        const size_t bytes = c.k * c.n * sizeof(u64);
-        cuda_check(cudaMalloc(reinterpret_cast<void **>(&out.d_pow), bytes), "cudaMalloc(secret key)");
-        cuda_check(cudaMemcpy(out.d_pow, h_sk, bytes, cudaMemcpyHostToDevice), "upload secret key");
+        out.d_pow = DevBuf<u64>(c.k * c.n, true);
+        cuda_check(cudaMemcpy(out.d_pow.get(), h_sk, out.d_pow.bytes(), cudaMemcpyHostToDevice), "upload secret key");
         out.ctx = &c, out.powers = 1;
     }
     // Decryptor::compute_secret_key_array (decryptor.cpp:199-310): s^p = s^(p-1) * s, dyadic at the key level
@@ -987,16 +889,10 @@ namespace sb
         if (powers <= sk.powers)
             return;
         const size_t row = c.k * c.n;
-        u64 *grown = nullptr;
-        cuda_check(cudaDeviceSynchronize(), "sync before key array growth");
-        cuda_check(cudaMalloc(reinterpret_cast<void **>(&grown), powers * row * sizeof(u64)), "cudaMalloc(secret key array)");
-        cuda_check(cudaMemcpy(grown, sk.d_pow, sk.powers * row * sizeof(u64), cudaMemcpyDeviceToDevice), "copy");
-        cuda_check(cudaMemset(sk.d_pow, 0, sk.powers * row * sizeof(u64)), "wipe"); // secret material never goes back to the allocator in clear
-        cuda_check(cudaDeviceSynchronize(), "sync after wipe");
-        cudaFree(sk.d_pow);
-        sk.d_pow = grown;
+        sk.d_pow.grow(powers * row, true); // the old powers are wiped as they are freed
+        u64 *s = sk.d_pow.get();
         for (size_t p = sk.powers; p < powers; p++)
-            op_multiply_plain(c, c.k, 1, 1, sk.d_pow + (p - 1) * row, sk.d_pow, sk.d_pow + p * row, st);
+            op_multiply_plain(c, c.k, 1, 1, s + (p - 1) * row, s, s + p * row, st);
         sk.powers = powers;
     }
 
@@ -1193,11 +1089,9 @@ namespace sb
         std::vector<Tw> invp(L);
         for (size_t j = 0; j < L; j++)
             invp[j] = Tw{ h.inv_punctured[j].w, h.inv_punctured[j].wq };
-        cuda_check(cudaMalloc(&lv.d_big, big.size() * sizeof(u64)), "cudaMalloc(crt level)");
-        cuda_check(cudaMalloc(&lv.d_invp, L * sizeof(Tw)), "cudaMalloc(crt level)");
-        cuda_check(cudaMemcpy(lv.d_big, big.data(), big.size() * sizeof(u64), cudaMemcpyHostToDevice), "upload crt level");
-        cuda_check(cudaMemcpy(lv.d_invp, invp.data(), L * sizeof(Tw), cudaMemcpyHostToDevice), "upload crt level");
-        return c.crt_levels.emplace(L, lv).first->second;
+        lv.d_big = upload<u64>(c, big);
+        lv.d_invp = upload<Tw>(c, invp);
+        return c.crt_levels.emplace(L, std::move(lv)).first->second;
     }
     static const Context::DecryptLevel &decrypt_level(Context &c, size_t L)
     {
@@ -1239,9 +1133,8 @@ namespace sb
             dl.neg_inv_q_mod_t = inv_t ? t - inv_t : 0, dl.neg_inv_q_mod_g = inv_g ? gamma - inv_g : 0;
         }
         dl.q_mod_t = q_t;
-        cuda_check(cudaMalloc(&dl.d_consts, L * sizeof(DecConst)), "cudaMalloc(decrypt consts)");
-        cuda_check(cudaMemcpy(dl.d_consts, h.data(), L * sizeof(DecConst), cudaMemcpyHostToDevice), "upload decrypt consts");
-        return c.decrypt_levels.emplace(L, dl).first->second;
+        dl.d_consts = upload<DecConst>(c, h);
+        return c.decrypt_levels.emplace(L, std::move(dl)).first->second;
     }
 
     // The coefficient-form phase of ciphertexts ct [batch][size][L][n] (BFV / BGV), in chunks of the batch that fit the scratch arena:
@@ -1277,7 +1170,7 @@ namespace sb
                 op_ntt(c, false, L, size - 1, B, X, st);
                 c.stats.begin("decrypt_phase", 0, 8.0 * total * size, st);
                 phase_kernel<false><<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(X, static_cast<long long>(size - 1) * poly, nullptr, 0,
-                                                                                                sk.d_pow, sk_ps, T, c.d_primes, c.logn,
+                                                                                                sk.d_pow.get(), sk_ps, T, c.d_primes.get(), c.logn,
                                                                                                 static_cast<int>(L), npow, total);
                 c.stats.end(st);
                 cuda_check(cudaGetLastError(), "phase_kernel");
@@ -1285,8 +1178,8 @@ namespace sb
             else
             {
                 c.stats.begin("decrypt_phase", 0, 8.0 * total * (size + 1), st);
-                phase_kernel<true><<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(in + poly, ct_bs, in, ct_bs, sk.d_pow, sk_ps, T,
-                                                                                               c.d_primes, c.logn, static_cast<int>(L), npow, total);
+                phase_kernel<true><<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(in + poly, ct_bs, in, ct_bs, sk.d_pow.get(), sk_ps, T,
+                                                                                               c.d_primes.get(), c.logn, static_cast<int>(L), npow, total);
                 c.stats.end(st);
                 cuda_check(cudaGetLastError(), "phase_kernel");
             }
@@ -1314,8 +1207,8 @@ namespace sb
                 const long long total = static_cast<long long>(B) * poly;
                 const u64 *in = ct + b0 * ct_bs;
                 c.stats.begin("decrypt_phase", 0, 8.0 * total * (size + 1), st);
-                phase_kernel<true><<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(in + poly, ct_bs, in, ct_bs, sk.d_pow, sk_ps,
-                                                                                               plain + b0 * poly, c.d_primes, c.logn,
+                phase_kernel<true><<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(in + poly, ct_bs, in, ct_bs, sk.d_pow.get(), sk_ps,
+                                                                                               plain + b0 * poly, c.d_primes.get(), c.logn,
                                                                                                static_cast<int>(L), npow, total);
                 c.stats.end(st);
                 cuda_check(cudaGetLastError(), "phase_kernel");
@@ -1335,7 +1228,7 @@ namespace sb
                 const long long tn = static_cast<long long>(B) * n;
                 c.stats.begin("bfv_scale_round", 0, 8.0 * tn * (2 * L + 1), st);
                 bfv_scale_round_kernel<<<static_cast<unsigned>((tn + 127) / 128), 128, 0, st>>>(
-                    T, in, ct_bs, plain + b0 * c.n, static_cast<const DecConst *>(dl.d_consts), c.d_primes, c.t, c.t_ratio_lo, c.t_ratio_hi, gamma,
+                    T, in, ct_bs, plain + b0 * c.n, dl.d_consts.get(), c.d_primes.get(), c.t, c.t_ratio_lo, c.t_ratio_hi, gamma,
                     g_rlo, g_rhi, dl.neg_inv_q_mod_t, dl.neg_inv_q_mod_g, inv_gamma_t, c.logn, static_cast<int>(L), tn);
                 c.stats.end(st);
                 cuda_check(cudaGetLastError(), "bfv_scale_round_kernel");
@@ -1361,8 +1254,8 @@ namespace sb
                 d_fix = extra;
             }
             c.stats.begin("bgv_modt", 0, 8.0 * tn * (L + 1), st);
-            bgv_modt_kernel<<<static_cast<unsigned>((tn + 127) / 128), 128, 0, st>>>(T, plain + b0 * c.n, static_cast<const DecConst *>(dl.d_consts),
-                                                                                     c.d_primes, d_fix, c.t, c.t_ratio_lo, c.t_ratio_hi, dl.q_mod_t,
+            bgv_modt_kernel<<<static_cast<unsigned>((tn + 127) / 128), 128, 0, st>>>(T, plain + b0 * c.n, dl.d_consts.get(),
+                                                                                     c.d_primes.get(), d_fix, c.t, c.t_ratio_lo, c.t_ratio_hi, dl.q_mod_t,
                                                                                      c.logn, static_cast<int>(L), tn);
             c.stats.end(st);
             cuda_check(cudaGetLastError(), "bgv_modt_kernel");
@@ -1397,10 +1290,10 @@ namespace sb
             const dim3 grid(static_cast<unsigned>(B), static_cast<unsigned>((c.n + 127) / 128));
             c.stats.begin("noise_norm", 0, 8.0 * B * c.n * (bfv ? 2 * L : L), st);
             if (bfv)
-                noise_norm_kernel<true><<<grid, 128, 0, st>>>(T, in, ct_bs, c.d_t_mod_q, lv.d_big, lv.d_invp, c.d_primes, c.logn, static_cast<int>(L),
+                noise_norm_kernel<true><<<grid, 128, 0, st>>>(T, in, ct_bs, c.d_t_mod_q.get(), lv.d_big.get(), lv.d_invp.get(), c.d_primes.get(), c.logn, static_cast<int>(L),
                                                               budgets + b0);
             else
-                noise_norm_kernel<false><<<grid, 128, 0, st>>>(T, in, ct_bs, c.d_t_mod_q, lv.d_big, lv.d_invp, c.d_primes, c.logn, static_cast<int>(L),
+                noise_norm_kernel<false><<<grid, 128, 0, st>>>(T, in, ct_bs, c.d_t_mod_q.get(), lv.d_big.get(), lv.d_invp.get(), c.d_primes.get(), c.logn, static_cast<int>(L),
                                                                budgets + b0);
             c.stats.end(st);
             cuda_check(cudaGetLastError(), "noise_norm_kernel");
@@ -2029,24 +1922,24 @@ namespace sb
         case 0: // forward butterflies at the column-pass launch shape (512 threads x 3 CTAs per SM)
             ops = static_cast<double>(sms) * 3 * 16 * rounds * 12.0;
             if (c.fast_q)
-                run([&] { selftest_bfly_kernel<0, 512, 3><<<sms * 3, 512, 0, st>>>(d, c.d_primes, rounds, nmask); });
+                run([&] { selftest_bfly_kernel<0, 512, 3><<<sms * 3, 512, 0, st>>>(d, c.d_primes.get(), rounds, nmask); });
             else
-                run([&] { selftest_bfly_kernel<1, 512, 3><<<sms * 3, 512, 0, st>>>(d, c.d_primes, rounds, nmask); });
+                run([&] { selftest_bfly_kernel<1, 512, 3><<<sms * 3, 512, 0, st>>>(d, c.d_primes.get(), rounds, nmask); });
             break;
         case 1: // forward butterflies at the fused kernel's launch shape (256 threads x 2 CTAs per SM)
             ops = static_cast<double>(sms) * 2 * 8 * rounds * 12.0;
             if (c.fast_q)
-                run([&] { selftest_bfly_kernel<0, 256, 2><<<sms * 2, 256, 0, st>>>(d, c.d_primes, rounds, nmask); });
+                run([&] { selftest_bfly_kernel<0, 256, 2><<<sms * 2, 256, 0, st>>>(d, c.d_primes.get(), rounds, nmask); });
             else
-                run([&] { selftest_bfly_kernel<1, 256, 2><<<sms * 2, 256, 0, st>>>(d, c.d_primes, rounds, nmask); });
+                run([&] { selftest_bfly_kernel<1, 256, 2><<<sms * 2, 256, 0, st>>>(d, c.d_primes.get(), rounds, nmask); });
             break;
         case 2: // inverse butterflies
             ops = static_cast<double>(sms) * 3 * 16 * rounds * 12.0;
-            run([&] { selftest_bfly_kernel<2, 512, 3><<<sms * 3, 512, 0, st>>>(d, c.d_primes, rounds, nmask); });
+            run([&] { selftest_bfly_kernel<2, 512, 3><<<sms * 3, 512, 0, st>>>(d, c.d_primes.get(), rounds, nmask); });
             break;
         case 3: // key multiply-accumulates of the fused kernel
             ops = static_cast<double>(sms) * 2 * 8 * rounds * 16.0;
-            run([&] { selftest_mac_kernel<<<sms * 2, 256, 0, st>>>(d, c.d_primes, rounds); });
+            run([&] { selftest_mac_kernel<<<sms * 2, 256, 0, st>>>(d, c.d_primes.get(), rounds); });
             break;
         default: throw std::invalid_argument("unknown selftest");
         }
@@ -2099,7 +1992,7 @@ namespace sb
         if (ntt_in)
         {
             OpKsIntt op{ target, s.D, c.logn, Li };
-            cuda_check(launch_ntt_inv(op, static_cast<int>(B * L), c.logn, c.d_primes, st, c.stats, "ks_target_intt"), "ks intt");
+            cuda_check(launch_ntt_inv(op, static_cast<int>(B * L), c.logn, c.d_primes.get(), st, c.stats, "ks_target_intt"), "ks intt");
             dsrc = Src{ s.D, static_cast<long long>(L) * n, nullptr, 0, c.logn };
         }
         const bool fused = c.logn >= 12; // two-pass transforms: fuse the in-block stages with the key multiply-accumulate
@@ -2111,7 +2004,7 @@ namespace sb
                 qmax = std::max(qmax, c.q[i]), qmin = std::min(qmin, c.q[i]);
             qmin = std::min(qmin, c.q[c.k - 1]);
             const int reduce = (qmax >> 2) >= qmin ? 1 : 0;
-            OpKsDigit op{ dsrc, s.E, c.d_primes, c.logn, Li, ki, ntt_in ? 1 : 0, reduce };
+            OpKsDigit op{ dsrc, s.E, c.d_primes.get(), c.logn, Li, ki, ntt_in ? 1 : 0, reduce };
             const int active = static_cast<int>(B * (ntt_in ? L * L : (L + 1) * L));
             active_rows = active;
             const bool plain_rows = !reduce && dsrc.perm == nullptr && dsrc.ginv == 0;
@@ -2120,19 +2013,19 @@ namespace sb
                 c.stats.begin("ks_digit_ntt", 1, 16.0 * active * n, st, 0.5 * active * n * (c.logn - kLocalLog));
                 switch (c.logn - kLocalLog)
                 {
-                case 4: launch_ks_digit_col<4>(op, static_cast<int>(B), c.fast_q, plain_rows, c.d_primes, st); break;
-                case 5: launch_ks_digit_col<5>(op, static_cast<int>(B), c.fast_q, plain_rows, c.d_primes, st); break;
-                case 6: launch_ks_digit_col<6>(op, static_cast<int>(B), c.fast_q, plain_rows, c.d_primes, st); break;
-                case 7: launch_ks_digit_col<7>(op, static_cast<int>(B), c.fast_q, plain_rows, c.d_primes, st); break;
-                case 8: launch_ks_digit_col<8>(op, static_cast<int>(B), c.fast_q, plain_rows, c.d_primes, st); break;
-                case 9: launch_ks_digit_col<9>(op, static_cast<int>(B), c.fast_q, plain_rows, c.d_primes, st); break;
+                case 4: launch_ks_digit_col<4>(op, static_cast<int>(B), c.fast_q, plain_rows, c.d_primes.get(), st); break;
+                case 5: launch_ks_digit_col<5>(op, static_cast<int>(B), c.fast_q, plain_rows, c.d_primes.get(), st); break;
+                case 6: launch_ks_digit_col<6>(op, static_cast<int>(B), c.fast_q, plain_rows, c.d_primes.get(), st); break;
+                case 7: launch_ks_digit_col<7>(op, static_cast<int>(B), c.fast_q, plain_rows, c.d_primes.get(), st); break;
+                case 8: launch_ks_digit_col<8>(op, static_cast<int>(B), c.fast_q, plain_rows, c.d_primes.get(), st); break;
+                case 9: launch_ks_digit_col<9>(op, static_cast<int>(B), c.fast_q, plain_rows, c.d_primes.get(), st); break;
                 default: throw std::logic_error("unsupported transform size");
                 }
                 c.stats.end(st);
                 cuda_check(cudaGetLastError(), "ks_digit_col_kernel");
             }
             else
-                cuda_check(launch_ntt_fwd(op, static_cast<int>(B * (L + 1) * L), c.logn, c.d_primes, st, c.stats, "ks_digit_ntt", active, c.fast_q),
+                cuda_check(launch_ntt_fwd(op, static_cast<int>(B * (L + 1) * L), c.logn, c.d_primes.get(), st, c.stats, "ks_digit_ntt", active, c.fast_q),
                            "ks digit ntt");
         }
         // digits in + 2 accumulated components out per (b, I), plus one pass over the key
@@ -2146,7 +2039,7 @@ namespace sb
                 constexpr size_t smem = KsMacSmem::total;
                 cuda_check(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)), "smem attr");
                 c.stats.begin("ks_local_mac", 0, mac_bytes, st, 0.5 * active_rows * n * kLocalLog, 2.0 * B * (L + 1) * L * n);
-                kern<<<grid, 256, smem, st>>>(s.E, target, ntt_in ? 1 : 0, key.d_key, s.Pp, c.d_primes, c.logn, Li, ki, static_cast<int>(B));
+                kern<<<grid, 256, smem, st>>>(s.E, target, ntt_in ? 1 : 0, key.d_key.get(), s.Pp, c.d_primes.get(), c.logn, Li, ki, static_cast<int>(B));
             };
             if (c.fast_q)
                 plain_tgt ? launch(ks_local_mac_kernel<true, true>) : launch(ks_local_mac_kernel<true, false>);
@@ -2160,7 +2053,7 @@ namespace sb
             int threads = std::min(n, 256);
             dim3 grid(static_cast<unsigned>(B), (n + threads - 1) / threads, static_cast<unsigned>(L + 1));
             c.stats.begin("ks_mac", 0, mac_bytes, st, 0, 2.0 * B * (L + 1) * L * n);
-            ks_mac_kernel<<<grid, threads, 0, st>>>(s.E, target, ntt_in ? 1 : 0, key.d_key, s.Pp, c.d_primes, c.logn, Li, ki);
+            ks_mac_kernel<<<grid, threads, 0, st>>>(s.E, target, ntt_in ? 1 : 0, key.d_key.get(), s.Pp, c.d_primes.get(), c.logn, Li, ki);
             c.stats.end(st);
             cuda_check(cudaGetLastError(), "ks_mac_kernel");
         }
@@ -2169,29 +2062,29 @@ namespace sb
             OpTopIntt op{ s.Pp + static_cast<long long>(L) * n, pp_bs, pp_ps, s.U, c.logn, ki - 1 };
             if (bgv)
                 bgv_top(c, op, s.K, c.k - 1);
-            cuda_check(launch_ntt_inv(op, static_cast<int>(B * 2), c.logn, c.d_primes, st, c.stats, "ks_top_intt"), "ks top intt");
+            cuda_check(launch_ntt_inv(op, static_cast<int>(B * 2), c.logn, c.d_primes.get(), st, c.stats, "ks_top_intt"), "ks top intt");
         }
-        const Tw *inv_top = c.d_invq + (c.k - 1) * c.k;
+        const Tw *inv_top = c.d_invq.get() + (c.k - 1) * c.k;
         const long long o_ps = static_cast<long long>(L) * n, o_bs = out_bs ? out_bs : 2 * o_ps;
         if (bgv)
         {
             OpModDownFwdBgv op{ { s.U, s.Pp, pp_bs, pp_ps, s.T, out, o_bs, o_ps, inv_top, base, c.q[c.k - 1], c.logn, Li },
-                                s.K, c.d_qmod + (c.k - 1) * c.k, c.t };
-            cuda_check(launch_ntt_fwd(op, static_cast<int>(B * 2 * L), c.logn, c.d_primes, st, c.stats, "ks_moddown_ntt", -1, c.fast_q), "ks moddown ntt");
+                                s.K, c.d_qmod.get() + (c.k - 1) * c.k, c.t };
+            cuda_check(launch_ntt_fwd(op, static_cast<int>(B * 2 * L), c.logn, c.d_primes.get(), st, c.stats, "ks_moddown_ntt", -1, c.fast_q), "ks moddown ntt");
         }
         else if (ntt_in)
         {
             OpModDownFwd op{ s.U, s.Pp, pp_bs, pp_ps, s.T, out, o_bs, o_ps, inv_top, base, c.q[c.k - 1], c.logn, Li };
-            cuda_check(launch_ntt_fwd(op, static_cast<int>(B * 2 * L), c.logn, c.d_primes, st, c.stats, "ks_moddown_ntt", -1, c.fast_q), "ks moddown ntt");
+            cuda_check(launch_ntt_fwd(op, static_cast<int>(B * 2 * L), c.logn, c.d_primes.get(), st, c.stats, "ks_moddown_ntt", -1, c.fast_q), "ks moddown ntt");
         }
         else
         {
             OpProdIntt op{ s.Pp, c.logn, Li };
-            cuda_check(launch_ntt_inv(op, static_cast<int>(B * 2 * L), c.logn, c.d_primes, st, c.stats, "ks_prod_intt"), "ks prod intt");
+            cuda_check(launch_ntt_inv(op, static_cast<int>(B * 2 * L), c.logn, c.d_primes.get(), st, c.stats, "ks_prod_intt"), "ks prod intt");
             long long total = static_cast<long long>(B) * 2 * L * n;
             c.stats.begin("moddown_coeff", 0, 32.0 * total, st);
             moddown_coeff_kernel<false><<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(
-                s.U, 2LL * n, n, s.Pp, pp_bs, pp_ps, out, o_bs, o_ps, inv_top, base, c.q[c.k - 1], c.d_primes, c.logn, Li, total);
+                s.U, 2LL * n, n, s.Pp, pp_bs, pp_ps, out, o_bs, o_ps, inv_top, base, c.q[c.k - 1], c.d_primes.get(), c.logn, Li, total);
             c.stats.end(st);
             cuda_check(cudaGetLastError(), "moddown_coeff_kernel");
         }
@@ -2322,14 +2215,17 @@ namespace sb
     bool op_residues_in_range(Context &c, size_t L, size_t rows, const u64 *d, cudaStream_t st)
     {
         if (!c.d_flag)
-            cuda_check(cudaMalloc(reinterpret_cast<void **>(&c.d_flag), sizeof(int)), "cudaMalloc(flag)");
-        int *flag = c.d_flag; // a word of its own: the aux arena may be in use by an operation in flight on another stream
+        {
+            c.d_flag = DevBuf<int>(1);
+            c.table_bytes += c.d_flag.bytes();
+        }
+        int *flag = c.d_flag.get(); // a word of its own: the aux arena may be in use by an operation in flight on another stream
         cuda_check(cudaMemsetAsync(flag, 0, sizeof(int), st), "memset");
         const size_t step = std::max<size_t>(1, (size_t(1) << 31) / c.n);
         for (size_t r0 = 0; r0 < rows; r0 += step * L)
         {
             const long long total = static_cast<long long>(std::min(step * L, rows - r0) * c.n);
-            range_check_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(d + r0 * c.n, c.d_primes, c.logn, static_cast<int>(L),
+            range_check_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(d + r0 * c.n, c.d_primes.get(), c.logn, static_cast<int>(L),
                                                                                             total, flag);
             cuda_check(cudaGetLastError(), "range_check_kernel");
             c.stats.launches++;
@@ -2363,12 +2259,12 @@ namespace sb
             const u64 *src = in + p0 * L * c.n;
             const long long i_ps = static_cast<long long>(L) * n, i_bs = 2 * i_ps;
             OpTopIntt top{ src + (L - 1) * c.n, i_bs, i_ps, U, c.logn, static_cast<int>(L - 1) };
-            cuda_check(launch_ntt_inv(top, static_cast<int>(P), c.logn, c.d_primes, st, c.stats, "rescale_top_intt"), "rescale intt");
+            cuda_check(launch_ntt_inv(top, static_cast<int>(P), c.logn, c.d_primes.get(), st, c.stats, "rescale_top_intt"), "rescale intt");
             BaseSrc none;
             const long long o_ps = static_cast<long long>(Lout) * n, o_bs = 2 * o_ps;
-            OpModDownFwd op{ U, src, i_bs, i_ps, T, out + p0 * Lout * c.n, o_bs, o_ps, c.d_invq + (L - 1) * c.k, none, c.q[L - 1],
+            OpModDownFwd op{ U, src, i_bs, i_ps, T, out + p0 * Lout * c.n, o_bs, o_ps, c.d_invq.get() + (L - 1) * c.k, none, c.q[L - 1],
                              c.logn, static_cast<int>(Lout) };
-            cuda_check(launch_ntt_fwd(op, static_cast<int>(P * Lout), c.logn, c.d_primes, st, c.stats, "rescale_ntt", -1, c.fast_q), "rescale ntt");
+            cuda_check(launch_ntt_fwd(op, static_cast<int>(P * Lout), c.logn, c.d_primes.get(), st, c.stats, "rescale_ntt", -1, c.fast_q), "rescale ntt");
         }
     }
 
@@ -2401,13 +2297,13 @@ namespace sb
                 const long long i_ps = static_cast<long long>(L) * n, i_bs = 2 * i_ps;
                 OpTopIntt top{ src + (L - 1) * c.n, i_bs, i_ps, U, c.logn, static_cast<int>(L - 1) };
                 bgv_top(c, top, K, L - 1);
-                cuda_check(launch_ntt_inv(top, static_cast<int>(P), c.logn, c.d_primes, st, c.stats, "modswitch_top_intt"), "mod switch intt");
+                cuda_check(launch_ntt_inv(top, static_cast<int>(P), c.logn, c.d_primes.get(), st, c.stats, "modswitch_top_intt"), "mod switch intt");
                 BaseSrc none;
                 const long long o_ps = static_cast<long long>(Lout) * n, o_bs = 2 * o_ps;
-                OpModDownFwdBgv op{ { U, src, i_bs, i_ps, T, out + p0 * Lout * c.n, o_bs, o_ps, c.d_invq + (L - 1) * c.k, none, c.q[L - 1],
+                OpModDownFwdBgv op{ { U, src, i_bs, i_ps, T, out + p0 * Lout * c.n, o_bs, o_ps, c.d_invq.get() + (L - 1) * c.k, none, c.q[L - 1],
                                       c.logn, static_cast<int>(Lout) },
-                                    K, c.d_qmod + (L - 1) * c.k, c.t };
-                cuda_check(launch_ntt_fwd(op, static_cast<int>(P * Lout), c.logn, c.d_primes, st, c.stats, "modswitch_ntt", -1, c.fast_q),
+                                    K, c.d_qmod.get() + (L - 1) * c.k, c.t };
+                cuda_check(launch_ntt_fwd(op, static_cast<int>(P * Lout), c.logn, c.d_primes.get(), st, c.stats, "modswitch_ntt", -1, c.fast_q),
                            "mod switch ntt");
             }
             return;
@@ -2423,7 +2319,7 @@ namespace sb
             c.stats.begin("moddown_coeff", 0, 24.0 * total, st);
             moddown_coeff_kernel<true><<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(
                 src + (L - 1) * c.n, 2 * i_ps, i_ps, src, 2 * i_ps, i_ps, out + p0 * Lout * c.n, 2 * o_ps, o_ps,
-                c.d_invq + (L - 1) * c.k, none, c.q[L - 1], c.d_primes, c.logn, static_cast<int>(Lout), total);
+                c.d_invq.get() + (L - 1) * c.k, none, c.q[L - 1], c.d_primes.get(), c.logn, static_cast<int>(Lout), total);
             c.stats.end(st);
             cuda_check(cudaGetLastError(), "moddown_coeff_kernel");
         }

@@ -1,6 +1,7 @@
 // seal_b200/csrc/sb_engine.cuh -- device context + operation drivers (declarations).
 #pragma once
 #include "sb_host.hpp"
+#include "sb_mem.cuh"
 #include "sb_ntt.cuh"
 #include "sb_ksint.cuh"
 #include "sb_wire.hpp"
@@ -13,20 +14,16 @@
 
 namespace sb
 {
-    struct CudaError : std::runtime_error
-    {
-        using std::runtime_error::runtime_error;
-    };
-    void cuda_check(cudaError_t e, const char *what);
-
     // device copy of sbh::BehzLevel (BFV multiply), see sb_bfv.cu
     struct BehzDev;
+    // decryption constants of one prime (sb_engine.cu)
+    struct DecConst;
 
     // the secret key on the device for decryption: powers s^1 .. s^powers in NTT form at the key level, [powers][k][n]
     struct SecretKey
     {
         struct Context *ctx = nullptr;
-        u64 *d_pow = nullptr;
+        DevBuf<u64> d_pow; // made with wipe set: zeroed before it is freed
         size_t powers = 0;
     };
 
@@ -34,33 +31,30 @@ namespace sb
     struct PublicKey
     {
         struct Context *ctx = nullptr;
-        u64 *d_key = nullptr;
+        DevBuf<u64> d_key;
     };
 
     struct KSwitchKey
     {
         struct Context *ctx = nullptr;
-        u64 *d_key = nullptr; // [digits][2][k][n]
-        uint32_t *d_key32 = nullptr; // [S][digits][2][k][n]: the key modulo the auxiliary primes, transformed (sb_ksint.cuh)
+        DevBuf<u64> d_key;        // [digits][2][k][n]
+        DevBuf<uint32_t> d_key32; // [S][digits][2][k][n]: the key modulo the auxiliary primes, transformed (sb_ksint.cuh)
         size_t digits = 0;
     };
 
     // staging for the host-buffer entry points (sb_api.cu: HostPipe)
     struct IoArena
     {
-        bool ready = false;
-        cudaStream_t s_in = nullptr, s_comp = nullptr, s_out = nullptr;
-        cudaEvent_t ev_in[2] = {}, ev_comp[2] = {}, ev_out[2] = {};
-        u64 *buf[2][3] = {};
-        size_t cap[2][3] = {};
+        Stream s_in, s_comp, s_out;
+        Event ev_in[2], ev_comp[2], ev_out[2];
+        DevBuf<u64> buf[2][3];
         // page-locked staging of sb200_upload_rows ([0]) / sb200_download_rows ([1]): separate double buffers, streams and locks,
         // so that an upload, a download and the kernels of a third batch overlap (three host threads, or one thread per direction)
         struct Lane
         {
-            void *pin[2] = {};
-            size_t cap = 0;
-            cudaEvent_t ev[2] = {}, order = nullptr;
-            cudaStream_t st = nullptr;
+            PinnedBuf pin[2];
+            Event ev[2], order;
+            Stream st;
             std::mutex mu;
         } lane[2];
     };
@@ -74,58 +68,56 @@ namespace sb
         std::vector<u64> q;                  // key-level primes
         std::vector<sbh::PrimeTables> tabs;  // host tables; ids [0,k) = q primes, [k, ...) = BEHZ auxiliary primes
         std::vector<u64> aux;                // auxiliary prime list [m_sk, gamma, B_0, B_1, ...] (BFV)
-        std::vector<Tw *> d_fwd, d_inv;      // per prime id
-        PrimeDev *d_primes = nullptr;        // [nprimes]
+        std::vector<DevBuf<Tw>> d_fwd, d_inv; // per prime id
+        DevBuf<PrimeDev> d_primes;           // [nprimes]
         size_t nprimes = 0;
-        Tw *d_invq = nullptr;                // [k][k]: d_invq[j*k+i] = q_j^-1 mod q_i  (i != j)
-        Tw *d_qmod = nullptr;                // BGV, [k][k]: d_qmod[j*k+i] = q_j mod q_i
+        DevBuf<Tw> d_invq;                   // [k][k]: d_invq[j*k+i] = q_j^-1 mod q_i  (i != j)
+        DevBuf<Tw> d_qmod;                   // BGV, [k][k]: d_qmod[j*k+i] = q_j mod q_i
         u64 t_ratio = 0;                     // BGV: floor(2^64 / t)
         std::vector<u64> inv_q_mod_t;        // BGV: q_j^-1 mod t
-        // decryption constants per level (sb_engine.cu: decrypt_level): [L] x {Tw c, u64 m_t, u64 m_g}
+        // decryption constants per level (sb_engine.cu: decrypt_level)
         struct DecryptLevel
         {
-            void *d_consts = nullptr;
+            DevBuf<DecConst> d_consts; // [L]
             u64 neg_inv_q_mod_t = 0, neg_inv_q_mod_g = 0, q_mod_t = 0;
         };
         std::map<size_t, DecryptLevel> decrypt_levels;
         // BatchEncoder on the device (BFV / BGV with an NTT-friendly plain modulus): prime id of t and the inverse slot map
         int t_pid = -1;
-        uint32_t *d_batch_inv_map = nullptr; // coefficient index -> matrix slot
+        DevBuf<uint32_t> d_batch_inv_map;    // coefficient index -> matrix slot
         // coefficient-form plaintext operations (BFV / BGV): per-level constants, built on first use (sb_engine.cu: plain_level)
         struct PlainLevel
         {
-            Tw *d_delta = nullptr;  // [L]: floor(q / t) mod q_i (ContextData::coeff_div_plain_modulus, context.cpp:300-318)
+            DevBuf<Tw> d_delta;     // [L]: floor(q / t) mod q_i (ContextData::coeff_div_plain_modulus, context.cpp:300-318)
             u64 q_mod_t = 0;        // ContextData::coeff_modulus_mod_plain_modulus
         };
         std::map<size_t, PlainLevel> plain_levels;
         // CKKSEncoder on the device (sb_ckks.cu): complex root tables + slot map, built on first use
         struct CkksEncoder
         {
-            bool ready = false;
-            void *d_roots = nullptr, *d_inv_roots = nullptr; // double2 [n]
-            uint32_t *d_map = nullptr;                       // matrix_reps_index_map_
-            void *d_stat = nullptr;                          // { max |coefficient| bits, flags }
+            DevBuf<double2> d_roots, d_inv_roots; // [n]
+            DevBuf<uint32_t> d_map;               // matrix_reps_index_map_
+            DevBuf<u64> d_stat;                   // { max |coefficient| bits, flags }
         } ckks;
         // per-level big integers of the CRT composition (crt_compose, sb_device.cuh), built on first use (crt_level); they depend on
         // the primes only: CKKS decode and the BFV / BGV invariant noise budget share them
         struct CrtLevel
         {
             int total_bits = 0;
-            u64 *d_big = nullptr; // [Q | (Q+1)/2 | Q/q_j ...] words
-            Tw *d_invp = nullptr; // (Q/q_j)^-1 mod q_j
+            DevBuf<u64> d_big; // [Q | (Q+1)/2 | Q/q_j ...] words
+            DevBuf<Tw> d_invp; // (Q/q_j)^-1 mod q_j
         };
         std::map<size_t, CrtLevel> crt_levels;
-        u64 *d_t_mod_q = nullptr;   // [k]: t mod q_i
+        DevBuf<u64> d_t_mod_q;      // [k]: t mod q_i
         u64 t_ratio_lo = 0, t_ratio_hi = 0; // floor(2^128 / t)
         std::vector<std::array<u64, 4>> parms_ids; // parms_ids[L-1] = parms_id of the level with L primes (sb_wire.hpp)
-        std::map<uint32_t, uint32_t *> galois_tables; // NTT-form permutation tables (device)
+        std::map<uint32_t, DevBuf<uint32_t>> galois_tables; // NTT-form permutation tables
         std::map<size_t, std::shared_ptr<BehzDev>> behz; // per level L
-        void *scratch = nullptr;
-        int *d_flag = nullptr;               // result word of the range check (op_residues_in_range)
-        void *aux_buf = nullptr;             // second grow-only arena (size-3 intermediate of BFV multiply+relinearize)
-        size_t aux_bytes = 0;
+        DevBuf<unsigned char> scratch;
+        DevBuf<int> d_flag;                  // result word of the range check (op_residues_in_range)
+        DevBuf<unsigned char> aux_buf;       // second grow-only arena (size-3 intermediate of BFV multiply+relinearize)
         size_t scratch_used = 0, aux_used = 0; // bytes of the latest ensure_scratch / ensure_aux request (what wipe_* clears)
-        size_t scratch_bytes = 0, table_bytes = 0, scratch_budget = size_t(8) << 30;
+        size_t table_bytes = 0, scratch_budget = size_t(8) << 30;
         size_t ks_chunk_max = 0;                       // 0 = derived from scratch_budget (sb200_context_set_limit)
         size_t host_stage_bytes = size_t(640) << 20;   // per pipeline slot of the *_host entry points
         LaunchStats stats;
@@ -143,11 +135,11 @@ namespace sb
         IoArena io;
         std::mutex mu;
         // cross-stream ordering of calls that share the scratch arenas (sb_api.cu: StreamOrder)
-        cudaEvent_t order_event = nullptr;
+        Event order_event;
         cudaStream_t order_stream = nullptr;
         bool order_valid = false;
 
-        ~Context();
+        ~Context() { cudaSetDevice(device); } // the members free their memory on this device
         void *ensure_scratch(size_t bytes);
         void *ensure_aux(size_t bytes);
         // secret-dependent intermediates (decryption phases, encryption noise) do not stay in the arenas: the reference keeps them in
@@ -157,6 +149,19 @@ namespace sb
         const uint32_t *galois_table(uint32_t elt);
         size_t prime_id_aux(size_t aux_index) const { return k + aux_index; }
     };
+
+    // a host array as a device table of the context, counted in table_bytes.  T is the device type of the same bytes (Tw for
+    // sbh::TwPair, uint2 for pairs of uint32_t, ...)
+    template <class T, class S>
+    DevBuf<T> upload(Context &c, const std::vector<S> &h)
+    {
+        static_assert(sizeof(T) % sizeof(S) == 0, "layout");
+        DevBuf<T> d(h.size() * sizeof(S) / sizeof(T));
+        if (d)
+            cuda_check(cudaMemcpy(d.get(), h.data(), d.bytes(), cudaMemcpyHostToDevice), "upload table");
+        c.table_bytes += d.bytes();
+        return d;
+    }
 
     std::unique_ptr<Context> make_context(int scheme, size_t n, const u64 *moduli, size_t k, u64 t, int device);
 

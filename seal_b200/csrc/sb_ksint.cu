@@ -815,13 +815,13 @@ namespace sb
     }
     // returns the kernel that ran: 0 register tile, 1 key tile, 2 tensor cores
     template <int LOGN>
-    static int launch_mac(const KsIntScratch &s, const uint32_t *key32, const KsInt &d, int L, int k, int digits, int B, int nbt, int n,
+    static int launch_mac(const KsIntScratch &s, const uint32_t *key32, const KsInt &d, bool mma, int L, int k, int digits, int B, int nbt, int n,
                           cudaStream_t st)
     {
         // below 16 ciphertexts the key tile every CTA stages outweighs the products: the integer kernels take those chunks (H100,
         // n = 65536, 31 digits, ms per multiply + relinearize call with / without the tensor cores: 3.1 / 1.6 at B = 1, 8.1 / 8.2 at
         // B = 15, 8.4 / 9.0 at B = 16)
-        if (d.mac_mma && L <= kMmaMaxDigits && B >= 16)
+        if (mma && L <= kMmaMaxDigits && B >= 16)
         {
             const size_t smem = mac_mma_smem((2 * (L + 1) + 7) / 8);
             cuda_check(cudaFuncSetAttribute(ks32_mac_mma<LOGN>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)), "smem attr");
@@ -844,18 +844,18 @@ namespace sb
         ks32_mac<LOGN><<<grid, 128, kMacSmem, st>>>(s.Dh, key32, s.Acc, d.prm, L, k, digits, B, nbt);
         return 0;
     }
-    static int launch_mac_logn(const KsIntScratch &s, const uint32_t *key32, const KsInt &d, int L, int k, int digits, int B, int nbt, int logn,
-                               cudaStream_t st)
+    static int launch_mac_logn(const KsIntScratch &s, const uint32_t *key32, const KsInt &d, bool mma, int L, int k, int digits, int B, int nbt,
+                               int logn, cudaStream_t st)
     {
         const int n = 1 << logn;
         switch (logn)
         {
-        case 12: return launch_mac<12>(s, key32, d, L, k, digits, B, nbt, n, st);
-        case 13: return launch_mac<13>(s, key32, d, L, k, digits, B, nbt, n, st);
-        case 14: return launch_mac<14>(s, key32, d, L, k, digits, B, nbt, n, st);
-        case 15: return launch_mac<15>(s, key32, d, L, k, digits, B, nbt, n, st);
-        case 16: return launch_mac<16>(s, key32, d, L, k, digits, B, nbt, n, st);
-        case 17: return launch_mac<17>(s, key32, d, L, k, digits, B, nbt, n, st);
+        case 12: return launch_mac<12>(s, key32, d, mma, L, k, digits, B, nbt, n, st);
+        case 13: return launch_mac<13>(s, key32, d, mma, L, k, digits, B, nbt, n, st);
+        case 14: return launch_mac<14>(s, key32, d, mma, L, k, digits, B, nbt, n, st);
+        case 15: return launch_mac<15>(s, key32, d, mma, L, k, digits, B, nbt, n, st);
+        case 16: return launch_mac<16>(s, key32, d, mma, L, k, digits, B, nbt, n, st);
+        case 17: return launch_mac<17>(s, key32, d, mma, L, k, digits, B, nbt, n, st);
         default: throw std::logic_error("unsupported transform size");
         }
     }
@@ -1076,9 +1076,9 @@ namespace sb
     static void launch_crt_logn(const CrtArgs &A, const KsInt &d, bool fuse, size_t B, cudaStream_t st)
     {
         if (fuse)
-            ks32_crt_kernel<MODE, LOGN, true><<<static_cast<unsigned>(B * 2 * 32), 128, 0, st>>>(A, d.prm, d.d_inv_outer);
+            ks32_crt_kernel<MODE, LOGN, true><<<static_cast<unsigned>(B * 2 * 32), 128, 0, st>>>(A, d.prm, d.d_inv_outer.get());
         else
-            ks32_crt_kernel<MODE, LOGN, false><<<static_cast<unsigned>((A.total + 255) / 256), 256, 0, st>>>(A, d.prm, d.d_inv_outer);
+            ks32_crt_kernel<MODE, LOGN, false><<<static_cast<unsigned>((A.total + 255) / 256), 256, 0, st>>>(A, d.prm, d.d_inv_outer.get());
     }
     template <int MODE>
     static void launch_crt(const CrtArgs &A, const KsInt &d, bool fuse, size_t B, int logn, cudaStream_t st)
@@ -1180,14 +1180,14 @@ namespace sb
     {
         if (top)
         {
-            ks32_crt_kernel<MODE, LOGNA + kLocalLog, true, true><<<static_cast<unsigned>(B * 2 * 32), 128, 0, st>>>(A, d.prm, d.d_inv_outer);
+            ks32_crt_kernel<MODE, LOGNA + kLocalLog, true, true><<<static_cast<unsigned>(B * 2 * 32), 128, 0, st>>>(A, d.prm, d.d_inv_outer.get());
             return;
         }
         auto kern = fast ? ks32_inv_crt_ntt<MODE, LOGNA, true> : ks32_inv_crt_ntt<MODE, LOGNA, false>;
         const size_t smem = crt_ntt_smem<LOGNA>(d.prm.S);
         cuda_check(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)), "smem attr");
         const dim3 grid(static_cast<unsigned>(B * 2 * A.L), static_cast<unsigned>((1 << kLocalLog) / (kTile >> LOGNA)));
-        kern<<<grid, kColThreads, smem, st>>>(A, d.prm, d.d_inv_outer, mid);
+        kern<<<grid, kColThreads, smem, st>>>(A, d.prm, d.d_inv_outer.get(), mid);
     }
     // top: the special prime's value (ks32_crt_kernel<..., TOP = true>); otherwise ks32_inv_crt_ntt into mid.  n = 8192 .. 65536
     template <int MODE>
@@ -1256,16 +1256,6 @@ namespace sb
     };
 
     // ------------------------------------------------------------------------------------------------ host side ----
-    template <class T>
-    static T *upload(const std::vector<T> &v, size_t &bytes)
-    {
-        T *d = nullptr;
-        cuda_check(cudaMalloc(reinterpret_cast<void **>(&d), std::max<size_t>(1, v.size()) * sizeof(T)), "cudaMalloc(ksint table)");
-        cuda_check(cudaMemcpy(d, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice), "upload ksint table");
-        bytes += v.size() * sizeof(T);
-        return d;
-    }
-
     void ksint_init(Context &c)
     {
         c.ksint.ready = false;
@@ -1284,17 +1274,17 @@ namespace sb
             d.prm.red[t] = make_uint2(h.red[2 * t], h.red[2 * t + 1]);
             d.prm.c1[t] = make_uint2(h.c1[2 * t], h.c1[2 * t + 1]);
         }
-        d.d_fwd_outer = reinterpret_cast<uint2 *>(upload(h.fwd_outer, c.table_bytes));
-        d.d_inv_outer = reinterpret_cast<uint2 *>(upload(h.inv_outer, c.table_bytes));
-        d.d_fwd_local = reinterpret_cast<uint2 *>(upload(h.fwd_local, c.table_bytes));
-        d.d_inv_local = reinterpret_cast<uint2 *>(upload(h.inv_local, c.table_bytes));
-        d.d_punct = upload(h.punct_mod_q, c.table_bytes);
-        d.d_neg = upload(h.neg_mod_q, c.table_bytes);
+        d.d_fwd_outer = upload<uint2>(c, h.fwd_outer);
+        d.d_inv_outer = upload<uint2>(c, h.inv_outer);
+        d.d_fwd_local = upload<uint2>(c, h.fwd_local);
+        d.d_inv_local = upload<uint2>(c, h.inv_local);
+        d.d_punct = upload<u64>(c, h.punct_mod_q);
+        d.d_neg = upload<u64>(c, h.neg_mod_q);
         {
             std::vector<u64> hm(c.k);
             for (size_t i = 0; i < c.k; i++)
                 hm[i] = (c.q[c.k - 1] >> 1) % c.q[i];
-            d.d_half_mod = upload(hm, c.table_bytes);
+            d.d_half_mod = upload<u64>(c, hm);
         }
         cuda_check(cudaFuncSetAttribute(ks32_fwd_local, cudaFuncAttributeMaxDynamicSharedMemorySize, kKsLocalSmem), "smem attr");
         cuda_check(cudaFuncSetAttribute(ks32_inv_local, cudaFuncAttributeMaxDynamicSharedMemorySize, kKsLocalSmem), "smem attr");
@@ -1307,12 +1297,6 @@ namespace sb
         if (const char *e = std::getenv("SB200_KS_MAC_MMA"))
             d.mac_mma = std::atoi(e) != 0;
         d.ready = true;
-    }
-    void ksint_free(Context &c)
-    {
-        KsInt &d = c.ksint;
-        cudaFree(d.d_fwd_outer), cudaFree(d.d_inv_outer), cudaFree(d.d_fwd_local), cudaFree(d.d_inv_local), cudaFree(d.d_punct), cudaFree(d.d_neg), cudaFree(d.d_half_mod);
-        d = KsInt{};
     }
 
     // the digit slab holds ceil(B / TB) * TB ciphertexts (register tiles of the product kernel); the per-ciphertext figure counts one
@@ -1342,12 +1326,12 @@ namespace sb
         const unsigned grid = static_cast<unsigned>(rows) * 16u;
         switch (d.prm.r)
         {
-        case 0: ks32_fwd_outer<0, PLAIN><<<grid, 256, 0, st>>>(dsrc, L, c.d_primes, d.prm, d.d_fwd_outer, Dh, map); break;
-        case 1: ks32_fwd_outer<1, PLAIN><<<grid, 256, 0, st>>>(dsrc, L, c.d_primes, d.prm, d.d_fwd_outer, Dh, map); break;
-        case 2: ks32_fwd_outer<2, PLAIN><<<grid, 256, 0, st>>>(dsrc, L, c.d_primes, d.prm, d.d_fwd_outer, Dh, map); break;
-        case 3: ks32_fwd_outer<3, PLAIN><<<grid, 256, 0, st>>>(dsrc, L, c.d_primes, d.prm, d.d_fwd_outer, Dh, map); break;
-        case 4: ks32_fwd_outer<4, PLAIN><<<grid, 256, 0, st>>>(dsrc, L, c.d_primes, d.prm, d.d_fwd_outer, Dh, map); break;
-        case 5: ks32_fwd_outer<5, PLAIN><<<grid, 256, 0, st>>>(dsrc, L, c.d_primes, d.prm, d.d_fwd_outer, Dh, map); break;
+        case 0: ks32_fwd_outer<0, PLAIN><<<grid, 256, 0, st>>>(dsrc, L, c.d_primes.get(), d.prm, d.d_fwd_outer.get(), Dh, map); break;
+        case 1: ks32_fwd_outer<1, PLAIN><<<grid, 256, 0, st>>>(dsrc, L, c.d_primes.get(), d.prm, d.d_fwd_outer.get(), Dh, map); break;
+        case 2: ks32_fwd_outer<2, PLAIN><<<grid, 256, 0, st>>>(dsrc, L, c.d_primes.get(), d.prm, d.d_fwd_outer.get(), Dh, map); break;
+        case 3: ks32_fwd_outer<3, PLAIN><<<grid, 256, 0, st>>>(dsrc, L, c.d_primes.get(), d.prm, d.d_fwd_outer.get(), Dh, map); break;
+        case 4: ks32_fwd_outer<4, PLAIN><<<grid, 256, 0, st>>>(dsrc, L, c.d_primes.get(), d.prm, d.d_fwd_outer.get(), Dh, map); break;
+        case 5: ks32_fwd_outer<5, PLAIN><<<grid, 256, 0, st>>>(dsrc, L, c.d_primes.get(), d.prm, d.d_fwd_outer.get(), Dh, map); break;
         default: throw std::logic_error("unsupported transform size");
         }
     }
@@ -1371,7 +1355,7 @@ namespace sb
         dim3 grid(static_cast<unsigned>((map.rows_out + kRowsPerCta - 1) / kRowsPerCta), static_cast<unsigned>(d.prm.S << d.prm.r));
         c.stats.begin("ks32_fwd_local", 0, rows * n * 8.0 * S, st, 0, 0);
         c.stats.work32(0.5 * rows * n * S * 12, 0);
-        ks32_fwd_local<<<grid, 256, kKsLocalSmem, st>>>(Dh, map.rows_out, 1, map.rows_out, d.prm, d.d_fwd_local);
+        ks32_fwd_local<<<grid, 256, kKsLocalSmem, st>>>(Dh, map.rows_out, 1, map.rows_out, d.prm, d.d_fwd_local.get());
         c.stats.end(st);
         cuda_check(cudaGetLastError(), "ks32_fwd_local");
     }
@@ -1382,35 +1366,29 @@ namespace sb
             return;
         const size_t rows = key.digits * 2 * c.k, words = rows * c.n, S = c.ksint.prm.S;
         // + 8 rows: the last register tile of the product kernel may read (and discard) up to 7 rows past the end
-        cuda_check(cudaMalloc(reinterpret_cast<void **>(&key.d_key32), (S * words + 8 * c.n) * sizeof(uint32_t)), "cudaMalloc(key, auxiliary primes)");
-        cuda_check(cudaMemsetAsync(key.d_key32 + S * words, 0, 8 * c.n * sizeof(uint32_t), st), "memset");
+        DevBuf<uint32_t> key32(S * words + 8 * c.n);
+        cuda_check(cudaMemsetAsync(key32.get() + S * words, 0, 8 * c.n * sizeof(uint32_t), st), "memset");
         // coefficient form of every key row (row % k = its prime), then the digit path's forward transforms: khat[t][row][n]
-        u64 *tmp = nullptr;
-        cuda_check(cudaMalloc(reinterpret_cast<void **>(&tmp), words * sizeof(u64)), "cudaMalloc(key staging)");
-        const bool prof = c.stats.profiling; // a one-time conversion: not part of any timed operation
+        DevBuf<u64> tmp(words);
+        struct Quiet // a one-time conversion, not part of any timed operation: no profile records until the scope ends
+        {
+            LaunchStats &s;
+            bool prof;
+            ~Quiet() { s.profiling = prof; }
+        } quiet{ c.stats, c.stats.profiling };
         c.stats.profiling = false;
-        try
-        {
-            cuda_check(cudaMemcpyAsync(tmp, key.d_key, words * sizeof(u64), cudaMemcpyDeviceToDevice, st), "key copy");
-            op_ntt(c, true, c.k, 2, key.digits, tmp, st);
-            ksint_forward(c, Src{ tmp, 0, nullptr, 0, c.logn }, static_cast<int>(rows), static_cast<int>(rows), key.d_key32,
-                          RowMap{ 2, static_cast<int>(c.k), static_cast<int>(rows) }, st);
-            cuda_check(cudaStreamSynchronize(st), "synchronize");
-        }
-        catch (...)
-        {
-            c.stats.profiling = prof;
-            cudaFree(tmp); // the key's own buffers belong to the handle and go with it
-            throw;
-        }
-        c.stats.profiling = prof;
-        cuda_check(cudaFree(tmp), "cudaFree(key staging)");
+        cuda_check(cudaMemcpyAsync(tmp.get(), key.d_key.get(), words * sizeof(u64), cudaMemcpyDeviceToDevice, st), "key copy");
+        op_ntt(c, true, c.k, 2, key.digits, tmp.get(), st);
+        ksint_forward(c, Src{ tmp.get(), 0, nullptr, 0, c.logn }, static_cast<int>(rows), static_cast<int>(rows), key32.get(),
+                      RowMap{ 2, static_cast<int>(c.k), static_cast<int>(rows) }, st);
+        cuda_check(cudaStreamSynchronize(st), "synchronize");
+        key.d_key32 = std::move(key32);
     }
 
     template <int R>
     static void launch_inv_outer_r(uint32_t *data, unsigned grid, const KsInt &d, cudaStream_t st)
     {
-        ks32_inv_outer<R><<<grid, 256, 0, st>>>(data, d.prm, d.d_inv_outer);
+        ks32_inv_outer<R><<<grid, 256, 0, st>>>(data, d.prm, d.d_inv_outer.get());
     }
 
     static void launch_inverse(Context &c, uint32_t *data, int arows, cudaStream_t st, bool outer = true);
@@ -1419,12 +1397,12 @@ namespace sb
     static void launch_intt_fwd_outer_logna(Context &c, const OpKsIntt &op, int rows, uint32_t *Dh, RowMap map, cudaStream_t st)
     {
         const dim3 grid(static_cast<unsigned>(rows), static_cast<unsigned>((1 << kLocalLog) / (kTile >> LOGNA)));
-        ks32_intt_fwd_outer<LOGNA><<<grid, kColThreads, 0, st>>>(op, c.d_primes, c.ksint.prm, c.ksint.d_fwd_outer, Dh, map);
+        ks32_intt_fwd_outer<LOGNA><<<grid, kColThreads, 0, st>>>(op, c.d_primes.get(), c.ksint.prm, c.ksint.d_fwd_outer.get(), Dh, map);
     }
     // the target's inverse transforms (CKKS / BGV: NTT form); fused: their column passes end in the forward outer pass
     static void ksint_target_intt(Context &c, const OpKsIntt &op, int rows, uint32_t *Dh, RowMap map, bool fused, cudaStream_t st)
     {
-        cuda_check(launch_ntt_inv(op, rows, c.logn, c.d_primes, st, c.stats, "ks_target_intt", -1, fused), "ks intt");
+        cuda_check(launch_ntt_inv(op, rows, c.logn, c.d_primes.get(), st, c.stats, "ks_target_intt", -1, fused), "ks intt");
         if (!fused)
             return;
         const double n = static_cast<double>(c.n), S = c.ksint.prm.S;
@@ -1470,7 +1448,7 @@ namespace sb
             // one pass over the key + the transformed digits in, the sums out
             c.stats.begin("ks32_mac", 0, 4.0 * n * S * (static_cast<double>(Li) * 2 * (Li + 1) + rows + arows), st);
             // integer-pipe multiply-accumulates only: the tensor-core kernel's products are not work against the mac32 ceiling (DESIGN 4)
-            if (launch_mac_logn(s, key.d_key32, d, Li, ki, static_cast<int>(key.digits), Bi, nbt, static_cast<int>(c.logn), st) != 2)
+            if (launch_mac_logn(s, key.d_key32.get(), d, d.mac_mma, Li, ki, static_cast<int>(key.digits), Bi, nbt, static_cast<int>(c.logn), st) != 2)
                 c.stats.work32(0, static_cast<double>(arows) * Li * S * n);
             c.stats.end(st);
             cuda_check(cudaGetLastError(), "ks32_mac");
@@ -1483,14 +1461,14 @@ namespace sb
             o_bs = 2 * o_ps;
         {
             CrtArgs A{};
-            A.Acc = s.Acc, A.punct = d.d_punct, A.neg = d.d_neg, A.primes = c.d_primes;
-            A.inv_top = c.d_invq + (c.k - 1) * c.k;
-            A.half_mod = d.d_half_mod;
+            A.Acc = s.Acc, A.punct = d.d_punct.get(), A.neg = d.d_neg.get(), A.primes = c.d_primes.get();
+            A.inv_top = c.d_invq.get() + (c.k - 1) * c.k;
+            A.half_mod = d.d_half_mod.get();
             A.R = s.R, A.out = out, A.o_bs = o_bs, A.o_ps = o_ps, A.base = base, A.L = Li, A.k = ki;
             A.total = static_cast<long long>(B) * 2 * c.n;
             if (c.scheme == 3)
             {
-                A.qtop_mod = c.d_qmod + (c.k - 1) * c.k;
+                A.qtop_mod = c.d_qmod.get() + (c.k - 1) * c.k;
                 A.t = c.t, A.t_ratio = c.t_ratio;
                 A.inv_top_mod_t = Tw{ c.inv_q_mod_t[c.k - 1], sbh::shoup(c.inv_q_mod_t[c.k - 1], c.t) };
             }
@@ -1509,7 +1487,7 @@ namespace sb
                 c.stats.end(st);
                 cuda_check(cudaGetLastError(), "ks32_inv_crt_ntt");
                 OpAddBaseFwd op{ s.R, out, o_bs, o_ps, base, c.logn, Li };
-                cuda_check(launch_ntt_fwd(op, static_cast<int>(B * 2 * L), c.logn, c.d_primes, st, c.stats, "ks_result_ntt", -1, c.fast_q, true),
+                cuda_check(launch_ntt_fwd(op, static_cast<int>(B * 2 * L), c.logn, c.d_primes.get(), st, c.stats, "ks_result_ntt", -1, c.fast_q, true),
                            "ks result ntt");
                 return;
             }
@@ -1529,7 +1507,7 @@ namespace sb
         if (c.scheme != 1)
         {
             OpAddBaseFwd op{ s.R, out, o_bs, o_ps, base, c.logn, Li };
-            cuda_check(launch_ntt_fwd(op, static_cast<int>(B * 2 * L), c.logn, c.d_primes, st, c.stats, "ks_result_ntt", -1, c.fast_q), "ks result ntt");
+            cuda_check(launch_ntt_fwd(op, static_cast<int>(B * 2 * L), c.logn, c.d_primes.get(), st, c.stats, "ks_result_ntt", -1, c.fast_q), "ks result ntt");
         }
     }
 
@@ -1541,7 +1519,7 @@ namespace sb
         dim3 grid(static_cast<unsigned>((arows + kRowsPerCta - 1) / kRowsPerCta), static_cast<unsigned>(S << d.prm.r));
         c.stats.begin("ks32_inv_local", 0, 8.0 * arows * S * n, st);
         c.stats.work32(0.5 * arows * S * n * 12, 0);
-        ks32_inv_local<<<grid, 256, kKsLocalSmem, st>>>(data, arows, S, 1, d.prm, d.d_inv_local);
+        ks32_inv_local<<<grid, 256, kKsLocalSmem, st>>>(data, arows, S, 1, d.prm, d.d_inv_local.get());
         c.stats.end(st);
         cuda_check(cudaGetLastError(), "ks32_inv_local");
         if (d.prm.r > 0 && outer)
@@ -1591,8 +1569,7 @@ namespace sb
             throw std::logic_error("integer key-switching path is not available for this context");
         if (L < 1 || B < 1 || static_cast<size_t>(L) > c.ksint.max_digits)
             throw std::invalid_argument("product: 1 <= L <= max_digits and B >= 1");
-        KsInt d = c.ksint;
-        d.mac_mma = mma != 0;
+        const KsInt &d = c.ksint;
         const size_t S = d.prm.S, n = c.n, Bpad = (B + kMacTB - 1) / kMacTB * kMacTB, k = L + 1;
         const size_t dh_words = S * L * Bpad * n, key_words = S * L * 2 * k * n, acc_words = B * 2 * k * S * n;
         // + 8 key rows of slack, as ksint_prepare_key allocates them
@@ -1606,7 +1583,7 @@ namespace sb
                                 cudaMemcpyHostToDevice), "upload");
         cuda_check(cudaMemcpy(key, h_key, key_words * sizeof(uint32_t), cudaMemcpyHostToDevice), "upload");
         cuda_check(cudaMemset(key + key_words, 0, 8 * n * sizeof(uint32_t)), "memset");
-        const int ran = launch_mac_logn(s, key, d, L, static_cast<int>(k), L, B, static_cast<int>(Bpad / kMacTB), static_cast<int>(c.logn), nullptr);
+        const int ran = launch_mac_logn(s, key, d, mma != 0, L, static_cast<int>(k), L, B, static_cast<int>(Bpad / kMacTB), static_cast<int>(c.logn), nullptr);
         cuda_check(cudaGetLastError(), "ks32_mac");
         cuda_check(cudaMemcpy(h_Acc, s.Acc, acc_words * sizeof(uint32_t), cudaMemcpyDeviceToHost), "download");
         return ran;

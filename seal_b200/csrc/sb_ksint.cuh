@@ -14,6 +14,7 @@
 // the 64-bit one, and the L (L+1) digit transforms become S L forward + 2 S (L+1) inverse small ones.  Results are word-identical
 // to the reference (same residues mod q_I), which the parity tests check against the reference itself.
 #pragma once
+#include "sb_mem.cuh"
 #include "sb_src.cuh"
 #include <cstddef>
 #include <cstdint>
@@ -41,10 +42,10 @@ namespace sb
         bool fuse_ntt = true;  // entry and exit inside the column passes of the 64-bit transforms (env SB200_KS_FUSE_NTT)
         size_t max_digits = 0; // sbh::KsIntHost::max_digits (64 at n = 4096)
         KsIntParams prm;
-        uint2 *d_fwd_outer = nullptr, *d_inv_outer = nullptr; // [S][2^r]
-        uint2 *d_fwd_local = nullptr, *d_inv_local = nullptr; // [S][2^r][4096]
-        u64 *d_punct = nullptr, *d_neg = nullptr;              // [k][S]
-        u64 *d_half_mod = nullptr;                             // [k]: floor(q_special / 2) mod q_i
+        DevBuf<uint2> d_fwd_outer, d_inv_outer; // [S][2^r]
+        DevBuf<uint2> d_fwd_local, d_inv_local; // [S][2^r][4096]
+        DevBuf<u64> d_punct, d_neg;             // [k][S]
+        DevBuf<u64> d_half_mod;                 // [k]: floor(q_special / 2) mod q_i
     };
 
     // per-ciphertext scratch of the integer path (bytes): digits' transforms, accumulated products, coefficient-form result
@@ -59,7 +60,6 @@ namespace sb
     KsIntScratch ksint_carve(const Context &c, size_t L, size_t B, void *base);
 
     void ksint_init(Context &c);
-    void ksint_free(Context &c);
     // khat[t][J][c][ki][n] from the uploaded key [digits][2][k][n]
     void ksint_prepare_key(Context &c, KSwitchKey &key, cudaStream_t st);
     // target (CKKS / BGV: NTT form, BFV: coefficient form) -> out = base + key-switched polynomials; D: [B][L][n] scratch of the

@@ -365,7 +365,7 @@ namespace sb
                 continue; // more rejections than spare words (probability far below 2^-40 at the first attempt): take more
             const long long total = need * static_cast<long long>(B);
             c.stats.begin("seed_reduce", 0, 16.0 * total, st);
-            seed_reduce_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(W, words_per_ct, d_out, d_off, c.d_primes, c.logn,
+            seed_reduce_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(W, words_per_ct, d_out, d_off, c.d_primes.get(), c.logn,
                                                                                            static_cast<int>(L), total);
             c.stats.end(st);
             cuda_check(cudaGetLastError(), "seed_reduce_kernel");
@@ -498,12 +498,12 @@ namespace sb
             cuda_check(cudaMemcpyAsync(h_public_seeds, d_pub, B * 8 * sizeof(u64), cudaMemcpyDeviceToHost, st), "public seeds D2H");
         const unsigned grid = static_cast<unsigned>((total + 255) / 256);
         const unsigned char *boot = reinterpret_cast<const unsigned char *>(Wb);
-        const u64 *s = sk.d_pow; // s^1, [k][n] at the key level: the first L rows are the level's primes
+        const u64 *s = sk.d_pow.get(); // s^1, [k][n] at the key level: the first L rows are the level's primes
         const int logn = c.logn, Li = static_cast<int>(L);
         const KsFactor f = ks ? *ks : KsFactor{};
 #define SB_ENC(MODE, name)                                                                                           \
     c.stats.begin(name, 0, 24.0 * total, st);                                                                         \
-    enc_kernel<MODE><<<grid, 256, 0, st>>>(d_out, tmp, s, boot, boot_bytes, mult, f, c.d_primes, logn, Li, total);    \
+    enc_kernel<MODE><<<grid, 256, 0, st>>>(d_out, tmp, s, boot, boot_bytes, mult, f, c.d_primes.get(), logn, Li, total);    \
     c.stats.end(st);                                                                                                  \
     cuda_check(cudaGetLastError(), name);
         if (is_ntt_form)
@@ -587,11 +587,11 @@ namespace sb
         check_key(c, sk, boot_prng, ct_prng);
         KsFactor f{};
         if (galois_elt)
-            f.new_key = sk.d_pow, f.perm = c.galois_table(galois_elt);
+            f.new_key = sk.d_pow.get(), f.perm = c.galois_table(galois_elt);
         else
         {
             ensure_key_powers(c, sk, 2, st);
-            f.new_key = sk.d_pow + c.k * c.n;
+            f.new_key = sk.d_pow.get() + c.k * c.n;
         }
         const size_t digits = c.k - 1, poly = c.k * c.n;
         // per digit: the noise / product polynomial (aux arena) and the c_1 stream (scratch arena, expand_impl), plus the bootstrap stream
@@ -707,17 +707,11 @@ namespace sb
 
     void public_key_create(Context &c, const u64 *h_pk, PublicKey &out)
     {
-        const size_t words = 2 * c.k * c.n;
-        std::vector<u64> rows(c.k);
-        cuda_check(cudaMalloc(&out.d_key, words * sizeof(u64)), "cudaMalloc(public key)");
+        out.d_key = DevBuf<u64>(2 * c.k * c.n);
         out.ctx = &c;
-        cuda_check(cudaMemcpy(out.d_key, h_pk, words * sizeof(u64), cudaMemcpyHostToDevice), "upload public key");
-        if (!op_residues_in_range(c, c.k, 2 * c.k, out.d_key, nullptr))
-        {
-            cudaFree(out.d_key);
-            out.d_key = nullptr;
+        cuda_check(cudaMemcpy(out.d_key.get(), h_pk, out.d_key.bytes(), cudaMemcpyHostToDevice), "upload public key");
+        if (!op_residues_in_range(c, c.k, 2 * c.k, out.d_key.get(), nullptr))
             throw std::invalid_argument("public key is not valid for encryption parameters");
-        }
     }
 
     // h_seeds [B][8]: the seed of each ciphertext's PRNG; d_out [B][2][L][n] at the level with L primes (L == k: the key level)
@@ -759,8 +753,8 @@ namespace sb
         const long long bn = static_cast<long long>(B) * n;
         const int logn = c.logn, Lpi = static_cast<int>(Lp);
         c.stats.begin("enc_ternary", 0, (4.0 + 8.0 * Lp) * bn, st);
-        enc_ternary_kernel<<<static_cast<unsigned>((bn + 255) / 256), 256, 0, st>>>(W, words, U, d_pos, c.d_primes, logn, Lpi, bn);
-        enc_ternary_fix_kernel<<<static_cast<unsigned>(B), 32, 0, st>>>(W, words, U, d_pos, c.d_primes, logn, Lpi, d_over);
+        enc_ternary_kernel<<<static_cast<unsigned>((bn + 255) / 256), 256, 0, st>>>(W, words, U, d_pos, c.d_primes.get(), logn, Lpi, bn);
+        enc_ternary_fix_kernel<<<static_cast<unsigned>(B), 32, 0, st>>>(W, words, U, d_pos, c.d_primes.get(), logn, Lpi, d_over);
         c.stats.end(st);
         cuda_check(cudaGetLastError(), "enc_ternary_kernel");
         op_ntt(c, false, Lp, 1, B, U, st);
@@ -768,7 +762,7 @@ namespace sb
         const unsigned grid = static_cast<unsigned>((total2 + 255) / 256);
 #define SB_ENC(MODE, name)                                                                                                          \
     c.stats.begin(name, 0, 24.0 * total2, st);                                                                                       \
-    enc_pk_kernel<MODE><<<grid, 256, 0, st>>>(dst, U, pk.d_key, pk_poly, W, words, d_pos, mult, c.d_primes, logn, Lpi, total2);      \
+    enc_pk_kernel<MODE><<<grid, 256, 0, st>>>(dst, U, pk.d_key.get(), pk_poly, W, words, d_pos, mult, c.d_primes.get(), logn, Lpi, total2);      \
     c.stats.end(st);                                                                                                                 \
     cuda_check(cudaGetLastError(), name);
         if (c.scheme != 1 /* CKKS, BGV */)
