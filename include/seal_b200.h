@@ -216,6 +216,28 @@ int sb200_add_plain_coeff(sb200_context *ctx, size_t L, size_t size, size_t batc
  * (t prime, t = 1 mod 2n: "encryption parameters are not valid for batching" otherwise).  No aliasing. */
 int sb200_batch_encode(sb200_context *ctx, size_t batch, const uint64_t *d_values, uint64_t *d_plain, void *stream);
 int sb200_batch_decode(sb200_context *ctx, size_t batch, const uint64_t *d_plain, uint64_t *d_values, void *stream);
+/* ---- plaintext operations with plain_count plaintexts: plain_count = batch (one per ciphertext, as the three entry points above)
+ * or 1 (one plaintext for the whole batch: a weight, a constant, a mask; it is read, and a coefficient-form one lifted and
+ * transformed, once per stream call, and once per staging chunk in the _host forms, which upload it once per call).  Any other plain_count is SB200_E_INVALID_ARG.  The ciphertext may be updated in place
+ * (d_out = d_a); a shared plaintext must not alias d_out (SB200_E_INVALID_ARG when d_out == d_plain).
+ * sb200_multiply_plain with d_plain [plain_count][L][n] (evaluator.cpp:1975-2019, multiply_plain_ntt :2157-2195). */
+int sb200_multiply_plain_n(sb200_context *ctx, size_t L, size_t size, size_t batch, size_t plain_count, const uint64_t *d_a,
+                           const uint64_t *d_plain, uint64_t *d_out, void *stream);
+/* sb200_multiply_plain_coeff with d_plain [plain_count][n] (multiply_plain_normal :2021-2155; transform_to_ntt_inplace(Plaintext&)
+ * :2196-2287 then multiply_plain_ntt for NTT-form ciphertexts) */
+int sb200_multiply_plain_coeff_n(sb200_context *ctx, size_t L, size_t size, size_t batch, size_t plain_count, int ct_is_ntt,
+                                 const uint64_t *d_a, const uint64_t *d_plain, uint64_t *d_out, void *stream);
+/* sb200_add_plain_coeff with d_plain [plain_count][n] (add_plain_inplace :1759-1866, sub_plain_inplace :1867-1974).
+ * h_correction_factors: one BGV correction factor per plaintext ([plain_count] host words), or NULL (= 1); with a shared
+ * plaintext it is the single correction factor of the batch. */
+int sb200_add_plain_coeff_n(sb200_context *ctx, size_t L, size_t size, size_t batch, size_t plain_count, int subtract, const uint64_t *d_a,
+                            const uint64_t *d_plain, const uint64_t *h_correction_factors, uint64_t *d_out, void *stream);
+/* CKKS Evaluator::add_plain / sub_plain (add_plain_inplace :1759-1866, sub_plain_inplace :1867-1974): c_0 +/- the NTT-form
+ * plaintext d_plain [plain_count][L][n] at the ciphertext's level (add_poly_coeffmod / sub_poly_coeffmod); c_1.. are copied
+ * (in place: only c_0 is read and written).  The caller checks parms_id and scale as the reference does.  A BFV or BGV
+ * context is SB200_E_INVALID_ARG ("BFV plain cannot be in NTT form" / "BGV plain cannot be in NTT form"). */
+int sb200_add_plain_ntt(sb200_context *ctx, size_t L, size_t size, size_t batch, size_t plain_count, int subtract, const uint64_t *d_a,
+                        const uint64_t *d_plain, uint64_t *d_out, void *stream);
 /* Evaluator::relinearize_inplace, size 3 -> 2 (evaluator.cpp:1144-1199 + 2561-2867) */
 int sb200_relinearize(sb200_context *ctx, size_t L, size_t batch, const uint64_t *d_in3,
                       const sb200_kswitch_key *relin_key, uint64_t *d_out2, void *stream);
@@ -257,6 +279,14 @@ int sb200_multiply_plain_coeff_host(sb200_context *ctx, size_t L, size_t size, s
                                     const uint64_t *h_plain, uint64_t *h_out);
 int sb200_add_plain_coeff_host(sb200_context *ctx, size_t L, size_t size, size_t batch, int subtract, const uint64_t *h_a,
                                const uint64_t *h_plain, const uint64_t *h_correction_factors, uint64_t *h_out);
+int sb200_multiply_plain_n_host(sb200_context *ctx, size_t L, size_t size, size_t batch, size_t plain_count, const uint64_t *h_a,
+                                const uint64_t *h_plain, uint64_t *h_out);
+int sb200_multiply_plain_coeff_n_host(sb200_context *ctx, size_t L, size_t size, size_t batch, size_t plain_count, int ct_is_ntt,
+                                      const uint64_t *h_a, const uint64_t *h_plain, uint64_t *h_out);
+int sb200_add_plain_coeff_n_host(sb200_context *ctx, size_t L, size_t size, size_t batch, size_t plain_count, int subtract,
+                                 const uint64_t *h_a, const uint64_t *h_plain, const uint64_t *h_correction_factors, uint64_t *h_out);
+int sb200_add_plain_ntt_host(sb200_context *ctx, size_t L, size_t size, size_t batch, size_t plain_count, int subtract, const uint64_t *h_a,
+                             const uint64_t *h_plain, uint64_t *h_out);
 int sb200_batch_encode_host(sb200_context *ctx, size_t batch, const uint64_t *h_values, uint64_t *h_plain);
 int sb200_batch_decode_host(sb200_context *ctx, size_t batch, const uint64_t *h_plain, uint64_t *h_values);
 int sb200_relinearize_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *h_in3,

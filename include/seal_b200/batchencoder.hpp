@@ -75,6 +75,43 @@ namespace seal_b200
             }
             run_encode(slots, destination);
         }
+        // ---- device-resident plaintexts: B matrices -> a PlaintextBatch [B][n] in coefficient form, encoded on the device
+        // (sb200_batch_encode).  Each matrix is checked as the single-plaintext overloads above check it.  Build the encoder with the
+        // Evaluator (BatchEncoder(context, evaluator)) for that Evaluator to accept the batch.
+        void encode(const std::vector<std::vector<std::uint64_t>> &values_matrices, PlaintextBatch &destination) const
+        {
+            std::vector<std::uint64_t> slots(values_matrices.size() * slots_, 0);
+            for (std::size_t b = 0; b < values_matrices.size(); b++)
+            {
+                auto &m = values_matrices[b];
+                if (m.size() > slots_)
+                    throw std::invalid_argument("values_matrix size is too large");
+                for (auto v : m)
+                    if (v >= modulus_)
+                        throw std::invalid_argument("input value is larger than plain_modulus");
+                std::copy(m.begin(), m.end(), slots.begin() + b * slots_);
+            }
+            run_encode(slots, values_matrices.size(), destination);
+        }
+        void encode(const std::vector<std::vector<std::int64_t>> &values_matrices, PlaintextBatch &destination) const
+        {
+            std::vector<std::uint64_t> slots(values_matrices.size() * slots_, 0);
+            for (std::size_t b = 0; b < values_matrices.size(); b++)
+            {
+                auto &m = values_matrices[b];
+                if (m.size() > slots_)
+                    throw std::invalid_argument("values_matrix size is too large");
+                for (std::size_t i = 0; i < m.size(); i++)
+                {
+                    const std::int64_t v = m[i];
+                    const std::uint64_t magnitude = v < 0 ? 0 - static_cast<std::uint64_t>(v) : static_cast<std::uint64_t>(v);
+                    if (magnitude > (modulus_ >> 1))
+                        throw std::invalid_argument("input value is larger than plain_modulus");
+                    slots[b * slots_ + i] = v < 0 ? modulus_ + static_cast<std::uint64_t>(v) : static_cast<std::uint64_t>(v);
+                }
+            }
+            run_encode(slots, values_matrices.size(), destination);
+        }
         // batchencoder.cpp:229-266
         void decode(const seal::Plaintext &plain, std::vector<std::uint64_t> &destination,
                     seal::MemoryPoolHandle pool = seal::MemoryManager::GetPool()) const
@@ -121,6 +158,22 @@ namespace seal_b200
             destination.resize(slots_);
             destination.parms_id() = seal::parms_id_zero;
             status(sb200_batch_encode_host(ctx_, 1, slots.data(), destination.data()));
+        }
+        void run_encode(const std::vector<std::uint64_t> &slots, std::size_t B, PlaintextBatch &destination) const
+        {
+            if (!B)
+                throw std::invalid_argument("batch cannot be empty");
+            std::uint64_t *d_values = nullptr;
+            status(sb200_device_malloc(ctx_, slots.size() * sizeof(std::uint64_t), &d_values));
+            int rc = sb200_memcpy_h2d(ctx_, d_values, slots.data(), slots.size() * sizeof(std::uint64_t), nullptr);
+            if (rc == SB200_OK)
+                rc = destination.reserve(ctx_, slots.size());
+            if (rc == SB200_OK)
+                rc = sb200_batch_encode(ctx_, B, d_values, destination.d_, nullptr);
+            sb200_device_free(ctx_, d_values);
+            status(rc);
+            destination.batch_ = B, destination.L_ = 1, destination.n_ = slots_;
+            destination.parms_id_ = seal::parms_id_zero, destination.ntt_ = false, destination.scale_ = 1.0;
         }
         std::vector<std::uint64_t> run_decode(const seal::Plaintext &plain, const seal::MemoryPoolHandle &pool) const
         {

@@ -97,6 +97,44 @@ namespace seal_b200
             }
         }
 
+        // ---- device-resident plaintexts: B vectors -> a PlaintextBatch [B][L][n] in NTT form at parms_id, encoded on the device
+        // (sb200_ckks_encode).  Build the encoder with the Evaluator (CKKSEncoder(context, evaluator)) for that Evaluator to accept it.
+        template <typename T>
+        void encode(const std::vector<std::vector<T>> &values, seal::parms_id_type parms_id, double scale, PlaintextBatch &destination) const
+        {
+            auto cd = context_.get_context_data(parms_id);
+            if (!cd)
+                throw std::invalid_argument("parms_id is not valid for encryption parameters");
+            if (values.empty())
+                throw std::invalid_argument("batch cannot be empty");
+            const std::size_t B = values.size(), L = cd->parms().coeff_modulus().size(), n = slots_ * 2;
+            std::size_t count = 0;
+            for (auto &v : values)
+                count = std::max(count, v.size());
+            if (count > slots_)
+                throw std::invalid_argument("values_size is too large");
+            std::vector<T> flat(B * count, T(0));
+            for (std::size_t b = 0; b < B; b++)
+                std::copy(values[b].begin(), values[b].end(), flat.begin() + b * count);
+            std::uint64_t *d_values = nullptr;
+            int rc = SB200_OK;
+            if (count)
+            {
+                status(sb200_device_malloc(ctx_, flat.size() * sizeof(T), &d_values));
+                rc = sb200_memcpy_h2d(ctx_, d_values, flat.data(), flat.size() * sizeof(T), nullptr);
+            }
+            if (rc == SB200_OK)
+                rc = destination.reserve(ctx_, B * L * n);
+            if (rc == SB200_OK)
+                rc = sb200_ckks_encode(ctx_, L, B, reinterpret_cast<const double *>(d_values), count,
+                                       std::is_same<T, std::complex<double>>::value ? 1 : 0, scale, destination.d_, nullptr);
+            if (d_values)
+                sb200_device_free(ctx_, d_values);
+            status(rc);
+            destination.batch_ = B, destination.L_ = L, destination.n_ = n;
+            destination.parms_id_ = parms_id, destination.ntt_ = true, destination.scale_ = scale;
+        }
+
     private:
         template <typename T>
         void encode_internal(const T *values, std::size_t values_size, seal::parms_id_type parms_id, double scale, seal::Plaintext &destination) const

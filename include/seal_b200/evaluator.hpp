@@ -28,6 +28,8 @@ namespace seal_b200
 {
     class Evaluator;
     class Decryptor;
+    class BatchEncoder;
+    class CKKSEncoder;
 
     // ---- device-resident ciphertexts ---------------------------------------------------------------------------------
     // A batch of B ciphertexts of one shape that stays on the GPU between Evaluator calls.  It carries exactly the metadata
@@ -86,6 +88,75 @@ namespace seal_b200
         bool ntt_ = false;
         double scale_ = 1.0;
         std::uint64_t cf_ = 1;
+    };
+
+    // ---- device-resident plaintexts ----------------------------------------------------------------------------------
+    // B plaintexts of one shape on the GPU, with seal::Plaintext's metadata (plaintext.h: parms_id, zero in coefficient form;
+    // is_ntt_form; scale), shared by all members.  The slab is [B][L][n] in NTT form (Plaintext::data() at that parms_id) or [B][n]
+    // in coefficient form (words below t, zero-padded above coeff_count).  B may be 1: one plaintext applied to every ciphertext
+    // of a CiphertextBatch (the plaintext operations accept B = 1 or B = the ciphertext batch size).  Same ownership rules as
+    // CiphertextBatch: allocated from the Evaluator's context (or an encoder sharing it), movable, not copyable.
+    class PlaintextBatch
+    {
+    public:
+        PlaintextBatch() = default;
+        ~PlaintextBatch() { release(); }
+        PlaintextBatch(const PlaintextBatch &) = delete;
+        PlaintextBatch &operator=(const PlaintextBatch &) = delete;
+        PlaintextBatch(PlaintextBatch &&o) noexcept { *this = std::move(o); }
+        PlaintextBatch &operator=(PlaintextBatch &&o) noexcept
+        {
+            if (this != &o)
+            {
+                release();
+                ctx_ = o.ctx_, d_ = o.d_, cap_ = o.cap_, batch_ = o.batch_, L_ = o.L_, n_ = o.n_;
+                parms_id_ = o.parms_id_, ntt_ = o.ntt_, scale_ = o.scale_;
+                o.ctx_ = nullptr, o.d_ = nullptr, o.cap_ = o.batch_ = o.L_ = o.n_ = 0;
+            }
+            return *this;
+        }
+        std::size_t batch_size() const noexcept { return batch_; }
+        std::size_t coeff_modulus_size() const noexcept { return ntt_ ? L_ : 0; } // primes of an NTT-form plaintext
+        std::size_t poly_modulus_degree() const noexcept { return n_; }
+        const seal::parms_id_type &parms_id() const noexcept { return parms_id_; }
+        bool is_ntt_form() const noexcept { return ntt_; }
+        double scale() const noexcept { return scale_; }
+        std::uint64_t *device_data() noexcept { return d_; }
+        const std::uint64_t *device_data() const noexcept { return d_; }
+        std::size_t words_per_plaintext() const noexcept { return ntt_ ? L_ * n_ : n_; }
+        void release() noexcept
+        {
+            if (d_ && ctx_)
+                sb200_device_free(ctx_, d_);
+            d_ = nullptr, cap_ = 0;
+        }
+
+    private:
+        friend class Evaluator;
+        friend class BatchEncoder;
+        friend class CKKSEncoder;
+        // room for `words` words from the context ctx (a status code of include/seal_b200.h)
+        int reserve(sb200_context *ctx, std::size_t words)
+        {
+            if (ctx_ != ctx)
+            {
+                release();
+                ctx_ = ctx;
+            }
+            if (cap_ >= words)
+                return SB200_OK;
+            release();
+            const int rc = sb200_device_malloc(ctx_, words * sizeof(std::uint64_t), &d_);
+            cap_ = rc == SB200_OK ? words : 0;
+            return rc;
+        }
+        sb200_context *ctx_ = nullptr;
+        std::uint64_t *d_ = nullptr;
+        std::size_t cap_ = 0; // words
+        std::size_t batch_ = 0, L_ = 0, n_ = 0;
+        seal::parms_id_type parms_id_ = seal::parms_id_zero;
+        bool ntt_ = false;
+        double scale_ = 1.0;
     };
 
     class Evaluator
@@ -973,6 +1044,142 @@ namespace seal_b200
             check(sb200_ntt_inverse(ctx_, encrypted_ntt.L_, encrypted_ntt.size_, encrypted_ntt.batch_, encrypted_ntt.d_, nullptr));
             encrypted_ntt.ntt_ = false;
         }
+        // ---- device-resident plaintexts (PlaintextBatch): the same checks, exception types and metadata updates as the
+        // seal::Plaintext overloads above, all made before anything is written; between upload and download only the stream
+        // entry points run.  A PlaintextBatch of size 1 is applied to every ciphertext of the batch (read once per call).
+        void upload(const std::vector<seal::Plaintext> &plains, PlaintextBatch &destination) const
+        {
+            upload(plains.data(), plains.size(), destination);
+        }
+        void upload(const seal::Plaintext *first, std::size_t count, PlaintextBatch &destination) const
+        {
+            if (!first || !count)
+                throw std::invalid_argument("batch cannot be empty");
+            const seal::Plaintext &f = first[0];
+            for (std::size_t i = 0; i < count; i++)
+            {
+                const seal::Plaintext &p = first[i];
+                if (!seal::is_metadata_valid_for(p, context_) || !seal::is_buffer_valid(p))
+                    throw std::invalid_argument("plain is not valid for encryption parameters");
+                const double s1 = p.scale(), s2 = f.scale();
+                if (p.parms_id() != f.parms_id() || std::memcmp(&s1, &s2, sizeof(double)) != 0)
+                    throw std::invalid_argument("batch members must share parms_id, NTT form and scale");
+            }
+            const bool ntt = f.is_ntt_form();
+            const std::size_t n = context_.first_context_data()->parms().poly_modulus_degree();
+            const std::size_t L = ntt ? context_.get_context_data(f.parms_id())->parms().coeff_modulus().size() : 1, words = L * n;
+            std::vector<std::uint64_t> flat(count * words, 0); // coefficient form: zero above coeff_count
+            for (std::size_t i = 0; i < count; i++)
+                std::copy_n(first[i].data(), std::min(first[i].coeff_count(), words), flat.data() + i * words);
+            std::lock_guard<std::mutex> lock(mu_);
+            check(destination.reserve(ctx_, flat.size()));
+            check(sb200_memcpy_h2d(ctx_, destination.d_, flat.data(), flat.size() * sizeof(std::uint64_t), nullptr));
+            destination.batch_ = count, destination.L_ = L, destination.n_ = n;
+            destination.parms_id_ = f.parms_id(), destination.ntt_ = ntt, destination.scale_ = f.scale();
+        }
+        void download(const PlaintextBatch &source, std::vector<seal::Plaintext> &plains) const
+        {
+            owned(source);
+            const std::size_t words = source.words_per_plaintext();
+            std::vector<std::uint64_t> flat(source.batch_ * words);
+            check(sb200_memcpy_d2h(ctx_, flat.data(), source.d_, flat.size() * sizeof(std::uint64_t), nullptr));
+            check(sb200_stream_synchronize(ctx_, nullptr));
+            plains.resize(source.batch_);
+            for (std::size_t i = 0; i < source.batch_; i++)
+            {
+                plains[i].parms_id() = seal::parms_id_zero;
+                plains[i].resize(words);
+                std::copy_n(flat.data() + i * words, words, plains[i].data());
+                plains[i].parms_id() = source.parms_id_;
+                plains[i].scale() = source.scale_;
+            }
+        }
+        // transform_to_ntt_inplace(Plaintext&, parms_id) (evaluator.cpp:2196-2287)
+        void transform_to_ntt_inplace(PlaintextBatch &plain, seal::parms_id_type parms_id) const
+        {
+            owned(plain);
+            auto cd = context_.get_context_data(parms_id);
+            if (!cd)
+                throw std::invalid_argument("parms_id is not valid for the current context");
+            if (plain.ntt_)
+                throw std::invalid_argument("plain is already in NTT form");
+            const std::size_t L = cd->parms().coeff_modulus().size();
+            std::lock_guard<std::mutex> lock(mu_);
+            PlaintextBatch out;
+            check(out.reserve(ctx_, plain.batch_ * L * plain.n_));
+            check(sb200_plain_to_ntt(ctx_, L, plain.batch_, plain.d_, out.d_, nullptr));
+            std::swap(plain.d_, out.d_), std::swap(plain.cap_, out.cap_);
+            plain.L_ = L, plain.ntt_ = true, plain.parms_id_ = parms_id;
+        }
+        // mod_switch_to_next_inplace / mod_switch_to_inplace(Plaintext&) (evaluator.cpp:1369-1402, :1475-1501): NTT-form plaintexts
+        // lose their last prime -- a 2-D copy of the first L - 1 rows of every plaintext
+        void mod_switch_to_next_inplace(PlaintextBatch &plain) const
+        {
+            owned(plain);
+            auto cd = context_.get_context_data(plain.parms_id_);
+            if (!plain.ntt_)
+                throw std::invalid_argument("plain is not in NTT form");
+            if (!cd->next_context_data())
+                throw std::invalid_argument("end of modulus switching chain reached");
+            auto &next = *cd->next_context_data();
+            if (!scale_within_bounds(plain.scale_, next))
+                throw std::invalid_argument("scale out of bounds");
+            const std::size_t L = plain.L_, n = plain.n_, row = (L - 1) * n * sizeof(std::uint64_t);
+            std::lock_guard<std::mutex> lock(mu_);
+            PlaintextBatch out;
+            check(out.reserve(ctx_, plain.batch_ * (L - 1) * n));
+            check(sb200_memcpy_d2d_2d(ctx_, out.d_, row, plain.d_, L * n * sizeof(std::uint64_t), row, plain.batch_, nullptr));
+            std::swap(plain.d_, out.d_), std::swap(plain.cap_, out.cap_);
+            plain.L_ = L - 1, plain.parms_id_ = next.parms_id();
+        }
+        void mod_switch_to_inplace(PlaintextBatch &plain, seal::parms_id_type parms_id) const
+        {
+            owned(plain);
+            auto cur = context_.get_context_data(plain.parms_id_);
+            auto target = context_.get_context_data(parms_id);
+            if (!target)
+                throw std::invalid_argument("parms_id is not valid for encryption parameters");
+            if (!plain.ntt_)
+                throw std::invalid_argument("plain is not in NTT form");
+            if (cur->chain_index() < target->chain_index())
+                throw std::invalid_argument("cannot switch to higher level modulus");
+            while (plain.parms_id_ != parms_id)
+                mod_switch_to_next_inplace(plain);
+        }
+        // multiply_plain_inplace (evaluator.cpp:1975-2019): the four-way dispatch on the NTT forms
+        void multiply_plain_inplace(CiphertextBatch &encrypted, const PlaintextBatch &plain) const
+        {
+            owned(encrypted), owned(plain);
+            plain_count(encrypted, plain);
+            const std::size_t L = encrypted.L_, size = encrypted.size_, B = encrypted.batch_;
+            if (!plain.ntt_)
+            {
+                // multiply_plain_normal (:2021-2155) / transform + multiply_plain_ntt (:1999-2004)
+                if (scheme_ == seal::scheme_type::ckks)
+                    throw std::invalid_argument("plain is not valid for encryption parameters"); // CKKS plaintexts are always in NTT form
+                std::lock_guard<std::mutex> lock(mu_);
+                check(sb200_multiply_plain_coeff_n(ctx_, L, size, B, plain.batch_, encrypted.ntt_ ? 1 : 0, encrypted.d_, plain.d_, encrypted.d_,
+                                                   nullptr));
+                return;
+            }
+            if (encrypted.parms_id_ != plain.parms_id_)
+                throw std::invalid_argument("encrypted_ntt and plain_ntt parameter mismatch"); // :2164-2167
+            const double new_scale = encrypted.scale_ * plain.scale_;
+            if (!scale_within_bounds(new_scale, *context_.get_context_data(encrypted.parms_id_)))
+                throw std::invalid_argument("scale out of bounds"); // :2189-2193
+            const bool back = !encrypted.ntt_; // :2006-2011: to NTT form, multiply, back
+            std::lock_guard<std::mutex> lock(mu_);
+            if (back)
+                check(sb200_ntt_forward(ctx_, L, size, B, encrypted.d_, nullptr));
+            check(sb200_multiply_plain_n(ctx_, L, size, B, plain.batch_, encrypted.d_, plain.d_, encrypted.d_, nullptr));
+            if (back)
+                check(sb200_ntt_inverse(ctx_, L, size, B, encrypted.d_, nullptr));
+            encrypted.scale_ = new_scale;
+        }
+        // add_plain_inplace / sub_plain_inplace (evaluator.cpp:1759-1866, :1867-1974)
+        void add_plain_inplace(CiphertextBatch &encrypted, const PlaintextBatch &plain) const { plain_linear_batch(encrypted, plain, false); }
+        void sub_plain_inplace(CiphertextBatch &encrypted, const PlaintextBatch &plain) const { plain_linear_batch(encrypted, plain, true); }
+
         // waits for all device work queued by this Evaluator (the batch members above only enqueue)
         void synchronize() const { check(sb200_stream_synchronize(ctx_, nullptr)); }
 
@@ -1311,6 +1518,48 @@ namespace seal_b200
             for (std::size_t i = 0; i < count; i++)
                 rows[i] = cts[i].data();
             check(sb200_upload_rows(ctx_, destination.d_, rows.data(), destination.words_per_ciphertext() * sizeof(std::uint64_t), count));
+        }
+        void owned(const PlaintextBatch &p) const
+        {
+            if (p.ctx_ != ctx_ || !p.d_ || !p.batch_ || (p.ntt_ && !context_.get_context_data(p.parms_id_)))
+                throw std::invalid_argument("plain is not valid for encryption parameters");
+        }
+        static void plain_count(const CiphertextBatch &encrypted, const PlaintextBatch &plain)
+        {
+            if (plain.batch_ != 1 && plain.batch_ != encrypted.batch_)
+                throw std::invalid_argument("plain batch size must be 1 or the ciphertext batch size");
+        }
+        void plain_linear_batch(CiphertextBatch &encrypted, const PlaintextBatch &plain, bool subtract) const
+        {
+            owned(encrypted), owned(plain);
+            plain_count(encrypted, plain);
+            const std::size_t L = encrypted.L_, size = encrypted.size_, B = encrypted.batch_;
+            if (scheme_ != seal::scheme_type::ckks)
+            {
+                const bool bfv = scheme_ == seal::scheme_type::bfv;
+                if (bfv && encrypted.ntt_)
+                    throw std::invalid_argument("BFV encrypted cannot be in NTT form");
+                if (!bfv && !encrypted.ntt_)
+                    throw std::invalid_argument("BGV encrypted must be in NTT form");
+                if (plain.ntt_)
+                    throw std::invalid_argument(bfv ? "BFV plain cannot be in NTT form" : "BGV plain cannot be in NTT form");
+                // the batch's one correction factor, once per plaintext (BGV, :1840-1843)
+                const std::vector<std::uint64_t> cf(plain.batch_, encrypted.cf_);
+                std::lock_guard<std::mutex> lock(mu_);
+                check(sb200_add_plain_coeff_n(ctx_, L, size, B, plain.batch_, subtract ? 1 : 0, encrypted.d_, plain.d_, bfv ? nullptr : cf.data(),
+                                              encrypted.d_, nullptr));
+                return;
+            }
+            if (!encrypted.ntt_)
+                throw std::invalid_argument("CKKS encrypted must be in NTT form");
+            if (!plain.ntt_)
+                throw std::invalid_argument("CKKS plain must be in NTT form");
+            if (encrypted.parms_id_ != plain.parms_id_)
+                throw std::invalid_argument("encrypted and plain parameter mismatch");
+            if (!seal::util::are_close<double>(encrypted.scale_, plain.scale_))
+                throw std::invalid_argument("scale mismatch");
+            std::lock_guard<std::mutex> lock(mu_);
+            check(sb200_add_plain_ntt(ctx_, L, size, B, plain.batch_, subtract ? 1 : 0, encrypted.d_, plain.d_, encrypted.d_, nullptr));
         }
         void owned(const CiphertextBatch &b) const
         {

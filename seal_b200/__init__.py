@@ -30,6 +30,8 @@ SYMBOLS = [
     "sb200_ntt_inverse", "sb200_multiply", "sb200_multiply_sized", "sb200_square", "sb200_add", "sb200_sub", "sb200_negate", "sb200_multiply_plain", "sb200_batch_encode", "sb200_batch_decode", "sb200_plain_to_ntt", "sb200_multiply_plain_coeff", "sb200_add_plain_coeff", "sb200_relinearize", "sb200_multiply_relinearize", "sb200_rescale_to_next",
     "sb200_mod_switch_to_next", "sb200_apply_galois", "sb200_ntt_forward_host", "sb200_ntt_inverse_host",
     "sb200_multiply_host", "sb200_multiply_sized_host", "sb200_square_host", "sb200_add_host", "sb200_sub_host", "sb200_negate_host", "sb200_multiply_plain_host", "sb200_batch_encode_host", "sb200_batch_decode_host", "sb200_plain_to_ntt_host", "sb200_multiply_plain_coeff_host", "sb200_add_plain_coeff_host",
+    "sb200_multiply_plain_n", "sb200_multiply_plain_coeff_n", "sb200_add_plain_coeff_n", "sb200_add_plain_ntt", "sb200_multiply_plain_n_host",
+    "sb200_multiply_plain_coeff_n_host", "sb200_add_plain_coeff_n_host", "sb200_add_plain_ntt_host",
     "sb200_relinearize_host", "sb200_multiply_relinearize_host", "sb200_rescale_to_next_host",
     "sb200_mod_switch_to_next_host", "sb200_apply_galois_host", "sb200_get_parms_id", "sb200_ciphertext_inspect",
     "sb200_ciphertext_save_size", "sb200_ciphertext_load", "sb200_ciphertext_save", "sb200_secret_key_create",
@@ -114,6 +116,14 @@ def lib():
         L.sb200_plain_to_ntt_host.argtypes = [vp, sz, sz, _u64p, _u64p]
         L.sb200_multiply_plain_coeff_host.argtypes = [vp, sz, sz, sz, i32, _u64p, _u64p, _u64p]
         L.sb200_add_plain_coeff_host.argtypes = [vp, sz, sz, sz, i32, _u64p, _u64p, _u64p, _u64p]
+        L.sb200_multiply_plain_n.argtypes = [vp, sz, sz, sz, sz, vp, vp, vp, vp]
+        L.sb200_multiply_plain_coeff_n.argtypes = [vp, sz, sz, sz, sz, i32, vp, vp, vp, vp]
+        L.sb200_add_plain_coeff_n.argtypes = [vp, sz, sz, sz, sz, i32, vp, vp, _u64p, vp, vp]
+        L.sb200_add_plain_ntt.argtypes = [vp, sz, sz, sz, sz, i32, vp, vp, vp, vp]
+        L.sb200_multiply_plain_n_host.argtypes = [vp, sz, sz, sz, sz, _u64p, _u64p, _u64p]
+        L.sb200_multiply_plain_coeff_n_host.argtypes = [vp, sz, sz, sz, sz, i32, _u64p, _u64p, _u64p]
+        L.sb200_add_plain_coeff_n_host.argtypes = [vp, sz, sz, sz, sz, i32, _u64p, _u64p, _u64p, _u64p]
+        L.sb200_add_plain_ntt_host.argtypes = [vp, sz, sz, sz, sz, i32, _u64p, _u64p, _u64p]
         L.sb200_square_host.argtypes = [vp, sz, sz, _u64p, _u64p]
         L.sb200_add_host.argtypes = [vp, sz, sz, sz, _u64p, _u64p, _u64p]
         L.sb200_sub_host.argtypes = [vp, sz, sz, sz, _u64p, _u64p, _u64p]
@@ -590,6 +600,52 @@ class Context:
         _check(lib().sb200_add_plain_coeff_host(self.h, L, size, B, int(subtract), _hp(a), _hp(plain), cf, _hp(out)))
         return out[0] if single else out
 
+    # ---- plaintext operations with one plaintext per ciphertext ([B] leading axis) or one for the whole batch (no batch axis) ----
+    def _plains(self, plain, B, shape):
+        """plaintexts as (plain_count, contiguous uint64 array): [B] + shape, or shape alone (one plaintext for the batch)"""
+        p = np.ascontiguousarray(plain, dtype=np.uint64)
+        count = 1 if p.shape == tuple(shape) else B
+        assert p.shape in (tuple(shape), (B,) + tuple(shape)), (p.shape, shape)
+        return count, p
+
+    def multiply_plain_n(self, a, plain):
+        """Evaluator.multiply_plain, NTT-form ciphertexts [B][size][L][n] x NTT-form plaintexts [B][L][n] or one [L][n]"""
+        a, single = self._batched(a)
+        B, size, L, n = a.shape
+        count, p = self._plains(plain, B, (L, n))
+        out = np.zeros_like(a)
+        _check(lib().sb200_multiply_plain_n_host(self.h, L, size, B, count, _hp(a), _hp(p), _hp(out)))
+        return out[0] if single else out
+
+    def multiply_plain_coeff_n(self, a, plain, ct_is_ntt):
+        """Evaluator.multiply_plain with coefficient-form plaintexts [B][n] or one [n]"""
+        a, single = self._batched(a)
+        B, size, L, n = a.shape
+        count, p = self._plains(plain, B, (n,))
+        out = np.zeros_like(a)
+        _check(lib().sb200_multiply_plain_coeff_n_host(self.h, L, size, B, count, int(ct_is_ntt), _hp(a), _hp(p), _hp(out)))
+        return out[0] if single else out
+
+    def add_plain_coeff_n(self, a, plain, subtract=False, correction_factors=None):
+        """Evaluator.add_plain / sub_plain with coefficient-form plaintexts [B][n] or one [n] (BFV, BGV); correction_factors: one
+        per plaintext"""
+        a, single = self._batched(a)
+        B, size, L, n = a.shape
+        count, p = self._plains(plain, B, (n,))
+        out = np.zeros_like(a)
+        cf = None if correction_factors is None else _hp(np.ascontiguousarray(correction_factors, dtype=np.uint64).reshape(count))
+        _check(lib().sb200_add_plain_coeff_n_host(self.h, L, size, B, count, int(subtract), _hp(a), _hp(p), cf, _hp(out)))
+        return out[0] if single else out
+
+    def add_plain_ntt(self, a, plain, subtract=False):
+        """CKKS Evaluator.add_plain / sub_plain: c_0 +/- NTT-form plaintexts [B][L][n] or one [L][n]"""
+        a, single = self._batched(a)
+        B, size, L, n = a.shape
+        count, p = self._plains(plain, B, (L, n))
+        out = np.zeros_like(a)
+        _check(lib().sb200_add_plain_ntt_host(self.h, L, size, B, count, int(subtract), _hp(a), _hp(p), _hp(out)))
+        return out[0] if single else out
+
     def relinearize(self, c3, key):
         c3, single = self._batched(c3)
         B, _, L, n = c3.shape
@@ -656,6 +712,21 @@ class Context:
 
     def d_multiply_plain(self, a, plain, out, L, size, batch):
         _check(lib().sb200_multiply_plain(self.h, L, size, batch, _dp(a), _dp(plain), _dp(out), self._stream()))
+
+    def d_multiply_plain_n(self, a, plain, out, L, size, batch, plain_count):
+        _check(lib().sb200_multiply_plain_n(self.h, L, size, batch, plain_count, _dp(a), _dp(plain), _dp(out), self._stream()))
+
+    def d_multiply_plain_coeff_n(self, a, plain, out, L, size, batch, plain_count, ct_is_ntt):
+        _check(lib().sb200_multiply_plain_coeff_n(self.h, L, size, batch, plain_count, int(ct_is_ntt), _dp(a), _dp(plain), _dp(out),
+                                                  self._stream()))
+
+    def d_add_plain_coeff_n(self, a, plain, out, L, size, batch, plain_count, subtract=False, correction_factors=None):
+        cf = None if correction_factors is None else np.ascontiguousarray(correction_factors, dtype=np.uint64).reshape(plain_count)
+        _check(lib().sb200_add_plain_coeff_n(self.h, L, size, batch, plain_count, int(subtract), _dp(a), _dp(plain),
+                                             None if cf is None else _hp(cf), _dp(out), self._stream()))
+
+    def d_add_plain_ntt(self, a, plain, out, L, size, batch, plain_count, subtract=False):
+        _check(lib().sb200_add_plain_ntt(self.h, L, size, batch, plain_count, int(subtract), _dp(a), _dp(plain), _dp(out), self._stream()))
 
     def d_multiply_sized(self, a, b, out, L, size_a, size_b, batch):
         _check(lib().sb200_multiply_sized(self.h, L, size_a, size_b, batch, _dp(a), _dp(b), _dp(out), self._stream()))

@@ -797,6 +797,7 @@ namespace
         bool in_place = false;         // the output overwrites input a (out = a)
         const char *alias = nullptr;   // device slabs: the error when the output aliases an input (nullptr = allowed)
         size_t out_unit = sizeof(u64); // bytes of one output word (the noise budget returns one int per ciphertext)
+        bool shared_b = false;         // input b is one operand of b words for the whole batch (a plaintext shared by every ciphertext)
     };
 
     struct HostPipe
@@ -828,7 +829,7 @@ namespace
         void run(size_t batch, const Layout &w, const u64 *ha, const u64 *hb, u64 *ho, const Op &op)
         {
             StreamOrder order(c, s_comp); // the operation's kernels (and the scratch arenas they use) run on s_comp
-            const size_t wa = w.a, wb = w.b, wo = w.in_place ? 0 : w.out;
+            const size_t wa = w.a, wb = w.shared_b ? 0 : w.b, wo = w.in_place ? 0 : w.out;
             const size_t out_bytes = w.out * w.out_unit; // per ciphertext
             const size_t per_ct = (wa + wb) * sizeof(u64) + (w.in_place ? 0 : out_bytes);
             size_t chunk = std::max<size_t>(1, std::min<size_t>(batch, c.host_stage_bytes / std::max<size_t>(per_ct, 1)));
@@ -843,12 +844,20 @@ namespace
                 if (!w.in_place)
                     buffer(slot, 2, (chunk * wo * w.out_unit + sizeof(u64) - 1) / sizeof(u64));
             }
+            const u64 *d_shared = nullptr; // a shared operand crosses the bus once, ahead of the first chunk, and is never overwritten
+            if (w.shared_b)
+            {
+                u64 *d = buffer(0, 1, w.b);
+                cuda_check(cudaMemcpyAsync(d, hb, w.b * sizeof(u64), cudaMemcpyHostToDevice, s_in), "H2D");
+                d_shared = d;
+            }
             size_t i = 0;
             for (size_t b0 = 0; b0 < batch; b0 += chunk, i++)
             {
                 const size_t B = std::min(chunk, batch - b0);
                 const int slot = static_cast<int>(i & 1);
-                u64 *da = buffer(slot, 0, B * wa), *db = wb ? buffer(slot, 1, B * wb) : nullptr, *dout = w.in_place ? da : buffer(slot, 2, (B * wo * w.out_unit + sizeof(u64) - 1) / sizeof(u64));
+                u64 *db = wb ? buffer(slot, 1, B * wb) : nullptr;
+                u64 *da = buffer(slot, 0, B * wa), *dout = w.in_place ? da : buffer(slot, 2, (B * wo * w.out_unit + sizeof(u64) - 1) / sizeof(u64));
                 if (i >= 2)
                 {
                     // inputs of this slot are free once its previous kernels finished (and, in place, once copied out)
@@ -861,7 +870,7 @@ namespace
                 cuda_check(cudaStreamWaitEvent(s_comp, ev_in[slot], 0), "wait");
                 if (i >= 2 && !w.in_place)
                     cuda_check(cudaStreamWaitEvent(s_comp, ev_out[slot], 0), "wait"); // output staging of this slot drained
-                op(c, b0, B, da, db, dout, s_comp);
+                op(c, b0, B, da, w.shared_b ? d_shared : db, dout, s_comp);
                 cuda_check(cudaEventRecord(ev_comp[slot], s_comp), "record");
                 cuda_check(cudaStreamWaitEvent(s_out, ev_comp[slot], 0), "wait");
                 cuda_check(cudaMemcpyAsync(reinterpret_cast<uint8_t *>(ho) + b0 * out_bytes, dout, B * out_bytes, cudaMemcpyDeviceToHost, s_out), "D2H");
@@ -938,14 +947,45 @@ namespace
         }
     };
 
-    struct MultiplyPlain // b: NTT-form plaintexts [B][L][n]
+    // plain_count: one plaintext per ciphertext (batch) or one for the whole batch (1, a shared operand: Layout::shared_b).  The
+    // older entry points, which take one plaintext per ciphertext, stay on the per-ciphertext path at every batch size (shared =
+    // false, plain_count = batch); the _n entry points share the plaintext when plain_count = 1.
+    static void check_plain_count(size_t plain_count, size_t batch)
     {
-        size_t L, size;
-        void check(const Context &c, size_t batch) const { check_level(c, L, batch); }
-        Layout layout(const Context &c) const { return { size * L * c.n, L * c.n, size * L * c.n }; }
+        if (plain_count != 1 && plain_count != batch)
+            throw std::invalid_argument("plain_count must be 1 or batch");
+    }
+
+    struct MultiplyPlain // b: NTT-form plaintexts [plain_count][L][n]
+    {
+        size_t L, size, plain_count;
+        bool shared;
+        void check(const Context &c, size_t batch) const
+        {
+            check_level(c, L, batch);
+            check_plain_count(plain_count, batch);
+        }
+        Layout layout(const Context &c) const { return { size * L * c.n, L * c.n, size * L * c.n, false, nullptr, sizeof(u64), shared }; }
         void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *b, u64 *out, cudaStream_t st) const
         {
-            op_multiply_plain(c, L, size, B, a, b, out, st);
+            op_multiply_plain(c, L, size, B, shared, a, b, out, st);
+        }
+    };
+
+    struct AddPlainNtt // CKKS: b: NTT-form plaintexts [plain_count][L][n], added to (subtracted from) c_0
+    {
+        size_t L, size, plain_count;
+        bool shared;
+        bool subtract;
+        void check(const Context &c, size_t batch) const
+        {
+            check_level(c, L, batch);
+            check_plain_count(plain_count, batch);
+        }
+        Layout layout(const Context &c) const { return { size * L * c.n, L * c.n, size * L * c.n, false, nullptr, sizeof(u64), shared }; }
+        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *b, u64 *out, cudaStream_t st) const
+        {
+            op_add_plain_ntt(c, L, size, B, shared, subtract, a, b, out, st);
         }
     };
 
@@ -960,28 +1000,39 @@ namespace
         }
     };
 
-    struct MultiplyPlainCoeff // b: coefficient-form plaintexts [B][n]
+    struct MultiplyPlainCoeff // b: coefficient-form plaintexts [plain_count][n]
     {
-        size_t L, size;
+        size_t L, size, plain_count;
+        bool shared;
         bool ct_is_ntt;
-        void check(const Context &c, size_t batch) const { check_level(c, L, batch); }
-        Layout layout(const Context &c) const { return { size * L * c.n, c.n, size * L * c.n }; }
+        void check(const Context &c, size_t batch) const
+        {
+            check_level(c, L, batch);
+            check_plain_count(plain_count, batch);
+        }
+        Layout layout(const Context &c) const { return { size * L * c.n, c.n, size * L * c.n, false, nullptr, sizeof(u64), shared }; }
         void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *b, u64 *out, cudaStream_t st) const
         {
-            op_multiply_plain_coeff(c, L, size, B, ct_is_ntt, a, b, out, st);
+            op_multiply_plain_coeff(c, L, size, B, shared, ct_is_ntt, a, b, out, st);
         }
     };
 
-    struct AddPlainCoeff // b: coefficient-form plaintexts [B][n]; cf: BGV correction factors on the host, one per ciphertext
+    // b: coefficient-form plaintexts [plain_count][n]; cf: BGV correction factors on the host, one per plaintext (NULL = 1)
+    struct AddPlainCoeff
     {
-        size_t L, size;
+        size_t L, size, plain_count;
+        bool shared;
         bool subtract;
         const u64 *cf;
-        void check(const Context &c, size_t batch) const { check_level(c, L, batch); }
-        Layout layout(const Context &c) const { return { size * L * c.n, c.n, size * L * c.n }; }
+        void check(const Context &c, size_t batch) const
+        {
+            check_level(c, L, batch);
+            check_plain_count(plain_count, batch);
+        }
+        Layout layout(const Context &c) const { return { size * L * c.n, c.n, size * L * c.n, false, nullptr, sizeof(u64), shared }; }
         void operator()(Context &c, size_t b0, size_t B, const u64 *a, const u64 *b, u64 *out, cudaStream_t st) const
         {
-            op_add_plain_coeff(c, L, size, B, subtract, a, b, cf ? cf + b0 : nullptr, out, st);
+            op_add_plain_coeff(c, L, size, B, shared, subtract, a, b, cf && !shared ? cf + b0 : cf, out, st);
         }
     };
 
@@ -1163,6 +1214,8 @@ namespace
         const Layout w = op.layout(c);
         if (w.alias && (out == a || out == b))
             throw std::invalid_argument(w.alias);
+        if (w.shared_b && out == b)
+            throw std::invalid_argument("the shared plaintext must not alias the output slab");
         auto st = static_cast<cudaStream_t>(stream);
         op(c, 0, batch, static_cast<const u64 *>(a), static_cast<const u64 *>(b), static_cast<u64 *>(out), st);
         if (then)
@@ -1272,12 +1325,37 @@ int sb200_multiply_plain(sb200_context *ctx, size_t L, size_t size, size_t batch
                          void *stream)
 {
     SB_NEED(plain);
-    return on_stream(ctx, stream, batch, a, plain, out, MultiplyPlain{ L, size });
+    return on_stream(ctx, stream, batch, a, plain, out, MultiplyPlain{ L, size, batch, false });
 }
 int sb200_multiply_plain_host(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, const uint64_t *plain, uint64_t *out)
 {
     SB_NEED(plain);
-    return on_host(ctx, batch, a, plain, out, MultiplyPlain{ L, size });
+    return on_host(ctx, batch, a, plain, out, MultiplyPlain{ L, size, batch, false });
+}
+int sb200_multiply_plain_n(sb200_context *ctx, size_t L, size_t size, size_t batch, size_t plain_count, const uint64_t *a, const uint64_t *plain,
+                           uint64_t *out, void *stream)
+{
+    SB_NEED(plain);
+    return on_stream(ctx, stream, batch, a, plain, out, MultiplyPlain{ L, size, plain_count, plain_count == 1 });
+}
+int sb200_multiply_plain_n_host(sb200_context *ctx, size_t L, size_t size, size_t batch, size_t plain_count, const uint64_t *a,
+                                const uint64_t *plain, uint64_t *out)
+{
+    SB_NEED(plain);
+    return on_host(ctx, batch, a, plain, out, MultiplyPlain{ L, size, plain_count, plain_count == 1 });
+}
+
+int sb200_add_plain_ntt(sb200_context *ctx, size_t L, size_t size, size_t batch, size_t plain_count, int subtract, const uint64_t *a,
+                        const uint64_t *plain, uint64_t *out, void *stream)
+{
+    SB_NEED(plain);
+    return on_stream(ctx, stream, batch, a, plain, out, AddPlainNtt{ L, size, plain_count, plain_count == 1, subtract != 0 });
+}
+int sb200_add_plain_ntt_host(sb200_context *ctx, size_t L, size_t size, size_t batch, size_t plain_count, int subtract, const uint64_t *a,
+                             const uint64_t *plain, uint64_t *out)
+{
+    SB_NEED(plain);
+    return on_host(ctx, batch, a, plain, out, AddPlainNtt{ L, size, plain_count, plain_count == 1, subtract != 0 });
 }
 
 int sb200_plain_to_ntt(sb200_context *ctx, size_t L, size_t batch, const uint64_t *plain, uint64_t *out, void *stream)
@@ -1293,26 +1371,50 @@ int sb200_multiply_plain_coeff(sb200_context *ctx, size_t L, size_t size, size_t
                                uint64_t *out, void *stream)
 {
     SB_NEED(plain);
-    return on_stream(ctx, stream, batch, a, plain, out, MultiplyPlainCoeff{ L, size, ct_is_ntt != 0 });
+    return on_stream(ctx, stream, batch, a, plain, out, MultiplyPlainCoeff{ L, size, batch, false, ct_is_ntt != 0 });
 }
 int sb200_multiply_plain_coeff_host(sb200_context *ctx, size_t L, size_t size, size_t batch, int ct_is_ntt, const uint64_t *a,
                                     const uint64_t *plain, uint64_t *out)
 {
     SB_NEED(plain);
-    return on_host(ctx, batch, a, plain, out, MultiplyPlainCoeff{ L, size, ct_is_ntt != 0 });
+    return on_host(ctx, batch, a, plain, out, MultiplyPlainCoeff{ L, size, batch, false, ct_is_ntt != 0 });
+}
+int sb200_multiply_plain_coeff_n(sb200_context *ctx, size_t L, size_t size, size_t batch, size_t plain_count, int ct_is_ntt, const uint64_t *a,
+                                 const uint64_t *plain, uint64_t *out, void *stream)
+{
+    SB_NEED(plain);
+    return on_stream(ctx, stream, batch, a, plain, out, MultiplyPlainCoeff{ L, size, plain_count, plain_count == 1, ct_is_ntt != 0 });
+}
+int sb200_multiply_plain_coeff_n_host(sb200_context *ctx, size_t L, size_t size, size_t batch, size_t plain_count, int ct_is_ntt,
+                                      const uint64_t *a, const uint64_t *plain, uint64_t *out)
+{
+    SB_NEED(plain);
+    return on_host(ctx, batch, a, plain, out, MultiplyPlainCoeff{ L, size, plain_count, plain_count == 1, ct_is_ntt != 0 });
 }
 
 int sb200_add_plain_coeff(sb200_context *ctx, size_t L, size_t size, size_t batch, int subtract, const uint64_t *a, const uint64_t *plain,
                           const uint64_t *h_correction_factors, uint64_t *out, void *stream)
 {
     SB_NEED(plain);
-    return on_stream(ctx, stream, batch, a, plain, out, AddPlainCoeff{ L, size, subtract != 0, (const u64 *)h_correction_factors });
+    return on_stream(ctx, stream, batch, a, plain, out, AddPlainCoeff{ L, size, batch, false, subtract != 0, (const u64 *)h_correction_factors });
 }
 int sb200_add_plain_coeff_host(sb200_context *ctx, size_t L, size_t size, size_t batch, int subtract, const uint64_t *a, const uint64_t *plain,
                                const uint64_t *h_correction_factors, uint64_t *out)
 {
     SB_NEED(plain);
-    return on_host(ctx, batch, a, plain, out, AddPlainCoeff{ L, size, subtract != 0, (const u64 *)h_correction_factors });
+    return on_host(ctx, batch, a, plain, out, AddPlainCoeff{ L, size, batch, false, subtract != 0, (const u64 *)h_correction_factors });
+}
+int sb200_add_plain_coeff_n(sb200_context *ctx, size_t L, size_t size, size_t batch, size_t plain_count, int subtract, const uint64_t *a,
+                            const uint64_t *plain, const uint64_t *h_correction_factors, uint64_t *out, void *stream)
+{
+    SB_NEED(plain);
+    return on_stream(ctx, stream, batch, a, plain, out, AddPlainCoeff{ L, size, plain_count, plain_count == 1, subtract != 0, (const u64 *)h_correction_factors });
+}
+int sb200_add_plain_coeff_n_host(sb200_context *ctx, size_t L, size_t size, size_t batch, size_t plain_count, int subtract, const uint64_t *a,
+                                 const uint64_t *plain, const uint64_t *h_correction_factors, uint64_t *out)
+{
+    SB_NEED(plain);
+    return on_host(ctx, batch, a, plain, out, AddPlainCoeff{ L, size, plain_count, plain_count == 1, subtract != 0, (const u64 *)h_correction_factors });
 }
 
 int sb200_batch_encode(sb200_context *ctx, size_t batch, const uint64_t *values, uint64_t *plain, void *stream)

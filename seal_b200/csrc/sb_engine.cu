@@ -537,10 +537,73 @@ namespace sb
         out[e] = make_ulonglong2(mulmod_wide(canon_in(x.x, P), canon_in(y.x, P), P), mulmod_wide(canon_in(x.y, P), canon_in(y.y, P), P));
     }
 
-    void op_multiply_plain(Context &c, size_t L, size_t size, size_t batch, const u64 *a, const u64 *plain, u64 *out, cudaStream_t st)
+    // One plaintext [L][n] for the whole batch.  A thread owns one pair of plaintext words and keeps them in registers while it
+    // walks the rows of a group of G ciphertexts: MODE 0 multiplies every polynomial (dyadic_product_coeffmod, operands reduced on
+    // the way in as plain_mul_kernel does), MODE 1 / 2 add to / subtract from c_0 only (add_poly_coeffmod / sub_poly_coeffmod, as
+    // add_c0_kernel).  blockIdx.x is the ciphertext group, so the CTAs that read one plaintext slice run together and the slice
+    // crosses HBM once per launch.  (The per-ciphertext kernels with a plaintext stride of 0 re-read the plaintext from HBM once L2
+    // no longer holds it: at n = 65536 with 31 primes, 1.3x / 1.6x this kernel's time for multiply_plain / add_plain; DESIGN 7b.)
+    template <int MODE>
+    __global__ void __launch_bounds__(256) shared_plain_kernel(const ulonglong2 *__restrict__ a, const ulonglong2 *__restrict__ plain, ulonglong2 *out,
+                                                                const PrimeDev *__restrict__ primes, int logn, int L, int size, int batch, int G)
+    {
+        const long long half = static_cast<long long>(L) << (logn - 1); // pairs of one polynomial
+        const long long p = static_cast<long long>(blockIdx.y) * blockDim.x + threadIdx.x;
+        if (p >= half)
+            return;
+        const PrimeDev &P = primes[static_cast<int>(p >> (logn - 1))];
+        ulonglong2 y = plain[p];
+        if (MODE == 0)
+            y = make_ulonglong2(canon_in(y.x, P), canon_in(y.y, P));
+        const int b1 = min(batch, static_cast<int>(blockIdx.x + 1) * G), polys = MODE == 0 ? size : 1;
+        for (int b = blockIdx.x * G; b < b1; b++)
+            for (int s = 0; s < polys; s++)
+            {
+                const long long e = (static_cast<long long>(b) * size + s) * half + p;
+                const ulonglong2 x = a[e];
+                if (MODE == 0)
+                    out[e] = make_ulonglong2(mulmod_wide(canon_in(x.x, P), y.x, P), mulmod_wide(canon_in(x.y, P), y.y, P));
+                else if (MODE == 1)
+                    out[e] = make_ulonglong2(csub(x.x + y.x, P.q), csub(x.y + y.y, P.q));
+                else
+                    out[e] = make_ulonglong2(csub(x.x + P.q - y.x, P.q), csub(x.y + P.q - y.y, P.q));
+            }
+    }
+
+    static void launch_shared_plain(Context &c, int mode, const char *name, size_t L, size_t size, size_t batch, const u64 *a, const u64 *plain,
+                                    u64 *out, cudaStream_t st)
+    {
+        constexpr int G = 8;
+        const size_t half = L * c.n / 2, polys = mode == 0 ? size : 1;
+        const dim3 grid(static_cast<unsigned>((batch + G - 1) / G), static_cast<unsigned>((half + 255) / 256));
+        auto pa = reinterpret_cast<const ulonglong2 *>(a);
+        auto pp = reinterpret_cast<const ulonglong2 *>(plain);
+        auto po = reinterpret_cast<ulonglong2 *>(out);
+        const int l = static_cast<int>(L), sz = static_cast<int>(size), nb = static_cast<int>(batch);
+        c.stats.begin(name, 0, 8.0 * (2.0 * batch * polys + 1.0) * L * c.n, st);
+        if (mode == 0)
+            shared_plain_kernel<0><<<grid, 256, 0, st>>>(pa, pp, po, c.d_primes.get(), c.logn, l, sz, nb, G);
+        else if (mode == 1)
+            shared_plain_kernel<1><<<grid, 256, 0, st>>>(pa, pp, po, c.d_primes.get(), c.logn, l, sz, nb, G);
+        else
+            shared_plain_kernel<2><<<grid, 256, 0, st>>>(pa, pp, po, c.d_primes.get(), c.logn, l, sz, nb, G);
+        c.stats.end(st);
+        cuda_check(cudaGetLastError(), "shared_plain_kernel");
+    }
+
+    void op_multiply_plain(Context &c, size_t L, size_t size, size_t batch, bool shared, const u64 *a, const u64 *plain, u64 *out,
+                           cudaStream_t st)
     {
         if (c.n < 2 || size < 1)
             throw std::invalid_argument("encrypted is not valid for encryption parameters");
+        if (shared)
+        {
+            const size_t step = std::max<size_t>(1, (size_t(1) << 30) / (size * L * c.n));
+            for (size_t b0 = 0; b0 < batch; b0 += step)
+                launch_shared_plain(c, 0, "multiply_plain", L, size, std::min(step, batch - b0), a + b0 * size * L * c.n, plain,
+                                    out + b0 * size * L * c.n, st);
+            return;
+        }
         const size_t per = size * L * c.n, step = std::max<size_t>(1, (size_t(1) << 32) / per);
         for (size_t b0 = 0; b0 < batch; b0 += step)
         {
@@ -669,37 +732,49 @@ namespace sb
         }
     }
 
-    void op_multiply_plain_coeff(Context &c, size_t L, size_t size, size_t batch, bool ct_ntt, const u64 *ct, const u64 *plain, u64 *out,
-                                 cudaStream_t st)
+    void op_multiply_plain_coeff(Context &c, size_t L, size_t size, size_t batch, bool shared, bool ct_ntt, const u64 *ct, const u64 *plain,
+                                 u64 *out, cudaStream_t st)
     {
         if (size < 1)
             throw std::invalid_argument("encrypted is not valid for encryption parameters");
         const size_t per = size * L * c.n;
-        size_t chunk = std::min(batch, std::max<size_t>(1, c.scratch_budget / (L * c.n * sizeof(u64))));
+        // a shared plaintext is lifted and transformed once per call (L n scratch words); per-ciphertext plaintexts per chunk
+        size_t chunk = shared ? batch : std::min(batch, std::max<size_t>(1, c.scratch_budget / (L * c.n * sizeof(u64))));
         chunk = std::min<size_t>(chunk, std::max<size_t>(1, (size_t(1) << 30) / per));
+        u64 *T = nullptr;
+        if (shared)
+        {
+            T = static_cast<u64 *>(c.ensure_scratch(L * c.n * sizeof(u64)));
+            plain_to_ntt_dev(c, L, 1, plain, nullptr, T, st);
+        }
         for (size_t b0 = 0; b0 < batch; b0 += chunk)
         {
             const size_t B = std::min(chunk, batch - b0);
-            u64 *T = static_cast<u64 *>(c.ensure_scratch(B * L * c.n * sizeof(u64)));
-            plain_to_ntt_dev(c, L, B, plain + b0 * c.n, nullptr, T, st);
+            if (!shared)
+            {
+                T = static_cast<u64 *>(c.ensure_scratch(B * L * c.n * sizeof(u64)));
+                plain_to_ntt_dev(c, L, B, plain + b0 * c.n, nullptr, T, st);
+            }
             const u64 *in = ct + b0 * per;
             u64 *o = out + b0 * per;
             if (ct_ntt)
             {
-                op_multiply_plain(c, L, size, B, in, T, o, st); // evaluator.cpp:1999-2004
+                op_multiply_plain(c, L, size, B, shared, in, T, o, st); // evaluator.cpp:1999-2004
                 continue;
             }
             // multiply_plain_normal (evaluator.cpp:2130-2143): ciphertext to NTT form, dyadic product, back
             if (o != in)
                 cuda_check(cudaMemcpyAsync(o, in, B * per * sizeof(u64), cudaMemcpyDeviceToDevice, st), "copy");
             op_ntt(c, false, L, size, B, o, st);
-            op_multiply_plain(c, L, size, B, o, T, o, st);
+            op_multiply_plain(c, L, size, B, shared, o, T, o, st);
             op_ntt(c, true, L, size, B, o, st);
         }
     }
 
     // BFV: c_0 +/- round(q * m / t) (multiply_add / multiply_sub_plain_with_scaling_variant, util/scalingvariant.cpp:70-160)
-    __global__ void __launch_bounds__(256) bfv_add_plain_kernel(const u64 *__restrict__ plain, u64 *ct, long long ct_bs, const Tw *__restrict__ delta,
+    // plain [B][n] (plain_bs = n) or one [n] for the whole batch (plain_bs = 0)
+    __global__ void __launch_bounds__(256) bfv_add_plain_kernel(const u64 *__restrict__ plain, long long plain_bs, u64 *ct, long long ct_bs,
+                                                                 const Tw *__restrict__ delta,
                                                                  const PrimeDev *__restrict__ primes, u64 t, u64 t_ratio_lo, u64 t_ratio_hi,
                                                                  u64 q_mod_t, int logn, int L, int subtract, long long total)
     {
@@ -708,7 +783,7 @@ namespace sb
             return;
         const long long b = e >> logn;
         const int idx = static_cast<int>(e & ((1 << logn) - 1));
-        const u64 m = plain[e];
+        const u64 m = plain[b * plain_bs + idx];
         // fix = floor((m * (q mod t) + (t + 1) / 2) / t): quotient estimate from the Barrett ratio, corrected by the remainder
         u64 lo = m * q_mod_t, hi = __umul64hi(m, q_mod_t);
         const u64 half = (t + 1) >> 1;
@@ -735,7 +810,8 @@ namespace sb
         }
     }
 
-    // BGV: c_0 +/- T, T = [B][L][n] transformed plaintexts (evaluator.cpp:1838-1849)
+    // c_0 +/- T, T = [B][L][n] NTT-form plaintexts: BGV's transformed plaintexts (evaluator.cpp:1838-1849), CKKS's own
+    // (add_poly_coeffmod / sub_poly_coeffmod, :1831-1836, :1939-1944)
     __global__ void __launch_bounds__(256) add_c0_kernel(const u64 *__restrict__ T, u64 *ct, long long ct_bs, const PrimeDev *__restrict__ primes,
                                                           int logn, int L, int subtract, long long total)
     {
@@ -749,8 +825,21 @@ namespace sb
         *p = subtract ? csub(x + q - y, q) : csub(x + y, q);
     }
 
-    void op_add_plain_coeff(Context &c, size_t L, size_t size, size_t batch, bool subtract, const u64 *ct, const u64 *plain, const u64 *h_cf,
-                            u64 *out, cudaStream_t st)
+    static void launch_add_c0(Context &c, const char *name, size_t L, size_t size, size_t B, bool shared, bool subtract, const u64 *T, u64 *o,
+                              cudaStream_t st)
+    {
+        if (shared)
+            return launch_shared_plain(c, subtract ? 2 : 1, name, L, size, B, o, T, o, st);
+        const long long total = static_cast<long long>(B * L * c.n);
+        c.stats.begin(name, 0, 24.0 * total, st);
+        add_c0_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(T, o, static_cast<long long>(size * L * c.n), c.d_primes.get(),
+                                                                                  c.logn, static_cast<int>(L), subtract ? 1 : 0, total);
+        c.stats.end(st);
+        cuda_check(cudaGetLastError(), "add_c0_kernel");
+    }
+
+    void op_add_plain_coeff(Context &c, size_t L, size_t size, size_t batch, bool shared, bool subtract, const u64 *ct, const u64 *plain,
+                            const u64 *h_cf, u64 *out, cudaStream_t st)
     {
         if (size < 1)
             throw std::invalid_argument("encrypted is not valid for encryption parameters");
@@ -758,8 +847,14 @@ namespace sb
         const size_t per = size * L * c.n;
         if (out != ct)
             cuda_check(cudaMemcpyAsync(out, ct, batch * per * sizeof(u64), cudaMemcpyDeviceToDevice, st), "copy");
-        size_t chunk = std::min(batch, std::max<size_t>(1, c.scratch_budget / ((L * c.n + 1) * sizeof(u64))));
+        size_t chunk = shared ? batch : std::min(batch, std::max<size_t>(1, c.scratch_budget / ((L * c.n + 1) * sizeof(u64))));
         chunk = std::min<size_t>(chunk, std::max<size_t>(1, (size_t(1) << 30) / (L * c.n)));
+        u64 *T = nullptr;
+        if (shared && c.scheme != 1) // BGV: NTT(lift(m cf mod t)) of the one plaintext, once per call
+        {
+            T = static_cast<u64 *>(c.ensure_scratch((L * c.n + 1) * sizeof(u64)));
+            plain_to_ntt_dev(c, L, 1, plain, upload_cf(c, h_cf, 1, T + L * c.n, st), T, st);
+        }
         for (size_t b0 = 0; b0 < batch; b0 += chunk)
         {
             const size_t B = std::min(chunk, batch - b0);
@@ -767,23 +862,42 @@ namespace sb
             if (c.scheme == 1)
             {
                 const long long total = static_cast<long long>(B * c.n);
-                c.stats.begin("bfv_add_plain", 0, 8.0 * total * (1 + 2 * L), st);
+                c.stats.begin("bfv_add_plain", 0, 8.0 * ((shared ? c.n : total) + 2.0 * L * total), st);
                 bfv_add_plain_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(
-                    plain + b0 * c.n, o, static_cast<long long>(per), pl.d_delta.get(), c.d_primes.get(), c.t, c.t_ratio_lo, c.t_ratio_hi, pl.q_mod_t, c.logn,
-                    static_cast<int>(L), subtract ? 1 : 0, total);
+                    plain + (shared ? 0 : b0 * c.n), shared ? 0 : static_cast<long long>(c.n), o, static_cast<long long>(per), pl.d_delta.get(),
+                    c.d_primes.get(), c.t, c.t_ratio_lo, c.t_ratio_hi, pl.q_mod_t, c.logn, static_cast<int>(L), subtract ? 1 : 0, total);
                 c.stats.end(st);
                 cuda_check(cudaGetLastError(), "bfv_add_plain_kernel");
                 continue;
             }
-            u64 *T = static_cast<u64 *>(c.ensure_scratch((B * L * c.n + B) * sizeof(u64)));
-            const u64 *d_cf = upload_cf(c, h_cf ? h_cf + b0 : nullptr, B, T + B * L * c.n, st);
-            plain_to_ntt_dev(c, L, B, plain + b0 * c.n, d_cf, T, st);
-            const long long total = static_cast<long long>(B * L * c.n);
-            c.stats.begin("bgv_add_plain", 0, 24.0 * total, st);
-            add_c0_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(T, o, static_cast<long long>(per), c.d_primes.get(), c.logn,
-                                                                                      static_cast<int>(L), subtract ? 1 : 0, total);
-            c.stats.end(st);
-            cuda_check(cudaGetLastError(), "add_c0_kernel");
+            if (!shared)
+            {
+                T = static_cast<u64 *>(c.ensure_scratch((B * L * c.n + B) * sizeof(u64)));
+                const u64 *d_cf = upload_cf(c, h_cf ? h_cf + b0 : nullptr, B, T + B * L * c.n, st);
+                plain_to_ntt_dev(c, L, B, plain + b0 * c.n, d_cf, T, st);
+            }
+            launch_add_c0(c, "bgv_add_plain", L, size, B, shared, subtract, T, o, st);
+        }
+    }
+
+    void op_add_plain_ntt(Context &c, size_t L, size_t size, size_t batch, bool shared, bool subtract, const u64 *ct, const u64 *plain, u64 *out,
+                          cudaStream_t st)
+    {
+        if (c.scheme == 1) // evaluator.cpp:1774-1782, :1882-1890
+            throw std::invalid_argument("BFV plain cannot be in NTT form");
+        if (c.scheme == 3) // :1798-1806, :1906-1914
+            throw std::invalid_argument("BGV plain cannot be in NTT form");
+        if (c.n < 2 || size < 1)
+            throw std::invalid_argument("encrypted is not valid for encryption parameters");
+        const size_t per = size * L * c.n;
+        if (out != ct)
+            cuda_check(cudaMemcpyAsync(out, ct, batch * per * sizeof(u64), cudaMemcpyDeviceToDevice, st), "copy");
+        const size_t chunk = std::max<size_t>(1, (size_t(1) << 30) / (L * c.n));
+        for (size_t b0 = 0; b0 < batch; b0 += chunk)
+        {
+            const size_t B = std::min(chunk, batch - b0);
+            launch_add_c0(c, subtract ? "ckks_sub_plain" : "ckks_add_plain", L, size, B, shared, subtract, plain + (shared ? 0 : b0 * L * c.n),
+                          out + b0 * per, st);
         }
     }
 
@@ -892,7 +1006,7 @@ namespace sb
         sk.d_pow.grow(powers * row, true); // the old powers are wiped as they are freed
         u64 *s = sk.d_pow.get();
         for (size_t p = sk.powers; p < powers; p++)
-            op_multiply_plain(c, c.k, 1, 1, s + (p - 1) * row, s, s + p * row, st);
+            op_multiply_plain(c, c.k, 1, 1, false, s + (p - 1) * row, s, s + p * row, st);
         sk.powers = powers;
     }
 

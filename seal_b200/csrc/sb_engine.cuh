@@ -168,9 +168,12 @@ namespace sb
     // drivers (all stream-ordered, no synchronisation); slabs as documented in include/seal_b200.h
     void op_ntt(Context &c, bool inverse, size_t L, size_t size, size_t batch, u64 *d, cudaStream_t st);
     void op_linear(Context &c, int mode, size_t L, size_t size, size_t batch, const u64 *a, const u64 *b, u64 *out, cudaStream_t st);
-    void op_multiply_plain(Context &c, size_t L, size_t size, size_t batch, const u64 *a, const u64 *plain, u64 *out, cudaStream_t st);
-    // coefficient-form plaintexts [B][n] (words < t): lift + NTT, multiply_plain, add_plain / sub_plain (BFV, BGV);
-    // h_cf: per-ciphertext BGV correction factors on the host (nullptr = 1)
+    // Plaintext operations take one plaintext per ciphertext, or (shared) one plaintext for the whole batch.
+    // NTT-form plaintexts [B][L][n] or [L][n]: multiply_plain of NTT-form ciphertexts; CKKS add_plain / sub_plain (c_0 only)
+    void op_multiply_plain(Context &c, size_t L, size_t size, size_t batch, bool shared, const u64 *a, const u64 *plain, u64 *out,
+                           cudaStream_t st);
+    void op_add_plain_ntt(Context &c, size_t L, size_t size, size_t batch, bool shared, bool subtract, const u64 *ct, const u64 *plain, u64 *out,
+                          cudaStream_t st);
     // Decryptor::decrypt (decryptor.cpp:62-197): ct [B][size][L][n] -> CKKS: NTT-form plaintexts [B][L][n]; BFV / BGV:
     // coefficient-form plaintexts [B][n].  h_cf: BGV correction factors per ciphertext (nullptr = 1).
     void secret_key_create(Context &c, const u64 *h_sk, SecretKey &out);
@@ -186,11 +189,13 @@ namespace sb
     // BatchEncoder::encode / decode (batchencoder.cpp:84-330): values [B][n] (< t) <-> coefficient-form plaintexts [B][n]
     void op_batch_encode(Context &c, size_t batch, const u64 *values, u64 *plain, cudaStream_t st);
     void op_batch_decode(Context &c, size_t batch, const u64 *plain, u64 *values, cudaStream_t st);
+    // coefficient-form plaintexts [B][n] or [n] (words < t): lift + NTT, multiply_plain, add_plain / sub_plain (BFV, BGV);
+    // h_cf: BGV correction factors on the host, one per plaintext (nullptr = 1)
     void op_plain_to_ntt(Context &c, size_t L, size_t batch, const u64 *plain, const u64 *h_cf, u64 *out, cudaStream_t st);
-    void op_multiply_plain_coeff(Context &c, size_t L, size_t size, size_t batch, bool ct_ntt, const u64 *ct, const u64 *plain, u64 *out,
-                                 cudaStream_t st);
-    void op_add_plain_coeff(Context &c, size_t L, size_t size, size_t batch, bool subtract, const u64 *ct, const u64 *plain, const u64 *h_cf,
-                            u64 *out, cudaStream_t st);
+    void op_multiply_plain_coeff(Context &c, size_t L, size_t size, size_t batch, bool shared, bool ct_ntt, const u64 *ct, const u64 *plain,
+                                 u64 *out, cudaStream_t st);
+    void op_add_plain_coeff(Context &c, size_t L, size_t size, size_t batch, bool shared, bool subtract, const u64 *ct, const u64 *plain,
+                            const u64 *h_cf, u64 *out, cudaStream_t st);
     void op_ckks_multiply(Context &c, size_t L, size_t batch, const u64 *a, const u64 *b, u64 *out3, cudaStream_t st);
     void op_bfv_multiply(Context &c, size_t L, size_t batch, const u64 *a, const u64 *b, u64 *out3, cudaStream_t st);
     // general ciphertext sizes s1 x s2 -> s1+s2-1 (2 x 2 forwards to the specialised kernels above)

@@ -183,6 +183,64 @@ def noise_main():
     return rows
 
 
+PLAIN_BATCH = 512
+
+
+def alternate(fns, rounds=3, reps=5):
+    """median ms per call of each of fns, timed in rounds that alternate between them (CUDA events, warm-up in timeit)"""
+    times = [[] for _ in fns]
+    for _ in range(rounds):
+        for i, f in enumerate(fns):
+            times[i].append(timeit(f, reps))
+    return [sorted(t)[len(t) // 2] for t in times]
+
+
+def plain_main():
+    """plaintext operations on device-resident batches, one plaintext per ciphertext vs one shared by the batch, in place, batch
+    512: CKKS multiply_plain and add_plain at cfg5 and cfg2, BFV multiply_plain with a coefficient-form plaintext at cfg4 (coefficient-
+    form ciphertexts: multiply_plain_normal), BGV add_plain at the cfg4 shape.  Per-ciphertext us and algorithmic GB/s: bytes that
+    must cross HBM (per ciphertext: the polynomials read and written, plus its plaintext; a shared plaintext is counted once)."""
+    print(json.dumps({"gpu": torch.cuda.get_device_name(0), "power_limit": os.popen(
+        "nvidia-smi --query-gpu=power.limit --format=csv,noheader -i 0").read().strip()}), flush=True)
+    g = torch.Generator(device="cuda")
+    g.manual_seed(3)
+    batch, rows = PLAIN_BATCH, []
+    for cfg, scheme, n, bits, t in (("cfg5 CKKS n=65536 k=32", S.CKKS, 65536, [55] * 32, 0), ("cfg2 CKKS n=8192 k=4", S.CKKS, 8192, [54] * 4, 0),
+                                    ("cfg4 BFV n=16384 k=8", S.BFV, 16384, [54] * 8, 786433),
+                                    ("cfg4 shape BGV n=16384 k=8", S.BGV, 16384, [54] * 8, 786433)):
+        mods = S.coeff_modulus_create(n, bits)
+        L = len(mods) - 1
+        ctx = S.Context(scheme, n, mods, t)
+        a = rand_rows(mods, n, (batch, 2), L, g)
+        word = L * n * 8
+        if scheme == S.CKKS:
+            plain = rand_rows(mods, n, (batch,), L, g)
+            ops = [("multiply_plain", lambda cnt: ctx.d_multiply_plain_n(a, plain if cnt > 1 else plain[0], a, L, 2, batch, cnt),
+                    lambda cnt: (4 * batch + (batch if cnt > 1 else 1)) * word),
+                   ("add_plain", lambda cnt: ctx.d_add_plain_ntt(a, plain if cnt > 1 else plain[0], a, L, 2, batch, cnt),
+                    lambda cnt: (2 * batch + (batch if cnt > 1 else 1)) * word)]
+        else:
+            plain = torch.randint(0, t, (batch, n), generator=g, dtype=torch.int64, device="cuda")
+            if scheme == S.BFV:
+                ops = [("multiply_plain (coefficient-form plaintext)",
+                        lambda cnt: ctx.d_multiply_plain_coeff_n(a, plain if cnt > 1 else plain[0], a, L, 2, batch, cnt, False), None)]
+            else:
+                ops = [("add_plain", lambda cnt: ctx.d_add_plain_coeff_n(a, plain if cnt > 1 else plain[0], a, L, 2, batch, cnt),
+                        lambda cnt: 2 * batch * word + (batch if cnt > 1 else 1) * n * 8)]
+        for op, fn, nbytes in ops:
+            per_ms, shared_ms = alternate([lambda: fn(batch), lambda: fn(1)])
+            for form, cnt, ms in (("per-ciphertext", batch, per_ms), ("shared", 1, shared_ms)):
+                res = {"config": cfg, "batch": batch, "op": op, "plaintexts": form, "us_per_ct": ms * 1e3 / batch}
+                if nbytes:
+                    res["GBps"] = nbytes(cnt) / (ms * 1e-3) / 1e9
+                    res["of_HBM_peak"] = res["GBps"] / HBM_PEAK_GBPS
+                rows.append(res)
+                print(json.dumps(res), flush=True)
+        del ctx, a, plain
+        torch.cuda.empty_cache()
+    return rows
+
+
 # the reference on ONE core (BASELINE.md section 2, survey container), ops/s, for scale only
 CPU_1CORE = {
     "cfg1": {"multiply": 277.8, "relinearize": 1041.7, "multiply+relinearize": 219.3, "rotate (1 step)": 1408.5, "ct NTT+INTT": 3225.8},
@@ -230,5 +288,7 @@ if __name__ == "__main__":
         prng_main()
     elif len(sys.argv) == 2 and sys.argv[1] == "--noise-budget":
         noise_main()
+    elif len(sys.argv) == 2 and sys.argv[1] == "--plain":
+        plain_main()
     else:
         main()
