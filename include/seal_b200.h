@@ -355,7 +355,7 @@ int sb200_ciphertext_save(sb200_context *ctx, size_t batch, size_t L, size_t siz
  * level's last prime.  Per ciphertext ONE PRNG (Blake2xb of a 64-byte seed) yields the ternary polynomial u and the two noise
  * polynomials exactly as the reference draws them (u through std::uniform_int_distribution as libstdc++ >= 11 implements it),
  * so the same seed gives the reference's ciphertext bit for bit.  h_seeds = [batch][8] words or NULL = fresh seeds from the OS
- * entropy source.  Synchronises the stream.  Add the plaintext as for the symmetric variant to obtain Encryptor::encrypt. */
+ * entropy source.  Synchronises the stream.  sb200_encrypt_asymmetric adds the plaintext: Encryptor::encrypt. */
 int sb200_public_key_create(sb200_context *ctx, const uint64_t *h_public_key, sb200_public_key **out);
 int sb200_public_key_destroy(sb200_public_key *key);
 int sb200_encrypt_zero_asymmetric(sb200_context *ctx, sb200_public_key *key, size_t L, size_t batch, const uint64_t *h_seeds,
@@ -365,6 +365,15 @@ int sb200_encrypt_zero_asymmetric(sb200_context *ctx, sb200_public_key *key, siz
  * buffer b = SHAKE256(seed || b, 4096 bytes)); any other value returns SB200_E_INVALID_ARG. */
 int sb200_encrypt_zero_asymmetric_prng(sb200_context *ctx, sb200_public_key *key, size_t L, size_t batch, int prng, const uint64_t *h_seeds,
                                        uint64_t *d_out, void *stream);
+/* Encryptor(context, public_key)::encrypt(plain, destination) (encryptor.cpp:176-340) for a batch, one plaintext per ciphertext:
+ * sb200_encrypt_zero_asymmetric_prng, then the plaintexts added to c_0 in one pass over the batch (BGV: lift and transform, then
+ * the add).  d_plain = CKKS: [batch][L][n] NTT form at the level with L primes; BFV / BGV: [batch][n] words < t (zero above the
+ * plaintext's coeff_count), and L must be the first level (k - 1 primes, or 1 when k = 1): anything else is SB200_E_INVALID_ARG.
+ * The result is the reference's word for word under the same seeds (its parms_id: the plaintext's for CKKS, first_parms_id for
+ * BFV / BGV; scale: the plaintext's for CKKS).  d_plain NULL: SB200_E_POINTER; d_plain == d_out: SB200_E_INVALID_ARG.  Every
+ * check runs before the first launch.  Synchronises the stream. */
+int sb200_encrypt_asymmetric(sb200_context *ctx, sb200_public_key *key, size_t L, size_t batch, const uint64_t *d_plain, int prng,
+                             const uint64_t *h_seeds, uint64_t *d_out, void *stream);
 
 /* ---- CKKSEncoder (SURVEY 8f: the data format either side of the path): CKKSEncoder::encode(values, parms_id, scale, plain) and
  * CKKSEncoder::decode(plain, values) (ckks.h:455-807) for a batch.  values = doubles: [batch][count] complex numbers as (re, im)
@@ -395,8 +404,8 @@ int sb200_secret_key_destroy(sb200_secret_key *key);
  * the OS entropy source (what the reference's default UniformRandomGeneratorFactory does, randomgen.cpp:34-50).
  * save_seed != 0 selects the Serializable<Ciphertext> variant (differs for BFV only: which domain c_1 is sampled in);
  * h_public_seeds = NULL or [batch][8]: the seed each c_1 expands from (what a seeded stream carries instead of c_1: send
- * (c_0, seed) over the wire and let the receiver expand, sb200_ciphertext_load).  Add the plaintext (sb200_add for NTT-form CKKS plaintexts, sb200_add_plain_coeff for BFV / BGV)
- * to obtain Encryptor::encrypt_symmetric (encryptor.cpp:199-262). */
+ * (c_0, seed) over the wire and let the receiver expand, sb200_ciphertext_load).  sb200_encrypt_symmetric below adds the plaintext
+ * as c_0 is written: Encryptor::encrypt_symmetric. */
 int sb200_encrypt_zero_symmetric(sb200_context *ctx, sb200_secret_key *key, size_t L, size_t batch, const uint64_t *h_bootstrap_seeds,
                                  int save_seed, uint64_t *d_out, uint64_t *h_public_seeds, void *stream);
 /* the same with both PRNG types given (SEAL's prng_type: 1 = blake2xb, 2 = shake256; any other value returns SB200_E_INVALID_ARG).
@@ -407,6 +416,13 @@ int sb200_encrypt_zero_symmetric(sb200_context *ctx, sb200_secret_key *key, size
 int sb200_encrypt_zero_symmetric_prng(sb200_context *ctx, sb200_secret_key *key, size_t L, size_t batch, int bootstrap_prng,
                                       int ciphertext_prng, const uint64_t *h_bootstrap_seeds, int save_seed, uint64_t *d_out,
                                       uint64_t *h_public_seeds, void *stream);
+/* Encryptor::encrypt_symmetric(plain, destination) (encryptor.cpp:176-340) for a batch, one plaintext per ciphertext: the
+ * plaintext term is added inside the kernels that write c_0 (no extra pass).  Seeds, PRNG types, save_seed and h_public_seeds as
+ * for sb200_encrypt_zero_symmetric_prng; d_plain, levels and errors as for sb200_encrypt_asymmetric.  Both encryption paths cut
+ * the batch into chunks by SB200_LIMIT_SCRATCH_BYTES; the words do not depend on it. */
+int sb200_encrypt_symmetric(sb200_context *ctx, sb200_secret_key *key, size_t L, size_t batch, const uint64_t *d_plain, int bootstrap_prng,
+                            int ciphertext_prng, const uint64_t *h_bootstrap_seeds, int save_seed, uint64_t *d_out, uint64_t *h_public_seeds,
+                            void *stream);
 /* ---- key generation from a given secret key: KeyGenerator(context, secret_key) (keygenerator.cpp:35-52) ----------------------
  * The secret key itself is not sampled here: it comes from seal::KeyGenerator or is loaded.  Every key below is made of key-level
  * encryptions of zero under `key` in NTT form (for every scheme, BFV included; BGV multiplies the noise by t), each drawn from one

@@ -129,7 +129,50 @@ namespace seal_b200
                                                           : static_cast<std::int64_t>(raw[i]);
         }
 
+        // ---- device-resident plaintexts: a PlaintextBatch in coefficient form -> B matrices, decoded on the device
+        // (sb200_batch_decode); only the slots cross PCIe.  The batch must come from this encoder's device context.
+        void decode(const PlaintextBatch &plain, std::vector<std::vector<std::uint64_t>> &destination) const
+        {
+            const std::vector<std::uint64_t> raw = run_decode(plain);
+            destination.resize(plain.batch_);
+            for (std::size_t b = 0; b < plain.batch_; b++)
+                destination[b].assign(raw.begin() + b * slots_, raw.begin() + (b + 1) * slots_);
+        }
+        void decode(const PlaintextBatch &plain, std::vector<std::vector<std::int64_t>> &destination) const
+        {
+            const std::vector<std::uint64_t> raw = run_decode(plain);
+            destination.resize(plain.batch_);
+            for (std::size_t b = 0; b < plain.batch_; b++)
+            {
+                destination[b].resize(slots_);
+                for (std::size_t i = 0; i < slots_; i++)
+                {
+                    const std::uint64_t v = raw[b * slots_ + i];
+                    destination[b][i] = v > (modulus_ >> 1) ? static_cast<std::int64_t>(v) - static_cast<std::int64_t>(modulus_)
+                                                            : static_cast<std::int64_t>(v);
+                }
+            }
+        }
+
     private:
+        std::vector<std::uint64_t> run_decode(const PlaintextBatch &plain) const
+        {
+            if (plain.ctx_ != ctx_ || !plain.d_ || !plain.batch_ || plain.n_ != slots_)
+                throw std::invalid_argument("plain is not valid for encryption parameters");
+            if (plain.ntt_)
+                throw std::invalid_argument("plain cannot be in NTT form");
+            std::vector<std::uint64_t> out(plain.batch_ * slots_);
+            std::uint64_t *d_values = nullptr;
+            status(sb200_device_malloc(ctx_, out.size() * sizeof(std::uint64_t), &d_values));
+            int rc = sb200_batch_decode(ctx_, plain.batch_, plain.d_, d_values, nullptr);
+            if (rc == SB200_OK)
+                rc = sb200_memcpy_d2h(ctx_, out.data(), d_values, out.size() * sizeof(std::uint64_t), nullptr);
+            if (rc == SB200_OK)
+                rc = sb200_stream_synchronize(ctx_, nullptr);
+            sb200_device_free(ctx_, d_values); // on success it leaves the last error alone
+            status(rc);
+            return out;
+        }
         void check_context()
         {
             if (!context_.parameters_set())

@@ -135,6 +135,36 @@ namespace seal_b200
             destination.parms_id_ = parms_id, destination.ntt_ = true, destination.scale_ = scale;
         }
 
+        // ---- device-resident plaintexts: a PlaintextBatch in NTT form -> B vectors of slot_count() values, decoded on the device
+        // (sb200_ckks_decode) with the batch's scale; only the values cross PCIe.  The batch must come from this encoder's context.
+        template <typename T, typename = std::enable_if_t<std::is_same<std::remove_cv_t<T>, double>::value ||
+                                                          std::is_same<std::remove_cv_t<T>, std::complex<double>>::value>>
+        void decode(const PlaintextBatch &plain, std::vector<std::vector<T>> &destination) const
+        {
+            if (plain.ctx_ != ctx_ || !plain.d_ || !plain.batch_ || (plain.ntt_ && !context_.get_context_data(plain.parms_id_)))
+                throw std::invalid_argument("plain is not valid for encryption parameters");
+            if (!plain.ntt_)
+                throw std::invalid_argument("plain is not in NTT form");
+            const std::size_t B = plain.batch_;
+            std::vector<std::complex<double>> out(B * slots_);
+            std::uint64_t *d_values = nullptr;
+            status(sb200_device_malloc(ctx_, out.size() * sizeof(std::complex<double>), &d_values));
+            int rc = sb200_ckks_decode(ctx_, plain.L_, B, plain.d_, plain.scale_, reinterpret_cast<double *>(d_values), nullptr);
+            if (rc == SB200_OK)
+                rc = sb200_memcpy_d2h(ctx_, out.data(), d_values, out.size() * sizeof(std::complex<double>), nullptr);
+            if (rc == SB200_OK)
+                rc = sb200_stream_synchronize(ctx_, nullptr);
+            sb200_device_free(ctx_, d_values); // on success it leaves the last error alone
+            status(rc);
+            destination.resize(B);
+            for (std::size_t b = 0; b < B; b++)
+            {
+                destination[b].resize(slots_);
+                for (std::size_t i = 0; i < slots_; i++)
+                    destination[b][i] = from_complex<T>(out[b * slots_ + i]);
+            }
+        }
+
     private:
         template <typename T>
         void encode_internal(const T *values, std::size_t values_size, seal::parms_id_type parms_id, double scale, seal::Plaintext &destination) const

@@ -150,6 +150,30 @@ namespace seal_b200
             std::fill(plain.begin(), plain.end(), 0);
         }
 
+        // decrypt of every member of a device-resident batch into a device-resident PlaintextBatch: nothing leaves the GPU.  CKKS:
+        // [B][L][n] NTT form with the batch's parms_id and scale; BFV / BGV: [B][n] coefficient form, parms_id_zero (BGV with the
+        // batch's correction factor).  Checks as for the vector overload above.
+        void decrypt(const CiphertextBatch &encrypted, PlaintextBatch &destination)
+        {
+            owned(encrypted);
+            const auto scheme = context_.first_context_data()->parms().scheme();
+            if (encrypted.size_ < SEAL_CIPHERTEXT_SIZE_MIN)
+                throw std::invalid_argument("encrypted is empty");
+            if (scheme == seal::scheme_type::bfv && encrypted.ntt_)
+                throw std::invalid_argument("encrypted cannot be in NTT form");
+            if (scheme != seal::scheme_type::bfv && !encrypted.ntt_)
+                throw std::invalid_argument("encrypted must be in NTT form");
+            const std::size_t B = encrypted.batch_, L = encrypted.L_, n = encrypted.n_;
+            const bool ckks = scheme == seal::scheme_type::ckks;
+            std::vector<std::uint64_t> cf(B, encrypted.cf_);
+            status(destination.reserve(ctx_, B * (ckks ? L * n : n)));
+            status(sb200_decrypt(ctx_, key_, L, encrypted.size_, B, encrypted.d_, scheme == seal::scheme_type::bgv ? cf.data() : nullptr,
+                                 destination.d_, nullptr));
+            destination.batch_ = B, destination.L_ = ckks ? L : 1, destination.n_ = n;
+            destination.parms_id_ = ckks ? encrypted.parms_id_ : seal::parms_id_zero;
+            destination.ntt_ = ckks, destination.scale_ = ckks ? encrypted.scale_ : 1.0;
+        }
+
     private:
         // the reference's scheme and form checks of invariant_noise_budget, in its order (:424-436)
         void check_form(bool is_ntt_form) const

@@ -13,7 +13,8 @@
 // UniformRandomGeneratorFactory::DefaultFactory() (util/rlwe.cpp:329), i.e. of the reference this header is compiled against.
 // Public-key encryption (ternary u, two noise polynomials, the sample one level up divided down:
 // sb200_encrypt_zero_asymmetric_prng) follows the same rule.  Only a custom factory (prng_type::unknown) is rejected.
-// The plaintext is added by the evaluator's device path.  The Serializable<Ciphertext> overloads (seeded output) stay with
+// The plaintext is added on the device by the encryption entry points themselves (sb200_encrypt_symmetric / _asymmetric); device-
+// resident PlaintextBatch -> CiphertextBatch overloads keep the whole path on the GPU.  The Serializable<Ciphertext> overloads (seeded output) stay with
 // seal::Encryptor: Serializable<> cannot be constructed outside the reference.
 #pragma once
 
@@ -86,7 +87,7 @@ namespace seal_b200
         void encrypt_zero(seal::parms_id_type parms_id, seal::Ciphertext &destination, seal::MemoryPoolHandle pool = seal::MemoryManager::GetPool()) const
         {
             std::vector<seal::Ciphertext> one(1);
-            zero_batch(parms_id, 1, one.data(), nullptr, pool, true);
+            zero_batch(parms_id, 1, one.data(), pool, true);
             destination = std::move(one[0]);
         }
         void encrypt_zero(seal::Ciphertext &destination, seal::MemoryPoolHandle pool = seal::MemoryManager::GetPool()) const
@@ -101,7 +102,7 @@ namespace seal_b200
                                     seal::MemoryPoolHandle pool = seal::MemoryManager::GetPool()) const
         {
             std::vector<seal::Ciphertext> one(1);
-            zero_batch(parms_id, 1, one.data(), nullptr, pool, false);
+            zero_batch(parms_id, 1, one.data(), pool, false);
             destination = std::move(one[0]);
         }
         void encrypt_zero_symmetric(seal::Ciphertext &destination, seal::MemoryPoolHandle pool = seal::MemoryManager::GetPool()) const
@@ -123,6 +124,30 @@ namespace seal_b200
             destination.resize(plains.size());
             if (!plains.empty())
                 encrypt_batch(plains.data(), plains.size(), destination.data(), pool, false);
+        }
+
+        // ---- device-resident batches: PlaintextBatch -> CiphertextBatch, nothing crosses PCIe but the seeds ----
+        // Encryptor::encrypt_internal (encryptor.cpp:176-340) for every member, with its checks and messages, all made before anything
+        // is written; the plaintext is added on the device (sb200_encrypt_asymmetric / sb200_encrypt_symmetric).  The seeds come from the
+        // context's factory, one per ciphertext in member order, as the single-ciphertext overloads draw them.  The result carries the
+        // reference's metadata: parms_id the plaintext's (CKKS) or first_parms_id (BFV / BGV), size 2, NTT form for CKKS / BGV, the
+        // plaintext's scale (CKKS) or 1, correction factor 1.  The batches must belong to this encryptor's evaluator.
+        void encrypt(const PlaintextBatch &plain, CiphertextBatch &destination) const
+        {
+            encrypt_device(plain, destination, true);
+        }
+        void encrypt_symmetric(const PlaintextBatch &plain, CiphertextBatch &destination) const
+        {
+            encrypt_device(plain, destination, false);
+        }
+        // `count` encryptions of zero at parms_id into a device batch
+        void encrypt_zero(seal::parms_id_type parms_id, std::size_t count, CiphertextBatch &destination) const
+        {
+            zero_device(parms_id, count, destination, true);
+        }
+        void encrypt_zero_symmetric(seal::parms_id_type parms_id, std::size_t count, CiphertextBatch &destination) const
+        {
+            zero_device(parms_id, count, destination, false);
         }
 
     private:
@@ -168,101 +193,157 @@ namespace seal_b200
                 throw std::logic_error("unsupported prng_type: the device path implements Blake2xbPRNG and Shake256PRNG");
             return static_cast<int>(t);
         }
+        void check_key(bool is_asymmetric) const
+        {
+            if (is_asymmetric && !pk_)
+                throw std::logic_error("public key is not set"); // encryptor.cpp:181-194
+            if (!is_asymmetric && !key_)
+                throw std::logic_error("secret key is not set");
+        }
 
-        // encrypt_zero_internal (encryptor.cpp:88-174, symmetric branch) for `count` ciphertexts into a device slab that is either
-        // downloaded here (d_keep == nullptr) or handed to the caller for the plaintext addition
-        void zero_batch(seal::parms_id_type parms_id, std::size_t count, seal::Ciphertext *out, DeviceSlab *d_keep, const seal::MemoryPoolHandle &pool,
+        // `count` encryptions at the level with L primes into the device slab d_out [count][2][L][n]: of the device plaintexts d_plain
+        // (layout of sb200_encrypt_symmetric), or of zero when d_plain is null.  Seeds from the context's factory, wiped afterwards.
+        void launch(std::size_t L, std::size_t count, const std::uint64_t *d_plain, bool is_asymmetric, std::uint64_t *d_out) const
+        {
+            int prng = 0;
+            std::vector<std::uint64_t> seeds = bootstrap_seeds(count, prng);
+            const int ct_prng = prng_type_of(*seal::UniformRandomGeneratorFactory::DefaultFactory()->create());
+            int rc;
+            if (is_asymmetric)
+                rc = d_plain ? sb200_encrypt_asymmetric(ctx_, pk_, L, count, d_plain, prng, seeds.data(), d_out, nullptr)
+                             : sb200_encrypt_zero_asymmetric_prng(ctx_, pk_, L, count, prng, seeds.data(), d_out, nullptr);
+            else
+                rc = d_plain ? sb200_encrypt_symmetric(ctx_, key_, L, count, d_plain, prng, ct_prng, seeds.data(), 0, d_out, nullptr, nullptr)
+                             : sb200_encrypt_zero_symmetric_prng(ctx_, key_, L, count, prng, ct_prng, seeds.data(), 0, d_out, nullptr, nullptr);
+            seal::util::seal_memzero(seeds.data(), seeds.size() * sizeof(std::uint64_t)); // the seeds determine the noise
+            status(rc);
+        }
+        // storage and metadata of `count` fresh ciphertexts at parms_id (rlwe.cpp:282-287; encrypt_internal's scale)
+        void shape(CiphertextBatch &b, std::size_t count, seal::parms_id_type parms_id, std::size_t L, std::size_t n, double scale) const
+        {
+            const std::size_t words = count * 2 * L * n;
+            if (b.ctx_ != ctx_)
+            {
+                b.release();
+                b.ctx_ = ctx_;
+            }
+            if (b.cap_ < words)
+            {
+                b.release();
+                status(sb200_device_malloc(ctx_, words * sizeof(std::uint64_t), &b.d_));
+                b.cap_ = words;
+            }
+            b.batch_ = count, b.size_ = 2, b.L_ = L, b.n_ = n;
+            b.parms_id_ = parms_id, b.ntt_ = context_.key_context_data()->parms().scheme() != seal::scheme_type::bfv;
+            b.scale_ = scale, b.cf_ = 1;
+        }
+        // encrypt_internal's checks (encryptor.cpp:179-242) -> the parms_id of the result
+        seal::parms_id_type check_plain(bool ntt, seal::parms_id_type parms_id) const
+        {
+            const auto scheme = context_.key_context_data()->parms().scheme();
+            if (scheme == seal::scheme_type::ckks)
+            {
+                if (!ntt)
+                    throw std::invalid_argument("plain must be in NTT form");
+                if (!context_.get_context_data(parms_id))
+                    throw std::invalid_argument("plain is not valid for encryption parameters");
+                return parms_id;
+            }
+            if (ntt)
+                throw std::invalid_argument("plain cannot be in NTT form");
+            return context_.first_parms_id();
+        }
+
+        void encrypt_device(const PlaintextBatch &plain, CiphertextBatch &destination, bool is_asymmetric) const
+        {
+            check_key(is_asymmetric);
+            if (plain.ctx_ != ctx_ || !plain.d_ || !plain.batch_)
+                throw std::invalid_argument("plain is not valid for encryption parameters");
+            if (!plain.ntt_ && plain.n_ != context_.key_context_data()->parms().poly_modulus_degree())
+                throw std::invalid_argument("plain is not valid for encryption parameters");
+            const seal::parms_id_type parms_id = check_plain(plain.ntt_, plain.parms_id_);
+            auto cd = context_.get_context_data(parms_id);
+            const std::size_t L = cd->parms().coeff_modulus().size(), n = cd->parms().poly_modulus_degree();
+            const double scale = plain.ntt_ ? plain.scale_ : 1.0;
+            shape(destination, plain.batch_, parms_id, L, n, scale);
+            launch(L, plain.batch_, plain.d_, is_asymmetric, destination.d_);
+        }
+        void zero_device(seal::parms_id_type parms_id, std::size_t count, CiphertextBatch &destination, bool is_asymmetric) const
+        {
+            check_key(is_asymmetric);
+            auto cd = context_.get_context_data(parms_id);
+            if (!cd)
+                throw std::invalid_argument("parms_id is not valid for encryption parameters");
+            if (!count)
+                throw std::invalid_argument("batch cannot be empty");
+            const std::size_t L = cd->parms().coeff_modulus().size(), n = cd->parms().poly_modulus_degree();
+            shape(destination, count, parms_id, L, n, 1.0);
+            launch(L, count, nullptr, is_asymmetric, destination.d_);
+        }
+
+        // encrypt_zero_internal (encryptor.cpp:88-174) for `count` ciphertexts, downloaded into out
+        void zero_batch(seal::parms_id_type parms_id, std::size_t count, seal::Ciphertext *out, const seal::MemoryPoolHandle &pool,
                         bool is_asymmetric) const
         {
             if (!pool)
                 throw std::invalid_argument("pool is uninitialized");
-            if (is_asymmetric && !pk_)
-                throw std::logic_error("public key is not set"); // encryptor.cpp:181-187
-            if (!is_asymmetric && !key_)
-                throw std::logic_error("secret key is not set");
+            check_key(is_asymmetric);
             auto cd = context_.get_context_data(parms_id);
             if (!cd)
                 throw std::invalid_argument("parms_id is not valid for encryption parameters");
-            auto &parms = cd->parms();
-            const std::size_t L = parms.coeff_modulus().size(), n = parms.poly_modulus_degree(), words = 2 * L * n;
-            int prng = 0;
-            std::vector<std::uint64_t> seeds = bootstrap_seeds(count, prng);
-            const int ct_prng = prng_type_of(*seal::UniformRandomGeneratorFactory::DefaultFactory()->create());
-            DeviceSlab local(ctx_, d_keep ? 1 : count * words);
-            std::uint64_t *d = d_keep ? d_keep->d : local.d;
-            if (is_asymmetric)
-                status(sb200_encrypt_zero_asymmetric_prng(ctx_, pk_, L, count, prng, seeds.data(), d, nullptr));
-            else
-                status(sb200_encrypt_zero_symmetric_prng(ctx_, key_, L, count, prng, ct_prng, seeds.data(), 0, d, nullptr, nullptr));
-            seal::util::seal_memzero(seeds.data(), seeds.size() * sizeof(std::uint64_t)); // the seeds determine the noise
-            const bool ntt = parms.scheme() != seal::scheme_type::bfv;
+            const std::size_t L = cd->parms().coeff_modulus().size(), n = cd->parms().poly_modulus_degree(), words = 2 * L * n;
+            DeviceSlab d(ctx_, count * words);
+            launch(L, count, nullptr, is_asymmetric, d.d);
+            download(d.d, count, parms_id, words, 1.0, out);
+        }
+        void download(const std::uint64_t *d, std::size_t count, seal::parms_id_type parms_id, std::size_t words, double scale,
+                      seal::Ciphertext *out) const
+        {
+            const bool ntt = context_.key_context_data()->parms().scheme() != seal::scheme_type::bfv;
             for (std::size_t b = 0; b < count; b++)
             {
                 out[b].resize(context_, parms_id, 2); // rlwe.cpp:282-287
                 out[b].is_ntt_form() = ntt;
-                out[b].scale() = 1.0;
+                out[b].scale() = scale;
                 out[b].correction_factor() = 1;
             }
-            if (!d_keep)
-                download(d, count, words, out);
-        }
-        void download(const std::uint64_t *d, std::size_t count, std::size_t words, seal::Ciphertext *out) const
-        {
             status(sb200_stream_synchronize(ctx_, nullptr));
             for (std::size_t b = 0; b < count; b++)
                 status(sb200_memcpy_d2h(ctx_, out[b].data(), d + b * words, words * sizeof(std::uint64_t), nullptr));
             status(sb200_stream_synchronize(ctx_, nullptr));
         }
 
+        // one slab upload of the plaintexts, one encryption call, one download
         void encrypt_batch(const seal::Plaintext *plains, std::size_t count, seal::Ciphertext *out, const seal::MemoryPoolHandle &pool,
                            bool is_asymmetric) const
         {
-            if (is_asymmetric && !pk_)
-                throw std::logic_error("public key is not set"); // encryptor.cpp:181-194
-            if (!is_asymmetric && !key_)
-                throw std::logic_error("secret key is not set");
+            check_key(is_asymmetric);
             const auto scheme = context_.key_context_data()->parms().scheme();
             for (std::size_t b = 0; b < count; b++)
             {
                 if (!seal::is_valid_for(plains[b], context_))
                     throw std::invalid_argument("plain is not valid for encryption parameters"); // encryptor.cpp:196-200
-                if (scheme == seal::scheme_type::ckks && !plains[b].is_ntt_form())
-                    throw std::invalid_argument("plain must be in NTT form");
-                if (scheme != seal::scheme_type::ckks && plains[b].is_ntt_form())
-                    throw std::invalid_argument("plain cannot be in NTT form");
+                check_plain(plains[b].is_ntt_form(), plains[b].parms_id());
                 if (scheme == seal::scheme_type::ckks && plains[b].parms_id() != plains[0].parms_id())
                     throw std::invalid_argument("batch members must share parms_id");
             }
-            const seal::parms_id_type parms_id = scheme == seal::scheme_type::ckks ? plains[0].parms_id() : context_.first_parms_id();
+            if (!pool)
+                throw std::invalid_argument("pool is uninitialized");
+            const seal::parms_id_type parms_id = check_plain(plains[0].is_ntt_form(), plains[0].parms_id());
             auto cd = context_.get_context_data(parms_id);
-            if (!cd)
-                throw std::invalid_argument("plain is not valid for encryption parameters");
             const std::size_t L = cd->parms().coeff_modulus().size(), n = cd->parms().poly_modulus_degree(), words = 2 * L * n;
-            DeviceSlab ct(ctx_, count * words);
-            zero_batch(parms_id, count, out, &ct, pool, is_asymmetric);
+            // CKKS: [count][L][n] NTT form; BFV / BGV: [count][n] coefficients, zero above coeff_count
+            const std::size_t pw = scheme == seal::scheme_type::ckks ? L * n : n;
+            std::vector<std::uint64_t> host(count * pw, 0);
+            for (std::size_t b = 0; b < count; b++)
+                std::copy_n(plains[b].data(), std::min(plains[b].coeff_count(), pw), host.begin() + b * pw);
+            DeviceSlab p(ctx_, count * pw), ct(ctx_, count * words);
+            status(sb200_memcpy_h2d(ctx_, p.d, host.data(), host.size() * sizeof(std::uint64_t), nullptr));
+            launch(L, count, p.d, is_asymmetric, ct.d);
+            download(ct.d, count, parms_id, words, 1.0, out);
             if (scheme == seal::scheme_type::ckks)
-            {
-                // c_0 += plain (encryptor.cpp:231-236): the plaintexts go up as a [count][1][L][n] slab and are added row by row
-                DeviceSlab p(ctx_, count * L * n);
                 for (std::size_t b = 0; b < count; b++)
-                    status(sb200_memcpy_h2d(ctx_, p.d + b * L * n, plains[b].data(), L * n * sizeof(std::uint64_t), nullptr));
-                for (std::size_t b = 0; b < count; b++)
-                    status(sb200_add(ctx_, L, 1, 1, ct.d + b * words, p.d + b * L * n, ct.d + b * words, nullptr));
-                for (std::size_t b = 0; b < count; b++)
-                    out[b].scale() = plains[b].scale();
-            }
-            else
-            {
-                // BFV: c_0 += round(q m / t) (multiply_add_plain_with_scaling_variant, encryptor.cpp:211-214);
-                // BGV: c_0 += NTT(lift(m)) (encryptor.cpp:250-330)
-                std::vector<std::uint64_t> coeffs(count * n, 0);
-                for (std::size_t b = 0; b < count; b++)
-                    std::copy_n(plains[b].data(), plains[b].coeff_count(), coeffs.begin() + b * n);
-                DeviceSlab p(ctx_, count * n);
-                status(sb200_memcpy_h2d(ctx_, p.d, coeffs.data(), coeffs.size() * sizeof(std::uint64_t), nullptr));
-                status(sb200_add_plain_coeff(ctx_, L, 2, count, 0, ct.d, p.d, nullptr, ct.d, nullptr));
-            }
-            download(ct.d, count, words, out);
+                    out[b].scale() = plains[b].scale(); // encryptor.cpp:237
         }
 
         static void status(int rc)

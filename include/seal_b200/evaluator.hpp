@@ -80,6 +80,7 @@ namespace seal_b200
     private:
         friend class Evaluator;
         friend class Decryptor;
+        friend class Encryptor;
         sb200_context *ctx_ = nullptr;
         std::uint64_t *d_ = nullptr;
         std::size_t cap_ = 0; // words
@@ -135,6 +136,8 @@ namespace seal_b200
         friend class Evaluator;
         friend class BatchEncoder;
         friend class CKKSEncoder;
+        friend class Encryptor;
+        friend class Decryptor;
         // room for `words` words from the context ctx (a status code of include/seal_b200.h)
         int reserve(sb200_context *ctx, std::size_t words)
         {

@@ -35,7 +35,7 @@ SYMBOLS = [
     "sb200_relinearize_host", "sb200_multiply_relinearize_host", "sb200_rescale_to_next_host",
     "sb200_mod_switch_to_next_host", "sb200_apply_galois_host", "sb200_get_parms_id", "sb200_ciphertext_inspect",
     "sb200_ciphertext_save_size", "sb200_ciphertext_load", "sb200_ciphertext_save", "sb200_secret_key_create",
-    "sb200_secret_key_destroy", "sb200_decrypt", "sb200_decrypt_host", "sb200_invariant_noise_budget", "sb200_invariant_noise_budget_host", "sb200_encrypt_zero_symmetric", "sb200_public_key_create", "sb200_public_key_destroy", "sb200_encrypt_zero_asymmetric", "sb200_encrypt_zero_symmetric_prng", "sb200_encrypt_zero_asymmetric_prng", "sb200_kswitch_key_generate", "sb200_public_key_generate", "sb200_ckks_encode", "sb200_ckks_decode", "sb200_ckks_encode_host", "sb200_ckks_decode_host",
+    "sb200_secret_key_destroy", "sb200_decrypt", "sb200_decrypt_host", "sb200_invariant_noise_budget", "sb200_invariant_noise_budget_host", "sb200_encrypt_zero_symmetric", "sb200_public_key_create", "sb200_public_key_destroy", "sb200_encrypt_zero_asymmetric", "sb200_encrypt_zero_symmetric_prng", "sb200_encrypt_zero_asymmetric_prng", "sb200_encrypt_symmetric", "sb200_encrypt_asymmetric", "sb200_kswitch_key_generate", "sb200_public_key_generate", "sb200_ckks_encode", "sb200_ckks_decode", "sb200_ckks_encode_host", "sb200_ckks_decode_host",
     "sb200_group_create", "sb200_group_destroy", "sb200_group_size", "sb200_group_context", "sb200_group_slice",
     "sb200_group_kswitch_key_create", "sb200_group_kswitch_key_destroy", "sb200_group_multiply_relinearize_host",
     "sb200_group_relinearize_host", "sb200_group_apply_galois_host", "sb200_group_multiply_host", "sb200_group_rescale_to_next_host",
@@ -163,6 +163,8 @@ def lib():
         L.sb200_encrypt_zero_symmetric.argtypes = [vp, vp, sz, sz, _u64p, i32, vp, _u64p, vp]
         L.sb200_encrypt_zero_asymmetric_prng.argtypes = [vp, vp, sz, sz, i32, _u64p, vp, vp]
         L.sb200_encrypt_zero_symmetric_prng.argtypes = [vp, vp, sz, sz, i32, i32, _u64p, i32, vp, _u64p, vp]
+        L.sb200_encrypt_symmetric.argtypes = [vp, vp, sz, sz, vp, i32, i32, _u64p, i32, vp, _u64p, vp]
+        L.sb200_encrypt_asymmetric.argtypes = [vp, vp, sz, sz, vp, i32, _u64p, vp, vp]
         L.sb200_decrypt_host.argtypes = [vp, vp, sz, sz, sz, _u64p, _u64p, _u64p]
         L.sb200_kswitch_key_generate.argtypes = [vp, vp, u32, i32, i32, _u64p, _u64p, C.POINTER(vp)]
         L.sb200_public_key_generate.argtypes = [vp, vp, i32, i32, _u64p, _u64p, C.POINTER(vp)]
@@ -779,6 +781,55 @@ class Context:
                                                        None if seeds is None else _hp(seeds), int(save_seed), _dp(out2),
                                                        None if pub is None else _hp(pub), self._stream()))
         return pub
+
+    def d_encrypt_symmetric(self, sk, plain, out2, L, batch, bootstrap_seeds=None, save_seed=False, want_public_seeds=False,
+                            bootstrap_prng=1, ciphertext_prng=1):
+        """Encryptor.encrypt_symmetric of the device plaintexts `plain` (CKKS: [batch][L][n] NTT form; BFV / BGV: [batch][n] words < t
+        at the first level) into the device slab out2 [batch][2][L][n]; seeds, PRNG types and the returned public seeds as for
+        d_encrypt_zero_symmetric"""
+        seeds = None if bootstrap_seeds is None else np.ascontiguousarray(bootstrap_seeds, dtype=np.uint64).reshape(batch, 8)
+        pub = np.zeros((batch, 8), dtype=np.uint64) if want_public_seeds else None
+        _check(lib().sb200_encrypt_symmetric(self.h, sk.h, L, batch, _dp(plain), bootstrap_prng, ciphertext_prng,
+                                             None if seeds is None else _hp(seeds), int(save_seed), _dp(out2),
+                                             None if pub is None else _hp(pub), self._stream()))
+        return pub
+
+    def d_encrypt_asymmetric(self, pk, plain, out2, L, batch, seeds=None, prng=1):
+        """Encryptor(public key).encrypt of the device plaintexts `plain` (layout as d_encrypt_symmetric) into the device slab out2
+        [batch][2][L][n]; seeds as for d_encrypt_zero_asymmetric"""
+        seeds = None if seeds is None else np.ascontiguousarray(seeds, dtype=np.uint64).reshape(batch, 8)
+        _check(lib().sb200_encrypt_asymmetric(self.h, pk.h, L, batch, _dp(plain), prng, None if seeds is None else _hp(seeds), _dp(out2),
+                                              self._stream()))
+
+    def _encrypt_host(self, plain, L):
+        """host plaintexts -> (device copy, device output slab, batch, level, single) for the host encryption forms"""
+        import torch
+
+        p = np.ascontiguousarray(plain, dtype=np.uint64)
+        single = p.ndim == (2 if self.scheme == CKKS else 1)
+        p = p[None] if single else p
+        if L is None:
+            L = p.shape[1] if self.scheme == CKKS else max(self.k - 1, 1)
+        d_plain = torch.from_numpy(p.view(np.int64)).cuda()
+        out = torch.empty((p.shape[0], 2, L, self.n), dtype=torch.int64, device="cuda")
+        return d_plain, out, p.shape[0], L, single
+
+    def encrypt_symmetric(self, sk, plain, bootstrap_seeds=None, save_seed=False, want_public_seeds=False, bootstrap_prng=1,
+                          ciphertext_prng=1, L=None):
+        """d_encrypt_symmetric on host arrays: plaintexts [B][L][n] (CKKS) / [B][n] (BFV, BGV), or one without the batch axis ->
+        ciphertexts [B][2][L][n] (and the public seeds [B][8] when asked for)"""
+        d_plain, out, B, L, single = self._encrypt_host(plain, L)
+        pub = self.d_encrypt_symmetric(sk, d_plain, out, L, B, bootstrap_seeds, save_seed, want_public_seeds, bootstrap_prng, ciphertext_prng)
+        ct = out.cpu().numpy().view(np.uint64)
+        ct = ct[0] if single else ct
+        return (ct, pub) if want_public_seeds else ct
+
+    def encrypt_asymmetric(self, pk, plain, seeds=None, prng=1, L=None):
+        """d_encrypt_asymmetric on host arrays (layouts as encrypt_symmetric)"""
+        d_plain, out, B, L, single = self._encrypt_host(plain, L)
+        self.d_encrypt_asymmetric(pk, d_plain, out, L, B, seeds, prng)
+        ct = out.cpu().numpy().view(np.uint64)
+        return ct[0] if single else ct
 
     # ---- KeyGenerator(context, secret_key) ----
     def generate_kswitch_key(self, sk, galois_elt=0, seeds=None, bootstrap_prng=1, ciphertext_prng=1, host=True, device=True):

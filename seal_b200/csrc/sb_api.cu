@@ -1741,6 +1741,29 @@ int sb200_encrypt_zero_asymmetric_prng(sb200_context *ctx, sb200_public_key *key
     SB_CATCH
 }
 
+int sb200_encrypt_asymmetric(sb200_context *ctx, sb200_public_key *key, size_t L, size_t batch, const uint64_t *d_plain, int prng,
+                             const uint64_t *h_seeds, uint64_t *d_out, void *stream)
+{
+    SB_NEED(key);
+    SB_NEED(d_plain);
+    SB_NEED(d_out);
+    SB_TRY
+    SB_ENTER_STREAM(ctx, stream)
+    check_level(c, L, batch);
+    if (d_plain == d_out)
+        throw std::invalid_argument("d_plain must not alias d_out");
+    check_prng_type(prng);
+    std::unique_ptr<FreshSeeds> fresh;
+    if (!h_seeds)
+    {
+        fresh = std::make_unique<FreshSeeds>(batch);
+        h_seeds = reinterpret_cast<const uint64_t *>(fresh->words.data());
+    }
+    op_encrypt_asymmetric(c, key->k, L, batch, (const u64 *)d_plain, (const u64 *)h_seeds, prng, (u64 *)d_out, static_cast<cudaStream_t>(stream));
+    return SB200_OK;
+    SB_CATCH
+}
+
 // ---- CKKSEncoder::encode / decode (sb_ckks.cu) ----
 int sb200_ckks_encode(sb200_context *ctx, size_t L, size_t batch, const double *d_values, size_t count, int is_complex, double scale,
                       uint64_t *d_plain, void *stream)
@@ -1790,6 +1813,33 @@ int sb200_encrypt_zero_symmetric_prng(sb200_context *ctx, sb200_secret_key *key,
     op_encrypt_zero_symmetric(c, key->k, L, batch, (const u64 *)h_bootstrap_seeds, bootstrap_prng, ciphertext_prng, save_seed != 0, (u64 *)d_out,
                               (u64 *)h_public_seeds, static_cast<cudaStream_t>(stream));
     // op_encrypt_zero_symmetric synchronised the stream while expanding c_1: the seeds have been consumed and may be wiped
+    return SB200_OK;
+    SB_CATCH
+}
+
+int sb200_encrypt_symmetric(sb200_context *ctx, sb200_secret_key *key, size_t L, size_t batch, const uint64_t *d_plain, int bootstrap_prng,
+                            int ciphertext_prng, const uint64_t *h_bootstrap_seeds, int save_seed, uint64_t *d_out, uint64_t *h_public_seeds,
+                            void *stream)
+{
+    SB_NEED(key);
+    SB_NEED(d_plain);
+    SB_NEED(d_out);
+    SB_TRY
+    SB_ENTER_STREAM(ctx, stream)
+    check_level(c, L, batch);
+    if (d_plain == d_out)
+        throw std::invalid_argument("d_plain must not alias d_out");
+    check_prng_type(bootstrap_prng);
+    check_prng_type(ciphertext_prng);
+    std::unique_ptr<FreshSeeds> fresh;
+    if (!h_bootstrap_seeds)
+    {
+        fresh = std::make_unique<FreshSeeds>(batch);
+        h_bootstrap_seeds = reinterpret_cast<const uint64_t *>(fresh->words.data());
+    }
+    op_encrypt_symmetric(c, key->k, L, batch, (const u64 *)d_plain, (const u64 *)h_bootstrap_seeds, bootstrap_prng, ciphertext_prng, save_seed != 0,
+                         (u64 *)d_out, (u64 *)h_public_seeds, static_cast<cudaStream_t>(stream));
+    // as above: the stream was synchronised while c_1 was expanded
     return SB200_OK;
     SB_CATCH
 }

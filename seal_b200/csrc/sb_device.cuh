@@ -174,6 +174,45 @@ __device__ __forceinline__ u64 mulmod_barrett(u64 a, u64 b, const PrimeDev &P)
     return barrett128(a * b, __umul64hi(a, b), P.q, P.ratio_lo, P.ratio_hi);
 }
 
+// ---- coefficient-form plaintext words (BFV / BGV), shared by the plaintext operations and encryption ----
+// lift of one coefficient-form plaintext word v < t to the prime q: the representative in (-t/2, t/2] modulo q
+// (plain_upper_half_threshold / plain_upper_half_increment, evaluator.cpp:2240-2272, :2101-2127)
+__device__ __forceinline__ u64 plain_lift(u64 v, u64 t, u64 t_mod_q, const PrimeDev &P)
+{
+    u64 r = t > P.q ? barrett64(v, P.q, P.ratio_hi) : v;
+    if (v >= ((t + 1) >> 1))
+        r = csub(r + P.q - t_mod_q, P.q);
+    return r;
+}
+
+// BFV: round(q m / t) of a plaintext word m < t, in two parts (multiply_add_plain_with_scaling_variant, util/scalingvariant.cpp:70-160).
+// bfv_plain_fix = floor((m (q mod t) + (t + 1) / 2) / t), the same for every prime: quotient estimate from the Barrett ratio
+// floor((2^128 - 1) / t), corrected by the remainder.
+__device__ __forceinline__ u64 bfv_plain_fix(u64 m, u64 t, u64 t_ratio_lo, u64 t_ratio_hi, u64 q_mod_t)
+{
+    u64 lo = m * q_mod_t, hi = __umul64hi(m, q_mod_t);
+    const u64 half = (t + 1) >> 1;
+    lo += half, hi += (lo < half);
+    const u64 c0 = __umul64hi(lo, t_ratio_lo);
+    const u64 a_lo = lo * t_ratio_hi, a_hi = __umul64hi(lo, t_ratio_hi), b_lo = hi * t_ratio_lo, b_hi = __umul64hi(hi, t_ratio_lo);
+    u64 s1 = a_lo + c0, carry = (s1 < a_lo);
+    const u64 s2 = s1 + b_lo;
+    carry += (s2 < s1);
+    u64 fix = hi * t_ratio_hi + a_hi + b_hi + carry;
+    u64 rem = lo - fix * t;
+#pragma unroll
+    for (int r = 0; r < 2; r++)
+        if (rem >= t)
+            rem -= t, fix++;
+    return fix;
+}
+// ... and modulo one prime: m floor(q / t) + fix mod q_i, canonical (delta = floor(q / t) mod q_i with its Shoup quotient)
+__device__ __forceinline__ u64 bfv_plain_scaled(u64 m, u64 fix, u64 t, Tw delta, const PrimeDev &P)
+{
+    const u64 mm = t > P.q ? barrett64(m, P.q, P.ratio_hi) : m;
+    return csub(mul_shoup(mm, delta, P.q) + barrett64(fix, P.q, P.ratio_hi), P.q);
+}
+
 // 128-bit accumulate: (hi:lo) += a*b
 __device__ __forceinline__ void mac128(u64 &lo, u64 &hi, u64 a, u64 b)
 {

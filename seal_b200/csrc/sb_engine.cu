@@ -621,7 +621,7 @@ namespace sb
     }
 
     // ---- coefficient-form plaintexts (BFV / BGV): lift, transform, multiply_plain, add_plain / sub_plain ----------------
-    static const Context::PlainLevel &plain_level(Context &c, size_t L)
+    const Context::PlainLevel &plain_level(Context &c, size_t L)
     {
         if (c.scheme == 2 || c.t < 2)
             throw std::invalid_argument("unsupported operation for scheme type");
@@ -665,16 +665,6 @@ namespace sb
         cuda_check(cudaMemcpyAsync(slot, h_cf, B * sizeof(u64), cudaMemcpyHostToDevice, st), "upload correction factors");
         (void)c;
         return slot;
-    }
-
-    // lift of one coefficient-form plaintext word v < t to the prime q: the representative in (-t/2, t/2] modulo q
-    // (plain_upper_half_threshold / plain_upper_half_increment, evaluator.cpp:2240-2272, :2101-2127)
-    __device__ __forceinline__ u64 plain_lift(u64 v, u64 t, u64 t_mod_q, const PrimeDev &P)
-    {
-        u64 r = t > P.q ? barrett64(v, P.q, P.ratio_hi) : v;
-        if (v >= ((t + 1) >> 1))
-            r = csub(r + P.q - t_mod_q, P.q);
-        return r;
     }
 
     // forward transform of lifted plaintexts: rows (b, i) -> out[b][i][:]; cf (optional): plaintext times cf[b] mod t first
@@ -784,27 +774,12 @@ namespace sb
         const long long b = e >> logn;
         const int idx = static_cast<int>(e & ((1 << logn) - 1));
         const u64 m = plain[b * plain_bs + idx];
-        // fix = floor((m * (q mod t) + (t + 1) / 2) / t): quotient estimate from the Barrett ratio, corrected by the remainder
-        u64 lo = m * q_mod_t, hi = __umul64hi(m, q_mod_t);
-        const u64 half = (t + 1) >> 1;
-        lo += half, hi += (lo < half);
-        const u64 c0 = __umul64hi(lo, t_ratio_lo);
-        const u64 a_lo = lo * t_ratio_hi, a_hi = __umul64hi(lo, t_ratio_hi), b_lo = hi * t_ratio_lo, b_hi = __umul64hi(hi, t_ratio_lo);
-        u64 s1 = a_lo + c0, carry = (s1 < a_lo);
-        const u64 s2 = s1 + b_lo;
-        carry += (s2 < s1);
-        u64 fix = hi * t_ratio_hi + a_hi + b_hi + carry;
-        u64 rem = lo - fix * t;
-#pragma unroll
-        for (int r = 0; r < 2; r++)
-            if (rem >= t)
-                rem -= t, fix++;
+        const u64 fix = bfv_plain_fix(m, t, t_ratio_lo, t_ratio_hi, q_mod_t);
         u64 *dst = ct + b * ct_bs + idx;
         for (int i = 0; i < L; i++)
         {
             const PrimeDev P = primes[i];
-            const u64 mm = t > P.q ? barrett64(m, P.q, P.ratio_hi) : m;
-            const u64 scaled = csub(mul_shoup(mm, delta[i], P.q) + barrett64(fix, P.q, P.ratio_hi), P.q);
+            const u64 scaled = bfv_plain_scaled(m, fix, t, delta[i], P);
             const u64 x = dst[static_cast<long long>(i) << logn];
             dst[static_cast<long long>(i) << logn] = subtract ? csub(x + P.q - scaled, P.q) : csub(x + scaled, P.q);
         }

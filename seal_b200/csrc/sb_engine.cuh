@@ -196,6 +196,9 @@ namespace sb
                                  u64 *out, cudaStream_t st);
     void op_add_plain_coeff(Context &c, size_t L, size_t size, size_t batch, bool shared, bool subtract, const u64 *ct, const u64 *plain,
                             const u64 *h_cf, u64 *out, cudaStream_t st);
+    // the constants of the level with L primes for coefficient-form plaintexts (BFV / BGV; builds c.d_t_mod_q and the t ratio too);
+    // std::invalid_argument for CKKS
+    const Context::PlainLevel &plain_level(Context &c, size_t L);
     void op_ckks_multiply(Context &c, size_t L, size_t batch, const u64 *a, const u64 *b, u64 *out3, cudaStream_t st);
     void op_bfv_multiply(Context &c, size_t L, size_t batch, const u64 *a, const u64 *b, u64 *out3, cudaStream_t st);
     // general ciphertext sizes s1 x s2 -> s1+s2-1 (2 x 2 forwards to the specialised kernels above)
@@ -234,6 +237,10 @@ namespace sb
     // the type of the bootstrap PRNG (parms.random_generator()), ct_prng = the type c_1 is expanded with (the DefaultFactory's)
     void op_encrypt_zero_symmetric(Context &c, const SecretKey &sk, size_t L, size_t B, const u64 *h_boot_seeds, int boot_prng, int ct_prng,
                                    bool save_seed, u64 *d_out, u64 *h_public_seeds, cudaStream_t st);
+    // Encryptor::encrypt_symmetric on the device: op_encrypt_zero_symmetric with one plaintext per ciphertext added as c_0 is written.
+    // d_plain: CKKS [B][L][n] NTT form at the level; BFV / BGV [B][n] words < t (L = the first level).  d_plain must not alias d_out.
+    void op_encrypt_symmetric(Context &c, const SecretKey &sk, size_t L, size_t B, const u64 *d_plain, const u64 *h_boot_seeds, int boot_prng,
+                              int ct_prng, bool save_seed, u64 *d_out, u64 *h_public_seeds, cudaStream_t st);
     // KeyGenerator on the device (sb_prng.cu), for a secret key the caller supplies.  What turns a key-level encryption of zero into
     // digit digit0 + b of a key-switching key: s'_j[i] = new_key[j][perm ? perm[i] : i] (sb_prng.cu: enc_kernel MODE 7)
     struct KsFactor
@@ -253,6 +260,9 @@ namespace sb
     // Encryptor(public key)::encrypt_zero on the device (sb_prng.cu): seeds [B][8] on the host for PRNGs of type prng, out [B][2][L][n]
     void public_key_create(Context &c, const u64 *h_pk, PublicKey &out);
     void op_encrypt_zero_asymmetric(Context &c, const PublicKey &pk, size_t L, size_t B, const u64 *h_seeds, int prng, u64 *d_out, cudaStream_t st);
+    // Encryptor(public key)::encrypt: op_encrypt_zero_asymmetric, then the plaintexts (layout as op_encrypt_symmetric) added to c_0
+    void op_encrypt_asymmetric(Context &c, const PublicKey &pk, size_t L, size_t B, const u64 *d_plain, const u64 *h_seeds, int prng, u64 *d_out,
+                               cudaStream_t st);
     // CKKSEncoder::encode / decode (sb_ckks.cu): values = device doubles, [B][count] complex pairs (or reals); plain = [B][L][n] NTT form
     void op_ckks_encode(Context &c, size_t L, size_t B, const double *values, size_t count, bool is_complex, double scale, u64 *plain,
                         cudaStream_t st);

@@ -392,6 +392,14 @@ namespace sb
     // is re-read per prime from L2; the transforms are the library's own (op_ntt).
     namespace
     {
+        // the plaintexts an encryption adds to c_0, one per ciphertext (both pointers null: an encryption of zero)
+        struct EncPlain
+        {
+            const u64 *ntt = nullptr;     // CKKS: [B][L][n], NTT form at the level
+            const u64 *coeff = nullptr;   // BFV / BGV: [B][n], words < t
+            const Tw *delta = nullptr;    // BFV: [L] floor(q / t) mod q_j
+            u64 t = 0, t_ratio_lo = 0, t_ratio_hi = 0, q_mod_t = 0;
+        };
         __device__ __forceinline__ int cbd_noise(const unsigned char *boot, long long i)
         {
             const unsigned short *x = reinterpret_cast<const unsigned short *>(boot + 64 + 6 * i); // 64 + 6 i is even
@@ -406,17 +414,21 @@ namespace sb
             return v ? q - v : 0;
         }
         // MODE 0  tmp = m_j e                 (CKKS m = 1 / BGV m = t mod q_j; transformed afterwards)
-        // MODE 1  c_0 = -(s c_1 + tmp)        (NTT form schemes)
+        //         BGV with a plaintext: tmp = t e - lift(p)  (the transform is linear with canonical outputs, so MODE 1 then
+        //         gives -(s c_1 + NTT(t e)) + NTT(lift(p)), the reference's c_0 word for word: encryptor.cpp:245-336)
+        // MODE 1  c_0 = -(s c_1 + tmp)        (NTT form schemes); CKKS with a plaintext: + p (add_poly_coeffmod, encryptor.cpp:232-235)
         // MODE 2  tmp = c_1                   (BFV with the seed kept: the copy that gets transformed)
         // MODE 3  tmp = s tmp
         // MODE 4  c_0 = -(tmp + e)
         // MODE 5  c_0 = s c_1                 (BFV without the seed: both polynomials are inverse-transformed afterwards)
         // MODE 6  c_0 = -(c_0 + e)
+        //         MODES 4 / 6, BFV with a plaintext: + round(q p / t) (multiply_add_plain_with_scaling_variant, encryptor.cpp:210-213)
         // MODE 7  MODE 1, plus on row j = digit of each digit's c_0: (q_{k-1} mod q_j) s'_j  (a key-switching key, L = k)
         template <int MODE>
         __global__ void __launch_bounds__(256) enc_kernel(u64 *__restrict__ out, u64 *__restrict__ tmp, const u64 *__restrict__ sk,
                                                           const unsigned char *__restrict__ boot, long long boot_bytes, const u64 *__restrict__ mult,
-                                                          KsFactor ks, const PrimeDev *__restrict__ primes, int logn, int L, long long total)
+                                                          KsFactor ks, EncPlain pl, const PrimeDev *__restrict__ primes, int logn, int L,
+                                                          long long total)
         {
             const long long e = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; // over B * L * n
             if (e >= total)
@@ -433,19 +445,35 @@ namespace sb
                 noise = v >= 0 ? static_cast<u64>(v) : P.q - static_cast<u64>(-v);
             }
             if (MODE == 0)
-                tmp[e] = mult ? mulmod_barrett(noise, mult[j], P) : noise;
+            {
+                u64 v = mult ? mulmod_barrett(noise, mult[j], P) : noise;
+                if (pl.coeff)
+                    v = csub(v + P.q - plain_lift(pl.coeff[(b << logn) + i], pl.t, mult[j], P), P.q); // BGV: mult = t mod q_j
+                tmp[e] = v;
+            }
             else if (MODE == 1)
-                *c0 = neg_sum(mulmod_barrett(sk[r], *c1, P), tmp[e], P.q);
+            {
+                u64 v = neg_sum(mulmod_barrett(sk[r], *c1, P), tmp[e], P.q);
+                if (pl.ntt)
+                    v = csub(v + pl.ntt[e], P.q);
+                *c0 = v;
+            }
             else if (MODE == 2)
                 tmp[e] = *c1;
             else if (MODE == 3)
                 tmp[e] = mulmod_barrett(sk[r], tmp[e], P);
-            else if (MODE == 4)
-                *c0 = neg_sum(tmp[e], noise, P.q);
+            else if (MODE == 4 || MODE == 6)
+            {
+                u64 v = neg_sum(MODE == 4 ? tmp[e] : *c0, noise, P.q);
+                if (pl.coeff)
+                {
+                    const u64 m = pl.coeff[(b << logn) + i];
+                    v = csub(v + bfv_plain_scaled(m, bfv_plain_fix(m, pl.t, pl.t_ratio_lo, pl.t_ratio_hi, pl.q_mod_t), pl.t, pl.delta[j], P), P.q);
+                }
+                *c0 = v;
+            }
             else if (MODE == 5)
                 *c0 = mulmod_barrett(sk[r], *c1, P);
-            else if (MODE == 6)
-                *c0 = neg_sum(*c0, noise, P.q);
             else
             {
                 u64 v = neg_sum(mulmod_barrett(sk[r], *c1, P), tmp[e], P.q);
@@ -465,10 +493,11 @@ namespace sb
     // the callers.  h_boot_seeds [B][8]: the seeds of the bootstrap PRNGs (one per ciphertext); d_out [B][2][L][n]; is_ntt_form: the
     // reference's argument of that name (true: NTT form for every scheme, as KeyGenerator asks; false: BFV's coefficient form);
     // h_public_seeds: nullptr or [B][8], receives the seed c_1 of each ciphertext expands from (what Serializable<Ciphertext> stores);
-    // ks: nullptr, or the factor term that turns ciphertext b into digit ks->digit0 + b of a key-switching key (L = k, NTT form)
+    // ks: nullptr, or the factor term that turns ciphertext b into digit ks->digit0 + b of a key-switching key (L = k, NTT form);
+    // pl: the plaintexts added to c_0 (Encryptor::encrypt_internal, encryptor.cpp:176-340), or none
     static void encrypt_zero_symmetric_impl(Context &c, const SecretKey &sk, size_t L, size_t B, const u64 *h_boot_seeds, int boot_prng,
-                                            int ct_prng, bool is_ntt_form, bool save_seed, const KsFactor *ks, u64 *d_out, u64 *h_public_seeds,
-                                            cudaStream_t st)
+                                            int ct_prng, bool is_ntt_form, bool save_seed, const KsFactor *ks, const EncPlain &pl, u64 *d_out,
+                                            u64 *h_public_seeds, cudaStream_t st)
     {
         const long long poly = static_cast<long long>(L) * c.n, total = poly * static_cast<long long>(B);
         // bootstrap stream: whole PRNG buffers covering 64 + 6 n bytes
@@ -503,7 +532,7 @@ namespace sb
         const KsFactor f = ks ? *ks : KsFactor{};
 #define SB_ENC(MODE, name)                                                                                           \
     c.stats.begin(name, 0, 24.0 * total, st);                                                                         \
-    enc_kernel<MODE><<<grid, 256, 0, st>>>(d_out, tmp, s, boot, boot_bytes, mult, f, c.d_primes.get(), logn, Li, total);    \
+    enc_kernel<MODE><<<grid, 256, 0, st>>>(d_out, tmp, s, boot, boot_bytes, mult, f, pl, c.d_primes.get(), logn, Li, total); \
     c.stats.end(st);                                                                                                  \
     cuda_check(cudaGetLastError(), name);
         if (is_ntt_form)
@@ -539,6 +568,40 @@ namespace sb
             cuda_check(cudaStreamSynchronize(st), "synchronize");
     }
 
+    // ciphertexts per chunk of a symmetric encryption at the level with L primes: per ciphertext the noise / product polynomial (aux
+    // arena) and the c_1 stream (scratch arena, expand_impl), plus the bootstrap stream, within the scratch budget
+    static size_t enc_symmetric_chunk(const Context &c, size_t L, size_t B)
+    {
+        const size_t per = 2 * L * c.n * sizeof(u64) + 6 * c.n + kXof + 64;
+        return std::max<size_t>(1, std::min(B, c.scratch_budget / per));
+    }
+
+    static void check_encrypt_symmetric(const Context &c, const SecretKey &sk, size_t L)
+    {
+        if (L < 1 || L > c.k || (c.k > 1 && L == c.k))
+            throw std::invalid_argument("parms_id is not valid for encryption parameters");
+        if (!sk.d_pow || sk.ctx != &c)
+            throw std::invalid_argument("secret key is not valid for encryption parameters");
+    }
+
+    // the batch in chunks: each chunk is one encrypt_zero_symmetric_impl, which wipes its noise and streams.  The words do not depend
+    // on the chunk size: every ciphertext has its own bootstrap seed.
+    static void encrypt_symmetric_chunked(Context &c, const SecretKey &sk, size_t L, size_t B, const EncPlain &pl, const u64 *h_boot_seeds,
+                                          int boot_prng, int ct_prng, bool save_seed, u64 *d_out, u64 *h_public_seeds, cudaStream_t st)
+    {
+        const size_t chunk = enc_symmetric_chunk(c, L, B), poly = L * c.n;
+        for (size_t b0 = 0; b0 < B; b0 += chunk)
+        {
+            EncPlain p = pl;
+            if (p.ntt)
+                p.ntt += b0 * poly;
+            if (p.coeff)
+                p.coeff += b0 * c.n;
+            encrypt_zero_symmetric_impl(c, sk, L, std::min(chunk, B - b0), h_boot_seeds + b0 * 8, boot_prng, ct_prng, c.scheme != 1 /* CKKS, BGV */,
+                                        save_seed, nullptr, p, d_out + b0 * 2 * poly, h_public_seeds ? h_public_seeds + b0 * 8 : nullptr, st);
+        }
+    }
+
     // h_boot_seeds [B][8]: the seeds of the bootstrap PRNGs (one fresh seed per ciphertext); d_out [B][2][L][n];
     // h_public_seeds: nullptr or [B][8], receives the seed c_1 of each ciphertext expands from (what Serializable<Ciphertext> stores)
     void op_encrypt_zero_symmetric(Context &c, const SecretKey &sk, size_t L, size_t B, const u64 *h_boot_seeds, int boot_prng, int ct_prng,
@@ -548,12 +611,38 @@ namespace sb
         check_prng_type(ct_prng);
         if (!B)
             return;
-        if (L < 1 || L > c.k || (c.k > 1 && L == c.k))
-            throw std::invalid_argument("parms_id is not valid for encryption parameters");
-        if (!sk.d_pow || sk.ctx != &c)
-            throw std::invalid_argument("secret key is not valid for encryption parameters");
-        encrypt_zero_symmetric_impl(c, sk, L, B, h_boot_seeds, boot_prng, ct_prng, c.scheme != 1 /* CKKS, BGV */, save_seed, nullptr, d_out,
-                                    h_public_seeds, st);
+        check_encrypt_symmetric(c, sk, L);
+        encrypt_symmetric_chunked(c, sk, L, B, EncPlain{}, h_boot_seeds, boot_prng, ct_prng, save_seed, d_out, h_public_seeds, st);
+    }
+
+    // the level check of a plaintext encryption (BFV / BGV encrypt at first_parms_id, encryptor.cpp:209, :241) and its plaintext terms
+    static EncPlain encrypt_plain(Context &c, size_t L, const u64 *d_plain)
+    {
+        EncPlain pl;
+        if (c.scheme == 2 /* CKKS */)
+        {
+            pl.ntt = d_plain;
+            return pl;
+        }
+        if (L != (c.k > 1 ? c.k - 1 : 1))
+            throw std::invalid_argument("BFV and BGV encrypt at the first level");
+        const Context::PlainLevel &lv = plain_level(c, L);
+        pl.coeff = d_plain;
+        pl.delta = lv.d_delta.get();
+        pl.t = c.t, pl.t_ratio_lo = c.t_ratio_lo, pl.t_ratio_hi = c.t_ratio_hi, pl.q_mod_t = lv.q_mod_t;
+        return pl;
+    }
+
+    void op_encrypt_symmetric(Context &c, const SecretKey &sk, size_t L, size_t B, const u64 *d_plain, const u64 *h_boot_seeds, int boot_prng,
+                              int ct_prng, bool save_seed, u64 *d_out, u64 *h_public_seeds, cudaStream_t st)
+    {
+        check_prng_type(boot_prng);
+        check_prng_type(ct_prng);
+        if (!B)
+            return;
+        check_encrypt_symmetric(c, sk, L);
+        const EncPlain pl = encrypt_plain(c, L, d_plain);
+        encrypt_symmetric_chunked(c, sk, L, B, pl, h_boot_seeds, boot_prng, ct_prng, save_seed, d_out, h_public_seeds, st);
     }
 
     // ------------------------------------------------------------------------------------------------------------------------------
@@ -570,7 +659,7 @@ namespace sb
     void op_generate_public_key(Context &c, const SecretKey &sk, int boot_prng, int ct_prng, const u64 *h_boot_seed, u64 *d_out, cudaStream_t st)
     {
         check_key(c, sk, boot_prng, ct_prng);
-        encrypt_zero_symmetric_impl(c, sk, c.k, 1, h_boot_seed, boot_prng, ct_prng, true, false, nullptr, d_out, nullptr, st);
+        encrypt_zero_symmetric_impl(c, sk, c.k, 1, h_boot_seed, boot_prng, ct_prng, true, false, nullptr, EncPlain{}, d_out, nullptr, st);
     }
 
     // generate_one_kswitch_key: digit j = encrypt_zero_symmetric at the key level + (q_{k-1} mod q_j) s'_j on row j of c_0, with
@@ -594,14 +683,12 @@ namespace sb
             f.new_key = sk.d_pow.get() + c.k * c.n;
         }
         const size_t digits = c.k - 1, poly = c.k * c.n;
-        // per digit: the noise / product polynomial (aux arena) and the c_1 stream (scratch arena, expand_impl), plus the bootstrap stream
-        const size_t per = 2 * poly * sizeof(u64) + 6 * c.n + kXof + 64;
-        const size_t chunk = std::max<size_t>(1, std::min(digits, c.scratch_budget / per));
+        const size_t chunk = enc_symmetric_chunk(c, c.k, digits);
         for (size_t d0 = 0; d0 < digits; d0 += chunk)
         {
             f.digit0 = static_cast<long long>(d0);
             encrypt_zero_symmetric_impl(c, sk, c.k, std::min(chunk, digits - d0), h_boot_seeds + d0 * 8, boot_prng, ct_prng, true, false, &f,
-                                        d_out + d0 * 2 * poly, nullptr, st);
+                                        EncPlain{}, d_out + d0 * 2 * poly, nullptr, st);
         }
     }
 
@@ -714,20 +801,19 @@ namespace sb
             throw std::invalid_argument("public key is not valid for encryption parameters");
     }
 
-    // h_seeds [B][8]: the seed of each ciphertext's PRNG; d_out [B][2][L][n] at the level with L primes (L == k: the key level)
-    void op_encrypt_zero_asymmetric(Context &c, const PublicKey &pk, size_t L, size_t B, const u64 *h_seeds, int prng, u64 *d_out, cudaStream_t st)
+    // stream words per ciphertext: 4 n bytes of ternary words + 12 n bytes of noise + spare words for redraws, in whole PRNG buffers
+    static long long asym_stream_words(const Context &c)
     {
-        check_prng_type(prng);
-        if (!B)
-            return;
-        if (L < 1 || L > c.k)
-            throw std::invalid_argument("parms_id is not valid for encryption parameters");
-        if (!pk.d_key || pk.ctx != &c)
-            throw std::invalid_argument("public key is not valid for encryption parameters");
+        return ((16 * static_cast<long long>(c.n) + 256 + kXof - 1) / kXof) * kWordsPerBuffer;
+    }
+
+    // one chunk of op_encrypt_zero_asymmetric, checks done by the caller
+    static void encrypt_zero_asymmetric_impl(Context &c, const PublicKey &pk, size_t L, size_t B, const u64 *h_seeds, int prng, u64 *d_out,
+                                             cudaStream_t st)
+    {
         const size_t Lp = L < c.k ? L + 1 : L;
         const long long n = static_cast<long long>(c.n), poly = static_cast<long long>(Lp) * n, total1 = static_cast<long long>(B) * poly;
-        // stream: 4 n bytes of ternary words + 12 n bytes of noise + spare words for redraws, in whole PRNG buffers
-        const long long words = ((16 * n + 256 + kXof - 1) / kXof) * kWordsPerBuffer;
+        const long long words = asym_stream_words(c);
         const size_t bytes = (B * words + static_cast<size_t>(total1) * 3 + B * 8 + Lp) * sizeof(u64) + (B + 4) * sizeof(unsigned);
         u64 *W = static_cast<u64 *>(c.ensure_aux(bytes));
         u64 *U = W + B * words, *T = U + total1, *d_seeds = T + 2 * total1, *d_mult = d_seeds + B * 8;
@@ -792,5 +878,52 @@ namespace sb
                 op_mod_switch(c, Lp, 2 * B, T, d_out, st);
         }
         c.wipe_aux(st); // u, the noise and the PRNG stream (util/rlwe.cpp:195: clear-on-destruction pool)
+    }
+
+    static void check_encrypt_asymmetric(const Context &c, const PublicKey &pk, size_t L)
+    {
+        if (L < 1 || L > c.k)
+            throw std::invalid_argument("parms_id is not valid for encryption parameters");
+        if (!pk.d_key || pk.ctx != &c)
+            throw std::invalid_argument("public key is not valid for encryption parameters");
+    }
+
+    // the batch in chunks within the scratch budget (per ciphertext: the PRNG stream, u and the two sampled polynomials, one level
+    // above); each chunk wipes its streams.  The words do not depend on the chunk size: every ciphertext has its own seed.
+    static void encrypt_zero_asymmetric_chunked(Context &c, const PublicKey &pk, size_t L, size_t B, const u64 *h_seeds, int prng, u64 *d_out,
+                                                cudaStream_t st)
+    {
+        const size_t Lp = L < c.k ? L + 1 : L;
+        const size_t per = (static_cast<size_t>(asym_stream_words(c)) + 3 * Lp * c.n + 8) * sizeof(u64) + sizeof(unsigned);
+        const size_t chunk = std::max<size_t>(1, std::min(B, c.scratch_budget / per)), poly = L * c.n;
+        for (size_t b0 = 0; b0 < B; b0 += chunk)
+            encrypt_zero_asymmetric_impl(c, pk, L, std::min(chunk, B - b0), h_seeds + b0 * 8, prng, d_out + b0 * 2 * poly, st);
+    }
+
+    // h_seeds [B][8]: the seed of each ciphertext's PRNG; d_out [B][2][L][n] at the level with L primes (L == k: the key level)
+    void op_encrypt_zero_asymmetric(Context &c, const PublicKey &pk, size_t L, size_t B, const u64 *h_seeds, int prng, u64 *d_out, cudaStream_t st)
+    {
+        check_prng_type(prng);
+        if (!B)
+            return;
+        check_encrypt_asymmetric(c, pk, L);
+        encrypt_zero_asymmetric_chunked(c, pk, L, B, h_seeds, prng, d_out, st);
+    }
+
+    // Encryptor(public key)::encrypt (encryptor.cpp:176-340): the plaintexts are added to c_0 once the sample has been divided down,
+    // by the evaluator's add_plain code in one pass over the batch (BGV: its lift-and-transform, then the add)
+    void op_encrypt_asymmetric(Context &c, const PublicKey &pk, size_t L, size_t B, const u64 *d_plain, const u64 *h_seeds, int prng, u64 *d_out,
+                               cudaStream_t st)
+    {
+        check_prng_type(prng);
+        if (!B)
+            return;
+        check_encrypt_asymmetric(c, pk, L);
+        encrypt_plain(c, L, d_plain); // the level check, before any launch
+        encrypt_zero_asymmetric_chunked(c, pk, L, B, h_seeds, prng, d_out, st);
+        if (c.scheme == 2)
+            op_add_plain_ntt(c, L, 2, B, false, false, d_out, d_plain, d_out, st);
+        else
+            op_add_plain_coeff(c, L, 2, B, false, false, d_out, d_plain, nullptr, d_out, st);
     }
 } // namespace sb

@@ -241,6 +241,59 @@ def plain_main():
     return rows
 
 
+ENCRYPT_CONFIGS = [("CKKS n=65536 k=32", S.CKKS, 65536, [55] * 32, 0, 32), ("CKKS n=8192 k=3", S.CKKS, 8192, [54] * 3, 0, 256),
+                   ("BFV n=16384 k=8", S.BFV, 16384, [54] * 8, 786433, 128), ("BGV n=16384 k=8", S.BGV, 16384, [54] * 8, 786433, 128)]
+
+
+def encrypt_main():
+    """encryption of device-resident plaintexts at the first level, both key types: the fused entry points against the composition
+    they replace (sb200_encrypt_zero_*_prng, then sb200_add_plain_ntt / sb200_add_plain_coeff_n), the same seeds, timed in
+    alternating rounds; us per ciphertext and the launches of one call of each path"""
+    print(json.dumps({"gpu": torch.cuda.get_device_name(0), "power_limit": os.popen(
+        "nvidia-smi --query-gpu=power.limit --format=csv,noheader -i 0").read().strip()}), flush=True)
+    g = torch.Generator(device="cuda")
+    g.manual_seed(7)
+    rows = []
+    for cfg, scheme, n, bits, t, batch in ENCRYPT_CONFIGS:
+        mods = S.coeff_modulus_create(n, bits)
+        k, L = len(mods), len(mods) - 1
+        ctx = S.Context(scheme, n, mods, t)
+        rng = np.random.default_rng(11)
+        sk = ctx.load_secret_key(np.stack([rng.integers(0, mods[i], n, dtype=np.uint64) for i in range(k)]))
+        _, pk = ctx.generate_public_key(sk, seed=rng.integers(0, 2 ** 63, 8, dtype=np.uint64), host=False)
+        seeds = rng.integers(0, 2 ** 63, (batch, 8), dtype=np.uint64)
+        if scheme == S.CKKS:
+            plain = rand_rows(mods, n, (batch,), L, g)
+            add = lambda out: ctx.d_add_plain_ntt(out, plain, out, L, 2, batch, batch)  # noqa: E731
+        else:
+            plain = torch.randint(0, t, (batch, n), generator=g, dtype=torch.int64, device="cuda")
+            add = lambda out: ctx.d_add_plain_coeff_n(out, plain, out, L, 2, batch, batch)  # noqa: E731
+        fused_out = torch.empty((batch, 2, L, n), dtype=torch.int64, device="cuda")
+        comp_out = torch.empty_like(fused_out)
+        paths = {
+            "symmetric": (lambda: ctx.d_encrypt_symmetric(sk, plain, fused_out, L, batch, seeds),
+                          lambda: (ctx.d_encrypt_zero_symmetric(sk, comp_out, L, batch, seeds), add(comp_out))),
+            "public key": (lambda: ctx.d_encrypt_asymmetric(pk, plain, fused_out, L, batch, seeds),
+                           lambda: (ctx.d_encrypt_zero_asymmetric(pk, comp_out, L, batch, seeds), add(comp_out))),
+        }
+        for key, (fused, composed) in paths.items():
+            launches = []
+            for f in (fused, composed):
+                c0 = ctx.launch_count
+                f()
+                launches.append(ctx.launch_count - c0)
+            torch.cuda.synchronize()
+            assert torch.equal(fused_out, comp_out), "the fused and composed paths must give the same words"
+            fused_ms, comp_ms = alternate([fused, composed], rounds=3, reps=3)
+            res = {"config": cfg, "batch": batch, "key": key, "fused_us_per_ct": fused_ms * 1e3 / batch,
+                   "composed_us_per_ct": comp_ms * 1e3 / batch, "fused_launches": launches[0], "composed_launches": launches[1]}
+            rows.append(res)
+            print(json.dumps(res), flush=True)
+        del ctx, sk, pk, plain, fused_out, comp_out
+        torch.cuda.empty_cache()
+    return rows
+
+
 # the reference on ONE core (BASELINE.md section 2, survey container), ops/s, for scale only
 CPU_1CORE = {
     "cfg1": {"multiply": 277.8, "relinearize": 1041.7, "multiply+relinearize": 219.3, "rotate (1 step)": 1408.5, "ct NTT+INTT": 3225.8},
@@ -290,5 +343,7 @@ if __name__ == "__main__":
         noise_main()
     elif len(sys.argv) == 2 and sys.argv[1] == "--plain":
         plain_main()
+    elif len(sys.argv) == 2 and sys.argv[1] == "--encrypt":
+        encrypt_main()
     else:
         main()
