@@ -346,6 +346,18 @@ int sb200_ciphertext_load(sb200_context *ctx, size_t batch, const uint8_t *const
  * the bytes are in place. */
 int sb200_ciphertext_save(sb200_context *ctx, size_t batch, size_t L, size_t size, const uint64_t *d_in, const sb200_ct_info *meta,
                           uint8_t *const *outs, size_t capacity, void *stream);
+/* Serializable<Ciphertext>::save(compr_mode_type::none) of fresh symmetric encryptions (what Encryptor::encrypt_symmetric /
+ * encrypt_zero_symmetric return, ciphertext.cpp:190-247): per ciphertext c_0 and the 64-byte seed c_1 expands from, behind
+ * UniformRandomGeneratorInfo's own header (randomgen.cpp:95-118).  d_in [batch][2][L][n]: only c_0 is read.  d_in must come from
+ * sb200_encrypt_symmetric / sb200_encrypt_zero_symmetric_prng with save_seed != 0, h_public_seeds [batch][8] = the public seeds those
+ * calls returned and prng = their ciphertext_prng (1 blake2xb, 2 shake256): BFV's c_0 differs with and without save_seed, and a
+ * stream whose seed does not belong to its c_0 decrypts to garbage.  meta as for sb200_ciphertext_save.  Errors, all checked before
+ * any byte is written: NULL d_in / meta / h_public_seeds / outs (SB200_E_POINTER), an invalid level or batch 0, a NULL outs[b],
+ * capacity < sb200_ciphertext_save_seeded_size, a PRNG type other than 1 or 2 (SB200_E_INVALID_ARG).  Returns after the bytes are in
+ * place. */
+size_t sb200_ciphertext_save_seeded_size(const sb200_context *ctx, size_t L);
+int sb200_ciphertext_save_seeded(sb200_context *ctx, size_t batch, size_t L, const uint64_t *d_in, const sb200_ct_info *meta,
+                                 const uint64_t *h_public_seeds, int prng, uint8_t *const *outs, size_t capacity, void *stream);
 
 /* ---- public-key encryption (SURVEY 8f rank 4): Encryptor(context, public_key) and Encryptor::encrypt_zero(parms_id, destination)
  * (encryptor.cpp:88-174 -> util::encrypt_zero_asymmetric, util/rlwe.cpp:184-276) for a batch.
@@ -444,6 +456,25 @@ int sb200_kswitch_key_generate(sb200_context *ctx, sb200_secret_key *key, uint32
  * h_bootstrap_seed = [8] or NULL */
 int sb200_public_key_generate(sb200_context *ctx, sb200_secret_key *key, int bootstrap_prng, int ciphertext_prng,
                               const uint64_t *h_bootstrap_seed, uint64_t *h_public_key, sb200_public_key **out);
+/* ---- seed-compressed keys: what KeyGenerator's Serializable<...> overloads save with compr_mode_type::none, byte for byte under the
+ * same bootstrap seeds.  Every member is a seeded ciphertext stream (see sb200_ciphertext_save_seeded) at the key level, NTT form,
+ * scale 1, correction factor 1, whose seed expands with ciphertext_prng.  c_1 never leaves the device.
+ * KeyGenerator::create_public_key() (keygenerator.cpp:96-120): `capacity` >= sb200_ciphertext_save_seeded_size(ctx, k) bytes at out;
+ * *handle (may be NULL) receives the Encryptor key handle of the same key. */
+int sb200_public_key_generate_seeded(sb200_context *ctx, sb200_secret_key *key, int bootstrap_prng, int ciphertext_prng,
+                                     const uint64_t *h_bootstrap_seed, uint8_t *out, size_t capacity, sb200_public_key **handle);
+/* KeyGenerator::create_relin_keys() (galois_elts = {0}, count 1: a RelinKeys object of one slot) or create_galois_keys(galois_elts)
+ * (a GaloisKeys object of n slots; the elements in the order given, duplicates skipped as has_key does, empty slots a bare dim2 = 0),
+ * kswitchkeys.cpp:42-86.  h_bootstrap_seeds = [distinct elements][k-1][8] in draw order, or NULL = fresh seeds from the OS entropy
+ * source.  The digits are generated in the chunks of sb200_kswitch_key_generate; each chunk's c_0 rows are copied from the device to
+ * their place in `out` through the context's page-locked staging while the next chunk is generated, and the bytes do not depend on
+ * SB200_LIMIT_SCRATCH_BYTES.  The _size function returns the stream's length (0 for arguments the generator rejects).  Errors, all
+ * checked before anything is generated: k < 2 (SB200_E_LOGIC "keyswitching is not supported by the context"); an even element or one
+ * >= 2n, 0 mixed with Galois elements, a key of another context, a PRNG type other than 1 or 2, capacity below the _size
+ * (SB200_E_INVALID_ARG); NULL key, galois_elts or out (SB200_E_POINTER).  Synchronous (default stream). */
+size_t sb200_kswitch_keys_save_seeded_size(const sb200_context *ctx, const uint32_t *galois_elts, size_t count);
+int sb200_kswitch_keys_generate_seeded(sb200_context *ctx, sb200_secret_key *key, const uint32_t *galois_elts, size_t count, int bootstrap_prng,
+                                       int ciphertext_prng, const uint64_t *h_bootstrap_seeds, uint8_t *out, size_t capacity);
 /* d_ct [batch][size][L][n] in the scheme's own form -> d_plain: CKKS [batch][L][n] (NTT form, same level; the caller keeps
  * scale and parms_id); BFV [batch][n] coefficients mod t (dot product + decrypt_scale_and_round, rns.cpp:1133-1191);
  * BGV [batch][n] (dot product, INTT, exact base conversion rns.cpp:466-539, times the inverse of the ciphertext's

@@ -14,13 +14,16 @@
 // Public-key encryption (ternary u, two noise polynomials, the sample one level up divided down:
 // sb200_encrypt_zero_asymmetric_prng) follows the same rule.  Only a custom factory (prng_type::unknown) is rejected.
 // The plaintext is added on the device by the encryption entry points themselves (sb200_encrypt_symmetric / _asymmetric); device-
-// resident PlaintextBatch -> CiphertextBatch overloads keep the whole path on the GPU.  The Serializable<Ciphertext> overloads (seeded output) stay with
-// seal::Encryptor: Serializable<> cannot be constructed outside the reference.
+// resident PlaintextBatch -> CiphertextBatch overloads keep the whole path on the GPU.  The overloads without a destination return
+// seal_b200::Serializable<seal::Ciphertext> (serializable.hpp) as the reference's do: seeded for the symmetric ones (c_0 and the seed of
+// c_1, sb200_ciphertext_save_seeded), the full ciphertext for the public-key ones (sb200_ciphertext_save).
 #pragma once
 
 #include "../seal_b200.h"
 #include "evaluator.hpp"
+#include "serializable.hpp"
 #include "seal/seal.h"
+#include <algorithm>
 #include <cstdint>
 #include <cstring>
 #include <stdexcept>
@@ -150,6 +153,34 @@ namespace seal_b200
             zero_device(parms_id, count, destination, false);
         }
 
+        // ---- Serializable overloads (encryptor.h:142-162, 246-266, 302-317, 353-375) ----
+        Serializable<seal::Ciphertext> encrypt(const seal::Plaintext &plain, seal::MemoryPoolHandle pool = seal::MemoryManager::GetPool()) const
+        {
+            return serial(&plain, context_.first_parms_id(), pool, true);
+        }
+        Serializable<seal::Ciphertext> encrypt_zero(seal::parms_id_type parms_id, seal::MemoryPoolHandle pool = seal::MemoryManager::GetPool()) const
+        {
+            return serial(nullptr, parms_id, pool, true);
+        }
+        Serializable<seal::Ciphertext> encrypt_zero(seal::MemoryPoolHandle pool = seal::MemoryManager::GetPool()) const
+        {
+            return serial(nullptr, context_.first_parms_id(), pool, true);
+        }
+        Serializable<seal::Ciphertext> encrypt_symmetric(const seal::Plaintext &plain,
+                                                         seal::MemoryPoolHandle pool = seal::MemoryManager::GetPool()) const
+        {
+            return serial(&plain, context_.first_parms_id(), pool, false);
+        }
+        Serializable<seal::Ciphertext> encrypt_zero_symmetric(seal::parms_id_type parms_id,
+                                                              seal::MemoryPoolHandle pool = seal::MemoryManager::GetPool()) const
+        {
+            return serial(nullptr, parms_id, pool, false);
+        }
+        Serializable<seal::Ciphertext> encrypt_zero_symmetric(seal::MemoryPoolHandle pool = seal::MemoryManager::GetPool()) const
+        {
+            return serial(nullptr, context_.first_parms_id(), pool, false);
+        }
+
     private:
         struct DeviceSlab
         {
@@ -186,6 +217,11 @@ namespace seal_b200
             }
             return seeds;
         }
+        // c_1 is expanded with the default factory's PRNG (util/rlwe.cpp:329)
+        static int ciphertext_prng()
+        {
+            return prng_type_of(*seal::UniformRandomGeneratorFactory::DefaultFactory()->create());
+        }
         static int prng_type_of(seal::UniformRandomGenerator &prng)
         {
             const seal::prng_type t = prng.info().type();
@@ -203,18 +239,24 @@ namespace seal_b200
 
         // `count` encryptions at the level with L primes into the device slab d_out [count][2][L][n]: of the device plaintexts d_plain
         // (layout of sb200_encrypt_symmetric), or of zero when d_plain is null.  Seeds from the context's factory, wiped afterwards.
-        void launch(std::size_t L, std::size_t count, const std::uint64_t *d_plain, bool is_asymmetric, std::uint64_t *d_out) const
+        // public_seeds (symmetric only): nullptr, or [count][8] = the seeds of c_1, with the ciphertexts made for a seeded stream
+        // (save_seed: the Serializable<Ciphertext> variant)
+        void launch(std::size_t L, std::size_t count, const std::uint64_t *d_plain, bool is_asymmetric, std::uint64_t *d_out,
+                    std::uint64_t *public_seeds = nullptr) const
         {
             int prng = 0;
             std::vector<std::uint64_t> seeds = bootstrap_seeds(count, prng);
-            const int ct_prng = prng_type_of(*seal::UniformRandomGeneratorFactory::DefaultFactory()->create());
+            const int ct_prng = ciphertext_prng();
+            const int save_seed = public_seeds ? 1 : 0;
             int rc;
             if (is_asymmetric)
                 rc = d_plain ? sb200_encrypt_asymmetric(ctx_, pk_, L, count, d_plain, prng, seeds.data(), d_out, nullptr)
                              : sb200_encrypt_zero_asymmetric_prng(ctx_, pk_, L, count, prng, seeds.data(), d_out, nullptr);
             else
-                rc = d_plain ? sb200_encrypt_symmetric(ctx_, key_, L, count, d_plain, prng, ct_prng, seeds.data(), 0, d_out, nullptr, nullptr)
-                             : sb200_encrypt_zero_symmetric_prng(ctx_, key_, L, count, prng, ct_prng, seeds.data(), 0, d_out, nullptr, nullptr);
+                rc = d_plain ? sb200_encrypt_symmetric(ctx_, key_, L, count, d_plain, prng, ct_prng, seeds.data(), save_seed, d_out, public_seeds,
+                                                       nullptr)
+                             : sb200_encrypt_zero_symmetric_prng(ctx_, key_, L, count, prng, ct_prng, seeds.data(), save_seed, d_out,
+                                                                 public_seeds, nullptr);
             seal::util::seal_memzero(seeds.data(), seeds.size() * sizeof(std::uint64_t)); // the seeds determine the noise
             status(rc);
         }
@@ -344,6 +386,52 @@ namespace seal_b200
             if (scheme == seal::scheme_type::ckks)
                 for (std::size_t b = 0; b < count; b++)
                     out[b].scale() = plains[b].scale(); // encryptor.cpp:237
+        }
+
+        // one encryption (of `plain`, or of zero at parms_id) as a stream: encrypt_internal's checks and metadata (encryptor.cpp:176-340),
+        // then Serializable<Ciphertext>::save(none) of the result, seeded for the symmetric forms
+        Serializable<seal::Ciphertext> serial(const seal::Plaintext *plain, seal::parms_id_type parms_id, const seal::MemoryPoolHandle &pool,
+                                              bool is_asymmetric) const
+        {
+            check_key(is_asymmetric);
+            const auto scheme = context_.key_context_data()->parms().scheme();
+            double scale = 1.0;
+            if (plain)
+            {
+                if (!seal::is_valid_for(*plain, context_))
+                    throw std::invalid_argument("plain is not valid for encryption parameters"); // encryptor.cpp:196-200
+                parms_id = check_plain(plain->is_ntt_form(), plain->parms_id());
+                if (scheme == seal::scheme_type::ckks)
+                    scale = plain->scale(); // encryptor.cpp:237
+            }
+            else if (!context_.get_context_data(parms_id))
+                throw std::invalid_argument("parms_id is not valid for encryption parameters");
+            if (!pool)
+                throw std::invalid_argument("pool is uninitialized");
+            auto cd = context_.get_context_data(parms_id);
+            const std::size_t L = cd->parms().coeff_modulus().size(), n = cd->parms().poly_modulus_degree();
+            DeviceSlab ct(ctx_, 2 * L * n);
+            std::vector<std::uint64_t> pub(8);
+            std::uint64_t *seeds_out = is_asymmetric ? nullptr : pub.data();
+            if (plain)
+            {
+                // CKKS: [L][n] NTT form; BFV / BGV: [n] coefficients, zero above coeff_count
+                const std::size_t pw = scheme == seal::scheme_type::ckks ? L * n : n;
+                std::vector<std::uint64_t> host(pw, 0);
+                std::copy_n(plain->data(), std::min(plain->coeff_count(), pw), host.begin());
+                DeviceSlab p(ctx_, pw);
+                status(sb200_memcpy_h2d(ctx_, p.d, host.data(), host.size() * sizeof(std::uint64_t), nullptr));
+                launch(L, 1, p.d, is_asymmetric, ct.d, seeds_out);
+            }
+            else
+                launch(L, 1, nullptr, is_asymmetric, ct.d, seeds_out);
+            sb200_ct_info meta{};
+            meta.is_ntt_form = scheme != seal::scheme_type::bfv, meta.scale = scale, meta.correction_factor = 1;
+            std::vector<std::uint8_t> bytes(is_asymmetric ? sb200_ciphertext_save_size(ctx_, L, 2) : sb200_ciphertext_save_seeded_size(ctx_, L));
+            std::uint8_t *out = bytes.data();
+            status(is_asymmetric ? sb200_ciphertext_save(ctx_, 1, L, 2, ct.d, &meta, &out, bytes.size(), nullptr)
+                                 : sb200_ciphertext_save_seeded(ctx_, 1, L, ct.d, &meta, pub.data(), ciphertext_prng(), &out, bytes.size(), nullptr));
+            return Serializable<seal::Ciphertext>(std::move(bytes));
         }
 
         static void status(int rc)

@@ -11,13 +11,17 @@
 // exactly where and in the order the reference draws it (one for the public key, one per digit of every key-switching key, Galois
 // elements in the order given with duplicates skipped), so a context with a seeded factory (Blake2xbPRNGFactory or
 // Shake256PRNGFactory) reproduces the reference's keys bit for bit and the default factory draws from the OS entropy source as the
-// reference does.  Secret-key sampling and the Serializable<...> overloads (seed-compressed output) stay with seal::KeyGenerator:
-// the first is deliberately left to the reference, and Serializable<> cannot be constructed outside it (as in encryptor.hpp).
+// reference does.  The overloads without a destination return seal_b200::Serializable<...> (serializable.hpp): the seed-compressed
+// stream KeyGenerator's Serializable<...> would save, written on the device (sb200_public_key_generate_seeded,
+// sb200_kswitch_keys_generate_seeded) with c_1 never leaving it, from seeds drawn as the destination overloads draw them.
+// Secret-key sampling stays with seal::KeyGenerator, deliberately.
 #pragma once
 
 #include "../seal_b200.h"
 #include "evaluator.hpp"
+#include "serializable.hpp"
 #include "seal/seal.h"
+#include <algorithm>
 #include <cstdint>
 #include <cstring>
 #include <memory>
@@ -102,7 +106,68 @@ namespace seal_b200
             create_galois_keys(context_.key_context_data()->galois_tool()->get_elts_all(), destination);
         }
 
+        // ---- Serializable overloads (keygenerator.h:73-76, 102-105, 160-163, 216-223, 270-273): seeded streams ----
+        Serializable<seal::PublicKey> create_public_key() const
+        {
+            const std::size_t k = context_.key_context_data()->parms().coeff_modulus().size();
+            int prng = 0;
+            std::vector<std::uint64_t> seed = bootstrap_seeds(1, prng);
+            std::vector<std::uint8_t> bytes(sb200_ciphertext_save_seeded_size(ctx_, k));
+            const int rc = sb200_public_key_generate_seeded(ctx_, key_, prng, ciphertext_prng(), seed.data(), bytes.data(), bytes.size(), nullptr);
+            seal::util::seal_memzero(seed.data(), seed.size() * sizeof(std::uint64_t));
+            status(rc);
+            return Serializable<seal::PublicKey>(std::move(bytes));
+        }
+        Serializable<seal::RelinKeys> create_relin_keys()
+        {
+            if (!context_.using_keyswitching())
+                throw std::logic_error("keyswitching is not supported by the context");
+            return Serializable<seal::RelinKeys>(seeded_keys({ 0 }));
+        }
+        Serializable<seal::GaloisKeys> create_galois_keys(const std::vector<std::uint32_t> &galois_elts)
+        {
+            if (!context_.using_keyswitching())
+                throw std::logic_error("keyswitching is not supported by the context");
+            const std::size_t n = context_.key_context_data()->parms().poly_modulus_degree();
+            for (const std::uint32_t elt : galois_elts)
+                if (!(elt & 1) || elt >= 2 * n)
+                    throw std::invalid_argument("Galois element is not valid");
+            return Serializable<seal::GaloisKeys>(seeded_keys(galois_elts));
+        }
+        Serializable<seal::GaloisKeys> create_galois_keys(const std::vector<int> &steps)
+        {
+            if (!context_.key_context_data()->qualifiers().using_batching)
+                throw std::logic_error("encryption parameters do not support batching");
+            return create_galois_keys(context_.key_context_data()->galois_tool()->get_elts_from_steps(steps));
+        }
+        Serializable<seal::GaloisKeys> create_galois_keys()
+        {
+            return create_galois_keys(context_.key_context_data()->galois_tool()->get_elts_all());
+        }
+
     private:
+        // the stream of the keys for `elts` ({0}: relinearization), one bootstrap seed per digit of every distinct element, drawn in
+        // that order (generate_one_kswitch_key for each element, duplicates skipped)
+        std::vector<std::uint8_t> seeded_keys(const std::vector<std::uint32_t> &elts)
+        {
+            std::vector<std::uint32_t> distinct;
+            for (const std::uint32_t e : elts)
+                if (std::find(distinct.begin(), distinct.end(), e) == distinct.end())
+                    distinct.push_back(e);
+            const std::size_t digits = context_.first_context_data()->parms().coeff_modulus().size();
+            const std::uint32_t none = 0;
+            const std::uint32_t *e = elts.empty() ? &none : elts.data(); // an empty list: a GaloisKeys object without keys
+            std::vector<std::uint8_t> bytes(sb200_kswitch_keys_save_seeded_size(ctx_, e, elts.size()));
+            int prng = 0;
+            std::vector<std::uint64_t> seeds = bootstrap_seeds(distinct.size() * digits, prng);
+            if (distinct.empty())
+                prng = 1; // nothing is drawn or generated: an empty GaloisKeys object
+            const int rc = sb200_kswitch_keys_generate_seeded(ctx_, key_, e, elts.size(), prng, ciphertext_prng(), seeds.data(),
+                                                              bytes.data(), bytes.size());
+            seal::util::seal_memzero(seeds.data(), seeds.size() * sizeof(std::uint64_t));
+            status(rc);
+            return bytes;
+        }
         KeyGenerator(const seal::SEALContext &context, const seal::SecretKey &secret_key, const Evaluator *evaluator, int device)
             : context_(context)
         {

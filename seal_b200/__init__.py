@@ -35,7 +35,8 @@ SYMBOLS = [
     "sb200_relinearize_host", "sb200_multiply_relinearize_host", "sb200_rescale_to_next_host",
     "sb200_mod_switch_to_next_host", "sb200_apply_galois_host", "sb200_get_parms_id", "sb200_ciphertext_inspect",
     "sb200_ciphertext_save_size", "sb200_ciphertext_load", "sb200_ciphertext_save", "sb200_secret_key_create",
-    "sb200_secret_key_destroy", "sb200_decrypt", "sb200_decrypt_host", "sb200_invariant_noise_budget", "sb200_invariant_noise_budget_host", "sb200_encrypt_zero_symmetric", "sb200_public_key_create", "sb200_public_key_destroy", "sb200_encrypt_zero_asymmetric", "sb200_encrypt_zero_symmetric_prng", "sb200_encrypt_zero_asymmetric_prng", "sb200_encrypt_symmetric", "sb200_encrypt_asymmetric", "sb200_kswitch_key_generate", "sb200_public_key_generate", "sb200_ckks_encode", "sb200_ckks_decode", "sb200_ckks_encode_host", "sb200_ckks_decode_host",
+    "sb200_secret_key_destroy", "sb200_decrypt", "sb200_decrypt_host", "sb200_invariant_noise_budget", "sb200_invariant_noise_budget_host", "sb200_encrypt_zero_symmetric", "sb200_public_key_create", "sb200_public_key_destroy", "sb200_encrypt_zero_asymmetric", "sb200_encrypt_zero_symmetric_prng", "sb200_encrypt_zero_asymmetric_prng", "sb200_encrypt_symmetric", "sb200_encrypt_asymmetric", "sb200_kswitch_key_generate", "sb200_public_key_generate", "sb200_ciphertext_save_seeded_size", "sb200_ciphertext_save_seeded",
+    "sb200_public_key_generate_seeded", "sb200_kswitch_keys_save_seeded_size", "sb200_kswitch_keys_generate_seeded", "sb200_ckks_encode", "sb200_ckks_decode", "sb200_ckks_encode_host", "sb200_ckks_decode_host",
     "sb200_group_create", "sb200_group_destroy", "sb200_group_size", "sb200_group_context", "sb200_group_slice",
     "sb200_group_kswitch_key_create", "sb200_group_kswitch_key_destroy", "sb200_group_multiply_relinearize_host",
     "sb200_group_relinearize_host", "sb200_group_apply_galois_host", "sb200_group_multiply_host", "sb200_group_rescale_to_next_host",
@@ -168,6 +169,13 @@ def lib():
         L.sb200_decrypt_host.argtypes = [vp, vp, sz, sz, sz, _u64p, _u64p, _u64p]
         L.sb200_kswitch_key_generate.argtypes = [vp, vp, u32, i32, i32, _u64p, _u64p, C.POINTER(vp)]
         L.sb200_public_key_generate.argtypes = [vp, vp, i32, i32, _u64p, _u64p, C.POINTER(vp)]
+        L.sb200_ciphertext_save_seeded_size.restype = sz
+        L.sb200_ciphertext_save_seeded_size.argtypes = [vp, sz]
+        L.sb200_ciphertext_save_seeded.argtypes = [vp, sz, sz, vp, C.POINTER(CtInfo), _u64p, i32, C.POINTER(vp), sz, vp]
+        L.sb200_public_key_generate_seeded.argtypes = [vp, vp, i32, i32, _u64p, vp, sz, C.POINTER(vp)]
+        L.sb200_kswitch_keys_save_seeded_size.restype = sz
+        L.sb200_kswitch_keys_save_seeded_size.argtypes = [vp, C.POINTER(u32), sz]
+        L.sb200_kswitch_keys_generate_seeded.argtypes = [vp, vp, C.POINTER(u32), sz, i32, i32, _u64p, vp, sz]
         L.sb200_invariant_noise_budget.argtypes = [vp, vp, sz, sz, sz, vp, vp, vp]
         L.sb200_invariant_noise_budget_host.argtypes = [vp, vp, sz, sz, sz, _u64p, C.POINTER(i32)]
         _lib = L
@@ -759,6 +767,20 @@ class Context:
         _check(lib().sb200_ciphertext_save(self.h, batch, L, size, _dp(t), meta, outs, cap, self._stream()))
         return [b.raw for b in bufs]
 
+    def d_save_ciphertexts_seeded(self, t, L, batch, public_seeds, prng, is_ntt_form, scale=1.0, correction_factor=1):
+        """Serializable<Ciphertext>::save(compr_mode_type::none) of a device slab [batch][2][L][n] of seeded symmetric encryptions
+        (made with save_seed; public_seeds [batch][8] as they returned them, prng = their ciphertext_prng) -> list of bytes: c_0 and
+        the seed of c_1 per ciphertext"""
+        seeds = np.ascontiguousarray(public_seeds, dtype=np.uint64).reshape(batch, 8)
+        cap = lib().sb200_ciphertext_save_seeded_size(self.h, L)
+        bufs = [C.create_string_buffer(cap) for _ in range(batch)]
+        outs = (C.c_void_p * batch)(*[C.addressof(b) for b in bufs])
+        meta = (CtInfo * batch)()
+        for m in meta:
+            m.is_ntt_form, m.scale, m.correction_factor = int(is_ntt_form), scale, correction_factor
+        _check(lib().sb200_ciphertext_save_seeded(self.h, batch, L, _dp(t), meta, _hp(seeds), prng, outs, cap, self._stream()))
+        return [b.raw for b in bufs]
+
     def load_public_key(self, host_key):
         return PublicKey(self, host_key)
 
@@ -854,6 +876,34 @@ class Context:
         _check(lib().sb200_public_key_generate(self.h, sk.h, bootstrap_prng, ciphertext_prng, None if seed is None else _hp(seed),
                                                None if words is None else _hp(words), C.byref(h) if device else None))
         return words, (PublicKey.wrap(self, h) if device else None)
+
+    def generate_public_key_seeded(self, sk, seed=None, bootstrap_prng=1, ciphertext_prng=1, device=False):
+        """KeyGenerator.create_public_key() as its Serializable<PublicKey> saves it (compr_mode none), generated on the device; seed
+        [8] (None = fresh).  Returns (bytes, PublicKey or None)"""
+        seed = None if seed is None else np.ascontiguousarray(seed, dtype=np.uint64).reshape(8)
+        cap = lib().sb200_ciphertext_save_seeded_size(self.h, self.k)
+        buf = C.create_string_buffer(cap)
+        h = C.c_void_p()
+        _check(lib().sb200_public_key_generate_seeded(self.h, sk.h, bootstrap_prng, ciphertext_prng, None if seed is None else _hp(seed),
+                                                      C.addressof(buf), cap, C.byref(h) if device else None))
+        return buf.raw, (PublicKey.wrap(self, h) if device else None)
+
+    def kswitch_keys_seeded_size(self, galois_elts):
+        e = (C.c_uint32 * max(len(galois_elts), 1))(*galois_elts)
+        return lib().sb200_kswitch_keys_save_seeded_size(self.h, e, len(galois_elts))
+
+    def generate_kswitch_keys_seeded(self, sk, galois_elts, seeds=None, bootstrap_prng=1, ciphertext_prng=1, capacity=None):
+        """KeyGenerator.create_relin_keys() (galois_elts [0]) / create_galois_keys(galois_elts) as their Serializable saves them
+        (compr_mode none), generated on the device; seeds [distinct elements][k-1][8] in draw order (None = fresh) -> bytes"""
+        galois_elts = [int(x) for x in galois_elts]
+        e = (C.c_uint32 * max(len(galois_elts), 1))(*galois_elts)
+        size = lib().sb200_kswitch_keys_save_seeded_size(self.h, e, len(galois_elts))
+        cap = size if capacity is None else capacity
+        buf = C.create_string_buffer(max(cap, 1))
+        seeds = None if seeds is None else np.ascontiguousarray(seeds, dtype=np.uint64)
+        _check(lib().sb200_kswitch_keys_generate_seeded(self.h, sk.h, e, len(galois_elts), bootstrap_prng, ciphertext_prng,
+                                                        None if seeds is None else _hp(seeds), C.addressof(buf), cap))
+        return buf.raw[:size]
 
     def d_relinearize(self, in3, key, out2, L, batch):
         _check(lib().sb200_relinearize(self.h, L, batch, _dp(in3), key.h, _dp(out2), self._stream()))

@@ -369,8 +369,13 @@ namespace
     // The copies run on the lane's own non-blocking stream: they overlap kernels of other batches.  Ordering with the caller's
     // work: a download first waits for everything the legacy default stream has been given so far (the batch operations of the
     // C++ shim enqueue there); an upload returns when the data has arrived, so whatever the caller enqueues next sees it.
-    void rows_transfer(Context &c, bool upload, uint64_t *dev, const uint64_t *const *rows, size_t row_bytes, size_t count)
+    // dev_pitch: bytes from one device row to the next (0: rows are contiguous); after_default = false: the caller has already
+    // synchronised the work that wrote the rows, so the download does not wait for the legacy default stream
+    void rows_transfer(Context &c, bool upload, uint64_t *dev, const uint64_t *const *rows, size_t row_bytes, size_t count, size_t dev_pitch = 0,
+                       bool after_default = true)
     {
+        if (!dev_pitch)
+            dev_pitch = row_bytes;
         if (!count || !row_bytes)
             return;
         IoArena::Lane &ln = c.io.lane[upload ? 0 : 1];
@@ -379,7 +384,7 @@ namespace
         const size_t per = std::max<size_t>(1, (size_t(128) << 20) / row_bytes), stage_bytes = std::min(per, count) * row_bytes;
         ensure_lane(ln, stage_bytes);
         cudaStream_t st = ln.st.get();
-        if (!upload)
+        if (!upload && after_default)
         {
             cuda_check(cudaEventRecord(ln.order.get(), nullptr), "record");
             cuda_check(cudaStreamWaitEvent(st, ln.order.get(), 0), "wait");
@@ -403,8 +408,11 @@ namespace
                 rows_copy(true, stage, rows, row_bytes, r0, r1);
                 cuda_check(cudaMemcpyAsync(d + r0 * row_bytes, stage, (r1 - r0) * row_bytes, cudaMemcpyHostToDevice, st), "H2D");
             }
-            else
+            else if (dev_pitch == row_bytes)
                 cuda_check(cudaMemcpyAsync(stage, d + r0 * row_bytes, (r1 - r0) * row_bytes, cudaMemcpyDeviceToHost, st), "D2H");
+            else
+                cuda_check(cudaMemcpy2DAsync(stage, row_bytes, d + r0 * dev_pitch, dev_pitch, row_bytes, r1 - r0, cudaMemcpyDeviceToHost, st),
+                           "D2H");
             cuda_check(cudaEventRecord(ln.ev[slot].get(), st), "record");
             used[slot] = true, pend[slot] = r0, pend_n[slot] = r1 - r0;
         }
@@ -1911,6 +1919,233 @@ int sb200_kswitch_key_generate(sb200_context *ctx, sb200_secret_key *key, uint32
     SB_CATCH
 }
 
+} // extern "C"
+
+// ---- seed-compressed output: Serializable<Ciphertext> / <PublicKey> / <RelinKeys> / <GaloisKeys>::save(compr_mode_type::none) ----
+namespace
+{
+    // the metadata of a key-level member of a key (util/rlwe.cpp:282-287 with is_ntt_form = true): NTT form, scale 1, correction factor 1
+    sb200_ct_info key_member_info(const Context &c)
+    {
+        sb200_ct_info info{};
+        std::memcpy(info.parms_id, c.parms_ids[c.k - 1].data(), sizeof(info.parms_id));
+        info.size = 2, info.poly_modulus_degree = c.n, info.coeff_modulus_size = c.k, info.data_words = c.k * c.n;
+        info.is_ntt_form = 1, info.scale = 1.0, info.correction_factor = 1;
+        return info;
+    }
+
+    // The keys of one seeded RelinKeys / GaloisKeys stream.  {0} is create_relin_keys (one slot); otherwise create_galois_keys: the
+    // elements in the order given with duplicates skipped (GaloisKeys::has_key, keygenerator.cpp:190-205), in n slots.
+    struct KeySet
+    {
+        std::vector<uint32_t> elts;  // distinct elements in draw order
+        size_t slots = 0;
+        std::vector<size_t> filled;  // their slot indices, ascending
+        size_t slot_of(uint32_t elt) const { return slots == 1 ? 0 : (elt - 1) / 2; }
+    };
+    KeySet key_set(const Context &c, const uint32_t *elts, size_t count)
+    {
+        KeySet s;
+        const bool relin = count == 1 && elts[0] == 0;
+        s.slots = relin ? 1 : c.n;
+        for (size_t i = 0; i < count; i++)
+        {
+            const uint32_t e = elts[i];
+            if (!relin && e == 0)
+                throw std::invalid_argument("galois_elts: 0 (relinearization) cannot be mixed with Galois elements");
+            if (!relin && (!(e & 1) || e >= 2 * c.n))
+                throw std::invalid_argument("Galois element is not valid"); // keygenerator.cpp:195-199
+            if (std::find(s.elts.begin(), s.elts.end(), e) == s.elts.end())
+                s.elts.push_back(e);
+        }
+        for (const uint32_t e : s.elts)
+            s.filled.push_back(s.slot_of(e));
+        std::sort(s.filled.begin(), s.filled.end());
+        return s;
+    }
+    size_t kswitch_stream_bytes(const Context &c, const KeySet &s)
+    {
+        return sbw::kswitch_save_size(s.slots, s.elts.size(), c.k - 1, sbw::seeded_save_size(c.k * c.n));
+    }
+
+    // one staged download in flight on a helper thread while the calling thread generates the next chunk
+    struct PendingCopy
+    {
+        std::thread t;
+        std::exception_ptr err;
+        void wait()
+        {
+            if (t.joinable())
+                t.join();
+            if (err)
+            {
+                std::exception_ptr e = err;
+                err = nullptr;
+                std::rethrow_exception(e);
+            }
+        }
+        ~PendingCopy()
+        {
+            if (t.joinable())
+                t.join();
+        }
+    };
+} // namespace
+
+extern "C" {
+size_t sb200_ciphertext_save_seeded_size(const sb200_context *ctx, size_t L)
+{
+    return ctx ? sbw::seeded_save_size(L * ctx->c->n) : 0;
+}
+
+int sb200_ciphertext_save_seeded(sb200_context *ctx, size_t batch, size_t L, const uint64_t *d_in, const sb200_ct_info *meta,
+                                 const uint64_t *h_public_seeds, int prng, uint8_t *const *outs, size_t capacity, void *stream)
+{
+    SB_NEED(d_in);
+    SB_NEED(meta);
+    SB_NEED(h_public_seeds);
+    SB_NEED(outs);
+    SB_TRY
+    SB_ENTER_STREAM(ctx, stream)
+    check_level(c, L, batch);
+    check_prng_type(prng);
+    auto st = static_cast<cudaStream_t>(stream);
+    const size_t words = L * c.n; // c_0
+    if (capacity < sbw::seeded_save_size(words))
+        throw std::invalid_argument("insufficient size"); // Serialization::Save into a too small buffer
+    for (size_t b = 0; b < batch; b++)
+        if (!outs[b])
+            throw std::invalid_argument("out cannot be null");
+    for (size_t b = 0; b < batch; b++)
+    {
+        sb200_ct_info info = meta[b];
+        std::memcpy(info.parms_id, c.parms_ids[L - 1].data(), sizeof(info.parms_id));
+        info.size = 2, info.poly_modulus_degree = c.n, info.coeff_modulus_size = L, info.data_words = words;
+        sbw::write_seeded(info, prng, reinterpret_cast<const u64 *>(h_public_seeds) + b * 8, outs[b]);
+        cuda_check(cudaMemcpyAsync(outs[b] + sbw::kDataOffset, d_in + b * 2 * words, words * sizeof(u64), cudaMemcpyDeviceToHost, st), "D2H");
+    }
+    cuda_check(cudaStreamSynchronize(st), "synchronize");
+    return SB200_OK;
+    SB_CATCH
+}
+
+int sb200_public_key_generate_seeded(sb200_context *ctx, sb200_secret_key *key, int bootstrap_prng, int ciphertext_prng,
+                                     const uint64_t *h_bootstrap_seed, uint8_t *out, size_t capacity, sb200_public_key **handle)
+{
+    SB_NEED(key);
+    SB_NEED(out);
+    SB_TRY
+    SB_ENTER_STREAM(ctx, nullptr)
+    check_prng_type(bootstrap_prng);
+    check_prng_type(ciphertext_prng);
+    if (!key->k.d_pow || key->k.ctx != &c)
+        throw std::invalid_argument("secret key is not valid for encryption parameters");
+    const sb200_ct_info info = key_member_info(c);
+    if (capacity < sbw::seeded_save_size(info.data_words))
+        throw std::invalid_argument("insufficient size");
+    std::unique_ptr<FreshSeeds> fresh;
+    if (!h_bootstrap_seed)
+    {
+        fresh = std::make_unique<FreshSeeds>(1);
+        h_bootstrap_seed = reinterpret_cast<const uint64_t *>(fresh->words.data());
+    }
+    auto h = std::make_unique<sb200_public_key>();
+    h->k.d_key = DevBuf<u64>(2 * c.k * c.n);
+    h->k.ctx = &c;
+    u64 pub[8];
+    op_generate_public_key(c, key->k, bootstrap_prng, ciphertext_prng, (const u64 *)h_bootstrap_seed, h->k.d_key.get(), nullptr, pub);
+    sbw::write_seeded(info, ciphertext_prng, pub, out);
+    cuda_check(cudaMemcpy(out + sbw::kDataOffset, h->k.d_key.get(), info.data_words * sizeof(u64), cudaMemcpyDeviceToHost), "download c_0");
+    if (handle)
+        *handle = h.release();
+    return SB200_OK;
+    SB_CATCH
+}
+
+size_t sb200_kswitch_keys_save_seeded_size(const sb200_context *ctx, const uint32_t *galois_elts, size_t count)
+{
+    if (!ctx || !galois_elts || ctx->c->k < 2)
+        return 0;
+    try
+    {
+        return kswitch_stream_bytes(*ctx->c, key_set(*ctx->c, galois_elts, count));
+    }
+    catch (const std::exception &e)
+    {
+        g_last_error = e.what();
+        return 0;
+    }
+}
+
+// Each key's digits are generated into one of two device buffers (alternating by key, so that the download of one key's last chunk
+// overlaps the generation of the next key's first); after each chunk, the seed infos are written and the chunk's c_0 rows go to
+// their members through the context's page-locked download lane on a helper thread while the next chunk is generated.
+int sb200_kswitch_keys_generate_seeded(sb200_context *ctx, sb200_secret_key *key, const uint32_t *galois_elts, size_t count, int bootstrap_prng,
+                                       int ciphertext_prng, const uint64_t *h_bootstrap_seeds, uint8_t *out, size_t capacity)
+{
+    SB_NEED(key);
+    SB_NEED(galois_elts);
+    SB_NEED(out);
+    SB_TRY
+    SB_ENTER_STREAM(ctx, nullptr)
+    if (c.k < 2)
+        throw std::logic_error("keyswitching is not supported by the context"); // keygenerator.cpp:329-332
+    const KeySet ks = key_set(c, galois_elts, count);
+    check_prng_type(bootstrap_prng);
+    check_prng_type(ciphertext_prng);
+    if (!key->k.d_pow || key->k.ctx != &c)
+        throw std::invalid_argument("secret key is not valid for encryption parameters");
+    if (capacity < kswitch_stream_bytes(c, ks))
+        throw std::invalid_argument("insufficient size");
+    const size_t digits = c.k - 1, poly = c.k * c.n, E = ks.elts.size();
+    const sb200_ct_info info = key_member_info(c);
+    const size_t member = sbw::seeded_save_size(info.data_words);
+    std::unique_ptr<FreshSeeds> fresh;
+    if (!h_bootstrap_seeds)
+    {
+        fresh = std::make_unique<FreshSeeds>(E * digits);
+        h_bootstrap_seeds = reinterpret_cast<const uint64_t *>(fresh->words.data());
+    }
+    std::vector<size_t> first;
+    sbw::write_kswitch_frame(reinterpret_cast<const u64 *>(info.parms_id), ks.slots, ks.filled, digits, member, out, first);
+    DevBuf<u64> buf[2];
+    buf[0] = DevBuf<u64>(digits * 2 * poly);
+    if (E > 1)
+        buf[1] = DevBuf<u64>(digits * 2 * poly);
+    std::vector<u64> pub(digits * 8); // public seeds: what the stream carries
+    std::vector<uint64_t *> rows(digits);
+    PendingCopy pending; // declared last: joined before the buffers above go away
+    for (size_t e = 0; e < E; e++)
+    {
+        const size_t f = static_cast<size_t>(std::lower_bound(ks.filled.begin(), ks.filled.end(), ks.slot_of(ks.elts[e])) - ks.filled.begin());
+        uint8_t *slot = out + first[f];
+        u64 *d = buf[e & 1].get();
+        op_generate_kswitch_key(c, key->k, ks.elts[e], bootstrap_prng, ciphertext_prng, (const u64 *)h_bootstrap_seeds + e * digits * 8, d, nullptr,
+                                pub.data(), [&](size_t d0, size_t cnt) {
+                                    pending.wait();
+                                    for (size_t j = d0; j < d0 + cnt; j++)
+                                    {
+                                        sbw::write_seeded(info, ciphertext_prng, pub.data() + j * 8, slot + j * member);
+                                        rows[j] = reinterpret_cast<uint64_t *>(slot + j * member + sbw::kDataOffset);
+                                    }
+                                    // the chunk is complete (op_generate_kswitch_key synchronised): no wait on the default stream
+                                    pending.t = std::thread([&c, &pending, &rows, d, d0, cnt, poly] {
+                                        try
+                                        {
+                                            rows_transfer(c, false, reinterpret_cast<uint64_t *>(d + d0 * 2 * poly), rows.data() + d0, poly * sizeof(u64), cnt,
+                                                          2 * poly * sizeof(u64), false);
+                                        }
+                                        catch (...)
+                                        {
+                                            pending.err = std::current_exception();
+                                        }
+                                    });
+                                });
+    }
+    pending.wait();
+    return SB200_OK;
+    SB_CATCH
+}
 } // extern "C"
 
 // the decryption phases and plaintexts do not stay behind in the arenas (the reference decrypts inside a clear-on-destruction pool,

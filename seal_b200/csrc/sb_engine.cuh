@@ -6,6 +6,7 @@
 #include "sb_ksint.cuh"
 #include "sb_wire.hpp"
 #include <array>
+#include <functional>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -249,12 +250,15 @@ namespace sb
         const uint32_t *perm = nullptr; // NTT-form Galois table, or nullptr
         long long digit0 = 0;
     };
-    // KeyGenerator::create_public_key: h_boot_seed [8], d_out [2][k][n]
-    void op_generate_public_key(Context &c, const SecretKey &sk, int boot_prng, int ct_prng, const u64 *h_boot_seed, u64 *d_out, cudaStream_t st);
+    // KeyGenerator::create_public_key: h_boot_seed [8], d_out [2][k][n]; h_public_seed: nullptr or [8], the seed c_1 expands from
+    // (the stream synchronised on return)
+    void op_generate_public_key(Context &c, const SecretKey &sk, int boot_prng, int ct_prng, const u64 *h_boot_seed, u64 *d_out, cudaStream_t st,
+                                u64 *h_public_seed = nullptr);
     // KeyGenerator::create_relin_keys (galois_elt = 0) / the key of one Galois element: h_boot_seeds [k-1][8] (one per digit),
-    // d_out [k-1][2][k][n].  Returns once the host seeds have been consumed (they may be wiped then).
+    // d_out [k-1][2][k][n].  Returns once the host seeds have been consumed (they may be wiped then).  h_public_seeds: nullptr or
+    // [k-1][8], each digit's public seed; with it, on_chunk(d0, count) (if set) runs after each chunk of digits is complete on the device.
     void op_generate_kswitch_key(Context &c, SecretKey &sk, uint32_t galois_elt, int boot_prng, int ct_prng, const u64 *h_boot_seeds, u64 *d_out,
-                                 cudaStream_t st);
+                                 cudaStream_t st, u64 *h_public_seeds = nullptr, const std::function<void(size_t, size_t)> &on_chunk = {});
     // Decryptor::compute_secret_key_array (sb_engine.cu): s^1 .. s^powers at the key level in sk.d_pow
     void ensure_key_powers(Context &c, SecretKey &sk, size_t powers, cudaStream_t st);
     // Encryptor(public key)::encrypt_zero on the device (sb_prng.cu): seeds [B][8] on the host for PRNGs of type prng, out [B][2][L][n]

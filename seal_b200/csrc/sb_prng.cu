@@ -656,18 +656,20 @@ namespace sb
             throw std::invalid_argument("secret key is not valid for encryption parameters");
     }
 
-    void op_generate_public_key(Context &c, const SecretKey &sk, int boot_prng, int ct_prng, const u64 *h_boot_seed, u64 *d_out, cudaStream_t st)
+    void op_generate_public_key(Context &c, const SecretKey &sk, int boot_prng, int ct_prng, const u64 *h_boot_seed, u64 *d_out, cudaStream_t st,
+                                u64 *h_public_seed)
     {
         check_key(c, sk, boot_prng, ct_prng);
-        encrypt_zero_symmetric_impl(c, sk, c.k, 1, h_boot_seed, boot_prng, ct_prng, true, false, nullptr, EncPlain{}, d_out, nullptr, st);
+        encrypt_zero_symmetric_impl(c, sk, c.k, 1, h_boot_seed, boot_prng, ct_prng, true, false, nullptr, EncPlain{}, d_out, h_public_seed, st);
     }
 
     // generate_one_kswitch_key: digit j = encrypt_zero_symmetric at the key level + (q_{k-1} mod q_j) s'_j on row j of c_0, with
     // s' = s^2 (relinearization, the key array of compute_secret_key_array) or s seen through the NTT-form Galois permutation
     // (apply_galois_ntt, galois.cpp:148-160), which the combine kernel reads in place: the permuted key is never stored.  The digits
-    // are cut into chunks by the scratch budget; each chunk is one batch of encryptions and wipes its noise and streams.
+    // are cut into chunks by the scratch budget; each chunk is one batch of encryptions and wipes its noise and streams.  With
+    // h_public_seeds, each chunk's public seeds are in place and its digits complete when on_chunk(d0, count) is called.
     void op_generate_kswitch_key(Context &c, SecretKey &sk, uint32_t galois_elt, int boot_prng, int ct_prng, const u64 *h_boot_seeds, u64 *d_out,
-                                 cudaStream_t st)
+                                 cudaStream_t st, u64 *h_public_seeds, const std::function<void(size_t, size_t)> &on_chunk)
     {
         if (galois_elt && (!(galois_elt & 1) || galois_elt >= 2 * c.n))
             throw std::invalid_argument("Galois element is not valid"); // keygenerator.cpp:195-199
@@ -687,8 +689,11 @@ namespace sb
         for (size_t d0 = 0; d0 < digits; d0 += chunk)
         {
             f.digit0 = static_cast<long long>(d0);
-            encrypt_zero_symmetric_impl(c, sk, c.k, std::min(chunk, digits - d0), h_boot_seeds + d0 * 8, boot_prng, ct_prng, true, false, &f,
-                                        EncPlain{}, d_out + d0 * 2 * poly, nullptr, st);
+            const size_t cnt = std::min(chunk, digits - d0);
+            encrypt_zero_symmetric_impl(c, sk, c.k, cnt, h_boot_seeds + d0 * 8, boot_prng, ct_prng, true, false, &f, EncPlain{},
+                                        d_out + d0 * 2 * poly, h_public_seeds ? h_public_seeds + d0 * 8 : nullptr, st);
+            if (on_chunk)
+                on_chunk(d0, cnt);
         }
     }
 

@@ -245,10 +245,55 @@ namespace sbw
         info.stream_bytes = outer.size;
     }
 
+    namespace
+    {
+        // the prefix of a ciphertext stream of `object_bytes` bytes in all (SEALHeader::size)
+        void write_prefix_sized(const sb200_ct_info &info, uint8_t *out, size_t object_bytes);
+    }
     void write_prefix(const sb200_ct_info &info, uint8_t *out)
     {
+        write_prefix_sized(info, out, save_size(info.data_words));
+    }
+
+    void write_seeded(const sb200_ct_info &info, int prng, const u64 seed[8], uint8_t *out)
+    {
+        write_prefix_sized(info, out, seeded_save_size(info.data_words));
+        uint8_t *w = out + kDataOffset + 8 * info.data_words;
+        const Header h{ kMagic, static_cast<uint8_t>(kHeaderBytes), kMajor, kMinor, 0, 0, kSeedInfoBytes };
+        put(w, h);
+        put<uint8_t>(w, static_cast<uint8_t>(prng));
+        std::memcpy(w, seed, 64);
+    }
+
+    void write_kswitch_frame(const u64 parms_id[4], size_t slots, const std::vector<size_t> &filled, size_t digits, size_t member_bytes,
+                             uint8_t *out, std::vector<size_t> &first_member)
+    {
         uint8_t *w = out;
-        Header h{ kMagic, static_cast<uint8_t>(kHeaderBytes), kMajor, kMinor, 0, 0, save_size(info.data_words) };
+        const Header h{ kMagic, static_cast<uint8_t>(kHeaderBytes), kMajor, kMinor, 0, 0,
+                        kswitch_save_size(slots, filled.size(), digits, member_bytes) };
+        put(w, h);
+        for (int i = 0; i < 4; i++)
+            put<uint64_t>(w, parms_id[i]);
+        put<uint64_t>(w, slots);
+        first_member.assign(filled.size(), 0);
+        for (size_t slot = 0, f = 0; slot < slots; slot++)
+        {
+            const bool full = f < filled.size() && filled[f] == slot;
+            put<uint64_t>(w, full ? digits : 0);
+            if (full)
+            {
+                first_member[f++] = static_cast<size_t>(w - out);
+                w += digits * member_bytes;
+            }
+        }
+    }
+
+    namespace
+    {
+    void write_prefix_sized(const sb200_ct_info &info, uint8_t *out, size_t object_bytes)
+    {
+        uint8_t *w = out;
+        Header h{ kMagic, static_cast<uint8_t>(kHeaderBytes), kMajor, kMinor, 0, 0, object_bytes };
         put(w, h);
         for (int i = 0; i < 4; i++)
             put<uint64_t>(w, info.parms_id[i]);
@@ -262,6 +307,7 @@ namespace sbw
         put(w, h);
         put<uint64_t>(w, info.data_words);
     }
+    } // namespace
     void inspect_kswitch(const uint8_t *p, size_t len, size_t index, KSwitchEntry &entry)
     {
         if (!p)

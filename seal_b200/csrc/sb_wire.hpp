@@ -34,6 +34,26 @@ namespace sbw
     inline size_t save_size(size_t words) { return kDataOffset + 8 * words; }
     // writes everything in front of the coefficient words (kDataOffset bytes) for a ciphertext of info.data_words words
     void write_prefix(const sb200_ct_info &info, uint8_t *out);
+
+    // ---- seed-compressed objects (Serializable<Ciphertext> / <PublicKey> / <RelinKeys> / <GaloisKeys> saved with compr_mode none) ----
+    // A seeded ciphertext stream (ciphertext.cpp:190-247, the has_seed_marker branch): the prefix above with a DynArray of the c_0 words
+    // only, the words, then UniformRandomGeneratorInfo::save (randomgen.cpp:95-118): its own SEALHeader, prng_type (1 byte), seed (64 bytes).
+    constexpr size_t kSeedInfoBytes = kHeaderBytes + 1 + 64;
+    inline size_t seeded_save_size(size_t c0_words) { return kDataOffset + 8 * c0_words + kSeedInfoBytes; }
+    // writes everything of a seeded stream except the c_0 words (out + kDataOffset .. + 8 info.data_words): info.data_words = L n,
+    // info.size = 2; prng = the prng_type c_1 expands with, seed = its 8 words
+    void write_seeded(const sb200_ct_info &info, int prng, const u64 seed[8], uint8_t *out);
+    // A KSwitchKeys stream (kswitchkeys.cpp:42-86): SEALHeader, parms_id, dim1 = slots, then per slot dim2 and dim2 member streams.
+    // `filled` = the indices of the slots that hold `digits` members of member_bytes each, in ascending order; every other slot is a
+    // bare dim2 = 0.  RelinKeys: slots 1, filled {0}; GaloisKeys: slots n, filled {(elt - 1) / 2}.
+    inline size_t kswitch_save_size(size_t slots, size_t filled, size_t digits, size_t member_bytes)
+    {
+        return kHeaderBytes + 32 + 8 + 8 * slots + filled * digits * member_bytes;
+    }
+    // writes the frame (header, parms_id, dim1, every dim2) and returns in first_member[i] the byte offset of the first member of
+    // filled[i]; the members of a slot follow one another
+    void write_kswitch_frame(const u64 parms_id[4], size_t slots, const std::vector<size_t> &filled, size_t digits, size_t member_bytes,
+                             uint8_t *out, std::vector<size_t> &first_member);
     // One entry of a serialized KSwitchKeys object (RelinKeys / GaloisKeys saved with compr_mode_type::none,
     // kswitchkeys.cpp:42-86: SEALHeader, parms_id, dim1, then per slot dim2 and dim2 PublicKey = Ciphertext streams).
     // Returns the byte offsets (from p) of the coefficient words of data()[index][j], j < digits, each 2*L*n words, or L*n words
