@@ -193,6 +193,22 @@ int sb200_square(sb200_context *ctx, size_t L, size_t batch, const uint64_t *d_a
 int sb200_add(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *d_a, const uint64_t *d_b, uint64_t *d_out, void *stream);
 int sb200_sub(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *d_a, const uint64_t *d_b, uint64_t *d_out, void *stream);
 int sb200_negate(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *d_a, uint64_t *d_out, void *stream);
+/* Evaluator::add_many (evaluator.cpp:236-262) generalised to a left fold of add_inplace / sub_inplace steps (:155-350), in one
+ * pass over the operands.  Operand j (0 <= j < count) is d_operands[j], [batch][sizes[j]][L][n], 1 <= sizes[j] <= 16; d_out is
+ * [batch][max sizes[j]][L][n].  Step j >= 1 folds operand j into the accumulator with modes[j - 1]: SB200_FOLD_ADD (0) or
+ * SB200_FOLD_SUB (1), optionally ORed with SB200_FOLD_SCALED (2): before the step the accumulator's present polynomials are
+ * multiplied by h_factors[2 (j - 1)] and operand j by h_factors[2 (j - 1) + 1] (BGV correction-factor balancing,
+ * :188-209; the factors are host words, reduced mod each prime here).  modes may be NULL (every step adds); h_factors may be
+ * NULL when no step is scaled.  A polynomial no earlier operand has is copied (add) or negated (sub), as the reference copies or
+ * negates the longer operand's tail.  The words equal those of the chained add / sub calls for any input words.
+ * Errors, all before the first launch: count = 0 or a size outside 1..16 or a mode outside 0..3 (SB200_E_INVALID_ARG); a NULL
+ * operand, d_out, sizes or (with a scaled step) h_factors (SB200_E_POINTER); d_out equal to an operand other than operand 0, or
+ * to operand 0 when sizes[0] is not the largest size (SB200_E_INVALID_ARG). */
+#define SB200_FOLD_ADD 0
+#define SB200_FOLD_SUB 1
+#define SB200_FOLD_SCALED 2
+int sb200_add_many(sb200_context *ctx, size_t L, size_t batch, size_t count, const size_t *sizes, const uint64_t *const *d_operands,
+                   const int *modes, const uint64_t *h_factors, uint64_t *d_out, void *stream);
 /* Evaluator::multiply_plain with ciphertext and plaintext both in NTT form (evaluator.cpp:1975-1994 -> multiply_plain_ntt
  * :2157-2195): every polynomial of the ciphertext times the plaintext, dyadic.  d_plain is [batch][L][n]: one NTT-form
  * plaintext per ciphertext, at the ciphertext's level (Plaintext::data() with parms_id == the ciphertext's).  May run in place. */
@@ -272,6 +288,8 @@ int sb200_square_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t
 int sb200_add_host(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *h_a, const uint64_t *h_b, uint64_t *h_out);
 int sb200_sub_host(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *h_a, const uint64_t *h_b, uint64_t *h_out);
 int sb200_negate_host(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *h_a, uint64_t *h_out);
+int sb200_add_many_host(sb200_context *ctx, size_t L, size_t batch, size_t count, const size_t *sizes, const uint64_t *const *h_operands,
+                        const int *modes, const uint64_t *h_factors, uint64_t *h_out);
 int sb200_multiply_plain_host(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *h_a, const uint64_t *h_plain,
                               uint64_t *h_out);
 int sb200_plain_to_ntt_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *h_plain, uint64_t *h_out);

@@ -18,6 +18,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstring>
+#include <deque>
 #include <map>
 #include <mutex>
 #include <stdexcept>
@@ -976,9 +977,100 @@ namespace seal_b200
                 throw std::invalid_argument("end of modulus switching chain reached");
             mod_switch_batch(encrypted, false);
         }
-        // add / sub / negate (evaluator.cpp:130-350) on batches of equal shape
+        // add / sub / negate (evaluator.cpp:130-350), any sizes and correction factors: the result takes the larger size, the longer
+        // operand's tail is copied (add) or negated (sub), and BGV operands with different correction factors are first scaled by
+        // the balancing factors -- all in one sb200_add_many pass
         void add_inplace(CiphertextBatch &encrypted1, const CiphertextBatch &encrypted2) const { linear_batch(encrypted1, encrypted2, false); }
         void sub_inplace(CiphertextBatch &encrypted1, const CiphertextBatch &encrypted2) const { linear_batch(encrypted1, encrypted2, true); }
+        // add_many (evaluator.cpp:236-262), member-wise: member i of destination is add_many of member i of every operand.  One
+        // sb200_add_many pass reads every operand once and writes destination once (the reference's chain of add_inplace calls
+        // moves 3 (m - 1) slabs); the chain's correction factors are replayed on the host to fill the steps.
+        void add_many(const std::vector<CiphertextBatch> &encrypteds, CiphertextBatch &destination) const
+        {
+            if (encrypteds.empty())
+                throw std::invalid_argument("encrypteds cannot be empty");
+            for (auto &e : encrypteds)
+                if (&e == &destination)
+                    throw std::invalid_argument("encrypteds must be different from destination");
+            std::vector<const CiphertextBatch *> ops;
+            for (auto &e : encrypteds)
+                ops.push_back(&e);
+            const Fold f = plan_fold(ops, std::vector<int>(ops.size() - 1, SB200_FOLD_ADD));
+            const CiphertextBatch &e0 = encrypteds[0];
+            std::lock_guard<std::mutex> lock(mu_);
+            shape(destination, e0.batch_, f.out_size, e0.L_, e0.n_);
+            copy_meta(e0, destination);
+            destination.cf_ = f.cf;
+            check(sb200_add_many(ctx_, e0.L_, e0.batch_, ops.size(), f.sizes.data(), f.ptrs.data(), f.modes.data(),
+                                 f.factors.empty() ? nullptr : f.factors.data(), destination.d_, nullptr));
+        }
+        // multiply_many (evaluator.cpp:1649-1724), member-wise, BFV and BGV.  The reference's queue of products is replayed on
+        // operand ids (schedule_products); products that do not depend on each other run as one wave: their operand pairs are staged
+        // into two slabs and multiplied and relinearized by one sb200_multiply_relinearize call, one pass over the relinearization
+        // key per key-switching chunk.  Each product is a function of its two operands alone, so the words are the reference's.
+        void multiply_many(const std::vector<CiphertextBatch> &encrypteds, const seal::RelinKeys &relin_keys, CiphertextBatch &destination) const
+        {
+            if (encrypteds.empty())
+                throw std::invalid_argument("encrypteds vector must not be empty");
+            for (auto &e : encrypteds)
+                if (&e == &destination)
+                    throw std::invalid_argument("encrypteds must be different from destination");
+            if (!context_.get_context_data(encrypteds[0].parms_id_))
+                throw std::invalid_argument("encrypteds is not valid for encryption parameters");
+            if (scheme_ != seal::scheme_type::bfv && scheme_ != seal::scheme_type::bgv)
+                throw std::logic_error("unsupported scheme");
+            std::vector<const CiphertextBatch *> leaves;
+            std::vector<std::pair<std::size_t, std::uint64_t>> runs;
+            for (auto &e : encrypteds)
+            {
+                runs.emplace_back(leaves.size(), 1);
+                leaves.push_back(&e);
+            }
+            run_products(leaves, schedule_products(leaves.size(), runs), relin_keys, destination);
+        }
+        // exponentiate (evaluator.cpp:1726-1757): multiply_many of `exponent` copies of encrypted, with the copies' queue kept in
+        // run-length form so that the schedule costs O(log exponent) and equal products are computed once (4 products for exponent
+        // 16, 5 for 13, against the reference's exponent - 1).  The reference allocates the copies and fails with std::bad_alloc
+        // for an exponent it cannot allocate; this member allocates no copies and does not reproduce that failure.
+        void exponentiate_inplace(CiphertextBatch &encrypted, std::uint64_t exponent, const seal::RelinKeys &relin_keys) const
+        {
+            if (!context_.get_context_data(encrypted.parms_id_))
+                throw std::invalid_argument("encrypted is not valid for encryption parameters");
+            if (!context_.get_context_data(relin_keys.parms_id()))
+                throw std::invalid_argument("relin_keys is not valid for encryption parameters");
+            if (exponent == 0)
+                throw std::invalid_argument("exponent cannot be 0");
+            if (exponent == 1)
+                return;
+            if (scheme_ != seal::scheme_type::bfv && scheme_ != seal::scheme_type::bgv)
+                throw std::logic_error("unsupported scheme");
+            CiphertextBatch result;
+            run_products({ &encrypted }, schedule_products(1, { { 0, exponent } }), relin_keys, result);
+            encrypted = std::move(result);
+        }
+        void exponentiate(const CiphertextBatch &encrypted, std::uint64_t exponent, const seal::RelinKeys &relin_keys,
+                          CiphertextBatch &destination) const
+        {
+            copy(encrypted, destination);
+            exponentiate_inplace(destination, exponent, relin_keys);
+        }
+        // mod_switch_to / rescale_to (evaluator.cpp:1451-1473, :1543-1590): the reference's checks, then single steps down to parms_id
+        void mod_switch_to_inplace(CiphertextBatch &encrypted, seal::parms_id_type parms_id) const
+        {
+            owned(encrypted);
+            check_target_level(encrypted.parms_id_, parms_id);
+            while (encrypted.parms_id_ != parms_id)
+                mod_switch_to_next_inplace(encrypted);
+        }
+        void rescale_to_inplace(CiphertextBatch &encrypted, seal::parms_id_type parms_id) const
+        {
+            owned(encrypted);
+            check_target_level(encrypted.parms_id_, parms_id);
+            if (scheme_ != seal::scheme_type::ckks)
+                throw std::invalid_argument("unsupported operation for scheme type");
+            while (encrypted.parms_id_ != parms_id)
+                rescale_to_next_inplace(encrypted);
+        }
         void negate_inplace(CiphertextBatch &encrypted) const
         {
             owned(encrypted);
@@ -1332,7 +1424,11 @@ namespace seal_b200
         }
         void check_target_level(const seal::Ciphertext &encrypted, const seal::parms_id_type &parms_id) const
         {
-            auto cur = context_.get_context_data(encrypted.parms_id());
+            check_target_level(encrypted.parms_id(), parms_id);
+        }
+        void check_target_level(const seal::parms_id_type &current, const seal::parms_id_type &parms_id) const
+        {
+            auto cur = context_.get_context_data(current);
             auto target = context_.get_context_data(parms_id);
             if (!cur)
                 throw std::invalid_argument("encrypted is not valid for encryption parameters");
@@ -1650,20 +1746,253 @@ namespace seal_b200
             if (bgv)
                 e.cf_ = seal::util::multiply_uint_mod(e.cf_, cd->rns_tool()->inv_q_last_mod_t(), next->parms().plain_modulus());
         }
+        // the arguments of one sb200_add_many call folding ops[0] op ops[1] op ... with modes[j - 1], after the checks of every step
+        // of the reference's chain (add_inplace / sub_inplace, evaluator.cpp:155-350) and with its correction factors replayed
+        struct Fold
+        {
+            std::vector<std::size_t> sizes;
+            std::vector<const std::uint64_t *> ptrs;
+            std::vector<int> modes;
+            std::vector<std::uint64_t> factors; // [count - 1][2], empty when no step is scaled
+            std::size_t out_size = 0;
+            std::uint64_t cf = 1; // the result's correction factor
+        };
+        Fold plan_fold(const std::vector<const CiphertextBatch *> &ops, std::vector<int> modes) const
+        {
+            const CiphertextBatch &a = *ops[0];
+            Fold f;
+            f.cf = a.cf_;
+            f.out_size = a.size_;
+            std::vector<std::uint64_t> factors(2 * (ops.size() - 1), 0);
+            bool scaled = false;
+            for (std::size_t j = 0; j < ops.size(); j++)
+            {
+                const CiphertextBatch &b = *ops[j];
+                owned(a), owned(b);
+                if (j)
+                {
+                    if (a.parms_id_ != b.parms_id_ || a.batch_ != b.batch_)
+                        throw std::invalid_argument("encrypted1 and encrypted2 parameter mismatch");
+                    if (a.ntt_ != b.ntt_)
+                        throw std::invalid_argument("NTT form mismatch");
+                    if (!seal::util::are_close<double>(a.scale_, b.scale_))
+                        throw std::invalid_argument("scale mismatch");
+                    if (f.cf != b.cf_)
+                    {
+                        // BGV: both sides scaled by the balancing factors (:188-209, :305-326)
+                        std::uint64_t g, e1, e2;
+                        balance_factors(f.cf, b.cf_, context_.get_context_data(a.parms_id_)->parms().plain_modulus(), g, e1, e2);
+                        modes[j - 1] |= SB200_FOLD_SCALED;
+                        factors[2 * (j - 1)] = e1, factors[2 * (j - 1) + 1] = e2;
+                        f.cf = g;
+                        scaled = true;
+                    }
+                    f.out_size = std::max(f.out_size, b.size_);
+                }
+                f.sizes.push_back(b.size_);
+                f.ptrs.push_back(b.d_);
+            }
+            f.modes = std::move(modes);
+            if (scaled)
+                f.factors = std::move(factors);
+            return f;
+        }
         void linear_batch(CiphertextBatch &a, const CiphertextBatch &b, bool subtract) const
         {
-            owned(a), owned(b);
-            if (a.parms_id_ != b.parms_id_ || a.batch_ != b.batch_)
-                throw std::invalid_argument("encrypted1 and encrypted2 parameter mismatch");
-            if (a.ntt_ != b.ntt_)
-                throw std::invalid_argument("NTT form mismatch");
-            if (!seal::util::are_close<double>(a.scale_, b.scale_))
-                throw std::invalid_argument("scale mismatch");
-            if (a.size_ != b.size_ || a.cf_ != b.cf_)
-                throw std::logic_error("seal_b200: batch add / sub needs operands of equal size and correction factor");
+            const Fold f = plan_fold({ &a, &b }, { subtract ? SB200_FOLD_SUB : SB200_FOLD_ADD });
             std::lock_guard<std::mutex> lock(mu_);
-            check(subtract ? sb200_sub(ctx_, a.L_, a.size_, a.batch_, a.d_, b.d_, a.d_, nullptr)
-                           : sb200_add(ctx_, a.L_, a.size_, a.batch_, a.d_, b.d_, a.d_, nullptr));
+            // in place when the result keeps a's size and b is another slab; otherwise into the result slab
+            const bool in_place = a.size_ == f.out_size && a.d_ != b.d_;
+            std::uint64_t *out = in_place ? a.d_ : out_slab(a.batch_ * f.out_size * a.L_ * a.n_, a);
+            check(sb200_add_many(ctx_, a.L_, a.batch_, 2, f.sizes.data(), f.ptrs.data(), f.modes.data(),
+                                 f.factors.empty() ? nullptr : f.factors.data(), out, nullptr));
+            if (!in_place)
+                adopt(a);
+            a.size_ = f.out_size;
+            a.cf_ = f.cf;
+        }
+        // ---- the product schedule of multiply_many / exponentiate ----
+        // The reference's queue (evaluator.cpp:1649-1724): products of operand pairs (0,1), (2,3), ... with an odd operand appended
+        // at the end, then pairs taken from the front with each product appended at the back, until one is left.  It is replayed on
+        // ids: leaves are 0 .. leaves-1, product p is id leaves + p.  The queue holds runs (id, count) of equal ids, so e copies of
+        // one operand cost O(log e) steps; a product is hash-consed on (left id, right id) and made once, and products are grouped
+        // into waves by their depth (a wave's products depend only on earlier waves).
+        struct ProductSchedule
+        {
+            std::size_t leaves = 0, root = 0;
+            std::vector<std::pair<std::size_t, std::size_t>> products; // (left id, right id)
+            std::vector<std::vector<std::size_t>> waves;               // product indices
+        };
+        static ProductSchedule schedule_products(std::size_t leaves, const std::vector<std::pair<std::size_t, std::uint64_t>> &operand_runs)
+        {
+            ProductSchedule s;
+            s.leaves = leaves;
+            std::map<std::pair<std::size_t, std::size_t>, std::size_t> made;
+            std::vector<std::size_t> depth(leaves, 0);
+            auto product = [&](std::size_t l, std::size_t r) {
+                auto it = made.find({ l, r });
+                if (it != made.end())
+                    return it->second;
+                const std::size_t id = leaves + s.products.size(), d = std::max(depth[l], depth[r]) + 1;
+                s.products.emplace_back(l, r);
+                depth.push_back(d);
+                if (s.waves.size() < d)
+                    s.waves.resize(d);
+                s.waves[d - 1].push_back(id - leaves);
+                return made[{ l, r }] = id;
+            };
+            std::deque<std::pair<std::size_t, std::uint64_t>> q;
+            auto push = [&q](std::size_t id, std::uint64_t count) {
+                if (!q.empty() && q.back().first == id)
+                    q.back().second += count;
+                else
+                    q.emplace_back(id, count);
+            };
+            // first level: consecutive operand pairs, the odd operand last
+            bool pending = false;
+            std::size_t odd = 0;
+            for (auto [id, count] : operand_runs)
+            {
+                if (pending && count)
+                    push(product(odd, id), 1), count--, pending = false;
+                if (count / 2)
+                    push(product(id, id), count / 2);
+                if (count & 1)
+                    pending = true, odd = id;
+            }
+            if (pending)
+                push(odd, 1);
+            // then pairs from the front of the queue, products to the back
+            while (q.size() > 1 || q.front().second > 1)
+            {
+                auto [id, count] = q.front();
+                q.pop_front();
+                if (count / 2)
+                    push(product(id, id), count / 2);
+                if (count & 1)
+                {
+                    const std::size_t other = q.front().first;
+                    if (--q.front().second == 0)
+                        q.pop_front();
+                    push(product(id, other), 1);
+                }
+            }
+            s.root = q.front().first;
+            return s;
+        }
+        // runs a schedule over the leaf batches; the result goes to destination with the reference's metadata
+        void run_products(const std::vector<const CiphertextBatch *> &leaves, const ProductSchedule &s, const seal::RelinKeys &relin_keys,
+                          CiphertextBatch &destination) const
+        {
+            const CiphertextBatch &f = *leaves[0];
+            const bool bgv = scheme_ == seal::scheme_type::bgv;
+            // every check of every product's multiply_inplace and relinearize_inplace runs before the first write
+            for (auto *l : leaves)
+            {
+                owned(*l);
+                if (l->parms_id_ != f.parms_id_ || l->batch_ != f.batch_)
+                    throw std::invalid_argument("encrypted1 and encrypted2 parameter mismatch");
+                if (bgv != l->ntt_)
+                    throw std::invalid_argument(bgv ? "encrypted1 or encrypted2 must be in NTT form" : "encrypted1 or encrypted2 cannot be in NTT form");
+            }
+            if (!s.products.empty())
+            {
+                if (relin_keys.parms_id() != context_.key_parms_id())
+                    throw std::invalid_argument("relin_keys is not valid for encryption parameters");
+                if (!context_.using_keyswitching())
+                    throw std::logic_error("keyswitching is not supported by the context");
+                for (auto &pr : s.products)
+                {
+                    const std::size_t s1 = pr.first < s.leaves ? leaves[pr.first]->size_ : 2, s2 = pr.second < s.leaves ? leaves[pr.second]->size_ : 2;
+                    if (s1 + s2 - 1 > SEAL_CIPHERTEXT_SIZE_MAX)
+                        throw std::invalid_argument("invalid size");
+                    if (s1 + s2 - 1 < 2)
+                        throw std::invalid_argument("destination_size must be at least 2 and less than or equal to current count");
+                    if (relin_keys.size() < s1 + s2 - 3)
+                        throw std::invalid_argument("not enough relinearization keys");
+                }
+            }
+            if (s.products.empty())
+            {
+                copy(*leaves[s.root], destination);
+                return;
+            }
+            const auto cd = context_.get_context_data(f.parms_id_);
+            const seal::Modulus &t = cd->parms().plain_modulus();
+            const std::size_t B = f.batch_, L = f.L_, ct = 2 * L * f.n_, bytes = B * ct * sizeof(std::uint64_t);
+            const std::size_t P = s.products.size();
+            std::vector<const std::uint64_t *> data(P);     // device words of each product, [B][2][L][n]
+            std::vector<std::uint64_t> cf(P);
+            std::vector<CiphertextBatch> slabs;              // owners of the wave outputs
+            auto id_data = [&](std::size_t id) { return id < s.leaves ? leaves[id]->d_ : data[id - s.leaves]; };
+            auto id_cf = [&](std::size_t id) { return id < s.leaves ? leaves[id]->cf_ : cf[id - s.leaves]; };
+            auto id_size = [&](std::size_t id) { return id < s.leaves ? leaves[id]->size_ : std::size_t(2); };
+            for (const auto &wave : s.waves)
+            {
+                std::vector<std::size_t> fused, single; // size-2 pairs run together; other sizes one by one
+                for (std::size_t p : wave)
+                    (id_size(s.products[p].first) == 2 && id_size(s.products[p].second) == 2 ? fused : single).push_back(p);
+                for (std::size_t p : single)
+                {
+                    CiphertextBatch x, y;
+                    const CiphertextBatch *l = s.products[p].first < s.leaves ? leaves[s.products[p].first] : nullptr;
+                    const CiphertextBatch *r = s.products[p].second < s.leaves ? leaves[s.products[p].second] : nullptr;
+                    wrap(x, l, id_data(s.products[p].first), f);
+                    wrap(y, r, id_data(s.products[p].second), f);
+                    multiply_inplace(x, y);
+                    relinearize_inplace(x, relin_keys);
+                    x.cf_ = bgv ? seal::util::multiply_uint_mod(id_cf(s.products[p].first), id_cf(s.products[p].second), t) : 1;
+                    data[p] = x.d_;
+                    cf[p] = x.cf_;
+                    slabs.push_back(std::move(x));
+                }
+                std::lock_guard<std::mutex> lock(mu_);
+                const std::size_t chunk = sb200_keyswitch_chunk(ctx_, L, fused.size() * B, 1);
+                const std::size_t group = std::max<std::size_t>(1, chunk / B);
+                for (std::size_t g0 = 0; g0 < fused.size(); g0 += group)
+                {
+                    const std::size_t G = std::min(group, fused.size() - g0);
+                    CiphertextBatch a, b;
+                    shape(a, G * B, 2, L, f.n_);
+                    shape(b, G * B, 2, L, f.n_);
+                    for (std::size_t i = 0; i < G; i++)
+                    {
+                        const auto &pr = s.products[fused[g0 + i]];
+                        check(sb200_memcpy_d2d(ctx_, a.d_ + i * B * ct, id_data(pr.first), bytes, nullptr));
+                        check(sb200_memcpy_d2d(ctx_, b.d_ + i * B * ct, id_data(pr.second), bytes, nullptr));
+                    }
+                    sb200_kswitch_key *key = key_for(relin_keys, seal::RelinKeys::get_index(2), L);
+                    check(sb200_multiply_relinearize(ctx_, L, G * B, a.d_, b.d_, key, a.d_, nullptr));
+                    for (std::size_t i = 0; i < G; i++)
+                    {
+                        const std::size_t p = fused[g0 + i];
+                        data[p] = a.d_ + i * B * ct;
+                        cf[p] = bgv ? seal::util::multiply_uint_mod(id_cf(s.products[p].first), id_cf(s.products[p].second), t) : 1;
+                    }
+                    slabs.push_back(std::move(a));
+                }
+            }
+            const std::size_t r = s.root - s.leaves;
+            {
+                std::lock_guard<std::mutex> lock(mu_);
+                shape(destination, B, 2, L, f.n_);
+                copy_meta(f, destination);
+                destination.cf_ = bgv ? cf[r] : f.cf_;
+                check(sb200_memcpy_d2d(ctx_, destination.d_, data[r], bytes, nullptr));
+            }
+        }
+        // a batch object over a leaf (a copy) or over product words (size 2), with the leaves' metadata, for the one-by-one products
+        void wrap(CiphertextBatch &x, const CiphertextBatch *leaf, const std::uint64_t *words, const CiphertextBatch &meta) const
+        {
+            if (leaf)
+            {
+                copy(*leaf, x);
+                return;
+            }
+            std::lock_guard<std::mutex> lock(mu_);
+            shape(x, meta.batch_, 2, meta.L_, meta.n_);
+            copy_meta(meta, x);
+            check(sb200_memcpy_d2d(ctx_, x.d_, words, meta.batch_ * 2 * meta.L_ * meta.n_ * sizeof(std::uint64_t), nullptr));
         }
         void rotate_batch(CiphertextBatch &encrypted, int steps, const seal::GaloisKeys &galois_keys) const
         {

@@ -14,6 +14,8 @@ import os
 import numpy as np
 
 BFV, CKKS, BGV = 1, 2, 3
+# step modes of add_many (SB200_FOLD_*): add or sub, optionally ORed with FOLD_SCALED
+FOLD_ADD, FOLD_SUB, FOLD_SCALED = 0, 1, 2
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libseal_b200.so")
 _u64p = C.POINTER(C.c_uint64)
@@ -32,7 +34,7 @@ SYMBOLS = [
     "sb200_multiply_host", "sb200_multiply_sized_host", "sb200_square_host", "sb200_add_host", "sb200_sub_host", "sb200_negate_host", "sb200_multiply_plain_host", "sb200_batch_encode_host", "sb200_batch_decode_host", "sb200_plain_to_ntt_host", "sb200_multiply_plain_coeff_host", "sb200_add_plain_coeff_host",
     "sb200_multiply_plain_n", "sb200_multiply_plain_coeff_n", "sb200_add_plain_coeff_n", "sb200_add_plain_ntt", "sb200_multiply_plain_n_host",
     "sb200_multiply_plain_coeff_n_host", "sb200_add_plain_coeff_n_host", "sb200_add_plain_ntt_host",
-    "sb200_relinearize_host", "sb200_multiply_relinearize_host", "sb200_rescale_to_next_host",
+    "sb200_add_many", "sb200_add_many_host", "sb200_relinearize_host", "sb200_multiply_relinearize_host", "sb200_rescale_to_next_host",
     "sb200_mod_switch_to_next_host", "sb200_apply_galois_host", "sb200_get_parms_id", "sb200_ciphertext_inspect",
     "sb200_ciphertext_save_size", "sb200_ciphertext_load", "sb200_ciphertext_save", "sb200_secret_key_create",
     "sb200_secret_key_destroy", "sb200_decrypt", "sb200_decrypt_host", "sb200_invariant_noise_budget", "sb200_invariant_noise_budget_host", "sb200_encrypt_zero_symmetric", "sb200_public_key_create", "sb200_public_key_destroy", "sb200_encrypt_zero_asymmetric", "sb200_encrypt_zero_symmetric_prng", "sb200_encrypt_zero_asymmetric_prng", "sb200_encrypt_symmetric", "sb200_encrypt_asymmetric", "sb200_kswitch_key_generate", "sb200_public_key_generate", "sb200_ciphertext_save_seeded_size", "sb200_ciphertext_save_seeded",
@@ -127,6 +129,8 @@ def lib():
         L.sb200_add_plain_ntt_host.argtypes = [vp, sz, sz, sz, sz, i32, _u64p, _u64p, _u64p]
         L.sb200_square_host.argtypes = [vp, sz, sz, _u64p, _u64p]
         L.sb200_add_host.argtypes = [vp, sz, sz, sz, _u64p, _u64p, _u64p]
+        L.sb200_add_many.argtypes = [vp, sz, sz, sz, C.POINTER(sz), C.POINTER(vp), C.POINTER(i32), _u64p, vp, vp]
+        L.sb200_add_many_host.argtypes = [vp, sz, sz, sz, C.POINTER(sz), C.POINTER(vp), C.POINTER(i32), _u64p, _u64p]
         L.sb200_sub_host.argtypes = [vp, sz, sz, sz, _u64p, _u64p, _u64p]
         L.sb200_negate_host.argtypes = [vp, sz, sz, sz, _u64p, _u64p]
         L.sb200_relinearize.argtypes = [vp, sz, sz, vp, vp, vp, vp]
@@ -500,6 +504,29 @@ class Context:
     def negate(self, a):
         return self._linear(lib().sb200_negate_host, a)
 
+    @staticmethod
+    def _fold_args(sizes, modes, factors):
+        """ctypes arrays of sb200_add_many: sizes [count], modes [count - 1] or None, factors [count - 1][2] or None"""
+        count = len(sizes)
+        c_sizes = (C.c_size_t * max(count, 1))(*sizes)
+        c_modes = None if modes is None else (C.c_int * max(count - 1, 1))(*[int(m) for m in modes])
+        f = None if factors is None else np.ascontiguousarray(factors, dtype=np.uint64).reshape(-1)
+        return c_sizes, c_modes, f
+
+    def add_many(self, operands, modes=None, factors=None):
+        """Evaluator.add_many generalised (sb200_add_many): operands [B][size_j][L][n] (sizes may differ) folded left in one pass;
+        modes[j - 1] is step j's FOLD_* mode (None: every step adds), factors[j - 1] = (e1_j, e2_j) the scalars of a scaled step.
+        Returns [B][max size_j][L][n]."""
+        ops = [self._batched(a)[0] for a in operands]
+        single = len(operands) > 0 and np.asarray(operands[0]).ndim == 3
+        B, _, L, n = ops[0].shape if ops else (0, 0, 0, 0)
+        sizes = [a.shape[1] for a in ops]
+        c_sizes, c_modes, f = self._fold_args(sizes, modes, factors)
+        out = np.zeros((B, max(sizes) if sizes else 0, L, n), dtype=np.uint64)
+        ptrs = (C.c_void_p * max(len(ops), 1))(*[a.ctypes.data for a in ops])
+        _check(lib().sb200_add_many_host(self.h, L, B, len(ops), c_sizes, ptrs, c_modes, None if f is None else _hp(f), _hp(out)))
+        return out[0] if single else out
+
     def multiply_plain(self, a, plain):
         """Evaluator.multiply_plain, NTT-form ciphertext [B][size][L][n] x NTT-form plaintexts [B][L][n]"""
         a, single = self._batched(a)
@@ -737,6 +764,14 @@ class Context:
 
     def d_add_plain_ntt(self, a, plain, out, L, size, batch, plain_count, subtract=False):
         _check(lib().sb200_add_plain_ntt(self.h, L, size, batch, plain_count, int(subtract), _dp(a), _dp(plain), _dp(out), self._stream()))
+
+    def d_add_many(self, operands, out, L, batch, sizes, modes=None, factors=None):
+        """sb200_add_many on device tensors: operands [batch][sizes[j]][L][n] (tensors or raw device pointers), out
+        [batch][max sizes][L][n]; modes / factors as in add_many"""
+        c_sizes, c_modes, f = self._fold_args(sizes, modes, factors)
+        ptrs = (C.c_void_p * max(len(operands), 1))(*[_dp(t).value for t in operands])
+        _check(lib().sb200_add_many(self.h, L, batch, len(operands), c_sizes, ptrs, c_modes, None if f is None else _hp(f), _dp(out),
+                                    self._stream()))
 
     def d_multiply_sized(self, a, b, out, L, size_a, size_b, batch):
         _check(lib().sb200_multiply_sized(self.h, L, size_a, size_b, batch, _dp(a), _dp(b), _dp(out), self._stream()))

@@ -955,6 +955,127 @@ namespace
         }
     };
 
+    // count operands of sizes[j] polynomials folded into one of the largest size (op_add_many); it does not fit Layout's two inputs,
+    // so it has its own two drivers below, add_many_on_stream and add_many_on_host
+    struct AddMany
+    {
+        size_t L, count;
+        const size_t *sizes;
+        const int *modes;
+        const u64 *factors;
+        size_t out_size = 0;
+        void check(const Context &c, size_t batch)
+        {
+            check_level(c, L, batch);
+            if (count == 0)
+                throw std::invalid_argument("encrypteds cannot be empty");
+            out_size = 0;
+            for (size_t j = 0; j < count; j++)
+            {
+                check_size(sizes[j]);
+                out_size = std::max(out_size, sizes[j]);
+            }
+            for (size_t j = 1; j < count && modes; j++)
+                if (modes[j - 1] < 0 || modes[j - 1] > 3)
+                    throw std::invalid_argument("invalid add_many mode");
+        }
+        // operand 0 may be the output (in place) when it has the output's size; no other operand may
+        void check_alias(const u64 *const *ops, const u64 *out) const
+        {
+            for (size_t j = 1; j < count; j++)
+                if (ops[j] == out)
+                    throw std::invalid_argument("add_many: the output slab must not alias an operand other than operand 0");
+            if (ops[0] == out && sizes[0] != out_size)
+                throw std::invalid_argument("add_many: the output slab may alias operand 0 only when operand 0 has the output's size");
+        }
+        bool scaled() const
+        {
+            for (size_t j = 1; j < count && modes; j++)
+                if (modes[j - 1] & SB200_FOLD_SCALED)
+                    return true;
+            return false;
+        }
+        void operator()(Context &c, size_t B, const u64 *const *ops, u64 *out, cudaStream_t st) const
+        {
+            std::vector<int> m(count ? count - 1 : 0, SB200_FOLD_ADD);
+            if (modes)
+                std::copy(modes, modes + m.size(), m.begin());
+            op_add_many(c, L, B, count, sizes, ops, m.data(), factors, out, st);
+        }
+    };
+
+    int add_many_on_stream(sb200_context *ctx, void *stream, size_t batch, const uint64_t *const *ops, uint64_t *out, AddMany op)
+    {
+        SB_NEED(op.sizes);
+        SB_NEED(ops);
+        SB_NEED(out);
+        for (size_t j = 0; j < op.count; j++)
+            SB_NEED(ops[j]);
+        SB_TRY
+        SB_ENTER_STREAM(ctx, stream)
+        op.check(c, batch);
+        if (op.scaled() && !op.factors)
+        {
+            g_last_error = "null pointer: h_factors";
+            return SB200_E_POINTER;
+        }
+        op.check_alias(reinterpret_cast<const u64 *const *>(ops), reinterpret_cast<const u64 *>(out));
+        op(c, batch, reinterpret_cast<const u64 *const *>(ops), reinterpret_cast<u64 *>(out), static_cast<cudaStream_t>(stream));
+        return SB200_OK;
+        SB_CATCH
+    }
+
+    // host buffers: the batch in chunks of the context's staging size; every operand's chunk is uploaded behind the previous one
+    int add_many_on_host(sb200_context *ctx, size_t batch, const uint64_t *const *ops, uint64_t *out, AddMany op)
+    {
+        SB_NEED(op.sizes);
+        SB_NEED(ops);
+        SB_NEED(out);
+        for (size_t j = 0; j < op.count; j++)
+            SB_NEED(ops[j]);
+        SB_TRY
+        SB_ENTER(ctx)
+        op.check(c, batch);
+        if (op.scaled() && !op.factors)
+        {
+            g_last_error = "null pointer: h_factors";
+            return SB200_E_POINTER;
+        }
+        op.check_alias(reinterpret_cast<const u64 *const *>(ops), reinterpret_cast<const u64 *>(out));
+        const size_t poly = op.L * c.n;
+        size_t in_words = 0; // per ciphertext, all operands
+        for (size_t j = 0; j < op.count; j++)
+            in_words += op.sizes[j] * poly;
+        const size_t per_ct = (in_words + op.out_size * poly) * sizeof(u64);
+        const size_t chunk = std::max<size_t>(1, std::min(batch, c.host_stage_bytes / per_ct));
+        if (!c.io.s_comp)
+            c.io.s_comp = make_stream();
+        cudaStream_t st = c.io.s_comp.get();
+        StreamOrder order(c, st);
+        DevBuf<u64> &din = c.io.buf[0][0], &dout = c.io.buf[0][2];
+        din.grow(chunk * in_words);
+        dout.grow(chunk * op.out_size * poly);
+        std::vector<const u64 *> dops(op.count);
+        for (size_t b0 = 0; b0 < batch; b0 += chunk)
+        {
+            const size_t B = std::min(chunk, batch - b0);
+            u64 *d = din.get();
+            for (size_t j = 0; j < op.count; j++)
+            {
+                const size_t w = op.sizes[j] * poly;
+                cuda_check(cudaMemcpyAsync(d, ops[j] + b0 * w, B * w * sizeof(u64), cudaMemcpyHostToDevice, st), "H2D");
+                dops[j] = d;
+                d += B * w;
+            }
+            op(c, B, dops.data(), dout.get(), st);
+            cuda_check(cudaMemcpyAsync(out + b0 * op.out_size * poly, dout.get(), B * op.out_size * poly * sizeof(u64), cudaMemcpyDeviceToHost, st),
+                       "D2H");
+            cuda_check(cudaStreamSynchronize(st), "synchronize");
+        }
+        return SB200_OK;
+        SB_CATCH
+    }
+
     // plain_count: one plaintext per ciphertext (batch) or one for the whole batch (1, a shared operand: Layout::shared_b).  The
     // older entry points, which take one plaintext per ciphertext, stay on the per-ciphertext path at every batch size (shared =
     // false, plain_count = batch); the _n entry points share the plaintext when plain_count = 1.
@@ -1327,6 +1448,17 @@ int sb200_negate(sb200_context *ctx, size_t L, size_t size, size_t batch, const 
 int sb200_negate_host(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, uint64_t *out)
 {
     return on_host(ctx, batch, a, nullptr, out, Linear{ 2, L, size });
+}
+
+int sb200_add_many(sb200_context *ctx, size_t L, size_t batch, size_t count, const size_t *sizes, const uint64_t *const *ops, const int *modes,
+                   const uint64_t *factors, uint64_t *out, void *stream)
+{
+    return add_many_on_stream(ctx, stream, batch, ops, out, AddMany{ L, count, sizes, modes, reinterpret_cast<const u64 *>(factors) });
+}
+int sb200_add_many_host(sb200_context *ctx, size_t L, size_t batch, size_t count, const size_t *sizes, const uint64_t *const *ops, const int *modes,
+                        const uint64_t *factors, uint64_t *out)
+{
+    return add_many_on_host(ctx, batch, ops, out, AddMany{ L, count, sizes, modes, reinterpret_cast<const u64 *>(factors) });
 }
 
 int sb200_multiply_plain(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, const uint64_t *plain, uint64_t *out,

@@ -519,6 +519,133 @@ namespace sb
         }
     }
 
+    // ---- add_many: a left fold of add_inplace / sub_inplace steps in one pass (evaluator.cpp:155-262, :263-350) ------------
+    // Operand j is [B][stride_j][L][n] with size_j polynomials present.  Every output word gets the word operations the reference's
+    // chain of add_inplace / sub_inplace performs on it, in the chain's order, in registers: acc = x_0, then per step j >= 1
+    //   scaled (BGV balancing, multiply_poly_scalar_coeffmod over the present polynomials): acc = acc * e1_j, y = x_j * e2_j (Shoup);
+    //   add: acc = csub(acc + y, q);  sub: acc = csub(acc + q - y, q);
+    //   polynomial absent from every earlier operand: acc = y (add, set_poly_array) or -y (sub, negate_poly_coeffmod).
+    // Absence is tracked, never stood in for by zero: csub(0 + y, q) != y for a word y >= q.
+    struct FoldLaunch
+    {
+        const ulonglong2 *x[kFoldMaxOperands];
+        int size[kFoldMaxOperands];   // polynomials present in operand j
+        int stride[kFoldMaxOperands]; // polynomials per ciphertext in operand j's slab
+        int mode[kFoldMaxOperands];   // step j (j >= 1): bit 0 sub, bit 1 scaled; the scalars of step j at tab[(j - 1) L + i]
+        int count, polys, out_stride; // operands; polynomials written; polynomials per ciphertext of the output slab
+    };
+
+    __global__ void __launch_bounds__(256) fold_kernel(const __grid_constant__ FoldLaunch f, const Tw *__restrict__ tab, ulonglong2 *out,
+                                                       const PrimeDev *__restrict__ primes, int logn, int L, long long total2)
+    {
+        const long long e = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; // over the batch's pairs of one polynomial
+        if (e >= total2)
+            return;
+        const long long half = static_cast<long long>(L) << (logn - 1);
+        const long long b = e / half, r = e - b * half;
+        const int i = static_cast<int>((r * 2) >> logn);
+        const u64 q = primes[i].q;
+        for (int p = 0; p < f.polys; p++)
+        {
+            ulonglong2 acc = make_ulonglong2(0, 0);
+            bool have = false;
+            for (int j = 0; j < f.count; j++)
+            {
+                const int m = j ? f.mode[j] : 0;
+                if (m & 2)
+                {
+                    const Tw e1 = tab[(2 * (j - 1)) * L + i], e2 = tab[(2 * (j - 1) + 1) * L + i];
+                    if (have)
+                        acc = make_ulonglong2(mul_shoup(acc.x, e1, q), mul_shoup(acc.y, e1, q));
+                    if (p < f.size[j])
+                    {
+                        const ulonglong2 v = f.x[j][(b * f.stride[j] + p) * half + r];
+                        const ulonglong2 y = make_ulonglong2(mul_shoup(v.x, e2, q), mul_shoup(v.y, e2, q));
+                        acc = !have ? ((m & 1) ? make_ulonglong2(y.x ? q - y.x : 0, y.y ? q - y.y : 0) : y)
+                              : (m & 1) ? make_ulonglong2(csub(acc.x + q - y.x, q), csub(acc.y + q - y.y, q))
+                                        : make_ulonglong2(csub(acc.x + y.x, q), csub(acc.y + y.y, q));
+                        have = true;
+                    }
+                }
+                else if (p < f.size[j])
+                {
+                    const ulonglong2 y = f.x[j][(b * f.stride[j] + p) * half + r];
+                    acc = !have ? ((m & 1) ? make_ulonglong2(y.x ? q - y.x : 0, y.y ? q - y.y : 0) : y)
+                          : (m & 1) ? make_ulonglong2(csub(acc.x + q - y.x, q), csub(acc.y + q - y.y, q))
+                                    : make_ulonglong2(csub(acc.x + y.x, q), csub(acc.y + y.y, q));
+                    have = true;
+                }
+            }
+            out[(b * f.out_stride + p) * half + r] = acc;
+        }
+    }
+
+    void op_add_many(Context &c, size_t L, size_t batch, size_t count, const size_t *sizes, const u64 *const *ops, const int *modes,
+                     const u64 *factors, u64 *out, cudaStream_t st)
+    {
+        size_t out_size = 0;
+        bool scaled = false;
+        for (size_t j = 0; j < count; j++)
+        {
+            out_size = std::max(out_size, sizes[j]);
+            scaled |= j && (modes[j - 1] & 2);
+        }
+        // (e1_j, e2_j) mod q_i with their Shoup quotients: tab[(2 (j - 1) + {0, 1}) L + i]
+        const Tw *d_tab = nullptr;
+        if (scaled)
+        {
+            std::vector<Tw> tab(2 * (count - 1) * L);
+            for (size_t j = 1; j < count; j++)
+                if (modes[j - 1] & 2)
+                    for (int h = 0; h < 2; h++)
+                        for (size_t i = 0; i < L; i++)
+                        {
+                            const u64 v = factors[2 * (j - 1) + h] % c.q[i];
+                            tab[(2 * (j - 1) + h) * L + i] = Tw{ v, sbh::shoup(v, c.q[i]) };
+                        }
+            auto *d = static_cast<Tw *>(c.ensure_scratch(tab.size() * sizeof(Tw)));
+            cuda_check(cudaMemcpyAsync(d, tab.data(), tab.size() * sizeof(Tw), cudaMemcpyHostToDevice, st), "upload scalars");
+            d_tab = d;
+        }
+        const long long half = static_cast<long long>(L * c.n / 2), total2 = static_cast<long long>(batch) * half;
+        const unsigned blocks = static_cast<unsigned>((total2 + 255) / 256);
+        // operand 0 of every launch after the first is the partial result in out (its present polynomials so far); the words do not
+        // depend on where the fold is cut, since the accumulator of a word is that word
+        size_t j0 = 0, acc_size = 0;
+        while (j0 < count)
+        {
+            FoldLaunch f{};
+            int k = 0;
+            double words = 0;
+            if (j0)
+            {
+                f.x[0] = reinterpret_cast<const ulonglong2 *>(out), f.size[0] = static_cast<int>(acc_size), f.stride[0] = static_cast<int>(out_size);
+                words += static_cast<double>(acc_size);
+                k = 1;
+            }
+            size_t polys = acc_size;
+            const size_t first = j0;
+            for (; k < kFoldMaxOperands && j0 < count; k++, j0++)
+            {
+                f.x[k] = reinterpret_cast<const ulonglong2 *>(ops[j0]);
+                f.size[k] = f.stride[k] = static_cast<int>(sizes[j0]);
+                // the scalars stay indexed by the step's place in the whole fold: shift the table so that launch slot k finds them
+                f.mode[k] = j0 ? modes[j0 - 1] : 0;
+                polys = std::max(polys, sizes[j0]);
+                words += static_cast<double>(sizes[j0]);
+            }
+            f.count = k, f.polys = static_cast<int>(polys), f.out_stride = static_cast<int>(out_size);
+            // slot k of this launch holds step (first - (first ? 1 : 0)) + k of the fold; its scalars start at that step's entry
+            const size_t step0 = first ? first - 1 : 0;
+            const Tw *t = d_tab ? d_tab + 2 * step0 * L : nullptr;
+            c.stats.begin("add_many", 0, 8.0 * (words + static_cast<double>(polys)) * static_cast<double>(L * c.n) * static_cast<double>(batch), st);
+            fold_kernel<<<blocks, 256, 0, st>>>(f, t, reinterpret_cast<ulonglong2 *>(out), c.d_primes.get(), c.logn, static_cast<int>(L), total2);
+            c.stats.end(st);
+            cuda_check(cudaGetLastError(), "fold_kernel");
+            acc_size = polys;
+        }
+    }
+
     // ---- multiply_plain, NTT x NTT (evaluator.cpp:2157-2195: dyadic_product_coeffmod of every polynomial with the plaintext) ----
     // ct [B][size][L][n], plain [B][L][n] (one NTT-form plaintext per ciphertext, at the ciphertext's level)
     __global__ void __launch_bounds__(256) plain_mul_kernel(const ulonglong2 *__restrict__ a, const ulonglong2 *__restrict__ plain,

@@ -169,6 +169,12 @@ namespace sb
     // drivers (all stream-ordered, no synchronisation); slabs as documented in include/seal_b200.h
     void op_ntt(Context &c, bool inverse, size_t L, size_t size, size_t batch, u64 *d, cudaStream_t st);
     void op_linear(Context &c, int mode, size_t L, size_t size, size_t batch, const u64 *a, const u64 *b, u64 *out, cudaStream_t st);
+    // add_many (sb200_add_many): count operands [B][sizes[j]][L][n] folded left into out [B][max size][L][n]; modes[j - 1] is step j's
+    // mode (bit 0 sub, bit 1 scaled by the pair factors[2 (j - 1)], factors[2 (j - 1) + 1]).  One launch takes kFoldMaxOperands operands;
+    // longer folds continue from the partial result in out.  ops[0] may be out when sizes[0] is the largest size.
+    constexpr int kFoldMaxOperands = 16;
+    void op_add_many(Context &c, size_t L, size_t batch, size_t count, const size_t *sizes, const u64 *const *ops, const int *modes,
+                     const u64 *factors, u64 *out, cudaStream_t st);
     // Plaintext operations take one plaintext per ciphertext, or (shared) one plaintext for the whole batch.
     // NTT-form plaintexts [B][L][n] or [L][n]: multiply_plain of NTT-form ciphertexts; CKKS add_plain / sub_plain (c_0 only)
     void op_multiply_plain(Context &c, size_t L, size_t size, size_t batch, bool shared, const u64 *a, const u64 *plain, u64 *out,
