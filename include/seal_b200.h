@@ -169,6 +169,17 @@ int sb200_kswitch_key_destroy(sb200_kswitch_key *key);
  * index = RelinKeys::get_index(2) = 0 for relinearization, GaloisKeys::get_index(galois_elt) = (galois_elt - 1) / 2 for a
  * rotation (relinkeys.h:58-65, galoiskeys.h:48-51).  SB200_E_OUT_OF_RANGE: no such slot; SB200_E_INVALID_ARG: empty slot. */
 int sb200_kswitch_key_load(sb200_context *ctx, const uint8_t *stream, size_t len, size_t index, sb200_kswitch_key **out);
+/* KSwitchKeys::load of several entries in one pass: the object is inflated at most once and its frame parsed once, and every
+ * seeded digit expands on the device.  out[i] = the handle sb200_kswitch_key_load(..., indices[i]) makes, i < count.  indices ==
+ * NULL: every non-empty slot in slot order, count = the capacity of out and out_indices.  out_indices (may be NULL) receives each
+ * handle's slot, *out_count the number of handles.  Errors, all checked before the first handle is made: SB200_E_OUT_OF_RANGE an
+ * index at or past the slot count; SB200_E_INVALID_ARG an empty slot, a duplicated index, or too small a capacity for the NULL
+ * form; SB200_E_LOGIC keys of another context.  A failure after that (a word >= its modulus: SB200_E_LOGIC) destroys the
+ * handles made so far; out is written only on success.  sb200_kswitch_key_load is the count = 1 case. */
+int sb200_kswitch_keys_load(sb200_context *ctx, const uint8_t *stream, size_t len, const size_t *indices, size_t count,
+                            sb200_kswitch_key **out, size_t *out_indices, size_t *out_count);
+/* bytes the handle holds on the device: the key words plus the integer path's copy (0 for NULL) */
+size_t sb200_kswitch_key_device_bytes(const sb200_kswitch_key *key);
 
 /* ---- device-resident batch operations (stream = cudaStream_t, may be NULL) ----------------------------------
  * Output slabs must not alias input slabs unless noted: multiply_relinearize may write over d_a or d_b, add/sub/negate/multiply_plain

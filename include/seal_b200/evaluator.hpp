@@ -163,6 +163,84 @@ namespace seal_b200
         double scale_ = 1.0;
     };
 
+    // ---- device-resident key sets ------------------------------------------------------------------------------------
+    // RelinKeys / GaloisKeys whose key-switching keys live on the GPU, one key handle (sb200_kswitch_key) per non-empty slot of
+    // KSwitchKeys::data(), owned by this object.  Filled by Evaluator::load (straight from a stream: none, zlib or seeded) or
+    // Evaluator::upload (from a seal:: object), or by KeyGenerator on the device; the batch members of Evaluator take them wherever
+    // they take seal::RelinKeys / seal::GaloisKeys.  Same ownership rules as CiphertextBatch: allocated from the Evaluator's context,
+    // movable, not copyable, and they must not outlive that context.  They are never entered in the Evaluator's key cache and never
+    // evicted.  device_bytes() is what the set holds on the device: at n >= 4096 a key holds its 64-bit words and the integer
+    // key-switching path's copy, 3.5x the words (n = 65536, k = 32: 1.04 GB + 2.6 GB per key).
+    class DeviceKSwitchKeys
+    {
+    public:
+        DeviceKSwitchKeys() = default;
+        ~DeviceKSwitchKeys() { release(); }
+        DeviceKSwitchKeys(const DeviceKSwitchKeys &) = delete;
+        DeviceKSwitchKeys &operator=(const DeviceKSwitchKeys &) = delete;
+        DeviceKSwitchKeys(DeviceKSwitchKeys &&o) noexcept { *this = std::move(o); }
+        DeviceKSwitchKeys &operator=(DeviceKSwitchKeys &&o) noexcept
+        {
+            if (this != &o)
+            {
+                release();
+                ctx_ = o.ctx_, keys_ = std::move(o.keys_), parms_id_ = o.parms_id_;
+                o.ctx_ = nullptr, o.keys_.clear(), o.parms_id_ = seal::parms_id_zero;
+            }
+            return *this;
+        }
+        // the key level (KSwitchKeys::parms_id)
+        const seal::parms_id_type &parms_id() const noexcept { return parms_id_; }
+        // non-empty slots (KSwitchKeys::size)
+        std::size_t size() const noexcept
+        {
+            return static_cast<std::size_t>(std::count_if(keys_.begin(), keys_.end(), [](const sb200_kswitch_key *k) { return k != nullptr; }));
+        }
+        std::size_t device_bytes() const noexcept
+        {
+            std::size_t bytes = 0;
+            for (const sb200_kswitch_key *k : keys_)
+                bytes += sb200_kswitch_key_device_bytes(k);
+            return bytes;
+        }
+        void release() noexcept
+        {
+            for (sb200_kswitch_key *k : keys_)
+                if (k)
+                    sb200_kswitch_key_destroy(k);
+            keys_.clear();
+            ctx_ = nullptr, parms_id_ = seal::parms_id_zero;
+        }
+
+    protected:
+        bool has_slot(std::size_t index) const noexcept { return index < keys_.size() && keys_[index]; }
+
+    private:
+        friend class Evaluator;
+        friend class KeyGenerator;
+        // replaces the contents with `keys` (indexed by slot, nullptr = empty), which this object then owns
+        void assign(sb200_context *ctx, const seal::parms_id_type &parms_id, std::vector<sb200_kswitch_key *> &&keys) noexcept
+        {
+            release();
+            ctx_ = ctx, parms_id_ = parms_id, keys_ = std::move(keys);
+        }
+        sb200_context *ctx_ = nullptr;
+        std::vector<sb200_kswitch_key *> keys_;
+        seal::parms_id_type parms_id_ = seal::parms_id_zero;
+    };
+    // RelinKeys on the device: slot RelinKeys::get_index(key_power)
+    class DeviceRelinKeys : public DeviceKSwitchKeys
+    {
+    public:
+        bool has_key(std::size_t key_power) const { return has_slot(seal::RelinKeys::get_index(key_power)); }
+    };
+    // GaloisKeys on the device: slot GaloisKeys::get_index(galois_elt); has_key throws like GaloisKeys::has_key for an even element
+    class DeviceGaloisKeys : public DeviceKSwitchKeys
+    {
+    public:
+        bool has_key(std::uint32_t galois_elt) const { return has_slot(seal::GaloisKeys::get_index(galois_elt)); }
+    };
+
     class Evaluator
     {
     public:
@@ -861,6 +939,83 @@ namespace seal_b200
             copy_meta(source, destination);
             check(sb200_memcpy_d2d(ctx_, destination.d_, source.d_, source.batch_ * source.words_per_ciphertext() * sizeof(std::uint64_t), nullptr));
         }
+        // Ciphertext::load / unsafe_load (ciphertext.cpp:249-395) of `count` streams into one batch: none, zlib and seeded streams,
+        // words copied from the streams to the device and seeded c_1s expanded there (sb200_ciphertext_load).  The members must share
+        // parms_id, size, NTT form, scale and correction factor (std::invalid_argument, raised before anything is written); a stream
+        // the reference rejects throws what Ciphertext::load throws.  destination changes only on success.
+        void load(const seal::seal_byte *const *streams, const std::size_t *sizes, std::size_t count, CiphertextBatch &destination) const
+        {
+            load_batch(streams, sizes, count, true, destination);
+        }
+        void unsafe_load(const seal::seal_byte *const *streams, const std::size_t *sizes, std::size_t count, CiphertextBatch &destination) const
+        {
+            load_batch(streams, sizes, count, false, destination);
+        }
+        // Ciphertext::save (ciphertext.cpp:190-247) of every member: streams[i] = the bytes seal::Ciphertext::save(compr_mode) writes for
+        // member i.  compr_mode none is written from the device (sb200_ciphertext_save); other modes hand those members to
+        // seal::Serialization::Save, as Ciphertext::save does.
+        void save(const CiphertextBatch &source, std::vector<std::vector<seal::seal_byte>> &streams,
+                  seal::compr_mode_type compr_mode = seal::Serialization::compr_mode_default) const
+        {
+            owned(source);
+            const std::size_t plain = sb200_ciphertext_save_size(ctx_, source.L_, source.size_), B = source.batch_;
+            std::vector<std::vector<seal::seal_byte>> out(B, std::vector<seal::seal_byte>(plain));
+            std::vector<std::uint8_t *> ptrs(B);
+            std::vector<sb200_ct_info> meta(B);
+            for (std::size_t i = 0; i < B; i++)
+            {
+                ptrs[i] = reinterpret_cast<std::uint8_t *>(out[i].data());
+                meta[i].is_ntt_form = source.ntt_ ? 1 : 0, meta[i].scale = source.scale_, meta[i].correction_factor = source.cf_;
+            }
+            {
+                std::lock_guard<std::mutex> lock(mu_);
+                check(sb200_ciphertext_save(ctx_, B, source.L_, source.size_, source.d_, meta.data(), ptrs.data(), plain, nullptr));
+            }
+            if (compr_mode != seal::compr_mode_type::none)
+                for (auto &s : out)
+                {
+                    std::vector<seal::seal_byte> z(static_cast<std::size_t>(save_size_of(plain, compr_mode)));
+                    const auto got = seal::Serialization::Save(
+                        [&s](std::ostream &o) { o.write(reinterpret_cast<const char *>(s.data() + kSealHeader), static_cast<std::streamsize>(s.size() - kSealHeader)); },
+                        static_cast<std::streamoff>(s.size()), z.data(), z.size(), compr_mode, false);
+                    z.resize(static_cast<std::size_t>(got));
+                    s = std::move(z);
+                }
+            streams = std::move(out);
+        }
+        // Ciphertext::save_size of one member (an upper bound for compressed modes, as the reference's)
+        std::streamoff save_size(const CiphertextBatch &source, seal::compr_mode_type compr_mode = seal::Serialization::compr_mode_default) const
+        {
+            owned(source);
+            return save_size_of(sb200_ciphertext_save_size(ctx_, source.L_, source.size_), compr_mode);
+        }
+
+        // ---- device-resident key sets (DeviceRelinKeys / DeviceGaloisKeys) ----
+        // RelinKeys::load / GaloisKeys::load (kswitchkeys.cpp:42-160) straight onto the device, for streams saved with compr_mode none
+        // or zlib and the seeded streams of KeyGenerator's Serializable overloads: the object is inflated and parsed once, and seeded
+        // c_1s expand on the device (sb200_kswitch_keys_load).  A stream the reference rejects throws what its load throws.
+        // destination changes only on success.
+        void load(const seal::seal_byte *in, std::size_t size, DeviceRelinKeys &destination) const { load_keys(in, size, nullptr, 0, destination); }
+        void load(const seal::seal_byte *in, std::size_t size, DeviceGaloisKeys &destination) const
+        {
+            load_keys(in, size, nullptr, context_.key_context_data()->parms().poly_modulus_degree(), destination);
+        }
+        // only the keys of galois_elts (any order, duplicates ignored): at n = 65536 a server loads the keys that fit on the device.  An
+        // element without a key in the stream: std::invalid_argument.
+        void load(const seal::seal_byte *in, std::size_t size, const std::vector<std::uint32_t> &galois_elts, DeviceGaloisKeys &destination) const
+        {
+            std::vector<std::size_t> slots;
+            for (const std::uint32_t elt : galois_elts)
+            {
+                const std::size_t s = seal::GaloisKeys::get_index(elt);
+                if (std::find(slots.begin(), slots.end(), s) == slots.end())
+                    slots.push_back(s);
+            }
+            load_keys(in, size, &slots, context_.key_context_data()->parms().poly_modulus_degree(), destination);
+        }
+        // the non-empty slots of a seal:: key object, one device key each (sb200_kswitch_key_create)
+        void upload(const seal::RelinKeys &keys, DeviceRelinKeys &destination) const { upload_keys(keys, destination); }
+        void upload(const seal::GaloisKeys &keys, DeviceGaloisKeys &destination) const { upload_keys(keys, destination); }
         // Evaluator::multiply_inplace (evaluator.cpp:352-393), any sizes
         void multiply_inplace(CiphertextBatch &encrypted1, const CiphertextBatch &encrypted2) const
         {
@@ -890,8 +1045,23 @@ namespace seal_b200
                 encrypted1.cf_ = seal::util::multiply_uint_mod(encrypted1.cf_, encrypted2.cf_, cd->parms().plain_modulus());
         }
         void square_inplace(CiphertextBatch &encrypted) const { multiply_inplace(encrypted, encrypted); }
-        // Evaluator::relinearize_inplace (evaluator.cpp:1144-1199)
-        void relinearize_inplace(CiphertextBatch &encrypted, const seal::RelinKeys &relin_keys) const
+        // Evaluator::relinearize_inplace (evaluator.cpp:1144-1199).  Every key-switching member of a batch takes the keys as a seal::
+        // object (uploaded through the key cache) or as a device key set; both overloads share one body, which differs only in key_for.
+        void relinearize_inplace(CiphertextBatch &encrypted, const seal::RelinKeys &relin_keys) const { relinearize_batch(encrypted, relin_keys); }
+        void relinearize_inplace(CiphertextBatch &encrypted, const DeviceRelinKeys &relin_keys) const { relinearize_batch(encrypted, relin_keys); }
+        // multiply + relinearize in one device pass (both operands size 2); the result replaces encrypted1
+        void multiply_relinearize_inplace(CiphertextBatch &encrypted1, const CiphertextBatch &encrypted2, const seal::RelinKeys &relin_keys) const
+        {
+            multiply_relinearize_batch(encrypted1, encrypted2, relin_keys);
+        }
+        void multiply_relinearize_inplace(CiphertextBatch &encrypted1, const CiphertextBatch &encrypted2, const DeviceRelinKeys &relin_keys) const
+        {
+            multiply_relinearize_batch(encrypted1, encrypted2, relin_keys);
+        }
+
+    private:
+        template <class RelinKeys>
+        void relinearize_batch(CiphertextBatch &encrypted, const RelinKeys &relin_keys) const
         {
             owned(encrypted);
             if (relin_keys.parms_id() != context_.key_parms_id())
@@ -929,8 +1099,8 @@ namespace seal_b200
             adopt(encrypted);
             encrypted.size_ = 2;
         }
-        // multiply + relinearize in one device pass (both operands size 2); the result replaces encrypted1
-        void multiply_relinearize_inplace(CiphertextBatch &encrypted1, const CiphertextBatch &encrypted2, const seal::RelinKeys &relin_keys) const
+        template <class RelinKeys>
+        void multiply_relinearize_batch(CiphertextBatch &encrypted1, const CiphertextBatch &encrypted2, const RelinKeys &relin_keys) const
         {
             owned(encrypted1), owned(encrypted2);
             if (encrypted1.parms_id_ != encrypted2.parms_id_ || encrypted1.batch_ != encrypted2.batch_)
@@ -960,6 +1130,8 @@ namespace seal_b200
             if (bgv)
                 encrypted1.cf_ = seal::util::multiply_uint_mod(encrypted1.cf_, encrypted2.cf_, cd->parms().plain_modulus());
         }
+
+    public:
         // Evaluator::rescale_to_next_inplace / mod_switch_to_next_inplace (evaluator.cpp:1404-1541), any size
         void rescale_to_next_inplace(CiphertextBatch &encrypted) const
         {
@@ -1010,6 +1182,41 @@ namespace seal_b200
         // key per key-switching chunk.  Each product is a function of its two operands alone, so the words are the reference's.
         void multiply_many(const std::vector<CiphertextBatch> &encrypteds, const seal::RelinKeys &relin_keys, CiphertextBatch &destination) const
         {
+            multiply_many_batch(encrypteds, relin_keys, destination);
+        }
+        void multiply_many(const std::vector<CiphertextBatch> &encrypteds, const DeviceRelinKeys &relin_keys, CiphertextBatch &destination) const
+        {
+            multiply_many_batch(encrypteds, relin_keys, destination);
+        }
+        // exponentiate (evaluator.cpp:1726-1757): multiply_many of `exponent` copies of encrypted, with the copies' queue kept in
+        // run-length form so that the schedule costs O(log exponent) and equal products are computed once (4 products for exponent
+        // 16, 5 for 13, against the reference's exponent - 1).  The reference allocates the copies and fails with std::bad_alloc
+        // for an exponent it cannot allocate; this member allocates no copies and does not reproduce that failure.
+        void exponentiate_inplace(CiphertextBatch &encrypted, std::uint64_t exponent, const seal::RelinKeys &relin_keys) const
+        {
+            exponentiate_batch(encrypted, exponent, relin_keys);
+        }
+        void exponentiate_inplace(CiphertextBatch &encrypted, std::uint64_t exponent, const DeviceRelinKeys &relin_keys) const
+        {
+            exponentiate_batch(encrypted, exponent, relin_keys);
+        }
+        void exponentiate(const CiphertextBatch &encrypted, std::uint64_t exponent, const seal::RelinKeys &relin_keys,
+                          CiphertextBatch &destination) const
+        {
+            copy(encrypted, destination);
+            exponentiate_inplace(destination, exponent, relin_keys);
+        }
+        void exponentiate(const CiphertextBatch &encrypted, std::uint64_t exponent, const DeviceRelinKeys &relin_keys,
+                          CiphertextBatch &destination) const
+        {
+            copy(encrypted, destination);
+            exponentiate_inplace(destination, exponent, relin_keys);
+        }
+
+    private:
+        template <class RelinKeys>
+        void multiply_many_batch(const std::vector<CiphertextBatch> &encrypteds, const RelinKeys &relin_keys, CiphertextBatch &destination) const
+        {
             if (encrypteds.empty())
                 throw std::invalid_argument("encrypteds vector must not be empty");
             for (auto &e : encrypteds)
@@ -1028,11 +1235,8 @@ namespace seal_b200
             }
             run_products(leaves, schedule_products(leaves.size(), runs), relin_keys, destination);
         }
-        // exponentiate (evaluator.cpp:1726-1757): multiply_many of `exponent` copies of encrypted, with the copies' queue kept in
-        // run-length form so that the schedule costs O(log exponent) and equal products are computed once (4 products for exponent
-        // 16, 5 for 13, against the reference's exponent - 1).  The reference allocates the copies and fails with std::bad_alloc
-        // for an exponent it cannot allocate; this member allocates no copies and does not reproduce that failure.
-        void exponentiate_inplace(CiphertextBatch &encrypted, std::uint64_t exponent, const seal::RelinKeys &relin_keys) const
+        template <class RelinKeys>
+        void exponentiate_batch(CiphertextBatch &encrypted, std::uint64_t exponent, const RelinKeys &relin_keys) const
         {
             if (!context_.get_context_data(encrypted.parms_id_))
                 throw std::invalid_argument("encrypted is not valid for encryption parameters");
@@ -1048,12 +1252,8 @@ namespace seal_b200
             run_products({ &encrypted }, schedule_products(1, { { 0, exponent } }), relin_keys, result);
             encrypted = std::move(result);
         }
-        void exponentiate(const CiphertextBatch &encrypted, std::uint64_t exponent, const seal::RelinKeys &relin_keys,
-                          CiphertextBatch &destination) const
-        {
-            copy(encrypted, destination);
-            exponentiate_inplace(destination, exponent, relin_keys);
-        }
+
+    public:
         // mod_switch_to / rescale_to (evaluator.cpp:1451-1473, :1543-1590): the reference's checks, then single steps down to parms_id
         void mod_switch_to_inplace(CiphertextBatch &encrypted, seal::parms_id_type parms_id) const
         {
@@ -1080,6 +1280,49 @@ namespace seal_b200
         // apply_galois / rotations (evaluator.cpp:2384-2559)
         void apply_galois_inplace(CiphertextBatch &encrypted, std::uint32_t galois_elt, const seal::GaloisKeys &galois_keys) const
         {
+            apply_galois_batch(encrypted, galois_elt, galois_keys);
+        }
+        void apply_galois_inplace(CiphertextBatch &encrypted, std::uint32_t galois_elt, const DeviceGaloisKeys &galois_keys) const
+        {
+            apply_galois_batch(encrypted, galois_elt, galois_keys);
+        }
+        void rotate_rows_inplace(CiphertextBatch &encrypted, int steps, const seal::GaloisKeys &galois_keys) const
+        {
+            rotate_rows_batch(encrypted, steps, galois_keys);
+        }
+        void rotate_rows_inplace(CiphertextBatch &encrypted, int steps, const DeviceGaloisKeys &galois_keys) const
+        {
+            rotate_rows_batch(encrypted, steps, galois_keys);
+        }
+        void rotate_vector_inplace(CiphertextBatch &encrypted, int steps, const seal::GaloisKeys &galois_keys) const
+        {
+            rotate_vector_batch(encrypted, steps, galois_keys);
+        }
+        void rotate_vector_inplace(CiphertextBatch &encrypted, int steps, const DeviceGaloisKeys &galois_keys) const
+        {
+            rotate_vector_batch(encrypted, steps, galois_keys);
+        }
+        void rotate_columns_inplace(CiphertextBatch &encrypted, const seal::GaloisKeys &galois_keys) const
+        {
+            rotate_columns_batch(encrypted, galois_keys);
+        }
+        void rotate_columns_inplace(CiphertextBatch &encrypted, const DeviceGaloisKeys &galois_keys) const
+        {
+            rotate_columns_batch(encrypted, galois_keys);
+        }
+        void complex_conjugate_inplace(CiphertextBatch &encrypted, const seal::GaloisKeys &galois_keys) const
+        {
+            complex_conjugate_batch(encrypted, galois_keys);
+        }
+        void complex_conjugate_inplace(CiphertextBatch &encrypted, const DeviceGaloisKeys &galois_keys) const
+        {
+            complex_conjugate_batch(encrypted, galois_keys);
+        }
+
+    private:
+        template <class GaloisKeys>
+        void apply_galois_batch(CiphertextBatch &encrypted, std::uint32_t galois_elt, const GaloisKeys &galois_keys) const
+        {
             owned(encrypted);
             if (galois_keys.parms_id() != context_.key_parms_id())
                 throw std::invalid_argument("galois_keys is not valid for encryption parameters");
@@ -1096,30 +1339,36 @@ namespace seal_b200
             check(sb200_apply_galois(ctx_, encrypted.L_, encrypted.batch_, encrypted.d_, galois_elt, key, out, nullptr));
             adopt(encrypted);
         }
-        void rotate_rows_inplace(CiphertextBatch &encrypted, int steps, const seal::GaloisKeys &galois_keys) const
+        template <class GaloisKeys>
+        void rotate_rows_batch(CiphertextBatch &encrypted, int steps, const GaloisKeys &galois_keys) const
         {
             if (scheme_ != seal::scheme_type::bfv && scheme_ != seal::scheme_type::bgv)
                 throw std::logic_error("unsupported scheme");
             rotate_batch(encrypted, steps, galois_keys);
         }
-        void rotate_vector_inplace(CiphertextBatch &encrypted, int steps, const seal::GaloisKeys &galois_keys) const
+        template <class GaloisKeys>
+        void rotate_vector_batch(CiphertextBatch &encrypted, int steps, const GaloisKeys &galois_keys) const
         {
             if (scheme_ != seal::scheme_type::ckks)
                 throw std::logic_error("unsupported scheme");
             rotate_batch(encrypted, steps, galois_keys);
         }
-        void rotate_columns_inplace(CiphertextBatch &encrypted, const seal::GaloisKeys &galois_keys) const
+        template <class GaloisKeys>
+        void rotate_columns_batch(CiphertextBatch &encrypted, const GaloisKeys &galois_keys) const
         {
             if (scheme_ != seal::scheme_type::bfv && scheme_ != seal::scheme_type::bgv)
                 throw std::logic_error("unsupported scheme");
             conjugate_batch(encrypted, galois_keys);
         }
-        void complex_conjugate_inplace(CiphertextBatch &encrypted, const seal::GaloisKeys &galois_keys) const
+        template <class GaloisKeys>
+        void complex_conjugate_batch(CiphertextBatch &encrypted, const GaloisKeys &galois_keys) const
         {
             if (scheme_ != seal::scheme_type::ckks)
                 throw std::logic_error("unsupported scheme");
             conjugate_batch(encrypted, galois_keys);
         }
+
+    public:
         // transform_to_ntt_inplace / transform_from_ntt_inplace (evaluator.cpp:2289-2382)
         void transform_to_ntt_inplace(CiphertextBatch &encrypted) const
         {
@@ -1600,6 +1849,137 @@ namespace seal_b200
             evict(h);
             return h;
         }
+        // a device key set's handle, with the checks of the overload above (its keys always have k - 1 >= L digits)
+        sb200_kswitch_key *key_for(const DeviceKSwitchKeys &keys, std::size_t index, std::size_t) const
+        {
+            if (keys.parms_id_ != context_.key_parms_id())
+                throw std::invalid_argument("parameter mismatch");
+            if (keys.ctx_ != ctx_)
+                throw std::invalid_argument("keys are not on this evaluator's device context");
+            if (index >= keys.keys_.size())
+                throw std::out_of_range("kswitch_keys_index");
+            if (!keys.keys_[index])
+                throw std::invalid_argument("keyswitching key does not exist");
+            return keys.keys_[index];
+        }
+        // ---- helpers of the stream and key-set members ----
+        static constexpr std::size_t kSealHeader = sizeof(seal::Serialization::SEALHeader);
+        // Ciphertext::save_size from the uncompressed size: header + ComprSizeEstimate(members)
+        static std::streamoff save_size_of(std::size_t plain, seal::compr_mode_type compr_mode)
+        {
+            return static_cast<std::streamoff>(kSealHeader + seal::Serialization::ComprSizeEstimate(plain - kSealHeader, compr_mode));
+        }
+        void load_batch(const seal::seal_byte *const *streams, const std::size_t *sizes, std::size_t count, bool validate,
+                        CiphertextBatch &destination) const
+        {
+            if (!streams || !sizes || !count)
+                throw std::invalid_argument("batch cannot be empty");
+            std::vector<const std::uint8_t *> in(count);
+            sb200_ct_info f{};
+            for (std::size_t i = 0; i < count; i++)
+            {
+                if (!streams[i])
+                    throw std::invalid_argument("in cannot be null");
+                in[i] = reinterpret_cast<const std::uint8_t *>(streams[i]);
+                sb200_ct_info info{};
+                check(sb200_ciphertext_inspect(in[i], sizes[i], &info));
+                if (i == 0)
+                    f = info;
+                else if (std::memcmp(info.parms_id, f.parms_id, sizeof(f.parms_id)) != 0 || info.size != f.size ||
+                         info.is_ntt_form != f.is_ntt_form || info.correction_factor != f.correction_factor ||
+                         std::memcmp(&info.scale, &f.scale, sizeof(double)) != 0)
+                    throw std::invalid_argument("batch members must share parms_id, size, NTT form, scale and correction factor");
+            }
+            seal::parms_id_type pid;
+            std::memcpy(pid.data(), f.parms_id, sizeof(f.parms_id));
+            auto cd = context_.get_context_data(pid);
+            if (!cd || cd->parms().coeff_modulus().size() != f.coeff_modulus_size) // is_metadata_valid_for (ciphertext.cpp:299-302)
+                throw std::logic_error("ciphertext data is invalid");
+            CiphertextBatch loaded;
+            std::lock_guard<std::mutex> lock(mu_);
+            shape(loaded, count, f.size, f.coeff_modulus_size, f.poly_modulus_degree);
+            check(sb200_ciphertext_load(ctx_, count, in.data(), sizes, f.coeff_modulus_size, f.size, validate ? 1 : 0, loaded.d_, nullptr, nullptr));
+            loaded.parms_id_ = pid, loaded.ntt_ = f.is_ntt_form != 0, loaded.scale_ = f.scale, loaded.cf_ = f.correction_factor;
+            destination = std::move(loaded);
+        }
+        // slots == nullptr: every non-empty slot; min_slots = the slot count the set reports at least (GaloisKeys: n)
+        void load_keys(const seal::seal_byte *in, std::size_t size, const std::vector<std::size_t> *slots, std::size_t min_slots,
+                       DeviceKSwitchKeys &destination) const
+        {
+            if (!in)
+                throw std::invalid_argument("in cannot be null");
+            const std::size_t cap = slots ? slots->size() : std::max<std::size_t>(context_.key_context_data()->parms().poly_modulus_degree(), 64);
+            const std::size_t none = 0;
+            std::vector<sb200_kswitch_key *> out(std::max<std::size_t>(cap, 1), nullptr);
+            std::vector<std::size_t> got(out.size());
+            std::size_t made = 0;
+            check(sb200_kswitch_keys_load(ctx_, reinterpret_cast<const std::uint8_t *>(in), size, slots ? (slots->empty() ? &none : slots->data()) : nullptr,
+                                          cap, out.data(), got.data(), &made));
+            adopt_keys(out.data(), got.data(), made, min_slots, destination);
+        }
+        // takes ownership of `count` handles for the slots `slots` (destroyed if this throws)
+        void adopt_keys(sb200_kswitch_key **handles, const std::size_t *slots, std::size_t count, std::size_t min_slots,
+                        DeviceKSwitchKeys &destination) const
+        {
+            try
+            {
+                std::size_t n_slots = min_slots;
+                for (std::size_t i = 0; i < count; i++)
+                    n_slots = std::max(n_slots, slots[i] + 1);
+                std::vector<sb200_kswitch_key *> by_slot(n_slots, nullptr);
+                for (std::size_t i = 0; i < count; i++)
+                    by_slot[slots[i]] = handles[i];
+                destination.assign(ctx_, context_.key_parms_id(), std::move(by_slot));
+            }
+            catch (...)
+            {
+                for (std::size_t i = 0; i < count; i++)
+                    sb200_kswitch_key_destroy(handles[i]);
+                throw;
+            }
+        }
+        void upload_keys(const seal::KSwitchKeys &keys, DeviceKSwitchKeys &destination) const
+        {
+            if (keys.parms_id() != context_.key_parms_id())
+                throw std::invalid_argument("keys is not valid for encryption parameters");
+            const std::size_t K = context_.key_context_data()->parms().coeff_modulus().size();
+            const std::size_t n = context_.key_context_data()->parms().poly_modulus_degree(), row = 2 * K * n;
+            for (auto &kv : keys.data()) // is_valid_for(KSwitchKeys) (valcheck.cpp:292-323): k - 1 valid public keys per non-empty slot
+            {
+                if (!kv.empty() && kv.size() != K - 1)
+                    throw std::invalid_argument("keys is not valid for encryption parameters");
+                for (auto &each : kv)
+                    if (!seal::is_metadata_valid_for(each, context_) || !seal::is_buffer_valid(each))
+                        throw std::invalid_argument("keys is not valid for encryption parameters");
+            }
+            std::vector<sb200_kswitch_key *> handles;
+            std::vector<std::size_t> slots;
+            handles.reserve(keys.data().size()), slots.reserve(keys.data().size());
+            try
+            {
+                std::vector<std::uint64_t> flat;
+                for (std::size_t i = 0; i < keys.data().size(); i++)
+                {
+                    auto &kv = keys.data()[i];
+                    if (kv.empty())
+                        continue;
+                    flat.resize(kv.size() * row);
+                    for (std::size_t j = 0; j < kv.size(); j++)
+                        std::memcpy(flat.data() + j * row, kv[j].data().data(), row * sizeof(std::uint64_t));
+                    sb200_kswitch_key *h = nullptr;
+                    check(sb200_kswitch_key_create(ctx_, flat.data(), kv.size(), &h));
+                    handles.push_back(h);
+                    slots.push_back(i);
+                }
+            }
+            catch (...)
+            {
+                for (sb200_kswitch_key *h : handles)
+                    sb200_kswitch_key_destroy(h);
+                throw;
+            }
+            adopt_keys(handles.data(), slots.data(), handles.size(), keys.data().size(), destination);
+        }
         // ---- helpers of the CiphertextBatch members ----
         // data of already validated ciphertexts of one shape -> one device slab; metadata of the first member
         void upload_rows(const seal::Ciphertext *cts, std::size_t count, CiphertextBatch &destination) const
@@ -1881,7 +2261,8 @@ namespace seal_b200
             return s;
         }
         // runs a schedule over the leaf batches; the result goes to destination with the reference's metadata
-        void run_products(const std::vector<const CiphertextBatch *> &leaves, const ProductSchedule &s, const seal::RelinKeys &relin_keys,
+        template <class RelinKeys>
+        void run_products(const std::vector<const CiphertextBatch *> &leaves, const ProductSchedule &s, const RelinKeys &relin_keys,
                           CiphertextBatch &destination) const
         {
             const CiphertextBatch &f = *leaves[0];
@@ -1994,7 +2375,8 @@ namespace seal_b200
             copy_meta(meta, x);
             check(sb200_memcpy_d2d(ctx_, x.d_, words, meta.batch_ * 2 * meta.L_ * meta.n_ * sizeof(std::uint64_t), nullptr));
         }
-        void rotate_batch(CiphertextBatch &encrypted, int steps, const seal::GaloisKeys &galois_keys) const
+        template <class GaloisKeys>
+        void rotate_batch(CiphertextBatch &encrypted, int steps, const GaloisKeys &galois_keys) const
         {
             owned(encrypted);
             auto cd = context_.get_context_data(encrypted.parms_id_);
@@ -2018,7 +2400,8 @@ namespace seal_b200
                 if (static_cast<std::size_t>(std::abs(st)) != (n >> 1))
                     rotate_batch(encrypted, st, galois_keys);
         }
-        void conjugate_batch(CiphertextBatch &encrypted, const seal::GaloisKeys &galois_keys) const
+        template <class GaloisKeys>
+        void conjugate_batch(CiphertextBatch &encrypted, const GaloisKeys &galois_keys) const
         {
             owned(encrypted);
             auto cd = context_.get_context_data(encrypted.parms_id_);

@@ -106,6 +106,50 @@ namespace seal_b200
             create_galois_keys(context_.key_context_data()->galois_tool()->get_elts_all(), destination);
         }
 
+        // ---- device key sets: the same keys, from the same seed draws, made on the device and kept there (sb200_kswitch_key_generate
+        // with no host copy).  The keys belong to this generator's device context: to use them with an Evaluator, construct the
+        // generator with that Evaluator. ----
+        void create_relin_keys(DeviceRelinKeys &destination)
+        {
+            std::vector<sb200_kswitch_key *> keys(1, nullptr);
+            generate_device(0, keys[0]);
+            destination.assign(ctx_, context_.key_parms_id(), std::move(keys));
+        }
+        void create_galois_keys(const std::vector<std::uint32_t> &galois_elts, DeviceGaloisKeys &destination)
+        {
+            const std::size_t n = context_.key_context_data()->parms().poly_modulus_degree();
+            std::vector<sb200_kswitch_key *> keys(n, nullptr);
+            try
+            {
+                for (const std::uint32_t elt : galois_elts)
+                {
+                    if (!(elt & 1) || elt >= 2 * n)
+                        throw std::invalid_argument("Galois element is not valid");
+                    sb200_kswitch_key *&slot = keys[seal::GaloisKeys::get_index(elt)];
+                    if (!slot)
+                        generate_device(elt, slot);
+                }
+            }
+            catch (...)
+            {
+                for (sb200_kswitch_key *k : keys)
+                    if (k)
+                        sb200_kswitch_key_destroy(k);
+                throw;
+            }
+            destination.assign(ctx_, context_.key_parms_id(), std::move(keys));
+        }
+        void create_galois_keys(const std::vector<int> &steps, DeviceGaloisKeys &destination)
+        {
+            if (!context_.key_context_data()->qualifiers().using_batching)
+                throw std::logic_error("encryption parameters do not support batching");
+            create_galois_keys(context_.key_context_data()->galois_tool()->get_elts_from_steps(steps), destination);
+        }
+        void create_galois_keys(DeviceGaloisKeys &destination)
+        {
+            create_galois_keys(context_.key_context_data()->galois_tool()->get_elts_all(), destination);
+        }
+
         // ---- Serializable overloads (keygenerator.h:73-76, 102-105, 160-163, 216-223, 270-273): seeded streams ----
         Serializable<seal::PublicKey> create_public_key() const
         {
@@ -202,6 +246,18 @@ namespace seal_b200
                 prepare(cd, destination[j]);
                 std::memcpy(destination[j].data().data(), h.data() + j * words, words * sizeof(std::uint64_t));
             }
+        }
+        // generate_one_kswitch_key with the key left on the device: the same seed draws as generate_one
+        void generate_device(std::uint32_t galois_elt, sb200_kswitch_key *&out)
+        {
+            if (!context_.using_keyswitching())
+                throw std::logic_error("keyswitching is not supported by the context");
+            const std::size_t digits = context_.first_context_data()->parms().coeff_modulus().size();
+            int prng = 0;
+            std::vector<std::uint64_t> seeds = bootstrap_seeds(digits, prng);
+            const int rc = sb200_kswitch_key_generate(ctx_, key_, galois_elt, prng, ciphertext_prng(), seeds.data(), nullptr, &out);
+            seal::util::seal_memzero(seeds.data(), seeds.size() * sizeof(std::uint64_t));
+            status(rc);
         }
         // the destination of util::encrypt_zero_symmetric at the key level with is_ntt_form = true (util/rlwe.cpp:282-287)
         void prepare(const seal::SEALContext::ContextData &cd, seal::PublicKey &pk) const

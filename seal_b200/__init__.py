@@ -28,7 +28,8 @@ SYMBOLS = [
     "sb200_last_error", "sb200_context_create", "sb200_context_destroy", "sb200_coeff_modulus_create",
     "sb200_get_ntt_tables", "sb200_get_base_bsk", "sb200_galois_elt_from_step", "sb200_launch_count",
     "sb200_device_bytes", "sb200_context_set_limit", "sb200_device_malloc", "sb200_device_free", "sb200_host_malloc", "sb200_host_free", "sb200_memcpy_h2d", "sb200_memcpy_d2h", "sb200_memcpy_d2d", "sb200_memcpy_d2d_2d", "sb200_stream_synchronize", "sb200_upload_rows", "sb200_download_rows", "sb200_rescale_to_next_sized", "sb200_mod_switch_to_next_sized", "sb200_relinearize_sized", "sb200_rescale_to_next_sized_host", "sb200_mod_switch_to_next_sized_host", "sb200_relinearize_sized_host", "sb200_device_numa_node", "sb200_device_index", "sb200_keyswitch_chunk", "sb200_profile_enable", "sb200_profile_reset", "sb200_profile_read", "sb200_profile_read_work", "sb200_selftest_rate", "sb200_profile_read_work32", "sb200_selftest_ksint_info", "sb200_selftest_ksint_forward", "sb200_selftest_ksint_inverse", "sb200_selftest_ksint_product",
-    "sb200_kswitch_key_create", "sb200_kswitch_key_load", "sb200_kswitch_key_destroy", "sb200_ntt_forward",
+    "sb200_kswitch_key_create", "sb200_kswitch_key_load", "sb200_kswitch_keys_load", "sb200_kswitch_key_device_bytes",
+    "sb200_kswitch_key_destroy", "sb200_ntt_forward",
     "sb200_ntt_inverse", "sb200_multiply", "sb200_multiply_sized", "sb200_square", "sb200_add", "sb200_sub", "sb200_negate", "sb200_multiply_plain", "sb200_batch_encode", "sb200_batch_decode", "sb200_plain_to_ntt", "sb200_multiply_plain_coeff", "sb200_add_plain_coeff", "sb200_relinearize", "sb200_multiply_relinearize", "sb200_rescale_to_next",
     "sb200_mod_switch_to_next", "sb200_apply_galois", "sb200_ntt_forward_host", "sb200_ntt_inverse_host",
     "sb200_multiply_host", "sb200_multiply_sized_host", "sb200_square_host", "sb200_add_host", "sb200_sub_host", "sb200_negate_host", "sb200_multiply_plain_host", "sb200_batch_encode_host", "sb200_batch_decode_host", "sb200_plain_to_ntt_host", "sb200_multiply_plain_coeff_host", "sb200_add_plain_coeff_host",
@@ -98,6 +99,9 @@ def lib():
         L.sb200_kswitch_key_create.argtypes = [vp, _u64p, sz, C.POINTER(vp)]
         L.sb200_kswitch_key_destroy.argtypes = [vp]
         L.sb200_kswitch_key_load.argtypes = [vp, C.c_char_p, sz, sz, C.POINTER(vp)]
+        L.sb200_kswitch_keys_load.argtypes = [vp, C.c_char_p, sz, C.POINTER(sz), sz, C.POINTER(vp), C.POINTER(sz), C.POINTER(sz)]
+        L.sb200_kswitch_key_device_bytes.restype = sz
+        L.sb200_kswitch_key_device_bytes.argtypes = [vp]
         L.sb200_ntt_forward.argtypes = [vp, sz, sz, sz, vp, vp]
         L.sb200_ntt_inverse.argtypes = [vp, sz, sz, sz, vp, vp]
         L.sb200_multiply.argtypes = [vp, sz, sz, vp, vp, vp, vp]
@@ -243,6 +247,11 @@ class KSwitchKey:
         self = cls.__new__(cls)
         self.ctx, self.h = ctx, handle
         return self
+
+    @property
+    def device_bytes(self):
+        """bytes the key holds on the device: its words plus the integer key-switching path's copy"""
+        return lib().sb200_kswitch_key_device_bytes(self.h)
 
     def __del__(self):
         try:
@@ -939,6 +948,27 @@ class Context:
         _check(lib().sb200_kswitch_keys_generate_seeded(self.h, sk.h, e, len(galois_elts), bootstrap_prng, ciphertext_prng,
                                                         None if seeds is None else _hp(seeds), C.addressof(buf), cap))
         return buf.raw[:size]
+
+    def load_kswitch_keys(self, stream, indices=None, capacity=None):
+        """KSwitchKeys::load of the entries `indices` of a RelinKeys / GaloisKeys stream (none, zlib or seeded) in one pass; None =
+        every non-empty slot, at most `capacity` of them (default n, the slot count of a GaloisKeys object).  Returns a list of
+        KSwitchKey, each with its slot in `.slot`"""
+        if indices is None:
+            cap = self.n if capacity is None else capacity
+            idx = None
+        else:
+            cap = len(indices)
+            idx = (C.c_size_t * max(cap, 1))(*[int(i) for i in indices])
+        out = (C.c_void_p * max(cap, 1))()
+        slots = (C.c_size_t * max(cap, 1))()
+        got = C.c_size_t(0)
+        _check(lib().sb200_kswitch_keys_load(self.h, stream, len(stream), idx, cap, out, slots, C.byref(got)))
+        keys = []
+        for i in range(got.value):
+            key = KSwitchKey.wrap(self, C.c_void_p(out[i]))
+            key.slot = slots[i]
+            keys.append(key)
+        return keys
 
     def d_relinearize(self, in3, key, out2, L, batch):
         _check(lib().sb200_relinearize(self.h, L, batch, _dp(in3), key.h, _dp(out2), self._stream()))

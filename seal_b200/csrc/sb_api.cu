@@ -677,58 +677,108 @@ int sb200_kswitch_key_create(sb200_context *ctx, const uint64_t *h_key, size_t d
     SB_CATCH
 }
 
+} // extern "C"
+
+// KSwitchKeys::load of the entries data()[indices[i]] (indices == nullptr: every non-empty slot, at most `capacity` of them) in one
+// pass: the object is inflated at most once and its frame parsed once, every argument and metadata check runs before the first
+// handle is made, then each entry's rows go host -> device (c_0 only for a seeded member) and its seeded c_1s expand on the device.
+// Returns the handles in the order of `slots`; if anything throws, the handles made so far are destroyed with the vector.
+static std::vector<std::unique_ptr<sb200_kswitch_key>> kswitch_keys_load(Context &c, const uint8_t *stream, size_t len, const size_t *indices,
+                                                                         size_t count, std::vector<size_t> &slots)
+{
+    if (c.k < 2)
+        throw std::logic_error("keyswitching is not supported by the context");
+    std::vector<sbw::KSwitchEntry> entries;
+    std::vector<uint8_t> plain; // KSwitchKeys saved with compr_mode_type::zlib: inflate the object, then parse as usual
+    // bound: a GaloisKeys object holds at most 2 log2(n) + 1 < 64 keys of k-1 digits, plus one size word per slot
+    if (sbw::inflate_stream(stream, len, 64 * (c.k - 1) * sbw::save_size(2 * c.k * c.n) + 16 * c.n + 4096, plain))
+        stream = plain.data(), len = plain.size();
+    sbw::inspect_kswitch_slots(stream, len, indices, count, slots, entries);
+    if (!indices && entries.size() > count)
+        throw std::invalid_argument("out has too few entries for the keys present");
+    for (const sbw::KSwitchEntry &e : entries)
+    {
+        // is_valid_for(KSwitchKeys): keys live at the key level of this context (valcheck.cpp, kswitchkeys.cpp:149-153)
+        if (e.n != c.n || e.L != c.k || std::memcmp(e.parms_id, c.parms_ids[c.k - 1].data(), sizeof(e.parms_id)) != 0)
+            throw std::logic_error("KSwitchKeys data is invalid");
+        // is_valid_for(KSwitchKeys) (valcheck.cpp:292-323): one public key per decomposition prime, i.e. exactly k-1 digits
+        if (e.offsets.size() != c.k - 1)
+            throw std::logic_error("KSwitchKeys data is invalid");
+    }
+    const size_t digits = c.k - 1, row = 2 * c.k * c.n * sizeof(u64);
+    std::lock_guard<std::mutex> lock(c.mu);
+    cuda_check(cudaSetDevice(c.device), "cudaSetDevice");
+    std::vector<std::unique_ptr<sb200_kswitch_key>> keys;
+    keys.reserve(entries.size());
+    for (const sbw::KSwitchEntry &e : entries)
+    {
+        keys.push_back(kswitch_key_alloc(c, digits));
+        u64 *d_key = keys.back()->k.d_key.get();
+        // a seed-compressed member carries c_0 only (k n words) and the seed of c_1 = sample_poly_uniform at the key level
+        // (KSwitchKeys::load -> PublicKey::load -> Ciphertext::expand_seed, ciphertext.cpp:118-150)
+        std::vector<u64> seeds;
+        std::vector<int> types;
+        std::vector<long long> seed_dst;
+        for (size_t j = 0; j < digits; j++)
+        {
+            cuda_check(cudaMemcpy(reinterpret_cast<uint8_t *>(d_key) + j * row, stream + e.offsets[j], e.seeded[j] ? row / 2 : row,
+                                  cudaMemcpyHostToDevice),
+                       "upload key");
+            if (e.seeded[j])
+            {
+                u64 sd[8];
+                std::memcpy(sd, stream + e.seed_offsets[j], sizeof(sd));
+                seeds.insert(seeds.end(), sd, sd + 8);
+                types.push_back(e.seeded[j]);
+                seed_dst.push_back(static_cast<long long>((2 * j + 1) * c.k * c.n));
+            }
+        }
+        if (!seed_dst.empty())
+            op_expand_seeded(c, c.k, seed_dst.size(), seeds.data(), types.data(), seed_dst.data(), d_key, nullptr);
+        if (!kswitch_key_finish(c, keys.back()->k)) // KSwitchKeys::load ends in is_valid_for (kswitchkeys.cpp:149-153)
+            throw std::logic_error("KSwitchKeys data is invalid");
+    }
+    return keys;
+}
+
+extern "C" {
 int sb200_kswitch_key_load(sb200_context *ctx, const uint8_t *stream, size_t len, size_t index, sb200_kswitch_key **out)
 {
     SB_NEED(ctx);
     SB_NEED(stream);
     SB_NEED(out);
     SB_TRY
-    Context &c = *ctx->c;
-    if (c.k < 2)
-        throw std::logic_error("keyswitching is not supported by the context");
-    sbw::KSwitchEntry e;
-    std::vector<uint8_t> plain; // KSwitchKeys saved with compr_mode_type::zlib: inflate the object, then parse as usual
-    // bound: a GaloisKeys object holds at most 2 log2(n) + 1 < 64 keys of k-1 digits, plus one size word per slot
-    if (sbw::inflate_stream(stream, len, 64 * (c.k - 1) * sbw::save_size(2 * c.k * c.n) + 16 * c.n + 4096, plain))
-        stream = plain.data(), len = plain.size();
-    sbw::inspect_kswitch(stream, len, index, e);
-    // is_valid_for(KSwitchKeys): keys live at the key level of this context (valcheck.cpp, kswitchkeys.cpp:149-153)
-    if (e.n != c.n || e.L != c.k || std::memcmp(e.parms_id, c.parms_ids[c.k - 1].data(), sizeof(e.parms_id)) != 0)
-        throw std::logic_error("KSwitchKeys data is invalid");
-    const size_t digits = e.offsets.size();
-    // is_valid_for(KSwitchKeys) (valcheck.cpp:292-323): one public key per decomposition prime, i.e. exactly k-1 digits
-    if (digits != c.k - 1)
-        throw std::logic_error("KSwitchKeys data is invalid");
-    const size_t row = 2 * c.k * c.n * sizeof(u64);
-    std::lock_guard<std::mutex> lock(c.mu);
-    cuda_check(cudaSetDevice(c.device), "cudaSetDevice");
-    auto h = kswitch_key_alloc(c, digits);
-    // a seed-compressed member carries c_0 only (k n words) and the seed of c_1 = sample_poly_uniform at the key level
-    // (KSwitchKeys::load -> PublicKey::load -> Ciphertext::expand_seed, ciphertext.cpp:118-150)
-    std::vector<u64> seeds;
-    std::vector<int> types;
-    std::vector<long long> seed_dst;
-    for (size_t j = 0; j < digits; j++)
-    {
-        cuda_check(cudaMemcpy(reinterpret_cast<uint8_t *>(h->k.d_key.get()) + j * row, stream + e.offsets[j], e.seeded[j] ? row / 2 : row,
-                              cudaMemcpyHostToDevice),
-                   "upload key");
-        if (e.seeded[j])
-        {
-            u64 sd[8];
-            std::memcpy(sd, stream + e.seed_offsets[j], sizeof(sd));
-            seeds.insert(seeds.end(), sd, sd + 8);
-            types.push_back(e.seeded[j]);
-            seed_dst.push_back(static_cast<long long>((2 * j + 1) * c.k * c.n));
-        }
-    }
-    if (!seed_dst.empty())
-        op_expand_seeded(c, c.k, seed_dst.size(), seeds.data(), types.data(), seed_dst.data(), h->k.d_key.get(), nullptr);
-    if (!kswitch_key_finish(c, h->k)) // KSwitchKeys::load ends in is_valid_for (kswitchkeys.cpp:149-153)
-        throw std::logic_error("KSwitchKeys data is invalid");
-    *out = h.release();
+    std::vector<size_t> slots;
+    auto keys = kswitch_keys_load(*ctx->c, stream, len, &index, 1, slots);
+    *out = keys[0].release();
     return SB200_OK;
     SB_CATCH
+}
+
+int sb200_kswitch_keys_load(sb200_context *ctx, const uint8_t *stream, size_t len, const size_t *indices, size_t count,
+                            sb200_kswitch_key **out, size_t *out_indices, size_t *out_count)
+{
+    SB_NEED(ctx);
+    SB_NEED(stream);
+    SB_NEED(out);
+    SB_NEED(out_count);
+    SB_TRY
+    std::vector<size_t> slots;
+    auto keys = kswitch_keys_load(*ctx->c, stream, len, indices, count, slots);
+    for (size_t i = 0; i < keys.size(); i++)
+    {
+        out[i] = keys[i].release();
+        if (out_indices)
+            out_indices[i] = slots[i];
+    }
+    *out_count = keys.size();
+    return SB200_OK;
+    SB_CATCH
+}
+
+size_t sb200_kswitch_key_device_bytes(const sb200_kswitch_key *key)
+{
+    return key ? key->k.d_key.bytes() + key->k.d_key32.bytes() : 0;
 }
 
 int sb200_kswitch_key_destroy(sb200_kswitch_key *key)

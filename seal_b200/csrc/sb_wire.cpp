@@ -308,7 +308,8 @@ namespace sbw
         put<uint64_t>(w, info.data_words);
     }
     } // namespace
-    void inspect_kswitch(const uint8_t *p, size_t len, size_t index, KSwitchEntry &entry)
+    void inspect_kswitch_slots(const uint8_t *p, size_t len, const size_t *indices, size_t count, std::vector<size_t> &slots,
+                               std::vector<KSwitchEntry> &entries)
     {
         if (!p)
             throw std::invalid_argument("in cannot be null");
@@ -318,44 +319,79 @@ namespace sbw
         if (outer.size > len || outer.size < kHeaderBytes + 32 + 8)
             throw std::logic_error("loaded SEALHeader is invalid");
         const uint8_t *r = p + kHeaderBytes, *end = p + outer.size;
+        u64 pid[4];
         for (int i = 0; i < 4; i++)
-            entry.parms_id[i] = take<uint64_t>(r);
+            pid[i] = take<uint64_t>(r);
         const uint64_t dim1 = take<uint64_t>(r);
         if (dim1 > 131072)
             throw std::logic_error("KSwitchKeys outer dimension is invalid"); // kswitchkeys.cpp:121-125
-        entry.slots = static_cast<size_t>(dim1);
-        entry.offsets.clear();
-        entry.seeded.clear();
-        entry.seed_offsets.clear();
-        if (index >= dim1)
-            throw std::out_of_range("kswitch_keys_index");
-        for (uint64_t slot = 0; slot < dim1; slot++)
+        slots.clear();
+        entries.clear();
+        // want[slot] = 1 + the slot's position in `indices`, 0 = not requested; the frame is parsed up to the last slot needed
+        std::vector<size_t> want;
+        uint64_t last = dim1;
+        if (indices)
+        {
+            for (size_t i = 0; i < count; i++)
+                if (indices[i] >= dim1)
+                    throw std::out_of_range("kswitch_keys_index");
+            want.assign(static_cast<size_t>(dim1), 0);
+            last = 0;
+            for (size_t i = 0; i < count; i++)
+            {
+                if (want[indices[i]])
+                    throw std::invalid_argument("kswitch_keys_index is duplicated");
+                want[indices[i]] = i + 1;
+                last = std::max<uint64_t>(last, indices[i] + 1);
+            }
+            slots.assign(indices, indices + count);
+            entries.resize(count);
+        }
+        for (uint64_t slot = 0; slot < last; slot++)
         {
             if (static_cast<size_t>(end - r) < 8)
                 throw std::logic_error("loaded data is invalid");
             const uint64_t dim2 = take<uint64_t>(r);
             if (dim2 > 256)
                 throw std::logic_error("KSwitchKeys inner dimension is invalid");
+            if (!indices && dim2)
+            {
+                slots.push_back(static_cast<size_t>(slot));
+                entries.emplace_back();
+            }
+            KSwitchEntry *entry = indices ? (want[slot] ? &entries[want[slot] - 1] : nullptr) : (dim2 ? &entries.back() : nullptr);
+            if (entry)
+            {
+                std::memcpy(entry->parms_id, pid, sizeof(pid));
+                entry->slots = static_cast<size_t>(dim1);
+            }
             for (uint64_t j = 0; j < dim2; j++)
             {
                 sb200_ct_info info;
                 inspect(r, static_cast<size_t>(end - r), info);
-                if (slot == index)
+                if (entry)
                 {
-                    if (info.size != 2 || !info.is_ntt_form || std::memcmp(info.parms_id, entry.parms_id, sizeof(info.parms_id)) != 0 ||
-                        (j > 0 && (info.coeff_modulus_size != entry.L || info.poly_modulus_degree != entry.n)))
+                    if (info.size != 2 || !info.is_ntt_form || std::memcmp(info.parms_id, pid, sizeof(pid)) != 0 ||
+                        (j > 0 && (info.coeff_modulus_size != entry->L || info.poly_modulus_degree != entry->n)))
                         throw std::logic_error("key data is invalid");
-                    entry.L = static_cast<size_t>(info.coeff_modulus_size), entry.n = static_cast<size_t>(info.poly_modulus_degree);
-                    entry.offsets.push_back(static_cast<size_t>(r - p) + static_cast<size_t>(info.data_offset));
-                    entry.seeded.push_back(info.seeded);
-                    entry.seed_offsets.push_back(info.seeded ? static_cast<size_t>(r - p) + static_cast<size_t>(info.seed_offset) : 0);
+                    entry->L = static_cast<size_t>(info.coeff_modulus_size), entry->n = static_cast<size_t>(info.poly_modulus_degree);
+                    entry->offsets.push_back(static_cast<size_t>(r - p) + static_cast<size_t>(info.data_offset));
+                    entry->seeded.push_back(info.seeded);
+                    entry->seed_offsets.push_back(info.seeded ? static_cast<size_t>(r - p) + static_cast<size_t>(info.seed_offset) : 0);
                 }
                 r += info.stream_bytes;
             }
-            if (slot == index)
-                break; // later slots are not needed
         }
-        if (entry.offsets.empty())
-            throw std::invalid_argument("key not present"); // an empty slot (relinkeys.h:84-95, galoiskeys.h:75-86)
+        for (const KSwitchEntry &e : entries)
+            if (e.offsets.empty())
+                throw std::invalid_argument("key not present"); // an empty slot (relinkeys.h:84-95, galoiskeys.h:75-86)
+    }
+
+    void inspect_kswitch(const uint8_t *p, size_t len, size_t index, KSwitchEntry &entry)
+    {
+        std::vector<size_t> slots;
+        std::vector<KSwitchEntry> entries;
+        inspect_kswitch_slots(p, len, &index, 1, slots, entries);
+        entry = std::move(entries[0]);
     }
 } // namespace sbw

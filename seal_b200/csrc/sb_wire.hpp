@@ -68,4 +68,10 @@ namespace sbw
         std::vector<size_t> seed_offsets; // per digit: byte offset (from p) of the 64-byte seed of a seeded member, 0 otherwise
     };
     void inspect_kswitch(const uint8_t *p, size_t len, size_t index, KSwitchEntry &entry);
+    // Several entries in one pass over the object: entries[i] describes data()[slots[i]].  indices != nullptr: slots = indices[0..count);
+    // nullptr: every non-empty slot in slot order (count is ignored).  The frame is parsed up to the last slot needed.  Errors: an index
+    // at or past dim1 (std::out_of_range), a duplicated index (std::invalid_argument), a malformed object (std::logic_error), then an
+    // empty requested slot (std::invalid_argument, "key not present").  inspect_kswitch is the one-index case.
+    void inspect_kswitch_slots(const uint8_t *p, size_t len, const size_t *indices, size_t count, std::vector<size_t> &slots,
+                               std::vector<KSwitchEntry> &entries);
 } // namespace sbw
