@@ -43,8 +43,10 @@ def auxiliary_product(aux):
 # (p_{I mod S} - 1) delta_0.  Their transforms modulo p_t are those constants at every point, so for b = I = t (mod S) the sum
 # reaches L (p_t - 1)^2, the largest value the accumulators can see at this level; one call covers every auxiliary prime.  At
 # n = 4096 the largest auxiliary prime is 536813569 and L (p - 1)^2 < 2^64 holds up to L = 64 digits: deeper levels must leave the
-# integer path (Context::ksint_on).  The result of a constant input is a constant row per (b, c, i), in closed form below.
-@pytest.mark.parametrize("k", [41, 42, 64, 65, 66, 67, 256])
+# integer path (Context::ksint_on).  The result of a constant input is a constant row per (b, c, i), in closed form below.  Up to
+# 32 digits (k = 9, 33) the chunks of 16 ciphertexts take the INT8 tensor-core kernel, whose class sums the same rows drive to their largest
+# values; at k = 33 a level below the key level (strided key rows) is checked against the closed form too.
+@pytest.mark.parametrize("k", [9, 33, 41, 42, 64, 65, 66, 67, 256])
 def test_integer_path_accumulator_width(k):
     S = sb()
     n, L = 4096, k - 1
@@ -55,7 +57,9 @@ def test_integer_path_accumulator_width(k):
     assert aux and max(aux) < min(mods), "every constant below must be a canonical residue of every coefficient prime"
     max_digits = (2 ** 64 - 1) // (max(aux) - 1) ** 2
     assert max_digits == 64
-    batch = 16 if k <= 67 else St  # 16: the key-tile product kernel runs (up to 40 digits); above, the register-tile one
+    # 32: the host entry points cut a batch of 4 or more into at least two pipeline chunks, here two key-switching chunks of 16, where
+    # the tensor-core product kernel runs up to 32 digits, the key-tile one up to 40; above, the register-tile one
+    batch = 32 if k <= 67 else St
     cb = [aux[b % St] - 1 for b in range(batch)]
     kI = [aux[I % St] - 1 for I in range(k)]
     c3 = np.empty((batch, 3, L, n), dtype=np.uint64)
@@ -73,19 +77,41 @@ def test_integer_path_accumulator_width(k):
         assert reach >= 0.98 * L / 64 * 2 ** 64
     # closed form: digit sum at prime I = L c_b K_I (a constant polynomial), mod-down, added to the NTT-form constant rows
     qsp = int(mods[k - 1])
-    want = np.empty((batch, 2, L, n), dtype=np.uint64)
-    for b in range(batch):
-        acc_sp = L * cb[b] * kI[k - 1] % qsp
-        for i in range(L):
-            q = int(mods[i])
-            r = mod_down(L * cb[b] * kI[i] % q, acc_sp, q, qsp)
-            want[b, :, i, :] = (q - 1 + r) % q
+
+    def closed_form(Lv):
+        want = np.empty((batch, 2, Lv, n), dtype=np.uint64)
+        for b in range(batch):
+            acc_sp = Lv * cb[b] * kI[k - 1] % qsp
+            for i in range(Lv):
+                q = int(mods[i])
+                r = mod_down(Lv * cb[b] * kI[i] % q, acc_sp, q, qsp)
+                want[b, :, i, :] = (q - 1 + r) % q
+        return want
+
+    def relinearize_int(x, Lv):
+        """the integer path, and from the profile which product kernel ran: no 32-bit multiply-accumulates = the tensor cores"""
+        ctx.profile(True)
+        out = ctx.relinearize(x, rk)
+        macs = [r[7] for r in ctx.profile_read_work32() if r[0] == "ks32_mac"]
+        ctx.profile(False)
+        if Lv <= max_digits:
+            assert macs and (sum(macs) == 0) == (Lv <= 32), f"L = {Lv}: the tensor-core kernel runs for L <= 32 digits and chunks of 16"
+        else:
+            assert not macs, f"L = {Lv}: levels past {max_digits} digits leave the integer path"
+        return out
+
+    want = closed_form(L)
     rk = ctx.load_key(key)
     got = {}
     for mode in (KS_INT, KS_AUTO, KS_64):
         ctx.set_limit(S.Context.LIMIT_KS_ALGORITHM, mode)
-        got[mode] = ctx.relinearize(c3, rk)
+        got[mode] = relinearize_int(c3, L) if mode == KS_INT else ctx.relinearize(c3, rk)
         assert_words(got[mode], want, f"relinearize, k = {k}, key-switching mode {mode}, vs the closed form")
+    if k == 33:
+        Ll = k - 3
+        ctx.set_limit(S.Context.LIMIT_KS_ALGORITHM, KS_INT)
+        assert_words(relinearize_int(np.ascontiguousarray(c3[:, :, :Ll]), Ll), closed_form(Ll),
+                     f"relinearize at L = {Ll} (key rows strided by k = {k}) vs the closed form")
     if k <= 64:
         oc = O.Oracle(O.CKKS, n, mods)
         for b in (0, St - 1):
