@@ -421,6 +421,9 @@ int sb200_encrypt_asymmetric(sb200_context *ctx, sb200_public_key *key, size_t L
  * pairs when is_complex, else [batch][count] reals; count <= n/2, missing slots are zero.  plain = [batch][L][n] NTT form at the
  * level with L primes (Plaintext::data() of each plaintext; its parms_id is sb200_get_parms_id(L), its scale the scale given).
  * Bit-exact with the reference: the double-precision transform performs the reference's operations in the reference's order.
+ * Decode can produce non-finite slots (a plaintext whose coefficients exceed the double range after scaling, e.g. one that does not
+ * decrypt to a small value): each slot has the reference's class (finite, +inf, -inf or NaN), and every slot the reference does
+ * not make NaN has its bits.  A NaN's sign and payload are not specified (IEEE 754 leaves them to the implementation).
  * Errors as the reference throws them (SB200_E_INVALID_ARG): "scale out of bounds", "values must be finite", "encoded values are
  * too large" (the plaintext buffer is left unspecified), "unsupported scheme" for a non-CKKS context.
  * decode writes [batch][n/2] complex numbers as (re, im) pairs; `scale` is Plaintext::scale().  The encode entry points

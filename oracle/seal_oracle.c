@@ -1268,9 +1268,51 @@ typedef struct
 {
     double re, im;
 } cplx;
-static cplx c_mul(cplx a, cplx b)
+/* std::complex<double> * std::complex<double> as C99 Annex G (G.5.1) specifies it and g++ compiles it: (ac - bd, ad + bc), and
+ * when both parts come out NaN the infinities are recovered (an infinite factor is "boxed" to +-1 / +-0 with the other factor's
+ * NaNs made 0, or, when only a partial product overflowed, every NaN is made 0) and the product recomputed times infinity.  This
+ * only changes non-finite results: a decoded slot the naive formula would make NaN can be +-inf. */
+static cplx c_mul(cplx z, cplx w)
 {
-    cplx r = { a.re * b.re - a.im * b.im, a.re * b.im + a.im * b.re };
+    double a = z.re, b = z.im, c = w.re, d = w.im;
+    const double ac = a * c, bd = b * d, ad = a * d, bc = b * c;
+    cplx r = { ac - bd, ad + bc };
+    if (isnan(r.re) && isnan(r.im))
+    {
+        int recalc = 0;
+        if (isinf(a) || isinf(b))
+        {
+            a = copysign(isinf(a) ? 1.0 : 0.0, a), b = copysign(isinf(b) ? 1.0 : 0.0, b);
+            if (isnan(c))
+                c = copysign(0.0, c);
+            if (isnan(d))
+                d = copysign(0.0, d);
+            recalc = 1;
+        }
+        if (isinf(c) || isinf(d))
+        {
+            c = copysign(isinf(c) ? 1.0 : 0.0, c), d = copysign(isinf(d) ? 1.0 : 0.0, d);
+            if (isnan(a))
+                a = copysign(0.0, a);
+            if (isnan(b))
+                b = copysign(0.0, b);
+            recalc = 1;
+        }
+        if (!recalc && (isinf(ac) || isinf(bd) || isinf(ad) || isinf(bc)))
+        {
+            if (isnan(a))
+                a = copysign(0.0, a);
+            if (isnan(b))
+                b = copysign(0.0, b);
+            if (isnan(c))
+                c = copysign(0.0, c);
+            if (isnan(d))
+                d = copysign(0.0, d);
+            recalc = 1;
+        }
+        if (recalc)
+            r.re = INFINITY * (a * c - b * d), r.im = INFINITY * (a * d + b * c);
+    }
     return r;
 }
 /* util/croots.cpp:16-70: one eighth of the m-th roots from polar(), the rest through the 8-fold symmetry */

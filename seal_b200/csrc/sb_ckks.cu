@@ -5,7 +5,7 @@
 // values, rounds every coefficient to an integer and reduces it modulo each prime, so a plaintext is only reproducible bit for
 // bit if every floating-point operation is the reference's, in the reference's order.  Each butterfly below is therefore written
 // with the round-to-nearest intrinsics (__dadd_rn / __dsub_rn / __dmul_rn: never contracted into FMA), a complex product is
-// (ac - bd, ad + bc) exactly as std::complex multiplies, the scaling by scale / n is merged into the last stage as
+// (ac - bd, ad + bc) exactly as std::complex multiplies (with its Annex G recovery of infinities when both parts are NaN), the scaling by scale / n is merged into the last stage as
 // DWTHandler::transform_from_rev does, and the root tables come from the host (sbh::ckks_tables: std::polar on one eighth of the
 // circle + symmetry, util/croots.cpp).  The butterflies of one stage are independent, so the parallel schedule does not change
 // any value.  After the transform the three decomposition branches of the reference (coefficients below 2^64, below 2^128,
@@ -32,9 +32,42 @@ namespace sb
         {
             return make_double2(__dsub_rn(a.x, b.x), __dsub_rn(a.y, b.y));
         }
-        __device__ __forceinline__ double2 cmul(double2 a, double2 r) // std::complex product: (ac - bd, ad + bc)
+        // C99 Annex G (G.5.1) recovery of a complex product whose parts both came out NaN, as std::complex<double> multiplies under
+        // g++: an infinite factor is boxed to +-1 / +-0 with the other factor's NaNs made 0 (or, when only a partial product overflowed,
+        // every NaN is made 0), then the product is recomputed times infinity.  Reached only by non-finite operands.
+        __device__ __noinline__ double2 cmul_recover(double2 p, double a, double b, double c, double d, bool overflowed)
         {
-            return make_double2(__dsub_rn(__dmul_rn(a.x, r.x), __dmul_rn(a.y, r.y)), __dadd_rn(__dmul_rn(a.x, r.y), __dmul_rn(a.y, r.x)));
+            bool recalc = false;
+            if (isinf(a) || isinf(b))
+            {
+                a = copysign(isinf(a) ? 1.0 : 0.0, a), b = copysign(isinf(b) ? 1.0 : 0.0, b);
+                c = isnan(c) ? copysign(0.0, c) : c, d = isnan(d) ? copysign(0.0, d) : d;
+                recalc = true;
+            }
+            if (isinf(c) || isinf(d))
+            {
+                c = copysign(isinf(c) ? 1.0 : 0.0, c), d = copysign(isinf(d) ? 1.0 : 0.0, d);
+                a = isnan(a) ? copysign(0.0, a) : a, b = isnan(b) ? copysign(0.0, b) : b;
+                recalc = true;
+            }
+            if (!recalc && overflowed)
+            {
+                a = isnan(a) ? copysign(0.0, a) : a, b = isnan(b) ? copysign(0.0, b) : b;
+                c = isnan(c) ? copysign(0.0, c) : c, d = isnan(d) ? copysign(0.0, d) : d;
+                recalc = true;
+            }
+            if (!recalc)
+                return p;
+            const double inf = __longlong_as_double(0x7ff0000000000000ll);
+            return make_double2(__dmul_rn(inf, __dsub_rn(__dmul_rn(a, c), __dmul_rn(b, d))), __dmul_rn(inf, __dadd_rn(__dmul_rn(a, d), __dmul_rn(b, c))));
+        }
+        __device__ __forceinline__ double2 cmul(double2 a, double2 r) // std::complex product: (ac - bd, ad + bc), Annex G on NaN
+        {
+            const double ac = __dmul_rn(a.x, r.x), bd = __dmul_rn(a.y, r.y), ad = __dmul_rn(a.x, r.y), bc = __dmul_rn(a.y, r.x);
+            const double2 p = make_double2(__dsub_rn(ac, bd), __dadd_rn(ad, bc));
+            if (isnan(p.x) && isnan(p.y))
+                return cmul_recover(p, a.x, a.y, r.x, r.y, isinf(ac) || isinf(bd) || isinf(ad) || isinf(bc));
+            return p;
         }
         __device__ __forceinline__ double2 cscale(double2 a, double s)
         {

@@ -117,6 +117,53 @@ def alternating_extreme_ct(moduli, n, size, L, batch=None):
     return out
 
 
+# ---- big integers behind RNS rows and decoded slots (tests/test_gpu_depth.py, tests/test_depth_oracle.py) ----
+
+def residue_rows(values, moduli, L):
+    """[L][n] residues of the signed Python ints `values` modulo the first L primes"""
+    v = np.array([int(x) for x in values], dtype=object)
+    return np.stack([(v % int(moduli[i])).astype(np.uint64) for i in range(L)])
+
+
+def crt_values(rows, moduli):
+    """the CRT composition in [0, Q) of every column of the coefficient-form rows [L][n], as Python ints"""
+    L = rows.shape[0]
+    Q = product(moduli[:L])
+    acc = np.zeros(rows.shape[1], dtype=object)
+    for i in range(L):
+        q = int(moduli[i])
+        m = Q // q
+        acc = acc + rows[i].astype(object) * (m * pow(m % q, -1, q))
+    return [int(x) % Q for x in acc]
+
+
+def centred(values, Q):
+    """representatives in (-Q/2, Q/2]"""
+    return [v - Q if v > Q // 2 else v for v in values]
+
+
+def ternary_secret_key(rng, moduli, n, ntt_rows):
+    """a secret key with coefficients in {-1, 0, 1}, in NTT form at the key level ([k][n]); ntt_rows maps [k][n] coefficient rows to
+    NTT form"""
+    s = rng.integers(-1, 2, n)
+    return ntt_rows(np.stack([np.where(s < 0, int(q) - 1, s).astype(np.uint64) for q in moduli]))
+
+
+def assert_slots(got, want, what):
+    """decoded complex slots: every double the reference (want) does not make NaN is bit-identical, and exactly its NaNs are NaN
+    (IEEE 754 fixes when an operation gives NaN but not the NaN's sign or payload)"""
+    g = np.ascontiguousarray(got, dtype=np.complex128).view(np.float64)
+    w = np.ascontiguousarray(want, dtype=np.complex128).view(np.float64)
+    assert g.shape == w.shape, (what, g.shape, w.shape)
+    nan = np.isnan(w)
+    bad = np.argwhere(np.isnan(g) != nan)
+    assert len(bad) == 0, f"{what}: {len(bad)} doubles differ in NaN-ness, first at index {tuple(int(v) for v in bad[0])}: " \
+                          f"got {g[tuple(bad[0])]}, want {w[tuple(bad[0])]}"
+    gw, ww = g.view(np.uint64).copy(), w.view(np.uint64).copy()
+    gw[nan] = ww[nan] = 0
+    assert_words(gw, ww, what)
+
+
 # ---- primes (numth.cpp:278-311) ----
 
 def is_prime(m):
