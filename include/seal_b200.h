@@ -435,6 +435,30 @@ int sb200_ckks_encode_host(sb200_context *ctx, size_t L, size_t batch, const dou
                            uint64_t *h_plain);
 int sb200_ckks_decode_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *h_plain, double scale, double *h_values);
 
+/* CKKSEncoder::encode of one scalar per plaintext (ckks.h:272-377) for a batch: values = [batch] doubles (SB200_CKKS_SCALAR_REAL,
+ * encode(double value, parms_id, scale, plain), ckks.cpp:75-230), [batch] (re, im) pairs of doubles (SB200_CKKS_SCALAR_COMPLEX,
+ * encode(std::complex<double>, ...), ckks.h:794-800: the vector encode of n/2 copies) or [batch] int64_t (SB200_CKKS_SCALAR_INT64,
+ * encode(std::int64_t value, parms_id, plain), ckks.cpp:232-287; scale is ignored, the plaintext's scale is 1.0).  plain =
+ * [batch][L][n] NTT form at the level with L primes, word for word the reference's.  Real and int64 plaintexts are constant
+ * polynomials, written on the device by one fill kernel; a negative int64 v is reduced as the reference reduces it,
+ * (uint64_t)v + q_j, which is (2^64 - |v|) mod q_j and not -|v| mod q_j when |v| > q_j.
+ * Errors (SB200_E_INVALID_ARG), checked before any launch that writes plain, on the first failing plaintext in batch order:
+ * a kind outside 0..2; "unsupported scheme" for a non-CKKS context; "parms_id is not valid for encryption parameters" for L outside
+ * 1..k; batch 0.  Real: "scale out of bounds" (!isfinite(scale), scale <= 0 or (int)log2(scale) >= the level's total bit count:
+ * unlike the vector encode, a subnormal scale and (int)log2(scale) = total bits - 1 are accepted), "value must be finite",
+ * "encoded value is too large" (value * scale not finite, or its bit count + 1 at or above the total bit count).  Int64: "encoded
+ * value is too large" (significant bits of |v| + 2 at or above the total bit count, |INT64_MIN| taken as 2^63).  Complex: the
+ * vector encode's checks and messages ("scale out of bounds", "values must be finite", "encoded values are too large").  NULL
+ * values or plain: SB200_E_POINTER.  Real and int64 copy the values to the host and synchronise the stream once; complex
+ * synchronises it as sb200_ckks_encode does. */
+#define SB200_CKKS_SCALAR_REAL 0
+#define SB200_CKKS_SCALAR_COMPLEX 1
+#define SB200_CKKS_SCALAR_INT64 2
+int sb200_ckks_encode_scalar(sb200_context *ctx, size_t L, size_t batch, int kind, const void *d_values, double scale, uint64_t *d_plain,
+                             void *stream);
+int sb200_ckks_encode_scalar_host(sb200_context *ctx, size_t L, size_t batch, int kind, const void *h_values, double scale,
+                                  uint64_t *h_plain);
+
 /* ---- decryption (SURVEY 8f rank 4): Decryptor(context, secret_key) and Decryptor::decrypt (decryptor.cpp:62-197) ------
  * h_secret_key = SecretKey::data().data(): [k][n] words, NTT form at the key level.  Powers of the key for ciphertexts
  * of size > 2 are built on the device on first use (compute_secret_key_array, :199-310). */

@@ -6,7 +6,10 @@
 //
 // The embedding transform (double-precision complex FFT), the rounding and the residue decomposition run on the device
 // (sb200_ckks_encode / sb200_ckks_decode) and reproduce the reference's plaintexts and decoded values bit for bit; the checks and
-// exception types are the reference's (ckks.h:455-807).  The batch members are the extension the reference does not have.
+// exception types are the reference's (ckks.h:455-807).  The scalar overloads (ckks.h:272-377: one double, complex number or int64
+// in every slot) have the reference's declarations and make the same plaintexts (sb200_ckks_encode_scalar_host).  The batch
+// members are the extension the reference does not have, among them the scalar ones on PlaintextBatch (encode of one value,
+// encode_scalars of one value per plaintext).
 #pragma once
 
 #include "../seal_b200.h"
@@ -49,6 +52,47 @@ namespace seal_b200
         {
             encode_internal(values.data(), values.size(), context_.first_parms_id(), scale, destination);
         }
+        // ---- one scalar in every slot (ckks.h:272-377): the reference's six declarations, so that calls written for seal::CKKSEncoder
+        // select the same overload (encode(i + 1, plain) with a size_t takes the int64 one).  The pool is checked, as the reference
+        // checks it, and not otherwise used: the plaintext is made on the device (sb200_ckks_encode_scalar_host)
+        void encode(double value, seal::parms_id_type parms_id, double scale, seal::Plaintext &destination,
+                    seal::MemoryPoolHandle pool = seal::MemoryManager::GetPool()) const
+        {
+            auto cd = context_.get_context_data(parms_id);
+            if (!cd)
+                throw std::invalid_argument("parms_id is not valid for encryption parameters"); // ckks.cpp:79-88
+            if (!pool)
+                throw std::invalid_argument("pool is uninitialized");
+            encode_scalar_internal(&value, SB200_CKKS_SCALAR_REAL, cd->parms().coeff_modulus().size(), parms_id, scale, destination);
+        }
+        void encode(double value, double scale, seal::Plaintext &destination, seal::MemoryPoolHandle pool = seal::MemoryManager::GetPool()) const
+        {
+            encode(value, context_.first_parms_id(), scale, destination, std::move(pool));
+        }
+        void encode(std::complex<double> value, seal::parms_id_type parms_id, double scale, seal::Plaintext &destination,
+                    seal::MemoryPoolHandle pool = seal::MemoryManager::GetPool()) const
+        {
+            auto cd = context_.get_context_data(parms_id);
+            if (!cd)
+                throw std::invalid_argument("parms_id is not valid for encryption parameters"); // ckks.h:462-466
+            if (!pool)
+                throw std::invalid_argument("pool is uninitialized");
+            encode_scalar_internal(&value, SB200_CKKS_SCALAR_COMPLEX, cd->parms().coeff_modulus().size(), parms_id, scale, destination);
+        }
+        void encode(std::complex<double> value, double scale, seal::Plaintext &destination,
+                    seal::MemoryPoolHandle pool = seal::MemoryManager::GetPool()) const
+        {
+            encode(value, context_.first_parms_id(), scale, destination, std::move(pool));
+        }
+        void encode(std::int64_t value, seal::parms_id_type parms_id, seal::Plaintext &destination) const
+        {
+            auto cd = context_.get_context_data(parms_id);
+            if (!cd)
+                throw std::invalid_argument("parms_id is not valid for encryption parameters"); // ckks.cpp:235-239
+            encode_scalar_internal(&value, SB200_CKKS_SCALAR_INT64, cd->parms().coeff_modulus().size(), parms_id, 1.0, destination);
+        }
+        void encode(std::int64_t value, seal::Plaintext &destination) const { encode(value, context_.first_parms_id(), destination); }
+
         // ckks.h:365-372
         template <typename T, typename = std::enable_if_t<std::is_same<std::remove_cv_t<T>, double>::value ||
                                                           std::is_same<std::remove_cv_t<T>, std::complex<double>>::value>>
@@ -135,6 +179,35 @@ namespace seal_b200
             destination.parms_id_ = parms_id, destination.ntt_ = true, destination.scale_ = scale;
         }
 
+        // ---- device-resident scalar plaintexts (sb200_ckks_encode_scalar): encode(value, ..., PlaintextBatch &) makes a batch of one
+        // plaintext, which every PlaintextBatch consumer applies to a whole CiphertextBatch; encode_scalars makes one plaintext per
+        // value (a distinct name: encode(std::vector<double>, ...) means one slot vector).  Checks and messages as the Plaintext overloads.
+        void encode(double value, seal::parms_id_type parms_id, double scale, PlaintextBatch &destination) const
+        {
+            encode_scalars_internal(&value, 1, SB200_CKKS_SCALAR_REAL, parms_id, scale, destination);
+        }
+        void encode(std::complex<double> value, seal::parms_id_type parms_id, double scale, PlaintextBatch &destination) const
+        {
+            encode_scalars_internal(&value, 1, SB200_CKKS_SCALAR_COMPLEX, parms_id, scale, destination);
+        }
+        void encode(std::int64_t value, seal::parms_id_type parms_id, PlaintextBatch &destination) const
+        {
+            encode_scalars_internal(&value, 1, SB200_CKKS_SCALAR_INT64, parms_id, 1.0, destination);
+        }
+        void encode_scalars(const std::vector<double> &values, seal::parms_id_type parms_id, double scale, PlaintextBatch &destination) const
+        {
+            encode_scalars_internal(values.data(), values.size(), SB200_CKKS_SCALAR_REAL, parms_id, scale, destination);
+        }
+        void encode_scalars(const std::vector<std::complex<double>> &values, seal::parms_id_type parms_id, double scale,
+                            PlaintextBatch &destination) const
+        {
+            encode_scalars_internal(values.data(), values.size(), SB200_CKKS_SCALAR_COMPLEX, parms_id, scale, destination);
+        }
+        void encode_scalars(const std::vector<std::int64_t> &values, seal::parms_id_type parms_id, PlaintextBatch &destination) const
+        {
+            encode_scalars_internal(values.data(), values.size(), SB200_CKKS_SCALAR_INT64, parms_id, 1.0, destination);
+        }
+
         // ---- device-resident plaintexts: a PlaintextBatch in NTT form -> B vectors of slot_count() values, decoded on the device
         // (sb200_ckks_decode) with the batch's scale; only the values cross PCIe.  The batch must come from this encoder's context.
         template <typename T, typename = std::enable_if_t<std::is_same<std::remove_cv_t<T>, double>::value ||
@@ -166,6 +239,42 @@ namespace seal_b200
         }
 
     private:
+        // one scalar (kind SB200_CKKS_SCALAR_*) -> destination, which changes only on success
+        void encode_scalar_internal(const void *value, int kind, std::size_t L, seal::parms_id_type parms_id, double scale,
+                                    seal::Plaintext &destination) const
+        {
+            const std::size_t n = slots_ * 2;
+            std::vector<std::uint64_t> words(L * n);
+            status(sb200_ckks_encode_scalar_host(ctx_, L, 1, kind, value, scale, words.data()));
+            destination.parms_id() = seal::parms_id_zero; // ckks.cpp:129-132
+            destination.resize(L * n);
+            std::copy(words.begin(), words.end(), destination.data());
+            destination.parms_id() = parms_id;
+            destination.scale() = scale;
+        }
+        // B scalars (host) -> a PlaintextBatch [B][L][n] made on the device
+        void encode_scalars_internal(const void *values, std::size_t B, int kind, seal::parms_id_type parms_id, double scale,
+                                     PlaintextBatch &destination) const
+        {
+            auto cd = context_.get_context_data(parms_id);
+            if (!cd)
+                throw std::invalid_argument("parms_id is not valid for encryption parameters");
+            if (!B)
+                throw std::invalid_argument("batch cannot be empty");
+            const std::size_t L = cd->parms().coeff_modulus().size(), n = slots_ * 2;
+            const std::size_t bytes = B * (kind == SB200_CKKS_SCALAR_COMPLEX ? 16 : 8);
+            std::uint64_t *d_values = nullptr;
+            status(sb200_device_malloc(ctx_, bytes, &d_values));
+            int rc = sb200_memcpy_h2d(ctx_, d_values, values, bytes, nullptr);
+            if (rc == SB200_OK)
+                rc = destination.reserve(ctx_, B * L * n);
+            if (rc == SB200_OK)
+                rc = sb200_ckks_encode_scalar(ctx_, L, B, kind, d_values, scale, destination.d_, nullptr);
+            sb200_device_free(ctx_, d_values);
+            status(rc);
+            destination.batch_ = B, destination.L_ = L, destination.n_ = n;
+            destination.parms_id_ = parms_id, destination.ntt_ = true, destination.scale_ = scale;
+        }
         template <typename T>
         void encode_internal(const T *values, std::size_t values_size, seal::parms_id_type parms_id, double scale, seal::Plaintext &destination) const
         {

@@ -40,6 +40,7 @@ SYMBOLS = [
     "sb200_ciphertext_save_size", "sb200_ciphertext_load", "sb200_ciphertext_save", "sb200_secret_key_create",
     "sb200_secret_key_destroy", "sb200_decrypt", "sb200_decrypt_host", "sb200_invariant_noise_budget", "sb200_invariant_noise_budget_host", "sb200_encrypt_zero_symmetric", "sb200_public_key_create", "sb200_public_key_destroy", "sb200_encrypt_zero_asymmetric", "sb200_encrypt_zero_symmetric_prng", "sb200_encrypt_zero_asymmetric_prng", "sb200_encrypt_symmetric", "sb200_encrypt_asymmetric", "sb200_kswitch_key_generate", "sb200_public_key_generate", "sb200_ciphertext_save_seeded_size", "sb200_ciphertext_save_seeded",
     "sb200_public_key_generate_seeded", "sb200_kswitch_keys_save_seeded_size", "sb200_kswitch_keys_generate_seeded", "sb200_ckks_encode", "sb200_ckks_decode", "sb200_ckks_encode_host", "sb200_ckks_decode_host",
+    "sb200_ckks_encode_scalar", "sb200_ckks_encode_scalar_host",
     "sb200_group_create", "sb200_group_destroy", "sb200_group_size", "sb200_group_context", "sb200_group_slice",
     "sb200_group_kswitch_key_create", "sb200_group_kswitch_key_destroy", "sb200_group_multiply_relinearize_host",
     "sb200_group_relinearize_host", "sb200_group_apply_galois_host", "sb200_group_multiply_host", "sb200_group_rescale_to_next_host",
@@ -166,6 +167,8 @@ def lib():
         L.sb200_ckks_decode.argtypes = [vp, sz, sz, vp, C.c_double, vp, vp]
         L.sb200_ckks_encode_host.argtypes = [vp, sz, sz, vp, sz, i32, C.c_double, _u64p]
         L.sb200_ckks_decode_host.argtypes = [vp, sz, sz, _u64p, C.c_double, vp]
+        L.sb200_ckks_encode_scalar.argtypes = [vp, sz, sz, i32, vp, C.c_double, vp, vp]
+        L.sb200_ckks_encode_scalar_host.argtypes = [vp, sz, sz, i32, vp, C.c_double, _u64p]
         L.sb200_public_key_create.argtypes = [vp, _u64p, C.POINTER(vp)]
         L.sb200_public_key_destroy.argtypes = [vp]
         L.sb200_encrypt_zero_asymmetric.argtypes = [vp, vp, sz, sz, _u64p, vp, vp]
@@ -587,6 +590,30 @@ class Context:
 
     def d_ckks_encode(self, values, plain, L, batch, count, is_complex, scale):
         _check(lib().sb200_ckks_encode(self.h, L, batch, _dp(values), count, int(is_complex), float(scale), _dp(plain), self._stream()))
+
+    CKKS_SCALAR_REAL, CKKS_SCALAR_COMPLEX, CKKS_SCALAR_INT64 = 0, 1, 2
+
+    def ckks_encode_scalar(self, values, L, scale=1.0):
+        """CKKSEncoder.encode of one scalar per plaintext: values [B] (or a scalar) float64 / complex128 / int64, the kind taken from
+        the dtype (scale is ignored for int64) -> plaintexts [B][L][n] (or [L][n]), NTT form"""
+        v = np.asarray(values)
+        if v.dtype == np.float64:
+            kind = self.CKKS_SCALAR_REAL
+        elif v.dtype == np.complex128:
+            kind = self.CKKS_SCALAR_COMPLEX
+        elif v.dtype == np.int64:
+            kind = self.CKKS_SCALAR_INT64
+        else:
+            raise TypeError(f"ckks_encode_scalar takes float64, complex128 or int64 values, not {v.dtype}")
+        single = v.ndim == 0
+        v = np.ascontiguousarray(v.reshape(-1))
+        B = v.shape[0]
+        out = np.zeros((B, L, self.n), dtype=np.uint64)
+        _check(lib().sb200_ckks_encode_scalar_host(self.h, L, B, kind, v.ctypes.data, float(scale), _hp(out)))
+        return out[0] if single else out
+
+    def d_ckks_encode_scalar(self, values, plain, L, batch, kind, scale):
+        _check(lib().sb200_ckks_encode_scalar(self.h, L, batch, int(kind), _dp(values), float(scale), _dp(plain), self._stream()))
 
     def d_ckks_decode(self, plain, values, L, batch, scale):
         _check(lib().sb200_ckks_decode(self.h, L, batch, _dp(plain), float(scale), _dp(values), self._stream()))

@@ -1336,6 +1336,28 @@ namespace
         }
     };
 
+    // a: one scalar per plaintext, one word (real, int64) or two (complex).  h_values: the host entry point's values, checked in full
+    // before the first chunk is staged, so that an error leaves h_plain untouched; the stream entry point checks inside the op
+    struct CkksEncodeScalar
+    {
+        size_t L;
+        int kind;
+        double scale;
+        const u64 *h_values;
+        void check(const Context &c, size_t batch) const
+        {
+            check_ckks_scalar(c, L, kind, scale);
+            check_batch(batch);
+            if (h_values)
+                check_ckks_scalar_values(c, L, batch, kind, h_values, scale);
+        }
+        Layout layout(const Context &c) const { return { kind == kCkksScalarComplex ? size_t(2) : size_t(1), 0, L * c.n }; }
+        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
+        {
+            op_ckks_encode_scalar(c, L, B, kind, a, scale, out, st);
+        }
+    };
+
     struct CkksDecode // out: n / 2 complex values (n doubles) per plaintext
     {
         size_t L;
@@ -1964,6 +1986,17 @@ int sb200_ckks_encode_host(sb200_context *ctx, size_t L, size_t batch, const dou
                            uint64_t *h_plain)
 {
     return on_host(ctx, batch, h_values, nullptr, h_plain, CkksEncode{ L, count, is_complex != 0, h_values != nullptr, scale });
+}
+
+int sb200_ckks_encode_scalar(sb200_context *ctx, size_t L, size_t batch, int kind, const void *d_values, double scale, uint64_t *d_plain,
+                             void *stream)
+{
+    return on_stream(ctx, stream, batch, d_values, nullptr, d_plain, CkksEncodeScalar{ L, kind, scale, nullptr });
+}
+int sb200_ckks_encode_scalar_host(sb200_context *ctx, size_t L, size_t batch, int kind, const void *h_values, double scale,
+                                  uint64_t *h_plain)
+{
+    return on_host(ctx, batch, h_values, nullptr, h_plain, CkksEncodeScalar{ L, kind, scale, static_cast<const u64 *>(h_values) });
 }
 
 int sb200_ckks_decode(sb200_context *ctx, size_t L, size_t batch, const uint64_t *d_plain, double scale, double *d_values, void *stream)

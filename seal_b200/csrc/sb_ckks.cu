@@ -74,21 +74,22 @@ namespace sb
             return make_double2(__dmul_rn(a.x, s), __dmul_rn(a.y, s));
         }
 
-        // values [B][count] (complex: (re, im) pairs; real: one double) -> V[b][map[i]] = v, V[b][map[i + slots]] = conj(v)
-        __global__ void __launch_bounds__(256) ckks_scatter_kernel(const double *__restrict__ values, int is_complex, long long count,
+        // values [B][count] (complex: (re, im) pairs; real: one double) -> V[b][map[i]] = v, V[b][map[i + slots]] = conj(v).
+        // broadcast: values [B], member b's one value in every slot (CKKSEncoder::encode of one complex number, ckks.h:794-800)
+        __global__ void __launch_bounds__(256) ckks_scatter_kernel(const double *__restrict__ values, int is_complex, int broadcast, long long count,
                                                                    const uint32_t *__restrict__ map, double2 *__restrict__ V, int logn,
                                                                    long long total, int *flags)
         {
             const long long e = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
             if (e >= total)
                 return;
-            const long long b = e / count, i = e % count;
+            const long long b = e / count, i = e % count, src = broadcast ? b : e;
             const long long n = 1ll << logn, slots = n >> 1;
             double re, im = 0.0;
             if (is_complex)
-                re = values[2 * e], im = values[2 * e + 1];
+                re = values[2 * src], im = values[2 * src + 1];
             else
-                re = values[e];
+                re = values[src];
             if (!isfinite(re) || !isfinite(im))
                 atomicOr(flags, 1); // "values must be finite"
             V[b * n + map[i]] = make_double2(re, im);
@@ -183,7 +184,43 @@ namespace sb
                 atomicMax(max_bits, bits);
         }
 
-        // round(Re c) -> residues modulo every prime of the level (ckks.h:556-668): |round(c)| = mant * 2^ex exactly
+        // round(c) of a finite double as sign and magnitude, |round(c)| = mant * 2^ex exactly.  The reference's three decomposition
+        // branches (below 2^64, below 2^128, multi-precision: ckks.h:556-668 for vectors, ckks.cpp:152-226 for one real) all reduce
+        // this same integer, so every encoder reduces it through ckks_decompose + ckks_residue
+        struct CkksCoeff
+        {
+            u64 mant;
+            int ex;
+            bool negative;
+        };
+        __device__ __forceinline__ CkksCoeff ckks_decompose(double c)
+        {
+            double d = round(c); // half away from zero, like std::round
+            CkksCoeff k{ 0, 0, static_cast<bool>(signbit(d)) };
+            d = fabs(d);
+            if (d >= 1.0)
+            {
+                if (d < 18446744073709551616.0)
+                    k.mant = __double2ull_rz(d);
+                else
+                {
+                    const long long bits = __double_as_longlong(d);
+                    k.ex = static_cast<int>((bits >> 52) & 0x7ff) - 1075; // d = (2^52 + fraction) * 2^ex, ex >= 12 here
+                    k.mant = (static_cast<u64>(bits) & 0xFFFFFFFFFFFFFull) | (1ull << 52);
+                }
+            }
+            return k;
+        }
+        // round(c) mod q, canonical; a negative value is negated modulo q with 0 kept as 0 (negate_uint_mod)
+        __device__ __forceinline__ u64 ckks_residue(const CkksCoeff &k, const PrimeDev &P)
+        {
+            u64 r = barrett64(k.mant, P.q, P.ratio_hi);
+            for (int left = k.ex; left > 0; left -= 32) // times 2^ex, 32 bits at a time (large coefficients only)
+                r = mulmod_barrett(r, 1ull << (left >= 32 ? 32 : left), P);
+            return k.negative && r ? P.q - r : r;
+        }
+
+        // round(Re c) -> residues modulo every prime of the level (ckks.h:556-668)
         __global__ void __launch_bounds__(256) ckks_reduce_kernel(const double2 *__restrict__ V, u64 *__restrict__ out, const PrimeDev *__restrict__ primes,
                                                                   int logn, int L, long long total)
         {
@@ -191,30 +228,51 @@ namespace sb
             if (e >= total)
                 return;
             const long long n = 1ll << logn, b = e >> logn, i = e & (n - 1);
-            double d = round(V[e].x); // half away from zero, like std::round
-            const bool negative = signbit(d);
-            d = fabs(d);
-            u64 mant = 0;
-            int ex = 0;
-            if (d >= 1.0)
-            {
-                if (d < 18446744073709551616.0)
-                    mant = __double2ull_rz(d);
-                else
-                {
-                    const long long bits = __double_as_longlong(d);
-                    ex = static_cast<int>((bits >> 52) & 0x7ff) - 1075; // d = (2^52 + fraction) * 2^ex, ex >= 12 here
-                    mant = (static_cast<u64>(bits) & 0xFFFFFFFFFFFFFull) | (1ull << 52);
-                }
-            }
+            const CkksCoeff k = ckks_decompose(V[e].x);
             u64 *dst = out + b * L * n + i;
             for (int j = 0; j < L; j++)
             {
                 const PrimeDev P = primes[j];
-                u64 r = barrett64(mant, P.q, P.ratio_hi);
-                for (int left = ex; left > 0; left -= 32) // times 2^ex, 32 bits at a time (large coefficients only)
-                    r = mulmod_barrett(r, 1ull << (left >= 32 ? 32 : left), P);
-                dst[static_cast<long long>(j) * n] = negative && r ? P.q - r : r;
+                dst[static_cast<long long>(j) * n] = ckks_residue(k, P);
+            }
+        }
+
+        // CKKSEncoder::encode of one real (kind kCkksScalarReal: value * scale, ckks.cpp:75-230) or one int64 (kCkksScalarInt64,
+        // ckks.cpp:232-287) per member: the plaintext is the constant polynomial, so in NTT form every word of row (b, j) of out
+        // [B][L][n] is the same residue.  One CTA per row: thread 0 computes the residue once, then the CTA writes the row with
+        // 16-byte stores (VEC; 8-byte stores when out is not 16-byte aligned).  A pure write stream of B L n 8 bytes.
+        template <bool VEC>
+        __global__ void __launch_bounds__(256) ckks_fill_kernel(const u64 *__restrict__ values, int kind, double scale, const PrimeDev *__restrict__ primes,
+                                                                int logn, int L, u64 *__restrict__ out)
+        {
+            __shared__ u64 word;
+            const long long row = blockIdx.x, n = 1ll << logn;
+            if (threadIdx.x == 0)
+            {
+                const long long b = row / L;
+                const PrimeDev P = primes[row % L];
+                const u64 v = values[b];
+                if (kind == kCkksScalarInt64)
+                    // the reference adds q_j to the two's-complement word of a negative value before its Barrett reduction. For |v| > q_j
+                    // that 64-bit sum does not wrap, so the word is (2^64 - |v|) mod q_j rather than -|v| mod q_j: kept, to be bit-exact
+                    word = barrett64(static_cast<long long>(v) < 0 ? v + P.q : v, P.q, P.ratio_hi);
+                else
+                    word = ckks_residue(ckks_decompose(__dmul_rn(__longlong_as_double(static_cast<long long>(v)), scale)), P);
+            }
+            __syncthreads();
+            const u64 w = word;
+            if (VEC)
+            {
+                ulonglong2 *dst = reinterpret_cast<ulonglong2 *>(out + row * n);
+                const ulonglong2 w2 = make_ulonglong2(w, w);
+                for (long long i = threadIdx.x; i < n / 2; i += blockDim.x)
+                    dst[i] = w2;
+            }
+            else
+            {
+                u64 *dst = out + row * n;
+                for (long long i = threadIdx.x; i < n; i += blockDim.x)
+                    dst[i] = w;
             }
         }
 
@@ -342,7 +400,7 @@ namespace sb
     // values: device, [B][count] complex (re, im) pairs or reals; plain: device, [B][L][n] NTT form.  Synchronises the stream once
     // (the reference's "encoded values are too large" check needs the largest coefficient before the plaintext is produced).
     void op_ckks_encode(Context &c, size_t L, size_t B, const double *values, size_t count, bool is_complex, double scale, u64 *plain,
-                        cudaStream_t st)
+                        cudaStream_t st, bool broadcast)
     {
         auto &enc = ckks_encoder(c);
         if (L < 1 || L > c.k)
@@ -367,8 +425,8 @@ namespace sb
         {
             const long long total = static_cast<long long>(B) * static_cast<long long>(count);
             c.stats.begin("ckks_scatter", 0, 48.0 * total, st);
-            ckks_scatter_kernel<<<grid_for(total, 256), 256, 0, st>>>(values, is_complex ? 1 : 0, static_cast<long long>(count), enc.d_map.get(), V,
-                                                                      static_cast<int>(logn), total, d_flags);
+            ckks_scatter_kernel<<<grid_for(total, 256), 256, 0, st>>>(values, is_complex ? 1 : 0, broadcast ? 1 : 0, static_cast<long long>(count),
+                                                                      enc.d_map.get(), V, static_cast<int>(logn), total, d_flags);
             c.stats.end(st);
             cuda_check(cudaGetLastError(), "ckks_scatter_kernel");
         }
@@ -417,6 +475,73 @@ namespace sb
         c.stats.end(st);
         cuda_check(cudaGetLastError(), "ckks_reduce_kernel");
         op_ntt(c, false, L, 1, B, plain, st);
+    }
+
+    void check_ckks_scalar(const Context &c, size_t L, int kind, double scale)
+    {
+        if (kind != kCkksScalarReal && kind != kCkksScalarComplex && kind != kCkksScalarInt64)
+            throw std::invalid_argument("kind must be SB200_CKKS_SCALAR_REAL, SB200_CKKS_SCALAR_COMPLEX or SB200_CKKS_SCALAR_INT64");
+        if (c.scheme != 2)
+            throw std::invalid_argument("unsupported scheme"); // ckks.cpp:22-25
+        if (L < 1 || L > c.k)
+            throw std::invalid_argument("parms_id is not valid for encryption parameters");
+        const int total_bits = sbh::product_bit_count(c.q.data(), L);
+        // one real: ckks.cpp:96-101 (isfinite, no +1); one complex: the vector path's test, ckks.h:494-499
+        if (kind == kCkksScalarReal && (!std::isfinite(scale) || scale <= 0 || static_cast<int>(std::log2(scale)) >= total_bits))
+            throw std::invalid_argument("scale out of bounds");
+        if (kind == kCkksScalarComplex && (!std::isnormal(scale) || scale <= 0 || static_cast<int>(std::log2(scale)) + 1 >= total_bits))
+            throw std::invalid_argument("scale out of bounds");
+    }
+
+    void check_ckks_scalar_values(const Context &c, size_t L, size_t B, int kind, const u64 *h_values, double scale)
+    {
+        const int total_bits = sbh::product_bit_count(c.q.data(), L);
+        for (size_t b = 0; b < B; b++)
+        {
+            if (kind == kCkksScalarInt64) // ckks.cpp:253-257; |INT64_MIN| = 2^63, which llabs yields on two's-complement targets
+            {
+                const u64 v = h_values[b], mag = static_cast<int64_t>(v) < 0 ? 0 - v : v;
+                if ((mag ? 64 - __builtin_clzll(mag) : 0) + 2 >= total_bits)
+                    throw std::invalid_argument("encoded value is too large");
+            }
+            else if (kind == kCkksScalarReal) // ckks.cpp:103-124; value * scale is the kernel's product (one IEEE multiply)
+            {
+                double value;
+                std::memcpy(&value, h_values + b, sizeof(double));
+                if (!std::isfinite(value))
+                    throw std::invalid_argument("value must be finite");
+                const double p = value * scale;
+                if (!std::isfinite(p))
+                    throw std::invalid_argument("encoded value is too large");
+                const int coeff_bit_count = std::fabs(p) < 1.0 ? 2 : static_cast<int>(std::log2(std::fabs(p))) + 2;
+                if (coeff_bit_count >= total_bits)
+                    throw std::invalid_argument("encoded value is too large");
+            }
+        }
+    }
+
+    void op_ckks_encode_scalar(Context &c, size_t L, size_t B, int kind, const u64 *values, double scale, u64 *plain, cudaStream_t st)
+    {
+        check_ckks_scalar(c, L, kind, scale);
+        if (!B)
+            return;
+        if (kind == kCkksScalarComplex) // ckks.h:794-800: slots copies through the vector path, read from one pair per member
+        {
+            op_ckks_encode(c, L, B, reinterpret_cast<const double *>(values), c.n / 2, true, scale, plain, st, true);
+            return;
+        }
+        std::vector<u64> h(B);
+        cuda_check(cudaMemcpyAsync(h.data(), values, B * sizeof(u64), cudaMemcpyDeviceToHost, st), "values D2H");
+        cuda_check(cudaStreamSynchronize(st), "synchronize");
+        check_ckks_scalar_values(c, L, B, kind, h.data(), scale);
+        const unsigned rows = static_cast<unsigned>(B * L);
+        c.stats.begin("ckks_fill", 0, 8.0 * B * L * c.n, st);
+        if (reinterpret_cast<uintptr_t>(plain) % sizeof(ulonglong2) == 0)
+            ckks_fill_kernel<true><<<rows, 256, 0, st>>>(values, kind, scale, c.d_primes.get(), c.logn, static_cast<int>(L), plain);
+        else
+            ckks_fill_kernel<false><<<rows, 256, 0, st>>>(values, kind, scale, c.d_primes.get(), c.logn, static_cast<int>(L), plain);
+        c.stats.end(st);
+        cuda_check(cudaGetLastError(), "ckks_fill_kernel");
     }
 
     // plain: device [B][L][n] NTT form, scale = Plaintext::scale(); values out: device [B][n/2] complex (re, im)

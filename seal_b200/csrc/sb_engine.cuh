@@ -273,9 +273,19 @@ namespace sb
     // Encryptor(public key)::encrypt: op_encrypt_zero_asymmetric, then the plaintexts (layout as op_encrypt_symmetric) added to c_0
     void op_encrypt_asymmetric(Context &c, const PublicKey &pk, size_t L, size_t B, const u64 *d_plain, const u64 *h_seeds, int prng, u64 *d_out,
                                cudaStream_t st);
-    // CKKSEncoder::encode / decode (sb_ckks.cu): values = device doubles, [B][count] complex pairs (or reals); plain = [B][L][n] NTT form
+    // CKKSEncoder::encode / decode (sb_ckks.cu): values = device doubles, [B][count] complex pairs (or reals); plain = [B][L][n] NTT form.
+    // broadcast: values holds one value per member, encoded into every one of count slots
     void op_ckks_encode(Context &c, size_t L, size_t B, const double *values, size_t count, bool is_complex, double scale, u64 *plain,
-                        cudaStream_t st);
+                        cudaStream_t st, bool broadcast = false);
+    // CKKSEncoder::encode of one scalar per member (ckks.h:272-377): values = device words [B] (kind real: a double, int64: an int64_t)
+    // or [B][2] (complex: re, im); plain = [B][L][n] NTT form.  Real and int64 synchronise the stream once to check the values on the
+    // host, then one fill kernel writes the constant polynomials; complex is the vector encode of n/2 copies.  scale is ignored for int64.
+    constexpr int kCkksScalarReal = 0, kCkksScalarComplex = 1, kCkksScalarInt64 = 2; // SB200_CKKS_SCALAR_*
+    void op_ckks_encode_scalar(Context &c, size_t L, size_t B, int kind, const u64 *values, double scale, u64 *plain, cudaStream_t st);
+    // the checks of op_ckks_encode_scalar that need no values (kind, scheme, level, scale), and those of B host values (real, int64),
+    // each in the reference's order and with its messages (std::invalid_argument)
+    void check_ckks_scalar(const Context &c, size_t L, int kind, double scale);
+    void check_ckks_scalar_values(const Context &c, size_t L, size_t B, int kind, const u64 *h_values, double scale);
     void op_ckks_decode(Context &c, size_t L, size_t B, const u64 *plain, double scale, double *values, cudaStream_t st);
     const sbh::BehzLevel &behz_host(Context &c, size_t L);
     // wire format support (sb_api.cu): 1 if any residue of data [rows][n] (prime of a row = row % L) is >= its modulus
