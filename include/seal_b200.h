@@ -220,6 +220,29 @@ int sb200_negate(sb200_context *ctx, size_t L, size_t size, size_t batch, const 
 #define SB200_FOLD_SCALED 2
 int sb200_add_many(sb200_context *ctx, size_t L, size_t batch, size_t count, const size_t *sizes, const uint64_t *const *d_operands,
                    const int *modes, const uint64_t *h_factors, uint64_t *d_out, void *stream);
+/* Sums of plaintext products: a plaintext matrix times a vector of ciphertexts in one pass.  Member b of d_outs[j] (j < outputs = M)
+ * has the words of the chain t_i = multiply_plain(member b of d_cts[i], plaintext b (or the shared one) of d_plains[j K + i]) for
+ * i < count = K, then sb200_add_many(t_0 .. t_{K-1}, modes, h_factors) (evaluator.cpp:1975-2195, :155-262), for any input words.
+ *   d_cts[i]: [batch][sizes[i]][L][n], 1 <= sizes[i] <= 16, all in NTT form (ct_is_ntt = 1) or all in coefficient form (0, BFV);
+ *   d_plains[j K + i]: plain_counts[j K + i] plaintexts (1: shared by the batch, or batch), all NTT form [count][L][n] at the
+ *     ciphertexts' level (plain_is_ntt = 1) or all coefficient form [count][n], words < t, zero above coeff_count (0, BFV / BGV);
+ *   modes [K - 1] / h_factors [K - 1][2]: as for sb200_add_many (NULL: every step adds; BGV correction-factor balancing);
+ *   d_outs[j]: [batch][max sizes[i]][L][n], in the ciphertexts' form.
+ * The four NTT-form cases of multiply_plain are covered: coefficient-form plaintexts are lifted and transformed (sb200_plain_to_ntt)
+ * and coefficient-form ciphertexts transformed into scratch, in chunks of terms, and each output gets one inverse transform.
+ * The 128-bit sums are reduced once per window of terms: 256 when every prime of the level is below 2^60, fewer for larger
+ * primes (64 at 61 bits); the fold's factors enter as one constant per term.  Errors, all before the first launch, in the
+ * chain's order (multiply_plain's, then add_many's): count = 0 or outputs = 0, a plain count neither 1 nor batch, a size outside
+ * 1..16, a mode outside 0..3, coefficient-form plaintexts in a CKKS context (SB200_E_INVALID_ARG); a NULL array, operand or
+ * output, or (with a scaled step) h_factors (SB200_E_POINTER); an output slab overlapping an operand's slab or another output's
+ * (SB200_E_INVALID_ARG).  The _host form
+ * stages the batch in chunks of SB200_LIMIT_HOST_STAGE_BYTES and uploads each shared plaintext once per call. */
+int sb200_multiply_plain_sum(sb200_context *ctx, size_t L, size_t batch, size_t count, size_t outputs, const size_t *sizes,
+                             const uint64_t *const *d_cts, const size_t *plain_counts, const uint64_t *const *d_plains, int ct_is_ntt,
+                             int plain_is_ntt, const int *modes, const uint64_t *h_factors, uint64_t *const *d_outs, void *stream);
+int sb200_multiply_plain_sum_host(sb200_context *ctx, size_t L, size_t batch, size_t count, size_t outputs, const size_t *sizes,
+                                  const uint64_t *const *h_cts, const size_t *plain_counts, const uint64_t *const *h_plains, int ct_is_ntt,
+                                  int plain_is_ntt, const int *modes, const uint64_t *h_factors, uint64_t *const *h_outs);
 /* Evaluator::multiply_plain with ciphertext and plaintext both in NTT form (evaluator.cpp:1975-1994 -> multiply_plain_ntt
  * :2157-2195): every polynomial of the ciphertext times the plaintext, dyadic.  d_plain is [batch][L][n]: one NTT-form
  * plaintext per ciphertext, at the ciphertext's level (Plaintext::data() with parms_id == the ciphertext's).  May run in place. */

@@ -1176,6 +1176,44 @@ namespace seal_b200
             check(sb200_add_many(ctx_, e0.L_, e0.batch_, ops.size(), f.sizes.data(), f.ptrs.data(), f.modes.data(),
                                  f.factors.empty() ? nullptr : f.factors.data(), destination.d_, nullptr));
         }
+        // Sums of plaintext products, member-wise: destination j is add_many over i of multiply_plain(encrypteds[i], plains[j K + i])
+        // (K = encrypteds.size()), with the chain's checks, messages and metadata: multiply_plain_inplace's for terms 0 .. K - 1 in
+        // order, then add_many's (correction factors balanced as plan_fold balances them), output by output.  One
+        // sb200_multiply_plain_sum pass reads every ciphertext once per tile of outputs and every plaintext once.  The plaintexts must
+        // all be in NTT form or all in coefficient form.
+        void multiply_plain_sum(const std::vector<CiphertextBatch> &encrypteds, const std::vector<PlaintextBatch> &plains,
+                                CiphertextBatch &destination) const
+        {
+            if (encrypteds.empty())
+                throw std::invalid_argument("encrypteds cannot be empty");
+            for (auto &e : encrypteds)
+                if (&e == &destination)
+                    throw std::invalid_argument("encrypteds must be different from destination");
+            if (plains.size() != encrypteds.size())
+                throw std::invalid_argument("plains must hold one plaintext batch per encrypted");
+            const PlainSum p = plan_plain_sum(encrypteds, plains, 1);
+            std::lock_guard<std::mutex> lock(mu_);
+            std::uint64_t *out = plain_sum_output(encrypteds[0], p, 0, destination);
+            run_plain_sum(encrypteds, plains, p, &out);
+        }
+        void multiply_plain_sum(const std::vector<CiphertextBatch> &encrypteds, const std::vector<PlaintextBatch> &plains,
+                                std::vector<CiphertextBatch> &destinations) const
+        {
+            if (encrypteds.empty())
+                throw std::invalid_argument("encrypteds cannot be empty");
+            if (&destinations == &encrypteds)
+                throw std::invalid_argument("encrypteds must be different from destination");
+            if (plains.empty() || plains.size() % encrypteds.size() != 0)
+                throw std::invalid_argument("plains must hold K plaintext batches per destination");
+            const std::size_t M = plains.size() / encrypteds.size();
+            const PlainSum p = plan_plain_sum(encrypteds, plains, M);
+            std::lock_guard<std::mutex> lock(mu_);
+            destinations.resize(M);
+            std::vector<std::uint64_t *> outs(M);
+            for (std::size_t j = 0; j < M; j++)
+                outs[j] = plain_sum_output(encrypteds[0], p, j, destinations[j]);
+            run_plain_sum(encrypteds, plains, p, outs.data());
+        }
         // multiply_many (evaluator.cpp:1649-1724), member-wise, BFV and BGV.  The reference's queue of products is replayed on
         // operand ids (schedule_products); products that do not depend on each other run as one wave: their operand pairs are staged
         // into two slabs and multiplied and relinearized by one sb200_multiply_relinearize call, one pass over the relinearization
@@ -2176,6 +2214,89 @@ namespace seal_b200
             if (scaled)
                 f.factors = std::move(factors);
             return f;
+        }
+        // ---- multiply_plain_sum: the chain's checks replayed on the products' metadata, before anything is written ----
+        struct PlainSum
+        {
+            Fold fold;                  // the add_many of every output (the factors depend on the ciphertexts only)
+            std::vector<double> scales; // [M] the result's scale: the first product's
+        };
+        PlainSum plan_plain_sum(const std::vector<CiphertextBatch> &encrypteds, const std::vector<PlaintextBatch> &plains, std::size_t M) const
+        {
+            const std::size_t K = encrypteds.size();
+            PlainSum p;
+            // the products t_i: the ciphertexts' metadata with multiply_plain's scale; their slabs are borrowed for plan_fold's
+            // checks only and handed back before these shells go out of scope
+            std::vector<CiphertextBatch> prods(K);
+            auto give_back = [&prods] {
+                for (auto &t : prods)
+                    t.d_ = nullptr;
+            };
+            try
+            {
+                for (std::size_t j = 0; j < M; j++)
+                {
+                    for (std::size_t i = 0; i < K; i++)
+                    {
+                        const CiphertextBatch &e = encrypteds[i];
+                        const PlaintextBatch &pl = plains[j * K + i];
+                        // multiply_plain_inplace (evaluator.cpp:1975-2019), as the batch member above checks it
+                        owned(e), owned(pl);
+                        plain_count(e, pl);
+                        CiphertextBatch &t = prods[i];
+                        t.ctx_ = e.ctx_, t.d_ = e.d_, t.batch_ = e.batch_, t.size_ = e.size_, t.L_ = e.L_, t.n_ = e.n_;
+                        copy_meta(e, t);
+                        if (!pl.ntt_)
+                        {
+                            if (scheme_ == seal::scheme_type::ckks)
+                                throw std::invalid_argument("plain is not valid for encryption parameters");
+                            continue;
+                        }
+                        if (e.parms_id_ != pl.parms_id_)
+                            throw std::invalid_argument("encrypted_ntt and plain_ntt parameter mismatch"); // :2164-2167
+                        t.scale_ = e.scale_ * pl.scale_;
+                        if (!scale_within_bounds(t.scale_, *context_.get_context_data(e.parms_id_)))
+                            throw std::invalid_argument("scale out of bounds"); // :2189-2193
+                    }
+                    std::vector<const CiphertextBatch *> ops;
+                    for (auto &t : prods)
+                        ops.push_back(&t);
+                    p.fold = plan_fold(ops, std::vector<int>(K - 1, SB200_FOLD_ADD)); // add_many (evaluator.cpp:236-262)
+                    p.scales.push_back(prods[0].scale_);
+                }
+            }
+            catch (...)
+            {
+                give_back();
+                throw;
+            }
+            give_back();
+            for (auto &pl : plains)
+                if (pl.ntt_ != plains[0].ntt_)
+                    throw std::invalid_argument("plains must all be in NTT form or all in coefficient form");
+            for (std::size_t i = 0; i < K; i++)
+                p.fold.ptrs[i] = encrypteds[i].d_;
+            return p;
+        }
+        // destination j shaped and given the chain's metadata; caller holds mu_
+        std::uint64_t *plain_sum_output(const CiphertextBatch &e0, const PlainSum &p, std::size_t j, CiphertextBatch &d) const
+        {
+            shape(d, e0.batch_, p.fold.out_size, e0.L_, e0.n_);
+            copy_meta(e0, d);
+            d.scale_ = p.scales[j], d.cf_ = p.fold.cf;
+            return d.d_;
+        }
+        void run_plain_sum(const std::vector<CiphertextBatch> &encrypteds, const std::vector<PlaintextBatch> &plains, const PlainSum &p,
+                           std::uint64_t *const *outs) const
+        {
+            const CiphertextBatch &e0 = encrypteds[0];
+            std::vector<std::size_t> counts;
+            std::vector<const std::uint64_t *> ptrs;
+            for (auto &pl : plains)
+                counts.push_back(pl.batch_), ptrs.push_back(pl.d_);
+            check(sb200_multiply_plain_sum(ctx_, e0.L_, e0.batch_, encrypteds.size(), p.scales.size(), p.fold.sizes.data(), p.fold.ptrs.data(),
+                                           counts.data(), ptrs.data(), e0.ntt_ ? 1 : 0, plains[0].ntt_ ? 1 : 0, p.fold.modes.data(),
+                                           p.fold.factors.empty() ? nullptr : p.fold.factors.data(), outs, nullptr));
         }
         void linear_batch(CiphertextBatch &a, const CiphertextBatch &b, bool subtract) const
         {

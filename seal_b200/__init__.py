@@ -35,7 +35,7 @@ SYMBOLS = [
     "sb200_multiply_host", "sb200_multiply_sized_host", "sb200_square_host", "sb200_add_host", "sb200_sub_host", "sb200_negate_host", "sb200_multiply_plain_host", "sb200_batch_encode_host", "sb200_batch_decode_host", "sb200_plain_to_ntt_host", "sb200_multiply_plain_coeff_host", "sb200_add_plain_coeff_host",
     "sb200_multiply_plain_n", "sb200_multiply_plain_coeff_n", "sb200_add_plain_coeff_n", "sb200_add_plain_ntt", "sb200_multiply_plain_n_host",
     "sb200_multiply_plain_coeff_n_host", "sb200_add_plain_coeff_n_host", "sb200_add_plain_ntt_host",
-    "sb200_add_many", "sb200_add_many_host", "sb200_relinearize_host", "sb200_multiply_relinearize_host", "sb200_rescale_to_next_host",
+    "sb200_add_many", "sb200_add_many_host", "sb200_multiply_plain_sum", "sb200_multiply_plain_sum_host", "sb200_relinearize_host", "sb200_multiply_relinearize_host", "sb200_rescale_to_next_host",
     "sb200_mod_switch_to_next_host", "sb200_apply_galois_host", "sb200_get_parms_id", "sb200_ciphertext_inspect",
     "sb200_ciphertext_save_size", "sb200_ciphertext_load", "sb200_ciphertext_save", "sb200_secret_key_create",
     "sb200_secret_key_destroy", "sb200_decrypt", "sb200_decrypt_host", "sb200_invariant_noise_budget", "sb200_invariant_noise_budget_host", "sb200_encrypt_zero_symmetric", "sb200_public_key_create", "sb200_public_key_destroy", "sb200_encrypt_zero_asymmetric", "sb200_encrypt_zero_symmetric_prng", "sb200_encrypt_zero_asymmetric_prng", "sb200_encrypt_symmetric", "sb200_encrypt_asymmetric", "sb200_kswitch_key_generate", "sb200_public_key_generate", "sb200_ciphertext_save_seeded_size", "sb200_ciphertext_save_seeded",
@@ -136,6 +136,10 @@ def lib():
         L.sb200_add_host.argtypes = [vp, sz, sz, sz, _u64p, _u64p, _u64p]
         L.sb200_add_many.argtypes = [vp, sz, sz, sz, C.POINTER(sz), C.POINTER(vp), C.POINTER(i32), _u64p, vp, vp]
         L.sb200_add_many_host.argtypes = [vp, sz, sz, sz, C.POINTER(sz), C.POINTER(vp), C.POINTER(i32), _u64p, _u64p]
+        L.sb200_multiply_plain_sum.argtypes = [vp, sz, sz, sz, sz, C.POINTER(sz), C.POINTER(vp), C.POINTER(sz), C.POINTER(vp), i32, i32,
+                                               C.POINTER(i32), _u64p, C.POINTER(vp), vp]
+        L.sb200_multiply_plain_sum_host.argtypes = [vp, sz, sz, sz, sz, C.POINTER(sz), C.POINTER(vp), C.POINTER(sz), C.POINTER(vp), i32, i32,
+                                                    C.POINTER(i32), _u64p, C.POINTER(vp)]
         L.sb200_sub_host.argtypes = [vp, sz, sz, sz, _u64p, _u64p, _u64p]
         L.sb200_negate_host.argtypes = [vp, sz, sz, sz, _u64p, _u64p]
         L.sb200_relinearize.argtypes = [vp, sz, sz, vp, vp, vp, vp]
@@ -539,6 +543,26 @@ class Context:
         _check(lib().sb200_add_many_host(self.h, L, B, len(ops), c_sizes, ptrs, c_modes, None if f is None else _hp(f), _hp(out)))
         return out[0] if single else out
 
+    def multiply_plain_sum(self, cts, plains, modes=None, factors=None, ct_is_ntt=True, plain_is_ntt=True):
+        """sb200_multiply_plain_sum_host: cts = K arrays [B][size_i][L][n], plains = M K arrays, plains[j K + i] [count][L][n] (NTT
+        form) or [count][n] (coefficient form), count 1 (shared) or B; modes / factors as in add_many.  Returns M arrays
+        [B][max size_i][L][n]: output j = add_many over i of multiply_plain(cts[i], plains[j K + i])."""
+        cts = [np.ascontiguousarray(a, dtype=np.uint64) for a in cts]
+        plains = [np.ascontiguousarray(p, dtype=np.uint64) for p in plains]
+        K = len(cts)
+        M = len(plains) // K if K else 0
+        B, _, L, n = cts[0].shape if cts else (0, 0, 0, 0)
+        sizes = [a.shape[1] for a in cts]
+        c_sizes, c_modes, f = self._fold_args(sizes, modes, factors)
+        outs = [np.zeros((B, max(sizes) if sizes else 0, L, n), dtype=np.uint64) for _ in range(M)]
+        counts = (C.c_size_t * max(len(plains), 1))(*[p.shape[0] for p in plains])
+        p_cts = (C.c_void_p * max(K, 1))(*[a.ctypes.data for a in cts])
+        p_plains = (C.c_void_p * max(len(plains), 1))(*[p.ctypes.data for p in plains])
+        p_outs = (C.c_void_p * max(M, 1))(*[o.ctypes.data for o in outs])
+        _check(lib().sb200_multiply_plain_sum_host(self.h, L, B, K, M, c_sizes, p_cts, counts, p_plains, int(ct_is_ntt), int(plain_is_ntt),
+                                                   c_modes, None if f is None else _hp(f), p_outs))
+        return outs
+
     def multiply_plain(self, a, plain):
         """Evaluator.multiply_plain, NTT-form ciphertext [B][size][L][n] x NTT-form plaintexts [B][L][n]"""
         a, single = self._batched(a)
@@ -808,6 +832,18 @@ class Context:
         ptrs = (C.c_void_p * max(len(operands), 1))(*[_dp(t).value for t in operands])
         _check(lib().sb200_add_many(self.h, L, batch, len(operands), c_sizes, ptrs, c_modes, None if f is None else _hp(f), _dp(out),
                                     self._stream()))
+
+    def d_multiply_plain_sum(self, cts, plains, outs, L, batch, sizes, plain_counts, ct_is_ntt=True, plain_is_ntt=True, modes=None,
+                             factors=None):
+        """sb200_multiply_plain_sum on device tensors (or raw device pointers): cts [K] of [batch][sizes[i]][L][n], plains [M K] with
+        plain_counts [M K], outs [M] of [batch][max sizes][L][n]; modes / factors as in add_many"""
+        c_sizes, c_modes, f = self._fold_args(sizes, modes, factors)
+        counts = (C.c_size_t * max(len(plain_counts), 1))(*plain_counts)
+        p_cts = (C.c_void_p * max(len(cts), 1))(*[_dp(t).value for t in cts])
+        p_plains = (C.c_void_p * max(len(plains), 1))(*[_dp(t).value for t in plains])
+        p_outs = (C.c_void_p * max(len(outs), 1))(*[_dp(t).value for t in outs])
+        _check(lib().sb200_multiply_plain_sum(self.h, L, batch, len(cts), len(outs), c_sizes, p_cts, counts, p_plains, int(ct_is_ntt),
+                                              int(plain_is_ntt), c_modes, None if f is None else _hp(f), p_outs, self._stream()))
 
     def d_multiply_sized(self, a, b, out, L, size_a, size_b, batch):
         _check(lib().sb200_multiply_sized(self.h, L, size_a, size_b, batch, _dp(a), _dp(b), _dp(out), self._stream()))

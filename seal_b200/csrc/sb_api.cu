@@ -1126,6 +1126,170 @@ namespace
         SB_CATCH
     }
 
+    // M outputs, each a fold over K terms of multiply_plain(ct_t, plain_{j K + t}) (op_multiply_plain_sum); K ciphertext operands
+    // and M K plaintext operands do not fit Layout either, so it has its own two drivers, plain_sum_on_stream and plain_sum_on_host.
+    // The fold's modes and factors are AddMany's, and are checked by it.
+    static void check_plain_count(size_t plain_count, size_t batch);
+    struct PlainSum
+    {
+        AddMany fold; // L, K, sizes, modes, factors; out_size after check
+        size_t M;
+        const size_t *plain_counts;
+        bool ct_ntt, plain_ntt;
+        size_t K() const { return fold.count; }
+        size_t plain_words(const Context &c) const { return plain_ntt ? fold.L * c.n : c.n; }
+        // in the chain's order: multiply_plain's checks of every term (the plaintext counts), then add_many's (sizes, modes)
+        void check(Context &c, size_t batch)
+        {
+            check_level(c, fold.L, batch);
+            if (K() == 0)
+                throw std::invalid_argument("encrypteds cannot be empty");
+            if (M == 0)
+                throw std::invalid_argument("outputs cannot be empty");
+            for (size_t j = 0; j < M * K(); j++)
+                check_plain_count(plain_counts[j], batch);
+            fold.check(c, batch);
+            if (!plain_ntt)
+                plain_level(c, fold.L); // "unsupported operation for scheme type" for CKKS
+        }
+        // no output slab may overlap an operand's slab or another output's
+        void check_alias(const Context &c, size_t batch, const u64 *const *cts, const u64 *const *plains, const u64 *const *outs) const
+        {
+            const size_t poly = fold.L * c.n, ow = batch * fold.out_size * poly;
+            auto overlap = [](const u64 *a, size_t na, const u64 *b, size_t nb) { return a < b + nb && b < a + na; };
+            for (size_t j = 0; j < M; j++)
+            {
+                for (size_t t = 0; t < K(); t++)
+                    if (overlap(outs[j], ow, cts[t], batch * fold.sizes[t] * poly))
+                        throw std::invalid_argument("multiply_plain_sum: an output slab must not overlap a ciphertext operand");
+                for (size_t x = 0; x < M * K(); x++)
+                    if (overlap(outs[j], ow, plains[x], plain_counts[x] * plain_words(c)))
+                        throw std::invalid_argument("multiply_plain_sum: an output slab must not overlap a plaintext operand");
+                for (size_t u = 0; u < j; u++)
+                    if (overlap(outs[j], ow, outs[u], ow))
+                        throw std::invalid_argument("multiply_plain_sum: output slabs must not overlap");
+            }
+        }
+        // counts: the plaintext counts of this call (1 or B)
+        void operator()(Context &c, size_t B, const u64 *const *cts, const size_t *counts, const u64 *const *plains, u64 *const *outs,
+                        cudaStream_t st) const
+        {
+            op_multiply_plain_sum(c, fold.L, B, K(), M, fold.sizes, cts, counts, plains, ct_ntt, plain_ntt, fold.modes, fold.factors, outs, st);
+        }
+    };
+
+    int plain_sum_on_stream(sb200_context *ctx, void *stream, size_t batch, const uint64_t *const *cts, const uint64_t *const *plains,
+                            uint64_t *const *outs, PlainSum op)
+    {
+        SB_NEED(op.fold.sizes);
+        SB_NEED(op.plain_counts);
+        SB_NEED(cts);
+        SB_NEED(plains);
+        SB_NEED(outs);
+        for (size_t t = 0; t < op.K(); t++)
+            SB_NEED(cts[t]);
+        for (size_t t = 0; t < op.M * op.K(); t++)
+            SB_NEED(plains[t]);
+        for (size_t j = 0; j < op.M; j++)
+            SB_NEED(outs[j]);
+        SB_TRY
+        SB_ENTER_STREAM(ctx, stream)
+        op.check(c, batch);
+        if (op.fold.scaled() && !op.fold.factors)
+        {
+            g_last_error = "null pointer: h_factors";
+            return SB200_E_POINTER;
+        }
+        op.check_alias(c, batch, reinterpret_cast<const u64 *const *>(cts), reinterpret_cast<const u64 *const *>(plains),
+                       reinterpret_cast<const u64 *const *>(outs));
+        op(c, batch, reinterpret_cast<const u64 *const *>(cts), op.plain_counts, reinterpret_cast<const u64 *const *>(plains),
+           reinterpret_cast<u64 *const *>(outs), static_cast<cudaStream_t>(stream));
+        return SB200_OK;
+        SB_CATCH
+    }
+
+    // host buffers: shared plaintexts are uploaded once per call; the batch goes in chunks of the context's staging size, every
+    // ciphertext operand, per-member plaintext and output of a chunk staged behind the previous one
+    int plain_sum_on_host(sb200_context *ctx, size_t batch, const uint64_t *const *cts, const uint64_t *const *plains, uint64_t *const *outs,
+                          PlainSum op)
+    {
+        SB_NEED(op.fold.sizes);
+        SB_NEED(op.plain_counts);
+        SB_NEED(cts);
+        SB_NEED(plains);
+        SB_NEED(outs);
+        for (size_t t = 0; t < op.K(); t++)
+            SB_NEED(cts[t]);
+        for (size_t t = 0; t < op.M * op.K(); t++)
+            SB_NEED(plains[t]);
+        for (size_t j = 0; j < op.M; j++)
+            SB_NEED(outs[j]);
+        SB_TRY
+        SB_ENTER(ctx)
+        op.check(c, batch);
+        if (op.fold.scaled() && !op.fold.factors)
+        {
+            g_last_error = "null pointer: h_factors";
+            return SB200_E_POINTER;
+        }
+        op.check_alias(c, batch, reinterpret_cast<const u64 *const *>(cts), reinterpret_cast<const u64 *const *>(plains),
+                       reinterpret_cast<const u64 *const *>(outs));
+        const size_t K = op.K(), M = op.M, poly = op.fold.L * c.n, pw = op.plain_words(c), out_words = op.fold.out_size * poly;
+        const auto shared = [&](size_t x) { return op.plain_counts[x] == 1; };
+        size_t in_words = 0, shared_words = 0; // per ciphertext, all operands; the shared plaintexts once
+        for (size_t t = 0; t < K; t++)
+            in_words += op.fold.sizes[t] * poly;
+        for (size_t x = 0; x < M * K; x++)
+            (shared(x) ? shared_words : in_words) += pw;
+        const size_t per_ct = (in_words + M * out_words) * sizeof(u64);
+        const size_t chunk = std::max<size_t>(1, std::min(batch, c.host_stage_bytes / per_ct));
+        if (!c.io.s_comp)
+            c.io.s_comp = make_stream();
+        cudaStream_t st = c.io.s_comp.get();
+        StreamOrder order(c, st);
+        DevBuf<u64> &din = c.io.buf[0][0], &dshared = c.io.buf[0][1], &dout = c.io.buf[0][2];
+        din.grow(chunk * in_words);
+        dshared.grow(std::max<size_t>(1, shared_words));
+        dout.grow(chunk * M * out_words);
+        std::vector<const u64 *> dcts(K), dplains(M * K);
+        std::vector<u64 *> douts(M);
+        std::vector<size_t> counts(M * K);
+        u64 *s = dshared.get();
+        for (size_t x = 0; x < M * K; x++)
+            if (shared(x))
+            {
+                cuda_check(cudaMemcpyAsync(s, plains[x], pw * sizeof(u64), cudaMemcpyHostToDevice, st), "H2D");
+                dplains[x] = s, s += pw;
+            }
+        for (size_t b0 = 0; b0 < batch; b0 += chunk)
+        {
+            const size_t B = std::min(chunk, batch - b0);
+            u64 *d = din.get();
+            for (size_t t = 0; t < K; t++)
+            {
+                const size_t w = op.fold.sizes[t] * poly;
+                cuda_check(cudaMemcpyAsync(d, cts[t] + b0 * w, B * w * sizeof(u64), cudaMemcpyHostToDevice, st), "H2D");
+                dcts[t] = d, d += B * w;
+            }
+            for (size_t x = 0; x < M * K; x++)
+            {
+                counts[x] = shared(x) ? 1 : B;
+                if (shared(x))
+                    continue;
+                cuda_check(cudaMemcpyAsync(d, plains[x] + b0 * pw, B * pw * sizeof(u64), cudaMemcpyHostToDevice, st), "H2D");
+                dplains[x] = d, d += B * pw;
+            }
+            for (size_t j = 0; j < M; j++)
+                douts[j] = dout.get() + j * B * out_words;
+            op(c, B, dcts.data(), counts.data(), dplains.data(), douts.data(), st);
+            for (size_t j = 0; j < M; j++)
+                cuda_check(cudaMemcpyAsync(outs[j] + b0 * out_words, douts[j], B * out_words * sizeof(u64), cudaMemcpyDeviceToHost, st), "D2H");
+            cuda_check(cudaStreamSynchronize(st), "synchronize");
+        }
+        return SB200_OK;
+        SB_CATCH
+    }
+
     // plain_count: one plaintext per ciphertext (batch) or one for the whole batch (1, a shared operand: Layout::shared_b).  The
     // older entry points, which take one plaintext per ciphertext, stay on the per-ciphertext path at every batch size (shared =
     // false, plain_count = batch); the _n entry points share the plaintext when plain_count = 1.
@@ -1531,6 +1695,23 @@ int sb200_add_many_host(sb200_context *ctx, size_t L, size_t batch, size_t count
                         const uint64_t *factors, uint64_t *out)
 {
     return add_many_on_host(ctx, batch, ops, out, AddMany{ L, count, sizes, modes, reinterpret_cast<const u64 *>(factors) });
+}
+
+int sb200_multiply_plain_sum(sb200_context *ctx, size_t L, size_t batch, size_t count, size_t outputs, const size_t *sizes,
+                             const uint64_t *const *cts, const size_t *plain_counts, const uint64_t *const *plains, int ct_is_ntt,
+                             int plain_is_ntt, const int *modes, const uint64_t *factors, uint64_t *const *outs, void *stream)
+{
+    return plain_sum_on_stream(ctx, stream, batch, cts, plains, outs,
+                               PlainSum{ AddMany{ L, count, sizes, modes, reinterpret_cast<const u64 *>(factors) }, outputs, plain_counts,
+                                         ct_is_ntt != 0, plain_is_ntt != 0 });
+}
+int sb200_multiply_plain_sum_host(sb200_context *ctx, size_t L, size_t batch, size_t count, size_t outputs, const size_t *sizes,
+                                  const uint64_t *const *cts, const size_t *plain_counts, const uint64_t *const *plains, int ct_is_ntt,
+                                  int plain_is_ntt, const int *modes, const uint64_t *factors, uint64_t *const *outs)
+{
+    return plain_sum_on_host(ctx, batch, cts, plains, outs,
+                             PlainSum{ AddMany{ L, count, sizes, modes, reinterpret_cast<const u64 *>(factors) }, outputs, plain_counts,
+                                       ct_is_ntt != 0, plain_is_ntt != 0 });
 }
 
 int sb200_multiply_plain(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, const uint64_t *plain, uint64_t *out,

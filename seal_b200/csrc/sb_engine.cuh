@@ -175,6 +175,14 @@ namespace sb
     constexpr int kFoldMaxOperands = 16;
     void op_add_many(Context &c, size_t L, size_t batch, size_t count, const size_t *sizes, const u64 *const *ops, const int *modes,
                      const u64 *factors, u64 *out, cudaStream_t st);
+    // sums of plaintext products (sb_plainsum.cu, sb200_multiply_plain_sum): outs[j] [B][max sizes][L][n] = the fold (modes /
+    // factors as op_add_many) over t < K of multiply_plain(cts[t] [B][sizes[t]][L][n], plains[j K + t]), plains[j K + t] =
+    // [plain_counts[j K + t]][L][n] (NTT form) or [..][n] (coefficient form), a count of 1 shared by the batch.  Operands not in
+    // NTT form are transformed into scratch; the 128-bit sums are reduced once per kPlainSumWindow terms.
+    constexpr int kPlainSumWindow = 256;
+    void op_multiply_plain_sum(Context &c, size_t L, size_t batch, size_t K, size_t M, const size_t *sizes, const u64 *const *cts,
+                               const size_t *plain_counts, const u64 *const *plains, bool ct_ntt, bool plain_ntt, const int *modes,
+                               const u64 *factors, u64 *const *outs, cudaStream_t st);
     // Plaintext operations take one plaintext per ciphertext, or (shared) one plaintext for the whole batch.
     // NTT-form plaintexts [B][L][n] or [L][n]: multiply_plain of NTT-form ciphertexts; CKKS add_plain / sub_plain (c_0 only)
     void op_multiply_plain(Context &c, size_t L, size_t size, size_t batch, bool shared, const u64 *a, const u64 *plain, u64 *out,
