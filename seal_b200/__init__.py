@@ -146,6 +146,8 @@ def lib():
         L.sb200_multiply_relinearize.argtypes = [vp, sz, sz, vp, vp, vp, vp, vp]
         L.sb200_rescale_to_next.argtypes = [vp, sz, sz, vp, vp, vp]
         L.sb200_mod_switch_to_next.argtypes = [vp, sz, sz, vp, vp, vp]
+        L.sb200_rescale_to_next_sized.argtypes = [vp, sz, sz, sz, vp, vp, vp]
+        L.sb200_mod_switch_to_next_sized.argtypes = [vp, sz, sz, sz, vp, vp, vp]
         L.sb200_apply_galois.argtypes = [vp, sz, sz, vp, u32, vp, vp, vp]
         L.sb200_ntt_forward_host.argtypes = [vp, sz, sz, sz, _u64p]
         L.sb200_ntt_inverse_host.argtypes = [vp, sz, sz, sz, _u64p]
@@ -1044,6 +1046,14 @@ class Context:
 
     def d_mod_switch_to_next(self, in2, out2, L, batch):
         _check(lib().sb200_mod_switch_to_next(self.h, L, batch, _dp(in2), _dp(out2), self._stream()))
+
+    def d_rescale_to_next_sized(self, a, out, L, size, batch):
+        """rescale_to_next of ciphertexts of `size` polynomials: [batch][size][L][n] -> [batch][size][L-1][n]"""
+        _check(lib().sb200_rescale_to_next_sized(self.h, L, size, batch, _dp(a), _dp(out), self._stream()))
+
+    def d_mod_switch_to_next_sized(self, a, out, L, size, batch):
+        """mod_switch_to_next of ciphertexts of `size` polynomials: [batch][size][L][n] -> [batch][size][L-1][n]"""
+        _check(lib().sb200_mod_switch_to_next_sized(self.h, L, size, batch, _dp(a), _dp(out), self._stream()))
 
     def d_apply_galois(self, in2, galois_elt, key, out2, L, batch):
         _check(lib().sb200_apply_galois(self.h, L, batch, _dp(in2), galois_elt, key.h, _dp(out2), self._stream()))

@@ -8,7 +8,7 @@ import pytest
 
 import oracle as O
 import refseal as R
-from common import golden, rand_ct
+from common import assert_words, golden, max_ct, rand_ct
 
 pytestmark = pytest.mark.gpu
 needs_ref = pytest.mark.skipif(not R.available(), reason="oracle/_ref/libsealref.so not present")
@@ -80,6 +80,23 @@ def test_ntt_vs_oracle_and_roundtrip(logn):
     qv = np.array(mods, dtype=np.uint64)[None, None, :, None]
     s = (x + y) % qv  # primes <= 60 bits so the sum cannot wrap
     assert (ctx.transform_to_ntt(s) == (f + ctx.transform_to_ntt(y)) % qv).all()
+
+
+@pytest.mark.parametrize("fast", [True, False], ids=["q57", "q60"])
+@pytest.mark.parametrize("logn", [1, 3, 6, 7, 8, 9, 11, 12, 13, 14, 15, 16, 17])
+def test_ntt_butterfly_classes_vs_oracle(logn, fast):
+    """transform_to_ntt / transform_from_ntt word for word against the oracle in both butterfly classes: every prime below 2^57,
+    the largest 57-bit prime among them (the guard-free forward instantiations ntt_fwd_col<LOGNA, true> / ntt_fwd_local<true>), or
+    a 60-bit prime in the set (guarded); every small-kernel thread count and every LOGNA; uniform words and every word q_i - 1"""
+    n = 1 << logn
+    mods = O.coeff_modulus_create(n, [50, 57 if fast else 60, 30])
+    assert all(q < 2 ** 57 for q in mods) == fast
+    ctx = sb().Context(sb().CKKS, n, mods)
+    oc = O.Oracle(O.CKKS, n, mods)
+    rng = np.random.default_rng(100 + logn)
+    for what, x in (("uniform", rand_ct(rng, mods, n, 2, 3)), ("q - 1", max_ct(mods, n, 2, 3))):
+        assert_words(ctx.transform_to_ntt(x), oc.ntt_forward(3, x), f"forward, {what} words")
+        assert_words(ctx.transform_from_ntt(x), oc.ntt_inverse(3, x), f"inverse, {what} words")
 
 
 @needs_ref
