@@ -363,6 +363,26 @@ __device__ __forceinline__ void tma_load_1d(void *dst_smem, const void *src_gmem
                  "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar))
                  : "memory");
 }
+// 1-D bulk async copy shared -> global, one bulk group per copy.  The threads that wrote the source run fence_proxy_async() before
+// the barrier that precedes the copy; the source may be rewritten after bulk_wait_read, the CTA may exit after bulk_wait
+__device__ __forceinline__ void tma_store_1d(void *dst_gmem, const void *src_smem, uint32_t bytes)
+{
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst_gmem), "r"(smem_u32(src_smem)), "r"(bytes)
+                 : "memory");
+    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+}
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// all but the newest N bulk groups of this thread have read their sources / have completed
+template <int N>
+__device__ __forceinline__ void bulk_wait_read()
+{
+    asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+template <int N>
+__device__ __forceinline__ void bulk_wait()
+{
+    asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
+}
 __device__ __forceinline__ void mbar_wait(u64 *bar, uint32_t phase)
 {
     asm volatile("{\n"

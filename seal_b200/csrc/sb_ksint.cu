@@ -195,159 +195,171 @@ namespace sb
     }
 
     // -------------------------------------------------------------------------------- local passes (12 stages) ----
-    // One CTA (256 threads) transforms 4096-element blocks in shared memory: three radix-16 register passes.  The block's 4095
-    // twiddles are the same for every row: staged once per CTA with one TMA bulk copy (32 KB), reused for kRowsPerCta rows.
-    // Shared-memory layout of the data: idx ^ (bit 8 -> bit 4) ^ (bits 5,6 -> bits 2,3): every access pattern below is
-    // conflict-free (pass 1: lanes consecutive; pass 2: half-warps 256 apart; pass 3: 16 consecutive words per lane as 4 x 16 B).
-    constexpr int kKsLocalSmem = 4096 * 8 + 4096 * 4 + 16;
-    constexpr int kRowsPerCta = 8;
+    // One CTA (256 threads) transforms up to kRowsPerCta 4096-word blocks (one per row, 16 KB, contiguous) with three radix-16
+    // register passes each.  The blocks stream through a ring of kRing linear buffers: one thread loads each block with a bulk
+    // asynchronous copy (mbarrier completion) kRing - 1 blocks ahead and stores the result from the same buffer with a bulk copy, so
+    // the global traffic is whole lines and the next block is in flight while the current one is transformed.  The block's 4095
+    // twiddles are the same for every row: staged once per CTA with one bulk copy (32 KB).  The exchanges between passes go through
+    // a tile in the layout idx ^ (bit 8 -> bit 4) ^ (bits 5,6 -> bits 2,3).  Every shared-memory access is conflict-free, on the
+    // tile and on the linear buffers: lanes consecutive (tid + 256 e), half-warps 256 apart (pass 2), and 16 consecutive words per
+    // lane as 4 x 16 B, visited in the order h ^ hx.
+    constexpr int kRowsPerCta = 16, kRing = 3;
+    constexpr int kKsLocalSmem = 4096 * 8 + 4096 * 4 + kRing * 4096 * 4 + (kRing + 1) * 8;
     __device__ __forceinline__ int swz32(int idx) { return idx ^ (((idx >> 8) & 1) << 4) ^ (((idx >> 5) & 3) << 2); }
 
-    // rows: row rr of this launch lives at data + ((rr * rstride + t) << logn); grid = (row groups, S * 2^r)
-    __global__ void __launch_bounds__(256, 3) ks32_fwd_local(uint32_t *__restrict__ data, int rows, long long rstride, long long tstride,
-                                                              KsIntParams prm, const uint2 *__restrict__ tw_local)
+    // a[4 h + i] <-> a[4 (h ^ x) + i]: the 16-byte groups of a lane's words in the order its accesses of a linear buffer visit them
+    // (x varies across the lanes: selects, not a register index that only the run time knows)
+    __device__ __forceinline__ void xor_groups(uint32_t (&a)[16], int x)
     {
-        extern __shared__ __align__(16) unsigned char ks32_smem[];
-        uint2 *tws = reinterpret_cast<uint2 *>(ks32_smem);
-        uint32_t *xs = reinterpret_cast<uint32_t *>(ks32_smem + 4096 * 8);
-        u64 *bar = reinterpret_cast<u64 *>(ks32_smem + 4096 * 12);
-        const int nb = 1 << prm.r, t = blockIdx.y / nb, g = blockIdx.y - t * nb, tid = threadIdx.x;
-        if (tid == 0)
-            mbar_init(bar, 1);
-        __syncthreads();
-        if (tid == 0)
-        {
-            mbar_expect_tx(bar, 4096 * 8);
-            tma_load_1d(tws, tw_local + (static_cast<size_t>(blockIdx.y) << 12), 4096 * 8, bar);
-        }
-        const P32 P = make_p32(prm.p[t]);
-        const int row0 = blockIdx.x * kRowsPerCta, row1 = min(rows, row0 + kRowsPerCta);
-        const int blk = tid >> 4, l16 = tid & 15;
-        const int p3 = ((16 * tid) ^ (((tid >> 4) & 1) << 4)), hx = (tid >> 1) & 3;
-        bool first = true;
-        // the words of row r+1 are requested before the three passes of row r: their latency hides behind a whole row of arithmetic
-        uint32_t nxt[16];
-        if (row0 < row1)
-        {
-            const uint32_t *b0 = data + ((row0 * rstride + t * tstride) << prm.logn) + (g << 12);
+        const bool s1 = x & 1, s2 = x & 2;
 #pragma unroll
-            for (int e = 0; e < 16; e++)
-                nxt[e] = b0[tid + 256 * e];
-        }
-        for (int row = row0; row < row1; row++)
+        for (int i = 0; i < 4; i++)
         {
-            uint32_t *base = data + ((row * rstride + t * tstride) << prm.logn) + (g << 12);
-            uint32_t a[16];
 #pragma unroll
-            for (int e = 0; e < 16; e++)
-                a[e] = nxt[e];
-            if (row + 1 < row1)
+            for (int h = 0; h < 4; h += 2)
             {
-                const uint32_t *bn = data + (((row + 1) * rstride + t * tstride) << prm.logn) + (g << 12);
-#pragma unroll
-                for (int e = 0; e < 16; e++)
-                    nxt[e] = bn[tid + 256 * e];
+                const uint32_t u = a[4 * h + i], v = a[4 * h + 4 + i];
+                a[4 * h + i] = s1 ? v : u, a[4 * h + 4 + i] = s1 ? u : v;
             }
-            if (first)
-                mbar_wait(bar, 0), first = false;
-            radix_fwd<4>(a, [&](int lvl, int gg) { return tws[(1 << lvl) + gg]; }, P);
 #pragma unroll
-            for (int e = 0; e < 16; e++)
-                xs[swz32(tid + 256 * e)] = a[e];
-            __syncthreads();
-#pragma unroll
-            for (int e = 0; e < 16; e++)
-                a[e] = xs[swz32((blk << 8) + l16 + 16 * e)];
-            radix_fwd<4>(a, [&](int lvl, int gg) { return tws[(16 << lvl) + (blk << lvl) + gg]; }, P);
-#pragma unroll
-            for (int e = 0; e < 16; e++)
-                xs[swz32((blk << 8) + l16 + 16 * e)] = a[e];
-            __syncthreads();
-#pragma unroll
-            for (int h = 0; h < 4; h++)
+            for (int h = 0; h < 2; h++)
             {
-                const uint4 q = *reinterpret_cast<const uint4 *>(xs + p3 + 4 * (h ^ hx));
-                a[4 * h] = q.x, a[4 * h + 1] = q.y, a[4 * h + 2] = q.z, a[4 * h + 3] = q.w;
+                const uint32_t u = a[4 * h + i], v = a[4 * h + 8 + i];
+                a[4 * h + i] = s2 ? v : u, a[4 * h + 8 + i] = s2 ? u : v;
             }
-            radix_fwd<4>(a, [&](int lvl, int gg) { return tws[256 + (((1 << lvl) - 1 + gg) << 8) + tid]; }, P);
-#pragma unroll
-            for (int e = 0; e < 16; e++)
-                a[e] = minsub(minsub(a[e], P.p2), P.p); // canonical: the multiply-accumulate sums L products in 64 bits
-#pragma unroll
-            for (int h = 0; h < 4; h++)
-                *reinterpret_cast<uint4 *>(base + 16 * tid + 4 * h) = make_uint4(a[4 * h], a[4 * h + 1], a[4 * h + 2], a[4 * h + 3]);
-            __syncthreads();
         }
     }
 
-    // inverse: inputs in [0, 2p), outputs in [0, 2p) (the scaling by n^-1 is folded into the CRT constants)
-    __global__ void __launch_bounds__(256, 3) ks32_inv_local(uint32_t *__restrict__ data, int rows, long long rstride, long long tstride,
-                                                              KsIntParams prm, const uint2 *__restrict__ tw_local)
+    // rows: row rr of this launch lives at data + ((rr * rstride + t) << logn).  In place.  One-dimensional grid, the block index of
+    // the row (auxiliary prime t, 4096-word block g; S * 2^r of them) fastest: the CTAs in flight together cover a few groups of
+    // consecutive rows completely instead of one block of many rows that lie tstride or rstride rows apart
+    // Forward: outputs canonical.  Inverse: inputs in [0, 2p), outputs in [0, 2p) (the scaling by n^-1 is folded into the CRT
+    // constants)
+    template <bool INV>
+    __device__ __forceinline__ void ks32_local(uint32_t *__restrict__ data, int rows, long long rstride, long long tstride,
+                                               const KsIntParams &prm, const uint2 *__restrict__ tw_local)
     {
         extern __shared__ __align__(16) unsigned char ks32_smem[];
         uint2 *tws = reinterpret_cast<uint2 *>(ks32_smem);
         uint32_t *xs = reinterpret_cast<uint32_t *>(ks32_smem + 4096 * 8);
-        u64 *bar = reinterpret_cast<u64 *>(ks32_smem + 4096 * 12);
-        const int nb = 1 << prm.r, t = blockIdx.y / nb, g = blockIdx.y - t * nb, tid = threadIdx.x;
+        uint32_t *ring = xs + 4096;
+        u64 *bar = reinterpret_cast<u64 *>(ring + kRing * 4096); // [0]: twiddles, [1 + s]: ring buffer s
+        const int ntg = prm.S << prm.r, tg = blockIdx.x % ntg, t = tg >> prm.r, g = tg - (t << prm.r), tid = threadIdx.x;
+        const int row0 = blockIdx.x / ntg * kRowsPerCta, nrows = min(rows - row0, kRowsPerCta);
+        auto block = [&](int i) { return data + (((row0 + i) * rstride + t * tstride) << prm.logn) + (g << 12); };
+        auto fetch = [&](int i) {
+            u64 *b = bar + 1 + i % kRing;
+            mbar_expect_tx(b, 4096 * 4);
+            tma_load_1d(ring + (i % kRing) * 4096, block(i), 4096 * 4, b);
+        };
         if (tid == 0)
-            mbar_init(bar, 1);
+            for (int s = 0; s <= kRing; s++)
+                mbar_init(bar + s, 1);
         __syncthreads();
         if (tid == 0)
         {
             mbar_expect_tx(bar, 4096 * 8);
-            tma_load_1d(tws, tw_local + (static_cast<size_t>(blockIdx.y) << 12), 4096 * 8, bar);
+            tma_load_1d(tws, tw_local + (static_cast<size_t>(tg) << 12), 4096 * 8, bar);
+            for (int i = 0; i < min(nrows, kRing - 1); i++)
+                fetch(i);
         }
         const P32 P = make_p32(prm.p[t]);
-        const int row0 = blockIdx.x * kRowsPerCta, row1 = min(rows, row0 + kRowsPerCta);
         const int blk = tid >> 4, l16 = tid & 15;
         const int p3 = ((16 * tid) ^ (((tid >> 4) & 1) << 4)), hx = (tid >> 1) & 3;
-        bool first = true;
-        uint4 nxt[4]; // row r+1 is requested before the three passes of row r
-        if (row0 < row1)
+        mbar_wait(bar, 0);
+        for (int i = 0; i < nrows; i++)
         {
-            const uint32_t *b0 = data + ((row0 * rstride + t * tstride) << prm.logn) + (g << 12);
-#pragma unroll
-            for (int h = 0; h < 4; h++)
-                nxt[h] = *reinterpret_cast<const uint4 *>(b0 + 16 * tid + 4 * h);
-        }
-        for (int row = row0; row < row1; row++)
-        {
-            uint32_t *base = data + ((row * rstride + t * tstride) << prm.logn) + (g << 12);
+            uint32_t *buf = ring + (i % kRing) * 4096;
+            mbar_wait(bar + 1 + i % kRing, (i / kRing) & 1);
             uint32_t a[16];
-#pragma unroll
-            for (int h = 0; h < 4; h++)
-                a[4 * h] = nxt[h].x, a[4 * h + 1] = nxt[h].y, a[4 * h + 2] = nxt[h].z, a[4 * h + 3] = nxt[h].w;
-            if (row + 1 < row1)
+            if constexpr (!INV)
             {
-                const uint32_t *bn = data + (((row + 1) * rstride + t * tstride) << prm.logn) + (g << 12);
+#pragma unroll
+                for (int e = 0; e < 16; e++)
+                    a[e] = buf[tid + 256 * e];
+                radix_fwd<4>(a, [&](int lvl, int gg) { return tws[(1 << lvl) + gg]; }, P);
+#pragma unroll
+                for (int e = 0; e < 16; e++)
+                    xs[swz32(tid + 256 * e)] = a[e];
+                __syncthreads();
+#pragma unroll
+                for (int e = 0; e < 16; e++)
+                    a[e] = xs[swz32((blk << 8) + l16 + 16 * e)];
+                radix_fwd<4>(a, [&](int lvl, int gg) { return tws[(16 << lvl) + (blk << lvl) + gg]; }, P);
+#pragma unroll
+                for (int e = 0; e < 16; e++)
+                    xs[swz32((blk << 8) + l16 + 16 * e)] = a[e];
+                __syncthreads();
 #pragma unroll
                 for (int h = 0; h < 4; h++)
-                    nxt[h] = *reinterpret_cast<const uint4 *>(bn + 16 * tid + 4 * h);
+                {
+                    const uint4 q = *reinterpret_cast<const uint4 *>(xs + p3 + 4 * (h ^ hx));
+                    a[4 * h] = q.x, a[4 * h + 1] = q.y, a[4 * h + 2] = q.z, a[4 * h + 3] = q.w;
+                }
+                radix_fwd<4>(a, [&](int lvl, int gg) { return tws[256 + (((1 << lvl) - 1 + gg) << 8) + tid]; }, P);
+#pragma unroll
+                for (int e = 0; e < 16; e++)
+                    a[e] = minsub(minsub(a[e], P.p2), P.p); // canonical: the multiply-accumulate sums L products in 64 bits
+                xor_groups(a, hx);
+#pragma unroll
+                for (int h = 0; h < 4; h++)
+                    *reinterpret_cast<uint4 *>(buf + 16 * tid + 4 * (h ^ hx)) = make_uint4(a[4 * h], a[4 * h + 1], a[4 * h + 2], a[4 * h + 3]);
             }
-            if (first)
-                mbar_wait(bar, 0), first = false;
-            radix_inv<4>(a, [&](int lvl, int gg) { return tws[256 + (((1 << lvl) - 1 + gg) << 8) + tid]; }, P);
+            else
+            {
 #pragma unroll
-            for (int h = 0; h < 4; h++)
-                *reinterpret_cast<uint4 *>(xs + p3 + 4 * (h ^ hx)) = make_uint4(a[4 * h], a[4 * h + 1], a[4 * h + 2], a[4 * h + 3]);
+                for (int h = 0; h < 4; h++)
+                {
+                    const uint4 q = *reinterpret_cast<const uint4 *>(buf + 16 * tid + 4 * (h ^ hx));
+                    a[4 * h] = q.x, a[4 * h + 1] = q.y, a[4 * h + 2] = q.z, a[4 * h + 3] = q.w;
+                }
+                xor_groups(a, hx);
+                radix_inv<4>(a, [&](int lvl, int gg) { return tws[256 + (((1 << lvl) - 1 + gg) << 8) + tid]; }, P);
+#pragma unroll
+                for (int h = 0; h < 4; h++)
+                    *reinterpret_cast<uint4 *>(xs + p3 + 4 * (h ^ hx)) = make_uint4(a[4 * h], a[4 * h + 1], a[4 * h + 2], a[4 * h + 3]);
+                __syncthreads();
+#pragma unroll
+                for (int e = 0; e < 16; e++)
+                    a[e] = xs[swz32((blk << 8) + l16 + 16 * e)];
+                radix_inv<4>(a, [&](int lvl, int gg) { return tws[(16 << lvl) + (blk << lvl) + gg]; }, P);
+#pragma unroll
+                for (int e = 0; e < 16; e++)
+                    xs[swz32((blk << 8) + l16 + 16 * e)] = a[e];
+                __syncthreads();
+#pragma unroll
+                for (int e = 0; e < 16; e++)
+                    a[e] = xs[swz32(tid + 256 * e)];
+                radix_inv<4>(a, [&](int lvl, int gg) { return tws[(1 << lvl) + gg]; }, P);
+#pragma unroll
+                for (int e = 0; e < 16; e++)
+                    buf[tid + 256 * e] = a[e];
+            }
+            // the buffer goes out once every thread's words are in it; the tile is free for the next row
+            fence_proxy_async();
             __syncthreads();
-#pragma unroll
-            for (int e = 0; e < 16; e++)
-                a[e] = xs[swz32((blk << 8) + l16 + 16 * e)];
-            radix_inv<4>(a, [&](int lvl, int gg) { return tws[(16 << lvl) + (blk << lvl) + gg]; }, P);
-#pragma unroll
-            for (int e = 0; e < 16; e++)
-                xs[swz32((blk << 8) + l16 + 16 * e)] = a[e];
-            __syncthreads();
-#pragma unroll
-            for (int e = 0; e < 16; e++)
-                a[e] = xs[swz32(tid + 256 * e)];
-            radix_inv<4>(a, [&](int lvl, int gg) { return tws[(1 << lvl) + gg]; }, P);
-#pragma unroll
-            for (int e = 0; e < 16; e++)
-                base[tid + 256 * e] = a[e];
-            __syncthreads();
+            if (tid == 0)
+            {
+                tma_store_1d(block(i), buf, 4096 * 4);
+                if (i + kRing - 1 < nrows)
+                {
+                    bulk_wait_read<1>(); // the buffer of row i + kRing - 1 last held row i - 1: its store has read it
+                    fetch(i + kRing - 1);
+                }
+            }
         }
+        if (tid == 0)
+            bulk_wait<0>(); // no store may still read shared memory when the CTA exits
+    }
+    __global__ void __launch_bounds__(256, 2) ks32_fwd_local(uint32_t *__restrict__ data, int rows, long long rstride, long long tstride,
+                                                              KsIntParams prm, const uint2 *__restrict__ tw_local)
+    {
+        ks32_local<false>(data, rows, rstride, tstride, prm, tw_local);
+    }
+    __global__ void __launch_bounds__(256, 2) ks32_inv_local(uint32_t *__restrict__ data, int rows, long long rstride, long long tstride,
+                                                              KsIntParams prm, const uint2 *__restrict__ tw_local)
+    {
+        ks32_local<true>(data, rows, rstride, tstride, prm, tw_local);
     }
 
     // ------------------------------------------------------------------------------ (3b) inverse, outer pass ----
@@ -1352,7 +1364,7 @@ namespace sb
             cuda_check(cudaGetLastError(), "ks32_fwd_outer");
         }
         // (padding rows of the digit layout are transformed too: a few uninitialised rows whose products are never stored)
-        dim3 grid(static_cast<unsigned>((map.rows_out + kRowsPerCta - 1) / kRowsPerCta), static_cast<unsigned>(d.prm.S << d.prm.r));
+        const unsigned grid = static_cast<unsigned>((map.rows_out + kRowsPerCta - 1) / kRowsPerCta * (d.prm.S << d.prm.r));
         c.stats.begin("ks32_fwd_local", 0, rows * n * 8.0 * S, st, 0, 0);
         c.stats.work32(0.5 * rows * n * S * 12, 0);
         ks32_fwd_local<<<grid, 256, kKsLocalSmem, st>>>(Dh, map.rows_out, 1, map.rows_out, d.prm, d.d_fwd_local.get());
@@ -1516,7 +1528,7 @@ namespace sb
         const KsInt &d = c.ksint;
         const int S = d.prm.S;
         const double n = static_cast<double>(c.n);
-        dim3 grid(static_cast<unsigned>((arows + kRowsPerCta - 1) / kRowsPerCta), static_cast<unsigned>(S << d.prm.r));
+        const unsigned grid = static_cast<unsigned>((arows + kRowsPerCta - 1) / kRowsPerCta * (S << d.prm.r));
         c.stats.begin("ks32_inv_local", 0, 8.0 * arows * S * n, st);
         c.stats.work32(0.5 * arows * S * n * 12, 0);
         ks32_inv_local<<<grid, 256, kKsLocalSmem, st>>>(data, arows, S, 1, d.prm, d.d_inv_local.get());
