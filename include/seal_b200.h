@@ -243,6 +243,26 @@ int sb200_multiply_plain_sum(sb200_context *ctx, size_t L, size_t batch, size_t 
 int sb200_multiply_plain_sum_host(sb200_context *ctx, size_t L, size_t batch, size_t count, size_t outputs, const size_t *sizes,
                                   const uint64_t *const *h_cts, const size_t *plain_counts, const uint64_t *const *h_plains, int ct_is_ntt,
                                   int plain_is_ntt, const int *modes, const uint64_t *h_factors, uint64_t *const *h_outs);
+/* Sums of ciphertext products: sum_i lhs_{j K + i} * rhs_i in one pass, with one size-3 result per sum (the lazy-relinearization
+ * idiom: relinearize the sum once).  Member b of d_outs[j] (j < outputs = M) has the words of the chain t_i = sb200_multiply(member b
+ * of d_lhs[j K + i], member b of d_rhs[i]) for i < count = K, then sb200_add_many(t_0 .. t_{K-1}, modes, h_factors)
+ * (evaluator.cpp:352-841, :155-262), for any input words.
+ *   d_lhs[j K + i], d_rhs[i]: [batch][2][L][n], in the scheme's form (NTT form for CKKS and BGV, coefficient form for BFV);
+ *     a left operand may be the right one (a square);
+ *   modes [K - 1] / h_factors [K - 1][2]: as for sb200_add_many (NULL: every step adds; BGV correction-factor balancing);
+ *   d_outs[j]: [batch][3][L][n].
+ * CKKS and BGV: one kernel pass reads every right operand once per tile of outputs and every left operand once; the 128-bit sums
+ * are reduced once per window of terms (128 when every prime of the level is below 2^60, 32 at 61 bits) and the fold's factors
+ * enter as one constant per term.  BFV: the chain's sb200_multiply into scratch, as many terms at a time as
+ * SB200_LIMIT_SCRATCH_BYTES holds, each chunk folded into the output (no caller-side intermediates).  Errors, all before the first
+ * launch, in the chain's order (multiply's, then add_many's): count = 0 or outputs = 0, a BFV level above sb200_multiply's limit,
+ * a mode outside 0..3 (SB200_E_INVALID_ARG); a NULL array, operand or output, or (with a scaled step) h_factors (SB200_E_POINTER);
+ * an output slab overlapping an operand's slab or another output's (SB200_E_INVALID_ARG).  The _host form stages the batch in
+ * chunks of SB200_LIMIT_HOST_STAGE_BYTES. */
+int sb200_multiply_sum(sb200_context *ctx, size_t L, size_t batch, size_t count, size_t outputs, const uint64_t *const *d_lhs,
+                       const uint64_t *const *d_rhs, const int *modes, const uint64_t *h_factors, uint64_t *const *d_outs, void *stream);
+int sb200_multiply_sum_host(sb200_context *ctx, size_t L, size_t batch, size_t count, size_t outputs, const uint64_t *const *h_lhs,
+                            const uint64_t *const *h_rhs, const int *modes, const uint64_t *h_factors, uint64_t *const *h_outs);
 /* Evaluator::multiply_plain with ciphertext and plaintext both in NTT form (evaluator.cpp:1975-1994 -> multiply_plain_ntt
  * :2157-2195): every polynomial of the ciphertext times the plaintext, dyadic.  d_plain is [batch][L][n]: one NTT-form
  * plaintext per ciphertext, at the ciphertext's level (Plaintext::data() with parms_id == the ciphertext's).  May run in place. */

@@ -1214,6 +1214,56 @@ namespace seal_b200
                 outs[j] = plain_sum_output(encrypteds[0], p, j, destinations[j]);
             run_plain_sum(encrypteds, plains, p, outs.data());
         }
+        // Sums of ciphertext products, member-wise: destination j is add_many over i of multiply(encrypteds1[j K + i], encrypteds2[i])
+        // (K = encrypteds2.size()), the size-3 products summed before any relinearization (the lazy-relinearization idiom of
+        // inner products and encrypted matrix x encrypted vector by diagonals).  The chain's checks, messages and metadata:
+        // multiply_inplace's for terms 0 .. K - 1 in order, then add_many's (correction factors cf(a) cf(b) mod t balanced as
+        // plan_fold balances them), output by output, all before anything is written.  When every operand has size 2, one
+        // sb200_multiply_sum call forms every output (one per output when BGV's balancing differs between outputs); other sizes take
+        // the chain itself (a copy, multiply_inplace, then add_many).  An operand of encrypteds1 may be one of encrypteds2 (squares).
+        void multiply_sum(const std::vector<CiphertextBatch> &encrypteds1, const std::vector<CiphertextBatch> &encrypteds2,
+                          CiphertextBatch &destination) const
+        {
+            check_sum_destination(encrypteds1, encrypteds2, destination);
+            if (encrypteds1.size() != encrypteds2.size())
+                throw std::invalid_argument("encrypteds1 must hold K ciphertext batches per destination");
+            const MultiplySum p = plan_multiply_sum(encrypteds1, encrypteds2, 1);
+            CiphertextBatch *d = &destination;
+            run_multiply_sum(encrypteds1, encrypteds2, p, &d);
+        }
+        void multiply_sum(const std::vector<CiphertextBatch> &encrypteds1, const std::vector<CiphertextBatch> &encrypteds2,
+                          std::vector<CiphertextBatch> &destinations) const
+        {
+            const std::size_t M = sum_outputs(encrypteds1, encrypteds2, destinations);
+            const MultiplySum p = plan_multiply_sum(encrypteds1, encrypteds2, M);
+            destinations.resize(M);
+            std::vector<CiphertextBatch *> d;
+            for (auto &x : destinations)
+                d.push_back(&x);
+            run_multiply_sum(encrypteds1, encrypteds2, p, d.data());
+        }
+        // multiply_sum, then relinearize_inplace of every destination: one key switch per sum.  relinearize_inplace's checks run
+        // with the others, before anything is written.
+        void multiply_relinearize_sum(const std::vector<CiphertextBatch> &encrypteds1, const std::vector<CiphertextBatch> &encrypteds2,
+                                      const seal::RelinKeys &relin_keys, CiphertextBatch &destination) const
+        {
+            multiply_relinearize_sum_one(encrypteds1, encrypteds2, relin_keys, destination);
+        }
+        void multiply_relinearize_sum(const std::vector<CiphertextBatch> &encrypteds1, const std::vector<CiphertextBatch> &encrypteds2,
+                                      const DeviceRelinKeys &relin_keys, CiphertextBatch &destination) const
+        {
+            multiply_relinearize_sum_one(encrypteds1, encrypteds2, relin_keys, destination);
+        }
+        void multiply_relinearize_sum(const std::vector<CiphertextBatch> &encrypteds1, const std::vector<CiphertextBatch> &encrypteds2,
+                                      const seal::RelinKeys &relin_keys, std::vector<CiphertextBatch> &destinations) const
+        {
+            multiply_relinearize_sum_many(encrypteds1, encrypteds2, relin_keys, destinations);
+        }
+        void multiply_relinearize_sum(const std::vector<CiphertextBatch> &encrypteds1, const std::vector<CiphertextBatch> &encrypteds2,
+                                      const DeviceRelinKeys &relin_keys, std::vector<CiphertextBatch> &destinations) const
+        {
+            multiply_relinearize_sum_many(encrypteds1, encrypteds2, relin_keys, destinations);
+        }
         // multiply_many (evaluator.cpp:1649-1724), member-wise, BFV and BGV.  The reference's queue of products is replayed on
         // operand ids (schedule_products); products that do not depend on each other run as one wave: their operand pairs are staged
         // into two slabs and multiplied and relinearized by one sb200_multiply_relinearize call, one pass over the relinearization
@@ -2297,6 +2347,180 @@ namespace seal_b200
             check(sb200_multiply_plain_sum(ctx_, e0.L_, e0.batch_, encrypteds.size(), p.scales.size(), p.fold.sizes.data(), p.fold.ptrs.data(),
                                            counts.data(), ptrs.data(), e0.ntt_ ? 1 : 0, plains[0].ntt_ ? 1 : 0, p.fold.modes.data(),
                                            p.fold.factors.empty() ? nullptr : p.fold.factors.data(), outs, nullptr));
+        }
+        // ---- multiply_sum: the chain's checks replayed on the products' metadata, before anything is written ----
+        struct MultiplySum
+        {
+            std::vector<Fold> folds;    // [M] the add_many of every output (BGV's factors depend on both operands)
+            std::vector<double> scales; // [M] the result's scale: the first product's
+            bool fused = true;          // every operand has size 2: sb200_multiply_sum
+        };
+        void check_sum_destination(const std::vector<CiphertextBatch> &e1, const std::vector<CiphertextBatch> &e2, const CiphertextBatch &d) const
+        {
+            if (e2.empty())
+                throw std::invalid_argument("encrypteds cannot be empty");
+            for (auto *v : { &e1, &e2 })
+                for (auto &e : *v)
+                    if (&e == &d)
+                        throw std::invalid_argument("encrypteds must be different from destination");
+        }
+        static std::size_t sum_outputs(const std::vector<CiphertextBatch> &e1, const std::vector<CiphertextBatch> &e2,
+                                       const std::vector<CiphertextBatch> &d)
+        {
+            if (e2.empty())
+                throw std::invalid_argument("encrypteds cannot be empty");
+            if (&d == &e1 || &d == &e2)
+                throw std::invalid_argument("encrypteds must be different from destination");
+            if (e1.empty() || e1.size() % e2.size() != 0)
+                throw std::invalid_argument("encrypteds1 must hold K ciphertext batches per destination");
+            return e1.size() / e2.size();
+        }
+        MultiplySum plan_multiply_sum(const std::vector<CiphertextBatch> &e1, const std::vector<CiphertextBatch> &e2, std::size_t M) const
+        {
+            const std::size_t K = e2.size();
+            const bool ckks = scheme_ == seal::scheme_type::ckks, bgv = scheme_ == seal::scheme_type::bgv;
+            MultiplySum p;
+            // the products t_i: metadata as multiply_inplace leaves it; their slabs are borrowed (the left operand's) for
+            // plan_fold's checks only and handed back before these shells go out of scope
+            std::vector<CiphertextBatch> prods(K);
+            auto give_back = [&prods] {
+                for (auto &t : prods)
+                    t.d_ = nullptr;
+            };
+            try
+            {
+                for (std::size_t j = 0; j < M; j++)
+                {
+                    for (std::size_t i = 0; i < K; i++)
+                    {
+                        const CiphertextBatch &a = e1[j * K + i], &b = e2[i];
+                        // multiply_inplace (evaluator.cpp:352-393), as the batch member above checks it
+                        owned(a), owned(b);
+                        if (a.parms_id_ != b.parms_id_ || a.batch_ != b.batch_)
+                            throw std::invalid_argument("encrypted1 and encrypted2 parameter mismatch");
+                        if ((ckks || bgv) && !(a.ntt_ && b.ntt_))
+                            throw std::invalid_argument("encrypted1 or encrypted2 must be in NTT form");
+                        if (!(ckks || bgv) && (a.ntt_ || b.ntt_))
+                            throw std::invalid_argument("encrypted1 or encrypted2 cannot be in NTT form");
+                        auto cd = context_.get_context_data(a.parms_id_);
+                        const std::size_t so = a.size_ + b.size_ - 1;
+                        if (so > SEAL_CIPHERTEXT_SIZE_MAX)
+                            throw std::invalid_argument("invalid size");
+                        CiphertextBatch &t = prods[i];
+                        t.ctx_ = a.ctx_, t.d_ = a.d_, t.batch_ = a.batch_, t.size_ = so, t.L_ = a.L_, t.n_ = a.n_;
+                        copy_meta(a, t);
+                        if (ckks)
+                        {
+                            t.scale_ = a.scale_ * b.scale_;
+                            if (!scale_within_bounds(t.scale_, *cd))
+                                throw std::invalid_argument("scale out of bounds");
+                        }
+                        if (bgv)
+                            t.cf_ = seal::util::multiply_uint_mod(a.cf_, b.cf_, cd->parms().plain_modulus());
+                        p.fused = p.fused && a.size_ == 2 && b.size_ == 2;
+                    }
+                    std::vector<const CiphertextBatch *> ops;
+                    for (auto &t : prods)
+                        ops.push_back(&t);
+                    p.folds.push_back(plan_fold(ops, std::vector<int>(K - 1, SB200_FOLD_ADD))); // add_many (evaluator.cpp:236-262)
+                    p.scales.push_back(prods[0].scale_);
+                }
+            }
+            catch (...)
+            {
+                give_back();
+                throw;
+            }
+            give_back();
+            return p;
+        }
+        void run_multiply_sum(const std::vector<CiphertextBatch> &e1, const std::vector<CiphertextBatch> &e2, const MultiplySum &p,
+                              CiphertextBatch *const *dest) const
+        {
+            const std::size_t K = e2.size(), M = p.folds.size();
+            if (!p.fused) // other sizes: the chain itself
+            {
+                for (std::size_t j = 0; j < M; j++)
+                {
+                    std::vector<CiphertextBatch> terms(K);
+                    for (std::size_t i = 0; i < K; i++)
+                    {
+                        copy(e1[j * K + i], terms[i]);
+                        multiply_inplace(terms[i], e2[i]);
+                    }
+                    add_many(terms, *dest[j]);
+                }
+                return;
+            }
+            const CiphertextBatch &b0 = e2[0];
+            std::lock_guard<std::mutex> lock(mu_);
+            for (std::size_t j = 0; j < M; j++)
+            {
+                CiphertextBatch &d = *dest[j];
+                shape(d, b0.batch_, 3, b0.L_, b0.n_);
+                copy_meta(e1[j * K], d);
+                d.scale_ = p.scales[j], d.cf_ = p.folds[j].cf;
+            }
+            std::vector<const std::uint64_t *> lhs, rhs;
+            std::vector<std::uint64_t *> outs;
+            for (auto &e : e1)
+                lhs.push_back(e.d_);
+            for (auto &e : e2)
+                rhs.push_back(e.d_);
+            for (std::size_t j = 0; j < M; j++)
+                outs.push_back(dest[j]->d_);
+            // one call for every output when the outputs share the fold's steps (always, but for BGV with differing correction factors)
+            bool same = true;
+            for (auto &f : p.folds)
+                same = same && f.modes == p.folds[0].modes && f.factors == p.folds[0].factors;
+            for (std::size_t j0 = 0, m = same ? M : 1; j0 < M; j0 += m)
+            {
+                const Fold &f = p.folds[j0];
+                check(sb200_multiply_sum(ctx_, b0.L_, b0.batch_, K, m, lhs.data() + j0 * K, rhs.data(), f.modes.empty() ? nullptr : f.modes.data(),
+                                         f.factors.empty() ? nullptr : f.factors.data(), outs.data() + j0, nullptr));
+            }
+        }
+        // relinearize_inplace's checks (relinearize_batch) for a result of `size` polynomials
+        template <class RelinKeys>
+        void check_relinearize(const RelinKeys &relin_keys, std::size_t size, bool ntt) const
+        {
+            if (relin_keys.parms_id() != context_.key_parms_id())
+                throw std::invalid_argument("relin_keys is not valid for encryption parameters");
+            if (size < 2)
+                throw std::invalid_argument("destination_size must be at least 2 and less than or equal to current count");
+            if (relin_keys.size() < size - 2)
+                throw std::invalid_argument("not enough relinearization keys");
+            if (size > 2)
+                check_keyswitch_form(ntt);
+        }
+        template <class RelinKeys>
+        void multiply_relinearize_sum_one(const std::vector<CiphertextBatch> &e1, const std::vector<CiphertextBatch> &e2, const RelinKeys &relin_keys,
+                                          CiphertextBatch &destination) const
+        {
+            check_sum_destination(e1, e2, destination);
+            if (e1.size() != e2.size())
+                throw std::invalid_argument("encrypteds1 must hold K ciphertext batches per destination");
+            const MultiplySum p = plan_multiply_sum(e1, e2, 1);
+            check_relinearize(relin_keys, p.folds[0].out_size, e1[0].ntt_);
+            CiphertextBatch *d = &destination;
+            run_multiply_sum(e1, e2, p, &d);
+            relinearize_inplace(destination, relin_keys);
+        }
+        template <class RelinKeys>
+        void multiply_relinearize_sum_many(const std::vector<CiphertextBatch> &e1, const std::vector<CiphertextBatch> &e2, const RelinKeys &relin_keys,
+                                           std::vector<CiphertextBatch> &destinations) const
+        {
+            const std::size_t M = sum_outputs(e1, e2, destinations);
+            const MultiplySum p = plan_multiply_sum(e1, e2, M);
+            for (std::size_t j = 0; j < M; j++)
+                check_relinearize(relin_keys, p.folds[j].out_size, e1[j * e2.size()].ntt_);
+            destinations.resize(M);
+            std::vector<CiphertextBatch *> d;
+            for (auto &x : destinations)
+                d.push_back(&x);
+            run_multiply_sum(e1, e2, p, d.data());
+            for (auto &x : destinations)
+                relinearize_inplace(x, relin_keys);
         }
         void linear_batch(CiphertextBatch &a, const CiphertextBatch &b, bool subtract) const
         {

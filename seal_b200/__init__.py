@@ -35,7 +35,7 @@ SYMBOLS = [
     "sb200_multiply_host", "sb200_multiply_sized_host", "sb200_square_host", "sb200_add_host", "sb200_sub_host", "sb200_negate_host", "sb200_multiply_plain_host", "sb200_batch_encode_host", "sb200_batch_decode_host", "sb200_plain_to_ntt_host", "sb200_multiply_plain_coeff_host", "sb200_add_plain_coeff_host",
     "sb200_multiply_plain_n", "sb200_multiply_plain_coeff_n", "sb200_add_plain_coeff_n", "sb200_add_plain_ntt", "sb200_multiply_plain_n_host",
     "sb200_multiply_plain_coeff_n_host", "sb200_add_plain_coeff_n_host", "sb200_add_plain_ntt_host",
-    "sb200_add_many", "sb200_add_many_host", "sb200_multiply_plain_sum", "sb200_multiply_plain_sum_host", "sb200_relinearize_host", "sb200_multiply_relinearize_host", "sb200_rescale_to_next_host",
+    "sb200_add_many", "sb200_add_many_host", "sb200_multiply_plain_sum", "sb200_multiply_plain_sum_host", "sb200_multiply_sum", "sb200_multiply_sum_host", "sb200_relinearize_host", "sb200_multiply_relinearize_host", "sb200_rescale_to_next_host",
     "sb200_mod_switch_to_next_host", "sb200_apply_galois_host", "sb200_get_parms_id", "sb200_ciphertext_inspect",
     "sb200_ciphertext_save_size", "sb200_ciphertext_load", "sb200_ciphertext_save", "sb200_secret_key_create",
     "sb200_secret_key_destroy", "sb200_decrypt", "sb200_decrypt_host", "sb200_invariant_noise_budget", "sb200_invariant_noise_budget_host", "sb200_encrypt_zero_symmetric", "sb200_public_key_create", "sb200_public_key_destroy", "sb200_encrypt_zero_asymmetric", "sb200_encrypt_zero_symmetric_prng", "sb200_encrypt_zero_asymmetric_prng", "sb200_encrypt_symmetric", "sb200_encrypt_asymmetric", "sb200_kswitch_key_generate", "sb200_public_key_generate", "sb200_ciphertext_save_seeded_size", "sb200_ciphertext_save_seeded",
@@ -140,6 +140,8 @@ def lib():
                                                C.POINTER(i32), _u64p, C.POINTER(vp), vp]
         L.sb200_multiply_plain_sum_host.argtypes = [vp, sz, sz, sz, sz, C.POINTER(sz), C.POINTER(vp), C.POINTER(sz), C.POINTER(vp), i32, i32,
                                                     C.POINTER(i32), _u64p, C.POINTER(vp)]
+        L.sb200_multiply_sum.argtypes = [vp, sz, sz, sz, sz, C.POINTER(vp), C.POINTER(vp), C.POINTER(i32), _u64p, C.POINTER(vp), vp]
+        L.sb200_multiply_sum_host.argtypes = [vp, sz, sz, sz, sz, C.POINTER(vp), C.POINTER(vp), C.POINTER(i32), _u64p, C.POINTER(vp)]
         L.sb200_sub_host.argtypes = [vp, sz, sz, sz, _u64p, _u64p, _u64p]
         L.sb200_negate_host.argtypes = [vp, sz, sz, sz, _u64p, _u64p]
         L.sb200_relinearize.argtypes = [vp, sz, sz, vp, vp, vp, vp]
@@ -565,6 +567,22 @@ class Context:
                                                    c_modes, None if f is None else _hp(f), p_outs))
         return outs
 
+    def multiply_sum(self, lhs, rhs, modes=None, factors=None):
+        """sb200_multiply_sum_host: lhs = M K arrays and rhs = K arrays, each [B][2][L][n]; modes / factors as in add_many.  Returns
+        M arrays [B][3][L][n]: output j = add_many over i of multiply(lhs[j K + i], rhs[i])."""
+        lhs = [np.ascontiguousarray(a, dtype=np.uint64) for a in lhs]
+        rhs = [np.ascontiguousarray(a, dtype=np.uint64) for a in rhs]
+        K = len(rhs)
+        M = len(lhs) // K if K else 0
+        B, _, L, n = rhs[0].shape if rhs else (0, 0, 0, 0)
+        _, c_modes, f = self._fold_args([3] * K, modes, factors)
+        outs = [np.zeros((B, 3, L, n), dtype=np.uint64) for _ in range(M)]
+        p_lhs = (C.c_void_p * max(len(lhs), 1))(*[a.ctypes.data for a in lhs])
+        p_rhs = (C.c_void_p * max(K, 1))(*[a.ctypes.data for a in rhs])
+        p_outs = (C.c_void_p * max(M, 1))(*[o.ctypes.data for o in outs])
+        _check(lib().sb200_multiply_sum_host(self.h, L, B, K, M, p_lhs, p_rhs, c_modes, None if f is None else _hp(f), p_outs))
+        return outs
+
     def multiply_plain(self, a, plain):
         """Evaluator.multiply_plain, NTT-form ciphertext [B][size][L][n] x NTT-form plaintexts [B][L][n]"""
         a, single = self._batched(a)
@@ -846,6 +864,16 @@ class Context:
         p_outs = (C.c_void_p * max(len(outs), 1))(*[_dp(t).value for t in outs])
         _check(lib().sb200_multiply_plain_sum(self.h, L, batch, len(cts), len(outs), c_sizes, p_cts, counts, p_plains, int(ct_is_ntt),
                                               int(plain_is_ntt), c_modes, None if f is None else _hp(f), p_outs, self._stream()))
+
+    def d_multiply_sum(self, lhs, rhs, outs, L, batch, modes=None, factors=None):
+        """sb200_multiply_sum on device tensors (or raw device pointers): lhs [M K] and rhs [K] of [batch][2][L][n], outs [M] of
+        [batch][3][L][n]; modes / factors as in add_many"""
+        _, c_modes, f = self._fold_args([3] * len(rhs), modes, factors)
+        p_lhs = (C.c_void_p * max(len(lhs), 1))(*[_dp(t).value for t in lhs])
+        p_rhs = (C.c_void_p * max(len(rhs), 1))(*[_dp(t).value for t in rhs])
+        p_outs = (C.c_void_p * max(len(outs), 1))(*[_dp(t).value for t in outs])
+        _check(lib().sb200_multiply_sum(self.h, L, batch, len(rhs), len(outs), p_lhs, p_rhs, c_modes, None if f is None else _hp(f), p_outs,
+                                        self._stream()))
 
     def d_multiply_sized(self, a, b, out, L, size_a, size_b, batch):
         _check(lib().sb200_multiply_sized(self.h, L, size_a, size_b, batch, _dp(a), _dp(b), _dp(out), self._stream()))

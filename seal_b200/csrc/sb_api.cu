@@ -1290,6 +1290,141 @@ namespace
         SB_CATCH
     }
 
+    // M outputs, each a fold over K terms of multiply(lhs_{j K + t}, rhs_t) of size-2 operands (op_multiply_sum); like PlainSum it has
+    // its own two drivers, multiply_sum_on_stream and multiply_sum_on_host.  The fold's modes and factors are AddMany's, checked by it
+    // on the products' size 3.
+    struct MultiplySum
+    {
+        size_t L, K, M;
+        const int *modes;
+        const u64 *factors;
+        AddMany fold(const size_t *sizes) const { return AddMany{ L, K, sizes, modes, factors }; }
+        bool scaled() const { return fold(nullptr).scaled(); }
+        // in the chain's order: multiply's checks of every term (the level, BFV's multiplication limit), then add_many's (modes)
+        void check(const Context &c, size_t batch) const
+        {
+            check_level(c, L, batch);
+            if (K == 0)
+                throw std::invalid_argument("encrypteds cannot be empty");
+            if (M == 0)
+                throw std::invalid_argument("outputs cannot be empty");
+            check_bfv_multiply_level(c, L);
+            const std::vector<size_t> sizes(K, 3);
+            fold(sizes.data()).check(c, batch);
+        }
+        // no output slab may overlap an operand's slab or another output's
+        void check_alias(const Context &c, size_t batch, const u64 *const *lhs, const u64 *const *rhs, const u64 *const *outs) const
+        {
+            const size_t poly = L * c.n, iw = batch * 2 * poly, ow = batch * 3 * poly;
+            auto overlap = [](const u64 *a, size_t na, const u64 *b, size_t nb) { return a < b + nb && b < a + na; };
+            for (size_t j = 0; j < M; j++)
+            {
+                for (size_t x = 0; x < M * K; x++)
+                    if (overlap(outs[j], ow, lhs[x], iw))
+                        throw std::invalid_argument("multiply_sum: an output slab must not overlap a left-hand operand");
+                for (size_t t = 0; t < K; t++)
+                    if (overlap(outs[j], ow, rhs[t], iw))
+                        throw std::invalid_argument("multiply_sum: an output slab must not overlap a right-hand operand");
+                for (size_t u = 0; u < j; u++)
+                    if (overlap(outs[j], ow, outs[u], ow))
+                        throw std::invalid_argument("multiply_sum: output slabs must not overlap");
+            }
+        }
+        void operator()(Context &c, size_t B, const u64 *const *lhs, const u64 *const *rhs, u64 *const *outs, cudaStream_t st) const
+        {
+            op_multiply_sum(c, L, B, K, M, lhs, rhs, modes, factors, outs, st);
+        }
+    };
+
+    // the pointer checks of a MultiplySum call: SB200_E_POINTER, or SB200_OK when every array and entry is present
+    int multiply_sum_pointers(const uint64_t *const *lhs, const uint64_t *const *rhs, uint64_t *const *outs, const MultiplySum &op)
+    {
+        SB_NEED(lhs);
+        SB_NEED(rhs);
+        SB_NEED(outs);
+        for (size_t x = 0; x < op.M * op.K; x++)
+            SB_NEED(lhs[x]);
+        for (size_t t = 0; t < op.K; t++)
+            SB_NEED(rhs[t]);
+        for (size_t j = 0; j < op.M; j++)
+            SB_NEED(outs[j]);
+        return SB200_OK;
+    }
+
+    int multiply_sum_on_stream(sb200_context *ctx, void *stream, size_t batch, const uint64_t *const *lhs, const uint64_t *const *rhs,
+                               uint64_t *const *outs, MultiplySum op)
+    {
+        if (const int e = multiply_sum_pointers(lhs, rhs, outs, op); e != SB200_OK)
+            return e;
+        SB_TRY
+        SB_ENTER_STREAM(ctx, stream)
+        op.check(c, batch);
+        if (op.scaled() && !op.factors)
+        {
+            g_last_error = "null pointer: h_factors";
+            return SB200_E_POINTER;
+        }
+        op.check_alias(c, batch, reinterpret_cast<const u64 *const *>(lhs), reinterpret_cast<const u64 *const *>(rhs),
+                       reinterpret_cast<const u64 *const *>(outs));
+        op(c, batch, reinterpret_cast<const u64 *const *>(lhs), reinterpret_cast<const u64 *const *>(rhs), reinterpret_cast<u64 *const *>(outs),
+           static_cast<cudaStream_t>(stream));
+        return SB200_OK;
+        SB_CATCH
+    }
+
+    // host buffers: the batch in chunks of the context's staging size, every operand and output of a chunk staged behind the previous one
+    int multiply_sum_on_host(sb200_context *ctx, size_t batch, const uint64_t *const *lhs, const uint64_t *const *rhs, uint64_t *const *outs,
+                             MultiplySum op)
+    {
+        if (const int e = multiply_sum_pointers(lhs, rhs, outs, op); e != SB200_OK)
+            return e;
+        SB_TRY
+        SB_ENTER(ctx)
+        op.check(c, batch);
+        if (op.scaled() && !op.factors)
+        {
+            g_last_error = "null pointer: h_factors";
+            return SB200_E_POINTER;
+        }
+        op.check_alias(c, batch, reinterpret_cast<const u64 *const *>(lhs), reinterpret_cast<const u64 *const *>(rhs),
+                       reinterpret_cast<const u64 *const *>(outs));
+        const size_t K = op.K, M = op.M, in_w = 2 * op.L * c.n, out_w = 3 * op.L * c.n;
+        const size_t per_ct = ((M * K + K) * in_w + M * out_w) * sizeof(u64);
+        const size_t chunk = std::max<size_t>(1, std::min(batch, c.host_stage_bytes / per_ct));
+        if (!c.io.s_comp)
+            c.io.s_comp = make_stream();
+        cudaStream_t st = c.io.s_comp.get();
+        StreamOrder order(c, st);
+        DevBuf<u64> &din = c.io.buf[0][0], &dout = c.io.buf[0][2];
+        din.grow(chunk * (M * K + K) * in_w);
+        dout.grow(chunk * M * out_w);
+        std::vector<const u64 *> dl(M * K), dr(K);
+        std::vector<u64 *> douts(M);
+        for (size_t b0 = 0; b0 < batch; b0 += chunk)
+        {
+            const size_t B = std::min(chunk, batch - b0);
+            u64 *d = din.get();
+            auto stage = [&](const uint64_t *h) {
+                cuda_check(cudaMemcpyAsync(d, h + b0 * in_w, B * in_w * sizeof(u64), cudaMemcpyHostToDevice, st), "H2D");
+                const u64 *p = d;
+                d += B * in_w;
+                return p;
+            };
+            for (size_t x = 0; x < M * K; x++)
+                dl[x] = stage(lhs[x]);
+            for (size_t t = 0; t < K; t++)
+                dr[t] = stage(rhs[t]);
+            for (size_t j = 0; j < M; j++)
+                douts[j] = dout.get() + j * B * out_w;
+            op(c, B, dl.data(), dr.data(), douts.data(), st);
+            for (size_t j = 0; j < M; j++)
+                cuda_check(cudaMemcpyAsync(outs[j] + b0 * out_w, douts[j], B * out_w * sizeof(u64), cudaMemcpyDeviceToHost, st), "D2H");
+            cuda_check(cudaStreamSynchronize(st), "synchronize");
+        }
+        return SB200_OK;
+        SB_CATCH
+    }
+
     // plain_count: one plaintext per ciphertext (batch) or one for the whole batch (1, a shared operand: Layout::shared_b).  The
     // older entry points, which take one plaintext per ciphertext, stay on the per-ciphertext path at every batch size (shared =
     // false, plain_count = batch); the _n entry points share the plaintext when plain_count = 1.
@@ -1712,6 +1847,17 @@ int sb200_multiply_plain_sum_host(sb200_context *ctx, size_t L, size_t batch, si
     return plain_sum_on_host(ctx, batch, cts, plains, outs,
                              PlainSum{ AddMany{ L, count, sizes, modes, reinterpret_cast<const u64 *>(factors) }, outputs, plain_counts,
                                        ct_is_ntt != 0, plain_is_ntt != 0 });
+}
+
+int sb200_multiply_sum(sb200_context *ctx, size_t L, size_t batch, size_t count, size_t outputs, const uint64_t *const *lhs,
+                       const uint64_t *const *rhs, const int *modes, const uint64_t *factors, uint64_t *const *outs, void *stream)
+{
+    return multiply_sum_on_stream(ctx, stream, batch, lhs, rhs, outs, MultiplySum{ L, count, outputs, modes, reinterpret_cast<const u64 *>(factors) });
+}
+int sb200_multiply_sum_host(sb200_context *ctx, size_t L, size_t batch, size_t count, size_t outputs, const uint64_t *const *lhs,
+                            const uint64_t *const *rhs, const int *modes, const uint64_t *factors, uint64_t *const *outs)
+{
+    return multiply_sum_on_host(ctx, batch, lhs, rhs, outs, MultiplySum{ L, count, outputs, modes, reinterpret_cast<const u64 *>(factors) });
 }
 
 int sb200_multiply_plain(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, const uint64_t *plain, uint64_t *out,

@@ -183,6 +183,14 @@ namespace sb
     void op_multiply_plain_sum(Context &c, size_t L, size_t batch, size_t K, size_t M, const size_t *sizes, const u64 *const *cts,
                                const size_t *plain_counts, const u64 *const *plains, bool ct_ntt, bool plain_ntt, const int *modes,
                                const u64 *factors, u64 *const *outs, cudaStream_t st);
+    // sums of ciphertext products (sb_plainsum.cu, sb200_multiply_sum): outs[j] [B][3][L][n] = the fold (modes / factors as
+    // op_add_many) over t < K of multiply(lhs[j K + t], rhs[t]), every operand [B][2][L][n].  CKKS and BGV: one multiply_sum_kernel
+    // pass, output tiles of kMultiplySumTile, the 128-bit sums reduced once per window of at most kMultiplySumWindow terms.  BFV:
+    // op_bfv_multiply into the aux arena, a chunk of terms at a time, each chunk folded into the output by op_add_many.
+    constexpr int kMultiplySumWindow = 128;
+    constexpr int kMultiplySumTile = 2; // 72 / 102 / 178 registers at tiles of 1 / 2 / 4; a tile of 4 ran slower (DESIGN 3.4)
+    void op_multiply_sum(Context &c, size_t L, size_t batch, size_t K, size_t M, const u64 *const *lhs, const u64 *const *rhs, const int *modes,
+                         const u64 *factors, u64 *const *outs, cudaStream_t st);
     // Plaintext operations take one plaintext per ciphertext, or (shared) one plaintext for the whole batch.
     // NTT-form plaintexts [B][L][n] or [L][n]: multiply_plain of NTT-form ciphertexts; CKKS add_plain / sub_plain (c_0 only)
     void op_multiply_plain(Context &c, size_t L, size_t size, size_t batch, bool shared, const u64 *a, const u64 *plain, u64 *out,
