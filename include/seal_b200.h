@@ -331,6 +331,28 @@ int sb200_relinearize_sized(sb200_context *ctx, size_t L, size_t size, size_t ba
  * rotate_rows / rotate_vector(step) = apply_galois(sb200_galois_elt_from_step(step)) with that element's key. */
 int sb200_apply_galois(sb200_context *ctx, size_t L, size_t batch, const uint64_t *d_in2, uint32_t galois_elt,
                        const sb200_kswitch_key *galois_key, uint64_t *d_out2, void *stream);
+/* d_out2 = d_addend2 + apply_galois(d_in2): Evaluator::apply_galois_inplace followed by Evaluator::add_inplace (evaluator.cpp:2384-2502,
+ * :155-261) on a copy of the input, with the addition in the key switch's last pass (no copy, no add pass; the same words).  All
+ * three slabs are [batch][2][L][n] in the scheme's form (BFV coefficient, CKKS / BGV NTT).  d_out2 may be d_addend2 (accumulate
+ * rotated terms into one destination) and d_addend2 may be d_in2 (y + rotate(y)); d_out2 == d_in2 is rejected
+ * (SB200_E_INVALID_ARG).  Other errors as sb200_apply_galois's, plus a NULL d_addend2 (SB200_E_POINTER); all before the first
+ * launch, so the output is unchanged on error.  The _host form: h_a is the input, h_b the addend, h_out2 may be h_b. */
+int sb200_apply_galois_add(sb200_context *ctx, size_t L, size_t batch, const uint64_t *d_in2, uint32_t galois_elt,
+                           const sb200_kswitch_key *galois_key, const uint64_t *d_addend2, uint64_t *d_out2, void *stream);
+int sb200_apply_galois_add_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *h_a, uint32_t galois_elt,
+                                const sb200_kswitch_key *galois_key, const uint64_t *h_b, uint64_t *h_out2);
+/* Sums of rotations: y_0 = in, y_{j+1} = y_j + apply_galois(y_j, galois_elts[j]) with galois_keys[j] (sb200_apply_galois_add with
+ * the addend equal to the input), d_out2 = y_steps.  With the elements of steps s, 2s, 4s, ... this is the slot sum
+ * x[i] + x[i + s] + ... of rotate_rows / rotate_vector; it replaces the reference's loop of Evaluator::rotate_rows_inplace /
+ * rotate_vector_inplace (evaluator.h:1072-1251, evaluator.cpp:2504-2559) on a copy and add_inplace.  d_out2 may be d_in2; steps = 0 copies.  Each chunk of
+ * the key-switching scratch (SB200_LIMIT_SCRATCH_BYTES, SB200_LIMIT_KS_CHUNK) runs every step, through one chunk-sized temporary.
+ * Errors, all before the first launch (the output is unchanged): every element and key checked as by sb200_apply_galois; a NULL
+ * galois_elts, galois_keys or entry (SB200_E_POINTER).  The _host form stages each chunk of SB200_LIMIT_HOST_STAGE_BYTES once for
+ * the whole chain. */
+int sb200_rotate_sum(sb200_context *ctx, size_t L, size_t batch, const uint64_t *d_in2, size_t steps, const uint32_t *galois_elts,
+                     const sb200_kswitch_key *const *galois_keys, uint64_t *d_out2, void *stream);
+int sb200_rotate_sum_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *h_in2, size_t steps, const uint32_t *galois_elts,
+                          const sb200_kswitch_key *const *galois_keys, uint64_t *h_out2);
 
 /* ---- host-buffer variants: H2D copy, operation, D2H copy, synchronise (the plugin-facing end-to-end path) ---- */
 int sb200_ntt_forward_host(sb200_context *ctx, size_t L, size_t size, size_t batch, uint64_t *h_data);

@@ -19,6 +19,7 @@
 #include <cmath>
 #include <cstring>
 #include <deque>
+#include <limits>
 #include <map>
 #include <mutex>
 #include <stdexcept>
@@ -1406,10 +1407,43 @@ namespace seal_b200
         {
             complex_conjugate_batch(encrypted, galois_keys);
         }
+        // Sums of rotations.  apply_galois_add_inplace: destination += apply_galois(encrypted), the words of
+        //     t = encrypted (a copy); apply_galois_inplace(t, galois_elt, galois_keys); add_inplace(destination, t);
+        // with the addition in the key switch's last pass (sb200_apply_galois_add): no copy and no add pass.  destination may be
+        // encrypted.  The chain's checks and messages run first, apply_galois_inplace's then add_inplace's; BGV operands with
+        // different correction factors, or a destination of another size than 2, take the chain itself.
+        void apply_galois_add_inplace(CiphertextBatch &destination, const CiphertextBatch &encrypted, std::uint32_t galois_elt,
+                                      const seal::GaloisKeys &galois_keys) const
+        {
+            apply_galois_add_batch(destination, encrypted, galois_elt, galois_keys);
+        }
+        void apply_galois_add_inplace(CiphertextBatch &destination, const CiphertextBatch &encrypted, std::uint32_t galois_elt,
+                                      const DeviceGaloisKeys &galois_keys) const
+        {
+            apply_galois_add_batch(destination, encrypted, galois_elt, galois_keys);
+        }
+        // rotate_sum_inplace: slot i becomes the sum over m < count of slot i + m step (cyclic within a row), the words of
+        //     for (j = 0; (1 << j) < count; j++) { t = encrypted; rotate_X_inplace(t, step << j, galois_keys); add_inplace(encrypted, t); }
+        // with rotate_X = rotate_vector (CKKS) or rotate_rows (BFV / BGV), in one sb200_rotate_sum call.  count is a power of two
+        // (1 leaves the batch unchanged); step = 0 throws std::invalid_argument.  Scheme and batching errors, "step count too large"
+        // and missing keys throw what the chain throws, before anything is written; when a step's key is absent but the reference's
+        // NAF decomposition of it is covered by other keys, the chain itself runs.  No key of the call is evicted from the key cache
+        // while it runs.
+        // Every slot of a BFV batch (n slots, two rows of n / 2): rotate_sum_inplace(y, 1, n / 2, gk) sums each row, then
+        // apply_galois_add_inplace(y, y, 2 n - 1, gk) adds the other row (element 2n - 1 swaps the rows, rotate_columns).
+        void rotate_sum_inplace(CiphertextBatch &encrypted, int step, std::size_t count, const seal::GaloisKeys &galois_keys) const
+        {
+            rotate_sum_batch(encrypted, step, count, galois_keys);
+        }
+        void rotate_sum_inplace(CiphertextBatch &encrypted, int step, std::size_t count, const DeviceGaloisKeys &galois_keys) const
+        {
+            rotate_sum_batch(encrypted, step, count, galois_keys);
+        }
 
     private:
+        // apply_galois_inplace's checks (evaluator.cpp:2384-2430), in its order, up to the key lookup
         template <class GaloisKeys>
-        void apply_galois_batch(CiphertextBatch &encrypted, std::uint32_t galois_elt, const GaloisKeys &galois_keys) const
+        void check_apply_galois(const CiphertextBatch &encrypted, std::uint32_t galois_elt, const GaloisKeys &galois_keys) const
         {
             owned(encrypted);
             if (galois_keys.parms_id() != context_.key_parms_id())
@@ -1421,6 +1455,96 @@ namespace seal_b200
             if (encrypted.size_ != 2)
                 throw std::invalid_argument("encrypted size must be 2");
             check_keyswitch_form(encrypted.ntt_);
+        }
+        template <class GaloisKeys>
+        void apply_galois_add_batch(CiphertextBatch &destination, const CiphertextBatch &encrypted, std::uint32_t galois_elt,
+                                    const GaloisKeys &galois_keys) const
+        {
+            check_apply_galois(encrypted, galois_elt, galois_keys);
+            {
+                std::lock_guard<std::mutex> lock(mu_);
+                sb200_kswitch_key *key = key_for(galois_keys, seal::GaloisKeys::get_index(galois_elt), encrypted.L_);
+                const Fold f = plan_fold({ &destination, &encrypted }, { SB200_FOLD_ADD }); // add_inplace(destination, t)
+                if (f.factors.empty() && destination.size_ == 2)
+                {
+                    const bool same = &destination == &encrypted; // out must not be the input: through the result slab
+                    std::uint64_t *out = same ? out_slab(destination.batch_ * destination.words_per_ciphertext(), destination) : destination.d_;
+                    check(sb200_apply_galois_add(ctx_, encrypted.L_, encrypted.batch_, encrypted.d_, galois_elt, key, destination.d_, out, nullptr));
+                    if (same)
+                        adopt(destination);
+                    return;
+                }
+            }
+            CiphertextBatch t;
+            copy(encrypted, t);
+            apply_galois_batch(t, galois_elt, galois_keys);
+            add_inplace(destination, t);
+        }
+        template <class GaloisKeys>
+        void rotate_sum_batch(CiphertextBatch &encrypted, int step, std::size_t count, const GaloisKeys &galois_keys) const
+        {
+            if (step == 0)
+                throw std::invalid_argument("step must be nonzero");
+            if (count == 0 || (count & (count - 1)))
+                throw std::invalid_argument("count must be a power of two");
+            if (count == 1)
+                return;
+            const bool ckks = scheme_ == seal::scheme_type::ckks;
+            if (!ckks && scheme_ != seal::scheme_type::bfv && scheme_ != seal::scheme_type::bgv)
+                throw std::logic_error("unsupported scheme");
+            owned(encrypted);
+            auto cd = context_.get_context_data(encrypted.parms_id_);
+            if (!cd->qualifiers().using_batching)
+                throw std::logic_error("encryption parameters do not support batching");
+            if (galois_keys.parms_id() != context_.key_parms_id())
+                throw std::invalid_argument("galois_keys is not valid for encryption parameters");
+            std::vector<std::uint32_t> elts;
+            bool naf = false;
+            for (std::size_t j = 0; (std::size_t(1) << j) < count; j++)
+            {
+                const long long s = static_cast<long long>(step) * (1ll << j);
+                if (s > std::numeric_limits<int>::max() || s < std::numeric_limits<int>::min())
+                    throw std::invalid_argument("step count too large");
+                const std::uint32_t elt = cd->galois_tool()->get_elt_from_step(static_cast<int>(s)); // "step count too large"
+                if (!galois_keys.has_key(elt))
+                {
+                    if (seal::util::naf(static_cast<int>(s)).size() == 1)
+                        throw std::invalid_argument("Galois key not present");
+                    naf = true;
+                }
+                elts.push_back(elt);
+            }
+            if (naf)
+            {
+                for (std::size_t j = 0; j < elts.size(); j++)
+                {
+                    CiphertextBatch t;
+                    copy(encrypted, t);
+                    rotate_batch(t, static_cast<int>(static_cast<long long>(step) * (1ll << j)), galois_keys);
+                    add_inplace(encrypted, t);
+                }
+                return;
+            }
+            check_apply_galois(encrypted, elts[0], galois_keys);
+            std::lock_guard<std::mutex> lock(mu_);
+            std::vector<const sb200_kswitch_key *> keys;
+            struct Unpin // the keys of this call stay in the cache until it returns
+            {
+                std::vector<const sb200_kswitch_key *> &pinned;
+                ~Unpin() { pinned.clear(); }
+            } unpin{ pinned_ };
+            for (std::uint32_t elt : elts)
+            {
+                sb200_kswitch_key *k = key_for(galois_keys, seal::GaloisKeys::get_index(elt), encrypted.L_);
+                pinned_.push_back(k);
+                keys.push_back(k);
+            }
+            check(sb200_rotate_sum(ctx_, encrypted.L_, encrypted.batch_, encrypted.d_, elts.size(), elts.data(), keys.data(), encrypted.d_, nullptr));
+        }
+        template <class GaloisKeys>
+        void apply_galois_batch(CiphertextBatch &encrypted, std::uint32_t galois_elt, const GaloisKeys &galois_keys) const
+        {
+            check_apply_galois(encrypted, galois_elt, galois_keys);
             std::lock_guard<std::mutex> lock(mu_);
             sb200_kswitch_key *key = key_for(galois_keys, seal::GaloisKeys::get_index(galois_elt), encrypted.L_);
             std::uint64_t *out = out_slab(encrypted.batch_ * encrypted.words_per_ciphertext(), encrypted);
@@ -1895,7 +2019,8 @@ namespace seal_b200
             {
                 auto victim = keys_.end();
                 for (auto it = keys_.begin(); it != keys_.end(); ++it)
-                    if (it->second.handle != keep && (victim == keys_.end() || it->second.last_use < victim->second.last_use))
+                    if (it->second.handle != keep && std::find(pinned_.begin(), pinned_.end(), it->second.handle) == pinned_.end() &&
+                        (victim == keys_.end() || it->second.last_use < victim->second.last_use))
                         victim = it;
                 if (victim == keys_.end())
                     break;
@@ -2831,6 +2956,7 @@ namespace seal_b200
         sb200_context *ctx_ = nullptr;
         mutable std::mutex mu_;
         mutable std::map<std::uint64_t, KeyEntry> keys_;
+        mutable std::vector<const sb200_kswitch_key *> pinned_; // keys of a running call that evict() must keep (rotate_sum_inplace)
         mutable std::size_t key_cache_bytes_ = 0, key_cache_limit_ = std::size_t(24) << 30;
         mutable std::uint64_t key_clock_ = 0;
         mutable CiphertextBatch tmp_; // result slab of layout-changing batch operations

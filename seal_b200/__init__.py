@@ -36,7 +36,8 @@ SYMBOLS = [
     "sb200_multiply_plain_n", "sb200_multiply_plain_coeff_n", "sb200_add_plain_coeff_n", "sb200_add_plain_ntt", "sb200_multiply_plain_n_host",
     "sb200_multiply_plain_coeff_n_host", "sb200_add_plain_coeff_n_host", "sb200_add_plain_ntt_host",
     "sb200_add_many", "sb200_add_many_host", "sb200_multiply_plain_sum", "sb200_multiply_plain_sum_host", "sb200_multiply_sum", "sb200_multiply_sum_host", "sb200_relinearize_host", "sb200_multiply_relinearize_host", "sb200_rescale_to_next_host",
-    "sb200_mod_switch_to_next_host", "sb200_apply_galois_host", "sb200_get_parms_id", "sb200_ciphertext_inspect",
+    "sb200_mod_switch_to_next_host", "sb200_apply_galois_host", "sb200_apply_galois_add", "sb200_apply_galois_add_host",
+    "sb200_rotate_sum", "sb200_rotate_sum_host", "sb200_get_parms_id", "sb200_ciphertext_inspect",
     "sb200_ciphertext_save_size", "sb200_ciphertext_load", "sb200_ciphertext_save", "sb200_secret_key_create",
     "sb200_secret_key_destroy", "sb200_decrypt", "sb200_decrypt_host", "sb200_invariant_noise_budget", "sb200_invariant_noise_budget_host", "sb200_encrypt_zero_symmetric", "sb200_public_key_create", "sb200_public_key_destroy", "sb200_encrypt_zero_asymmetric", "sb200_encrypt_zero_symmetric_prng", "sb200_encrypt_zero_asymmetric_prng", "sb200_encrypt_symmetric", "sb200_encrypt_asymmetric", "sb200_kswitch_key_generate", "sb200_public_key_generate", "sb200_ciphertext_save_seeded_size", "sb200_ciphertext_save_seeded",
     "sb200_public_key_generate_seeded", "sb200_kswitch_keys_save_seeded_size", "sb200_kswitch_keys_generate_seeded", "sb200_ckks_encode", "sb200_ckks_decode", "sb200_ckks_encode_host", "sb200_ckks_decode_host",
@@ -159,6 +160,10 @@ def lib():
         L.sb200_rescale_to_next_host.argtypes = [vp, sz, sz, _u64p, _u64p]
         L.sb200_mod_switch_to_next_host.argtypes = [vp, sz, sz, _u64p, _u64p]
         L.sb200_apply_galois_host.argtypes = [vp, sz, sz, _u64p, u32, vp, _u64p]
+        L.sb200_apply_galois_add.argtypes = [vp, sz, sz, vp, u32, vp, vp, vp, vp]
+        L.sb200_apply_galois_add_host.argtypes = [vp, sz, sz, _u64p, u32, vp, _u64p, _u64p]
+        L.sb200_rotate_sum.argtypes = [vp, sz, sz, vp, sz, C.POINTER(u32), C.POINTER(vp), vp, vp]
+        L.sb200_rotate_sum_host.argtypes = [vp, sz, sz, _u64p, sz, C.POINTER(u32), C.POINTER(vp), _u64p]
         L.sb200_rescale_to_next_sized_host.argtypes = [vp, sz, sz, sz, _u64p, _u64p]
         L.sb200_mod_switch_to_next_sized_host.argtypes = [vp, sz, sz, sz, _u64p, _u64p]
         L.sb200_relinearize_sized_host.argtypes = [vp, sz, sz, sz, _u64p, vp, _u64p]
@@ -216,6 +221,15 @@ def ciphertext_inspect(stream):
 def _hp(a):
     assert isinstance(a, np.ndarray) and a.dtype == np.uint64 and a.flags["C_CONTIGUOUS"], "need C-contiguous uint64"
     return a.ctypes.data_as(_u64p)
+
+
+def _rotate_sum_args(galois_elts, keys):
+    """the element and key-handle arrays of a rotate_sum call (a None key stays a NULL entry)"""
+    assert len(galois_elts) == len(keys), "one key per Galois element"
+    m = len(galois_elts)
+    c_elts = (C.c_uint32 * max(m, 1))(*[int(e) for e in galois_elts])
+    c_keys = (C.c_void_p * max(m, 1))(*[None if k is None else k.h for k in keys])
+    return c_elts, c_keys
 
 
 def _dp(t):
@@ -807,6 +821,25 @@ class Context:
         _check(lib().sb200_apply_galois_host(self.h, L, B, _hp(a), galois_elt, key.h, _hp(out)))
         return out[0] if single else out
 
+    def apply_galois_add(self, a, galois_elt, key, b, out=None):
+        """sb200_apply_galois_add_host: b + apply_galois(a), a and b [B][2][L][n]; out (may be b) or a fresh array"""
+        a, single = self._batched(a)
+        b, _ = self._batched(b)
+        B, _, L, n = a.shape
+        if out is None:
+            out = np.zeros((B, 2, L, n), dtype=np.uint64)
+        _check(lib().sb200_apply_galois_add_host(self.h, L, B, _hp(a), galois_elt, None if key is None else key.h, _hp(b), _hp(out)))
+        return out[0] if single else out
+
+    def rotate_sum(self, a, galois_elts, keys):
+        """sb200_rotate_sum_host: y_0 = a, y_{j+1} = y_j + apply_galois(y_j, galois_elts[j]) with keys[j]; returns y_steps"""
+        a, single = self._batched(a)
+        B, _, L, n = a.shape
+        out = np.zeros((B, 2, L, n), dtype=np.uint64)
+        c_elts, c_keys = _rotate_sum_args(galois_elts, keys)
+        _check(lib().sb200_rotate_sum_host(self.h, L, B, _hp(a), len(galois_elts), c_elts, c_keys, _hp(out)))
+        return out[0] if single else out
+
     def rotate(self, a, step, key):
         """rotate_rows (BFV) / rotate_vector (CKKS) by `step` with the Galois key of that step's element"""
         return self.apply_galois(a, self.galois_elt_from_step(step), key)
@@ -1085,3 +1118,13 @@ class Context:
 
     def d_apply_galois(self, in2, galois_elt, key, out2, L, batch):
         _check(lib().sb200_apply_galois(self.h, L, batch, _dp(in2), galois_elt, key.h, _dp(out2), self._stream()))
+
+    def d_apply_galois_add(self, in2, galois_elt, key, addend2, out2, L, batch):
+        """sb200_apply_galois_add: out2 = addend2 + apply_galois(in2); out2 may be addend2, addend2 may be in2"""
+        _check(lib().sb200_apply_galois_add(self.h, L, batch, _dp(in2), galois_elt, None if key is None else key.h,
+                                            None if addend2 is None else _dp(addend2), _dp(out2), self._stream()))
+
+    def d_rotate_sum(self, in2, galois_elts, keys, out2, L, batch):
+        """sb200_rotate_sum: the chain y_{j+1} = y_j + apply_galois(y_j, galois_elts[j]) from in2, y_steps to out2 (may be in2)"""
+        c_elts, c_keys = _rotate_sum_args(galois_elts, keys)
+        _check(lib().sb200_rotate_sum(self.h, L, batch, _dp(in2), len(galois_elts), c_elts, c_keys, _dp(out2), self._stream()))

@@ -7,6 +7,7 @@
 #include "sb_engine.cuh"
 #include <random>
 #include <algorithm>
+#include <array>
 #include <cctype>
 #include <cstdio>
 #include <cstring>
@@ -856,6 +857,7 @@ namespace
         const char *alias = nullptr;   // device slabs: the error when the output aliases an input (nullptr = allowed)
         size_t out_unit = sizeof(u64); // bytes of one output word (the noise budget returns one int per ciphertext)
         bool shared_b = false;         // input b is one operand of b words for the whole batch (a plaintext shared by every ciphertext)
+        bool alias_b_ok = false;       // with alias set: the output may still be input b (an addend read and written by one thread)
     };
 
     struct HostPipe
@@ -1591,6 +1593,61 @@ namespace
         }
     };
 
+    // out = b + apply_galois(a); out may be b, b may be a
+    struct ApplyGaloisAdd
+    {
+        size_t L;
+        uint32_t elt;
+        const KSwitchKey &key;
+        void check(const Context &c, size_t batch) const
+        {
+            check_level(c, L, batch);
+            check_rotate_sum_args(c, L, 1, &elt, std::array<const KSwitchKey *, 1>{ &key }.data());
+        }
+        Layout layout(const Context &c) const
+        {
+            return { 2 * L * c.n, 2 * L * c.n, 2 * L * c.n, false, "apply_galois_add: in and out must not alias", sizeof(u64), false, true };
+        }
+        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *b, u64 *out, cudaStream_t st) const
+        {
+            op_apply_galois_add(c, L, B, a, elt, key, b, out, st);
+        }
+    };
+
+    // out = y_steps, y_{j+1} = y_j + apply_galois(y_j, elts[j]); out may be a.  A host chunk runs the whole chain once staged
+    struct RotateSum
+    {
+        size_t L, steps;
+        const uint32_t *elts;
+        const KSwitchKey *const *keys;
+        void check(const Context &c, size_t batch) const
+        {
+            check_level(c, L, batch);
+            check_rotate_sum_args(c, L, steps, elts, keys);
+        }
+        Layout layout(const Context &c) const { return { 2 * L * c.n, 0, 2 * L * c.n }; }
+        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
+        {
+            op_rotate_sum(c, L, B, a, steps, elts, keys, out, st);
+        }
+    };
+
+    // the key handles of a rotate_sum call, after the pointer checks (SB200_E_POINTER on a NULL array or entry)
+    int rotate_sum_keys(size_t steps, const uint32_t *elts, const sb200_kswitch_key *const *keys, std::vector<const KSwitchKey *> &out)
+    {
+        if (steps)
+        {
+            SB_NEED(elts);
+            SB_NEED(keys);
+        }
+        for (size_t j = 0; j < steps; j++)
+        {
+            SB_NEED(keys[j]);
+            out.push_back(&keys[j]->k);
+        }
+        return SB200_OK;
+    }
+
     struct ModSwitch // rescale_to_next (CKKS) or mod_switch_to_next of ciphertexts of any size: L primes -> L - 1
     {
         bool rescale;
@@ -1712,7 +1769,7 @@ namespace
         SB_ENTER_STREAM(ctx, stream)
         op.check(c, batch);
         const Layout w = op.layout(c);
-        if (w.alias && (out == a || out == b))
+        if (w.alias && (out == a || (out == b && !w.alias_b_ok)))
             throw std::invalid_argument(w.alias);
         if (w.shared_b && out == b)
             throw std::invalid_argument("the shared plaintext must not alias the output slab");
@@ -2057,6 +2114,36 @@ int sb200_apply_galois_host(sb200_context *ctx, size_t L, size_t batch, const ui
 {
     SB_NEED(key);
     return on_host(ctx, batch, in2, nullptr, out2, ApplyGalois{ L, elt, key->k });
+}
+int sb200_apply_galois_add(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, uint32_t elt, const sb200_kswitch_key *key,
+                           const uint64_t *addend2, uint64_t *out2, void *stream)
+{
+    SB_NEED(key);
+    SB_NEED(addend2);
+    return on_stream(ctx, stream, batch, in2, addend2, out2, ApplyGaloisAdd{ L, elt, key->k });
+}
+int sb200_apply_galois_add_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *a, uint32_t elt, const sb200_kswitch_key *key,
+                                const uint64_t *b, uint64_t *out2)
+{
+    SB_NEED(key);
+    SB_NEED(b);
+    return on_host(ctx, batch, a, b, out2, ApplyGaloisAdd{ L, elt, key->k });
+}
+int sb200_rotate_sum(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, size_t steps, const uint32_t *elts,
+                     const sb200_kswitch_key *const *keys, uint64_t *out2, void *stream)
+{
+    std::vector<const KSwitchKey *> k;
+    if (int e = rotate_sum_keys(steps, elts, keys, k))
+        return e;
+    return on_stream(ctx, stream, batch, in2, nullptr, out2, RotateSum{ L, steps, elts, k.data() });
+}
+int sb200_rotate_sum_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, size_t steps, const uint32_t *elts,
+                          const sb200_kswitch_key *const *keys, uint64_t *out2)
+{
+    std::vector<const KSwitchKey *> k;
+    if (int e = rotate_sum_keys(steps, elts, keys, k))
+        return e;
+    return on_host(ctx, batch, in2, nullptr, out2, RotateSum{ L, steps, elts, k.data() });
 }
 
 // ---- wire format (SURVEY 8f rank 3): Ciphertext::save / load, compr_mode none, between byte streams and device slabs ----

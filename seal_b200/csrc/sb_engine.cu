@@ -1894,6 +1894,7 @@ namespace sb
     // (4b) per data prime: NTT((u mod q_i) - (half mod q_i)), subtract from the accumulated component, scale by
     //      q_top^-1 and add into the ciphertext; evaluator.cpp:2819-2864 (CKKS branch), rns.cpp:863-900 (rescale).
     //      rows = (b, c, i), i < Lout
+    template <class Base = BaseSrc>
     struct OpModDownFwd
     {
         const u64 *U;            // [B][2][n]: (INTT(top component) + half) mod q_top
@@ -1903,7 +1904,7 @@ namespace sb
         u64 *out;                // out + b*o_bs + c*o_ps + i*n
         long long o_bs, o_ps;
         const Tw *inv_top;       // q_top^-1 mod q_i, i < Lout
-        BaseSrc base;
+        Base base;
         u64 q_top;
         int logn, Lout;
         __device__ __forceinline__ bool skip(int) const { return false; }
@@ -1926,7 +1927,7 @@ namespace sb
             u64 x = X[b * x_bs + c * x_ps + (static_cast<long long>(i) << logn) + idx];
             u64 r = mul_shoup(x + P.q - t, inv_top[i], P.q);
             r = csub(r + base.get(b, c, i, idx, P.q), P.q);
-            out[b * o_bs + c * o_ps + (static_cast<long long>(i) << logn) + idx] = r;
+            out[b * o_bs + c * o_ps + (static_cast<long long>(i) << logn) + idx] = plus_addend(base, b, c, i, logn, idx, r, P.q);
         }
         __device__ __forceinline__ void store8(int row, int idx0, u64 (&a)[8], const PrimeDev &P) const
         {
@@ -1954,6 +1955,11 @@ namespace sb
                     r0 = csub(r0 + base.get(b, c, i, idx0 + 2 * h, P.q), P.q);
                     r1 = csub(r1 + base.get(b, c, i, idx0 + 2 * h + 1, P.q), P.q);
                 }
+                if constexpr (Base::kAddend)
+                {
+                    const ulonglong2 av = reinterpret_cast<const ulonglong2 *>(base.arow(b, c, i, logn) + idx0)[h];
+                    r0 = csub(r0 + av.x, P.q), r1 = csub(r1 + av.y, P.q);
+                }
                 op_[h] = make_ulonglong2(r0, r1);
             }
         }
@@ -1961,29 +1967,30 @@ namespace sb
 
     // BGV: the correction polynomial is delta = (U mod q_i) + (K mod q_i) * (q_top mod q_i) instead of (u mod q_i) - half
     // (evaluator.cpp:2762-2805, rns.cpp:1216-1235); the transform and the epilogue are the ones above.
-    struct OpModDownFwdBgv : OpModDownFwd
+    template <class Base = BaseSrc>
+    struct OpModDownFwdBgv : OpModDownFwd<Base>
     {
         const u64 *K;            // [B][2][n]: -U * q_top^-1 mod t
         const Tw *qtop_mod;      // q_top mod q_i, i < Lout
         u64 t;
         __device__ __forceinline__ u64 load1(int row, int idx, const PrimeDev &P) const
         {
-            const long long e = (static_cast<long long>(row / Lout) << logn) + idx;
-            u64 u = U[e], kk = K[e];
-            if (q_top > P.q)
+            const long long e = (static_cast<long long>(row / this->Lout) << this->logn) + idx;
+            u64 u = this->U[e], kk = K[e];
+            if (this->q_top > P.q)
                 u = barrett64(u, P.q, P.ratio_hi);
             if (t > P.q)
                 kk = barrett64(kk, P.q, P.ratio_hi);
-            return u + mul_shoup(kk, qtop_mod[row % Lout], P.q); // < 2q
+            return u + mul_shoup(kk, qtop_mod[row % this->Lout], P.q); // < 2q
         }
     };
 
     // coefficient-form mod-down (BFV): evaluator.cpp:2819-2864 (bfv branch) and rns.cpp:789-828 (mod_switch).
     // ADD_HALF: U holds the raw top component (mod_switch); otherwise U already includes + half (key switch).
-    template <bool ADD_HALF>
+    template <bool ADD_HALF, class Base = BaseSrc>
     __global__ void __launch_bounds__(256) moddown_coeff_kernel(const u64 *__restrict__ U, long long u_bs, long long u_ps, const u64 *X,
                                                                  long long x_bs, long long x_ps, u64 *out, long long o_bs, long long o_ps,
-                                                                 const Tw *__restrict__ inv_top, BaseSrc base, u64 q_top,
+                                                                 const Tw *__restrict__ inv_top, Base base, u64 q_top,
                                                                  const PrimeDev *__restrict__ primes, int logn, int Lout, long long total)
     {
         long long e = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; // over B*2*Lout*n
@@ -2004,7 +2011,7 @@ namespace sb
         u64 x = X[b * x_bs + c * x_ps + (static_cast<long long>(i) << logn) + idx];
         u64 r = mul_shoup(x + P.q2 - t, inv_top[i], P.q);
         r = csub(r + base.get(b, c, i, idx, P.q), P.q);
-        out[b * o_bs + c * o_ps + (static_cast<long long>(i) << logn) + idx] = r;
+        out[b * o_bs + c * o_ps + (static_cast<long long>(i) << logn) + idx] = plus_addend(base, b, c, i, logn, idx, r, P.q);
     }
 
     struct KsScratch
@@ -2194,7 +2201,8 @@ namespace sb
 
     // ct[b] (= base) += key-switch(target[b]) for a chunk of B ciphertexts; writes out[b][2][L][n].
     //   out_bs = words between consecutive ciphertexts of out (0: the dense [B][2][L][n] slab)
-    static void key_switch_chunk(Context &c, size_t L, size_t B, const KsScratch &s, Src target, const KSwitchKey &key, BaseSrc base,
+    template <class Base>
+    static void key_switch_chunk(Context &c, size_t L, size_t B, const KsScratch &s, Src target, const KSwitchKey &key, Base base,
                                  u64 *out, cudaStream_t st, long long out_bs = 0)
     {
         const int n = static_cast<int>(c.n), Li = static_cast<int>(L), ki = static_cast<int>(c.k);
@@ -2284,13 +2292,13 @@ namespace sb
         const long long o_ps = static_cast<long long>(L) * n, o_bs = out_bs ? out_bs : 2 * o_ps;
         if (bgv)
         {
-            OpModDownFwdBgv op{ { s.U, s.Pp, pp_bs, pp_ps, s.T, out, o_bs, o_ps, inv_top, base, c.q[c.k - 1], c.logn, Li },
-                                s.K, c.d_qmod.get() + (c.k - 1) * c.k, c.t };
+            OpModDownFwdBgv<Base> op{ { s.U, s.Pp, pp_bs, pp_ps, s.T, out, o_bs, o_ps, inv_top, base, c.q[c.k - 1], c.logn, Li },
+                                      s.K, c.d_qmod.get() + (c.k - 1) * c.k, c.t };
             cuda_check(launch_ntt_fwd(op, static_cast<int>(B * 2 * L), c.logn, c.d_primes.get(), st, c.stats, "ks_moddown_ntt", -1, c.fast_q), "ks moddown ntt");
         }
         else if (ntt_in)
         {
-            OpModDownFwd op{ s.U, s.Pp, pp_bs, pp_ps, s.T, out, o_bs, o_ps, inv_top, base, c.q[c.k - 1], c.logn, Li };
+            OpModDownFwd<Base> op{ s.U, s.Pp, pp_bs, pp_ps, s.T, out, o_bs, o_ps, inv_top, base, c.q[c.k - 1], c.logn, Li };
             cuda_check(launch_ntt_fwd(op, static_cast<int>(B * 2 * L), c.logn, c.d_primes.get(), st, c.stats, "ks_moddown_ntt", -1, c.fast_q), "ks moddown ntt");
         }
         else
@@ -2299,7 +2307,7 @@ namespace sb
             cuda_check(launch_ntt_inv(op, static_cast<int>(B * 2 * L), c.logn, c.d_primes.get(), st, c.stats, "ks_prod_intt"), "ks prod intt");
             long long total = static_cast<long long>(B) * 2 * L * n;
             c.stats.begin("moddown_coeff", 0, 32.0 * total, st);
-            moddown_coeff_kernel<false><<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(
+            moddown_coeff_kernel<false, Base><<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(
                 s.U, 2LL * n, n, s.Pp, pp_bs, pp_ps, out, o_bs, o_ps, inv_top, base, c.q[c.k - 1], c.d_primes.get(), c.logn, Li, total);
             c.stats.end(st);
             cuda_check(cudaGetLastError(), "moddown_coeff_kernel");
@@ -2384,14 +2392,18 @@ namespace sb
         }
     }
 
-    void op_apply_galois(Context &c, size_t L, size_t batch, const u64 *in2, uint32_t elt, const KSwitchKey &key, u64 *out2,
-                         cudaStream_t st)
+    static void check_galois_args(const Context &c, size_t L, uint32_t elt, const KSwitchKey &key)
     {
         check_ks_args(c, L, key);
         if (!(elt & 1) || elt >= 2 * c.n)
             throw std::invalid_argument("Galois element is not valid"); // evaluator.cpp:2424-2427
-        if (in2 == out2)
-            throw std::invalid_argument("apply_galois: in and out must not alias");
+    }
+
+    // out = apply_galois(in) (Base = BaseSrc) or addend + apply_galois(in) (BaseAddSrc), in chunks of the key-switching scratch
+    template <class Base>
+    static void galois_chunks(Context &c, size_t L, size_t batch, const u64 *in2, uint32_t elt, const KSwitchKey &key, const u64 *addend2,
+                              u64 *out2, cudaStream_t st)
+    {
         const size_t poly = L * c.n, chunk = ks_chunk(c, L, batch, false);
         const uint32_t *perm = nullptr;
         uint32_t ginv = 0;
@@ -2411,12 +2423,78 @@ namespace sb
             KsScratch s = ks_carve(c, L, B, false);
             const u64 *in = in2 + b0 * 2 * poly;
             Src target{ in + poly, static_cast<long long>(2 * poly), perm, ginv, c.logn };
-            BaseSrc base;
+            Base base;
             base.s = Src{ in, static_cast<long long>(2 * poly), perm, ginv, c.logn };
             base.pstride = static_cast<long long>(poly);
             base.c1_zero = 1;
             base.present = 1;
+            if constexpr (Base::kAddend)
+            {
+                base.a = addend2 + b0 * 2 * poly;
+                base.a_bs = static_cast<long long>(2 * poly);
+                base.a_ps = static_cast<long long>(poly);
+            }
             key_switch_chunk(c, L, B, s, target, key, base, out2 + b0 * 2 * poly, st);
+        }
+    }
+
+    void op_apply_galois(Context &c, size_t L, size_t batch, const u64 *in2, uint32_t elt, const KSwitchKey &key, u64 *out2,
+                         cudaStream_t st)
+    {
+        check_galois_args(c, L, elt, key);
+        if (in2 == out2)
+            throw std::invalid_argument("apply_galois: in and out must not alias");
+        galois_chunks<BaseSrc>(c, L, batch, in2, elt, key, nullptr, out2, st);
+    }
+
+    void op_apply_galois_add(Context &c, size_t L, size_t batch, const u64 *in2, uint32_t elt, const KSwitchKey &key, const u64 *addend2,
+                             u64 *out2, cudaStream_t st)
+    {
+        check_galois_args(c, L, elt, key);
+        if (in2 == out2)
+            throw std::invalid_argument("apply_galois_add: in and out must not alias");
+        galois_chunks<BaseAddSrc>(c, L, batch, in2, elt, key, addend2, out2, st);
+    }
+
+    void check_rotate_sum_args(const Context &c, size_t L, size_t steps, const uint32_t *elts, const KSwitchKey *const *keys)
+    {
+        for (size_t j = 0; j < steps; j++)
+            check_galois_args(c, L, elts[j], *keys[j]);
+    }
+
+    // Each chunk of the key-switching scratch runs every step before the next chunk starts: the temporary is one chunk, not the
+    // batch, and every key is read once per chunk and step, as the chained apply_galois calls read it.
+    void op_rotate_sum(Context &c, size_t L, size_t batch, const u64 *in2, size_t steps, const uint32_t *elts, const KSwitchKey *const *keys,
+                       u64 *out2, cudaStream_t st)
+    {
+        check_rotate_sum_args(c, L, steps, elts, keys);
+        const size_t poly = L * c.n, bytes = 2 * poly * sizeof(u64);
+        if (steps == 0)
+        {
+            if (in2 != out2)
+                cuda_check(cudaMemcpyAsync(out2, in2, batch * bytes, cudaMemcpyDeviceToDevice, st), "rotate_sum copy");
+            return;
+        }
+        const size_t chunk = ks_chunk(c, L, batch, false);
+        u64 *tmp = static_cast<u64 *>(c.ensure_aux(chunk * bytes));
+        for (size_t b0 = 0; b0 < batch; b0 += chunk)
+        {
+            const size_t B = std::min(chunk, batch - b0);
+            const u64 *y = in2 + b0 * 2 * poly;
+            u64 *o = out2 + b0 * 2 * poly;
+            // y_j goes to o when steps - j is even and to tmp otherwise, so that y_steps ends in o; an input that is o itself
+            // and an odd step count start from a copy in tmp
+            if (y == o && (steps & 1))
+            {
+                cuda_check(cudaMemcpyAsync(tmp, y, B * bytes, cudaMemcpyDeviceToDevice, st), "rotate_sum copy");
+                y = tmp;
+            }
+            for (size_t j = 0; j < steps; j++)
+            {
+                u64 *dst = ((steps - j - 1) & 1) ? tmp : o;
+                galois_chunks<BaseAddSrc>(c, L, B, y, elts[j], *keys[j], y, dst, st);
+                y = dst;
+            }
         }
     }
 
@@ -2478,7 +2556,7 @@ namespace sb
             cuda_check(launch_ntt_inv(top, static_cast<int>(P), c.logn, c.d_primes.get(), st, c.stats, "rescale_top_intt"), "rescale intt");
             BaseSrc none;
             const long long o_ps = static_cast<long long>(Lout) * n, o_bs = 2 * o_ps;
-            OpModDownFwd op{ U, src, i_bs, i_ps, T, out + p0 * Lout * c.n, o_bs, o_ps, c.d_invq.get() + (L - 1) * c.k, none, c.q[L - 1],
+            OpModDownFwd<> op{ U, src, i_bs, i_ps, T, out + p0 * Lout * c.n, o_bs, o_ps, c.d_invq.get() + (L - 1) * c.k, none, c.q[L - 1],
                              c.logn, static_cast<int>(Lout) };
             cuda_check(launch_ntt_fwd(op, static_cast<int>(P * Lout), c.logn, c.d_primes.get(), st, c.stats, "rescale_ntt", -1, c.fast_q), "rescale ntt");
         }
@@ -2516,7 +2594,7 @@ namespace sb
                 cuda_check(launch_ntt_inv(top, static_cast<int>(P), c.logn, c.d_primes.get(), st, c.stats, "modswitch_top_intt"), "mod switch intt");
                 BaseSrc none;
                 const long long o_ps = static_cast<long long>(Lout) * n, o_bs = 2 * o_ps;
-                OpModDownFwdBgv op{ { U, src, i_bs, i_ps, T, out + p0 * Lout * c.n, o_bs, o_ps, c.d_invq.get() + (L - 1) * c.k, none, c.q[L - 1],
+                OpModDownFwdBgv<> op{ { U, src, i_bs, i_ps, T, out + p0 * Lout * c.n, o_bs, o_ps, c.d_invq.get() + (L - 1) * c.k, none, c.q[L - 1],
                                       c.logn, static_cast<int>(Lout) },
                                     K, c.d_qmod.get() + (L - 1) * c.k, c.t };
                 cuda_check(launch_ntt_fwd(op, static_cast<int>(P * Lout), c.logn, c.d_primes.get(), st, c.stats, "modswitch_ntt", -1, c.fast_q),

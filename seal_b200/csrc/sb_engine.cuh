@@ -244,6 +244,14 @@ namespace sb
     void op_relinearize_sized(Context &c, size_t L, size_t size, size_t batch, const u64 *in, const KSwitchKey &key, u64 *out, cudaStream_t st);
     void op_apply_galois(Context &c, size_t L, size_t batch, const u64 *in2, uint32_t elt, const KSwitchKey &key, u64 *out2,
                          cudaStream_t st);
+    // out = addend + apply_galois(in), the addition in the key switch's epilogue.  out may be addend (accumulate), addend may be in,
+    // out == in is rejected
+    void op_apply_galois_add(Context &c, size_t L, size_t batch, const u64 *in2, uint32_t elt, const KSwitchKey &key, const u64 *addend2,
+                             u64 *out2, cudaStream_t st);
+    // y_0 = in, y_{j+1} = y_j + apply_galois(y_j, elts[j]) with keys[j]; out = y_steps (out may be in; steps = 0 copies)
+    void check_rotate_sum_args(const Context &c, size_t L, size_t steps, const uint32_t *elts, const KSwitchKey *const *keys);
+    void op_rotate_sum(Context &c, size_t L, size_t batch, const u64 *in2, size_t steps, const uint32_t *elts, const KSwitchKey *const *keys,
+                       u64 *out2, cudaStream_t st);
     size_t keyswitch_chunk(const Context &c, size_t L, size_t batch, bool fused);
     // arithmetic ceilings measured in process: warp-level butterflies (kind 0-2) / multiply-accumulates (kind 3) per second
     double selftest_rate(Context &c, int kind, cudaStream_t st);

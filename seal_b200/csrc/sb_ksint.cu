@@ -873,6 +873,7 @@ namespace sb
     }
 
     // -------------------------------------------------------------- (4) reconstruction + mod-down, per coefficient ----
+    template <class Base = BaseSrc>
     struct CrtArgs
     {
         uint32_t *Acc;           // ks32_crt_kernel<..., TOP = true> leaves U in place of the special prime's first two residue rows
@@ -886,7 +887,7 @@ namespace sb
         u64 *R;                  // MODE 0 / 3: [B][2][L][n]
         u64 *out;                // MODE 1: out + b*o_bs + c*o_ps + i*n
         long long o_bs, o_ps;
-        BaseSrc base;
+        Base base;               // MODE 1 only
         int L, k;
         long long total;         // B * 2 * n
     };
@@ -923,14 +924,15 @@ namespace sb
     {
         return MODE == 3 ? U : csub(U + (T.q >> 1), T.q);
     }
-    __device__ __forceinline__ u64 crt_top_k(u64 U, const CrtArgs &A)
+    template <class Args>
+    __device__ __forceinline__ u64 crt_top_k(u64 U, const Args &A)
     {
         const u64 r = barrett64(U, A.t, A.t_ratio);
         return mul_shoup(r ? A.t - r : 0, A.inv_top_mod_t, A.t);
     }
     // residue a of output prime i, U = crt_top<MODE>(special prime's value), K = crt_top_k(U) (BGV) -> the mod-down result, canonical
-    template <int MODE>
-    __device__ __forceinline__ u64 crt_moddown(u64 a, u64 U, u64 K, int i, const PrimeDev &Q, const PrimeDev &T, const CrtArgs &A)
+    template <int MODE, class Args>
+    __device__ __forceinline__ u64 crt_moddown(u64 a, u64 U, u64 K, int i, const PrimeDev &Q, const PrimeDev &T, const Args &A)
     {
         u64 x; // a_i - delta_i + (multiple of q_i), in (0, 4 q_i)
         const u64 u = T.q < Q.q2 ? U : barrett64(U, Q.q, Q.ratio_hi); // u < q_top < 2 q_i: no reduction of u needed
@@ -949,8 +951,8 @@ namespace sb
     // TOP (with FUSE): only the special prime's value, crt_top<MODE>(U), stored as two 32-bit halves over the words of the special
     // prime's residue rows t = 0, 1 that the same thread has just read; ks32_inv_crt_ntt does the rest.
     // MODE 0: CKKS (coefficient-form result to R), 1: BFV (result + base to out), 3: BGV (R)
-    template <int MODE, int LOGN, bool FUSE, bool TOP = false>
-    __global__ void __launch_bounds__(FUSE ? 128 : 256) ks32_crt_kernel(CrtArgs A, KsIntParams prm, const uint2 *__restrict__ tw_outer)
+    template <int MODE, int LOGN, bool FUSE, bool TOP = false, class Base = BaseSrc>
+    __global__ void __launch_bounds__(FUSE ? 128 : 256) ks32_crt_kernel(CrtArgs<Base> A, KsIntParams prm, const uint2 *__restrict__ tw_outer)
     {
         constexpr int R = LOGN - 12, E = FUSE ? (1 << R) : 1;
         const int S = prm.S, L = A.L, k = A.k;
@@ -1078,22 +1080,23 @@ namespace sb
                 const u64 r = crt_moddown<MODE>(a[e], U[e], K[MODE == 3 ? e : 0], i, Q, T, A);
                 const int xi = j + (e << 12);
                 if (MODE == 1)
-                    A.out[b * A.o_bs + c * A.o_ps + (static_cast<long long>(i) << LOGN) + xi] = csub(r + A.base.get(b, c, i, xi, Q.q), Q.q);
+                    A.out[b * A.o_bs + c * A.o_ps + (static_cast<long long>(i) << LOGN) + xi] =
+                        plus_addend(A.base, b, c, i, LOGN, xi, csub(r + A.base.get(b, c, i, xi, Q.q), Q.q), Q.q);
                 else
                     A.R[((static_cast<size_t>(bc) * L + i) << LOGN) + xi] = r;
             }
         }
     }
-    template <int MODE, int LOGN>
-    static void launch_crt_logn(const CrtArgs &A, const KsInt &d, bool fuse, size_t B, cudaStream_t st)
+    template <int MODE, int LOGN, class Base>
+    static void launch_crt_logn(const CrtArgs<Base> &A, const KsInt &d, bool fuse, size_t B, cudaStream_t st)
     {
         if (fuse)
-            ks32_crt_kernel<MODE, LOGN, true><<<static_cast<unsigned>(B * 2 * 32), 128, 0, st>>>(A, d.prm, d.d_inv_outer.get());
+            ks32_crt_kernel<MODE, LOGN, true, false, Base><<<static_cast<unsigned>(B * 2 * 32), 128, 0, st>>>(A, d.prm, d.d_inv_outer.get());
         else
-            ks32_crt_kernel<MODE, LOGN, false><<<static_cast<unsigned>((A.total + 255) / 256), 256, 0, st>>>(A, d.prm, d.d_inv_outer.get());
+            ks32_crt_kernel<MODE, LOGN, false, false, Base><<<static_cast<unsigned>((A.total + 255) / 256), 256, 0, st>>>(A, d.prm, d.d_inv_outer.get());
     }
-    template <int MODE>
-    static void launch_crt(const CrtArgs &A, const KsInt &d, bool fuse, size_t B, int logn, cudaStream_t st)
+    template <int MODE, class Base>
+    static void launch_crt(const CrtArgs<Base> &A, const KsInt &d, bool fuse, size_t B, int logn, cudaStream_t st)
     {
         switch (logn)
         {
@@ -1117,7 +1120,7 @@ namespace sb
     template <int LOGNA>
     constexpr size_t crt_ntt_smem(int S) { return static_cast<size_t>(S > 2 ? S : 2) * kTile * 4 + (size_t(1) << LOGNA) * sizeof(Tw) + 8; }
     template <int MODE, int LOGNA, bool FAST>
-    __global__ void __launch_bounds__(kColThreads, 2) ks32_inv_crt_ntt(CrtArgs A, KsIntParams prm, const uint2 *__restrict__ tw_outer, u64 *__restrict__ mid)
+    __global__ void __launch_bounds__(kColThreads, 2) ks32_inv_crt_ntt(CrtArgs<> A, KsIntParams prm, const uint2 *__restrict__ tw_outer, u64 *__restrict__ mid)
     {
         constexpr int NA = 1 << LOGNA, C = kTile / NA, R = LOGNA - 4, E = 1 << R, G = kTile / E, LOGN = LOGNA + kLocalLog;
         extern __shared__ __align__(16) unsigned char ks_crt_smem[];
@@ -1188,7 +1191,7 @@ namespace sb
             m[((8 * ridx + j) << kLocalLog) + col0 + c] = a[j];
     }
     template <int MODE, int LOGNA>
-    static void launch_crt_ntt_logna(const CrtArgs &A, const KsInt &d, u64 *mid, size_t B, bool fast, bool top, cudaStream_t st)
+    static void launch_crt_ntt_logna(const CrtArgs<> &A, const KsInt &d, u64 *mid, size_t B, bool fast, bool top, cudaStream_t st)
     {
         if (top)
         {
@@ -1203,7 +1206,7 @@ namespace sb
     }
     // top: the special prime's value (ks32_crt_kernel<..., TOP = true>); otherwise ks32_inv_crt_ntt into mid.  n = 8192 .. 65536
     template <int MODE>
-    static void launch_crt_ntt(const CrtArgs &A, const KsInt &d, u64 *mid, size_t B, bool fast, bool top, int logn, cudaStream_t st)
+    static void launch_crt_ntt(const CrtArgs<> &A, const KsInt &d, u64 *mid, size_t B, bool fast, bool top, int logn, cudaStream_t st)
     {
         switch (logn)
         {
@@ -1216,12 +1219,13 @@ namespace sb
     }
 
     // ------------------------------------------------- (5) the result back to NTT form, added into the ciphertext ----
+    template <class Base = BaseSrc>
     struct OpAddBaseFwd
     {
         u64 *R;   // [B][2][L][n], transformed in place
         u64 *out; // out + b*o_bs + c*o_ps + i*n
         long long o_bs, o_ps;
-        BaseSrc base;
+        Base base;
         int logn, L;
         __device__ __forceinline__ bool skip(int) const { return false; }
         __device__ __forceinline__ int pid(int row) const { return row % L; }
@@ -1239,7 +1243,8 @@ namespace sb
         {
             const int i = row % L, bc = row / L, b = bc >> 1, c = bc & 1;
             const u64 t = csub(csub(v, P.q2), P.q);
-            out[b * o_bs + c * o_ps + (static_cast<long long>(i) << logn) + idx] = csub(t + base.get(b, c, i, idx, P.q), P.q);
+            out[b * o_bs + c * o_ps + (static_cast<long long>(i) << logn) + idx] =
+                plus_addend(base, b, c, i, logn, idx, csub(t + base.get(b, c, i, idx, P.q), P.q), P.q);
         }
         __device__ __forceinline__ void store8(int row, int idx0, u64 (&a)[8], const PrimeDev &P) const
         {
@@ -1261,6 +1266,11 @@ namespace sb
                 {
                     r0 = csub(r0 + base.get(b, c, i, idx0 + 2 * h, P.q), P.q);
                     r1 = csub(r1 + base.get(b, c, i, idx0 + 2 * h + 1, P.q), P.q);
+                }
+                if constexpr (Base::kAddend)
+                {
+                    const ulonglong2 av = reinterpret_cast<const ulonglong2 *>(base.arow(b, c, i, logn) + idx0)[h];
+                    r0 = csub(r0 + av.x, P.q), r1 = csub(r1 + av.y, P.q);
                 }
                 op_[h] = make_ulonglong2(r0, r1);
             }
@@ -1433,7 +1443,8 @@ namespace sb
         cuda_check(cudaGetLastError(), "ks32_intt_fwd_outer");
     }
 
-    void ksint_core(Context &c, size_t L, size_t B, const KsIntScratch &s, Src target, u64 *D, const KSwitchKey &key, BaseSrc base,
+    template <class Base>
+    void ksint_core(Context &c, size_t L, size_t B, const KsIntScratch &s, Src target, u64 *D, const KSwitchKey &key, Base base,
                     u64 *out, long long o_bs, cudaStream_t st)
     {
         const KsInt &d = c.ksint;
@@ -1472,7 +1483,7 @@ namespace sb
         if (!o_bs)
             o_bs = 2 * o_ps;
         {
-            CrtArgs A{};
+            CrtArgs<> A{}; // the base enters only in MODE 1 (BFV), through Ab below
             A.Acc = s.Acc, A.punct = d.d_punct.get(), A.neg = d.d_neg.get(), A.primes = c.d_primes.get();
             A.inv_top = c.d_invq.get() + (c.k - 1) * c.k;
             A.half_mod = d.d_half_mod.get();
@@ -1498,7 +1509,7 @@ namespace sb
                 c.scheme == 3 ? launch_crt_ntt<3>(A, d, s.R, B, c.fast_q, false, c.logn, st) : launch_crt_ntt<0>(A, d, s.R, B, c.fast_q, false, c.logn, st);
                 c.stats.end(st);
                 cuda_check(cudaGetLastError(), "ks32_inv_crt_ntt");
-                OpAddBaseFwd op{ s.R, out, o_bs, o_ps, base, c.logn, Li };
+                OpAddBaseFwd<Base> op{ s.R, out, o_bs, o_ps, base, c.logn, Li };
                 cuda_check(launch_ntt_fwd(op, static_cast<int>(B * 2 * L), c.logn, c.d_primes.get(), st, c.stats, "ks_result_ntt", -1, c.fast_q, true),
                            "ks result ntt");
                 return;
@@ -1509,7 +1520,11 @@ namespace sb
             if (c.scheme == 3)
                 launch_crt<3>(A, d, fuse_crt, B, c.logn, st);
             else if (c.scheme == 1)
-                launch_crt<1>(A, d, fuse_crt, B, c.logn, st);
+            {
+                CrtArgs<Base> Ab{ A.Acc, A.punct, A.neg, A.primes, A.inv_top, A.half_mod, A.qtop_mod, A.t, A.t_ratio, A.inv_top_mod_t,
+                                  A.R, A.out, A.o_bs, A.o_ps, base, A.L, A.k, A.total };
+                launch_crt<1>(Ab, d, fuse_crt, B, c.logn, st);
+            }
             else
                 launch_crt<0>(A, d, fuse_crt, B, c.logn, st);
             c.stats.end(st);
@@ -1518,10 +1533,14 @@ namespace sb
         // (5) CKKS / BGV: back to NTT form, added into the ciphertext
         if (c.scheme != 1)
         {
-            OpAddBaseFwd op{ s.R, out, o_bs, o_ps, base, c.logn, Li };
+            OpAddBaseFwd<Base> op{ s.R, out, o_bs, o_ps, base, c.logn, Li };
             cuda_check(launch_ntt_fwd(op, static_cast<int>(B * 2 * L), c.logn, c.d_primes.get(), st, c.stats, "ks_result_ntt", -1, c.fast_q), "ks result ntt");
         }
     }
+    template void ksint_core<BaseSrc>(Context &, size_t, size_t, const KsIntScratch &, Src, u64 *, const KSwitchKey &, BaseSrc, u64 *, long long,
+                                      cudaStream_t);
+    template void ksint_core<BaseAddSrc>(Context &, size_t, size_t, const KsIntScratch &, Src, u64 *, const KSwitchKey &, BaseAddSrc, u64 *,
+                                         long long, cudaStream_t);
 
     static void launch_inverse(Context &c, uint32_t *data, int arows, cudaStream_t st, bool outer)
     {

@@ -49,7 +49,31 @@ namespace sb
             t.p += c * pstride;
             return t.get(b, i, idx, q);
         }
+        static constexpr bool kAddend = false;
     };
+
+    // BaseSrc plus an addend: a plain [B][2][L][n] source added to both output components after the base term (apply_galois_add:
+    // out = addend + apply_galois(in)).  A type of its own, so that the kernels without an addend compile exactly as before.
+    struct BaseAddSrc : BaseSrc
+    {
+        const u64 *a = nullptr; // component c of item b, prime i at a + b*a_bs + c*a_ps + i*n
+        long long a_bs = 0, a_ps = 0;
+        static constexpr bool kAddend = true;
+        __device__ __forceinline__ const u64 *arow(int b, int c, int i, int logn) const
+        {
+            return a + b * a_bs + c * a_ps + (static_cast<long long>(i) << logn);
+        }
+    };
+
+    // r (canonical) + the addend word, canonical: a second csub, so words of q - 1 everywhere stay below q.  No-op without an addend.
+    template <class Base>
+    __device__ __forceinline__ u64 plus_addend(const Base &base, int b, int c, int i, int logn, int idx, u64 r, u64 q)
+    {
+        if constexpr (Base::kAddend)
+            return csub(r + base.arow(b, c, i, logn)[idx], q);
+        else
+            return r;
+    }
 
     // (1) target -> coefficient form (CKKS / BGV): rows (b, J); evaluator.cpp:2651-2658
     struct OpKsIntt
