@@ -1565,8 +1565,25 @@ namespace sb
         }
     };
 
+    // The digit sums of (3) add L products of canonical words, each below (q_I - 1)^2: without a reduction they fit 128 bits as long
+    // as L (q_max - 1)^2 < 2^128 at the largest output prime of the level: at every level of primes up to 60 bits (L <= 255), but only
+    // up to 64 digits of the largest 61-bit primes.  Deeper levels take the WINDOW instantiations, which reduce the sums after every
+    // kKsSumWindow digits: a carried residue plus 64 products, (q - 1) + 64 (q - 1)^2, stays below 2^128 at every prime below 2^61
+    // (the context's bound), and 65 products of the largest 61-bit primes do not (DESIGN 3.2b).
+    constexpr int kKsSumWindow = 64;
+    static bool ks_sum_needs_window(const Context &c, size_t L)
+    {
+        u64 qmax = c.q[c.k - 1];
+        for (size_t i = 0; i < L; i++)
+            qmax = std::max(qmax, c.q[i]);
+        const unsigned __int128 sq = static_cast<unsigned __int128>(qmax - 1) * (qmax - 1);
+        return sq > ~static_cast<unsigned __int128>(0) / L; // L (q_max - 1)^2 >= 2^128
+    }
+
     // (3) multiply-accumulate with the key, 128-bit lazy sums, one Barrett at the end; evaluator.cpp:2705-2755
     //     grid = (B, n/256, L+1): consecutive CTAs share the key tile of (I, coefficient range) through L2.
+    //     WINDOW: the sums are also reduced after every kKsSumWindow digits (ks_sum_needs_window).
+    template <bool WINDOW>
     __global__ void __launch_bounds__(256) ks_mac_kernel(const u64 *__restrict__ E, Src tgt, int ntt_in, const u64 *__restrict__ key,
                                                           u64 *__restrict__ Pp, const PrimeDev *__restrict__ primes, int logn, int L, int k)
     {
@@ -1579,12 +1596,18 @@ namespace sb
         const PrimeDev P = primes[ki];
         u64 lo0 = 0, hi0 = 0, lo1 = 0, hi1 = 0;
         const u64 *e = E + ((static_cast<long long>(b) * (L + 1) + I) * L << logn) + idx;
-        for (int J = 0; J < L; J++)
+        for (int J = 0, since = 0; J < L; J++)
         {
             u64 x = (ntt_in && I == J) ? tgt.get(b, J, idx, P.q) : e[static_cast<long long>(J) << logn];
             const u64 *kr = key + ((static_cast<long long>(J) * 2 * k + ki) << logn) + idx;
             mac128(lo0, hi0, x, __ldg(kr));
             mac128(lo1, hi1, x, __ldg(kr + (static_cast<long long>(k) << logn)));
+            if (WINDOW && ++since == kKsSumWindow)
+            {
+                since = 0;
+                lo0 = barrett128(lo0, hi0, P.q, P.ratio_lo, P.ratio_hi), hi0 = 0;
+                lo1 = barrett128(lo1, hi1, P.q, P.ratio_lo, P.ratio_hi), hi1 = 0;
+            }
         }
         u64 *o = Pp + (((static_cast<long long>(b) * 2) * (L + 1) + I) << logn) + idx;
         o[0] = barrett128(lo0, hi0, P.q, P.ratio_lo, P.ratio_hi);
@@ -1694,7 +1717,8 @@ namespace sb
         static constexpr size_t total = xs + acc + tw + 16;
     };
     // PLAIN: the target is a plain slab (relinearize / multiply_relinearize); rotations read it through a Galois view.
-    template <bool FAST, bool PLAIN>
+    // WINDOW (guarded primes only): the sums are also reduced after every kKsSumWindow digits, as in ks_mac_kernel.
+    template <bool FAST, bool PLAIN, bool WINDOW>
     __global__ void __launch_bounds__(256, SB_MAC_MIN_BLOCKS) ks_local_mac_kernel(const u64 *__restrict__ E, Src tgt, int ntt_in, const u64 *__restrict__ key,
                                                                    u64 *__restrict__ Pp, const PrimeDev *__restrict__ primes, int logn, int L, int k,
                                                                    int B)
@@ -1739,7 +1763,7 @@ namespace sb
         // key rows of output prime I: component c of digit J at key + ((J*2 + c)*k + ki) * n
         const long long kstep = (2LL * k) << logn, kcomp = static_cast<long long>(k) << logn;
         const u64 *krow = key + (static_cast<long long>(ki) << logn) + e0;
-        for (int J = 0; J < L; J++, krow += kstep)
+        for (int J = 0, since = 0; J < L; J++, krow += kstep)
         {
             u64 a[8];
             if (ntt_in && J == I)
@@ -1773,7 +1797,7 @@ namespace sb
                 {
 #pragma unroll
                     for (int j = 0; j < 8; j++)
-                        a[j] = csub(csub(csub(a[j], P.q4), P.q2), P.q); // keeps 256 summands below 2^128 for 60-bit primes
+                        a[j] = csub(csub(csub(a[j], P.q4), P.q2), P.q); // canonical: 256 summands fit 128 bits at 60 bits, 64 at 61 (WINDOW)
                 }
                 else if (L > 200)
                 {
@@ -1801,6 +1825,17 @@ namespace sb
                 mac128_4(t1.x, t1.y, a[2 * h + 1], v.y);
                 acc1[2 * h][threadIdx.x] = t0;
                 acc1[2 * h + 1][threadIdx.x] = t1;
+            }
+            if (WINDOW && ++since == kKsSumWindow)
+            {
+                since = 0;
+#pragma unroll
+                for (int j = 0; j < 8; j++)
+                {
+                    s0l[j] = barrett128(s0l[j], s0h[j], P.q, P.ratio_lo, P.ratio_hi), s0h[j] = 0;
+                    const ulonglong2 t = acc1[j][threadIdx.x];
+                    acc1[j][threadIdx.x] = make_ulonglong2(barrett128(t.x, t.y, P.q, P.ratio_lo, P.ratio_hi), 0);
+                }
             }
         }
         ulonglong2 *o0 = reinterpret_cast<ulonglong2 *>(Pp + (((static_cast<long long>(b) * 2) * (L + 1) + I) << logn) + e0);
@@ -2254,6 +2289,7 @@ namespace sb
         }
         // digits in + 2 accumulated components out per (b, I), plus one pass over the key
         const double mac_bytes = 8.0 * n * (static_cast<double>(B) * (L + 1) * (L + 2) + 2.0 * L * (L + 1));
+        const bool window = ks_sum_needs_window(c, L);
         if (fused)
         {
             const int na = n >> kLocalLog;
@@ -2265,10 +2301,12 @@ namespace sb
                 c.stats.begin("ks_local_mac", 0, mac_bytes, st, 0.5 * active_rows * n * kLocalLog, 2.0 * B * (L + 1) * L * n);
                 kern<<<grid, 256, smem, st>>>(s.E, target, ntt_in ? 1 : 0, key.d_key.get(), s.Pp, c.d_primes.get(), c.logn, Li, ki, static_cast<int>(B));
             };
-            if (c.fast_q)
-                plain_tgt ? launch(ks_local_mac_kernel<true, true>) : launch(ks_local_mac_kernel<true, false>);
+            if (c.fast_q) // primes below 2^57: 255 products of lazy operands (below 4q past 200 digits) stay below 2^128
+                plain_tgt ? launch(ks_local_mac_kernel<true, true, false>) : launch(ks_local_mac_kernel<true, false, false>);
+            else if (window)
+                plain_tgt ? launch(ks_local_mac_kernel<false, true, true>) : launch(ks_local_mac_kernel<false, false, true>);
             else
-                plain_tgt ? launch(ks_local_mac_kernel<false, true>) : launch(ks_local_mac_kernel<false, false>);
+                plain_tgt ? launch(ks_local_mac_kernel<false, true, false>) : launch(ks_local_mac_kernel<false, false, false>);
             c.stats.end(st);
             cuda_check(cudaGetLastError(), "ks_local_mac_kernel");
         }
@@ -2277,7 +2315,10 @@ namespace sb
             int threads = std::min(n, 256);
             dim3 grid(static_cast<unsigned>(B), (n + threads - 1) / threads, static_cast<unsigned>(L + 1));
             c.stats.begin("ks_mac", 0, mac_bytes, st, 0, 2.0 * B * (L + 1) * L * n);
-            ks_mac_kernel<<<grid, threads, 0, st>>>(s.E, target, ntt_in ? 1 : 0, key.d_key.get(), s.Pp, c.d_primes.get(), c.logn, Li, ki);
+            if (window)
+                ks_mac_kernel<true><<<grid, threads, 0, st>>>(s.E, target, ntt_in ? 1 : 0, key.d_key.get(), s.Pp, c.d_primes.get(), c.logn, Li, ki);
+            else
+                ks_mac_kernel<false><<<grid, threads, 0, st>>>(s.E, target, ntt_in ? 1 : 0, key.d_key.get(), s.Pp, c.d_primes.get(), c.logn, Li, ki);
             c.stats.end(st);
             cuda_check(cudaGetLastError(), "ks_mac_kernel");
         }
