@@ -15,6 +15,17 @@ typedef unsigned __int128 u128;
 static u64 mulmod(u64 a, u64 b, u64 q) { return (u64)(((u128)a * b) % q); }
 static u64 addmod(u64 a, u64 b, u64 q) { return (u64)(((u128)a + b) % q); }
 static u64 submod(u64 a, u64 b, u64 q) { return (u64)(((u128)(a % q) + q - (b % q)) % q); }
+/* the reference's words for add_poly_coeffmod / sub_poly_coeffmod / negate_poly_coeffmod on ANY 64-bit operands (release build,
+ * polyarithsmallmod.cpp:93-128, polyarithsmallmod.h:95-105): the sum wraps mod 2^64 and sheds q once; the difference is the
+ * 64-bit one plus q on a borrow, not reduced further; the negation is q - x mod 2^64 for x != 0.  On words below q they equal
+ * addmod / submod; on other words they are what a caller of the reference gets back. */
+static u64 add_word(u64 a, u64 b, u64 q)
+{
+    u64 s = a + b;
+    return s >= q ? s - q : s;
+}
+static u64 sub_word(u64 a, u64 b, u64 q) { return a - b + (a < b ? q : 0); }
+static u64 neg_word(u64 a, u64 q) { return a ? q - a : 0; }
 static u64 powmod(u64 a, u64 e, u64 q)
 {
     u64 r = 1 % q;
@@ -355,7 +366,7 @@ void orc_linear(const orc_ctx *c, int mode, size_t L, size_t size, const u64 *a,
             {
                 size_t e = (p * L + i) * n + j;
                 u64 q = c->q[i];
-                out[e] = mode == 0 ? addmod(a[e], b[e], q) : mode == 1 ? submod(a[e], b[e], q) : submod(0, a[e], q);
+                out[e] = mode == 0 ? add_word(a[e], b[e], q) : mode == 1 ? sub_word(a[e], b[e], q) : neg_word(a[e], q);
             }
 }
 
@@ -459,7 +470,7 @@ void orc_add_plain_coeff(const orc_ctx *c, size_t L, size_t size, int subtract, 
                 u64 m = plain[j];
                 u64 fix = (u64)(((u128)m * q_mod_t + ((t + 1) >> 1)) / t);
                 u64 scaled = addmod(mulmod(m % q, delta, q), fix % q, q);
-                out[i * n + j] = subtract ? submod(out[i * n + j], scaled, q) : addmod(out[i * n + j], scaled, q);
+                out[i * n + j] = subtract ? sub_word(out[i * n + j], scaled, q) : add_word(out[i * n + j], scaled, q);
             }
         }
         return;
@@ -470,7 +481,7 @@ void orc_add_plain_coeff(const orc_ctx *c, size_t L, size_t size, int subtract, 
     orc_plain_to_ntt(c, L, m, p);
     for (size_t i = 0; i < L; i++)
         for (size_t j = 0; j < n; j++)
-            out[i * n + j] = subtract ? submod(out[i * n + j], p[i * n + j], c->q[i]) : addmod(out[i * n + j], p[i * n + j], c->q[i]);
+            out[i * n + j] = subtract ? sub_word(out[i * n + j], p[i * n + j], c->q[i]) : add_word(out[i * n + j], p[i * n + j], c->q[i]);
     free(m), free(p);
 }
 

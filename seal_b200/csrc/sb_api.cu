@@ -1759,6 +1759,30 @@ namespace
     // an entry point's own last step, inside its lock and stream order (the decryption wipes)
     using Then = void (*)(Context &c, cudaStream_t st);
 
+    // Device slabs: the output's byte range may meet an input's only as the exact in-place cases the layout allows (the checks
+    // above have already refused out == a or out == b where the layout forbids them), and then only where every ciphertext's output
+    // sits where its input was: same start and same words per ciphertext.  Any other overlap lets one thread overwrite words
+    // another thread has still to read.  out == a with different words per ciphertext is refused for one ciphertext too: some
+    // kernels would be safe there (the 2 x 2 tensor reads a coefficient's words before writing them), others not (PlainToNtt,
+    // n -> L n words: row i > 0 reads the plaintext words that row 0 overwrites), and the rule does not depend on which.
+    void check_overlap(const Layout &w, size_t batch, const void *a, const void *b, const void *out)
+    {
+        const size_t out_bytes = batch * w.out * w.out_unit, out_stride = w.out * w.out_unit;
+        auto conflict = [&](const void *in, size_t in_bytes, size_t in_stride) {
+            if (!in || !in_bytes || !out_bytes)
+                return false;
+            const auto *x = static_cast<const uint8_t *>(in), *o = static_cast<const uint8_t *>(out);
+            if (!(o < x + in_bytes && x < o + out_bytes))
+                return false;
+            return !(o == x && out_stride == in_stride);
+        };
+        if (conflict(a, batch * w.a * sizeof(u64), w.a * sizeof(u64)))
+            throw std::invalid_argument("the output slab must not overlap input a other than exactly in place");
+        const size_t b_bytes = (w.shared_b ? 1 : batch) * w.b * sizeof(u64);
+        if (conflict(b, b_bytes, w.shared_b ? 0 : w.b * sizeof(u64)))
+            throw std::invalid_argument("the output slab must not overlap input b other than exactly in place");
+    }
+
     template <class Op>
     int on_stream(sb200_context *ctx, void *stream, size_t batch, const void *a, const void *b, void *out, const Op &op, Then then = nullptr)
     {
@@ -1773,6 +1797,7 @@ namespace
             throw std::invalid_argument(w.alias);
         if (w.shared_b && out == b)
             throw std::invalid_argument("the shared plaintext must not alias the output slab");
+        check_overlap(w, batch, a, b, out);
         auto st = static_cast<cudaStream_t>(stream);
         op(c, 0, batch, static_cast<const u64 *>(a), static_cast<const u64 *>(b), static_cast<u64 *>(out), st);
         if (then)

@@ -40,6 +40,15 @@ __device__ __forceinline__ u64 csub(u64 x, u64 q)
     return x >= q ? x - q : x;
 }
 
+// x - y mod q on words a caller handed in, in the reference's borrow form (sub_uint_mod, util/uintarithsmallmod.h:156-158, and
+// sub_poly_coeffmod, polyarithsmallmod.cpp:126-128, in a release build): the 64-bit difference, plus q when it borrowed, and no
+// further reduction.  For x, y < q this equals csub(x + q - y, q); for other words it is the reference's word, which x + q - y
+// is not (that sum wraps when x - y > 2^64 - q, and stays at or above q when y - x > q).
+__device__ __forceinline__ u64 sub_borrow(u64 x, u64 y, u64 q)
+{
+    return x - y + (x < y ? q : 0);
+}
+
 // ---- Shoup / Harvey multiplication tuned for the integer pipes (32-bit multipliers) -------------------------------------------
 // Integer multiplies issue on the FMA-heavy pipe only (ncu: the binding pipe of every transform kernel) and a
 // 32x32->64 multiply-add costs twice a 32-bit one, so the quotient estimate uses three wide products instead of the

@@ -488,7 +488,7 @@ namespace sb
         if (MODE == 0)
             r = make_ulonglong2(csub(x.x + y.x, q), csub(x.y + y.y, q));
         else if (MODE == 1)
-            r = make_ulonglong2(csub(x.x + q - y.x, q), csub(x.y + q - y.y, q));
+            r = make_ulonglong2(sub_borrow(x.x, y.x, q), sub_borrow(x.y, y.y, q));
         else
             r = make_ulonglong2(x.x ? q - x.x : 0, x.y ? q - x.y : 0);
         out[e] = r;
@@ -523,7 +523,7 @@ namespace sb
     // Operand j is [B][stride_j][L][n] with size_j polynomials present.  Every output word gets the word operations the reference's
     // chain of add_inplace / sub_inplace performs on it, in the chain's order, in registers: acc = x_0, then per step j >= 1
     //   scaled (BGV balancing, multiply_poly_scalar_coeffmod over the present polynomials): acc = acc * e1_j, y = x_j * e2_j (Shoup);
-    //   add: acc = csub(acc + y, q);  sub: acc = csub(acc + q - y, q);
+    //   add: acc = csub(acc + y, q);  sub: acc = sub_borrow(acc, y, q) (acc - y, plus q on a borrow);
     //   polynomial absent from every earlier operand: acc = y (add, set_poly_array) or -y (sub, negate_poly_coeffmod).
     // Absence is tracked, never stood in for by zero: csub(0 + y, q) != y for a word y >= q.
     struct FoldLaunch
@@ -562,7 +562,7 @@ namespace sb
                         const ulonglong2 v = f.x[j][(b * f.stride[j] + p) * half + r];
                         const ulonglong2 y = make_ulonglong2(mul_shoup(v.x, e2, q), mul_shoup(v.y, e2, q));
                         acc = !have ? ((m & 1) ? make_ulonglong2(y.x ? q - y.x : 0, y.y ? q - y.y : 0) : y)
-                              : (m & 1) ? make_ulonglong2(csub(acc.x + q - y.x, q), csub(acc.y + q - y.y, q))
+                              : (m & 1) ? make_ulonglong2(sub_borrow(acc.x, y.x, q), sub_borrow(acc.y, y.y, q))
                                         : make_ulonglong2(csub(acc.x + y.x, q), csub(acc.y + y.y, q));
                         have = true;
                     }
@@ -571,7 +571,7 @@ namespace sb
                 {
                     const ulonglong2 y = f.x[j][(b * f.stride[j] + p) * half + r];
                     acc = !have ? ((m & 1) ? make_ulonglong2(y.x ? q - y.x : 0, y.y ? q - y.y : 0) : y)
-                          : (m & 1) ? make_ulonglong2(csub(acc.x + q - y.x, q), csub(acc.y + q - y.y, q))
+                          : (m & 1) ? make_ulonglong2(sub_borrow(acc.x, y.x, q), sub_borrow(acc.y, y.y, q))
                                     : make_ulonglong2(csub(acc.x + y.x, q), csub(acc.y + y.y, q));
                     have = true;
                 }
@@ -675,26 +675,27 @@ namespace sb
                                                                 const PrimeDev *__restrict__ primes, int logn, int L, int size, int batch, int G)
     {
         const long long half = static_cast<long long>(L) << (logn - 1); // pairs of one polynomial
-        const long long p = static_cast<long long>(blockIdx.y) * blockDim.x + threadIdx.x;
-        if (p >= half)
-            return;
-        const PrimeDev &P = primes[static_cast<int>(p >> (logn - 1))];
-        ulonglong2 y = plain[p];
-        if (MODE == 0)
-            y = make_ulonglong2(canon_in(y.x, P), canon_in(y.y, P));
         const int b1 = min(batch, static_cast<int>(blockIdx.x + 1) * G), polys = MODE == 0 ? size : 1;
-        for (int b = blockIdx.x * G; b < b1; b++)
-            for (int s = 0; s < polys; s++)
-            {
-                const long long e = (static_cast<long long>(b) * size + s) * half + p;
-                const ulonglong2 x = a[e];
-                if (MODE == 0)
-                    out[e] = make_ulonglong2(mulmod_wide(canon_in(x.x, P), y.x, P), mulmod_wide(canon_in(x.y, P), y.y, P));
-                else if (MODE == 1)
-                    out[e] = make_ulonglong2(csub(x.x + y.x, P.q), csub(x.y + y.y, P.q));
-                else
-                    out[e] = make_ulonglong2(csub(x.x + P.q - y.x, P.q), csub(x.y + P.q - y.y, P.q));
-            }
+        // grid.y is capped at 65535 blocks and L n / 512 reaches 65536 at n = 131072 with 256 primes: the y blocks stride over the pairs
+        for (long long p = static_cast<long long>(blockIdx.y) * blockDim.x + threadIdx.x; p < half; p += static_cast<long long>(gridDim.y) * blockDim.x)
+        {
+            const PrimeDev &P = primes[static_cast<int>(p >> (logn - 1))];
+            ulonglong2 y = plain[p];
+            if (MODE == 0)
+                y = make_ulonglong2(canon_in(y.x, P), canon_in(y.y, P));
+            for (int b = blockIdx.x * G; b < b1; b++)
+                for (int s = 0; s < polys; s++)
+                {
+                    const long long e = (static_cast<long long>(b) * size + s) * half + p;
+                    const ulonglong2 x = a[e];
+                    if (MODE == 0)
+                        out[e] = make_ulonglong2(mulmod_wide(canon_in(x.x, P), y.x, P), mulmod_wide(canon_in(x.y, P), y.y, P));
+                    else if (MODE == 1)
+                        out[e] = make_ulonglong2(csub(x.x + y.x, P.q), csub(x.y + y.y, P.q));
+                    else
+                        out[e] = make_ulonglong2(sub_borrow(x.x, y.x, P.q), sub_borrow(x.y, y.y, P.q));
+                }
+        }
     }
 
     static void launch_shared_plain(Context &c, int mode, const char *name, size_t L, size_t size, size_t batch, const u64 *a, const u64 *plain,
@@ -702,7 +703,7 @@ namespace sb
     {
         constexpr int G = 8;
         const size_t half = L * c.n / 2, polys = mode == 0 ? size : 1;
-        const dim3 grid(static_cast<unsigned>((batch + G - 1) / G), static_cast<unsigned>((half + 255) / 256));
+        const dim3 grid(static_cast<unsigned>((batch + G - 1) / G), static_cast<unsigned>(std::min<size_t>((half + 255) / 256, 65535)));
         auto pa = reinterpret_cast<const ulonglong2 *>(a);
         auto pp = reinterpret_cast<const ulonglong2 *>(plain);
         auto po = reinterpret_cast<ulonglong2 *>(out);
@@ -908,7 +909,7 @@ namespace sb
             const PrimeDev P = primes[i];
             const u64 scaled = bfv_plain_scaled(m, fix, t, delta[i], P);
             const u64 x = dst[static_cast<long long>(i) << logn];
-            dst[static_cast<long long>(i) << logn] = subtract ? csub(x + P.q - scaled, P.q) : csub(x + scaled, P.q);
+            dst[static_cast<long long>(i) << logn] = subtract ? sub_borrow(x, scaled, P.q) : csub(x + scaled, P.q);
         }
     }
 
@@ -924,7 +925,7 @@ namespace sb
         const u64 q = primes[static_cast<int>(r >> logn)].q;
         u64 *p = ct + b * ct_bs + r;
         const u64 x = *p, y = T[e];
-        *p = subtract ? csub(x + q - y, q) : csub(x + y, q);
+        *p = subtract ? sub_borrow(x, y, q) : csub(x + y, q);
     }
 
     static void launch_add_c0(Context &c, const char *name, size_t L, size_t size, size_t B, bool shared, bool subtract, const u64 *T, u64 *o,

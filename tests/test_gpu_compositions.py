@@ -67,8 +67,11 @@ def restate(ops, mods, modes=None, factors=None):
                 y = [sc(v, e2) for v in y]
             for p, v in enumerate(y):
                 if p < len(acc):
-                    s = acc[p] + q - v if m & 1 else acc[p] + v
-                    acc[p] = np.where(s >= q, s - q, s)
+                    if m & 1:  # sub_poly_coeffmod's borrow form: the 64-bit difference, plus q when it borrowed
+                        acc[p] = np.where(acc[p] < v, acc[p] - v + q, acc[p] - v)
+                    else:
+                        s = acc[p] + v
+                        acc[p] = np.where(s >= q, s - q, s)
                 else:
                     acc.append(np.where(v != 0, q - v, np.uint64(0)) if m & 1 else v)
     return np.stack(acc, axis=1)
@@ -141,6 +144,31 @@ def test_bound_words_equal_chained_add_sub(word):
     got = ctx.add_many(ops, modes)
     assert_words(got, chained, f"fold vs chained add/sub at {word}")
     assert_words(got, restate(ops, mods, modes), f"fold vs restatement at {word}")
+
+
+def test_sub_steps_on_unreduced_words():
+    """sub steps whose words reach the borrow form's two branches away from the canonical range: x - 0 with x = 2^64 - 1 stays
+    2^64 - 1 (no borrow, no reduction), 0 - (2^64 - 1) is q + 1 (one q added on the borrow); then uniform 64-bit words.  The fold,
+    chained sb200_sub calls and the restatement agree word for word"""
+    n, bits, L, B, size = 4096, [50, 40, 60], 2, 2, 2
+    mods, ctx = context(n, bits)
+    top = np.uint64(2 ** 64 - 1)
+    rng = np.random.default_rng(64)
+    for x, y in ((top, np.uint64(0)), (np.uint64(0), top), (None, None)):
+        if x is None:
+            ops = [rng.integers(0, top, (B, size, L, n), dtype=np.uint64, endpoint=True) for _ in range(4)]
+        else:
+            ops = [np.full((B, size, L, n), x), np.full((B, size, L, n), y)]
+        modes = [1] * (len(ops) - 1)
+        want = restate(ops, mods, modes)
+        if x is not None:
+            first = int(want[0, 0, 0, 0])
+            assert first == (2 ** 64 - 1 if x == top else mods[0] + 1), first
+        chained = ops[0]
+        for j in range(1, len(ops)):
+            chained = ctx.sub(chained, ops[j])
+        assert_words(chained, want, f"chained sub from {x}, {y}")
+        assert_words(ctx.add_many(ops, modes), want, f"fold of sub steps from {x}, {y}")
 
 
 @needs_ref

@@ -151,6 +151,28 @@ def test_oracle_linear_and_square_vs_live_reference():
 
 
 @needs_ref
+def test_oracle_linear_and_plain_ops_on_unreduced_words_vs_live_reference():
+    """the oracle's add / sub / negate and the last step of add_plain / sub_plain take any 64-bit words as the reference's release
+    build does: the sum wraps and sheds q once, the difference is the borrow form (plus q on a borrow, no further reduction)"""
+    n = 64
+    mods = R.coeff_modulus_create(n, [30, 50, 57])
+    rng = np.random.default_rng(61)
+    top = np.uint64(2 ** 64 - 1)
+    L = 2
+    a = rng.integers(0, top, (2, L, n), dtype=np.uint64, endpoint=True)
+    b = rng.integers(0, top, (2, L, n), dtype=np.uint64, endpoint=True)
+    a[0, :, :4], b[0, :, :4] = [[top, 0, 0, top]] * L, [[0, top, 1, top]] * L
+    t = 65537
+    for sid in (R.BFV, R.BGV):
+        rc, oc = R.RefContext(sid, n, mods, t), O.Oracle(sid, n, mods, t)
+        for mode in (0, 1, 2):
+            assert (rc.linear(mode, L, a, b) == oc.linear(mode, L, a, b)).all(), (sid, mode)
+        plain, cf = rng.integers(0, t, n, dtype=np.uint64), 3 if sid == R.BGV else 1
+        for mode, sub in ((1, False), (2, True)):
+            assert (rc.plain_op_coeff(mode, L, a, plain, sid == R.BGV, cf) == oc.add_plain_coeff(L, a, plain, sub, cf)).all(), (sid, sub)
+
+
+@needs_ref
 @pytest.mark.parametrize("scheme", ["ckks", "bfv"])
 def test_oracle_multiply_plain_vs_live_reference(scheme):
     # Evaluator::multiply_plain with ciphertext and plaintext both in NTT form (evaluator.cpp:2157-2195)
