@@ -213,8 +213,9 @@ int sb200_negate(sb200_context *ctx, size_t L, size_t size, size_t batch, const 
  * NULL when no step is scaled.  A polynomial no earlier operand has is copied (add) or negated (sub), as the reference copies or
  * negates the longer operand's tail.  The words equal those of the chained add / sub calls for any input words.
  * Errors, all before the first launch: count = 0 or a size outside 1..16 or a mode outside 0..3 (SB200_E_INVALID_ARG); a NULL
- * operand, d_out, sizes or (with a scaled step) h_factors (SB200_E_POINTER); d_out equal to an operand other than operand 0, or
- * to operand 0 when sizes[0] is not the largest size (SB200_E_INVALID_ARG). */
+ * operand, d_out, sizes or (with a scaled step) h_factors (SB200_E_POINTER); d_out overlapping an operand other than exactly in
+ * place on operand 0 (d_out == d_operands[0] with sizes[0] the largest size) (SB200_E_INVALID_ARG).  The _host form stages the
+ * batch through the pipeline of every _host entry point, in chunks of SB200_LIMIT_HOST_STAGE_BYTES per pipeline slot. */
 #define SB200_FOLD_ADD 0
 #define SB200_FOLD_SUB 1
 #define SB200_FOLD_SCALED 2
@@ -235,8 +236,8 @@ int sb200_add_many(sb200_context *ctx, size_t L, size_t batch, size_t count, con
  * chain's order (multiply_plain's, then add_many's): count = 0 or outputs = 0, a plain count neither 1 nor batch, a size outside
  * 1..16, a mode outside 0..3, coefficient-form plaintexts in a CKKS context (SB200_E_INVALID_ARG); a NULL array, operand or
  * output, or (with a scaled step) h_factors (SB200_E_POINTER); an output slab overlapping an operand's slab or another output's
- * (SB200_E_INVALID_ARG).  The _host form
- * stages the batch in chunks of SB200_LIMIT_HOST_STAGE_BYTES and uploads each shared plaintext once per call. */
+ * (SB200_E_INVALID_ARG).  The _host form stages the batch through the pipeline of every _host entry point, in chunks of
+ * SB200_LIMIT_HOST_STAGE_BYTES per pipeline slot, and uploads each shared plaintext once per call. */
 int sb200_multiply_plain_sum(sb200_context *ctx, size_t L, size_t batch, size_t count, size_t outputs, const size_t *sizes,
                              const uint64_t *const *d_cts, const size_t *plain_counts, const uint64_t *const *d_plains, int ct_is_ntt,
                              int plain_is_ntt, const int *modes, const uint64_t *h_factors, uint64_t *const *d_outs, void *stream);
@@ -257,8 +258,8 @@ int sb200_multiply_plain_sum_host(sb200_context *ctx, size_t L, size_t batch, si
  * SB200_LIMIT_SCRATCH_BYTES holds, each chunk folded into the output (no caller-side intermediates).  Errors, all before the first
  * launch, in the chain's order (multiply's, then add_many's): count = 0 or outputs = 0, a BFV level above sb200_multiply's limit,
  * a mode outside 0..3 (SB200_E_INVALID_ARG); a NULL array, operand or output, or (with a scaled step) h_factors (SB200_E_POINTER);
- * an output slab overlapping an operand's slab or another output's (SB200_E_INVALID_ARG).  The _host form stages the batch in
- * chunks of SB200_LIMIT_HOST_STAGE_BYTES. */
+ * an output slab overlapping an operand's slab or another output's (SB200_E_INVALID_ARG).  The _host form stages the batch
+ * through the pipeline of every _host entry point, in chunks of SB200_LIMIT_HOST_STAGE_BYTES per pipeline slot. */
 int sb200_multiply_sum(sb200_context *ctx, size_t L, size_t batch, size_t count, size_t outputs, const uint64_t *const *d_lhs,
                        const uint64_t *const *d_rhs, const int *modes, const uint64_t *h_factors, uint64_t *const *d_outs, void *stream);
 int sb200_multiply_sum_host(sb200_context *ctx, size_t L, size_t batch, size_t count, size_t outputs, const uint64_t *const *h_lhs,

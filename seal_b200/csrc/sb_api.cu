@@ -12,7 +12,6 @@
 #include <cstdio>
 #include <cstring>
 #include <new>
-#include <type_traits>
 #include <thread>
 
 using namespace sb;
@@ -52,8 +51,19 @@ struct sb200_kswitch_key
     }
 };
 
+// a missing pointer found inside SB_TRY: SB200_E_POINTER, as SB_NEED returns
+struct null_pointer : std::runtime_error
+{
+    explicit null_pointer(const std::string &what) : std::runtime_error("null pointer: " + what) {}
+};
+
 #define SB_TRY try {
 #define SB_CATCH                                   \
+    }                                              \
+    catch (const null_pointer &e)                  \
+    {                                              \
+        g_last_error = e.what();                   \
+        return SB200_E_POINTER;                    \
     }                                              \
     catch (const std::invalid_argument &e)         \
     {                                              \
@@ -842,23 +852,86 @@ static void check_size(size_t size)
 }
 
 // ---- evaluator operations, encoder and decryptor ---------------------------------------------------------------------
-// Each operation is described once: what it checks, the layout of one ciphertext's slabs, and the launch on a chunk of B
-// ciphertexts starting at ciphertext b0.  Two drivers turn a description into its entry points: on_stream (device slabs, the
-// whole batch in one launch on the caller's stream) and on_host (host buffers).  The host-buffer entry points cut the batch into
-// chunks that flow through a 3-stage pipeline on three streams: H2D copy of chunk i+1 | kernels of chunk i | D2H copy of chunk
-// i-1, double-buffered device staging owned by the context (PCIe is full duplex, so with pinned host buffers both copy
-// directions overlap each other and the compute).  Pageable host memory works too, the copies then serialise inside the driver.
+// Each operation is described once: what it checks, its Layout (the input and output slabs of one ciphertext), and the launch
+// on a chunk of B ciphertexts starting at ciphertext b0, which takes the chunk's input and output slabs in the layout's order.
+// Two drivers turn a description into its entry points: on_stream (device slabs, the whole batch in one launch on the caller's
+// stream) and on_host (host buffers).  The host-buffer entry points cut the batch into chunks that flow through a 3-stage
+// pipeline on three streams: H2D copy of chunk i+1 | kernels of chunk i | D2H copy of chunk i-1, double-buffered device staging
+// owned by the context (PCIe is full duplex, so with pinned host buffers both copy directions overlap each other and the compute).
+// Pageable host memory works too, the copies then serialise inside the driver.
 namespace
 {
+    struct Slab // an input
+    {
+        size_t words;          // per ciphertext (0: none; the pointer may then be NULL)
+        const char *noun;      // what the pointer and overlap errors call it
+        bool in_place = false; // an output may sit exactly on it: the same start and the same bytes per ciphertext
+        bool shared = false;   // one operand of `words` words for the whole batch (a plaintext shared by every ciphertext)
+        bool optional = false; // may be NULL (the values of an empty CKKS vector); every other slab must be present
+    };
+    struct Out
+    {
+        size_t words;              // per ciphertext
+        size_t unit = sizeof(u64); // bytes of one word (the noise budget returns one int per ciphertext)
+    };
     struct Layout
     {
-        size_t a, b, out;              // words per ciphertext of input a, input b (0 = none) and the output
-        bool in_place = false;         // the output overwrites input a (out = a)
-        const char *alias = nullptr;   // device slabs: the error when the output aliases an input (nullptr = allowed)
-        size_t out_unit = sizeof(u64); // bytes of one output word (the noise budget returns one int per ciphertext)
-        bool shared_b = false;         // input b is one operand of b words for the whole batch (a plaintext shared by every ciphertext)
-        bool alias_b_ok = false;       // with alias set: the output may still be input b (an addend read and written by one thread)
+        std::vector<Slab> in;
+        std::vector<Out> out;
+        const char *name = nullptr;  // the operation the overlap errors name (nullptr: the one- and two-input operations)
+        const char *alias = nullptr; // the error when an output is exactly an input it may not sit on (nullptr: the overlap error)
+        bool in_place = false;       // the operation updates its one input (out = in): the host pipeline stages one buffer
     };
+    using Ins = std::vector<const u64 *>; // the caller's slabs in the layout's order
+    using Outs = std::vector<u64 *>;
+    // The caller's slabs as an entry point names them: a short list, or one or two operand arrays (each array checked non-NULL by
+    // the entry point).  Nothing is copied until the driver asks, inside its SB_TRY.
+    struct InSlabs
+    {
+        std::initializer_list<const void *> few;
+        const uint64_t *const *p = nullptr, *const *q = nullptr;
+        size_t n = 0, m = 0;
+        InSlabs(std::initializer_list<const void *> list) : few(list) {}
+        InSlabs(const uint64_t *const *p_, size_t n_, const uint64_t *const *q_ = nullptr, size_t m_ = 0) : p(p_), q(q_), n(n_), m(m_) {}
+        Ins get() const
+        {
+            Ins v;
+            for (const void *x : few)
+                v.push_back(static_cast<const u64 *>(x));
+            for (size_t i = 0; i < n + m; i++)
+                v.push_back(reinterpret_cast<const u64 *>(i < n ? p[i] : q[i - n]));
+            return v;
+        }
+    };
+    struct OutSlabs
+    {
+        std::initializer_list<void *> few;
+        uint64_t *const *p = nullptr;
+        size_t n = 0;
+        OutSlabs(std::initializer_list<void *> list) : few(list) {}
+        OutSlabs(uint64_t *const *p_, size_t n_) : p(p_), n(n_) {}
+        Outs get() const
+        {
+            Outs v;
+            for (void *x : few)
+                v.push_back(static_cast<u64 *>(x));
+            for (size_t i = 0; i < n; i++)
+                v.push_back(reinterpret_cast<u64 *>(p[i]));
+            return v;
+        }
+    };
+
+    // one- and two-input operations: input a (and b) and one output, which may sit exactly on an input unless alias names the error
+    Layout unary(size_t a, size_t out, const char *alias = nullptr)
+    {
+        return { { { a, "input a", !alias } }, { { out } }, nullptr, alias };
+    }
+    Layout binary(size_t a, size_t b, size_t out, const char *alias = nullptr)
+    {
+        Layout w = unary(a, out, alias);
+        w.in.push_back({ b, "input b", !alias });
+        return w;
+    }
 
     struct HostPipe
     {
@@ -879,61 +952,85 @@ namespace
             for (int i = 0; i < 2; i++)
                 ev_in[i] = io.ev_in[i].get(), ev_comp[i] = io.ev_comp[i].get(), ev_out[i] = io.ev_out[i].get();
         }
-        u64 *buffer(int slot, int which, size_t words)
-        {
-            DevBuf<u64> &b = c.io.buf[slot][which];
-            b.grow(words);
-            return b.get();
-        }
         template <class Op>
-        void run(size_t batch, const Layout &w, const u64 *ha, const u64 *hb, u64 *ho, const Op &op)
+        void run(size_t batch, const Layout &w, const Ins &h_in, const Outs &h_out, const Op &op)
         {
+            if (w.in_place && (w.in.size() != 1 || w.out.size() != 1 || w.in[0].words != w.out[0].words || w.out[0].unit != sizeof(u64)))
+                throw std::logic_error("an in-place layout has one input and one output of the same words");
             StreamOrder order(c, s_comp); // the operation's kernels (and the scratch arenas they use) run on s_comp
-            const size_t wa = w.a, wb = w.shared_b ? 0 : w.b, wo = w.in_place ? 0 : w.out;
-            const size_t out_bytes = w.out * w.out_unit; // per ciphertext
-            const size_t per_ct = (wa + wb) * sizeof(u64) + (w.in_place ? 0 : out_bytes);
+            size_t per_ct = 0;            // staged bytes per ciphertext
+            for (const Slab &s : w.in)
+                per_ct += s.shared ? 0 : s.words * sizeof(u64);
+            for (const Out &o : w.out)
+                per_ct += w.in_place ? 0 : o.words * o.unit;
             size_t chunk = std::max<size_t>(1, std::min<size_t>(batch, c.host_stage_bytes / std::max<size_t>(per_ct, 1)));
             if (chunk >= batch && batch >= 4)
                 chunk = (batch + 1) / 2; // at least two chunks so the copies overlap the kernels
-            // size all staging (and let the op grow its scratch) before the pipeline starts: growth synchronises the device
+            // A slot's staging: the per-ciphertext inputs of a chunk in buf[slot][0], its outputs in buf[slot][2] (in place: the
+            // output is staged on its input); the shared inputs in buf[0][1], uploaded once ahead of the first chunk and never overwritten.  Each slab
+            // starts at a 256-byte boundary.
+            const auto place = [](size_t &end, size_t words) {
+                const size_t at = (end + 31) & ~size_t(31);
+                end = at + words;
+                return at;
+            };
+            std::vector<size_t> in_at(w.in.size()), out_at(w.out.size());
+            size_t in_words = 0, shared_words = 0, out_words = 0;
+            for (size_t x = 0; x < w.in.size(); x++)
+                in_at[x] = w.in[x].shared ? place(shared_words, w.in[x].words) : place(in_words, chunk * w.in[x].words);
+            for (size_t y = 0; y < w.out.size(); y++)
+                out_at[y] = place(out_words, (chunk * w.out[y].words * w.out[y].unit + sizeof(u64) - 1) / sizeof(u64));
+            // size all staging before the pipeline starts: growth synchronises the device
             for (int slot = 0; slot < 2; slot++)
             {
-                buffer(slot, 0, chunk * wa);
-                if (wb)
-                    buffer(slot, 1, chunk * wb);
+                c.io.buf[slot][0].grow(in_words);
                 if (!w.in_place)
-                    buffer(slot, 2, (chunk * wo * w.out_unit + sizeof(u64) - 1) / sizeof(u64));
+                    c.io.buf[slot][2].grow(out_words);
             }
-            const u64 *d_shared = nullptr; // a shared operand crosses the bus once, ahead of the first chunk, and is never overwritten
-            if (w.shared_b)
+            if (shared_words)
+                c.io.buf[0][1].grow(shared_words);
+            std::vector<u64 *> din[2], dout[2];
+            for (int slot = 0; slot < 2; slot++)
             {
-                u64 *d = buffer(0, 1, w.b);
-                cuda_check(cudaMemcpyAsync(d, hb, w.b * sizeof(u64), cudaMemcpyHostToDevice, s_in), "H2D");
-                d_shared = d;
+                for (size_t x = 0; x < w.in.size(); x++)
+                    din[slot].push_back(w.in[x].words ? (w.in[x].shared ? c.io.buf[0][1] : c.io.buf[slot][0]).get() + in_at[x] : nullptr);
+                for (size_t y = 0; y < w.out.size(); y++)
+                    dout[slot].push_back(w.in_place ? din[slot][0] : c.io.buf[slot][2].get() + out_at[y]);
             }
+            for (size_t x = 0; x < w.in.size(); x++)
+                if (w.in[x].shared && w.in[x].words)
+                    cuda_check(cudaMemcpyAsync(din[0][x], h_in[x], w.in[x].words * sizeof(u64), cudaMemcpyHostToDevice, s_in), "H2D");
             size_t i = 0;
             for (size_t b0 = 0; b0 < batch; b0 += chunk, i++)
             {
                 const size_t B = std::min(chunk, batch - b0);
                 const int slot = static_cast<int>(i & 1);
-                u64 *db = wb ? buffer(slot, 1, B * wb) : nullptr;
-                u64 *da = buffer(slot, 0, B * wa), *dout = w.in_place ? da : buffer(slot, 2, (B * wo * w.out_unit + sizeof(u64) - 1) / sizeof(u64));
                 if (i >= 2)
                 {
                     // inputs of this slot are free once its previous kernels finished (and, in place, once copied out)
                     cuda_check(cudaStreamWaitEvent(s_in, w.in_place ? ev_out[slot] : ev_comp[slot], 0), "wait");
                 }
-                cuda_check(cudaMemcpyAsync(da, ha + b0 * wa, B * wa * sizeof(u64), cudaMemcpyHostToDevice, s_in), "H2D");
-                if (wb)
-                    cuda_check(cudaMemcpyAsync(db, hb + b0 * wb, B * wb * sizeof(u64), cudaMemcpyHostToDevice, s_in), "H2D");
+                for (size_t x = 0; x < w.in.size(); x++)
+                {
+                    const Slab &s = w.in[x];
+                    if (s.words && !s.shared)
+                        cuda_check(cudaMemcpyAsync(din[slot][x], h_in[x] + b0 * s.words, B * s.words * sizeof(u64),
+                                                   cudaMemcpyHostToDevice, s_in),
+                                   "H2D");
+                }
                 cuda_check(cudaEventRecord(ev_in[slot], s_in), "record");
                 cuda_check(cudaStreamWaitEvent(s_comp, ev_in[slot], 0), "wait");
                 if (i >= 2 && !w.in_place)
                     cuda_check(cudaStreamWaitEvent(s_comp, ev_out[slot], 0), "wait"); // output staging of this slot drained
-                op(c, b0, B, da, w.shared_b ? d_shared : db, dout, s_comp);
+                op(c, b0, B, din[slot].data(), dout[slot].data(), s_comp);
                 cuda_check(cudaEventRecord(ev_comp[slot], s_comp), "record");
                 cuda_check(cudaStreamWaitEvent(s_out, ev_comp[slot], 0), "wait");
-                cuda_check(cudaMemcpyAsync(reinterpret_cast<uint8_t *>(ho) + b0 * out_bytes, dout, B * out_bytes, cudaMemcpyDeviceToHost, s_out), "D2H");
+                for (size_t y = 0; y < w.out.size(); y++)
+                {
+                    const size_t bytes = w.out[y].words * w.out[y].unit; // per ciphertext
+                    cuda_check(cudaMemcpyAsync(reinterpret_cast<uint8_t *>(h_out[y]) + b0 * bytes, dout[slot][y], B * bytes, cudaMemcpyDeviceToHost, s_out),
+                               "D2H");
+                }
                 cuda_check(cudaEventRecord(ev_out[slot], s_out), "record");
             }
             cuda_check(cudaStreamSynchronize(s_out), "synchronize");
@@ -946,8 +1043,16 @@ namespace
         bool inverse;
         size_t L, size;
         void check(const Context &c, size_t batch) const { check_level(c, L, batch); }
-        Layout layout(const Context &c) const { return { size * L * c.n, 0, size * L * c.n, true }; }
-        void operator()(Context &c, size_t, size_t B, const u64 *, const u64 *, u64 *out, cudaStream_t st) const { op_ntt(c, inverse, L, size, B, out, st); }
+        Layout layout(const Context &c) const
+        {
+            Layout w = unary(size * L * c.n, size * L * c.n);
+            w.in_place = true;
+            return w;
+        }
+        void operator()(Context &c, size_t, size_t B, const u64 *const *, u64 *const *outs, cudaStream_t st) const
+        {
+            op_ntt(c, inverse, L, size, B, outs[0], st);
+        }
     };
 
     // two size-2 ciphertexts; square: b is a (one operand crosses the bus, the NTT-form schemes square with their own kernel when
@@ -961,15 +1066,14 @@ namespace
             check_level(c, L, batch);
             check_bfv_multiply_level(c, L);
         }
-        Layout layout(const Context &c) const { return { 2 * L * c.n, square ? 0 : 2 * L * c.n, 3 * L * c.n }; }
-        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *b, u64 *out, cudaStream_t st) const
+        Layout layout(const Context &c) const { return square ? unary(2 * L * c.n, 3 * L * c.n) : binary(2 * L * c.n, 2 * L * c.n, 3 * L * c.n); }
+        void operator()(Context &c, size_t, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
         {
-            if (square)
-                b = a;
+            const u64 *b = square ? ins[0] : ins[1];
             if (c.scheme != SB200_SCHEME_BFV) // CKKS and BGV share the NTT-form tensor (evaluator.cpp:569-708, :710-841)
-                op_ckks_multiply(c, L, B, a, b, out, st);
+                op_ckks_multiply(c, L, B, ins[0], b, outs[0], st);
             else
-                op_bfv_multiply(c, L, B, a, b, out, st);
+                op_bfv_multiply(c, L, B, ins[0], b, outs[0], st);
         }
     };
 
@@ -984,14 +1088,14 @@ namespace
         }
         Layout layout(const Context &c) const
         {
-            return { sa * L * c.n, sb * L * c.n, (sa + sb - 1) * L * c.n, false, "multiply: the output slab must not alias an input slab" };
+            return binary(sa * L * c.n, sb * L * c.n, (sa + sb - 1) * L * c.n, "multiply: the output slab must not alias an input slab");
         }
-        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *b, u64 *out, cudaStream_t st) const
+        void operator()(Context &c, size_t, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
         {
             if (c.scheme != SB200_SCHEME_BFV)
-                op_ckks_multiply(c, L, sa, sb, B, a, b, out, st);
+                op_ckks_multiply(c, L, sa, sb, B, ins[0], ins[1], outs[0], st);
             else
-                op_bfv_multiply(c, L, sa, sb, B, a, b, out, st);
+                op_bfv_multiply(c, L, sa, sb, B, ins[0], ins[1], outs[0], st);
         }
     };
 
@@ -1000,148 +1104,92 @@ namespace
         int mode;
         size_t L, size;
         void check(const Context &c, size_t batch) const { check_level(c, L, batch); }
-        Layout layout(const Context &c) const { return { size * L * c.n, mode == 2 ? 0 : size * L * c.n, size * L * c.n }; }
-        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *b, u64 *out, cudaStream_t st) const
+        Layout layout(const Context &c) const
         {
-            op_linear(c, mode, L, size, B, a, b, out, st);
+            const size_t w = size * L * c.n;
+            return mode == 2 ? unary(w, w) : binary(w, w, w);
+        }
+        void operator()(Context &c, size_t, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
+        {
+            op_linear(c, mode, L, size, B, ins[0], mode == 2 ? nullptr : ins[1], outs[0], st);
         }
     };
 
-    // count operands of sizes[j] polynomials folded into one of the largest size (op_add_many); it does not fit Layout's two inputs,
-    // so it has its own two drivers below, add_many_on_stream and add_many_on_host
+    // count operands of sizes[j] polynomials folded into one of the largest size (op_add_many).  The output may be operand 0 in
+    // place when it has the output's size; it may not meet any other operand
     struct AddMany
     {
         size_t L, count;
         const size_t *sizes;
         const int *modes;
         const u64 *factors;
-        size_t out_size = 0;
-        void check(const Context &c, size_t batch)
+        size_t out_size() const
+        {
+            size_t s = 0;
+            for (size_t j = 0; j < count; j++)
+                s = std::max(s, sizes[j]);
+            return s;
+        }
+        // the fold's own checks, and the factors a scaled step needs (SB200_E_POINTER) after every other check
+        void check_fold(const Context &c, size_t batch) const
         {
             check_level(c, L, batch);
             if (count == 0)
                 throw std::invalid_argument("encrypteds cannot be empty");
-            out_size = 0;
             for (size_t j = 0; j < count; j++)
-            {
                 check_size(sizes[j]);
-                out_size = std::max(out_size, sizes[j]);
-            }
             for (size_t j = 1; j < count && modes; j++)
                 if (modes[j - 1] < 0 || modes[j - 1] > 3)
                     throw std::invalid_argument("invalid add_many mode");
         }
-        // operand 0 may be the output (in place) when it has the output's size; no other operand may
-        void check_alias(const u64 *const *ops, const u64 *out) const
+        void need_factors() const
         {
-            for (size_t j = 1; j < count; j++)
-                if (ops[j] == out)
-                    throw std::invalid_argument("add_many: the output slab must not alias an operand other than operand 0");
-            if (ops[0] == out && sizes[0] != out_size)
-                throw std::invalid_argument("add_many: the output slab may alias operand 0 only when operand 0 has the output's size");
-        }
-        bool scaled() const
-        {
-            for (size_t j = 1; j < count && modes; j++)
+            for (size_t j = 1; j < count && modes && !factors; j++)
                 if (modes[j - 1] & SB200_FOLD_SCALED)
-                    return true;
-            return false;
+                    throw null_pointer("h_factors");
         }
-        void operator()(Context &c, size_t B, const u64 *const *ops, u64 *out, cudaStream_t st) const
+        void check(const Context &c, size_t batch) const
+        {
+            check_fold(c, batch);
+            need_factors();
+        }
+        Layout layout(const Context &c) const
+        {
+            Layout w{ {}, { { out_size() * L * c.n } }, "add_many", "add_many: the output slab must not alias an operand other than operand 0" };
+            for (size_t j = 0; j < count; j++)
+                w.in.push_back({ sizes[j] * L * c.n, "an operand", j == 0 });
+            return w;
+        }
+        void operator()(Context &c, size_t, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
         {
             std::vector<int> m(count ? count - 1 : 0, SB200_FOLD_ADD);
             if (modes)
                 std::copy(modes, modes + m.size(), m.begin());
-            op_add_many(c, L, B, count, sizes, ops, m.data(), factors, out, st);
+            op_add_many(c, L, B, count, sizes, ins, m.data(), factors, outs[0], st);
         }
     };
 
-    int add_many_on_stream(sb200_context *ctx, void *stream, size_t batch, const uint64_t *const *ops, uint64_t *out, AddMany op)
+    // plain_count: one plaintext per ciphertext (batch) or one for the whole batch (1, a shared operand: Slab::shared).  The
+    // older entry points, which take one plaintext per ciphertext, stay on the per-ciphertext path at every batch size (shared =
+    // false, plain_count = batch); the _n entry points share the plaintext when plain_count = 1.
+    void check_plain_count(size_t plain_count, size_t batch)
     {
-        SB_NEED(op.sizes);
-        SB_NEED(ops);
-        SB_NEED(out);
-        for (size_t j = 0; j < op.count; j++)
-            SB_NEED(ops[j]);
-        SB_TRY
-        SB_ENTER_STREAM(ctx, stream)
-        op.check(c, batch);
-        if (op.scaled() && !op.factors)
-        {
-            g_last_error = "null pointer: h_factors";
-            return SB200_E_POINTER;
-        }
-        op.check_alias(reinterpret_cast<const u64 *const *>(ops), reinterpret_cast<const u64 *>(out));
-        op(c, batch, reinterpret_cast<const u64 *const *>(ops), reinterpret_cast<u64 *>(out), static_cast<cudaStream_t>(stream));
-        return SB200_OK;
-        SB_CATCH
+        if (plain_count != 1 && plain_count != batch)
+            throw std::invalid_argument("plain_count must be 1 or batch");
     }
 
-    // host buffers: the batch in chunks of the context's staging size; every operand's chunk is uploaded behind the previous one
-    int add_many_on_host(sb200_context *ctx, size_t batch, const uint64_t *const *ops, uint64_t *out, AddMany op)
-    {
-        SB_NEED(op.sizes);
-        SB_NEED(ops);
-        SB_NEED(out);
-        for (size_t j = 0; j < op.count; j++)
-            SB_NEED(ops[j]);
-        SB_TRY
-        SB_ENTER(ctx)
-        op.check(c, batch);
-        if (op.scaled() && !op.factors)
-        {
-            g_last_error = "null pointer: h_factors";
-            return SB200_E_POINTER;
-        }
-        op.check_alias(reinterpret_cast<const u64 *const *>(ops), reinterpret_cast<const u64 *>(out));
-        const size_t poly = op.L * c.n;
-        size_t in_words = 0; // per ciphertext, all operands
-        for (size_t j = 0; j < op.count; j++)
-            in_words += op.sizes[j] * poly;
-        const size_t per_ct = (in_words + op.out_size * poly) * sizeof(u64);
-        const size_t chunk = std::max<size_t>(1, std::min(batch, c.host_stage_bytes / per_ct));
-        if (!c.io.s_comp)
-            c.io.s_comp = make_stream();
-        cudaStream_t st = c.io.s_comp.get();
-        StreamOrder order(c, st);
-        DevBuf<u64> &din = c.io.buf[0][0], &dout = c.io.buf[0][2];
-        din.grow(chunk * in_words);
-        dout.grow(chunk * op.out_size * poly);
-        std::vector<const u64 *> dops(op.count);
-        for (size_t b0 = 0; b0 < batch; b0 += chunk)
-        {
-            const size_t B = std::min(chunk, batch - b0);
-            u64 *d = din.get();
-            for (size_t j = 0; j < op.count; j++)
-            {
-                const size_t w = op.sizes[j] * poly;
-                cuda_check(cudaMemcpyAsync(d, ops[j] + b0 * w, B * w * sizeof(u64), cudaMemcpyHostToDevice, st), "H2D");
-                dops[j] = d;
-                d += B * w;
-            }
-            op(c, B, dops.data(), dout.get(), st);
-            cuda_check(cudaMemcpyAsync(out + b0 * op.out_size * poly, dout.get(), B * op.out_size * poly * sizeof(u64), cudaMemcpyDeviceToHost, st),
-                       "D2H");
-            cuda_check(cudaStreamSynchronize(st), "synchronize");
-        }
-        return SB200_OK;
-        SB_CATCH
-    }
-
-    // M outputs, each a fold over K terms of multiply_plain(ct_t, plain_{j K + t}) (op_multiply_plain_sum); K ciphertext operands
-    // and M K plaintext operands do not fit Layout either, so it has its own two drivers, plain_sum_on_stream and plain_sum_on_host.
-    // The fold's modes and factors are AddMany's, and are checked by it.
-    static void check_plain_count(size_t plain_count, size_t batch);
+    // inputs: K ciphertext operands, then M K plaintext operands; M outputs, each a fold over K terms of multiply_plain(ct_t,
+    // plain_{j K + t}) (op_multiply_plain_sum).  The fold's modes and factors are AddMany's, and are checked by it.  No output may
+    // meet an operand or another output.
     struct PlainSum
     {
-        AddMany fold; // L, K, sizes, modes, factors; out_size after check
+        AddMany fold; // L, K, sizes, modes, factors
         size_t M;
         const size_t *plain_counts;
         bool ct_ntt, plain_ntt;
         size_t K() const { return fold.count; }
-        size_t plain_words(const Context &c) const { return plain_ntt ? fold.L * c.n : c.n; }
         // in the chain's order: multiply_plain's checks of every term (the plaintext counts), then add_many's (sizes, modes)
-        void check(Context &c, size_t batch)
+        void check(Context &c, size_t batch) const
         {
             check_level(c, fold.L, batch);
             if (K() == 0)
@@ -1150,158 +1198,39 @@ namespace
                 throw std::invalid_argument("outputs cannot be empty");
             for (size_t j = 0; j < M * K(); j++)
                 check_plain_count(plain_counts[j], batch);
-            fold.check(c, batch);
+            fold.check_fold(c, batch);
             if (!plain_ntt)
                 plain_level(c, fold.L); // "unsupported operation for scheme type" for CKKS
+            fold.need_factors();
         }
-        // no output slab may overlap an operand's slab or another output's
-        void check_alias(const Context &c, size_t batch, const u64 *const *cts, const u64 *const *plains, const u64 *const *outs) const
+        Layout layout(const Context &c) const
         {
-            const size_t poly = fold.L * c.n, ow = batch * fold.out_size * poly;
-            auto overlap = [](const u64 *a, size_t na, const u64 *b, size_t nb) { return a < b + nb && b < a + na; };
-            for (size_t j = 0; j < M; j++)
-            {
-                for (size_t t = 0; t < K(); t++)
-                    if (overlap(outs[j], ow, cts[t], batch * fold.sizes[t] * poly))
-                        throw std::invalid_argument("multiply_plain_sum: an output slab must not overlap a ciphertext operand");
-                for (size_t x = 0; x < M * K(); x++)
-                    if (overlap(outs[j], ow, plains[x], plain_counts[x] * plain_words(c)))
-                        throw std::invalid_argument("multiply_plain_sum: an output slab must not overlap a plaintext operand");
-                for (size_t u = 0; u < j; u++)
-                    if (overlap(outs[j], ow, outs[u], ow))
-                        throw std::invalid_argument("multiply_plain_sum: output slabs must not overlap");
-            }
+            const size_t poly = fold.L * c.n;
+            Layout w{ {}, std::vector<Out>(M, Out{ fold.out_size() * poly }), "multiply_plain_sum" };
+            for (size_t t = 0; t < K(); t++)
+                w.in.push_back({ fold.sizes[t] * poly, "a ciphertext operand" });
+            for (size_t x = 0; x < M * K(); x++)
+                w.in.push_back({ plain_ntt ? poly : c.n, "a plaintext operand", false, plain_counts[x] == 1 });
+            return w;
         }
-        // counts: the plaintext counts of this call (1 or B)
-        void operator()(Context &c, size_t B, const u64 *const *cts, const size_t *counts, const u64 *const *plains, u64 *const *outs,
-                        cudaStream_t st) const
+        void operator()(Context &c, size_t, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
         {
-            op_multiply_plain_sum(c, fold.L, B, K(), M, fold.sizes, cts, counts, plains, ct_ntt, plain_ntt, fold.modes, fold.factors, outs, st);
+            std::vector<size_t> counts(M * K()); // of this chunk
+            for (size_t x = 0; x < M * K(); x++)
+                counts[x] = plain_counts[x] == 1 ? 1 : B;
+            op_multiply_plain_sum(c, fold.L, B, K(), M, fold.sizes, ins, counts.data(), ins + K(), ct_ntt, plain_ntt, fold.modes, fold.factors,
+                                  outs, st);
         }
     };
 
-    int plain_sum_on_stream(sb200_context *ctx, void *stream, size_t batch, const uint64_t *const *cts, const uint64_t *const *plains,
-                            uint64_t *const *outs, PlainSum op)
-    {
-        SB_NEED(op.fold.sizes);
-        SB_NEED(op.plain_counts);
-        SB_NEED(cts);
-        SB_NEED(plains);
-        SB_NEED(outs);
-        for (size_t t = 0; t < op.K(); t++)
-            SB_NEED(cts[t]);
-        for (size_t t = 0; t < op.M * op.K(); t++)
-            SB_NEED(plains[t]);
-        for (size_t j = 0; j < op.M; j++)
-            SB_NEED(outs[j]);
-        SB_TRY
-        SB_ENTER_STREAM(ctx, stream)
-        op.check(c, batch);
-        if (op.fold.scaled() && !op.fold.factors)
-        {
-            g_last_error = "null pointer: h_factors";
-            return SB200_E_POINTER;
-        }
-        op.check_alias(c, batch, reinterpret_cast<const u64 *const *>(cts), reinterpret_cast<const u64 *const *>(plains),
-                       reinterpret_cast<const u64 *const *>(outs));
-        op(c, batch, reinterpret_cast<const u64 *const *>(cts), op.plain_counts, reinterpret_cast<const u64 *const *>(plains),
-           reinterpret_cast<u64 *const *>(outs), static_cast<cudaStream_t>(stream));
-        return SB200_OK;
-        SB_CATCH
-    }
-
-    // host buffers: shared plaintexts are uploaded once per call; the batch goes in chunks of the context's staging size, every
-    // ciphertext operand, per-member plaintext and output of a chunk staged behind the previous one
-    int plain_sum_on_host(sb200_context *ctx, size_t batch, const uint64_t *const *cts, const uint64_t *const *plains, uint64_t *const *outs,
-                          PlainSum op)
-    {
-        SB_NEED(op.fold.sizes);
-        SB_NEED(op.plain_counts);
-        SB_NEED(cts);
-        SB_NEED(plains);
-        SB_NEED(outs);
-        for (size_t t = 0; t < op.K(); t++)
-            SB_NEED(cts[t]);
-        for (size_t t = 0; t < op.M * op.K(); t++)
-            SB_NEED(plains[t]);
-        for (size_t j = 0; j < op.M; j++)
-            SB_NEED(outs[j]);
-        SB_TRY
-        SB_ENTER(ctx)
-        op.check(c, batch);
-        if (op.fold.scaled() && !op.fold.factors)
-        {
-            g_last_error = "null pointer: h_factors";
-            return SB200_E_POINTER;
-        }
-        op.check_alias(c, batch, reinterpret_cast<const u64 *const *>(cts), reinterpret_cast<const u64 *const *>(plains),
-                       reinterpret_cast<const u64 *const *>(outs));
-        const size_t K = op.K(), M = op.M, poly = op.fold.L * c.n, pw = op.plain_words(c), out_words = op.fold.out_size * poly;
-        const auto shared = [&](size_t x) { return op.plain_counts[x] == 1; };
-        size_t in_words = 0, shared_words = 0; // per ciphertext, all operands; the shared plaintexts once
-        for (size_t t = 0; t < K; t++)
-            in_words += op.fold.sizes[t] * poly;
-        for (size_t x = 0; x < M * K; x++)
-            (shared(x) ? shared_words : in_words) += pw;
-        const size_t per_ct = (in_words + M * out_words) * sizeof(u64);
-        const size_t chunk = std::max<size_t>(1, std::min(batch, c.host_stage_bytes / per_ct));
-        if (!c.io.s_comp)
-            c.io.s_comp = make_stream();
-        cudaStream_t st = c.io.s_comp.get();
-        StreamOrder order(c, st);
-        DevBuf<u64> &din = c.io.buf[0][0], &dshared = c.io.buf[0][1], &dout = c.io.buf[0][2];
-        din.grow(chunk * in_words);
-        dshared.grow(std::max<size_t>(1, shared_words));
-        dout.grow(chunk * M * out_words);
-        std::vector<const u64 *> dcts(K), dplains(M * K);
-        std::vector<u64 *> douts(M);
-        std::vector<size_t> counts(M * K);
-        u64 *s = dshared.get();
-        for (size_t x = 0; x < M * K; x++)
-            if (shared(x))
-            {
-                cuda_check(cudaMemcpyAsync(s, plains[x], pw * sizeof(u64), cudaMemcpyHostToDevice, st), "H2D");
-                dplains[x] = s, s += pw;
-            }
-        for (size_t b0 = 0; b0 < batch; b0 += chunk)
-        {
-            const size_t B = std::min(chunk, batch - b0);
-            u64 *d = din.get();
-            for (size_t t = 0; t < K; t++)
-            {
-                const size_t w = op.fold.sizes[t] * poly;
-                cuda_check(cudaMemcpyAsync(d, cts[t] + b0 * w, B * w * sizeof(u64), cudaMemcpyHostToDevice, st), "H2D");
-                dcts[t] = d, d += B * w;
-            }
-            for (size_t x = 0; x < M * K; x++)
-            {
-                counts[x] = shared(x) ? 1 : B;
-                if (shared(x))
-                    continue;
-                cuda_check(cudaMemcpyAsync(d, plains[x] + b0 * pw, B * pw * sizeof(u64), cudaMemcpyHostToDevice, st), "H2D");
-                dplains[x] = d, d += B * pw;
-            }
-            for (size_t j = 0; j < M; j++)
-                douts[j] = dout.get() + j * B * out_words;
-            op(c, B, dcts.data(), counts.data(), dplains.data(), douts.data(), st);
-            for (size_t j = 0; j < M; j++)
-                cuda_check(cudaMemcpyAsync(outs[j] + b0 * out_words, douts[j], B * out_words * sizeof(u64), cudaMemcpyDeviceToHost, st), "D2H");
-            cuda_check(cudaStreamSynchronize(st), "synchronize");
-        }
-        return SB200_OK;
-        SB_CATCH
-    }
-
-    // M outputs, each a fold over K terms of multiply(lhs_{j K + t}, rhs_t) of size-2 operands (op_multiply_sum); like PlainSum it has
-    // its own two drivers, multiply_sum_on_stream and multiply_sum_on_host.  The fold's modes and factors are AddMany's, checked by it
-    // on the products' size 3.
+    // inputs: M K left-hand operands, then K right-hand ones, all of size 2; M outputs, each a fold over K terms of
+    // multiply(lhs_{j K + t}, rhs_t) (op_multiply_sum).  The fold's modes and factors are AddMany's, checked by it on the products'
+    // size 3.  No output may meet an operand or another output.
     struct MultiplySum
     {
         size_t L, K, M;
         const int *modes;
         const u64 *factors;
-        AddMany fold(const size_t *sizes) const { return AddMany{ L, K, sizes, modes, factors }; }
-        bool scaled() const { return fold(nullptr).scaled(); }
         // in the chain's order: multiply's checks of every term (the level, BFV's multiplication limit), then add_many's (modes)
         void check(const Context &c, size_t batch) const
         {
@@ -1312,128 +1241,26 @@ namespace
                 throw std::invalid_argument("outputs cannot be empty");
             check_bfv_multiply_level(c, L);
             const std::vector<size_t> sizes(K, 3);
-            fold(sizes.data()).check(c, batch);
+            AddMany{ L, K, sizes.data(), modes, factors }.check(c, batch);
         }
-        // no output slab may overlap an operand's slab or another output's
-        void check_alias(const Context &c, size_t batch, const u64 *const *lhs, const u64 *const *rhs, const u64 *const *outs) const
+        Layout layout(const Context &c) const
         {
-            const size_t poly = L * c.n, iw = batch * 2 * poly, ow = batch * 3 * poly;
-            auto overlap = [](const u64 *a, size_t na, const u64 *b, size_t nb) { return a < b + nb && b < a + na; };
-            for (size_t j = 0; j < M; j++)
-            {
-                for (size_t x = 0; x < M * K; x++)
-                    if (overlap(outs[j], ow, lhs[x], iw))
-                        throw std::invalid_argument("multiply_sum: an output slab must not overlap a left-hand operand");
-                for (size_t t = 0; t < K; t++)
-                    if (overlap(outs[j], ow, rhs[t], iw))
-                        throw std::invalid_argument("multiply_sum: an output slab must not overlap a right-hand operand");
-                for (size_t u = 0; u < j; u++)
-                    if (overlap(outs[j], ow, outs[u], ow))
-                        throw std::invalid_argument("multiply_sum: output slabs must not overlap");
-            }
+            Layout w{ std::vector<Slab>(M * K, Slab{ 2 * L * c.n, "a left-hand operand" }), std::vector<Out>(M, Out{ 3 * L * c.n }), "multiply_sum" };
+            w.in.resize(M * K + K, Slab{ 2 * L * c.n, "a right-hand operand" });
+            return w;
         }
-        void operator()(Context &c, size_t B, const u64 *const *lhs, const u64 *const *rhs, u64 *const *outs, cudaStream_t st) const
+        void operator()(Context &c, size_t, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
         {
-            op_multiply_sum(c, L, B, K, M, lhs, rhs, modes, factors, outs, st);
+            op_multiply_sum(c, L, B, K, M, ins, ins + M * K, modes, factors, outs, st);
         }
     };
 
-    // the pointer checks of a MultiplySum call: SB200_E_POINTER, or SB200_OK when every array and entry is present
-    int multiply_sum_pointers(const uint64_t *const *lhs, const uint64_t *const *rhs, uint64_t *const *outs, const MultiplySum &op)
+    // the plaintext operations: a ciphertext slab of ct words, which the output may overwrite in place, and plain_count plaintexts
+    // of pw words
+    Layout with_plain(size_t ct, size_t pw, bool shared)
     {
-        SB_NEED(lhs);
-        SB_NEED(rhs);
-        SB_NEED(outs);
-        for (size_t x = 0; x < op.M * op.K; x++)
-            SB_NEED(lhs[x]);
-        for (size_t t = 0; t < op.K; t++)
-            SB_NEED(rhs[t]);
-        for (size_t j = 0; j < op.M; j++)
-            SB_NEED(outs[j]);
-        return SB200_OK;
-    }
-
-    int multiply_sum_on_stream(sb200_context *ctx, void *stream, size_t batch, const uint64_t *const *lhs, const uint64_t *const *rhs,
-                               uint64_t *const *outs, MultiplySum op)
-    {
-        if (const int e = multiply_sum_pointers(lhs, rhs, outs, op); e != SB200_OK)
-            return e;
-        SB_TRY
-        SB_ENTER_STREAM(ctx, stream)
-        op.check(c, batch);
-        if (op.scaled() && !op.factors)
-        {
-            g_last_error = "null pointer: h_factors";
-            return SB200_E_POINTER;
-        }
-        op.check_alias(c, batch, reinterpret_cast<const u64 *const *>(lhs), reinterpret_cast<const u64 *const *>(rhs),
-                       reinterpret_cast<const u64 *const *>(outs));
-        op(c, batch, reinterpret_cast<const u64 *const *>(lhs), reinterpret_cast<const u64 *const *>(rhs), reinterpret_cast<u64 *const *>(outs),
-           static_cast<cudaStream_t>(stream));
-        return SB200_OK;
-        SB_CATCH
-    }
-
-    // host buffers: the batch in chunks of the context's staging size, every operand and output of a chunk staged behind the previous one
-    int multiply_sum_on_host(sb200_context *ctx, size_t batch, const uint64_t *const *lhs, const uint64_t *const *rhs, uint64_t *const *outs,
-                             MultiplySum op)
-    {
-        if (const int e = multiply_sum_pointers(lhs, rhs, outs, op); e != SB200_OK)
-            return e;
-        SB_TRY
-        SB_ENTER(ctx)
-        op.check(c, batch);
-        if (op.scaled() && !op.factors)
-        {
-            g_last_error = "null pointer: h_factors";
-            return SB200_E_POINTER;
-        }
-        op.check_alias(c, batch, reinterpret_cast<const u64 *const *>(lhs), reinterpret_cast<const u64 *const *>(rhs),
-                       reinterpret_cast<const u64 *const *>(outs));
-        const size_t K = op.K, M = op.M, in_w = 2 * op.L * c.n, out_w = 3 * op.L * c.n;
-        const size_t per_ct = ((M * K + K) * in_w + M * out_w) * sizeof(u64);
-        const size_t chunk = std::max<size_t>(1, std::min(batch, c.host_stage_bytes / per_ct));
-        if (!c.io.s_comp)
-            c.io.s_comp = make_stream();
-        cudaStream_t st = c.io.s_comp.get();
-        StreamOrder order(c, st);
-        DevBuf<u64> &din = c.io.buf[0][0], &dout = c.io.buf[0][2];
-        din.grow(chunk * (M * K + K) * in_w);
-        dout.grow(chunk * M * out_w);
-        std::vector<const u64 *> dl(M * K), dr(K);
-        std::vector<u64 *> douts(M);
-        for (size_t b0 = 0; b0 < batch; b0 += chunk)
-        {
-            const size_t B = std::min(chunk, batch - b0);
-            u64 *d = din.get();
-            auto stage = [&](const uint64_t *h) {
-                cuda_check(cudaMemcpyAsync(d, h + b0 * in_w, B * in_w * sizeof(u64), cudaMemcpyHostToDevice, st), "H2D");
-                const u64 *p = d;
-                d += B * in_w;
-                return p;
-            };
-            for (size_t x = 0; x < M * K; x++)
-                dl[x] = stage(lhs[x]);
-            for (size_t t = 0; t < K; t++)
-                dr[t] = stage(rhs[t]);
-            for (size_t j = 0; j < M; j++)
-                douts[j] = dout.get() + j * B * out_w;
-            op(c, B, dl.data(), dr.data(), douts.data(), st);
-            for (size_t j = 0; j < M; j++)
-                cuda_check(cudaMemcpyAsync(outs[j] + b0 * out_w, douts[j], B * out_w * sizeof(u64), cudaMemcpyDeviceToHost, st), "D2H");
-            cuda_check(cudaStreamSynchronize(st), "synchronize");
-        }
-        return SB200_OK;
-        SB_CATCH
-    }
-
-    // plain_count: one plaintext per ciphertext (batch) or one for the whole batch (1, a shared operand: Layout::shared_b).  The
-    // older entry points, which take one plaintext per ciphertext, stay on the per-ciphertext path at every batch size (shared =
-    // false, plain_count = batch); the _n entry points share the plaintext when plain_count = 1.
-    static void check_plain_count(size_t plain_count, size_t batch)
-    {
-        if (plain_count != 1 && plain_count != batch)
-            throw std::invalid_argument("plain_count must be 1 or batch");
+        return { { { ct, "input a", true }, { pw, "input b", !shared, shared } }, { { ct } }, nullptr,
+                 shared ? "the shared plaintext must not alias the output slab" : nullptr };
     }
 
     struct MultiplyPlain // b: NTT-form plaintexts [plain_count][L][n]
@@ -1445,10 +1272,10 @@ namespace
             check_level(c, L, batch);
             check_plain_count(plain_count, batch);
         }
-        Layout layout(const Context &c) const { return { size * L * c.n, L * c.n, size * L * c.n, false, nullptr, sizeof(u64), shared }; }
-        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *b, u64 *out, cudaStream_t st) const
+        Layout layout(const Context &c) const { return with_plain(size * L * c.n, L * c.n, shared); }
+        void operator()(Context &c, size_t, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
         {
-            op_multiply_plain(c, L, size, B, shared, a, b, out, st);
+            op_multiply_plain(c, L, size, B, shared, ins[0], ins[1], outs[0], st);
         }
     };
 
@@ -1462,10 +1289,10 @@ namespace
             check_level(c, L, batch);
             check_plain_count(plain_count, batch);
         }
-        Layout layout(const Context &c) const { return { size * L * c.n, L * c.n, size * L * c.n, false, nullptr, sizeof(u64), shared }; }
-        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *b, u64 *out, cudaStream_t st) const
+        Layout layout(const Context &c) const { return with_plain(size * L * c.n, L * c.n, shared); }
+        void operator()(Context &c, size_t, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
         {
-            op_add_plain_ntt(c, L, size, B, shared, subtract, a, b, out, st);
+            op_add_plain_ntt(c, L, size, B, shared, subtract, ins[0], ins[1], outs[0], st);
         }
     };
 
@@ -1473,10 +1300,10 @@ namespace
     {
         size_t L;
         void check(const Context &c, size_t batch) const { check_level(c, L, batch); }
-        Layout layout(const Context &c) const { return { c.n, 0, L * c.n }; }
-        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
+        Layout layout(const Context &c) const { return unary(c.n, L * c.n); }
+        void operator()(Context &c, size_t, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
         {
-            op_plain_to_ntt(c, L, B, a, nullptr, out, st);
+            op_plain_to_ntt(c, L, B, ins[0], nullptr, outs[0], st);
         }
     };
 
@@ -1490,10 +1317,10 @@ namespace
             check_level(c, L, batch);
             check_plain_count(plain_count, batch);
         }
-        Layout layout(const Context &c) const { return { size * L * c.n, c.n, size * L * c.n, false, nullptr, sizeof(u64), shared }; }
-        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *b, u64 *out, cudaStream_t st) const
+        Layout layout(const Context &c) const { return with_plain(size * L * c.n, c.n, shared); }
+        void operator()(Context &c, size_t, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
         {
-            op_multiply_plain_coeff(c, L, size, B, shared, ct_is_ntt, a, b, out, st);
+            op_multiply_plain_coeff(c, L, size, B, shared, ct_is_ntt, ins[0], ins[1], outs[0], st);
         }
     };
 
@@ -1509,10 +1336,10 @@ namespace
             check_level(c, L, batch);
             check_plain_count(plain_count, batch);
         }
-        Layout layout(const Context &c) const { return { size * L * c.n, c.n, size * L * c.n, false, nullptr, sizeof(u64), shared }; }
-        void operator()(Context &c, size_t b0, size_t B, const u64 *a, const u64 *b, u64 *out, cudaStream_t st) const
+        Layout layout(const Context &c) const { return with_plain(size * L * c.n, c.n, shared); }
+        void operator()(Context &c, size_t b0, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
         {
-            op_add_plain_coeff(c, L, size, B, shared, subtract, a, b, cf && !shared ? cf + b0 : cf, out, st);
+            op_add_plain_coeff(c, L, size, B, shared, subtract, ins[0], ins[1], cf && !shared ? cf + b0 : cf, outs[0], st);
         }
     };
 
@@ -1520,13 +1347,13 @@ namespace
     {
         bool decode;
         void check(const Context &, size_t batch) const { check_batch(batch); }
-        Layout layout(const Context &c) const { return { c.n, 0, c.n }; }
-        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
+        Layout layout(const Context &c) const { return unary(c.n, c.n); }
+        void operator()(Context &c, size_t, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
         {
             if (decode)
-                op_batch_decode(c, B, a, out, st);
+                op_batch_decode(c, B, ins[0], outs[0], st);
             else
-                op_batch_encode(c, B, a, out, st);
+                op_batch_encode(c, B, ins[0], outs[0], st);
         }
     };
 
@@ -1537,11 +1364,11 @@ namespace
         void check(const Context &c, size_t batch) const { check_level(c, L, batch); }
         Layout layout(const Context &c) const
         {
-            return { 3 * L * c.n, 0, 2 * L * c.n, false, "relinearize: input and output slabs must not alias (different layouts)" };
+            return unary(3 * L * c.n, 2 * L * c.n, "relinearize: input and output slabs must not alias (different layouts)");
         }
-        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
+        void operator()(Context &c, size_t, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
         {
-            op_relinearize(c, L, B, a, key, out, st);
+            op_relinearize(c, L, B, ins[0], key, outs[0], st);
         }
     };
 
@@ -1554,10 +1381,10 @@ namespace
             check_level(c, L, batch);
             check_bfv_multiply_level(c, L);
         }
-        Layout layout(const Context &c) const { return { 2 * L * c.n, 2 * L * c.n, 2 * L * c.n }; }
-        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *b, u64 *out, cudaStream_t st) const
+        Layout layout(const Context &c) const { return binary(2 * L * c.n, 2 * L * c.n, 2 * L * c.n); }
+        void operator()(Context &c, size_t, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
         {
-            op_multiply_relinearize(c, L, B, a, b, key, out, st);
+            op_multiply_relinearize(c, L, B, ins[0], ins[1], key, outs[0], st);
         }
     };
 
@@ -1572,11 +1399,11 @@ namespace
         }
         Layout layout(const Context &c) const
         {
-            return { size * L * c.n, 0, size * L * c.n, false, "relinearize: input and output slabs must not alias" };
+            return unary(size * L * c.n, size * L * c.n, "relinearize: input and output slabs must not alias");
         }
-        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
+        void operator()(Context &c, size_t, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
         {
-            op_relinearize_sized(c, L, size, B, a, key, out, st);
+            op_relinearize_sized(c, L, size, B, ins[0], key, outs[0], st);
         }
     };
 
@@ -1586,10 +1413,10 @@ namespace
         uint32_t elt;
         const KSwitchKey &key;
         void check(const Context &c, size_t batch) const { check_level(c, L, batch); }
-        Layout layout(const Context &c) const { return { 2 * L * c.n, 0, 2 * L * c.n }; }
-        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
+        Layout layout(const Context &c) const { return unary(2 * L * c.n, 2 * L * c.n); }
+        void operator()(Context &c, size_t, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
         {
-            op_apply_galois(c, L, B, a, elt, key, out, st);
+            op_apply_galois(c, L, B, ins[0], elt, key, outs[0], st);
         }
     };
 
@@ -1606,11 +1433,13 @@ namespace
         }
         Layout layout(const Context &c) const
         {
-            return { 2 * L * c.n, 2 * L * c.n, 2 * L * c.n, false, "apply_galois_add: in and out must not alias", sizeof(u64), false, true };
+            Layout w = binary(2 * L * c.n, 2 * L * c.n, 2 * L * c.n, "apply_galois_add: in and out must not alias");
+            w.in[1].in_place = true;
+            return w;
         }
-        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *b, u64 *out, cudaStream_t st) const
+        void operator()(Context &c, size_t, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
         {
-            op_apply_galois_add(c, L, B, a, elt, key, b, out, st);
+            op_apply_galois_add(c, L, B, ins[0], elt, key, ins[1], outs[0], st);
         }
     };
 
@@ -1625,10 +1454,10 @@ namespace
             check_level(c, L, batch);
             check_rotate_sum_args(c, L, steps, elts, keys);
         }
-        Layout layout(const Context &c) const { return { 2 * L * c.n, 0, 2 * L * c.n }; }
-        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
+        Layout layout(const Context &c) const { return unary(2 * L * c.n, 2 * L * c.n); }
+        void operator()(Context &c, size_t, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
         {
-            op_rotate_sum(c, L, B, a, steps, elts, keys, out, st);
+            op_rotate_sum(c, L, B, ins[0], steps, elts, keys, outs[0], st);
         }
     };
 
@@ -1661,20 +1490,21 @@ namespace
         }
         Layout layout(const Context &c) const
         {
-            return { size * L * c.n, 0, size * (L - 1) * c.n, false,
-                     rescale ? "rescale_to_next: input and output slabs must not alias (different layouts)"
-                             : "mod_switch_to_next: input and output slabs must not alias (different layouts)" };
+            return unary(size * L * c.n, size * (L - 1) * c.n,
+                         rescale ? "rescale_to_next: input and output slabs must not alias (different layouts)"
+                                 : "mod_switch_to_next: input and output slabs must not alias (different layouts)");
         }
-        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
+        void operator()(Context &c, size_t, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
         {
             if (rescale)
-                op_rescale(c, L, B * size, a, out, st);
+                op_rescale(c, L, B * size, ins[0], outs[0], st);
             else
-                op_mod_switch(c, L, B * size, a, out, st);
+                op_mod_switch(c, L, B * size, ins[0], outs[0], st);
         }
     };
 
-    struct CkksEncode // a: values, count doubles (reals) or count (re, im) pairs per plaintext; may be null when count = 0
+    // a: values, count doubles (reals) or count (re, im) pairs per plaintext; may be NULL, an error of check unless count = 0
+    struct CkksEncode
     {
         size_t L, count;
         bool is_complex, has_values;
@@ -1685,10 +1515,15 @@ namespace
             if (count && !has_values)
                 throw std::invalid_argument("values cannot be null");
         }
-        Layout layout(const Context &c) const { return { count * (is_complex ? 2 : 1), 0, L * c.n }; }
-        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
+        Layout layout(const Context &c) const
         {
-            op_ckks_encode(c, L, B, reinterpret_cast<const double *>(a), count, is_complex, scale, out, st);
+            Layout w = unary(count * (is_complex ? 2 : 1), L * c.n);
+            w.in[0].optional = true;
+            return w;
+        }
+        void operator()(Context &c, size_t, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
+        {
+            op_ckks_encode(c, L, B, reinterpret_cast<const double *>(ins[0]), count, is_complex, scale, outs[0], st);
         }
     };
 
@@ -1707,10 +1542,10 @@ namespace
             if (h_values)
                 check_ckks_scalar_values(c, L, batch, kind, h_values, scale);
         }
-        Layout layout(const Context &c) const { return { kind == kCkksScalarComplex ? size_t(2) : size_t(1), 0, L * c.n }; }
-        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
+        Layout layout(const Context &c) const { return unary(kind == kCkksScalarComplex ? 2 : 1, L * c.n); }
+        void operator()(Context &c, size_t, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
         {
-            op_ckks_encode_scalar(c, L, B, kind, a, scale, out, st);
+            op_ckks_encode_scalar(c, L, B, kind, ins[0], scale, outs[0], st);
         }
     };
 
@@ -1719,10 +1554,10 @@ namespace
         size_t L;
         double scale;
         void check(const Context &c, size_t batch) const { check_level(c, L, batch); }
-        Layout layout(const Context &c) const { return { L * c.n, 0, c.n }; }
-        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
+        Layout layout(const Context &c) const { return unary(L * c.n, c.n); }
+        void operator()(Context &c, size_t, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
         {
-            op_ckks_decode(c, L, B, a, scale, reinterpret_cast<double *>(out), st);
+            op_ckks_decode(c, L, B, ins[0], scale, reinterpret_cast<double *>(outs[0]), st);
         }
     };
 
@@ -1732,14 +1567,14 @@ namespace
         size_t L, size;
         const u64 *cf;
         void check(const Context &c, size_t batch) const { check_level(c, L, batch); }
-        Layout layout(const Context &c) const { return { size * L * c.n, 0, c.scheme == SB200_SCHEME_CKKS ? L * c.n : c.n }; }
-        void operator()(Context &c, size_t b0, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
+        Layout layout(const Context &c) const { return unary(size * L * c.n, c.scheme == SB200_SCHEME_CKKS ? L * c.n : c.n); }
+        void operator()(Context &c, size_t b0, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
         {
-            op_decrypt(c, key, L, size, B, a, cf ? cf + b0 : nullptr, out, st);
+            op_decrypt(c, key, L, size, B, ins[0], cf ? cf + b0 : nullptr, outs[0], st);
         }
     };
 
-    // budgets: one int per ciphertext (Layout::out_unit); ciphertexts in the scheme's own form (BFV coefficient, BGV NTT)
+    // budgets: one int per ciphertext (Out::unit); ciphertexts in the scheme's own form (BFV coefficient, BGV NTT)
     struct NoiseBudget
     {
         SecretKey &key;
@@ -1749,57 +1584,104 @@ namespace
             check_level(c, L, batch);
             check_noise_budget(c, key, L, size);
         }
-        Layout layout(const Context &c) const { return { size * L * c.n, 0, 1, false, nullptr, sizeof(int) }; }
-        void operator()(Context &c, size_t, size_t B, const u64 *a, const u64 *, u64 *out, cudaStream_t st) const
+        Layout layout(const Context &c) const
         {
-            op_invariant_noise_budget(c, key, L, size, B, a, reinterpret_cast<int *>(out), st);
+            Layout w = unary(size * L * c.n, 1);
+            w.out[0].unit = sizeof(int);
+            return w;
+        }
+        void operator()(Context &c, size_t, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
+        {
+            op_invariant_noise_budget(c, key, L, size, B, ins[0], reinterpret_cast<int *>(outs[0]), st);
         }
     };
 
     // an entry point's own last step, inside its lock and stream order (the decryption wipes)
     using Then = void (*)(Context &c, cudaStream_t st);
 
-    // Device slabs: the output's byte range may meet an input's only as the exact in-place cases the layout allows (the checks
-    // above have already refused out == a or out == b where the layout forbids them), and then only where every ciphertext's output
-    // sits where its input was: same start and same words per ciphertext.  Any other overlap lets one thread overwrite words
-    // another thread has still to read.  out == a with different words per ciphertext is refused for one ciphertext too: some
-    // kernels would be safe there (the 2 x 2 tensor reads a coefficient's words before writing them), others not (PlainToNtt,
-    // n -> L n words: row i > 0 reads the plaintext words that row 0 overwrites), and the rule does not depend on which.
-    void check_overlap(const Layout &w, size_t batch, const void *a, const void *b, const void *out)
+    // what the errors call input x: its noun and, in a several-operand layout, its index in the caller's array of that noun
+    std::string slab_name(const Layout &w, size_t x)
     {
-        const size_t out_bytes = batch * w.out * w.out_unit, out_stride = w.out * w.out_unit;
-        auto conflict = [&](const void *in, size_t in_bytes, size_t in_stride) {
-            if (!in || !in_bytes || !out_bytes)
-                return false;
-            const auto *x = static_cast<const uint8_t *>(in), *o = static_cast<const uint8_t *>(out);
-            if (!(o < x + in_bytes && x < o + out_bytes))
-                return false;
-            return !(o == x && out_stride == in_stride);
-        };
-        if (conflict(a, batch * w.a * sizeof(u64), w.a * sizeof(u64)))
-            throw std::invalid_argument("the output slab must not overlap input a other than exactly in place");
-        const size_t b_bytes = (w.shared_b ? 1 : batch) * w.b * sizeof(u64);
-        if (conflict(b, b_bytes, w.shared_b ? 0 : w.b * sizeof(u64)))
-            throw std::invalid_argument("the output slab must not overlap input b other than exactly in place");
+        std::string s = w.in[x].noun;
+        if (w.name)
+        {
+            size_t i = 0;
+            for (size_t u = 0; u < x; u++)
+                i += std::strcmp(w.in[u].noun, w.in[x].noun) == 0;
+            s += " [" + std::to_string(i) + "]";
+        }
+        return s;
     }
 
-    template <class Op>
-    int on_stream(sb200_context *ctx, void *stream, size_t batch, const void *a, const void *b, void *out, const Op &op, Then then = nullptr)
+    // every slab is present but an optional input
+    void need_slabs(const Layout &w, const Ins &ins, const Outs &outs)
     {
-        if (!std::is_same<Op, CkksEncode>::value) // the encoder takes no values for an empty vector (checked by CkksEncode)
-            SB_NEED(a);
-        SB_NEED(out);
+        if (ins.size() != w.in.size() || outs.size() != w.out.size())
+            throw std::logic_error("the slabs do not match the operation's layout");
+        for (size_t x = 0; x < ins.size(); x++)
+            if (!ins[x] && !w.in[x].optional)
+                throw null_pointer(slab_name(w, x));
+        for (size_t y = 0; y < outs.size(); y++)
+            if (!outs[y])
+                throw null_pointer(w.name ? "output slab [" + std::to_string(y) + "]" : "output slab");
+    }
+
+    // Device slabs: an output's byte range may meet an input's only where the input allows the output in place, and then only
+    // where every ciphertext's output sits where its input was: same start and same bytes per ciphertext.  It may not meet another
+    // output's.  Any other overlap lets one thread overwrite words another thread has still to read.  An output on an in-place
+    // input with different words per ciphertext is refused for one ciphertext too: some kernels would be safe there (the 2 x 2
+    // tensor reads a coefficient's words before writing them), others not (PlainToNtt, n -> L n words: row i > 0 reads the
+    // plaintext words that row 0 overwrites), and the rule does not depend on which.
+    void check_overlap(const Layout &w, size_t batch, const Ins &ins, const Outs &outs)
+    {
+        auto meet = [](const void *x, size_t nx, const void *y, size_t ny) {
+            const auto *p = static_cast<const uint8_t *>(x), *q = static_cast<const uint8_t *>(y);
+            return nx && ny && p < q + ny && q < p + nx;
+        };
+        if (w.alias) // an output exactly on an input it may not sit on: the operation's own error, ahead of any other overlap
+            for (const void *o : outs)
+                for (size_t x = 0; x < ins.size(); x++)
+                    if (o == ins[x] && !w.in[x].in_place)
+                        throw std::invalid_argument(w.alias);
+        const auto op = [&] { return w.name ? std::string(w.name) + ": " : std::string(); }; // the messages are built when thrown
+        for (size_t y = 0; y < outs.size(); y++)
+        {
+            const size_t stride = w.out[y].words * w.out[y].unit;
+            for (size_t x = 0; x < ins.size(); x++)
+            {
+                const Slab &s = w.in[x];
+                const size_t in_stride = s.shared ? 0 : s.words * sizeof(u64);
+                if (!meet(outs[y], batch * stride, ins[x], s.shared ? s.words * sizeof(u64) : batch * in_stride))
+                    continue;
+                if (outs[y] == ins[x] && s.in_place && stride == in_stride)
+                    continue;
+                throw std::invalid_argument(op() + (w.out.size() > 1 ? "an" : "the") + " output slab must not overlap " + slab_name(w, x) +
+                                            (s.in_place ? " other than exactly in place" : ""));
+            }
+            for (size_t u = 0; u < y; u++)
+                if (meet(outs[y], batch * stride, outs[u], batch * w.out[u].words * w.out[u].unit))
+                    throw std::invalid_argument(op() + "output slabs must not overlap");
+        }
+    }
+
+    // The checks of both drivers, in this order: the slab pointers, then (with the context entered) the operation's own, then the
+    // overlap rule: on device slabs always; on host buffers for the several-operand operations, whose outputs the pipeline could
+    // otherwise copy back over host words a later chunk has still to upload.  The one- and two-input operations keep accepting
+    // overlapping host buffers, as they always have.
+    template <class Op>
+    int on_stream(sb200_context *ctx, void *stream, size_t batch, const InSlabs &in, const OutSlabs &out, const Op &op, Then then = nullptr)
+    {
+        SB_NEED(ctx);
         SB_TRY
+        const Layout w = op.layout(*ctx->c);
+        const Ins ins = in.get();
+        const Outs outs = out.get();
+        need_slabs(w, ins, outs);
         SB_ENTER_STREAM(ctx, stream)
         op.check(c, batch);
-        const Layout w = op.layout(c);
-        if (w.alias && (out == a || (out == b && !w.alias_b_ok)))
-            throw std::invalid_argument(w.alias);
-        if (w.shared_b && out == b)
-            throw std::invalid_argument("the shared plaintext must not alias the output slab");
-        check_overlap(w, batch, a, b, out);
+        check_overlap(w, batch, ins, outs);
         auto st = static_cast<cudaStream_t>(stream);
-        op(c, 0, batch, static_cast<const u64 *>(a), static_cast<const u64 *>(b), static_cast<u64 *>(out), st);
+        op(c, 0, batch, ins.data(), outs.data(), st);
         if (then)
             then(c, st);
         return SB200_OK;
@@ -1807,352 +1689,353 @@ namespace
     }
 
     template <class Op>
-    int on_host(sb200_context *ctx, size_t batch, const void *a, const void *b, void *out, const Op &op, Then then = nullptr)
+    int on_host(sb200_context *ctx, size_t batch, const InSlabs &in, const OutSlabs &out, const Op &op, Then then = nullptr)
     {
-        if (!std::is_same<Op, CkksEncode>::value)
-            SB_NEED(a);
-        SB_NEED(out);
+        SB_NEED(ctx);
         SB_TRY
+        const Layout w = op.layout(*ctx->c);
+        const Ins ins = in.get();
+        const Outs outs = out.get();
+        need_slabs(w, ins, outs);
         SB_ENTER(ctx)
         op.check(c, batch);
-        HostPipe(c).run(batch, op.layout(c), static_cast<const u64 *>(a), static_cast<const u64 *>(b), static_cast<u64 *>(out), op);
+        if (w.name)
+            check_overlap(w, batch, ins, outs);
+        HostPipe(c).run(batch, w, ins, outs, op);
         if (then)
             then(c, c.io.s_comp.get());
         return SB200_OK;
         SB_CATCH
     }
+
 } // namespace
 
 extern "C" {
 
 int sb200_ntt_forward(sb200_context *ctx, size_t L, size_t size, size_t batch, uint64_t *d, void *stream)
 {
-    return on_stream(ctx, stream, batch, d, nullptr, d, Ntt{ false, L, size });
+    return on_stream(ctx, stream, batch, { d }, { d }, Ntt{ false, L, size });
 }
 int sb200_ntt_forward_host(sb200_context *ctx, size_t L, size_t size, size_t batch, uint64_t *h)
 {
-    return on_host(ctx, batch, h, nullptr, h, Ntt{ false, L, size });
+    return on_host(ctx, batch, { h }, { h }, Ntt{ false, L, size });
 }
 int sb200_ntt_inverse(sb200_context *ctx, size_t L, size_t size, size_t batch, uint64_t *d, void *stream)
 {
-    return on_stream(ctx, stream, batch, d, nullptr, d, Ntt{ true, L, size });
+    return on_stream(ctx, stream, batch, { d }, { d }, Ntt{ true, L, size });
 }
 int sb200_ntt_inverse_host(sb200_context *ctx, size_t L, size_t size, size_t batch, uint64_t *h)
 {
-    return on_host(ctx, batch, h, nullptr, h, Ntt{ true, L, size });
+    return on_host(ctx, batch, { h }, { h }, Ntt{ true, L, size });
 }
 
 int sb200_multiply(sb200_context *ctx, size_t L, size_t batch, const uint64_t *a, const uint64_t *b, uint64_t *out3, void *stream)
 {
-    SB_NEED(b);
-    return on_stream(ctx, stream, batch, a, b, out3, Multiply{ L, false });
+    return on_stream(ctx, stream, batch, { a, b }, { out3 }, Multiply{ L, false });
 }
 int sb200_multiply_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *a, const uint64_t *b, uint64_t *out3)
 {
-    SB_NEED(b);
-    return on_host(ctx, batch, a, b, out3, Multiply{ L, false });
+    return on_host(ctx, batch, { a, b }, { out3 }, Multiply{ L, false });
 }
 int sb200_square(sb200_context *ctx, size_t L, size_t batch, const uint64_t *a, uint64_t *out3, void *stream)
 {
-    return on_stream(ctx, stream, batch, a, nullptr, out3, Multiply{ L, true });
+    return on_stream(ctx, stream, batch, { a }, { out3 }, Multiply{ L, true });
 }
 int sb200_square_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *a, uint64_t *out3)
 {
-    return on_host(ctx, batch, a, nullptr, out3, Multiply{ L, true });
+    return on_host(ctx, batch, { a }, { out3 }, Multiply{ L, true });
 }
 
 int sb200_multiply_sized(sb200_context *ctx, size_t L, size_t size_a, size_t size_b, size_t batch, const uint64_t *a, const uint64_t *b,
                          uint64_t *out, void *stream)
 {
-    SB_NEED(b);
-    return on_stream(ctx, stream, batch, a, b, out, MultiplySized{ L, size_a, size_b });
+    return on_stream(ctx, stream, batch, { a, b }, { out }, MultiplySized{ L, size_a, size_b });
 }
 int sb200_multiply_sized_host(sb200_context *ctx, size_t L, size_t size_a, size_t size_b, size_t batch, const uint64_t *a, const uint64_t *b,
                               uint64_t *out)
 {
-    SB_NEED(b);
-    return on_host(ctx, batch, a, b, out, MultiplySized{ L, size_a, size_b });
+    return on_host(ctx, batch, { a, b }, { out }, MultiplySized{ L, size_a, size_b });
 }
 
 int sb200_add(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, const uint64_t *b, uint64_t *out, void *stream)
 {
-    SB_NEED(b);
-    return on_stream(ctx, stream, batch, a, b, out, Linear{ 0, L, size });
+    return on_stream(ctx, stream, batch, { a, b }, { out }, Linear{ 0, L, size });
 }
 int sb200_add_host(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, const uint64_t *b, uint64_t *out)
 {
-    SB_NEED(b);
-    return on_host(ctx, batch, a, b, out, Linear{ 0, L, size });
+    return on_host(ctx, batch, { a, b }, { out }, Linear{ 0, L, size });
 }
 int sb200_sub(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, const uint64_t *b, uint64_t *out, void *stream)
 {
-    SB_NEED(b);
-    return on_stream(ctx, stream, batch, a, b, out, Linear{ 1, L, size });
+    return on_stream(ctx, stream, batch, { a, b }, { out }, Linear{ 1, L, size });
 }
 int sb200_sub_host(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, const uint64_t *b, uint64_t *out)
 {
-    SB_NEED(b);
-    return on_host(ctx, batch, a, b, out, Linear{ 1, L, size });
+    return on_host(ctx, batch, { a, b }, { out }, Linear{ 1, L, size });
 }
 int sb200_negate(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, uint64_t *out, void *stream)
 {
-    return on_stream(ctx, stream, batch, a, nullptr, out, Linear{ 2, L, size });
+    return on_stream(ctx, stream, batch, { a }, { out }, Linear{ 2, L, size });
 }
 int sb200_negate_host(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, uint64_t *out)
 {
-    return on_host(ctx, batch, a, nullptr, out, Linear{ 2, L, size });
+    return on_host(ctx, batch, { a }, { out }, Linear{ 2, L, size });
 }
 
 int sb200_add_many(sb200_context *ctx, size_t L, size_t batch, size_t count, const size_t *sizes, const uint64_t *const *ops, const int *modes,
                    const uint64_t *factors, uint64_t *out, void *stream)
 {
-    return add_many_on_stream(ctx, stream, batch, ops, out, AddMany{ L, count, sizes, modes, reinterpret_cast<const u64 *>(factors) });
+    SB_NEED(sizes);
+    SB_NEED(ops);
+    return on_stream(ctx, stream, batch, InSlabs(ops, count), { out }, AddMany{ L, count, sizes, modes, reinterpret_cast<const u64 *>(factors) });
 }
 int sb200_add_many_host(sb200_context *ctx, size_t L, size_t batch, size_t count, const size_t *sizes, const uint64_t *const *ops, const int *modes,
                         const uint64_t *factors, uint64_t *out)
 {
-    return add_many_on_host(ctx, batch, ops, out, AddMany{ L, count, sizes, modes, reinterpret_cast<const u64 *>(factors) });
+    SB_NEED(sizes);
+    SB_NEED(ops);
+    return on_host(ctx, batch, InSlabs(ops, count), { out }, AddMany{ L, count, sizes, modes, reinterpret_cast<const u64 *>(factors) });
 }
 
 int sb200_multiply_plain_sum(sb200_context *ctx, size_t L, size_t batch, size_t count, size_t outputs, const size_t *sizes,
                              const uint64_t *const *cts, const size_t *plain_counts, const uint64_t *const *plains, int ct_is_ntt,
                              int plain_is_ntt, const int *modes, const uint64_t *factors, uint64_t *const *outs, void *stream)
 {
-    return plain_sum_on_stream(ctx, stream, batch, cts, plains, outs,
-                               PlainSum{ AddMany{ L, count, sizes, modes, reinterpret_cast<const u64 *>(factors) }, outputs, plain_counts,
-                                         ct_is_ntt != 0, plain_is_ntt != 0 });
+    SB_NEED(sizes);
+    SB_NEED(plain_counts);
+    SB_NEED(cts);
+    SB_NEED(plains);
+    SB_NEED(outs);
+    return on_stream(ctx, stream, batch, InSlabs(cts, count, plains, outputs * count), OutSlabs(outs, outputs),
+                     PlainSum{ AddMany{ L, count, sizes, modes, reinterpret_cast<const u64 *>(factors) }, outputs, plain_counts, ct_is_ntt != 0,
+                               plain_is_ntt != 0 });
 }
 int sb200_multiply_plain_sum_host(sb200_context *ctx, size_t L, size_t batch, size_t count, size_t outputs, const size_t *sizes,
                                   const uint64_t *const *cts, const size_t *plain_counts, const uint64_t *const *plains, int ct_is_ntt,
                                   int plain_is_ntt, const int *modes, const uint64_t *factors, uint64_t *const *outs)
 {
-    return plain_sum_on_host(ctx, batch, cts, plains, outs,
-                             PlainSum{ AddMany{ L, count, sizes, modes, reinterpret_cast<const u64 *>(factors) }, outputs, plain_counts,
-                                       ct_is_ntt != 0, plain_is_ntt != 0 });
+    SB_NEED(sizes);
+    SB_NEED(plain_counts);
+    SB_NEED(cts);
+    SB_NEED(plains);
+    SB_NEED(outs);
+    return on_host(ctx, batch, InSlabs(cts, count, plains, outputs * count), OutSlabs(outs, outputs),
+                   PlainSum{ AddMany{ L, count, sizes, modes, reinterpret_cast<const u64 *>(factors) }, outputs, plain_counts, ct_is_ntt != 0,
+                             plain_is_ntt != 0 });
 }
 
 int sb200_multiply_sum(sb200_context *ctx, size_t L, size_t batch, size_t count, size_t outputs, const uint64_t *const *lhs,
                        const uint64_t *const *rhs, const int *modes, const uint64_t *factors, uint64_t *const *outs, void *stream)
 {
-    return multiply_sum_on_stream(ctx, stream, batch, lhs, rhs, outs, MultiplySum{ L, count, outputs, modes, reinterpret_cast<const u64 *>(factors) });
+    SB_NEED(lhs);
+    SB_NEED(rhs);
+    SB_NEED(outs);
+    return on_stream(ctx, stream, batch, InSlabs(lhs, outputs * count, rhs, count), OutSlabs(outs, outputs),
+                     MultiplySum{ L, count, outputs, modes, reinterpret_cast<const u64 *>(factors) });
 }
 int sb200_multiply_sum_host(sb200_context *ctx, size_t L, size_t batch, size_t count, size_t outputs, const uint64_t *const *lhs,
                             const uint64_t *const *rhs, const int *modes, const uint64_t *factors, uint64_t *const *outs)
 {
-    return multiply_sum_on_host(ctx, batch, lhs, rhs, outs, MultiplySum{ L, count, outputs, modes, reinterpret_cast<const u64 *>(factors) });
+    SB_NEED(lhs);
+    SB_NEED(rhs);
+    SB_NEED(outs);
+    return on_host(ctx, batch, InSlabs(lhs, outputs * count, rhs, count), OutSlabs(outs, outputs),
+                   MultiplySum{ L, count, outputs, modes, reinterpret_cast<const u64 *>(factors) });
 }
 
 int sb200_multiply_plain(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, const uint64_t *plain, uint64_t *out,
                          void *stream)
 {
-    SB_NEED(plain);
-    return on_stream(ctx, stream, batch, a, plain, out, MultiplyPlain{ L, size, batch, false });
+    return on_stream(ctx, stream, batch, { a, plain }, { out }, MultiplyPlain{ L, size, batch, false });
 }
 int sb200_multiply_plain_host(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *a, const uint64_t *plain, uint64_t *out)
 {
-    SB_NEED(plain);
-    return on_host(ctx, batch, a, plain, out, MultiplyPlain{ L, size, batch, false });
+    return on_host(ctx, batch, { a, plain }, { out }, MultiplyPlain{ L, size, batch, false });
 }
 int sb200_multiply_plain_n(sb200_context *ctx, size_t L, size_t size, size_t batch, size_t plain_count, const uint64_t *a, const uint64_t *plain,
                            uint64_t *out, void *stream)
 {
-    SB_NEED(plain);
-    return on_stream(ctx, stream, batch, a, plain, out, MultiplyPlain{ L, size, plain_count, plain_count == 1 });
+    return on_stream(ctx, stream, batch, { a, plain }, { out }, MultiplyPlain{ L, size, plain_count, plain_count == 1 });
 }
 int sb200_multiply_plain_n_host(sb200_context *ctx, size_t L, size_t size, size_t batch, size_t plain_count, const uint64_t *a,
                                 const uint64_t *plain, uint64_t *out)
 {
-    SB_NEED(plain);
-    return on_host(ctx, batch, a, plain, out, MultiplyPlain{ L, size, plain_count, plain_count == 1 });
+    return on_host(ctx, batch, { a, plain }, { out }, MultiplyPlain{ L, size, plain_count, plain_count == 1 });
 }
 
 int sb200_add_plain_ntt(sb200_context *ctx, size_t L, size_t size, size_t batch, size_t plain_count, int subtract, const uint64_t *a,
                         const uint64_t *plain, uint64_t *out, void *stream)
 {
-    SB_NEED(plain);
-    return on_stream(ctx, stream, batch, a, plain, out, AddPlainNtt{ L, size, plain_count, plain_count == 1, subtract != 0 });
+    return on_stream(ctx, stream, batch, { a, plain }, { out }, AddPlainNtt{ L, size, plain_count, plain_count == 1, subtract != 0 });
 }
 int sb200_add_plain_ntt_host(sb200_context *ctx, size_t L, size_t size, size_t batch, size_t plain_count, int subtract, const uint64_t *a,
                              const uint64_t *plain, uint64_t *out)
 {
-    SB_NEED(plain);
-    return on_host(ctx, batch, a, plain, out, AddPlainNtt{ L, size, plain_count, plain_count == 1, subtract != 0 });
+    return on_host(ctx, batch, { a, plain }, { out }, AddPlainNtt{ L, size, plain_count, plain_count == 1, subtract != 0 });
 }
 
 int sb200_plain_to_ntt(sb200_context *ctx, size_t L, size_t batch, const uint64_t *plain, uint64_t *out, void *stream)
 {
-    return on_stream(ctx, stream, batch, plain, nullptr, out, PlainToNtt{ L });
+    return on_stream(ctx, stream, batch, { plain }, { out }, PlainToNtt{ L });
 }
 int sb200_plain_to_ntt_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *plain, uint64_t *out)
 {
-    return on_host(ctx, batch, plain, nullptr, out, PlainToNtt{ L });
+    return on_host(ctx, batch, { plain }, { out }, PlainToNtt{ L });
 }
 
 int sb200_multiply_plain_coeff(sb200_context *ctx, size_t L, size_t size, size_t batch, int ct_is_ntt, const uint64_t *a, const uint64_t *plain,
                                uint64_t *out, void *stream)
 {
-    SB_NEED(plain);
-    return on_stream(ctx, stream, batch, a, plain, out, MultiplyPlainCoeff{ L, size, batch, false, ct_is_ntt != 0 });
+    return on_stream(ctx, stream, batch, { a, plain }, { out }, MultiplyPlainCoeff{ L, size, batch, false, ct_is_ntt != 0 });
 }
 int sb200_multiply_plain_coeff_host(sb200_context *ctx, size_t L, size_t size, size_t batch, int ct_is_ntt, const uint64_t *a,
                                     const uint64_t *plain, uint64_t *out)
 {
-    SB_NEED(plain);
-    return on_host(ctx, batch, a, plain, out, MultiplyPlainCoeff{ L, size, batch, false, ct_is_ntt != 0 });
+    return on_host(ctx, batch, { a, plain }, { out }, MultiplyPlainCoeff{ L, size, batch, false, ct_is_ntt != 0 });
 }
 int sb200_multiply_plain_coeff_n(sb200_context *ctx, size_t L, size_t size, size_t batch, size_t plain_count, int ct_is_ntt, const uint64_t *a,
                                  const uint64_t *plain, uint64_t *out, void *stream)
 {
-    SB_NEED(plain);
-    return on_stream(ctx, stream, batch, a, plain, out, MultiplyPlainCoeff{ L, size, plain_count, plain_count == 1, ct_is_ntt != 0 });
+    return on_stream(ctx, stream, batch, { a, plain }, { out }, MultiplyPlainCoeff{ L, size, plain_count, plain_count == 1, ct_is_ntt != 0 });
 }
 int sb200_multiply_plain_coeff_n_host(sb200_context *ctx, size_t L, size_t size, size_t batch, size_t plain_count, int ct_is_ntt,
                                       const uint64_t *a, const uint64_t *plain, uint64_t *out)
 {
-    SB_NEED(plain);
-    return on_host(ctx, batch, a, plain, out, MultiplyPlainCoeff{ L, size, plain_count, plain_count == 1, ct_is_ntt != 0 });
+    return on_host(ctx, batch, { a, plain }, { out }, MultiplyPlainCoeff{ L, size, plain_count, plain_count == 1, ct_is_ntt != 0 });
 }
 
 int sb200_add_plain_coeff(sb200_context *ctx, size_t L, size_t size, size_t batch, int subtract, const uint64_t *a, const uint64_t *plain,
                           const uint64_t *h_correction_factors, uint64_t *out, void *stream)
 {
-    SB_NEED(plain);
-    return on_stream(ctx, stream, batch, a, plain, out, AddPlainCoeff{ L, size, batch, false, subtract != 0, (const u64 *)h_correction_factors });
+    return on_stream(ctx, stream, batch, { a, plain }, { out }, AddPlainCoeff{ L, size, batch, false, subtract != 0, (const u64 *)h_correction_factors });
 }
 int sb200_add_plain_coeff_host(sb200_context *ctx, size_t L, size_t size, size_t batch, int subtract, const uint64_t *a, const uint64_t *plain,
                                const uint64_t *h_correction_factors, uint64_t *out)
 {
-    SB_NEED(plain);
-    return on_host(ctx, batch, a, plain, out, AddPlainCoeff{ L, size, batch, false, subtract != 0, (const u64 *)h_correction_factors });
+    return on_host(ctx, batch, { a, plain }, { out }, AddPlainCoeff{ L, size, batch, false, subtract != 0, (const u64 *)h_correction_factors });
 }
 int sb200_add_plain_coeff_n(sb200_context *ctx, size_t L, size_t size, size_t batch, size_t plain_count, int subtract, const uint64_t *a,
                             const uint64_t *plain, const uint64_t *h_correction_factors, uint64_t *out, void *stream)
 {
-    SB_NEED(plain);
-    return on_stream(ctx, stream, batch, a, plain, out, AddPlainCoeff{ L, size, plain_count, plain_count == 1, subtract != 0, (const u64 *)h_correction_factors });
+    return on_stream(ctx, stream, batch, { a, plain }, { out }, AddPlainCoeff{ L, size, plain_count, plain_count == 1, subtract != 0, (const u64 *)h_correction_factors });
 }
 int sb200_add_plain_coeff_n_host(sb200_context *ctx, size_t L, size_t size, size_t batch, size_t plain_count, int subtract, const uint64_t *a,
                                  const uint64_t *plain, const uint64_t *h_correction_factors, uint64_t *out)
 {
-    SB_NEED(plain);
-    return on_host(ctx, batch, a, plain, out, AddPlainCoeff{ L, size, plain_count, plain_count == 1, subtract != 0, (const u64 *)h_correction_factors });
+    return on_host(ctx, batch, { a, plain }, { out }, AddPlainCoeff{ L, size, plain_count, plain_count == 1, subtract != 0, (const u64 *)h_correction_factors });
 }
 
 int sb200_batch_encode(sb200_context *ctx, size_t batch, const uint64_t *values, uint64_t *plain, void *stream)
 {
-    return on_stream(ctx, stream, batch, values, nullptr, plain, BatchCodec{ false });
+    return on_stream(ctx, stream, batch, { values }, { plain }, BatchCodec{ false });
 }
 int sb200_batch_encode_host(sb200_context *ctx, size_t batch, const uint64_t *values, uint64_t *plain)
 {
-    return on_host(ctx, batch, values, nullptr, plain, BatchCodec{ false });
+    return on_host(ctx, batch, { values }, { plain }, BatchCodec{ false });
 }
 int sb200_batch_decode(sb200_context *ctx, size_t batch, const uint64_t *plain, uint64_t *values, void *stream)
 {
-    return on_stream(ctx, stream, batch, plain, nullptr, values, BatchCodec{ true });
+    return on_stream(ctx, stream, batch, { plain }, { values }, BatchCodec{ true });
 }
 int sb200_batch_decode_host(sb200_context *ctx, size_t batch, const uint64_t *plain, uint64_t *values)
 {
-    return on_host(ctx, batch, plain, nullptr, values, BatchCodec{ true });
+    return on_host(ctx, batch, { plain }, { values }, BatchCodec{ true });
 }
 
 int sb200_relinearize(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in3, const sb200_kswitch_key *key, uint64_t *out2,
                       void *stream)
 {
     SB_NEED(key);
-    return on_stream(ctx, stream, batch, in3, nullptr, out2, Relinearize{ L, key->k });
+    return on_stream(ctx, stream, batch, { in3 }, { out2 }, Relinearize{ L, key->k });
 }
 int sb200_relinearize_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in3, const sb200_kswitch_key *key, uint64_t *out2)
 {
     SB_NEED(key);
-    return on_host(ctx, batch, in3, nullptr, out2, Relinearize{ L, key->k });
+    return on_host(ctx, batch, { in3 }, { out2 }, Relinearize{ L, key->k });
 }
 
 int sb200_multiply_relinearize(sb200_context *ctx, size_t L, size_t batch, const uint64_t *a, const uint64_t *b,
                                const sb200_kswitch_key *key, uint64_t *out2, void *stream)
 {
-    SB_NEED(b);
     SB_NEED(key);
-    return on_stream(ctx, stream, batch, a, b, out2, MultiplyRelinearize{ L, key->k });
+    return on_stream(ctx, stream, batch, { a, b }, { out2 }, MultiplyRelinearize{ L, key->k });
 }
 int sb200_multiply_relinearize_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *a, const uint64_t *b,
                                     const sb200_kswitch_key *key, uint64_t *out2)
 {
-    SB_NEED(b);
     SB_NEED(key);
-    return on_host(ctx, batch, a, b, out2, MultiplyRelinearize{ L, key->k });
+    return on_host(ctx, batch, { a, b }, { out2 }, MultiplyRelinearize{ L, key->k });
 }
 
 int sb200_rescale_to_next_sized(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *in, uint64_t *out, void *stream)
 {
-    return on_stream(ctx, stream, batch, in, nullptr, out, ModSwitch{ true, L, size });
+    return on_stream(ctx, stream, batch, { in }, { out }, ModSwitch{ true, L, size });
 }
 int sb200_rescale_to_next_sized_host(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *in, uint64_t *out)
 {
-    return on_host(ctx, batch, in, nullptr, out, ModSwitch{ true, L, size });
+    return on_host(ctx, batch, { in }, { out }, ModSwitch{ true, L, size });
 }
 int sb200_rescale_to_next(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, uint64_t *out2, void *stream)
 {
-    return on_stream(ctx, stream, batch, in2, nullptr, out2, ModSwitch{ true, L, 2 });
+    return on_stream(ctx, stream, batch, { in2 }, { out2 }, ModSwitch{ true, L, 2 });
 }
 int sb200_rescale_to_next_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, uint64_t *out2)
 {
-    return on_host(ctx, batch, in2, nullptr, out2, ModSwitch{ true, L, 2 });
+    return on_host(ctx, batch, { in2 }, { out2 }, ModSwitch{ true, L, 2 });
 }
 int sb200_mod_switch_to_next_sized(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *in, uint64_t *out, void *stream)
 {
-    return on_stream(ctx, stream, batch, in, nullptr, out, ModSwitch{ false, L, size });
+    return on_stream(ctx, stream, batch, { in }, { out }, ModSwitch{ false, L, size });
 }
 int sb200_mod_switch_to_next_sized_host(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *in, uint64_t *out)
 {
-    return on_host(ctx, batch, in, nullptr, out, ModSwitch{ false, L, size });
+    return on_host(ctx, batch, { in }, { out }, ModSwitch{ false, L, size });
 }
 int sb200_mod_switch_to_next(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, uint64_t *out2, void *stream)
 {
-    return on_stream(ctx, stream, batch, in2, nullptr, out2, ModSwitch{ false, L, 2 });
+    return on_stream(ctx, stream, batch, { in2 }, { out2 }, ModSwitch{ false, L, 2 });
 }
 int sb200_mod_switch_to_next_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, uint64_t *out2)
 {
-    return on_host(ctx, batch, in2, nullptr, out2, ModSwitch{ false, L, 2 });
+    return on_host(ctx, batch, { in2 }, { out2 }, ModSwitch{ false, L, 2 });
 }
 
 int sb200_relinearize_sized(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *in, const sb200_kswitch_key *key,
                             uint64_t *out, void *stream)
 {
     SB_NEED(key);
-    return on_stream(ctx, stream, batch, in, nullptr, out, RelinearizeSized{ L, size, key->k });
+    return on_stream(ctx, stream, batch, { in }, { out }, RelinearizeSized{ L, size, key->k });
 }
 int sb200_relinearize_sized_host(sb200_context *ctx, size_t L, size_t size, size_t batch, const uint64_t *in, const sb200_kswitch_key *key,
                                  uint64_t *out)
 {
     SB_NEED(key);
-    return on_host(ctx, batch, in, nullptr, out, RelinearizeSized{ L, size, key->k });
+    return on_host(ctx, batch, { in }, { out }, RelinearizeSized{ L, size, key->k });
 }
 
 int sb200_apply_galois(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, uint32_t elt, const sb200_kswitch_key *key,
                        uint64_t *out2, void *stream)
 {
     SB_NEED(key);
-    return on_stream(ctx, stream, batch, in2, nullptr, out2, ApplyGalois{ L, elt, key->k });
+    return on_stream(ctx, stream, batch, { in2 }, { out2 }, ApplyGalois{ L, elt, key->k });
 }
 int sb200_apply_galois_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, uint32_t elt, const sb200_kswitch_key *key,
                             uint64_t *out2)
 {
     SB_NEED(key);
-    return on_host(ctx, batch, in2, nullptr, out2, ApplyGalois{ L, elt, key->k });
+    return on_host(ctx, batch, { in2 }, { out2 }, ApplyGalois{ L, elt, key->k });
 }
 int sb200_apply_galois_add(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, uint32_t elt, const sb200_kswitch_key *key,
                            const uint64_t *addend2, uint64_t *out2, void *stream)
 {
     SB_NEED(key);
-    SB_NEED(addend2);
-    return on_stream(ctx, stream, batch, in2, addend2, out2, ApplyGaloisAdd{ L, elt, key->k });
+    return on_stream(ctx, stream, batch, { in2, addend2 }, { out2 }, ApplyGaloisAdd{ L, elt, key->k });
 }
 int sb200_apply_galois_add_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *a, uint32_t elt, const sb200_kswitch_key *key,
                                 const uint64_t *b, uint64_t *out2)
 {
     SB_NEED(key);
-    SB_NEED(b);
-    return on_host(ctx, batch, a, b, out2, ApplyGaloisAdd{ L, elt, key->k });
+    return on_host(ctx, batch, { a, b }, { out2 }, ApplyGaloisAdd{ L, elt, key->k });
 }
 int sb200_rotate_sum(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, size_t steps, const uint32_t *elts,
                      const sb200_kswitch_key *const *keys, uint64_t *out2, void *stream)
@@ -2160,7 +2043,7 @@ int sb200_rotate_sum(sb200_context *ctx, size_t L, size_t batch, const uint64_t 
     std::vector<const KSwitchKey *> k;
     if (int e = rotate_sum_keys(steps, elts, keys, k))
         return e;
-    return on_stream(ctx, stream, batch, in2, nullptr, out2, RotateSum{ L, steps, elts, k.data() });
+    return on_stream(ctx, stream, batch, { in2 }, { out2 }, RotateSum{ L, steps, elts, k.data() });
 }
 int sb200_rotate_sum_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, size_t steps, const uint32_t *elts,
                           const sb200_kswitch_key *const *keys, uint64_t *out2)
@@ -2168,7 +2051,7 @@ int sb200_rotate_sum_host(sb200_context *ctx, size_t L, size_t batch, const uint
     std::vector<const KSwitchKey *> k;
     if (int e = rotate_sum_keys(steps, elts, keys, k))
         return e;
-    return on_host(ctx, batch, in2, nullptr, out2, RotateSum{ L, steps, elts, k.data() });
+    return on_host(ctx, batch, { in2 }, { out2 }, RotateSum{ L, steps, elts, k.data() });
 }
 
 // ---- wire format (SURVEY 8f rank 3): Ciphertext::save / load, compr_mode none, between byte streams and device slabs ----
@@ -2419,32 +2302,32 @@ int sb200_encrypt_asymmetric(sb200_context *ctx, sb200_public_key *key, size_t L
 int sb200_ckks_encode(sb200_context *ctx, size_t L, size_t batch, const double *d_values, size_t count, int is_complex, double scale,
                       uint64_t *d_plain, void *stream)
 {
-    return on_stream(ctx, stream, batch, d_values, nullptr, d_plain, CkksEncode{ L, count, is_complex != 0, d_values != nullptr, scale });
+    return on_stream(ctx, stream, batch, { d_values }, { d_plain }, CkksEncode{ L, count, is_complex != 0, d_values != nullptr, scale });
 }
 int sb200_ckks_encode_host(sb200_context *ctx, size_t L, size_t batch, const double *h_values, size_t count, int is_complex, double scale,
                            uint64_t *h_plain)
 {
-    return on_host(ctx, batch, h_values, nullptr, h_plain, CkksEncode{ L, count, is_complex != 0, h_values != nullptr, scale });
+    return on_host(ctx, batch, { h_values }, { h_plain }, CkksEncode{ L, count, is_complex != 0, h_values != nullptr, scale });
 }
 
 int sb200_ckks_encode_scalar(sb200_context *ctx, size_t L, size_t batch, int kind, const void *d_values, double scale, uint64_t *d_plain,
                              void *stream)
 {
-    return on_stream(ctx, stream, batch, d_values, nullptr, d_plain, CkksEncodeScalar{ L, kind, scale, nullptr });
+    return on_stream(ctx, stream, batch, { d_values }, { d_plain }, CkksEncodeScalar{ L, kind, scale, nullptr });
 }
 int sb200_ckks_encode_scalar_host(sb200_context *ctx, size_t L, size_t batch, int kind, const void *h_values, double scale,
                                   uint64_t *h_plain)
 {
-    return on_host(ctx, batch, h_values, nullptr, h_plain, CkksEncodeScalar{ L, kind, scale, static_cast<const u64 *>(h_values) });
+    return on_host(ctx, batch, { h_values }, { h_plain }, CkksEncodeScalar{ L, kind, scale, static_cast<const u64 *>(h_values) });
 }
 
 int sb200_ckks_decode(sb200_context *ctx, size_t L, size_t batch, const uint64_t *d_plain, double scale, double *d_values, void *stream)
 {
-    return on_stream(ctx, stream, batch, d_plain, nullptr, d_values, CkksDecode{ L, scale });
+    return on_stream(ctx, stream, batch, { d_plain }, { d_values }, CkksDecode{ L, scale });
 }
 int sb200_ckks_decode_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *h_plain, double scale, double *h_values)
 {
-    return on_host(ctx, batch, h_plain, nullptr, h_values, CkksDecode{ L, scale });
+    return on_host(ctx, batch, { h_plain }, { h_values }, CkksDecode{ L, scale });
 }
 
 // Encryptor::encrypt_zero_symmetric for a batch (sb_prng.cu); h_bootstrap_seeds == nullptr: fresh seeds from the OS entropy source,
@@ -2822,14 +2705,14 @@ int sb200_decrypt(sb200_context *ctx, sb200_secret_key *key, size_t L, size_t si
                   const uint64_t *h_correction_factors, uint64_t *plain, void *stream)
 {
     SB_NEED(key);
-    return on_stream(ctx, stream, batch, ct, nullptr, plain, Decrypt{ key->k, L, size, (const u64 *)h_correction_factors }, wipe_stream);
+    return on_stream(ctx, stream, batch, { ct }, { plain }, Decrypt{ key->k, L, size, (const u64 *)h_correction_factors }, wipe_stream);
 }
 
 int sb200_decrypt_host(sb200_context *ctx, sb200_secret_key *key, size_t L, size_t size, size_t batch, const uint64_t *ct,
                        const uint64_t *h_correction_factors, uint64_t *plain)
 {
     SB_NEED(key);
-    return on_host(ctx, batch, ct, nullptr, plain, Decrypt{ key->k, L, size, (const u64 *)h_correction_factors }, wipe_host);
+    return on_host(ctx, batch, { ct }, { plain }, Decrypt{ key->k, L, size, (const u64 *)h_correction_factors }, wipe_host);
 }
 
 // Decryptor::invariant_noise_budget: the phases depend on the secret key, so the arenas are wiped as after a decryption
@@ -2837,14 +2720,14 @@ int sb200_invariant_noise_budget(sb200_context *ctx, sb200_secret_key *key, size
                                  int *d_budgets, void *stream)
 {
     SB_NEED(key);
-    return on_stream(ctx, stream, batch, d_ct, nullptr, d_budgets, NoiseBudget{ key->k, L, size }, wipe_stream);
+    return on_stream(ctx, stream, batch, { d_ct }, { d_budgets }, NoiseBudget{ key->k, L, size }, wipe_stream);
 }
 
 int sb200_invariant_noise_budget_host(sb200_context *ctx, sb200_secret_key *key, size_t L, size_t size, size_t batch, const uint64_t *h_ct,
                                       int *h_budgets)
 {
     SB_NEED(key);
-    return on_host(ctx, batch, h_ct, nullptr, h_budgets, NoiseBudget{ key->k, L, size }, wipe_host);
+    return on_host(ctx, batch, { h_ct }, { h_budgets }, NoiseBudget{ key->k, L, size }, wipe_host);
 }
 
 } // extern "C"

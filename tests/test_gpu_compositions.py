@@ -217,6 +217,26 @@ def test_chunked_by_scratch_limit():
     assert_words(_host(out), want, "small scratch budget")
 
 
+def test_host_staging_chunks():
+    """the host entry point cut into several staging chunks with a ragged last one, equal word for word to the stream form"""
+    import torch
+
+    S = sb()
+    n, bits, L, B = 4096, [50, 40, 60], 2, 7
+    mods = sb().coeff_modulus_create(n, bits)
+    ctx = S.Context(S.BGV, n, mods, batching_prime(n, 20))
+    rng = np.random.default_rng(13)
+    sizes = [3, 2, 4, 2]
+    ops = rand_ops(rng, mods, n, L, B, sizes)
+    modes, factors = [S.FOLD_SUB, S.FOLD_SCALED, S.FOLD_SUB | S.FOLD_SCALED], [[0, 0], [3, 5], [7, 11]]
+    out = _dev(np.zeros((B, 4, L, n), dtype=np.uint64))
+    ctx.d_add_many([_dev(o) for o in ops], out, L, B, sizes, modes, factors)
+    torch.cuda.synchronize()
+    per_ct = (sum(sizes) + 4) * L * n * 8
+    ctx.set_limit(ctx.LIMIT_HOST_STAGE_BYTES, 2 * per_ct)  # chunks of 2, 2, 2, 1 members
+    assert_words(ctx.add_many(ops, modes, factors), _host(out), "chunked host form vs stream form")
+
+
 def test_argument_errors_leave_output_untouched():
     S = sb()
     n, bits, L, B = 4096, [50, 40, 60], 2, 2
@@ -244,6 +264,15 @@ def test_argument_errors_leave_output_untouched():
         ctx.d_add_many([big, d[1]], big, L, B, [2, 3])
     with pytest.raises(ValueError):
         ctx.add_many([], None)
+    # the host form refuses the same overlaps: here the output on operand 0, which is smaller (SB200_E_INVALID_ARG, nothing written)
+    lib = S.lib()
+    h = rng.integers(0, 2**63, (B, 3, L, n), dtype=np.uint64)  # room for the output's three polynomials
+    before = h.copy()
+    c_sizes, c_modes, _ = ctx._fold_args([2, 3], None, None)
+    ptrs = (C.c_void_p * 2)(h.ctypes.data, np.ascontiguousarray(ops[1]).ctypes.data)
+    assert lib.sb200_add_many_host(ctx.h, L, B, 2, c_sizes, ptrs, c_modes, None, S._hp(h)) == -1
+    assert b"add_many: the output slab must not overlap an operand [0] other than exactly in place" in lib.sb200_last_error()
+    assert_words(h, before, "host output after a rejected call")
 
 
 @needs_ref

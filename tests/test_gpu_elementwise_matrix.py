@@ -613,7 +613,7 @@ def test_shared_plain_256_primes():
     DONE.add(f"n{n}-60-bit-k256")
 
 
-@pytest.mark.parametrize("op", ["add", "multiply", "rescale_to_next", "apply_galois"])
+@pytest.mark.parametrize("op", ["add", "multiply", "rescale_to_next", "apply_galois", "add_many"])
 def test_overlapping_slabs_refused(op):
     """a stream entry point refuses an output slab that overlaps an input slab other than exactly in place
     (SB200_E_INVALID_ARG), before any launch: the output words stay as they were.  Every slab lies inside one allocation large
@@ -639,6 +639,9 @@ def test_overlapping_slabs_refused(op):
     elif op == "rescale_to_next":  # the output of L - 1 primes starts inside the input
         call = lambda: ctx.d_rescale_to_next_sized(at(0), at(B * poly), L, 2, B)
         out_words = (B * poly, B * poly + 2 * B * (L - 1) * n)
+    elif op == "add_many":  # the output starts one polynomial inside operand 1, away from operand 0
+        call = lambda: ctx.d_add_many([at(8 * B * poly), at(0)], at(poly), L, B, [2, 2])
+        out_words = (poly, poly + 2 * B * poly)
     else:
         key = ctx.load_key(np.stack([np.stack([np.stack([rng.integers(0, mods[i], n, dtype=np.uint64) for i in range(k)])
                                                for _ in range(2)]) for _ in range(k - 1)]))
@@ -646,7 +649,8 @@ def test_overlapping_slabs_refused(op):
         out_words = (2 * poly, 2 * poly + 2 * B * poly)
     before = to_np(base[out_words[0]:out_words[1]]).copy()
     launches = ctx.launch_count
-    with pytest.raises(ValueError, match="must not overlap input"):  # SB200_E_INVALID_ARG from the overlap check
+    message = r"add_many: the output slab must not overlap an operand \[1\]" if op == "add_many" else "must not overlap input"
+    with pytest.raises(ValueError, match=message):  # SB200_E_INVALID_ARG from the overlap check
         call()
     torch.cuda.synchronize()
     assert ctx.launch_count == launches, op

@@ -289,6 +289,21 @@ def test_errors_leave_outputs_unchanged():
             assert_words(host(d_rhs[i]), rhs[i], f"right operand {i} unchanged after '{msg}'")
         for x in range(M * K):
             assert_words(host(d_lhs[x]), lhs[x], f"left operand {x} unchanged after '{msg}'")
+    # the host form refuses the same overlaps: here output 0 on left-hand operand 1 (SB200_E_INVALID_ARG, nothing written)
+    import ctypes as C
+
+    lib = S.lib()
+    h_lhs, h_rhs = [np.ascontiguousarray(a) for a in lhs], [np.ascontiguousarray(a) for a in rhs]
+    big = rng.integers(0, 2**64, (B, 3, L, n), dtype=np.uint64)  # left-hand operand 1 with room for the output's three polynomials
+    before = big.copy()
+    h_outs = [big, np.zeros((B, 3, L, n), dtype=np.uint64)]
+    p_lhs = (C.c_void_p * (M * K))(*[big.ctypes.data if x == 1 else h_lhs[x].ctypes.data for x in range(M * K)])
+    p_rhs = (C.c_void_p * K)(*[a.ctypes.data for a in h_rhs])
+    p_outs = (C.c_void_p * M)(*[o.ctypes.data for o in h_outs])
+    assert lib.sb200_multiply_sum_host(ctx.h, L, B, K, M, p_lhs, p_rhs, None, None, p_outs) == -1
+    assert b"multiply_sum: an output slab must not overlap a left-hand operand [1]" in lib.sb200_last_error()
+    assert_words(big, before, "host output after a rejected call")
+    assert_words(h_outs[1], np.zeros_like(h_outs[1]), "second host output after a rejected call")
     # BFV: a level above sb200_multiply's limit, raised before add_many's mode check (the chain's order)
     n_b, L_b = 4096, 65
     mods_b = [int(q) for q in O.get_primes(2 * n_b, 30, 66)]

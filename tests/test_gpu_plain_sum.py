@@ -268,7 +268,10 @@ def test_deep_levels(n, L, K, M):
 
 @pytest.mark.parametrize("forms", [(True, True), (False, False)])
 def test_host_staging_chunks(forms):
-    """the host entry point cut into several staging chunks (a ragged last one), shared plaintexts uploaded once"""
+    """the host entry point cut into several staging chunks (a ragged last one), shared plaintexts uploaded once, equal word for
+    word to the stream form"""
+    import torch
+
     n = 4096
     mods, t, ctx = context(sb().BFV, n, [50, 40, 60])
     rng = np.random.default_rng(6000 + forms[0])
@@ -282,9 +285,13 @@ def test_host_staging_chunks(forms):
     ctx.set_limit(ctx.LIMIT_HOST_STAGE_BYTES, 2 * per_ct)  # chunks of 2, 2, 2, 1 members
     cut = ctx.multiply_plain_sum(cts, plains, None, None, *forms)
     want = chain(ctx, cts, plains, K, M, *forms)
+    d_outs = [dev(np.zeros_like(w)) for w in whole]
+    ctx.d_multiply_plain_sum([dev(c) for c in cts], [dev(p) for p in plains], d_outs, L, B, sizes, counts, *forms)
+    torch.cuda.synchronize()
     for j in range(M):
-        assert_words(cut[j], whole[j], f"chunked vs one chunk, output {j}")
+        assert_words(cut[j], whole[j], f"chunked vs default staging, output {j}")
         assert_words(cut[j], want[j], f"chunked vs chain, output {j}")
+        assert_words(cut[j], host(d_outs[j]), f"chunked host form vs stream form, output {j}")
 
 
 def test_errors_leave_outputs_unchanged():
