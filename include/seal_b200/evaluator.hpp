@@ -24,6 +24,7 @@
 #include <mutex>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 namespace seal_b200
@@ -277,29 +278,14 @@ namespace seal_b200
         {
             validate(encrypted1, "encrypted1 is not valid for encryption parameters");
             validate(encrypted2, "encrypted2 is not valid for encryption parameters");
-            if (encrypted1.parms_id() != encrypted2.parms_id())
-                throw std::invalid_argument("encrypted1 and encrypted2 parameter mismatch");
-            if (!pool)
-                throw std::invalid_argument("pool is uninitialized");
-            const bool ckks = scheme_ == seal::scheme_type::ckks, bgv = scheme_ == seal::scheme_type::bgv;
-            if ((ckks || bgv) && !(encrypted1.is_ntt_form() && encrypted2.is_ntt_form()))
-                throw std::invalid_argument("encrypted1 or encrypted2 must be in NTT form"); // :571-574, :712-715
-            if (!(ckks || bgv) && (encrypted1.is_ntt_form() || encrypted2.is_ntt_form()))
-                throw std::invalid_argument("encrypted1 or encrypted2 cannot be in NTT form"); // :397-400
-            auto cd = context_.get_context_data(encrypted1.parms_id());
+            const Meta r = multiply_meta(meta(encrypted1), meta(encrypted2), &pool);
             const std::size_t L = encrypted1.coeff_modulus_size(), n = encrypted1.poly_modulus_degree();
             const std::size_t s1 = encrypted1.size(), s2 = encrypted2.size(); // any sizes: :524-560, :664-700, :796-833
             std::vector<std::uint64_t> a(encrypted1.data(), encrypted1.data() + s1 * L * n);
-            double new_scale = encrypted1.scale() * encrypted2.scale();
-            if (ckks && !scale_within_bounds(new_scale, *cd))
-                throw std::invalid_argument("scale out of bounds"); // :703-707
-            encrypted1.resize(context_, cd->parms_id(), s1 + s2 - 1); // throws on > SEAL_CIPHERTEXT_SIZE_MAX like the reference
+            encrypted1.resize(context_, r.parms_id, r.size);
             check(sb200_multiply_sized_host(ctx_, L, s1, s2, 1, a.data(), encrypted2.data(), encrypted1.data()));
-            if (ckks)
-                encrypted1.scale() = new_scale;
-            if (bgv) // :838-840
-                encrypted1.correction_factor() = seal::util::multiply_uint_mod(
-                    encrypted1.correction_factor(), encrypted2.correction_factor(), cd->parms().plain_modulus());
+            encrypted1.scale() = r.scale;
+            encrypted1.correction_factor() = r.cf;
             throw_if_transparent(encrypted1);
         }
         void multiply(const seal::Ciphertext &encrypted1, const seal::Ciphertext &encrypted2, seal::Ciphertext &destination,
@@ -378,11 +364,10 @@ namespace seal_b200
                 throw std::invalid_argument("plain is not valid for encryption parameters");
             if (!pool)
                 throw std::invalid_argument("pool is uninitialized");
+            const Meta r = multiply_plain_meta(meta(encrypted), meta(plain));
             if (!plain.is_ntt_form())
             {
                 // multiply_plain_normal (:2021-2155) / transform + multiply_plain_ntt (:1999-2004)
-                if (scheme_ == seal::scheme_type::ckks)
-                    throw std::invalid_argument("plain is not valid for encryption parameters"); // CKKS plaintexts are always in NTT form
                 const std::vector<std::uint64_t> words = padded(plain);
                 check(sb200_multiply_plain_coeff_host(ctx_, encrypted.coeff_modulus_size(), encrypted.size(), 1, encrypted.is_ntt_form() ? 1 : 0,
                                                       encrypted.data(), words.data(), encrypted.data()));
@@ -392,13 +377,9 @@ namespace seal_b200
             const bool back = !encrypted.is_ntt_form(); // :2006-2011: to NTT form, multiply, back
             if (back)
                 transform_to_ntt_inplace(encrypted);
-            if (encrypted.parms_id() != plain.parms_id())
-                throw std::invalid_argument("encrypted_ntt and plain_ntt parameter mismatch"); // :2164-2167
             check(sb200_multiply_plain_host(ctx_, encrypted.coeff_modulus_size(), encrypted.size(), 1, encrypted.data(), plain.data(),
                                             encrypted.data()));
-            encrypted.scale() *= plain.scale();
-            if (!scale_within_bounds(encrypted.scale(), *context_.get_context_data(encrypted.parms_id())))
-                throw std::invalid_argument("scale out of bounds"); // :2189-2193
+            encrypted.scale() = r.scale;
             if (back)
                 transform_from_ntt_inplace(encrypted);
             throw_if_transparent(encrypted);
@@ -518,7 +499,7 @@ namespace seal_b200
         void mod_switch_to_inplace(seal::Ciphertext &encrypted, seal::parms_id_type parms_id,
                                    seal::MemoryPoolHandle pool = seal::MemoryManager::GetPool()) const
         {
-            check_target_level(encrypted, parms_id);
+            check_target_level(encrypted.parms_id(), parms_id);
             while (encrypted.parms_id() != parms_id)
                 mod_switch_to_next_inplace(encrypted, pool);
         }
@@ -532,11 +513,7 @@ namespace seal_b200
                                 seal::MemoryPoolHandle pool = seal::MemoryManager::GetPool()) const
         {
             validate(encrypted, "encrypted is not valid for encryption parameters");
-            check_target_level(encrypted, parms_id);
-            if (!pool)
-                throw std::invalid_argument("pool is uninitialized");
-            if (scheme_ != seal::scheme_type::ckks)
-                throw std::invalid_argument("unsupported operation for scheme type");
+            check_target_level(encrypted.parms_id(), parms_id, true, &pool);
             while (encrypted.parms_id() != parms_id)
             {
                 seal::Ciphertext next;
@@ -556,10 +533,7 @@ namespace seal_b200
         void mod_reduce_to_next_inplace(seal::Ciphertext &encrypted, seal::MemoryPoolHandle pool = seal::MemoryManager::GetPool()) const
         {
             validate(encrypted, "encrypted is not valid for encryption parameters");
-            if (context_.last_parms_id() == encrypted.parms_id())
-                throw std::invalid_argument("end of modulus switching chain reached");
-            if (!pool)
-                throw std::invalid_argument("pool is uninitialized");
+            check_mod_switch_to_next(meta(encrypted), false, &pool);
             drop_last_component(encrypted);
             throw_if_transparent(encrypted);
         }
@@ -572,7 +546,7 @@ namespace seal_b200
         void mod_reduce_to_inplace(seal::Ciphertext &encrypted, seal::parms_id_type parms_id,
                                    seal::MemoryPoolHandle pool = seal::MemoryManager::GetPool()) const
         {
-            check_target_level(encrypted, parms_id);
+            check_target_level(encrypted.parms_id(), parms_id);
             while (encrypted.parms_id() != parms_id)
                 mod_reduce_to_next_inplace(encrypted, pool);
         }
@@ -587,14 +561,7 @@ namespace seal_b200
         {
             if (!seal::is_valid_for(plain, context_))
                 throw std::invalid_argument("plain is not valid for encryption parameters");
-            auto cd = context_.get_context_data(plain.parms_id());
-            if (!plain.is_ntt_form())
-                throw std::invalid_argument("plain is not in NTT form");
-            if (!cd->next_context_data())
-                throw std::invalid_argument("end of modulus switching chain reached");
-            auto &next = *cd->next_context_data();
-            if (!scale_within_bounds(plain.scale(), next))
-                throw std::invalid_argument("scale out of bounds");
+            auto &next = plain_next_level(meta(plain));
             const std::size_t words = next.parms().coeff_modulus().size() * next.parms().poly_modulus_degree();
             plain.parms_id() = seal::parms_id_zero;
             plain.resize(words);
@@ -607,16 +574,9 @@ namespace seal_b200
         }
         void mod_switch_to_inplace(seal::Plaintext &plain, seal::parms_id_type parms_id) const
         {
-            auto cur = context_.get_context_data(plain.parms_id());
-            auto target = context_.get_context_data(parms_id);
-            if (!cur)
+            if (!context_.get_context_data(plain.parms_id()))
                 throw std::invalid_argument("plain is not valid for encryption parameters");
-            if (!target)
-                throw std::invalid_argument("parms_id is not valid for encryption parameters");
-            if (!plain.is_ntt_form())
-                throw std::invalid_argument("plain is not in NTT form");
-            if (cur->chain_index() < target->chain_index())
-                throw std::invalid_argument("cannot switch to higher level modulus");
+            check_plain_target_level(meta(plain), parms_id);
             while (plain.parms_id() != parms_id)
                 mod_switch_to_next_inplace(plain);
         }
@@ -633,15 +593,11 @@ namespace seal_b200
             auto cd = context_.get_context_data(encrypted.parms_id());
             if (!cd)
                 throw std::invalid_argument("encrypted is not valid for encryption parameters");
-            if (relin_keys.parms_id() != context_.key_parms_id())
-                throw std::invalid_argument("relin_keys is not valid for encryption parameters");
-            if (encrypted.size() < 2)
-                throw std::invalid_argument("destination_size must be at least 2 and less than or equal to current count");
-            if (relin_keys.size() < encrypted.size() - 2)
-                throw std::invalid_argument("not enough relinearization keys");
+            check_relinearize(relin_keys, encrypted.size());
             if (encrypted.size() == 2)
                 return;
-            check_keyswitch_operand(encrypted, pool);
+            validate(encrypted, "encrypted is not valid for encryption parameters");
+            check_switch_key(encrypted.is_ntt_form(), &pool);
             const std::size_t L = encrypted.coeff_modulus_size(), n = encrypted.poly_modulus_degree(), size = encrypted.size();
             std::lock_guard<std::mutex> lock(mu_);
             if (size == 3)
@@ -678,12 +634,7 @@ namespace seal_b200
                              seal::MemoryPoolHandle pool = seal::MemoryManager::GetPool()) const
         {
             validate(encrypted, "encrypted is not valid for encryption parameters");
-            if (context_.last_parms_id() == encrypted.parms_id())
-                throw std::invalid_argument("end of modulus switching chain reached");
-            if (!pool)
-                throw std::invalid_argument("pool is uninitialized");
-            if (scheme_ != seal::scheme_type::ckks)
-                throw std::invalid_argument("unsupported operation for scheme type");
+            check_mod_switch_to_next(meta(encrypted), true, &pool);
             mod_switch_impl(encrypted, destination, true);
         }
         void rescale_to_next_inplace(seal::Ciphertext &encrypted, seal::MemoryPoolHandle pool = seal::MemoryManager::GetPool()) const
@@ -694,10 +645,7 @@ namespace seal_b200
                                 seal::MemoryPoolHandle pool = seal::MemoryManager::GetPool()) const
         {
             validate(encrypted, "encrypted is not valid for encryption parameters");
-            if (context_.last_parms_id() == encrypted.parms_id())
-                throw std::invalid_argument("end of modulus switching chain reached");
-            if (!pool)
-                throw std::invalid_argument("pool is uninitialized");
+            check_mod_switch_to_next(meta(encrypted), false, &pool);
             mod_switch_impl(encrypted, destination, false);
         }
         void mod_switch_to_next_inplace(seal::Ciphertext &encrypted, seal::MemoryPoolHandle pool = seal::MemoryManager::GetPool()) const
@@ -710,16 +658,8 @@ namespace seal_b200
                                   seal::MemoryPoolHandle pool = seal::MemoryManager::GetPool()) const
         {
             validate(encrypted, "encrypted is not valid for encryption parameters");
-            if (galois_keys.parms_id() != context_.key_parms_id())
-                throw std::invalid_argument("galois_keys is not valid for encryption parameters");
-            if (!galois_keys.has_key(galois_elt))
-                throw std::invalid_argument("Galois key not present");
+            check_apply_galois(meta(encrypted), galois_elt, galois_keys, &pool);
             const std::size_t L = encrypted.coeff_modulus_size(), n = encrypted.poly_modulus_degree();
-            if (!(galois_elt & 1) || galois_elt >= 2 * n)
-                throw std::invalid_argument("Galois element is not valid");
-            if (encrypted.size() != 2)
-                throw std::invalid_argument("encrypted size must be 2");
-            check_keyswitch_operand(encrypted, pool);
             std::lock_guard<std::mutex> lock(mu_); // the cached key stays valid (not evicted) while the operation uses it
             sb200_kswitch_key *key = key_for(galois_keys, seal::GaloisKeys::get_index(galois_elt), L);
             std::vector<std::uint64_t> in(encrypted.data(), encrypted.data() + 2 * L * n);
@@ -842,36 +782,27 @@ namespace seal_b200
         }
 
         // ---- batch extension: destination[i] = relinearize(multiply(a[i], b[i])), one device pass over the batch ----
-        // (upload through page-locked staging, fused multiply + relinearize on the device, download).  Scales and BGV correction
-        // factors may differ from ciphertext to ciphertext; they are computed before anything is written, so destination may
-        // alias a or b.
+        // (upload through page-locked staging, fused multiply + relinearize on the device, download).  The checks are
+        // multiply_inplace's for every entry, then relinearize_inplace's; the entries must have size 2 and share one level.  Scales and
+        // BGV correction factors may differ from ciphertext to ciphertext; they are computed before anything is written, so
+        // destination may alias a or b.
         void multiply_relinearize(const std::vector<seal::Ciphertext> &a, const std::vector<seal::Ciphertext> &b,
                                   const seal::RelinKeys &relin_keys, std::vector<seal::Ciphertext> &destination) const
         {
             if (a.size() != b.size() || a.empty())
                 throw std::invalid_argument("batch size mismatch");
-            if (relin_keys.parms_id() != context_.key_parms_id())
-                throw std::invalid_argument("relin_keys is not valid for encryption parameters");
             const std::size_t B = a.size();
-            const bool ckks = scheme_ == seal::scheme_type::ckks, ntt = scheme_ != seal::scheme_type::bfv;
-            auto cd = context_.get_context_data(a[0].parms_id());
-            std::vector<double> scales(B);
-            std::vector<std::uint64_t> factors(B);
+            std::vector<Meta> products;
             for (std::size_t i = 0; i < B; i++)
             {
                 validate(a[i], "encrypted1 is not valid for encryption parameters");
                 validate(b[i], "encrypted2 is not valid for encryption parameters");
-                if (a[i].parms_id() != a[0].parms_id() || b[i].parms_id() != a[0].parms_id())
-                    throw std::invalid_argument("encrypted1 and encrypted2 parameter mismatch");
-                if (a[i].size() != 2 || b[i].size() != 2 || a[i].is_ntt_form() != ntt || b[i].is_ntt_form() != ntt)
+                products.push_back(multiply_meta(meta(a[i]), meta(b[i])));
+                if (a[i].size() != 2 || b[i].size() != 2 || a[i].parms_id() != a[0].parms_id())
                     throw std::invalid_argument("batch entries must be fresh size-2 ciphertexts in the scheme's native form");
-                scales[i] = ckks ? a[i].scale() * b[i].scale() : a[i].scale(); // evaluator.cpp:703-707; BFV / BGV leave the scale alone
-                if (ckks && !scale_within_bounds(scales[i], *cd))
-                    throw std::invalid_argument("scale out of bounds");
-                factors[i] = scheme_ == seal::scheme_type::bgv
-                                 ? seal::util::multiply_uint_mod(a[i].correction_factor(), b[i].correction_factor(), cd->parms().plain_modulus())
-                                 : a[i].correction_factor();
             }
+            check_relinearize(relin_keys, 3);
+            check_switch_key(products[0].ntt);
             CiphertextBatch da, db;
             upload_rows(a.data(), B, da);
             upload_rows(b.data(), B, db);
@@ -880,8 +811,8 @@ namespace seal_b200
             download(da, destination);
             for (std::size_t i = 0; i < B; i++)
             {
-                destination[i].scale() = scales[i];
-                destination[i].correction_factor() = factors[i];
+                destination[i].scale() = products[i].scale;
+                destination[i].correction_factor() = products[i].cf;
             }
         }
 
@@ -937,7 +868,7 @@ namespace seal_b200
             owned(source);
             std::lock_guard<std::mutex> lock(mu_);
             shape(destination, source.batch_, source.size_, source.L_, source.n_);
-            copy_meta(source, destination);
+            assign(destination, meta(source));
             check(sb200_memcpy_d2d(ctx_, destination.d_, source.d_, source.batch_ * source.words_per_ciphertext() * sizeof(std::uint64_t), nullptr));
         }
         // Ciphertext::load / unsafe_load (ciphertext.cpp:249-395) of `count` streams into one batch: none, zlib and seeded streams,
@@ -1021,29 +952,13 @@ namespace seal_b200
         void multiply_inplace(CiphertextBatch &encrypted1, const CiphertextBatch &encrypted2) const
         {
             owned(encrypted1), owned(encrypted2);
-            if (encrypted1.parms_id_ != encrypted2.parms_id_ || encrypted1.batch_ != encrypted2.batch_)
-                throw std::invalid_argument("encrypted1 and encrypted2 parameter mismatch");
-            const bool ckks = scheme_ == seal::scheme_type::ckks, bgv = scheme_ == seal::scheme_type::bgv;
-            if ((ckks || bgv) && !(encrypted1.ntt_ && encrypted2.ntt_))
-                throw std::invalid_argument("encrypted1 or encrypted2 must be in NTT form");
-            if (!(ckks || bgv) && (encrypted1.ntt_ || encrypted2.ntt_))
-                throw std::invalid_argument("encrypted1 or encrypted2 cannot be in NTT form");
-            auto cd = context_.get_context_data(encrypted1.parms_id_);
-            const std::size_t s1 = encrypted1.size_, s2 = encrypted2.size_, so = s1 + s2 - 1;
-            if (so > SEAL_CIPHERTEXT_SIZE_MAX)
-                throw std::invalid_argument("invalid size");
-            const double new_scale = encrypted1.scale_ * encrypted2.scale_;
-            if (ckks && !scale_within_bounds(new_scale, *cd))
-                throw std::invalid_argument("scale out of bounds");
+            const Meta r = multiply_meta(meta(encrypted1), meta(encrypted2));
             std::lock_guard<std::mutex> lock(mu_);
-            std::uint64_t *out = out_slab(encrypted1.batch_ * so * encrypted1.L_ * encrypted1.n_, encrypted1);
-            check(sb200_multiply_sized(ctx_, encrypted1.L_, s1, s2, encrypted1.batch_, encrypted1.d_, encrypted2.d_, out, nullptr));
+            std::uint64_t *out = out_slab(encrypted1.batch_ * r.size * encrypted1.L_ * encrypted1.n_, encrypted1);
+            check(sb200_multiply_sized(ctx_, encrypted1.L_, encrypted1.size_, encrypted2.size_, encrypted1.batch_, encrypted1.d_, encrypted2.d_, out,
+                                       nullptr));
             adopt(encrypted1);
-            encrypted1.size_ = so;
-            if (ckks)
-                encrypted1.scale_ = new_scale;
-            if (bgv)
-                encrypted1.cf_ = seal::util::multiply_uint_mod(encrypted1.cf_, encrypted2.cf_, cd->parms().plain_modulus());
+            assign(encrypted1, r);
         }
         void square_inplace(CiphertextBatch &encrypted) const { multiply_inplace(encrypted, encrypted); }
         // Evaluator::relinearize_inplace (evaluator.cpp:1144-1199).  Every key-switching member of a batch takes the keys as a seal::
@@ -1065,15 +980,10 @@ namespace seal_b200
         void relinearize_batch(CiphertextBatch &encrypted, const RelinKeys &relin_keys) const
         {
             owned(encrypted);
-            if (relin_keys.parms_id() != context_.key_parms_id())
-                throw std::invalid_argument("relin_keys is not valid for encryption parameters");
-            if (encrypted.size_ < 2)
-                throw std::invalid_argument("destination_size must be at least 2 and less than or equal to current count");
-            if (relin_keys.size() < encrypted.size_ - 2)
-                throw std::invalid_argument("not enough relinearization keys");
+            check_relinearize(relin_keys, encrypted.size_);
             if (encrypted.size_ == 2)
                 return;
-            check_keyswitch_form(encrypted.ntt_);
+            check_switch_key(encrypted.ntt_);
             std::lock_guard<std::mutex> lock(mu_);
             const std::size_t size = encrypted.size_, poly = encrypted.L_ * encrypted.n_;
             if (size == 3)
@@ -1104,32 +1014,20 @@ namespace seal_b200
         void multiply_relinearize_batch(CiphertextBatch &encrypted1, const CiphertextBatch &encrypted2, const RelinKeys &relin_keys) const
         {
             owned(encrypted1), owned(encrypted2);
-            if (encrypted1.parms_id_ != encrypted2.parms_id_ || encrypted1.batch_ != encrypted2.batch_)
-                throw std::invalid_argument("encrypted1 and encrypted2 parameter mismatch");
-            if (relin_keys.parms_id() != context_.key_parms_id())
-                throw std::invalid_argument("relin_keys is not valid for encryption parameters");
             if (encrypted1.size_ != 2 || encrypted2.size_ != 2)
             {
                 multiply_inplace(encrypted1, encrypted2);
                 relinearize_inplace(encrypted1, relin_keys);
                 return;
             }
-            const bool ckks = scheme_ == seal::scheme_type::ckks, bgv = scheme_ == seal::scheme_type::bgv;
-            if ((ckks || bgv) != encrypted1.ntt_ || (ckks || bgv) != encrypted2.ntt_)
-                throw std::invalid_argument((ckks || bgv) ? "encrypted1 or encrypted2 must be in NTT form" : "encrypted1 or encrypted2 cannot be in NTT form");
-            auto cd = context_.get_context_data(encrypted1.parms_id_);
-            const double new_scale = encrypted1.scale_ * encrypted2.scale_;
-            if (ckks && !scale_within_bounds(new_scale, *cd))
-                throw std::invalid_argument("scale out of bounds");
-            if (!context_.using_keyswitching())
-                throw std::logic_error("keyswitching is not supported by the context");
+            Meta r = multiply_meta(meta(encrypted1), meta(encrypted2)); // the chain's checks: multiply_inplace's, relinearize_inplace's
+            check_relinearize(relin_keys, r.size);
+            check_switch_key(r.ntt);
             std::lock_guard<std::mutex> lock(mu_);
             sb200_kswitch_key *key = key_for(relin_keys, seal::RelinKeys::get_index(2), encrypted1.L_);
             check(sb200_multiply_relinearize(ctx_, encrypted1.L_, encrypted1.batch_, encrypted1.d_, encrypted2.d_, key, encrypted1.d_, nullptr));
-            if (ckks)
-                encrypted1.scale_ = new_scale;
-            if (bgv)
-                encrypted1.cf_ = seal::util::multiply_uint_mod(encrypted1.cf_, encrypted2.cf_, cd->parms().plain_modulus());
+            r.size = 2;
+            assign(encrypted1, r);
         }
 
     public:
@@ -1137,17 +1035,13 @@ namespace seal_b200
         void rescale_to_next_inplace(CiphertextBatch &encrypted) const
         {
             owned(encrypted);
-            if (context_.last_parms_id() == encrypted.parms_id_)
-                throw std::invalid_argument("end of modulus switching chain reached");
-            if (scheme_ != seal::scheme_type::ckks)
-                throw std::invalid_argument("unsupported operation for scheme type");
+            check_mod_switch_to_next(meta(encrypted), true);
             mod_switch_batch(encrypted, true);
         }
         void mod_switch_to_next_inplace(CiphertextBatch &encrypted) const
         {
             owned(encrypted);
-            if (context_.last_parms_id() == encrypted.parms_id_)
-                throw std::invalid_argument("end of modulus switching chain reached");
+            check_mod_switch_to_next(meta(encrypted), false);
             mod_switch_batch(encrypted, false);
         }
         // add / sub / negate (evaluator.cpp:130-350), any sizes and correction factors: the result takes the larger size, the longer
@@ -1165,16 +1059,20 @@ namespace seal_b200
             for (auto &e : encrypteds)
                 if (&e == &destination)
                     throw std::invalid_argument("encrypteds must be different from destination");
-            std::vector<const CiphertextBatch *> ops;
-            for (auto &e : encrypteds)
-                ops.push_back(&e);
-            const Fold f = plan_fold(ops, std::vector<int>(ops.size() - 1, SB200_FOLD_ADD));
             const CiphertextBatch &e0 = encrypteds[0];
+            owned(e0);
+            Fold f{ meta(e0), { e0.size_ }, {}, {} };
+            std::vector<const std::uint64_t *> ptrs{ e0.d_ };
+            for (std::size_t j = 1; j < encrypteds.size(); j++)
+            {
+                owned(encrypteds[j]);
+                fold_in(f, meta(encrypteds[j]), SB200_FOLD_ADD);
+                ptrs.push_back(encrypteds[j].d_);
+            }
             std::lock_guard<std::mutex> lock(mu_);
-            shape(destination, e0.batch_, f.out_size, e0.L_, e0.n_);
-            copy_meta(e0, destination);
-            destination.cf_ = f.cf;
-            check(sb200_add_many(ctx_, e0.L_, e0.batch_, ops.size(), f.sizes.data(), f.ptrs.data(), f.modes.data(),
+            shape(destination, e0.batch_, f.result.size, e0.L_, e0.n_);
+            assign(destination, f.result);
+            check(sb200_add_many(ctx_, e0.L_, e0.batch_, ptrs.size(), f.sizes.data(), ptrs.data(), f.modes.data(),
                                  f.factors.empty() ? nullptr : f.factors.data(), destination.d_, nullptr));
         }
         // Sums of plaintext products, member-wise: destination j is add_many over i of multiply_plain(encrypteds[i], plains[j K + i])
@@ -1354,9 +1252,7 @@ namespace seal_b200
         void rescale_to_inplace(CiphertextBatch &encrypted, seal::parms_id_type parms_id) const
         {
             owned(encrypted);
-            check_target_level(encrypted.parms_id_, parms_id);
-            if (scheme_ != seal::scheme_type::ckks)
-                throw std::invalid_argument("unsupported operation for scheme type");
+            check_target_level(encrypted.parms_id_, parms_id, true);
             while (encrypted.parms_id_ != parms_id)
                 rescale_to_next_inplace(encrypted);
         }
@@ -1441,30 +1337,17 @@ namespace seal_b200
         }
 
     private:
-        // apply_galois_inplace's checks (evaluator.cpp:2384-2430), in its order, up to the key lookup
-        template <class GaloisKeys>
-        void check_apply_galois(const CiphertextBatch &encrypted, std::uint32_t galois_elt, const GaloisKeys &galois_keys) const
-        {
-            owned(encrypted);
-            if (galois_keys.parms_id() != context_.key_parms_id())
-                throw std::invalid_argument("galois_keys is not valid for encryption parameters");
-            if (!galois_keys.has_key(galois_elt))
-                throw std::invalid_argument("Galois key not present");
-            if (!(galois_elt & 1) || galois_elt >= 2 * encrypted.n_)
-                throw std::invalid_argument("Galois element is not valid");
-            if (encrypted.size_ != 2)
-                throw std::invalid_argument("encrypted size must be 2");
-            check_keyswitch_form(encrypted.ntt_);
-        }
         template <class GaloisKeys>
         void apply_galois_add_batch(CiphertextBatch &destination, const CiphertextBatch &encrypted, std::uint32_t galois_elt,
                                     const GaloisKeys &galois_keys) const
         {
-            check_apply_galois(encrypted, galois_elt, galois_keys);
+            owned(encrypted);
+            check_apply_galois(meta(encrypted), galois_elt, galois_keys);
             {
                 std::lock_guard<std::mutex> lock(mu_);
                 sb200_kswitch_key *key = key_for(galois_keys, seal::GaloisKeys::get_index(galois_elt), encrypted.L_);
-                const Fold f = plan_fold({ &destination, &encrypted }, { SB200_FOLD_ADD }); // add_inplace(destination, t)
+                owned(destination);
+                const Fold f = plan_fold({ meta(destination), meta(encrypted) }, SB200_FOLD_ADD); // add_inplace(destination, t)
                 if (f.factors.empty() && destination.size_ == 2)
                 {
                     const bool same = &destination == &encrypted; // out must not be the input: through the result slab
@@ -1492,10 +1375,7 @@ namespace seal_b200
             const bool ckks = scheme_ == seal::scheme_type::ckks;
             if (!ckks && scheme_ != seal::scheme_type::bfv && scheme_ != seal::scheme_type::bgv)
                 throw std::logic_error("unsupported scheme");
-            owned(encrypted);
-            auto cd = context_.get_context_data(encrypted.parms_id_);
-            if (!cd->qualifiers().using_batching)
-                throw std::logic_error("encryption parameters do not support batching");
+            auto cd = batching_level(encrypted);
             if (galois_keys.parms_id() != context_.key_parms_id())
                 throw std::invalid_argument("galois_keys is not valid for encryption parameters");
             std::vector<std::uint32_t> elts;
@@ -1520,12 +1400,12 @@ namespace seal_b200
                 {
                     CiphertextBatch t;
                     copy(encrypted, t);
-                    rotate_batch(t, static_cast<int>(static_cast<long long>(step) * (1ll << j)), galois_keys);
+                    rotate_internal(t, static_cast<int>(static_cast<long long>(step) * (1ll << j)), galois_keys);
                     add_inplace(encrypted, t);
                 }
                 return;
             }
-            check_apply_galois(encrypted, elts[0], galois_keys);
+            check_apply_galois(meta(encrypted), elts[0], galois_keys);
             std::lock_guard<std::mutex> lock(mu_);
             std::vector<const sb200_kswitch_key *> keys;
             struct Unpin // the keys of this call stay in the cache until it returns
@@ -1544,7 +1424,8 @@ namespace seal_b200
         template <class GaloisKeys>
         void apply_galois_batch(CiphertextBatch &encrypted, std::uint32_t galois_elt, const GaloisKeys &galois_keys) const
         {
-            check_apply_galois(encrypted, galois_elt, galois_keys);
+            owned(encrypted);
+            check_apply_galois(meta(encrypted), galois_elt, galois_keys);
             std::lock_guard<std::mutex> lock(mu_);
             sb200_kswitch_key *key = key_for(galois_keys, seal::GaloisKeys::get_index(galois_elt), encrypted.L_);
             std::uint64_t *out = out_slab(encrypted.batch_ * encrypted.words_per_ciphertext(), encrypted);
@@ -1556,28 +1437,28 @@ namespace seal_b200
         {
             if (scheme_ != seal::scheme_type::bfv && scheme_ != seal::scheme_type::bgv)
                 throw std::logic_error("unsupported scheme");
-            rotate_batch(encrypted, steps, galois_keys);
+            rotate_internal(encrypted, steps, galois_keys);
         }
         template <class GaloisKeys>
         void rotate_vector_batch(CiphertextBatch &encrypted, int steps, const GaloisKeys &galois_keys) const
         {
             if (scheme_ != seal::scheme_type::ckks)
                 throw std::logic_error("unsupported scheme");
-            rotate_batch(encrypted, steps, galois_keys);
+            rotate_internal(encrypted, steps, galois_keys);
         }
         template <class GaloisKeys>
         void rotate_columns_batch(CiphertextBatch &encrypted, const GaloisKeys &galois_keys) const
         {
             if (scheme_ != seal::scheme_type::bfv && scheme_ != seal::scheme_type::bgv)
                 throw std::logic_error("unsupported scheme");
-            conjugate_batch(encrypted, galois_keys);
+            conjugate_internal(encrypted, galois_keys);
         }
         template <class GaloisKeys>
         void complex_conjugate_batch(CiphertextBatch &encrypted, const GaloisKeys &galois_keys) const
         {
             if (scheme_ != seal::scheme_type::ckks)
                 throw std::logic_error("unsupported scheme");
-            conjugate_batch(encrypted, galois_keys);
+            conjugate_internal(encrypted, galois_keys);
         }
 
     public:
@@ -1672,14 +1553,7 @@ namespace seal_b200
         void mod_switch_to_next_inplace(PlaintextBatch &plain) const
         {
             owned(plain);
-            auto cd = context_.get_context_data(plain.parms_id_);
-            if (!plain.ntt_)
-                throw std::invalid_argument("plain is not in NTT form");
-            if (!cd->next_context_data())
-                throw std::invalid_argument("end of modulus switching chain reached");
-            auto &next = *cd->next_context_data();
-            if (!scale_within_bounds(plain.scale_, next))
-                throw std::invalid_argument("scale out of bounds");
+            auto &next = plain_next_level(meta(plain));
             const std::size_t L = plain.L_, n = plain.n_, row = (L - 1) * n * sizeof(std::uint64_t);
             std::lock_guard<std::mutex> lock(mu_);
             PlaintextBatch out;
@@ -1691,14 +1565,7 @@ namespace seal_b200
         void mod_switch_to_inplace(PlaintextBatch &plain, seal::parms_id_type parms_id) const
         {
             owned(plain);
-            auto cur = context_.get_context_data(plain.parms_id_);
-            auto target = context_.get_context_data(parms_id);
-            if (!target)
-                throw std::invalid_argument("parms_id is not valid for encryption parameters");
-            if (!plain.ntt_)
-                throw std::invalid_argument("plain is not in NTT form");
-            if (cur->chain_index() < target->chain_index())
-                throw std::invalid_argument("cannot switch to higher level modulus");
+            check_plain_target_level(meta(plain), parms_id);
             while (plain.parms_id_ != parms_id)
                 mod_switch_to_next_inplace(plain);
         }
@@ -1707,22 +1574,16 @@ namespace seal_b200
         {
             owned(encrypted), owned(plain);
             plain_count(encrypted, plain);
+            const Meta r = multiply_plain_meta(meta(encrypted), meta(plain));
             const std::size_t L = encrypted.L_, size = encrypted.size_, B = encrypted.batch_;
             if (!plain.ntt_)
             {
                 // multiply_plain_normal (:2021-2155) / transform + multiply_plain_ntt (:1999-2004)
-                if (scheme_ == seal::scheme_type::ckks)
-                    throw std::invalid_argument("plain is not valid for encryption parameters"); // CKKS plaintexts are always in NTT form
                 std::lock_guard<std::mutex> lock(mu_);
                 check(sb200_multiply_plain_coeff_n(ctx_, L, size, B, plain.batch_, encrypted.ntt_ ? 1 : 0, encrypted.d_, plain.d_, encrypted.d_,
                                                    nullptr));
                 return;
             }
-            if (encrypted.parms_id_ != plain.parms_id_)
-                throw std::invalid_argument("encrypted_ntt and plain_ntt parameter mismatch"); // :2164-2167
-            const double new_scale = encrypted.scale_ * plain.scale_;
-            if (!scale_within_bounds(new_scale, *context_.get_context_data(encrypted.parms_id_)))
-                throw std::invalid_argument("scale out of bounds"); // :2189-2193
             const bool back = !encrypted.ntt_; // :2006-2011: to NTT form, multiply, back
             std::lock_guard<std::mutex> lock(mu_);
             if (back)
@@ -1730,7 +1591,7 @@ namespace seal_b200
             check(sb200_multiply_plain_n(ctx_, L, size, B, plain.batch_, encrypted.d_, plain.d_, encrypted.d_, nullptr));
             if (back)
                 check(sb200_ntt_inverse(ctx_, L, size, B, encrypted.d_, nullptr));
-            encrypted.scale_ = new_scale;
+            encrypted.scale_ = r.scale;
         }
         // add_plain_inplace / sub_plain_inplace (evaluator.cpp:1759-1866, :1867-1974)
         void add_plain_inplace(CiphertextBatch &encrypted, const PlaintextBatch &plain) const { plain_linear_batch(encrypted, plain, false); }
@@ -1769,24 +1630,17 @@ namespace seal_b200
         {
             validate(encrypted1, "encrypted1 is not valid for encryption parameters");
             validate(encrypted2, "encrypted2 is not valid for encryption parameters");
-            if (encrypted1.parms_id() != encrypted2.parms_id())
-                throw std::invalid_argument("encrypted1 and encrypted2 parameter mismatch");
-            if (encrypted1.is_ntt_form() != encrypted2.is_ntt_form())
-                throw std::invalid_argument("NTT form mismatch");
-            if (!seal::util::are_close<double>(encrypted1.scale(), encrypted2.scale()))
-                throw std::invalid_argument("scale mismatch");
+            const Fold f = plan_fold({ meta(encrypted1), meta(encrypted2) }, subtract ? SB200_FOLD_SUB : SB200_FOLD_ADD);
             auto cd = context_.get_context_data(encrypted1.parms_id());
             const std::size_t L = encrypted1.coeff_modulus_size(), n = encrypted1.poly_modulus_degree();
-            if (encrypted1.correction_factor() != encrypted2.correction_factor())
+            if (!f.factors.empty())
             {
-                // BGV: bring both operands to a common correction factor first (evaluator.cpp:188-209, :305-326)
-                std::uint64_t f, e1, e2;
-                balance_factors(encrypted1.correction_factor(), encrypted2.correction_factor(), cd->parms().plain_modulus(), f, e1, e2);
+                // BGV: bring both operands to a common correction factor first
                 seal::Ciphertext copy = encrypted2;
-                scale_by(encrypted1, e1, *cd);
-                scale_by(copy, e2, *cd);
-                encrypted1.correction_factor() = f;
-                copy.correction_factor() = f;
+                scale_by(encrypted1, f.factors[0], *cd);
+                scale_by(copy, f.factors[1], *cd);
+                encrypted1.correction_factor() = f.result.cf;
+                copy.correction_factor() = f.result.cf;
                 linear(encrypted1, copy, subtract);
                 return;
             }
@@ -1861,33 +1715,19 @@ namespace seal_b200
         // mod_switch_drop_to_next (evaluator.cpp:1296-1366): every polynomial keeps its first L-1 components
         void drop_last_component(seal::Ciphertext &encrypted) const
         {
-            auto cd = context_.get_context_data(encrypted.parms_id());
-            const auto scheme = cd->parms().scheme();
-            if (scheme == seal::scheme_type::bfv && encrypted.is_ntt_form())
-                throw std::invalid_argument("BFV encrypted cannot be in NTT form");
-            if (scheme == seal::scheme_type::ckks && !encrypted.is_ntt_form())
-                throw std::invalid_argument("CKKS encrypted must be in NTT form");
-            if (scheme == seal::scheme_type::bgv && !encrypted.is_ntt_form())
-                throw std::invalid_argument("BGV encrypted must be in NTT form");
-            auto &next = *cd->next_context_data();
-            if (!scale_within_bounds(encrypted.scale(), next))
-                throw std::invalid_argument("scale out of bounds");
+            const Meta r = mod_switch_to_next_meta(meta(encrypted), true);
             const std::size_t L = encrypted.coeff_modulus_size(), n = encrypted.poly_modulus_degree(), size = encrypted.size();
             std::vector<std::uint64_t> kept(size * (L - 1) * n);
             for (std::size_t p = 0; p < size; p++)
                 std::memcpy(kept.data() + p * (L - 1) * n, encrypted.data(p), (L - 1) * n * sizeof(std::uint64_t));
-            const bool ntt = encrypted.is_ntt_form();
-            const double scale = encrypted.scale();
-            const std::uint64_t correction = encrypted.correction_factor();
-            encrypted.resize(context_, next.parms_id(), size);
+            encrypted.resize(context_, r.parms_id, size);
             std::memcpy(encrypted.data(), kept.data(), kept.size() * sizeof(std::uint64_t));
-            encrypted.is_ntt_form() = ntt, encrypted.scale() = scale, encrypted.correction_factor() = correction;
+            encrypted.is_ntt_form() = r.ntt, encrypted.scale() = r.scale, encrypted.correction_factor() = r.cf;
         }
-        void check_target_level(const seal::Ciphertext &encrypted, const seal::parms_id_type &parms_id) const
-        {
-            check_target_level(encrypted.parms_id(), parms_id);
-        }
-        void check_target_level(const seal::parms_id_type &current, const seal::parms_id_type &parms_id) const
+        // the checks of mod_switch_to_inplace / rescale_to_inplace (evaluator.cpp:1451-1473, :1543-1590) and
+        // mod_reduce_to_inplace (:1625-1647) before their single steps; pool is the seal::Ciphertext members' pool
+        void check_target_level(const seal::parms_id_type &current, const seal::parms_id_type &parms_id, bool rescale = false,
+                                const seal::MemoryPoolHandle *pool = nullptr) const
         {
             auto cur = context_.get_context_data(current);
             auto target = context_.get_context_data(parms_id);
@@ -1897,22 +1737,20 @@ namespace seal_b200
                 throw std::invalid_argument("parms_id is not valid for encryption parameters");
             if (cur->chain_index() < target->chain_index())
                 throw std::invalid_argument("cannot switch to higher level modulus");
+            check_pool(pool);
+            if (rescale && scheme_ != seal::scheme_type::ckks)
+                throw std::invalid_argument("unsupported operation for scheme type");
         }
         void plain_linear(seal::Ciphertext &encrypted, const seal::Plaintext &plain, bool subtract) const
         {
             validate(encrypted, "encrypted is not valid for encryption parameters");
             if (!seal::is_metadata_valid_for(plain, context_) || !seal::is_buffer_valid(plain))
                 throw std::invalid_argument("plain is not valid for encryption parameters");
+            check_add_plain(meta(encrypted), meta(plain));
             if (scheme_ != seal::scheme_type::ckks)
             {
                 // BFV: scaling variant on c_0 (util/scalingvariant.cpp:70-160); BGV: correction factor, lift, NTT (:1838-1849)
                 const bool bfv = scheme_ == seal::scheme_type::bfv;
-                if (bfv && encrypted.is_ntt_form())
-                    throw std::invalid_argument("BFV encrypted cannot be in NTT form");
-                if (!bfv && !encrypted.is_ntt_form())
-                    throw std::invalid_argument("BGV encrypted must be in NTT form");
-                if (plain.is_ntt_form())
-                    throw std::invalid_argument(bfv ? "BFV plain cannot be in NTT form" : "BGV plain cannot be in NTT form");
                 const std::vector<std::uint64_t> words = padded(plain);
                 const std::uint64_t cf = encrypted.correction_factor();
                 check(sb200_add_plain_coeff_host(ctx_, encrypted.coeff_modulus_size(), encrypted.size(), 1, subtract ? 1 : 0, encrypted.data(),
@@ -1920,14 +1758,6 @@ namespace seal_b200
                 throw_if_transparent(encrypted);
                 return;
             }
-            if (!encrypted.is_ntt_form())
-                throw std::invalid_argument("CKKS encrypted must be in NTT form");
-            if (!plain.is_ntt_form())
-                throw std::invalid_argument("CKKS plain must be in NTT form");
-            if (encrypted.parms_id() != plain.parms_id())
-                throw std::invalid_argument("encrypted and plain parameter mismatch");
-            if (!seal::util::are_close<double>(encrypted.scale(), plain.scale()))
-                throw std::invalid_argument("scale mismatch");
             const std::size_t L = encrypted.coeff_modulus_size();
             // c_0 +/- plain: a one-polynomial slab (add_poly_coeffmod / sub_poly_coeffmod on encrypted[0], :1831-1836)
             check(subtract ? sb200_sub_host(ctx_, L, 1, 1, encrypted.data(), plain.data(), encrypted.data())
@@ -1970,20 +1800,257 @@ namespace seal_b200
                                                                         : cd.parms().plain_modulus().bit_count();
             return !(!std::isnormal(scale) || scale <= 0 || (static_cast<int>(std::log2(scale)) >= bound));
         }
-        // the parts of switch_key_inplace's prologue that concern the operand (evaluator.cpp:2573-2611)
-        void check_keyswitch_operand(const seal::Ciphertext &encrypted, const seal::MemoryPoolHandle &pool) const
+
+        // ---- the reference's preconditions, one function per rule, shared by the seal::Ciphertext and CiphertextBatch members ----
+        // Each runs its checks in the reference's order on the operands' metadata, after the member's own operand checks (validate()
+        // and the pool for a seal::Ciphertext, owned() and the batch counts for a batch), and returns the result's metadata where the
+        // operation changes it.  pool is the seal::Ciphertext members' pool, checked where they check it; batches pass none.
+        struct Meta
         {
-            validate(encrypted, "encrypted is not valid for encryption parameters");
+            seal::parms_id_type parms_id = seal::parms_id_zero;
+            std::size_t size = 0;
+            bool ntt = false;
+            double scale = 1.0;
+            std::uint64_t cf = 1;  // correction factor
+            std::size_t batch = 1; // 1 for a seal::Ciphertext
+        };
+        static Meta meta(const seal::Ciphertext &c)
+        {
+            return { c.parms_id(), c.size(), c.is_ntt_form(), c.scale(), c.correction_factor(), 1 };
+        }
+        static Meta meta(const CiphertextBatch &b) { return { b.parms_id_, b.size_, b.ntt_, b.scale_, b.cf_, b.batch_ }; }
+        static Meta meta(const seal::Plaintext &p) { return { p.parms_id(), 0, p.is_ntt_form(), p.scale() }; }
+        static Meta meta(const PlaintextBatch &p) { return { p.parms_id_, 0, p.ntt_, p.scale_, 1, p.batch_ }; }
+        static void assign(CiphertextBatch &b, const Meta &m)
+        {
+            b.parms_id_ = m.parms_id, b.size_ = m.size, b.ntt_ = m.ntt, b.scale_ = m.scale, b.cf_ = m.cf;
+        }
+        static void check_pool(const seal::MemoryPoolHandle *pool)
+        {
+            if (pool && !*pool)
+                throw std::invalid_argument("pool is uninitialized");
+        }
+        // the per-scheme form of an operand (mod_switch_scale_to_next, evaluator.cpp:1205-1217; mod_switch_drop_to_next :1300-1312;
+        // add_plain_inplace :1774-1808; switch_key_inplace :2601-2611)
+        void check_ntt_form(bool ntt) const
+        {
+            if (scheme_ == seal::scheme_type::bfv && ntt)
+                throw std::invalid_argument("BFV encrypted cannot be in NTT form");
+            if (scheme_ == seal::scheme_type::ckks && !ntt)
+                throw std::invalid_argument("CKKS encrypted must be in NTT form");
+            if (scheme_ == seal::scheme_type::bgv && !ntt)
+                throw std::invalid_argument("BGV encrypted must be in NTT form");
+        }
+        // multiply_inplace (evaluator.cpp:352-393; bfv_multiply :397-400, ckks_multiply :571-574, :703-707 with the resize's size
+        // check first, bgv_multiply :712-715, :838-840)
+        Meta multiply_meta(const Meta &a, const Meta &b, const seal::MemoryPoolHandle *pool = nullptr) const
+        {
+            if (a.parms_id != b.parms_id || a.batch != b.batch)
+                throw std::invalid_argument("encrypted1 and encrypted2 parameter mismatch");
+            check_pool(pool);
+            const bool bfv = scheme_ == seal::scheme_type::bfv;
+            if (bfv && (a.ntt || b.ntt))
+                throw std::invalid_argument("encrypted1 or encrypted2 cannot be in NTT form");
+            if (!bfv && !(a.ntt && b.ntt))
+                throw std::invalid_argument("encrypted1 or encrypted2 must be in NTT form");
+            Meta r = a;
+            r.size = a.size + b.size - 1;
+            if (r.size > SEAL_CIPHERTEXT_SIZE_MAX)
+                throw std::invalid_argument("invalid size");
+            auto &cd = *context_.get_context_data(a.parms_id);
+            if (scheme_ == seal::scheme_type::ckks)
+            {
+                r.scale = a.scale * b.scale;
+                if (!scale_within_bounds(r.scale, cd))
+                    throw std::invalid_argument("scale out of bounds");
+            }
+            if (scheme_ == seal::scheme_type::bgv)
+                r.cf = seal::util::multiply_uint_mod(a.cf, b.cf, cd.parms().plain_modulus());
+            return r;
+        }
+        // multiply_plain_inplace (evaluator.cpp:1975-2019): a coefficient-form plaintext (never CKKS) leaves the metadata alone;
+        // multiply_plain_ntt (:2157-2195) checks the level and the product's scale
+        Meta multiply_plain_meta(const Meta &encrypted, const Meta &plain) const
+        {
+            if (!plain.ntt)
+            {
+                if (scheme_ == seal::scheme_type::ckks)
+                    throw std::invalid_argument("plain is not valid for encryption parameters"); // CKKS plaintexts are always in NTT form
+                return encrypted;
+            }
+            if (encrypted.parms_id != plain.parms_id)
+                throw std::invalid_argument("encrypted_ntt and plain_ntt parameter mismatch"); // :2164-2167
+            Meta r = encrypted;
+            r.scale = encrypted.scale * plain.scale;
+            if (!scale_within_bounds(r.scale, *context_.get_context_data(encrypted.parms_id)))
+                throw std::invalid_argument("scale out of bounds"); // :2189-2193
+            return r;
+        }
+        // add_plain_inplace / sub_plain_inplace (evaluator.cpp:1759-1866, :1867-1974)
+        void check_add_plain(const Meta &encrypted, const Meta &plain) const
+        {
+            check_ntt_form(encrypted.ntt);
+            if (scheme_ == seal::scheme_type::bfv && plain.ntt)
+                throw std::invalid_argument("BFV plain cannot be in NTT form");
+            if (scheme_ == seal::scheme_type::bgv && plain.ntt)
+                throw std::invalid_argument("BGV plain cannot be in NTT form");
+            if (scheme_ != seal::scheme_type::ckks)
+                return;
+            if (!plain.ntt)
+                throw std::invalid_argument("CKKS plain must be in NTT form");
+            if (encrypted.parms_id != plain.parms_id)
+                throw std::invalid_argument("encrypted and plain parameter mismatch");
+            if (!seal::util::are_close<double>(encrypted.scale, plain.scale))
+                throw std::invalid_argument("scale mismatch");
+        }
+        // relinearize_internal down to size 2 (evaluator.cpp:1144-1168): the key level, the size and the number of keys
+        template <class RelinKeys>
+        void check_relinearize(const RelinKeys &relin_keys, std::size_t size) const
+        {
+            if (relin_keys.parms_id() != context_.key_parms_id())
+                throw std::invalid_argument("relin_keys is not valid for encryption parameters");
+            if (size < 2)
+                throw std::invalid_argument("destination_size must be at least 2 and less than or equal to current count");
+            if (relin_keys.size() < size - 2)
+                throw std::invalid_argument("not enough relinearization keys");
+        }
+        // the parts of switch_key_inplace's prologue that concern the operand (evaluator.cpp:2573-2611)
+        void check_switch_key(bool ntt, const seal::MemoryPoolHandle *pool = nullptr) const
+        {
             if (!context_.using_keyswitching())
                 throw std::logic_error("keyswitching is not supported by the context");
-            if (!pool)
-                throw std::invalid_argument("pool is uninitialized");
-            if (scheme_ == seal::scheme_type::bfv && encrypted.is_ntt_form())
-                throw std::invalid_argument("BFV encrypted cannot be in NTT form");
-            if (scheme_ == seal::scheme_type::ckks && !encrypted.is_ntt_form())
-                throw std::invalid_argument("CKKS encrypted must be in NTT form");
-            if (scheme_ == seal::scheme_type::bgv && !encrypted.is_ntt_form())
-                throw std::invalid_argument("BGV encrypted must be in NTT form");
+            check_pool(pool);
+            check_ntt_form(ntt);
+        }
+        // apply_galois_inplace (evaluator.cpp:2384-2430), up to the key lookup
+        template <class GaloisKeys>
+        void check_apply_galois(const Meta &encrypted, std::uint32_t galois_elt, const GaloisKeys &galois_keys,
+                                const seal::MemoryPoolHandle *pool = nullptr) const
+        {
+            if (galois_keys.parms_id() != context_.key_parms_id())
+                throw std::invalid_argument("galois_keys is not valid for encryption parameters");
+            if (!galois_keys.has_key(galois_elt))
+                throw std::invalid_argument("Galois key not present");
+            if (!(galois_elt & 1) || galois_elt >= 2 * context_.get_context_data(encrypted.parms_id)->parms().poly_modulus_degree())
+                throw std::invalid_argument("Galois element is not valid");
+            if (encrypted.size != 2)
+                throw std::invalid_argument("encrypted size must be 2");
+            check_switch_key(encrypted.ntt, pool);
+        }
+        // the first checks of rotate_internal / conjugate_internal (evaluator.cpp:2507-2515, evaluator.h:1358-1369): the operand's
+        // level, which must support batching
+        template <class Encrypted>
+        std::shared_ptr<const seal::SEALContext::ContextData> batching_level(const Encrypted &encrypted) const
+        {
+            if constexpr (std::is_same_v<Encrypted, CiphertextBatch>)
+                owned(encrypted);
+            auto cd = context_.get_context_data(meta(encrypted).parms_id);
+            if (!cd)
+                throw std::invalid_argument("encrypted is not valid for encryption parameters");
+            if (!cd->qualifiers().using_batching)
+                throw std::logic_error("encryption parameters do not support batching");
+            return cd;
+        }
+        // the entry of mod_switch_to_next / rescale_to_next (evaluator.cpp:1404-1440, :1503-1532) and mod_reduce_to_next (:1597-1623)
+        void check_mod_switch_to_next(const Meta &encrypted, bool rescale, const seal::MemoryPoolHandle *pool = nullptr) const
+        {
+            if (context_.last_parms_id() == encrypted.parms_id)
+                throw std::invalid_argument("end of modulus switching chain reached");
+            check_pool(pool);
+            if (rescale && scheme_ != seal::scheme_type::ckks)
+                throw std::invalid_argument("unsupported operation for scheme type");
+        }
+        // one level down: mod_switch_drop_to_next (evaluator.cpp:1296-1322) when drop, else mod_switch_scale_to_next (:1201-1294),
+        // which rescales CKKS and updates BGV's correction factor
+        Meta mod_switch_to_next_meta(const Meta &encrypted, bool drop) const
+        {
+            auto cd = context_.get_context_data(encrypted.parms_id);
+            auto &next = *cd->next_context_data();
+            check_ntt_form(encrypted.ntt);
+            Meta r = encrypted;
+            r.parms_id = next.parms_id();
+            if (drop)
+            {
+                if (!scale_within_bounds(encrypted.scale, next))
+                    throw std::invalid_argument("scale out of bounds");
+                return r;
+            }
+            if (scheme_ == seal::scheme_type::ckks)
+            {
+                if (!scale_within_bounds(encrypted.scale, *cd))
+                    throw std::invalid_argument("scale out of bounds");
+                r.scale = encrypted.scale / static_cast<double>(cd->parms().coeff_modulus().back().value());
+                if (!scale_within_bounds(r.scale, next))
+                    throw std::invalid_argument("scale out of bounds");
+            }
+            if (scheme_ == seal::scheme_type::bgv)
+                r.cf = seal::util::multiply_uint_mod(encrypted.cf, cd->rns_tool()->inv_q_last_mod_t(), next.parms().plain_modulus());
+            return r;
+        }
+        // mod_switch_drop_to_next(Plaintext &) (evaluator.cpp:1369-1392): the level below an NTT-form plaintext's
+        const seal::SEALContext::ContextData &plain_next_level(const Meta &plain) const
+        {
+            if (!plain.ntt)
+                throw std::invalid_argument("plain is not in NTT form");
+            auto cd = context_.get_context_data(plain.parms_id);
+            if (!cd->next_context_data())
+                throw std::invalid_argument("end of modulus switching chain reached");
+            auto &next = *cd->next_context_data();
+            if (!scale_within_bounds(plain.scale, next))
+                throw std::invalid_argument("scale out of bounds");
+            return next;
+        }
+        // mod_switch_to_inplace(Plaintext &, parms_id) (evaluator.cpp:1475-1501) after the plaintext's own check
+        void check_plain_target_level(const Meta &plain, const seal::parms_id_type &parms_id) const
+        {
+            auto target = context_.get_context_data(parms_id);
+            if (!target)
+                throw std::invalid_argument("parms_id is not valid for encryption parameters");
+            if (!plain.ntt)
+                throw std::invalid_argument("plain is not in NTT form");
+            if (context_.get_context_data(plain.parms_id)->chain_index() < target->chain_index())
+                throw std::invalid_argument("cannot switch to higher level modulus");
+        }
+        // the arguments of one sb200_add_many call folding operands 0, 1, ... in order (the caller supplies their device words), each
+        // step one add_inplace / sub_inplace of the reference's chain, with its checks and its correction factors (fold_in)
+        struct Fold
+        {
+            Meta result;                        // the chain's result so far
+            std::vector<std::size_t> sizes;     // every operand's
+            std::vector<int> modes;             // [count - 1]
+            std::vector<std::uint64_t> factors; // [count - 1][2], empty when no step is scaled
+        };
+        // add_inplace / sub_inplace (evaluator.cpp:155-350) of b into the fold; BGV operands with different correction factors are
+        // both scaled by the balancing factors first (:188-209, :305-326)
+        void fold_in(Fold &f, const Meta &b, int mode) const
+        {
+            const Meta &a = f.result;
+            if (a.parms_id != b.parms_id || a.batch != b.batch)
+                throw std::invalid_argument("encrypted1 and encrypted2 parameter mismatch");
+            if (a.ntt != b.ntt)
+                throw std::invalid_argument("NTT form mismatch");
+            if (!seal::util::are_close<double>(a.scale, b.scale))
+                throw std::invalid_argument("scale mismatch");
+            std::uint64_t e1 = 0, e2 = 0;
+            const bool scaled = a.cf != b.cf;
+            if (scaled)
+            {
+                balance_factors(a.cf, b.cf, context_.get_context_data(a.parms_id)->parms().plain_modulus(), f.result.cf, e1, e2);
+                mode |= SB200_FOLD_SCALED;
+                f.factors.resize(2 * f.modes.size(), 0); // the earlier steps' (unscaled) entries
+            }
+            if (scaled || !f.factors.empty())
+                f.factors.push_back(e1), f.factors.push_back(e2);
+            f.modes.push_back(mode);
+            f.sizes.push_back(b.size);
+            f.result.size = std::max(f.result.size, b.size);
+        }
+        Fold plan_fold(const std::vector<Meta> &ops, int mode) const
+        {
+            Fold f{ ops[0], { ops[0].size }, {}, {} };
+            for (std::size_t j = 1; j < ops.size(); j++)
+                fold_in(f, ops[j], mode);
+            return f;
         }
         // uploads KSwitchKeys::data()[index] (evaluator.cpp:2586-2648) and caches the device copy under a fingerprint of the
         // key's CONTENT (leading / trailing / strided words of every digit + its shape): a regenerated or reloaded key object
@@ -2225,16 +2292,11 @@ namespace seal_b200
         {
             owned(encrypted), owned(plain);
             plain_count(encrypted, plain);
+            check_add_plain(meta(encrypted), meta(plain));
             const std::size_t L = encrypted.L_, size = encrypted.size_, B = encrypted.batch_;
             if (scheme_ != seal::scheme_type::ckks)
             {
                 const bool bfv = scheme_ == seal::scheme_type::bfv;
-                if (bfv && encrypted.ntt_)
-                    throw std::invalid_argument("BFV encrypted cannot be in NTT form");
-                if (!bfv && !encrypted.ntt_)
-                    throw std::invalid_argument("BGV encrypted must be in NTT form");
-                if (plain.ntt_)
-                    throw std::invalid_argument(bfv ? "BFV plain cannot be in NTT form" : "BGV plain cannot be in NTT form");
                 // the batch's one correction factor, once per plaintext (BGV, :1840-1843)
                 const std::vector<std::uint64_t> cf(plain.batch_, encrypted.cf_);
                 std::lock_guard<std::mutex> lock(mu_);
@@ -2242,14 +2304,6 @@ namespace seal_b200
                                               encrypted.d_, nullptr));
                 return;
             }
-            if (!encrypted.ntt_)
-                throw std::invalid_argument("CKKS encrypted must be in NTT form");
-            if (!plain.ntt_)
-                throw std::invalid_argument("CKKS plain must be in NTT form");
-            if (encrypted.parms_id_ != plain.parms_id_)
-                throw std::invalid_argument("encrypted and plain parameter mismatch");
-            if (!seal::util::are_close<double>(encrypted.scale_, plain.scale_))
-                throw std::invalid_argument("scale mismatch");
             std::lock_guard<std::mutex> lock(mu_);
             check(sb200_add_plain_ntt(ctx_, L, size, B, plain.batch_, subtract ? 1 : 0, encrypted.d_, plain.d_, encrypted.d_, nullptr));
         }
@@ -2279,10 +2333,6 @@ namespace seal_b200
             reserve(b, batch * size * L * n);
             b.batch_ = batch, b.size_ = size, b.L_ = L, b.n_ = n;
         }
-        static void copy_meta(const CiphertextBatch &s, CiphertextBatch &d)
-        {
-            d.parms_id_ = s.parms_id_, d.ntt_ = s.ntt_, d.scale_ = s.scale_, d.cf_ = s.cf_;
-        }
         // result slab of a layout-changing operation; adopt() swaps it with the operand's storage, so a chain of operations
         // allocates nothing once the largest shape has been seen.  Caller holds mu_.
         // (never smaller than the slab it will be swapped with: every buffer in circulation then fits every level of a chain,
@@ -2297,98 +2347,16 @@ namespace seal_b200
             std::swap(b.d_, tmp_.d_);
             std::swap(b.cap_, tmp_.cap_);
         }
-        void check_keyswitch_form(bool ntt) const
-        {
-            if (!context_.using_keyswitching())
-                throw std::logic_error("keyswitching is not supported by the context");
-            if (scheme_ == seal::scheme_type::bfv && ntt)
-                throw std::invalid_argument("BFV encrypted cannot be in NTT form");
-            if (scheme_ == seal::scheme_type::ckks && !ntt)
-                throw std::invalid_argument("CKKS encrypted must be in NTT form");
-            if (scheme_ == seal::scheme_type::bgv && !ntt)
-                throw std::invalid_argument("BGV encrypted must be in NTT form");
-        }
         void mod_switch_batch(CiphertextBatch &e, bool rescale) const
         {
-            auto cd = context_.get_context_data(e.parms_id_);
-            auto next = cd->next_context_data();
-            const bool ckks = scheme_ == seal::scheme_type::ckks, bgv = scheme_ == seal::scheme_type::bgv;
-            if (ckks && !e.ntt_)
-                throw std::invalid_argument("CKKS encrypted must be in NTT form");
-            if (bgv && !e.ntt_)
-                throw std::invalid_argument("BGV encrypted must be in NTT form");
-            if (!ckks && !bgv && e.ntt_)
-                throw std::invalid_argument("BFV encrypted cannot be in NTT form");
-            double scale = e.scale_;
-            if (rescale)
-            {
-                if (!scale_within_bounds(e.scale_, *cd))
-                    throw std::invalid_argument("scale out of bounds");
-                scale = e.scale_ / static_cast<double>(cd->parms().coeff_modulus().back().value());
-            }
-            if ((rescale || ckks) && !scale_within_bounds(scale, *next))
-                throw std::invalid_argument("scale out of bounds"); // :1236-1241, mod_switch_drop_to_next :1318-1322
+            const Meta r = mod_switch_to_next_meta(meta(e), scheme_ == seal::scheme_type::ckks && !rescale);
             std::lock_guard<std::mutex> lock(mu_);
             std::uint64_t *out = out_slab(e.batch_ * e.size_ * (e.L_ - 1) * e.n_, e);
             check(rescale ? sb200_rescale_to_next_sized(ctx_, e.L_, e.size_, e.batch_, e.d_, out, nullptr)
                           : sb200_mod_switch_to_next_sized(ctx_, e.L_, e.size_, e.batch_, e.d_, out, nullptr));
             adopt(e);
             e.L_ -= 1;
-            e.parms_id_ = next->parms_id();
-            e.scale_ = scale;
-            if (bgv)
-                e.cf_ = seal::util::multiply_uint_mod(e.cf_, cd->rns_tool()->inv_q_last_mod_t(), next->parms().plain_modulus());
-        }
-        // the arguments of one sb200_add_many call folding ops[0] op ops[1] op ... with modes[j - 1], after the checks of every step
-        // of the reference's chain (add_inplace / sub_inplace, evaluator.cpp:155-350) and with its correction factors replayed
-        struct Fold
-        {
-            std::vector<std::size_t> sizes;
-            std::vector<const std::uint64_t *> ptrs;
-            std::vector<int> modes;
-            std::vector<std::uint64_t> factors; // [count - 1][2], empty when no step is scaled
-            std::size_t out_size = 0;
-            std::uint64_t cf = 1; // the result's correction factor
-        };
-        Fold plan_fold(const std::vector<const CiphertextBatch *> &ops, std::vector<int> modes) const
-        {
-            const CiphertextBatch &a = *ops[0];
-            Fold f;
-            f.cf = a.cf_;
-            f.out_size = a.size_;
-            std::vector<std::uint64_t> factors(2 * (ops.size() - 1), 0);
-            bool scaled = false;
-            for (std::size_t j = 0; j < ops.size(); j++)
-            {
-                const CiphertextBatch &b = *ops[j];
-                owned(a), owned(b);
-                if (j)
-                {
-                    if (a.parms_id_ != b.parms_id_ || a.batch_ != b.batch_)
-                        throw std::invalid_argument("encrypted1 and encrypted2 parameter mismatch");
-                    if (a.ntt_ != b.ntt_)
-                        throw std::invalid_argument("NTT form mismatch");
-                    if (!seal::util::are_close<double>(a.scale_, b.scale_))
-                        throw std::invalid_argument("scale mismatch");
-                    if (f.cf != b.cf_)
-                    {
-                        // BGV: both sides scaled by the balancing factors (:188-209, :305-326)
-                        std::uint64_t g, e1, e2;
-                        balance_factors(f.cf, b.cf_, context_.get_context_data(a.parms_id_)->parms().plain_modulus(), g, e1, e2);
-                        modes[j - 1] |= SB200_FOLD_SCALED;
-                        factors[2 * (j - 1)] = e1, factors[2 * (j - 1) + 1] = e2;
-                        f.cf = g;
-                        scaled = true;
-                    }
-                    f.out_size = std::max(f.out_size, b.size_);
-                }
-                f.sizes.push_back(b.size_);
-                f.ptrs.push_back(b.d_);
-            }
-            f.modes = std::move(modes);
-            if (scaled)
-                f.factors = std::move(factors);
-            return f;
+            assign(e, r);
         }
         // ---- multiply_plain_sum: the chain's checks replayed on the products' metadata, before anything is written ----
         struct PlainSum
@@ -2400,65 +2368,30 @@ namespace seal_b200
         {
             const std::size_t K = encrypteds.size();
             PlainSum p;
-            // the products t_i: the ciphertexts' metadata with multiply_plain's scale; their slabs are borrowed for plan_fold's
-            // checks only and handed back before these shells go out of scope
-            std::vector<CiphertextBatch> prods(K);
-            auto give_back = [&prods] {
-                for (auto &t : prods)
-                    t.d_ = nullptr;
-            };
-            try
+            for (std::size_t j = 0; j < M; j++)
             {
-                for (std::size_t j = 0; j < M; j++)
+                std::vector<Meta> prods; // the products t_i
+                for (std::size_t i = 0; i < K; i++)
                 {
-                    for (std::size_t i = 0; i < K; i++)
-                    {
-                        const CiphertextBatch &e = encrypteds[i];
-                        const PlaintextBatch &pl = plains[j * K + i];
-                        // multiply_plain_inplace (evaluator.cpp:1975-2019), as the batch member above checks it
-                        owned(e), owned(pl);
-                        plain_count(e, pl);
-                        CiphertextBatch &t = prods[i];
-                        t.ctx_ = e.ctx_, t.d_ = e.d_, t.batch_ = e.batch_, t.size_ = e.size_, t.L_ = e.L_, t.n_ = e.n_;
-                        copy_meta(e, t);
-                        if (!pl.ntt_)
-                        {
-                            if (scheme_ == seal::scheme_type::ckks)
-                                throw std::invalid_argument("plain is not valid for encryption parameters");
-                            continue;
-                        }
-                        if (e.parms_id_ != pl.parms_id_)
-                            throw std::invalid_argument("encrypted_ntt and plain_ntt parameter mismatch"); // :2164-2167
-                        t.scale_ = e.scale_ * pl.scale_;
-                        if (!scale_within_bounds(t.scale_, *context_.get_context_data(e.parms_id_)))
-                            throw std::invalid_argument("scale out of bounds"); // :2189-2193
-                    }
-                    std::vector<const CiphertextBatch *> ops;
-                    for (auto &t : prods)
-                        ops.push_back(&t);
-                    p.fold = plan_fold(ops, std::vector<int>(K - 1, SB200_FOLD_ADD)); // add_many (evaluator.cpp:236-262)
-                    p.scales.push_back(prods[0].scale_);
+                    // multiply_plain_inplace (evaluator.cpp:1975-2019), as the batch member above checks it
+                    owned(encrypteds[i]), owned(plains[j * K + i]);
+                    plain_count(encrypteds[i], plains[j * K + i]);
+                    prods.push_back(multiply_plain_meta(meta(encrypteds[i]), meta(plains[j * K + i])));
                 }
+                p.fold = plan_fold(prods, SB200_FOLD_ADD); // add_many (evaluator.cpp:236-262)
+                p.scales.push_back(prods[0].scale);
             }
-            catch (...)
-            {
-                give_back();
-                throw;
-            }
-            give_back();
             for (auto &pl : plains)
                 if (pl.ntt_ != plains[0].ntt_)
                     throw std::invalid_argument("plains must all be in NTT form or all in coefficient form");
-            for (std::size_t i = 0; i < K; i++)
-                p.fold.ptrs[i] = encrypteds[i].d_;
             return p;
         }
         // destination j shaped and given the chain's metadata; caller holds mu_
         std::uint64_t *plain_sum_output(const CiphertextBatch &e0, const PlainSum &p, std::size_t j, CiphertextBatch &d) const
         {
-            shape(d, e0.batch_, p.fold.out_size, e0.L_, e0.n_);
-            copy_meta(e0, d);
-            d.scale_ = p.scales[j], d.cf_ = p.fold.cf;
+            shape(d, e0.batch_, p.fold.result.size, e0.L_, e0.n_);
+            assign(d, p.fold.result);
+            d.scale_ = p.scales[j];
             return d.d_;
         }
         void run_plain_sum(const std::vector<CiphertextBatch> &encrypteds, const std::vector<PlaintextBatch> &plains, const PlainSum &p,
@@ -2466,19 +2399,20 @@ namespace seal_b200
         {
             const CiphertextBatch &e0 = encrypteds[0];
             std::vector<std::size_t> counts;
-            std::vector<const std::uint64_t *> ptrs;
+            std::vector<const std::uint64_t *> cts, ptrs;
+            for (auto &e : encrypteds)
+                cts.push_back(e.d_);
             for (auto &pl : plains)
                 counts.push_back(pl.batch_), ptrs.push_back(pl.d_);
-            check(sb200_multiply_plain_sum(ctx_, e0.L_, e0.batch_, encrypteds.size(), p.scales.size(), p.fold.sizes.data(), p.fold.ptrs.data(),
+            check(sb200_multiply_plain_sum(ctx_, e0.L_, e0.batch_, encrypteds.size(), p.scales.size(), p.fold.sizes.data(), cts.data(),
                                            counts.data(), ptrs.data(), e0.ntt_ ? 1 : 0, plains[0].ntt_ ? 1 : 0, p.fold.modes.data(),
                                            p.fold.factors.empty() ? nullptr : p.fold.factors.data(), outs, nullptr));
         }
         // ---- multiply_sum: the chain's checks replayed on the products' metadata, before anything is written ----
         struct MultiplySum
         {
-            std::vector<Fold> folds;    // [M] the add_many of every output (BGV's factors depend on both operands)
-            std::vector<double> scales; // [M] the result's scale: the first product's
-            bool fused = true;          // every operand has size 2: sb200_multiply_sum
+            std::vector<Fold> folds; // [M] the add_many of every output (BGV's factors depend on both operands)
+            bool fused = true;       // every operand has size 2: sb200_multiply_sum
         };
         void check_sum_destination(const std::vector<CiphertextBatch> &e1, const std::vector<CiphertextBatch> &e2, const CiphertextBatch &d) const
         {
@@ -2503,60 +2437,20 @@ namespace seal_b200
         MultiplySum plan_multiply_sum(const std::vector<CiphertextBatch> &e1, const std::vector<CiphertextBatch> &e2, std::size_t M) const
         {
             const std::size_t K = e2.size();
-            const bool ckks = scheme_ == seal::scheme_type::ckks, bgv = scheme_ == seal::scheme_type::bgv;
             MultiplySum p;
-            // the products t_i: metadata as multiply_inplace leaves it; their slabs are borrowed (the left operand's) for
-            // plan_fold's checks only and handed back before these shells go out of scope
-            std::vector<CiphertextBatch> prods(K);
-            auto give_back = [&prods] {
-                for (auto &t : prods)
-                    t.d_ = nullptr;
-            };
-            try
+            for (std::size_t j = 0; j < M; j++)
             {
-                for (std::size_t j = 0; j < M; j++)
+                std::vector<Meta> prods; // the products t_i
+                for (std::size_t i = 0; i < K; i++)
                 {
-                    for (std::size_t i = 0; i < K; i++)
-                    {
-                        const CiphertextBatch &a = e1[j * K + i], &b = e2[i];
-                        // multiply_inplace (evaluator.cpp:352-393), as the batch member above checks it
-                        owned(a), owned(b);
-                        if (a.parms_id_ != b.parms_id_ || a.batch_ != b.batch_)
-                            throw std::invalid_argument("encrypted1 and encrypted2 parameter mismatch");
-                        if ((ckks || bgv) && !(a.ntt_ && b.ntt_))
-                            throw std::invalid_argument("encrypted1 or encrypted2 must be in NTT form");
-                        if (!(ckks || bgv) && (a.ntt_ || b.ntt_))
-                            throw std::invalid_argument("encrypted1 or encrypted2 cannot be in NTT form");
-                        auto cd = context_.get_context_data(a.parms_id_);
-                        const std::size_t so = a.size_ + b.size_ - 1;
-                        if (so > SEAL_CIPHERTEXT_SIZE_MAX)
-                            throw std::invalid_argument("invalid size");
-                        CiphertextBatch &t = prods[i];
-                        t.ctx_ = a.ctx_, t.d_ = a.d_, t.batch_ = a.batch_, t.size_ = so, t.L_ = a.L_, t.n_ = a.n_;
-                        copy_meta(a, t);
-                        if (ckks)
-                        {
-                            t.scale_ = a.scale_ * b.scale_;
-                            if (!scale_within_bounds(t.scale_, *cd))
-                                throw std::invalid_argument("scale out of bounds");
-                        }
-                        if (bgv)
-                            t.cf_ = seal::util::multiply_uint_mod(a.cf_, b.cf_, cd->parms().plain_modulus());
-                        p.fused = p.fused && a.size_ == 2 && b.size_ == 2;
-                    }
-                    std::vector<const CiphertextBatch *> ops;
-                    for (auto &t : prods)
-                        ops.push_back(&t);
-                    p.folds.push_back(plan_fold(ops, std::vector<int>(K - 1, SB200_FOLD_ADD))); // add_many (evaluator.cpp:236-262)
-                    p.scales.push_back(prods[0].scale_);
+                    const CiphertextBatch &a = e1[j * K + i], &b = e2[i];
+                    // multiply_inplace (evaluator.cpp:352-393), as the batch member above checks it
+                    owned(a), owned(b);
+                    prods.push_back(multiply_meta(meta(a), meta(b)));
+                    p.fused = p.fused && a.size_ == 2 && b.size_ == 2;
                 }
+                p.folds.push_back(plan_fold(prods, SB200_FOLD_ADD)); // add_many (evaluator.cpp:236-262)
             }
-            catch (...)
-            {
-                give_back();
-                throw;
-            }
-            give_back();
             return p;
         }
         void run_multiply_sum(const std::vector<CiphertextBatch> &e1, const std::vector<CiphertextBatch> &e2, const MultiplySum &p,
@@ -2583,8 +2477,7 @@ namespace seal_b200
             {
                 CiphertextBatch &d = *dest[j];
                 shape(d, b0.batch_, 3, b0.L_, b0.n_);
-                copy_meta(e1[j * K], d);
-                d.scale_ = p.scales[j], d.cf_ = p.folds[j].cf;
+                assign(d, p.folds[j].result);
             }
             std::vector<const std::uint64_t *> lhs, rhs;
             std::vector<std::uint64_t *> outs;
@@ -2605,19 +2498,6 @@ namespace seal_b200
                                          f.factors.empty() ? nullptr : f.factors.data(), outs.data() + j0, nullptr));
             }
         }
-        // relinearize_inplace's checks (relinearize_batch) for a result of `size` polynomials
-        template <class RelinKeys>
-        void check_relinearize(const RelinKeys &relin_keys, std::size_t size, bool ntt) const
-        {
-            if (relin_keys.parms_id() != context_.key_parms_id())
-                throw std::invalid_argument("relin_keys is not valid for encryption parameters");
-            if (size < 2)
-                throw std::invalid_argument("destination_size must be at least 2 and less than or equal to current count");
-            if (relin_keys.size() < size - 2)
-                throw std::invalid_argument("not enough relinearization keys");
-            if (size > 2)
-                check_keyswitch_form(ntt);
-        }
         template <class RelinKeys>
         void multiply_relinearize_sum_one(const std::vector<CiphertextBatch> &e1, const std::vector<CiphertextBatch> &e2, const RelinKeys &relin_keys,
                                           CiphertextBatch &destination) const
@@ -2626,7 +2506,9 @@ namespace seal_b200
             if (e1.size() != e2.size())
                 throw std::invalid_argument("encrypteds1 must hold K ciphertext batches per destination");
             const MultiplySum p = plan_multiply_sum(e1, e2, 1);
-            check_relinearize(relin_keys, p.folds[0].out_size, e1[0].ntt_);
+            check_relinearize(relin_keys, p.folds[0].result.size);
+            if (p.folds[0].result.size > 2)
+                check_switch_key(p.folds[0].result.ntt);
             CiphertextBatch *d = &destination;
             run_multiply_sum(e1, e2, p, &d);
             relinearize_inplace(destination, relin_keys);
@@ -2637,8 +2519,12 @@ namespace seal_b200
         {
             const std::size_t M = sum_outputs(e1, e2, destinations);
             const MultiplySum p = plan_multiply_sum(e1, e2, M);
-            for (std::size_t j = 0; j < M; j++)
-                check_relinearize(relin_keys, p.folds[j].out_size, e1[j * e2.size()].ntt_);
+            for (const Fold &f : p.folds) // relinearize_inplace's checks of every sum
+            {
+                check_relinearize(relin_keys, f.result.size);
+                if (f.result.size > 2)
+                    check_switch_key(f.result.ntt);
+            }
             destinations.resize(M);
             std::vector<CiphertextBatch *> d;
             for (auto &x : destinations)
@@ -2649,17 +2535,18 @@ namespace seal_b200
         }
         void linear_batch(CiphertextBatch &a, const CiphertextBatch &b, bool subtract) const
         {
-            const Fold f = plan_fold({ &a, &b }, { subtract ? SB200_FOLD_SUB : SB200_FOLD_ADD });
+            owned(a), owned(b);
+            const Fold f = plan_fold({ meta(a), meta(b) }, subtract ? SB200_FOLD_SUB : SB200_FOLD_ADD);
+            const std::uint64_t *ptrs[2] = { a.d_, b.d_ };
             std::lock_guard<std::mutex> lock(mu_);
             // in place when the result keeps a's size and b is another slab; otherwise into the result slab
-            const bool in_place = a.size_ == f.out_size && a.d_ != b.d_;
-            std::uint64_t *out = in_place ? a.d_ : out_slab(a.batch_ * f.out_size * a.L_ * a.n_, a);
-            check(sb200_add_many(ctx_, a.L_, a.batch_, 2, f.sizes.data(), f.ptrs.data(), f.modes.data(),
-                                 f.factors.empty() ? nullptr : f.factors.data(), out, nullptr));
+            const bool in_place = a.size_ == f.result.size && a.d_ != b.d_;
+            std::uint64_t *out = in_place ? a.d_ : out_slab(a.batch_ * f.result.size * a.L_ * a.n_, a);
+            check(sb200_add_many(ctx_, a.L_, a.batch_, 2, f.sizes.data(), ptrs, f.modes.data(), f.factors.empty() ? nullptr : f.factors.data(),
+                                 out, nullptr));
             if (!in_place)
                 adopt(a);
-            a.size_ = f.out_size;
-            a.cf_ = f.cf;
+            assign(a, f.result);
         }
         // ---- the product schedule of multiply_many / exponentiate ----
         // The reference's queue (evaluator.cpp:1649-1724): products of operand pairs (0,1), (2,3), ... with an odd operand appended
@@ -2736,47 +2623,28 @@ namespace seal_b200
                           CiphertextBatch &destination) const
         {
             const CiphertextBatch &f = *leaves[0];
-            const bool bgv = scheme_ == seal::scheme_type::bgv;
-            // every check of every product's multiply_inplace and relinearize_inplace runs before the first write
             for (auto *l : leaves)
-            {
                 owned(*l);
-                if (l->parms_id_ != f.parms_id_ || l->batch_ != f.batch_)
-                    throw std::invalid_argument("encrypted1 and encrypted2 parameter mismatch");
-                if (bgv != l->ntt_)
-                    throw std::invalid_argument(bgv ? "encrypted1 or encrypted2 must be in NTT form" : "encrypted1 or encrypted2 cannot be in NTT form");
-            }
-            if (!s.products.empty())
-            {
-                if (relin_keys.parms_id() != context_.key_parms_id())
-                    throw std::invalid_argument("relin_keys is not valid for encryption parameters");
-                if (!context_.using_keyswitching())
-                    throw std::logic_error("keyswitching is not supported by the context");
-                for (auto &pr : s.products)
-                {
-                    const std::size_t s1 = pr.first < s.leaves ? leaves[pr.first]->size_ : 2, s2 = pr.second < s.leaves ? leaves[pr.second]->size_ : 2;
-                    if (s1 + s2 - 1 > SEAL_CIPHERTEXT_SIZE_MAX)
-                        throw std::invalid_argument("invalid size");
-                    if (s1 + s2 - 1 < 2)
-                        throw std::invalid_argument("destination_size must be at least 2 and less than or equal to current count");
-                    if (relin_keys.size() < s1 + s2 - 3)
-                        throw std::invalid_argument("not enough relinearization keys");
-                }
-            }
             if (s.products.empty())
             {
                 copy(*leaves[s.root], destination);
                 return;
             }
-            const auto cd = context_.get_context_data(f.parms_id_);
-            const seal::Modulus &t = cd->parms().plain_modulus();
-            const std::size_t B = f.batch_, L = f.L_, ct = 2 * L * f.n_, bytes = B * ct * sizeof(std::uint64_t);
+            // every check of every product's multiply_inplace and relinearize_inplace, in the chain's order, before the first write
             const std::size_t P = s.products.size();
+            std::vector<Meta> prods(P); // each product's metadata, relinearized
+            auto id_meta = [&](std::size_t id) { return id < s.leaves ? meta(*leaves[id]) : prods[id - s.leaves]; };
+            for (std::size_t p = 0; p < P; p++)
+            {
+                prods[p] = multiply_meta(id_meta(s.products[p].first), id_meta(s.products[p].second));
+                check_relinearize(relin_keys, prods[p].size);
+                check_switch_key(prods[p].ntt);
+                prods[p].size = 2;
+            }
+            const std::size_t B = f.batch_, L = f.L_, ct = 2 * L * f.n_, bytes = B * ct * sizeof(std::uint64_t);
             std::vector<const std::uint64_t *> data(P);     // device words of each product, [B][2][L][n]
-            std::vector<std::uint64_t> cf(P);
             std::vector<CiphertextBatch> slabs;              // owners of the wave outputs
             auto id_data = [&](std::size_t id) { return id < s.leaves ? leaves[id]->d_ : data[id - s.leaves]; };
-            auto id_cf = [&](std::size_t id) { return id < s.leaves ? leaves[id]->cf_ : cf[id - s.leaves]; };
             auto id_size = [&](std::size_t id) { return id < s.leaves ? leaves[id]->size_ : std::size_t(2); };
             for (const auto &wave : s.waves)
             {
@@ -2792,9 +2660,7 @@ namespace seal_b200
                     wrap(y, r, id_data(s.products[p].second), f);
                     multiply_inplace(x, y);
                     relinearize_inplace(x, relin_keys);
-                    x.cf_ = bgv ? seal::util::multiply_uint_mod(id_cf(s.products[p].first), id_cf(s.products[p].second), t) : 1;
                     data[p] = x.d_;
-                    cf[p] = x.cf_;
                     slabs.push_back(std::move(x));
                 }
                 std::lock_guard<std::mutex> lock(mu_);
@@ -2815,11 +2681,7 @@ namespace seal_b200
                     sb200_kswitch_key *key = key_for(relin_keys, seal::RelinKeys::get_index(2), L);
                     check(sb200_multiply_relinearize(ctx_, L, G * B, a.d_, b.d_, key, a.d_, nullptr));
                     for (std::size_t i = 0; i < G; i++)
-                    {
-                        const std::size_t p = fused[g0 + i];
-                        data[p] = a.d_ + i * B * ct;
-                        cf[p] = bgv ? seal::util::multiply_uint_mod(id_cf(s.products[p].first), id_cf(s.products[p].second), t) : 1;
-                    }
+                        data[fused[g0 + i]] = a.d_ + i * B * ct;
                     slabs.push_back(std::move(a));
                 }
             }
@@ -2827,13 +2689,12 @@ namespace seal_b200
             {
                 std::lock_guard<std::mutex> lock(mu_);
                 shape(destination, B, 2, L, f.n_);
-                copy_meta(f, destination);
-                destination.cf_ = bgv ? cf[r] : f.cf_;
+                assign(destination, prods[r]);
                 check(sb200_memcpy_d2d(ctx_, destination.d_, data[r], bytes, nullptr));
             }
         }
         // a batch object over a leaf (a copy) or over product words (size 2), with the leaves' metadata, for the one-by-one products
-        void wrap(CiphertextBatch &x, const CiphertextBatch *leaf, const std::uint64_t *words, const CiphertextBatch &meta) const
+        void wrap(CiphertextBatch &x, const CiphertextBatch *leaf, const std::uint64_t *words, const CiphertextBatch &like) const
         {
             if (leaf)
             {
@@ -2841,88 +2702,29 @@ namespace seal_b200
                 return;
             }
             std::lock_guard<std::mutex> lock(mu_);
-            shape(x, meta.batch_, 2, meta.L_, meta.n_);
-            copy_meta(meta, x);
-            check(sb200_memcpy_d2d(ctx_, x.d_, words, meta.batch_ * 2 * meta.L_ * meta.n_ * sizeof(std::uint64_t), nullptr));
-        }
-        template <class GaloisKeys>
-        void rotate_batch(CiphertextBatch &encrypted, int steps, const GaloisKeys &galois_keys) const
-        {
-            owned(encrypted);
-            auto cd = context_.get_context_data(encrypted.parms_id_);
-            if (!cd->qualifiers().using_batching)
-                throw std::logic_error("encryption parameters do not support batching");
-            if (galois_keys.parms_id() != context_.key_parms_id())
-                throw std::invalid_argument("galois_keys is not valid for encryption parameters");
-            if (steps == 0)
-                return;
-            const std::size_t n = cd->parms().poly_modulus_degree();
-            const std::uint32_t elt = cd->galois_tool()->get_elt_from_step(steps);
-            if (galois_keys.has_key(elt))
-            {
-                apply_galois_inplace(encrypted, elt, galois_keys);
-                return;
-            }
-            std::vector<int> naf_steps = seal::util::naf(steps);
-            if (naf_steps.size() == 1)
-                throw std::invalid_argument("Galois key not present");
-            for (int st : naf_steps)
-                if (static_cast<std::size_t>(std::abs(st)) != (n >> 1))
-                    rotate_batch(encrypted, st, galois_keys);
-        }
-        template <class GaloisKeys>
-        void conjugate_batch(CiphertextBatch &encrypted, const GaloisKeys &galois_keys) const
-        {
-            owned(encrypted);
-            auto cd = context_.get_context_data(encrypted.parms_id_);
-            if (!cd->qualifiers().using_batching)
-                throw std::logic_error("encryption parameters do not support batching");
-            apply_galois_inplace(encrypted, cd->galois_tool()->get_elt_from_step(0), galois_keys);
+            assign(x, meta(like));
+            shape(x, like.batch_, 2, like.L_, like.n_);
+            check(sb200_memcpy_d2d(ctx_, x.d_, words, like.batch_ * 2 * like.L_ * like.n_ * sizeof(std::uint64_t), nullptr));
         }
         void mod_switch_impl(const seal::Ciphertext &encrypted, seal::Ciphertext &destination, bool rescale) const
         {
-            auto cd = context_.get_context_data(encrypted.parms_id());
-            auto next = cd->next_context_data();
-            const bool ckks = scheme_ == seal::scheme_type::ckks, bgv = scheme_ == seal::scheme_type::bgv;
-            if (ckks && !encrypted.is_ntt_form())
-                throw std::invalid_argument("CKKS encrypted must be in NTT form");
-            if (bgv && !encrypted.is_ntt_form())
-                throw std::invalid_argument("BGV encrypted must be in NTT form"); // :1214-1217
-            if (!ckks && !bgv && encrypted.is_ntt_form())
-                throw std::invalid_argument("BFV encrypted cannot be in NTT form");
-            double scale = encrypted.scale();
-            if (rescale)
-            {
-                if (!scale_within_bounds(encrypted.scale(), *cd))
-                    throw std::invalid_argument("scale out of bounds");
-                scale = encrypted.scale() / static_cast<double>(cd->parms().coeff_modulus().back().value());
-                if (!scale_within_bounds(scale, *next))
-                    throw std::invalid_argument("scale out of bounds");
-            }
-            else if (ckks && !scale_within_bounds(scale, *next))
-                throw std::invalid_argument("scale out of bounds"); // mod_switch_drop_to_next, evaluator.cpp:1318-1322
+            const Meta r = mod_switch_to_next_meta(meta(encrypted), scheme_ == seal::scheme_type::ckks && !rescale);
             const std::size_t L = encrypted.coeff_modulus_size(), n = encrypted.poly_modulus_degree(), size = encrypted.size();
             std::vector<std::uint64_t> in(encrypted.data(), encrypted.data() + size * L * n);
-            const bool ntt = encrypted.is_ntt_form();
-            const std::uint64_t correction = encrypted.correction_factor();
-            destination.resize(context_, next->parms_id(), size);
+            destination.resize(context_, r.parms_id, size);
             check(rescale ? sb200_rescale_to_next_sized_host(ctx_, L, size, 1, in.data(), destination.data())
                           : sb200_mod_switch_to_next_sized_host(ctx_, L, size, 1, in.data(), destination.data()));
-            destination.is_ntt_form() = ntt;
-            destination.scale() = scale;
-            if (bgv) // :1288-1293
-                destination.correction_factor() =
-                    seal::util::multiply_uint_mod(correction, cd->rns_tool()->inv_q_last_mod_t(), next->parms().plain_modulus());
+            destination.is_ntt_form() = r.ntt;
+            destination.scale() = r.scale;
+            if (scheme_ == seal::scheme_type::bgv) // :1288-1293
+                destination.correction_factor() = r.cf;
             throw_if_transparent(destination);
         }
-        // evaluator.cpp:2504-2559
-        void rotate_internal(seal::Ciphertext &encrypted, int steps, const seal::GaloisKeys &galois_keys, seal::MemoryPoolHandle pool) const
+        // rotate_internal (evaluator.cpp:2504-2559) of a seal::Ciphertext (pool: its pool) or a batch (no pool)
+        template <class Encrypted, class GaloisKeys, class... Pool>
+        void rotate_internal(Encrypted &encrypted, int steps, const GaloisKeys &galois_keys, const Pool &...pool) const
         {
-            auto cd = context_.get_context_data(encrypted.parms_id());
-            if (!cd)
-                throw std::invalid_argument("encrypted is not valid for encryption parameters");
-            if (!cd->qualifiers().using_batching)
-                throw std::logic_error("encryption parameters do not support batching");
+            auto cd = batching_level(encrypted);
             if (galois_keys.parms_id() != context_.key_parms_id())
                 throw std::invalid_argument("galois_keys is not valid for encryption parameters");
             if (steps == 0)
@@ -2931,7 +2733,7 @@ namespace seal_b200
             const std::uint32_t elt = cd->galois_tool()->get_elt_from_step(steps);
             if (galois_keys.has_key(elt))
             {
-                apply_galois_inplace(encrypted, elt, galois_keys, std::move(pool));
+                apply_galois_inplace(encrypted, elt, galois_keys, pool...);
                 return;
             }
             std::vector<int> naf_steps = seal::util::naf(steps);
@@ -2939,16 +2741,13 @@ namespace seal_b200
                 throw std::invalid_argument("Galois key not present");
             for (int s : naf_steps)
                 if (static_cast<std::size_t>(std::abs(s)) != (n >> 1))
-                    rotate_internal(encrypted, s, galois_keys, pool);
+                    rotate_internal(encrypted, s, galois_keys, pool...);
         }
-        void conjugate_internal(seal::Ciphertext &encrypted, const seal::GaloisKeys &galois_keys, seal::MemoryPoolHandle pool) const
+        // conjugate_internal (evaluator.h:1354-1377)
+        template <class Encrypted, class GaloisKeys, class... Pool>
+        void conjugate_internal(Encrypted &encrypted, const GaloisKeys &galois_keys, const Pool &...pool) const
         {
-            auto cd = context_.get_context_data(encrypted.parms_id());
-            if (!cd)
-                throw std::invalid_argument("encrypted is not valid for encryption parameters");
-            if (!cd->qualifiers().using_batching)
-                throw std::logic_error("encryption parameters do not support batching");
-            apply_galois_inplace(encrypted, cd->galois_tool()->get_elt_from_step(0), galois_keys, std::move(pool));
+            apply_galois_inplace(encrypted, batching_level(encrypted)->galois_tool()->get_elt_from_step(0), galois_keys, pool...);
         }
 
         seal::SEALContext context_;

@@ -1126,6 +1126,356 @@ static void test_encoder_and_encryptor()
     }
 }
 
+// ---- precedence matrix: invalid operands through seal::Evaluator, seal_b200::Evaluator on the same ciphertexts and on batches
+// uploaded from them, with the exception type AND message compared; doubly-invalid cases show the order of the checks.  A batch
+// keeps its words and metadata when a member throws.
+template <class F>
+static std::string thrown(F f)
+{
+    try
+    {
+        f();
+        return "ok";
+    }
+    catch (const std::exception &e)
+    {
+        return outcome([] { throw; }) + ": " + e.what();
+    }
+}
+
+struct Precedence
+{
+    seal::Evaluator &ref;
+    seal_b200::Evaluator &gpu;
+    // two copies of ct on the device
+    seal_b200::CiphertextBatch up(const Ciphertext &ct) const
+    {
+        seal_b200::CiphertextBatch d;
+        gpu.upload(std::vector<Ciphertext>(2, ct), d);
+        return d;
+    }
+    seal_b200::PlaintextBatch up(const Plaintext &pt) const
+    {
+        seal_b200::PlaintextBatch d;
+        gpu.upload(std::vector<Plaintext>(2, pt), d);
+        return d;
+    }
+    // r(x) on the reference, s(x) on the drop-in, b(batch of x) on the drop-in: the same error, and the batch unchanged
+    template <class R, class S, class B>
+    void operator()(const char *name, const Ciphertext &x, R r, S s, B b) const
+    {
+        Ciphertext rx = x, sx = x;
+        const std::string want = thrown([&] { r(rx); }), one = thrown([&] { s(sx); });
+        seal_b200::CiphertextBatch d = up(x);
+        const std::string batch = thrown([&] { b(d); });
+        std::vector<Ciphertext> back;
+        gpu.download(d, back);
+        const bool kept = back.size() == 2 && same_ct(back[0], x) && same_ct(back[1], x);
+        g_checks++;
+        if (want == "ok" || one != want || batch != want || !kept)
+        {
+            g_fail++;
+            std::printf("FAIL precedence %s: reference [%s], Ciphertext [%s], batch [%s]%s\n", name, want.c_str(), one.c_str(), batch.c_str(),
+                        kept ? "" : ", batch changed");
+        }
+    }
+    // the same member on both evaluators and the batch: f(evaluator, operand) for the first two, g(batch) for the third
+    template <class F, class G>
+    void same(const char *name, const Ciphertext &x, F f, G g) const
+    {
+        (*this)(name, x, [&](Ciphertext &t) { f(ref, t); }, [&](Ciphertext &t) { f(gpu, t); }, g);
+    }
+    // a plaintext member: reference, drop-in and PlaintextBatch give the same error
+    template <class F>
+    void plain(const char *name, const Plaintext &p, F f) const
+    {
+        Plaintext rp = p, sp = p;
+        seal_b200::PlaintextBatch d = up(p);
+        const std::string want = thrown([&] { f(ref, rp); }), one = thrown([&] { f(gpu, sp); }), batch = thrown([&] { f(gpu, d); });
+        g_checks++;
+        if (want == "ok" || one != want || batch != want)
+        {
+            g_fail++;
+            std::printf("FAIL precedence %s: reference [%s], Plaintext [%s], batch [%s]\n", name, want.c_str(), one.c_str(), batch.c_str());
+        }
+    }
+};
+
+static void test_precedence_ckks()
+{
+    EncryptionParameters parms(scheme_type::ckks);
+    const size_t n = 16384;
+    parms.set_poly_modulus_degree(n);
+    parms.set_coeff_modulus(CoeffModulus::Create(n, { 60, 50, 50, 40, 60 })); // 200 bits at the first data level
+    SEALContext context(parms, true, sec_level_type::none);
+    KeyGenerator keygen(context);
+    PublicKey pk;
+    keygen.create_public_key(pk);
+    RelinKeys rlk;
+    keygen.create_relin_keys(rlk);
+    GaloisKeys glk;
+    keygen.create_galois_keys(std::vector<int>{ 1 }, glk);
+    Encryptor encryptor(context, pk);
+    CKKSEncoder encoder(context);
+    seal::Evaluator ref(context);
+    seal_b200::Evaluator gpu(context);
+    const Precedence check{ ref, gpu };
+    auto fresh = [&](double scale) {
+        Plaintext p;
+        encoder.encode(std::vector<double>(n / 2, 1.0), scale, p);
+        Ciphertext c;
+        encryptor.encrypt(p, c);
+        return c;
+    };
+    const double s40 = std::pow(2.0, 40);
+    Ciphertext x = fresh(s40), y = fresh(s40), y_low, y_coeff, x_coeff, x_last, x_big = x, m3, m4;
+    ref.mod_switch_to_next(y, y_low);
+    ref.transform_from_ntt(y, y_coeff);
+    ref.transform_from_ntt(x, x_coeff);
+    ref.mod_switch_to(x, context.last_parms_id(), x_last);
+    x_big.scale() = std::pow(2.0, 120);
+    ref.multiply(x, y, m3);
+    ref.multiply(m3, y, m4);
+    // size 9 by three unrelinearized products: at scale 2^10 the product of two is only too large, at 2^20 also out of bounds
+    auto size9 = [&](double scale) {
+        Ciphertext c = fresh(scale);
+        for (int i = 0; i < 3; i++)
+        {
+            const Ciphertext d = c;
+            ref.multiply_inplace(c, d);
+        }
+        return c;
+    };
+    const Ciphertext s9 = size9(std::pow(2.0, 10)), t9 = size9(std::pow(2.0, 20));
+    Plaintext p, p_low, p_big;
+    encoder.encode(std::vector<double>(n / 2, 2.0), s40, p);
+    ref.mod_switch_to_next(p, p_low);
+    p_big = p, p_big.scale() = std::pow(2.0, 120);
+
+    auto multiply = [&](const char *name, const Ciphertext &a, const Ciphertext &b) {
+        check.same(name, a, [&](auto &ev, Ciphertext &t) { ev.multiply_inplace(t, b); },
+                   [&](seal_b200::CiphertextBatch &d) { auto e = check.up(b); gpu.multiply_inplace(d, e); });
+    };
+    multiply("CKKS multiply parameter mismatch", x, y_low);
+    multiply("CKKS multiply form", x, y_coeff);
+    multiply("CKKS multiply size", s9, s9);
+    multiply("CKKS multiply scale", x_big, x_big);
+    multiply("CKKS multiply size and scale", t9, t9);
+    multiply("CKKS multiply mismatch and form", x_coeff, y_low);
+    auto add = [&](const char *name, const Ciphertext &a, const Ciphertext &b) {
+        check.same(name, a, [&](auto &ev, Ciphertext &t) { ev.sub_inplace(t, b); },
+                   [&](seal_b200::CiphertextBatch &d) { auto e = check.up(b); gpu.sub_inplace(d, e); });
+    };
+    Ciphertext y_scaled = y;
+    y_scaled.scale() *= 2;
+    add("CKKS sub parameter mismatch", x, y_low);
+    add("CKKS sub form", x, y_coeff);
+    add("CKKS sub scale", x, y_scaled);
+    add("CKKS sub form and scale", x_coeff, y_scaled);
+    auto multiply_plain = [&](const char *name, const Ciphertext &a, const Plaintext &q) {
+        check.same(name, a, [&](auto &ev, Ciphertext &t) { ev.multiply_plain_inplace(t, q); },
+                   [&](seal_b200::CiphertextBatch &d) { auto e = check.up(q); gpu.multiply_plain_inplace(d, e); });
+    };
+    multiply_plain("CKKS multiply_plain parameter mismatch", x, p_low);
+    multiply_plain("CKKS multiply_plain scale", x_big, p_big);
+    multiply_plain("CKKS multiply_plain mismatch and scale", x_big, [&] { Plaintext q = p_low; q.scale() = p_big.scale(); return q; }());
+    auto add_plain = [&](const char *name, const Ciphertext &a, const Plaintext &q) {
+        check.same(name, a, [&](auto &ev, Ciphertext &t) { ev.add_plain_inplace(t, q); },
+                   [&](seal_b200::CiphertextBatch &d) { auto e = check.up(q); gpu.add_plain_inplace(d, e); });
+    };
+    add_plain("CKKS add_plain form", x_coeff, p);
+    add_plain("CKKS add_plain parameter mismatch", x, p_low);
+    add_plain("CKKS add_plain scale", x, p_big);
+    add_plain("CKKS add_plain form and mismatch", x_coeff, p_low);
+    RelinKeys rlk_bad = rlk;
+    rlk_bad.parms_id() = parms_id_zero;
+    auto relinearize = [&](const char *name, const Ciphertext &a, const RelinKeys &k) {
+        check.same(name, a, [&](auto &ev, Ciphertext &t) { ev.relinearize_inplace(t, k); }, [&](seal_b200::CiphertextBatch &d) { gpu.relinearize_inplace(d, k); });
+    };
+    Ciphertext m3_coeff;
+    ref.transform_from_ntt(m3, m3_coeff);
+    relinearize("CKKS relinearize key level", m3, rlk_bad);
+    relinearize("CKKS relinearize too few keys", m4, rlk);
+    relinearize("CKKS relinearize form", m3_coeff, rlk);
+    relinearize("CKKS relinearize key level and too few keys", m4, rlk_bad);
+    GaloisKeys glk_bad = glk;
+    glk_bad.parms_id() = parms_id_zero;
+    const std::uint32_t e1 = context.key_context_data()->galois_tool()->get_elt_from_step(1);
+    const std::uint32_t e2 = context.key_context_data()->galois_tool()->get_elt_from_step(2);
+    auto galois = [&](const char *name, const Ciphertext &a, std::uint32_t elt, const GaloisKeys &k) {
+        check.same(name, a, [&](auto &ev, Ciphertext &t) { ev.apply_galois_inplace(t, elt, k); },
+                   [&](seal_b200::CiphertextBatch &d) { gpu.apply_galois_inplace(d, elt, k); });
+    };
+    galois("CKKS apply_galois key level", x, e1, glk_bad);
+    galois("CKKS apply_galois missing key", x, e2, glk);
+    galois("CKKS apply_galois even element", x, 4, glk);
+    galois("CKKS apply_galois element too large", x, 2 * n + 1, glk);
+    galois("CKKS apply_galois size", m3, e1, glk);
+    galois("CKKS apply_galois form", x_coeff, e1, glk);
+    galois("CKKS apply_galois size and form", m3_coeff, e1, glk);
+    check.same("CKKS rotate_rows scheme", x, [&](auto &ev, Ciphertext &t) { ev.rotate_rows_inplace(t, 1, glk); },
+               [&](seal_b200::CiphertextBatch &d) { gpu.rotate_rows_inplace(d, 1, glk); });
+    check.same("CKKS rotate_vector missing key", x, [&](auto &ev, Ciphertext &t) { ev.rotate_vector_inplace(t, 2, glk); },
+               [&](seal_b200::CiphertextBatch &d) { gpu.rotate_vector_inplace(d, 2, glk); });
+    check.same("CKKS rotate_vector key level and missing key", x, [&](auto &ev, Ciphertext &t) { ev.rotate_vector_inplace(t, 2, glk_bad); },
+               [&](seal_b200::CiphertextBatch &d) { gpu.rotate_vector_inplace(d, 2, glk_bad); });
+    check.same("CKKS complex_conjugate missing key", x, [&](auto &ev, Ciphertext &t) { ev.complex_conjugate_inplace(t, glk); },
+               [&](seal_b200::CiphertextBatch &d) { gpu.complex_conjugate_inplace(d, glk); });
+    check.same("CKKS rotate_columns scheme", x, [&](auto &ev, Ciphertext &t) { ev.rotate_columns_inplace(t, glk); },
+               [&](seal_b200::CiphertextBatch &d) { gpu.rotate_columns_inplace(d, glk); });
+    auto rescale = [&](const char *name, const Ciphertext &a) {
+        check.same(name, a, [&](auto &ev, Ciphertext &t) { ev.rescale_to_next_inplace(t); }, [&](seal_b200::CiphertextBatch &d) { gpu.rescale_to_next_inplace(d); });
+    };
+    Ciphertext x_huge = x, x_huge_coeff = x_coeff;
+    x_huge.scale() = x_huge_coeff.scale() = std::pow(2.0, 250);
+    rescale("CKKS rescale_to_next end of chain", x_last);
+    rescale("CKKS rescale_to_next form", x_coeff);
+    rescale("CKKS rescale_to_next scale", x_huge);
+    rescale("CKKS rescale_to_next form and scale", x_huge_coeff);
+    check.same("CKKS mod_switch_to_next form", x_coeff, [&](auto &ev, Ciphertext &t) { ev.mod_switch_to_next_inplace(t); },
+               [&](seal_b200::CiphertextBatch &d) { gpu.mod_switch_to_next_inplace(d); });
+    check.same("CKKS mod_switch_to_next scale", x_huge, [&](auto &ev, Ciphertext &t) { ev.mod_switch_to_next_inplace(t); },
+               [&](seal_b200::CiphertextBatch &d) { gpu.mod_switch_to_next_inplace(d); });
+    const parms_id_type top = x.parms_id();
+    check.same("CKKS rescale_to a higher level", y_low, [&](auto &ev, Ciphertext &t) { ev.rescale_to_inplace(t, top); },
+               [&](seal_b200::CiphertextBatch &d) { gpu.rescale_to_inplace(d, top); });
+    check.same("CKKS mod_switch_to a higher level", y_low, [&](auto &ev, Ciphertext &t) { ev.mod_switch_to_inplace(t, top); },
+               [&](seal_b200::CiphertextBatch &d) { gpu.mod_switch_to_inplace(d, top); });
+    Plaintext p_tight = p, p_last;
+    p_tight.scale() = std::pow(2.0, 170); // within the first level's 200 bits, not the next level's 160
+    ref.mod_switch_to(p, context.last_parms_id(), p_last);
+    check.plain("CKKS plaintext mod_switch_to_next scale", p_tight, [](auto &ev, auto &q) { ev.mod_switch_to_next_inplace(q); });
+    check.plain("CKKS plaintext mod_switch_to_next end of chain", p_last, [](auto &ev, auto &q) { ev.mod_switch_to_next_inplace(q); });
+    check.plain("CKKS plaintext mod_switch_to a higher level", p_low, [&](auto &ev, auto &q) { ev.mod_switch_to_inplace(q, top); });
+}
+
+// BFV and BGV: the per-scheme form rules, rotations, plaintext level changes and multiply_relinearize_inplace against its chain
+static void test_precedence_integer(scheme_type scheme)
+{
+    const bool bfv = scheme == scheme_type::bfv;
+    EncryptionParameters parms(scheme);
+    const size_t n = 4096;
+    parms.set_poly_modulus_degree(n);
+    parms.set_coeff_modulus(CoeffModulus::Create(n, { 30, 30, 40 }));
+    parms.set_plain_modulus(PlainModulus::Batching(n, 20));
+    SEALContext context(parms, true, sec_level_type::none);
+    KeyGenerator keygen(context);
+    PublicKey pk;
+    keygen.create_public_key(pk);
+    RelinKeys rlk;
+    keygen.create_relin_keys(rlk);
+    GaloisKeys glk;
+    keygen.create_galois_keys(std::vector<int>{ 1 }, glk);
+    Encryptor encryptor(context, pk);
+    BatchEncoder encoder(context);
+    seal::Evaluator ref(context);
+    seal_b200::Evaluator gpu(context);
+    const Precedence check{ ref, gpu };
+    Plaintext p, p_ntt, p_ntt_low, p_last;
+    encoder.encode(std::vector<std::uint64_t>(n, 3), p);
+    ref.transform_to_ntt(p, context.first_parms_id(), p_ntt);
+    ref.transform_to_ntt(p, context.last_parms_id(), p_ntt_low);
+    p_last = p_ntt_low;
+    Ciphertext x, y, x_wrong, y_low, x_last, x_last_wrong, m3, m3_wrong;
+    encryptor.encrypt(p, x);
+    encryptor.encrypt(p, y);
+    if (bfv)
+        ref.transform_to_ntt(x, x_wrong);
+    else
+        ref.transform_from_ntt(x, x_wrong);
+    ref.mod_switch_to_next(y, y_low);
+    ref.mod_switch_to_next(x, x_last);
+    if (bfv)
+        ref.transform_to_ntt(x_last, x_last_wrong);
+    else
+        ref.transform_from_ntt(x_last, x_last_wrong);
+    ref.multiply(x, y, m3);
+    if (bfv)
+        ref.transform_to_ntt(m3, m3_wrong);
+    else
+        ref.transform_from_ntt(m3, m3_wrong);
+    const std::string tag = bfv ? "BFV " : "BGV ";
+    auto name = [&](const char *what) { static std::string s; s = tag + what; return s.c_str(); };
+
+    auto multiply = [&](const char *what, const Ciphertext &a, const Ciphertext &b) {
+        check.same(name(what), a, [&](auto &ev, Ciphertext &t) { ev.multiply_inplace(t, b); },
+                   [&](seal_b200::CiphertextBatch &d) { auto e = check.up(b); gpu.multiply_inplace(d, e); });
+    };
+    multiply("multiply parameter mismatch", x, y_low);
+    multiply("multiply form", x_wrong, y);
+    multiply("multiply mismatch and form", x_wrong, y_low);
+    auto add_plain = [&](const char *what, const Ciphertext &a, const Plaintext &q) {
+        check.same(name(what), a, [&](auto &ev, Ciphertext &t) { ev.add_plain_inplace(t, q); },
+                   [&](seal_b200::CiphertextBatch &d) { auto e = check.up(q); gpu.add_plain_inplace(d, e); });
+    };
+    add_plain("add_plain encrypted form", x_wrong, p);
+    add_plain("add_plain plain form", x, p_ntt);
+    add_plain("add_plain both forms", x_wrong, p_ntt);
+    auto multiply_plain = [&](const char *what, const Ciphertext &a, const Plaintext &q) {
+        check.same(name(what), a, [&](auto &ev, Ciphertext &t) { ev.multiply_plain_inplace(t, q); },
+                   [&](seal_b200::CiphertextBatch &d) { auto e = check.up(q); gpu.multiply_plain_inplace(d, e); });
+    };
+    multiply_plain("multiply_plain parameter mismatch", x, p_ntt_low);
+    check.same(name("sub form"), x, [&](auto &ev, Ciphertext &t) { ev.sub_inplace(t, x_wrong); },
+               [&](seal_b200::CiphertextBatch &d) { auto e = check.up(x_wrong); gpu.sub_inplace(d, e); });
+    RelinKeys rlk_bad = rlk, rlk_none;
+    rlk_bad.parms_id() = parms_id_zero;
+    rlk_none.parms_id() = context.key_parms_id();
+    check.same(name("relinearize form"), m3_wrong, [&](auto &ev, Ciphertext &t) { ev.relinearize_inplace(t, rlk); },
+               [&](seal_b200::CiphertextBatch &d) { gpu.relinearize_inplace(d, rlk); });
+    // multiply_relinearize_inplace stands for multiply_inplace, then relinearize_inplace
+    auto multiply_relinearize = [&](const char *what, const Ciphertext &a, const Ciphertext &b, const RelinKeys &k) {
+        check(name(what), a, [&](Ciphertext &t) { ref.multiply_inplace(t, b); ref.relinearize_inplace(t, k); },
+              [&](Ciphertext &t) { gpu.multiply_inplace(t, b); gpu.relinearize_inplace(t, k); },
+              [&](seal_b200::CiphertextBatch &d) { auto e = check.up(b); gpu.multiply_relinearize_inplace(d, e, k); });
+    };
+    multiply_relinearize("multiply_relinearize key level", x, y, rlk_bad);
+    multiply_relinearize("multiply_relinearize no key", x, y, rlk_none);
+    multiply_relinearize("multiply_relinearize form", x_wrong, y, rlk);
+    multiply_relinearize("multiply_relinearize key level and form", x_wrong, y, rlk_bad);
+    check.same(name("rotate_vector scheme"), x, [&](auto &ev, Ciphertext &t) { ev.rotate_vector_inplace(t, 1, glk); },
+               [&](seal_b200::CiphertextBatch &d) { gpu.rotate_vector_inplace(d, 1, glk); });
+    check.same(name("rotate_rows missing key"), x, [&](auto &ev, Ciphertext &t) { ev.rotate_rows_inplace(t, 2, glk); },
+               [&](seal_b200::CiphertextBatch &d) { gpu.rotate_rows_inplace(d, 2, glk); });
+    check.same(name("rotate_columns missing key"), x, [&](auto &ev, Ciphertext &t) { ev.rotate_columns_inplace(t, glk); },
+               [&](seal_b200::CiphertextBatch &d) { gpu.rotate_columns_inplace(d, glk); });
+    check.same(name("complex_conjugate scheme"), x, [&](auto &ev, Ciphertext &t) { ev.complex_conjugate_inplace(t, glk); },
+               [&](seal_b200::CiphertextBatch &d) { gpu.complex_conjugate_inplace(d, glk); });
+    check.same(name("rescale_to_next scheme"), x, [&](auto &ev, Ciphertext &t) { ev.rescale_to_next_inplace(t); },
+               [&](seal_b200::CiphertextBatch &d) { gpu.rescale_to_next_inplace(d); });
+    check.same(name("rescale_to_next end of chain and scheme"), x_last, [&](auto &ev, Ciphertext &t) { ev.rescale_to_next_inplace(t); },
+               [&](seal_b200::CiphertextBatch &d) { gpu.rescale_to_next_inplace(d); });
+    check.same(name("mod_switch_to_next form"), x_wrong, [&](auto &ev, Ciphertext &t) { ev.mod_switch_to_next_inplace(t); },
+               [&](seal_b200::CiphertextBatch &d) { gpu.mod_switch_to_next_inplace(d); });
+    check.same(name("mod_switch_to_next end of chain and form"), x_last_wrong, [&](auto &ev, Ciphertext &t) { ev.mod_switch_to_next_inplace(t); },
+               [&](seal_b200::CiphertextBatch &d) { gpu.mod_switch_to_next_inplace(d); });
+    check.plain(name("plaintext mod_switch_to_next form"), p, [](auto &ev, auto &q) { ev.mod_switch_to_next_inplace(q); });
+    check.plain(name("plaintext mod_switch_to_next end of chain"), p_last, [](auto &ev, auto &q) { ev.mod_switch_to_next_inplace(q); });
+    if (!bfv)
+        return;
+    // parameters without batching: rotations fail on that before they look at the keys
+    EncryptionParameters nb(scheme_type::bfv);
+    nb.set_poly_modulus_degree(n);
+    nb.set_coeff_modulus(CoeffModulus::Create(n, { 30, 30, 40 }));
+    nb.set_plain_modulus(1024);
+    SEALContext nbc(nb, true, sec_level_type::none);
+    KeyGenerator nbk(nbc);
+    PublicKey nbpk;
+    nbk.create_public_key(nbpk);
+    Encryptor nbe(nbc, nbpk);
+    seal::Evaluator nbref(nbc);
+    seal_b200::Evaluator nbgpu(nbc);
+    const Precedence nbcheck{ nbref, nbgpu };
+    Plaintext one("1");
+    Ciphertext z;
+    nbe.encrypt(one, z);
+    GaloisKeys none;
+    nbcheck.same("BFV rotate_rows without batching", z, [&](auto &ev, Ciphertext &t) { ev.rotate_rows_inplace(t, 1, none); },
+                 [&](seal_b200::CiphertextBatch &d) { nbgpu.rotate_rows_inplace(d, 1, none); });
+    nbcheck.same("BFV rotate_columns without batching", z, [&](auto &ev, Ciphertext &t) { ev.rotate_columns_inplace(t, none); },
+                 [&](seal_b200::CiphertextBatch &d) { nbgpu.rotate_columns_inplace(d, none); });
+}
+
 int main()
 {
     try
@@ -1135,6 +1485,9 @@ int main()
         test_bgv();
         test_batches_and_keys();
         test_encoder_and_encryptor();
+        test_precedence_ckks();
+        test_precedence_integer(scheme_type::bfv);
+        test_precedence_integer(scheme_type::bgv);
     }
     catch (const std::exception &e)
     {
