@@ -354,6 +354,43 @@ int sb200_rotate_sum(sb200_context *ctx, size_t L, size_t batch, const uint64_t 
                      const sb200_kswitch_key *const *galois_keys, uint64_t *d_out2, void *stream);
 int sb200_rotate_sum_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *h_in2, size_t steps, const uint32_t *galois_elts,
                           const sb200_kswitch_key *const *galois_keys, uint64_t *h_out2);
+/* d_out2 = d_addend2 + d_plain * apply_galois(d_in2): Evaluator::apply_galois_inplace, Evaluator::multiply_plain_inplace and
+ * Evaluator::add_inplace (evaluator.cpp:2384-2502, :1975-2020, :155-261) on a copy of the input.  d_plain holds plain_count (1 for the
+ * whole batch, or batch) NTT-form plaintexts [L][n] at the input's level, in any 64-bit words (reduced as sb200_multiply_plain_n
+ * reduces them).  CKKS / BGV: one key switch, with the plaintext product and the addition in its last pass (no copy, no product or
+ * add pass; the same words).  BFV: the chain itself through one key-switching chunk of temporary (apply_galois, the ciphertext to NTT
+ * form, the product, back, the addition), as the reference multiplies a coefficient-form ciphertext by an NTT-form plaintext.
+ * Aliasing as sb200_apply_galois_add: d_out2 may be d_addend2, d_addend2 may be d_in2, d_out2 == d_in2 is SB200_E_INVALID_ARG.
+ * Errors, all before the first launch in the chain's order (the output is unchanged): sb200_apply_galois's, then a plain_count other
+ * than 1 or batch (SB200_E_INVALID_ARG); a NULL slab (SB200_E_POINTER); overlapping slabs (SB200_E_INVALID_ARG).  The _host form takes
+ * host buffers of the same layouts; h_out2 may be h_addend2. */
+int sb200_apply_galois_multiply_plain_add(sb200_context *ctx, size_t L, size_t batch, const uint64_t *d_in2, uint32_t galois_elt,
+                                          const sb200_kswitch_key *galois_key, size_t plain_count, const uint64_t *d_plain,
+                                          const uint64_t *d_addend2, uint64_t *d_out2, void *stream);
+int sb200_apply_galois_multiply_plain_add_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *h_in2, uint32_t galois_elt,
+                                               const sb200_kswitch_key *galois_key, size_t plain_count, const uint64_t *h_plain,
+                                               const uint64_t *h_addend2, uint64_t *h_out2);
+/* A plaintext matrix times an encrypted vector by diagonals: d_out2 = sum_i d_plains[i] * apply_galois(d_in2, galois_elts[i]), the
+ * reference's chain  t = encrypted; rotate_rows / rotate_vector / apply_galois_inplace(t, ...); multiply_plain_inplace(t, plain_i);
+ * i == 0 ? destination = t : add_inplace(destination, t)  (evaluator.cpp:2504-2559, :2384-2502, :1975-2020, :155-261) in one call.
+ * Element 1 is no rotation (rotate_internal's step 0): no key switch, and its galois_keys entry may be NULL.  d_plains[i] holds
+ * plain_counts[i] (1 or batch) plaintexts: NTT form [L][n] (plain_is_ntt != 0) or coefficient form [n] (BFV / BGV; each lifted and
+ * transformed as Evaluator::transform_to_ntt_inplace does).  Shared and per-member plaintexts may be mixed in one call.
+ * The identity terms go into one sb200_multiply_plain_sum pass that writes d_out2; each rotated term then accumulates into it.  CKKS
+ * and BGV: each rotated term is one key switch with the product and the addition in its last pass, with no batch-sized temporary.
+ * BFV: each rotated term is the chain itself through one key-switching chunk of temporary.  Each key-switching chunk
+ * (SB200_LIMIT_SCRATCH_BYTES, SB200_LIMIT_KS_CHUNK) runs every term, so each key is read once per chunk and term, as by the chain.
+ * d_out2 must not alias d_in2 (SB200_E_INVALID_ARG) and may not overlap any input.  Errors, all before the first launch in the chain's
+ * order (the output is unchanged): every rotated term's element and key as sb200_apply_galois checks them, then every plain_counts[i]
+ * (1 or batch) and coefficient-form plaintexts in CKKS, then count = 0 (all SB200_E_INVALID_ARG); a NULL array, plaintext slab or
+ * rotated term's key (SB200_E_POINTER); overlapping slabs (SB200_E_INVALID_ARG).  The _host form stages each chunk of
+ * SB200_LIMIT_HOST_STAGE_BYTES once, and each shared plaintext once per call. */
+int sb200_diagonal_sum(sb200_context *ctx, size_t L, size_t batch, const uint64_t *d_in2, size_t count, const uint32_t *galois_elts,
+                       const sb200_kswitch_key *const *galois_keys, const size_t *plain_counts, const uint64_t *const *d_plains,
+                       int plain_is_ntt, uint64_t *d_out2, void *stream);
+int sb200_diagonal_sum_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *h_in2, size_t count, const uint32_t *galois_elts,
+                            const sb200_kswitch_key *const *galois_keys, const size_t *plain_counts, const uint64_t *const *h_plains,
+                            int plain_is_ntt, uint64_t *h_out2);
 
 /* ---- host-buffer variants: H2D copy, operation, D2H copy, synchronise (the plugin-facing end-to-end path) ---- */
 int sb200_ntt_forward_host(sb200_context *ctx, size_t L, size_t size, size_t batch, uint64_t *h_data);

@@ -1335,6 +1335,51 @@ namespace seal_b200
         {
             rotate_sum_batch(encrypted, step, count, galois_keys);
         }
+        // Plaintext matrix times encrypted vector by diagonals.  apply_galois_multiply_plain_add_inplace: destination +=
+        // plain * apply_galois(encrypted), the words and metadata of
+        //     t = encrypted; apply_galois_inplace(t, galois_elt, galois_keys); multiply_plain_inplace(t, plain); add_inplace(destination, t);
+        // CKKS / BGV with an NTT-form plaintext: one sb200_apply_galois_multiply_plain_add, the product and the addition in the key
+        // switch's last pass.  destination may be encrypted.  The chain's checks and messages run first (apply_galois_inplace's,
+        // multiply_plain_inplace's, then add_inplace's, "scale mismatch" included); a coefficient-form plaintext, BFV, BGV operands
+        // whose correction factors need balancing, or a destination of another size than 2 take the chain itself.
+        void apply_galois_multiply_plain_add_inplace(CiphertextBatch &destination, const CiphertextBatch &encrypted, std::uint32_t galois_elt,
+                                                     const PlaintextBatch &plain, const seal::GaloisKeys &galois_keys) const
+        {
+            apply_galois_multiply_plain_add_batch(destination, encrypted, galois_elt, plain, galois_keys);
+        }
+        void apply_galois_multiply_plain_add_inplace(CiphertextBatch &destination, const CiphertextBatch &encrypted, std::uint32_t galois_elt,
+                                                     const PlaintextBatch &plain, const DeviceGaloisKeys &galois_keys) const
+        {
+            apply_galois_multiply_plain_add_batch(destination, encrypted, galois_elt, plain, galois_keys);
+        }
+        // diagonal_sum: destination = sum_i diagonals[i] * rotate(encrypted, steps[i]), the words and metadata of
+        //     for each i: t = encrypted; if (steps[i]) rotate_X_inplace(t, steps[i], galois_keys); multiply_plain_inplace(t, diagonals[i]);
+        //                 i == 0 ? destination = t : add_inplace(destination, t)
+        // with rotate_X = rotate_vector (CKKS) or rotate_rows (BFV / BGV); step 0 is no rotation, as in rotate_internal.  The
+        // destination's scale is the first term's (CKKS: the ciphertext's times the diagonal's, and every term's must match it or
+        // "scale mismatch" is thrown); BGV's correction factor is the ciphertext's.  One sb200_diagonal_sum call: every step-0 term in
+        // one multiply_plain_sum pass, every other term one key switch with the product and the addition in its last pass (CKKS /
+        // BGV); BFV runs the chain on the device through one key-switching chunk of temporary.  Every check of the chain, term by
+        // term in its order, runs before anything is written.  The chain itself runs when a step's key exists only through SEAL's
+        // NAF decomposition, when encrypted's size is not 2, when the diagonals mix NTT and coefficient form, or when BGV correction
+        // factors would need balancing.  No key of the call is evicted from the key cache while it runs.  destination must not be
+        // encrypted.
+        // A small matrix M (d x d, d dividing the slot count) times a vector v replicated across the slots, CKKS:
+        //     std::vector<int> steps(d); std::vector<PlaintextBatch> diags(d);
+        //     for (int i = 0; i < d; i++) { steps[i] = i; diags[i] = encode(slot j -> M[j % d][(j + i) % d]); }
+        //     evaluator.diagonal_sum(v, steps, diags, gk, y);     // slot j of y holds (M v)[j % d]
+        // Larger matrices by baby-step giant-step compose from the existing calls: the baby-step rotations once, each giant step's
+        // inner sum with multiply_plain_sum, and the giant-step rotations accumulated with apply_galois_add_inplace.
+        void diagonal_sum(const CiphertextBatch &encrypted, const std::vector<int> &steps, const std::vector<PlaintextBatch> &diagonals,
+                          const seal::GaloisKeys &galois_keys, CiphertextBatch &destination) const
+        {
+            diagonal_sum_batch(encrypted, steps, diagonals, galois_keys, destination);
+        }
+        void diagonal_sum(const CiphertextBatch &encrypted, const std::vector<int> &steps, const std::vector<PlaintextBatch> &diagonals,
+                          const DeviceGaloisKeys &galois_keys, CiphertextBatch &destination) const
+        {
+            diagonal_sum_batch(encrypted, steps, diagonals, galois_keys, destination);
+        }
 
     private:
         template <class GaloisKeys>
@@ -1420,6 +1465,120 @@ namespace seal_b200
                 keys.push_back(k);
             }
             check(sb200_rotate_sum(ctx_, encrypted.L_, encrypted.batch_, encrypted.d_, elts.size(), elts.data(), keys.data(), encrypted.d_, nullptr));
+        }
+        template <class GaloisKeys>
+        void apply_galois_multiply_plain_add_batch(CiphertextBatch &destination, const CiphertextBatch &encrypted, std::uint32_t galois_elt,
+                                                   const PlaintextBatch &plain, const GaloisKeys &galois_keys) const
+        {
+            owned(encrypted);
+            check_apply_galois(meta(encrypted), galois_elt, galois_keys);
+            owned(plain);
+            plain_count(encrypted, plain);
+            const Meta t = multiply_plain_meta(meta(encrypted), meta(plain)); // apply_galois leaves the metadata alone
+            {
+                std::lock_guard<std::mutex> lock(mu_);
+                sb200_kswitch_key *key = key_for(galois_keys, seal::GaloisKeys::get_index(galois_elt), encrypted.L_);
+                owned(destination);
+                const Fold f = plan_fold({ meta(destination), t }, SB200_FOLD_ADD); // add_inplace(destination, t)
+                if (scheme_ != seal::scheme_type::bfv && plain.ntt_ && f.factors.empty() && destination.size_ == 2)
+                {
+                    const bool same = &destination == &encrypted; // out must not be the input: through the result slab
+                    std::uint64_t *out = same ? out_slab(destination.batch_ * destination.words_per_ciphertext(), destination) : destination.d_;
+                    check(sb200_apply_galois_multiply_plain_add(ctx_, encrypted.L_, encrypted.batch_, encrypted.d_, galois_elt, key, plain.batch_,
+                                                                plain.d_, destination.d_, out, nullptr));
+                    if (same)
+                        adopt(destination);
+                    return;
+                }
+            }
+            CiphertextBatch tmp;
+            copy(encrypted, tmp);
+            apply_galois_batch(tmp, galois_elt, galois_keys);
+            multiply_plain_inplace(tmp, plain);
+            add_inplace(destination, tmp);
+        }
+        template <class GaloisKeys>
+        void diagonal_sum_batch(const CiphertextBatch &encrypted, const std::vector<int> &steps, const std::vector<PlaintextBatch> &diagonals,
+                                const GaloisKeys &galois_keys, CiphertextBatch &destination) const
+        {
+            if (steps.empty())
+                throw std::invalid_argument("steps cannot be empty");
+            if (diagonals.size() != steps.size())
+                throw std::invalid_argument("diagonals must hold one plaintext batch per step");
+            if (&destination == &encrypted)
+                throw std::invalid_argument("encrypted must be different from destination");
+            const bool ckks = scheme_ == seal::scheme_type::ckks;
+            if (!ckks && scheme_ != seal::scheme_type::bfv && scheme_ != seal::scheme_type::bgv)
+                throw std::logic_error("unsupported scheme");
+            // the chain's checks, term by term: rotate_internal's, multiply_plain_inplace's, add_inplace's
+            std::vector<std::uint32_t> elts;
+            bool naf = false;
+            Fold f;
+            for (std::size_t i = 0; i < steps.size(); i++)
+            {
+                auto cd = batching_level(encrypted);
+                if (galois_keys.parms_id() != context_.key_parms_id())
+                    throw std::invalid_argument("galois_keys is not valid for encryption parameters");
+                std::uint32_t elt = 1;
+                if (steps[i] != 0)
+                {
+                    elt = cd->galois_tool()->get_elt_from_step(steps[i]); // "step count too large"
+                    if (galois_keys.has_key(elt))
+                        check_apply_galois(meta(encrypted), elt, galois_keys);
+                    else if (seal::util::naf(steps[i]).size() == 1)
+                        throw std::invalid_argument("Galois key not present");
+                    else
+                        naf = true;
+                }
+                elts.push_back(elt);
+                owned(diagonals[i]);
+                plain_count(encrypted, diagonals[i]);
+                const Meta t = multiply_plain_meta(meta(encrypted), meta(diagonals[i]));
+                if (i == 0)
+                    f = Fold{ t, { t.size }, {}, {} };
+                else
+                    fold_in(f, t, SB200_FOLD_ADD);
+            }
+            bool mixed = false;
+            for (auto &d : diagonals)
+                mixed |= d.ntt_ != diagonals[0].ntt_;
+            if (naf || mixed || encrypted.size_ != 2 || !f.factors.empty() || encrypted.ntt_ != (scheme_ != seal::scheme_type::bfv))
+            {
+                for (std::size_t i = 0; i < steps.size(); i++)
+                {
+                    CiphertextBatch t;
+                    copy(encrypted, t);
+                    rotate_internal(t, steps[i], galois_keys);
+                    multiply_plain_inplace(t, diagonals[i]);
+                    if (i == 0)
+                        destination = std::move(t);
+                    else
+                        add_inplace(destination, t);
+                }
+                return;
+            }
+            std::lock_guard<std::mutex> lock(mu_);
+            struct Unpin // the keys of this call stay in the cache until it returns
+            {
+                std::vector<const sb200_kswitch_key *> &pinned;
+                ~Unpin() { pinned.clear(); }
+            } unpin{ pinned_ };
+            std::vector<const sb200_kswitch_key *> keys;
+            std::vector<std::size_t> counts;
+            std::vector<const std::uint64_t *> plains;
+            for (std::size_t i = 0; i < steps.size(); i++)
+            {
+                sb200_kswitch_key *k = elts[i] == 1 ? nullptr : key_for(galois_keys, seal::GaloisKeys::get_index(elts[i]), encrypted.L_);
+                if (k)
+                    pinned_.push_back(k);
+                keys.push_back(k);
+                counts.push_back(diagonals[i].batch_);
+                plains.push_back(diagonals[i].d_);
+            }
+            shape(destination, encrypted.batch_, 2, encrypted.L_, encrypted.n_);
+            assign(destination, f.result);
+            check(sb200_diagonal_sum(ctx_, encrypted.L_, encrypted.batch_, encrypted.d_, steps.size(), elts.data(), keys.data(), counts.data(),
+                                     plains.data(), diagonals[0].ntt_ ? 1 : 0, destination.d_, nullptr));
         }
         template <class GaloisKeys>
         void apply_galois_batch(CiphertextBatch &encrypted, std::uint32_t galois_elt, const GaloisKeys &galois_keys) const

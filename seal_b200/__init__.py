@@ -37,7 +37,8 @@ SYMBOLS = [
     "sb200_multiply_plain_coeff_n_host", "sb200_add_plain_coeff_n_host", "sb200_add_plain_ntt_host",
     "sb200_add_many", "sb200_add_many_host", "sb200_multiply_plain_sum", "sb200_multiply_plain_sum_host", "sb200_multiply_sum", "sb200_multiply_sum_host", "sb200_relinearize_host", "sb200_multiply_relinearize_host", "sb200_rescale_to_next_host",
     "sb200_mod_switch_to_next_host", "sb200_apply_galois_host", "sb200_apply_galois_add", "sb200_apply_galois_add_host",
-    "sb200_rotate_sum", "sb200_rotate_sum_host", "sb200_get_parms_id", "sb200_ciphertext_inspect",
+    "sb200_rotate_sum", "sb200_rotate_sum_host", "sb200_apply_galois_multiply_plain_add", "sb200_apply_galois_multiply_plain_add_host",
+    "sb200_diagonal_sum", "sb200_diagonal_sum_host", "sb200_get_parms_id", "sb200_ciphertext_inspect",
     "sb200_ciphertext_save_size", "sb200_ciphertext_load", "sb200_ciphertext_save", "sb200_secret_key_create",
     "sb200_secret_key_destroy", "sb200_decrypt", "sb200_decrypt_host", "sb200_invariant_noise_budget", "sb200_invariant_noise_budget_host", "sb200_encrypt_zero_symmetric", "sb200_public_key_create", "sb200_public_key_destroy", "sb200_encrypt_zero_asymmetric", "sb200_encrypt_zero_symmetric_prng", "sb200_encrypt_zero_asymmetric_prng", "sb200_encrypt_symmetric", "sb200_encrypt_asymmetric", "sb200_kswitch_key_generate", "sb200_public_key_generate", "sb200_ciphertext_save_seeded_size", "sb200_ciphertext_save_seeded",
     "sb200_public_key_generate_seeded", "sb200_kswitch_keys_save_seeded_size", "sb200_kswitch_keys_generate_seeded", "sb200_ckks_encode", "sb200_ckks_decode", "sb200_ckks_encode_host", "sb200_ckks_decode_host",
@@ -164,6 +165,10 @@ def lib():
         L.sb200_apply_galois_add_host.argtypes = [vp, sz, sz, _u64p, u32, vp, _u64p, _u64p]
         L.sb200_rotate_sum.argtypes = [vp, sz, sz, vp, sz, C.POINTER(u32), C.POINTER(vp), vp, vp]
         L.sb200_rotate_sum_host.argtypes = [vp, sz, sz, _u64p, sz, C.POINTER(u32), C.POINTER(vp), _u64p]
+        L.sb200_apply_galois_multiply_plain_add.argtypes = [vp, sz, sz, vp, u32, vp, sz, vp, vp, vp, vp]
+        L.sb200_apply_galois_multiply_plain_add_host.argtypes = [vp, sz, sz, _u64p, u32, vp, sz, _u64p, _u64p, _u64p]
+        L.sb200_diagonal_sum.argtypes = [vp, sz, sz, vp, sz, C.POINTER(u32), C.POINTER(vp), C.POINTER(sz), C.POINTER(vp), C.c_int, vp, vp]
+        L.sb200_diagonal_sum_host.argtypes = [vp, sz, sz, _u64p, sz, C.POINTER(u32), C.POINTER(vp), C.POINTER(sz), C.POINTER(vp), C.c_int, _u64p]
         L.sb200_rescale_to_next_sized_host.argtypes = [vp, sz, sz, sz, _u64p, _u64p]
         L.sb200_mod_switch_to_next_sized_host.argtypes = [vp, sz, sz, sz, _u64p, _u64p]
         L.sb200_relinearize_sized_host.argtypes = [vp, sz, sz, sz, _u64p, vp, _u64p]
@@ -831,6 +836,36 @@ class Context:
         _check(lib().sb200_apply_galois_add_host(self.h, L, B, _hp(a), galois_elt, None if key is None else key.h, _hp(b), _hp(out)))
         return out[0] if single else out
 
+    def apply_galois_multiply_plain_add(self, a, galois_elt, key, plain, b, out=None):
+        """sb200_apply_galois_multiply_plain_add_host: b + plain * apply_galois(a), a and b [B][2][L][n], plain [count][L][n] (NTT
+        form, count 1 or B); out (may be b) or a fresh array"""
+        a, single = self._batched(a)
+        b, _ = self._batched(b)
+        plain = np.ascontiguousarray(plain, dtype=np.uint64)
+        if plain.ndim == 2:
+            plain = plain[None]
+        B, _, L, n = a.shape
+        if out is None:
+            out = np.zeros((B, 2, L, n), dtype=np.uint64)
+        _check(lib().sb200_apply_galois_multiply_plain_add_host(self.h, L, B, _hp(a), galois_elt, None if key is None else key.h,
+                                                                plain.shape[0], _hp(plain), _hp(b), _hp(out)))
+        return out[0] if single else out
+
+    def diagonal_sum(self, a, galois_elts, keys, plains, plain_is_ntt=True):
+        """sb200_diagonal_sum_host: sum_i plains[i] * apply_galois(a, galois_elts[i]) with keys[i] (element 1: no rotation, its key may
+        be None); a [B][2][L][n], plains[i] [count_i][L][n] (NTT form) or [count_i][n] (coefficient form), count_i 1 or B"""
+        a, single = self._batched(a)
+        B, _, L, n = a.shape
+        plains = [np.ascontiguousarray(p, dtype=np.uint64) for p in plains]
+        out = np.zeros((B, 2, L, n), dtype=np.uint64)
+        c_elts, c_keys = _rotate_sum_args(galois_elts, keys)
+        m = len(plains)
+        counts = (C.c_size_t * max(m, 1))(*[p.shape[0] for p in plains])
+        p_plains = (C.c_void_p * max(m, 1))(*[p.ctypes.data for p in plains])
+        _check(lib().sb200_diagonal_sum_host(self.h, L, B, _hp(a), len(galois_elts), c_elts, c_keys, counts, p_plains, int(plain_is_ntt),
+                                             _hp(out)))
+        return out[0] if single else out
+
     def rotate_sum(self, a, galois_elts, keys):
         """sb200_rotate_sum_host: y_0 = a, y_{j+1} = y_j + apply_galois(y_j, galois_elts[j]) with keys[j]; returns y_steps"""
         a, single = self._batched(a)
@@ -1123,6 +1158,23 @@ class Context:
         """sb200_apply_galois_add: out2 = addend2 + apply_galois(in2); out2 may be addend2, addend2 may be in2"""
         _check(lib().sb200_apply_galois_add(self.h, L, batch, _dp(in2), galois_elt, None if key is None else key.h,
                                             None if addend2 is None else _dp(addend2), _dp(out2), self._stream()))
+
+    def d_apply_galois_multiply_plain_add(self, in2, galois_elt, key, plain, plain_count, addend2, out2, L, batch):
+        """sb200_apply_galois_multiply_plain_add: out2 = addend2 + plain * apply_galois(in2), plain_count (1 or batch) NTT-form
+        plaintexts [L][n]; out2 may be addend2, addend2 may be in2"""
+        _check(lib().sb200_apply_galois_multiply_plain_add(self.h, L, batch, _dp(in2), galois_elt, None if key is None else key.h, plain_count,
+                                                           None if plain is None else _dp(plain), None if addend2 is None else _dp(addend2),
+                                                           _dp(out2), self._stream()))
+
+    def d_diagonal_sum(self, in2, galois_elts, keys, plains, plain_counts, out2, L, batch, plain_is_ntt=True):
+        """sb200_diagonal_sum: out2 = sum_i plains[i] * apply_galois(in2, galois_elts[i]) with keys[i] (element 1: no rotation, key may
+        be None); plains[i] holds plain_counts[i] (1 or batch) plaintexts, NTT form [L][n] or coefficient form [n]"""
+        c_elts, c_keys = _rotate_sum_args(galois_elts, keys)
+        m = len(plains)
+        counts = (C.c_size_t * max(m, 1))(*plain_counts)
+        p_plains = (C.c_void_p * max(m, 1))(*[None if p is None else _dp(p).value for p in plains])
+        _check(lib().sb200_diagonal_sum(self.h, L, batch, _dp(in2), len(galois_elts), c_elts, c_keys, counts, p_plains, int(plain_is_ntt),
+                                        _dp(out2), self._stream()))
 
     def d_rotate_sum(self, in2, galois_elts, keys, out2, L, batch):
         """sb200_rotate_sum: the chain y_{j+1} = y_j + apply_galois(y_j, galois_elts[j]) from in2, y_steps to out2 (may be in2)"""

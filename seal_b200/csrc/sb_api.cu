@@ -1477,6 +1477,91 @@ namespace
         return SB200_OK;
     }
 
+    // out = c + b * apply_galois(a), b: NTT-form plaintexts [plain_count][L][n]; out may be c, c may be a.  The checks in the chain's
+    // order: apply_galois's (level, element, key), then multiply_plain's (the plaintext count)
+    struct ApplyGaloisMultiplyPlainAdd
+    {
+        size_t L, plain_count;
+        uint32_t elt;
+        const KSwitchKey &key;
+        void check(const Context &c, size_t batch) const
+        {
+            check_level(c, L, batch);
+            check_rotate_sum_args(c, L, 1, &elt, std::array<const KSwitchKey *, 1>{ &key }.data());
+            check_plain_count(plain_count, batch);
+        }
+        Layout layout(const Context &c) const
+        {
+            const size_t poly = L * c.n;
+            const bool shared = plain_count == 1;
+            return { { { 2 * poly, "input a" }, { poly, "the plaintext", false, shared }, { 2 * poly, "the addend", true } },
+                     { { 2 * poly } },
+                     nullptr,
+                     "apply_galois_multiply_plain_add: in and out must not alias" };
+        }
+        void operator()(Context &c, size_t, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
+        {
+            op_apply_galois_multiply_plain_add(c, L, B, ins[0], elt, key, plain_count == 1, ins[1], ins[2], outs[0], st);
+        }
+    };
+
+    // out = sum_t plains[t] * apply_galois(in, elts[t]) (op_diagonal_sum): input 0 is the ciphertext slab, inputs 1 .. count the
+    // plaintexts (NTT form [L][n] or coefficient form [n] per plaintext, plain_counts[t] of them).  The output may not meet any input.
+    struct DiagonalSum
+    {
+        size_t L, count;
+        const uint32_t *elts;
+        const KSwitchKey *const *keys;
+        const size_t *plain_counts;
+        bool plain_ntt;
+        // in the chain's order: apply_galois's checks of every rotated term, multiply_plain's of every term (the plaintext counts and,
+        // for coefficient-form plaintexts, the scheme), then add_many's (the term count)
+        void check(Context &c, size_t batch) const
+        {
+            check_level(c, L, batch);
+            check_diagonal_sum_args(c, L, count, elts, keys);
+            for (size_t t = 0; t < count; t++)
+                check_plain_count(plain_counts[t], batch);
+            if (!plain_ntt && count)
+                plain_level(c, L); // "unsupported operation for scheme type" for CKKS
+            if (count == 0)
+                throw std::invalid_argument("encrypteds cannot be empty");
+        }
+        Layout layout(const Context &c) const
+        {
+            const size_t poly = L * c.n;
+            Layout w{ { { 2 * poly, "input" } }, { { 2 * poly } }, "diagonal_sum", "diagonal_sum: in and out must not alias" };
+            for (size_t t = 0; t < count; t++)
+                w.in.push_back({ plain_ntt ? poly : c.n, "a plaintext operand", false, plain_counts[t] == 1 });
+            return w;
+        }
+        void operator()(Context &c, size_t, size_t B, const u64 *const *ins, u64 *const *outs, cudaStream_t st) const
+        {
+            std::vector<size_t> counts(count); // of this chunk
+            for (size_t t = 0; t < count; t++)
+                counts[t] = plain_counts[t] == 1 ? 1 : B;
+            op_diagonal_sum(c, L, B, ins[0], count, elts, keys, counts.data(), ins + 1, plain_ntt, outs[0], st);
+        }
+    };
+
+    // the key handles of a diagonal_sum call, after the pointer checks (SB200_E_POINTER on a NULL array, or a NULL key of a rotated
+    // term; element 1 needs none)
+    int diagonal_sum_keys(size_t count, const uint32_t *elts, const sb200_kswitch_key *const *keys, const size_t *plain_counts,
+                          const uint64_t *const *plains, std::vector<const KSwitchKey *> &out)
+    {
+        SB_NEED(elts);
+        SB_NEED(keys);
+        SB_NEED(plain_counts);
+        SB_NEED(plains);
+        for (size_t t = 0; t < count; t++)
+        {
+            if (elts[t] != 1)
+                SB_NEED(keys[t]);
+            out.push_back(keys[t] ? &keys[t]->k : nullptr);
+        }
+        return SB200_OK;
+    }
+
     struct ModSwitch // rescale_to_next (CKKS) or mod_switch_to_next of ciphertexts of any size: L primes -> L - 1
     {
         bool rescale;
@@ -2052,6 +2137,38 @@ int sb200_rotate_sum_host(sb200_context *ctx, size_t L, size_t batch, const uint
     if (int e = rotate_sum_keys(steps, elts, keys, k))
         return e;
     return on_host(ctx, batch, { in2 }, { out2 }, RotateSum{ L, steps, elts, k.data() });
+}
+int sb200_apply_galois_multiply_plain_add(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, uint32_t elt, const sb200_kswitch_key *key,
+                                          size_t plain_count, const uint64_t *plain, const uint64_t *addend2, uint64_t *out2, void *stream)
+{
+    SB_NEED(key);
+    return on_stream(ctx, stream, batch, { in2, plain, addend2 }, { out2 }, ApplyGaloisMultiplyPlainAdd{ L, plain_count, elt, key->k });
+}
+int sb200_apply_galois_multiply_plain_add_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, uint32_t elt,
+                                               const sb200_kswitch_key *key, size_t plain_count, const uint64_t *plain, const uint64_t *addend2,
+                                               uint64_t *out2)
+{
+    SB_NEED(key);
+    return on_host(ctx, batch, { in2, plain, addend2 }, { out2 }, ApplyGaloisMultiplyPlainAdd{ L, plain_count, elt, key->k });
+}
+int sb200_diagonal_sum(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, size_t count, const uint32_t *elts,
+                       const sb200_kswitch_key *const *keys, const size_t *plain_counts, const uint64_t *const *plains, int plain_is_ntt,
+                       uint64_t *out2, void *stream)
+{
+    std::vector<const KSwitchKey *> k;
+    if (int e = diagonal_sum_keys(count, elts, keys, plain_counts, plains, k))
+        return e;
+    return on_stream(ctx, stream, batch, InSlabs(&in2, 1, plains, count), { out2 },
+                     DiagonalSum{ L, count, elts, k.data(), plain_counts, plain_is_ntt != 0 });
+}
+int sb200_diagonal_sum_host(sb200_context *ctx, size_t L, size_t batch, const uint64_t *in2, size_t count, const uint32_t *elts,
+                            const sb200_kswitch_key *const *keys, const size_t *plain_counts, const uint64_t *const *plains, int plain_is_ntt,
+                            uint64_t *out2)
+{
+    std::vector<const KSwitchKey *> k;
+    if (int e = diagonal_sum_keys(count, elts, keys, plain_counts, plains, k))
+        return e;
+    return on_host(ctx, batch, InSlabs(&in2, 1, plains, count), { out2 }, DiagonalSum{ L, count, elts, k.data(), plain_counts, plain_is_ntt != 0 });
 }
 
 // ---- wire format (SURVEY 8f rank 3): Ciphertext::save / load, compr_mode none, between byte streams and device slabs ----

@@ -1963,7 +1963,7 @@ namespace sb
             u64 x = X[b * x_bs + c * x_ps + (static_cast<long long>(i) << logn) + idx];
             u64 r = mul_shoup(x + P.q - t, inv_top[i], P.q);
             r = csub(r + base.get(b, c, i, idx, P.q), P.q);
-            out[b * o_bs + c * o_ps + (static_cast<long long>(i) << logn) + idx] = plus_addend(base, b, c, i, logn, idx, r, P.q);
+            out[b * o_bs + c * o_ps + (static_cast<long long>(i) << logn) + idx] = finish(base, b, c, i, logn, idx, r, P);
         }
         __device__ __forceinline__ void store8(int row, int idx0, u64 (&a)[8], const PrimeDev &P) const
         {
@@ -1991,11 +1991,7 @@ namespace sb
                     r0 = csub(r0 + base.get(b, c, i, idx0 + 2 * h, P.q), P.q);
                     r1 = csub(r1 + base.get(b, c, i, idx0 + 2 * h + 1, P.q), P.q);
                 }
-                if constexpr (Base::kAddend)
-                {
-                    const ulonglong2 av = reinterpret_cast<const ulonglong2 *>(base.arow(b, c, i, logn) + idx0)[h];
-                    r0 = csub(r0 + av.x, P.q), r1 = csub(r1 + av.y, P.q);
-                }
+                finish2(base, b, c, i, logn, idx0, h, r0, r1, P);
                 op_[h] = make_ulonglong2(r0, r1);
             }
         }
@@ -2047,7 +2043,7 @@ namespace sb
         u64 x = X[b * x_bs + c * x_ps + (static_cast<long long>(i) << logn) + idx];
         u64 r = mul_shoup(x + P.q2 - t, inv_top[i], P.q);
         r = csub(r + base.get(b, c, i, idx, P.q), P.q);
-        out[b * o_bs + c * o_ps + (static_cast<long long>(i) << logn) + idx] = plus_addend(base, b, c, i, logn, idx, r, P.q);
+        out[b * o_bs + c * o_ps + (static_cast<long long>(i) << logn) + idx] = finish(base, b, c, i, logn, idx, r, P);
     }
 
     struct KsScratch
@@ -2343,6 +2339,8 @@ namespace sb
             OpModDownFwd<Base> op{ s.U, s.Pp, pp_bs, pp_ps, s.T, out, o_bs, o_ps, inv_top, base, c.q[c.k - 1], c.logn, Li };
             cuda_check(launch_ntt_fwd(op, static_cast<int>(B * 2 * L), c.logn, c.d_primes.get(), st, c.stats, "ks_moddown_ntt", -1, c.fast_q), "ks moddown ntt");
         }
+        else if constexpr (Base::kPlain) // BFV's result is in coefficient form: a plaintext product there is a convolution
+            throw std::logic_error("the key switch's plaintext product needs an NTT-form result (CKKS / BGV)");
         else
         {
             OpProdIntt op{ s.Pp, c.logn, Li };
@@ -2441,10 +2439,12 @@ namespace sb
             throw std::invalid_argument("Galois element is not valid"); // evaluator.cpp:2424-2427
     }
 
-    // out = apply_galois(in) (Base = BaseSrc) or addend + apply_galois(in) (BaseAddSrc), in chunks of the key-switching scratch
+    // out = apply_galois(in) (Base = BaseSrc), addend + apply_galois(in) (BaseAddSrc) or [addend +] plain * apply_galois(in)
+    // (BasePlainSrc, NTT-form plaintexts [P][L][n] with plain_bs words between members: 0 for one plaintext), in chunks of the
+    // key-switching scratch
     template <class Base>
     static void galois_chunks(Context &c, size_t L, size_t batch, const u64 *in2, uint32_t elt, const KSwitchKey &key, const u64 *addend2,
-                              u64 *out2, cudaStream_t st)
+                              u64 *out2, cudaStream_t st, const u64 *plain = nullptr, long long plain_bs = 0)
     {
         const size_t poly = L * c.n, chunk = ks_chunk(c, L, batch, false);
         const uint32_t *perm = nullptr;
@@ -2475,6 +2475,11 @@ namespace sb
                 base.a = addend2 + b0 * 2 * poly;
                 base.a_bs = static_cast<long long>(2 * poly);
                 base.a_ps = static_cast<long long>(poly);
+            }
+            if constexpr (Base::kPlain)
+            {
+                base.pl = plain + b0 * plain_bs;
+                base.p_bs = plain_bs;
             }
             key_switch_chunk(c, L, B, s, target, key, base, out2 + b0 * 2 * poly, st);
         }
@@ -2536,6 +2541,149 @@ namespace sb
                 u64 *dst = ((steps - j - 1) & 1) ? tmp : o;
                 galois_chunks<BaseAddSrc>(c, L, B, y, elts[j], *keys[j], y, dst, st);
                 y = dst;
+            }
+        }
+    }
+
+    // One rotated term of a diagonal sum on a chunk of B ciphertexts (at most one key-switching chunk): out = [addend +] plain *
+    // apply_galois(in), with out == addend allowed.  CKKS / BGV (NTT-form plaintexts): one key switch, the product and the addition in
+    // its last pass.  BFV: the chain itself through tmp ([B][2][L][n]): apply_galois, then multiply_plain as the reference multiplies
+    // a coefficient-form ciphertext (an NTT-form plaintext: to NTT form, dyadic product, back, evaluator.cpp:2005-2010; a
+    // coefficient-form one: multiply_plain_normal), then add_many's two-operand fold.
+    static void galois_plain_term(Context &c, size_t L, size_t B, const u64 *in2, uint32_t elt, const KSwitchKey &key, bool shared, const u64 *plain,
+                                  bool plain_ntt, const u64 *addend2, u64 *out2, u64 *tmp, cudaStream_t st)
+    {
+        if (c.scheme != 1)
+        {
+            if (!plain_ntt)
+                throw std::logic_error("the key switch's plaintext product takes NTT-form plaintexts");
+            const long long pbs = shared ? 0 : static_cast<long long>(L * c.n);
+            if (addend2)
+                galois_chunks<BasePlainSrc<true>>(c, L, B, in2, elt, key, addend2, out2, st, plain, pbs);
+            else
+                galois_chunks<BasePlainSrc<false>>(c, L, B, in2, elt, key, nullptr, out2, st, plain, pbs);
+            return;
+        }
+        galois_chunks<BaseSrc>(c, L, B, in2, elt, key, nullptr, tmp, st);
+        u64 *dst = addend2 ? tmp : out2;
+        if (plain_ntt)
+        {
+            op_ntt(c, false, L, 2, B, tmp, st);
+            op_multiply_plain(c, L, 2, B, shared, tmp, plain, dst, st);
+            op_ntt(c, true, L, 2, B, dst, st);
+        }
+        else
+            op_multiply_plain_coeff(c, L, 2, B, shared, false, tmp, plain, dst, st);
+        if (addend2)
+        {
+            const size_t sizes[2] = { 2, 2 };
+            const u64 *ops[2] = { addend2, tmp };
+            const int modes[1] = { SB200_FOLD_ADD };
+            op_add_many(c, L, B, 2, sizes, ops, modes, nullptr, out2, st);
+        }
+    }
+
+    void op_apply_galois_multiply_plain_add(Context &c, size_t L, size_t batch, const u64 *in2, uint32_t elt, const KSwitchKey &key, bool shared,
+                                            const u64 *plain, const u64 *addend2, u64 *out2, cudaStream_t st)
+    {
+        check_galois_args(c, L, elt, key);
+        if (in2 == out2)
+            throw std::invalid_argument("apply_galois_multiply_plain_add: in and out must not alias");
+        const size_t poly = L * c.n;
+        if (c.scheme != 1)
+        {
+            galois_chunks<BasePlainSrc<true>>(c, L, batch, in2, elt, key, addend2, out2, st, plain, shared ? 0 : static_cast<long long>(poly));
+            return;
+        }
+        const size_t chunk = ks_chunk(c, L, batch, false);
+        u64 *tmp = static_cast<u64 *>(c.ensure_aux(chunk * 2 * poly * sizeof(u64)));
+        for (size_t b0 = 0; b0 < batch; b0 += chunk)
+        {
+            const size_t B = std::min(chunk, batch - b0);
+            galois_plain_term(c, L, B, in2 + b0 * 2 * poly, elt, key, shared, shared ? plain : plain + b0 * poly, true, addend2 + b0 * 2 * poly,
+                              out2 + b0 * 2 * poly, tmp, st);
+        }
+    }
+
+    void check_diagonal_sum_args(const Context &c, size_t L, size_t count, const uint32_t *elts, const KSwitchKey *const *keys)
+    {
+        for (size_t t = 0; t < count; t++)
+            if (elts[t] != 1)
+                check_galois_args(c, L, elts[t], *keys[t]);
+    }
+
+    // Identity terms (element 1) first, all in one multiply_plain_sum pass that initialises out; then each rotated term accumulates
+    // into out through galois_plain_term (the first one writes out when there is no identity term).  Each chunk of the key-switching
+    // scratch runs every term before the next chunk starts, so every key is read once per chunk and term, as the chain reads it.
+    // Temporaries: none for CKKS and for BGV with NTT-form plaintexts.  BGV's coefficient-form plaintexts are lifted and transformed
+    // once into the aux arena (the reference's transform_to_ntt_inplace of each plaintext): the shared ones before the first chunk,
+    // the per-member ones of each chunk with it.  BFV's chain goes through one chunk-sized ciphertext there.
+    void op_diagonal_sum(Context &c, size_t L, size_t batch, const u64 *in2, size_t count, const uint32_t *elts, const KSwitchKey *const *keys,
+                         const size_t *plain_counts, const u64 *const *plains, bool plain_ntt, u64 *out2, cudaStream_t st)
+    {
+        check_diagonal_sum_args(c, L, count, elts, keys);
+        if (in2 == out2)
+            throw std::invalid_argument("diagonal_sum: in and out must not alias");
+        const size_t poly = L * c.n, pw = plain_ntt ? poly : c.n, chunk = ks_chunk(c, L, batch, false);
+        const bool bfv = c.scheme == 1, lift = c.scheme == 3 && !plain_ntt;
+        std::vector<size_t> ident, rot;
+        for (size_t t = 0; t < count; t++)
+            (elts[t] == 1 ? ident : rot).push_back(t);
+        // aux: [BFV's chunk of ciphertexts][the lifted shared plaintexts][the lifted per-member plaintexts of one chunk]
+        const size_t tmp_words = bfv && !rot.empty() ? chunk * 2 * poly : 0;
+        size_t shared_words = 0, member_words = 0;
+        for (size_t t = 0; t < count && lift; t++)
+            (plain_counts[t] == 1 ? shared_words : member_words) += (plain_counts[t] == 1 ? 1 : chunk) * poly;
+        const size_t aux_words = tmp_words + shared_words + member_words;
+        u64 *aux = aux_words ? static_cast<u64 *>(c.ensure_aux(aux_words * sizeof(u64))) : nullptr;
+        std::vector<const u64 *> p(count), id_cts(ident.size()), id_plains(ident.size());
+        std::vector<size_t> id_sizes(ident.size(), 2), id_counts(ident.size());
+        if (lift)
+        {
+            u64 *w = aux + tmp_words;
+            for (size_t t = 0; t < count; t++)
+                if (plain_counts[t] == 1)
+                {
+                    op_plain_to_ntt(c, L, 1, plains[t], nullptr, w, st);
+                    p[t] = w, w += poly;
+                }
+        }
+        for (size_t b0 = 0; b0 < batch; b0 += chunk)
+        {
+            const size_t B = std::min(chunk, batch - b0);
+            const u64 *x = in2 + b0 * 2 * poly;
+            u64 *o = out2 + b0 * 2 * poly;
+            u64 *w = aux ? aux + tmp_words + shared_words : nullptr;
+            for (size_t t = 0; t < count; t++)
+            {
+                if (plain_counts[t] == 1)
+                {
+                    if (!lift)
+                        p[t] = plains[t];
+                    continue;
+                }
+                p[t] = plains[t] + b0 * pw;
+                if (lift)
+                {
+                    op_plain_to_ntt(c, L, B, p[t], nullptr, w, st);
+                    p[t] = w, w += B * poly;
+                }
+            }
+            const bool pn = plain_ntt || lift;
+            for (size_t u = 0; u < ident.size(); u++)
+            {
+                id_cts[u] = x;
+                id_plains[u] = p[ident[u]];
+                id_counts[u] = plain_counts[ident[u]] == 1 ? 1 : B;
+            }
+            if (!ident.empty())
+                op_multiply_plain_sum(c, L, B, ident.size(), 1, id_sizes.data(), id_cts.data(), id_counts.data(), id_plains.data(), !bfv, pn,
+                                      nullptr, nullptr, &o, st);
+            bool first = ident.empty();
+            for (size_t t : rot)
+            {
+                galois_plain_term(c, L, B, x, elts[t], *keys[t], plain_counts[t] == 1, p[t], pn, first ? nullptr : o, o, aux, st);
+                first = false;
             }
         }
     }

@@ -252,6 +252,16 @@ namespace sb
     void check_rotate_sum_args(const Context &c, size_t L, size_t steps, const uint32_t *elts, const KSwitchKey *const *keys);
     void op_rotate_sum(Context &c, size_t L, size_t batch, const u64 *in2, size_t steps, const uint32_t *elts, const KSwitchKey *const *keys,
                        u64 *out2, cudaStream_t st);
+    // out = addend + plain * apply_galois(in), NTT-form plaintexts [P][L][n] (shared: P = 1).  CKKS / BGV: the product and the addition
+    // in the key switch's last pass; BFV: the chain through one chunk-sized temporary.  out may be addend, addend may be in, out == in
+    // is rejected
+    void op_apply_galois_multiply_plain_add(Context &c, size_t L, size_t batch, const u64 *in2, uint32_t elt, const KSwitchKey &key, bool shared,
+                                            const u64 *plain, const u64 *addend2, u64 *out2, cudaStream_t st);
+    // out = sum_t plains[t] * apply_galois(in, elts[t]); element 1 is no rotation (its key may be NULL).  plain_counts[t]: 1 or batch;
+    // plains NTT form [P][L][n] or (plain_ntt = false, BFV / BGV) coefficient form [P][n].  out must not alias in
+    void check_diagonal_sum_args(const Context &c, size_t L, size_t count, const uint32_t *elts, const KSwitchKey *const *keys);
+    void op_diagonal_sum(Context &c, size_t L, size_t batch, const u64 *in2, size_t count, const uint32_t *elts, const KSwitchKey *const *keys,
+                         const size_t *plain_counts, const u64 *const *plains, bool plain_ntt, u64 *out2, cudaStream_t st);
     size_t keyswitch_chunk(const Context &c, size_t L, size_t batch, bool fused);
     // arithmetic ceilings measured in process: warp-level butterflies (kind 0-2) / multiply-accumulates (kind 3) per second
     double selftest_rate(Context &c, int kind, cudaStream_t st);

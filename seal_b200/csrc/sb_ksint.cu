@@ -1081,7 +1081,7 @@ namespace sb
                 const int xi = j + (e << 12);
                 if (MODE == 1)
                     A.out[b * A.o_bs + c * A.o_ps + (static_cast<long long>(i) << LOGN) + xi] =
-                        plus_addend(A.base, b, c, i, LOGN, xi, csub(r + A.base.get(b, c, i, xi, Q.q), Q.q), Q.q);
+                        finish(A.base, b, c, i, LOGN, xi, csub(r + A.base.get(b, c, i, xi, Q.q), Q.q), Q);
                 else
                     A.R[((static_cast<size_t>(bc) * L + i) << LOGN) + xi] = r;
             }
@@ -1244,7 +1244,7 @@ namespace sb
             const int i = row % L, bc = row / L, b = bc >> 1, c = bc & 1;
             const u64 t = csub(csub(v, P.q2), P.q);
             out[b * o_bs + c * o_ps + (static_cast<long long>(i) << logn) + idx] =
-                plus_addend(base, b, c, i, logn, idx, csub(t + base.get(b, c, i, idx, P.q), P.q), P.q);
+                finish(base, b, c, i, logn, idx, csub(t + base.get(b, c, i, idx, P.q), P.q), P);
         }
         __device__ __forceinline__ void store8(int row, int idx0, u64 (&a)[8], const PrimeDev &P) const
         {
@@ -1267,11 +1267,7 @@ namespace sb
                     r0 = csub(r0 + base.get(b, c, i, idx0 + 2 * h, P.q), P.q);
                     r1 = csub(r1 + base.get(b, c, i, idx0 + 2 * h + 1, P.q), P.q);
                 }
-                if constexpr (Base::kAddend)
-                {
-                    const ulonglong2 av = reinterpret_cast<const ulonglong2 *>(base.arow(b, c, i, logn) + idx0)[h];
-                    r0 = csub(r0 + av.x, P.q), r1 = csub(r1 + av.y, P.q);
-                }
+                finish2(base, b, c, i, logn, idx0, h, r0, r1, P);
                 op_[h] = make_ulonglong2(r0, r1);
             }
         }
@@ -1521,9 +1517,14 @@ namespace sb
                 launch_crt<3>(A, d, fuse_crt, B, c.logn, st);
             else if (c.scheme == 1)
             {
-                CrtArgs<Base> Ab{ A.Acc, A.punct, A.neg, A.primes, A.inv_top, A.half_mod, A.qtop_mod, A.t, A.t_ratio, A.inv_top_mod_t,
-                                  A.R, A.out, A.o_bs, A.o_ps, base, A.L, A.k, A.total };
-                launch_crt<1>(Ab, d, fuse_crt, B, c.logn, st);
+                if constexpr (Base::kPlain) // BFV: a plaintext product of a coefficient-form result is a convolution
+                    throw std::logic_error("the key switch's plaintext product needs an NTT-form result (CKKS / BGV)");
+                else
+                {
+                    CrtArgs<Base> Ab{ A.Acc, A.punct, A.neg, A.primes, A.inv_top, A.half_mod, A.qtop_mod, A.t, A.t_ratio, A.inv_top_mod_t,
+                                      A.R, A.out, A.o_bs, A.o_ps, base, A.L, A.k, A.total };
+                    launch_crt<1>(Ab, d, fuse_crt, B, c.logn, st);
+                }
             }
             else
                 launch_crt<0>(A, d, fuse_crt, B, c.logn, st);
@@ -1541,6 +1542,10 @@ namespace sb
                                       cudaStream_t);
     template void ksint_core<BaseAddSrc>(Context &, size_t, size_t, const KsIntScratch &, Src, u64 *, const KSwitchKey &, BaseAddSrc, u64 *,
                                          long long, cudaStream_t);
+    template void ksint_core<BasePlainSrc<false>>(Context &, size_t, size_t, const KsIntScratch &, Src, u64 *, const KSwitchKey &,
+                                                  BasePlainSrc<false>, u64 *, long long, cudaStream_t);
+    template void ksint_core<BasePlainSrc<true>>(Context &, size_t, size_t, const KsIntScratch &, Src, u64 *, const KSwitchKey &,
+                                                 BasePlainSrc<true>, u64 *, long long, cudaStream_t);
 
     static void launch_inverse(Context &c, uint32_t *data, int arows, cudaStream_t st, bool outer)
     {

@@ -62,8 +62,9 @@ namespace sb
     void ksint_init(Context &c);
     // khat[t][J][c][ki][n] from the uploaded key [digits][2][k][n]
     void ksint_prepare_key(Context &c, KSwitchKey &key, cudaStream_t st);
-    // target (CKKS / BGV: NTT form, BFV: coefficient form) -> out = base + key-switched polynomials (+ the addend of a BaseAddSrc);
-    // D: [B][L][n] scratch of the target's inverse transforms.  See key_switch_chunk.  Instantiated for BaseSrc and BaseAddSrc
+    // target (CKKS / BGV: NTT form, BFV: coefficient form) -> out = base + key-switched polynomials (+ the addend of a BaseAddSrc;
+    // times the plaintext, then + the addend, of a BasePlainSrc: CKKS / BGV only).  D: [B][L][n] scratch of the target's inverse
+    // transforms.  See key_switch_chunk.  Instantiated for BaseSrc, BaseAddSrc, BasePlainSrc<false> and BasePlainSrc<true>
     template <class Base>
     void ksint_core(Context &c, size_t L, size_t B, const KsIntScratch &s, Src target, u64 *D, const KSwitchKey &key, Base base,
                     u64 *out, long long o_bs, cudaStream_t st);

@@ -50,6 +50,7 @@ namespace sb
             return t.get(b, i, idx, q);
         }
         static constexpr bool kAddend = false;
+        static constexpr bool kPlain = false;
     };
 
     // BaseSrc plus an addend: a plain [B][2][L][n] source added to both output components after the base term (apply_galois_add:
@@ -65,14 +66,46 @@ namespace sb
         }
     };
 
-    // r (canonical) + the addend word, canonical: a second csub, so words of q - 1 everywhere stay below q.  No-op without an addend.
-    template <class Base>
-    __device__ __forceinline__ u64 plus_addend(const Base &base, int b, int c, int i, int logn, int idx, u64 r, u64 q)
+    // BaseSrc times an NTT-form plaintext, plus an addend when ADD (apply_galois_multiply_plain_add: out = addend + plain *
+    // apply_galois(in)).  Both output components are multiplied by the same plaintext word, after the base term; the plaintext is
+    // [P][L][n] with P = 1 (p_bs = 0, one plaintext for the batch) or one per item.  CKKS / BGV only: the key switch's result is
+    // in NTT form there, so the plaintext product is element-wise.
+    template <bool ADD>
+    struct BasePlainSrc : BaseAddSrc
     {
+        const u64 *pl = nullptr; // prime i of item b's plaintext at pl + b*p_bs + i*n
+        long long p_bs = 0;
+        static constexpr bool kAddend = ADD;
+        static constexpr bool kPlain = true;
+        __device__ __forceinline__ const u64 *prow(int b, int i, int logn) const { return pl + b * p_bs + (static_cast<long long>(i) << logn); }
+    };
+
+    // the last step of every key-switching exit, on r (canonical, the base term added): r * plaintext word (reduced on the way in, as
+    // plain_mul_kernel reduces it: any 64-bit word is accepted), then + the addend word with a second csub, so words of q - 1
+    // everywhere stay below q.  No-op for BaseSrc.
+    template <class Base>
+    __device__ __forceinline__ u64 finish(const Base &base, int b, int c, int i, int logn, int idx, u64 r, const PrimeDev &P)
+    {
+        if constexpr (Base::kPlain)
+            r = mulmod_wide(r, canon_in(base.prow(b, i, logn)[idx], P), P);
         if constexpr (Base::kAddend)
-            return csub(r + base.arow(b, c, i, logn)[idx], q);
-        else
-            return r;
+            r = csub(r + base.arow(b, c, i, logn)[idx], P.q);
+        return r;
+    }
+    // the same on the coefficient pair 2h, 2h + 1 past idx0, with 16-byte loads (the store8 exits)
+    template <class Base>
+    __device__ __forceinline__ void finish2(const Base &base, int b, int c, int i, int logn, int idx0, int h, u64 &r0, u64 &r1, const PrimeDev &P)
+    {
+        if constexpr (Base::kPlain)
+        {
+            const ulonglong2 pv = reinterpret_cast<const ulonglong2 *>(base.prow(b, i, logn) + idx0)[h];
+            r0 = mulmod_wide(r0, canon_in(pv.x, P), P), r1 = mulmod_wide(r1, canon_in(pv.y, P), P);
+        }
+        if constexpr (Base::kAddend)
+        {
+            const ulonglong2 av = reinterpret_cast<const ulonglong2 *>(base.arow(b, c, i, logn) + idx0)[h];
+            r0 = csub(r0 + av.x, P.q), r1 = csub(r1 + av.y, P.q);
+        }
     }
 
     // (1) target -> coefficient form (CKKS / BGV): rows (b, J); evaluator.cpp:2651-2658
